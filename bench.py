@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the find_arb! dual-gradient sweep on B200 (BASELINE.json metric).
+"""bench.py -- the find_arb! dual-gradient sweep on H100 (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            # our CUDA path
   python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path
@@ -11,15 +11,20 @@ one L-BFGS-B function/gradient evaluation of route! costs on the pool side.
 Workload (config.workload): BASELINE.json configs[4] -- 10M ProductTwoCoin
 pools, 50k tokens -- per GPU.  It is the configuration the metric's target is
 quoted on (">= 10M find_arb! evaluations per sweep"), it fits one GPU, and at
-320 MB it is larger than the 126 MB L2, so every timed sweep streams from HBM
-without an explicit flush.  For N > 1 each rank owns its own 10M-pool shard
+320 MB it is larger than the L2 (50 MB on an H100), so every timed sweep streams
+from HBM without an explicit flush.  For N > 1 each rank owns its own 10M-pool shard
 (weak scaling) and the only exchange is the sum of [Ψ; acc] over NVLink peer
 memory after each sweep; `--scaling strong` splits the same 10M pools instead.
 
 Prints ONE JSON line (rank 0).  `value` = pools evaluated per second with ν and
 Ψ resident in HBM (CUDA events, max over ranks); `e2e` = the same through the
 public C-ABI call cfmm_sweep() with pinned HOST buffers (H2D ν and D2H Ψ inside
-the timed region).
+the timed region).  Every timed region runs exactly --steps steps.
+
+`--dump-outputs DIR` writes what the last timed step computed, the [Ψ; acc]
+vector a caller of the sweep receives, as DIR/psi.npy (float64 [n_tokens]) and
+DIR/acc.npy (float64 [1]).  The inputs are seeded, so two builds run with the
+same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -63,11 +68,13 @@ def parse_args():
     ap.add_argument("--nu", choices=["near", "wide", "ones"], default="near")
     ap.add_argument("--exact", type=int, default=0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--e2e-steps", type=int, default=0, help="0 = same as --steps (capped)")
+    ap.add_argument("--e2e-steps", type=int, default=0, help="0 = same as --steps")
     ap.add_argument("--no-flush", action="store_true", help="small workloads: L2-warm timing only")
     ap.add_argument("--verify", type=int, default=1, help="N > 1: check the reduced [Psi; acc] (outside the timed regions)")
     ap.add_argument("--opt", action="append", default=[], help="library option key=value (measurement)")
     ap.add_argument("--strong", type=int, default=1, help="N > 1 (weak): also time the same total pool count split over the ranks")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's [Psi; acc] as DIR/psi.npy and DIR/acc.npy")
     return ap.parse_args()
 
 
@@ -299,9 +306,10 @@ def run_ours(args):
         pools.set_option(kv.split("=")[0], int(kv.split("=")[1]))
     m_local = shard["m_local"]
     alg_bytes = float(shard["bytes"])
-    # working sets that fit in the 126 MB L2 are timed with an L2 flush before every step
+    # working sets that fit in the L2 are timed with an L2 flush before every step
     # (value, roofline) AND warm (reported beside it); larger ones stream from HBM anyway
-    flushed = alg_bytes <= 126e6 and not args.no_flush
+    l2_bytes = torch.cuda.get_device_properties(dev).L2_cache_size
+    flushed = alg_bytes <= l2_bytes and not args.no_flush
     if not (world > 1 and args.verify):
         shard = None
 
@@ -332,19 +340,22 @@ def run_ours(args):
     flush_rd = torch.zeros(32 << 20, dtype=torch.int64, device=dev) if flushed else None
 
     def flush_l2():
-        """Write 256 MB (> L2), then READ another 256 MB: the write alone would leave ~126 MB of dirty
+        """Write 256 MB (> L2), then READ another 256 MB: the write alone would leave an L2 full of dirty
         lines whose write-back the next (timed) kernel pays for; after the read pass the L2 holds
         clean lines of an unrelated buffer.  Both passes are outside the timed intervals."""
         flush_buf.zero_()
         flush_rd.sum()
+
+    last_result = [0]  # device address of the latest step's [Ψ; acc]
 
     def make_step(p):
         def step():
             if exchange == "nccl":  # NCCL needs the partial in a torch tensor
                 p.sweep_device(d_nu.data_ptr(), d_psi.data_ptr(), False, sptr)
                 dist.all_reduce(d_psi)
+                last_result[0] = d_psi.data_ptr()
             else:  # zero-copy: [Ψ; acc] stays in the context's device buffer
-                p.sweep_device_view(d_nu.data_ptr(), False, sptr)
+                last_result[0] = p.sweep_device_view(d_nu.data_ptr(), False, sptr)
         return step
 
     step = make_step(pools)
@@ -390,9 +401,9 @@ def run_ours(args):
 
     def spin_up(min_ms=20.0):
         """Untimed sweeps until the GPU has been busy for min_ms: after an idle period (setup, a
-        host-side pause between regions) the first ~20 launches run 2-4 us slower than the steady
-        state (tools/ramp_probe.py: 59.9 -> 57.8 -> 55.9 us over launches 0-5 / 5-20 / 20+); a short
-        synchronize does not bring that back.  Called right before every timed region's barrier."""
+        host-side pause between regions) the first launches can run slower than the steady state
+        (tools/ramp_probe.py measures the ramp); a short synchronize does not bring that back.
+        Called right before every timed region's barrier."""
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(stream)
         done = 0
@@ -426,17 +437,11 @@ def run_ours(args):
         ms_total = timed_region(args.steps, flush=flushed)
         launches = pools.launch_count - l0
         extra["host_enqueue_us_per_step"] = host_enqueue_us[0]
-        # a driver-sized K can be a millisecond of GPU time: also a region of >= 50 ms of the
-        # same steps (`sustained`), so that the clocks are sampled under load
-        ms_dec = ms_total
-        if world > 1:  # every rank must take the same branch and launch the same number of sweeps
-            t = torch.tensor([ms_total], dtype=torch.float64, device=dev)
-            dist.all_reduce(t, op=dist.ReduceOp.MAX)
-            ms_dec = t.item()
-        if ms_dec < 50.0 and not flushed:
-            k2 = int(min(50_000, max(args.steps, np.ceil(60.0 * args.steps / max(ms_dec, 1e-3)))))
-            ms2 = timed_region(k2)
-            extra["sustained"] = {"steps": k2, "ms_per_step": ms2 / k2}
+        if args.dump_outputs and rank == 0:  # (timed_region ended in a synchronize)
+            out = _view(torch, last_result[0], n + 1, dev).cpu().numpy()
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "psi.npy"), out[:n].astype(np.float64))
+            np.save(os.path.join(args.dump_outputs, "acc.npy"), out[n:].astype(np.float64))
         sampler.stop()
         sampler_ref[0] = None
         if flushed:
@@ -453,7 +458,7 @@ def run_ours(args):
         pools.set_option("profile", 0)
 
         # ---- e2e: public C-ABI call with pinned host buffers, copies inside ----
-        e2e_steps = args.e2e_steps or min(args.steps, 2000)
+        e2e_steps = args.e2e_steps or args.steps
         h_nu = torch.from_numpy(nu_host).pin_memory()
         h_out = torch.zeros(n + 1, dtype=torch.float64).pin_memory()  # [psi ; acc] contiguous
         h_psi, h_acc = h_out[:n], h_out[n:]
@@ -498,7 +503,7 @@ def run_ours(args):
         total_pools = int(tp.item())
     value = total_pools * args.steps / (ms_total * 1e-3)
     e2e_value = total_pools * e2e_steps / e2e_s
-    for key in ("sustained", "l2_warm"):
+    for key in ("l2_warm",):
         if key in extra:
             t = torch.tensor([extra[key]["ms_per_step"]], dtype=torch.float64, device=dev)
             if world > 1:
@@ -512,7 +517,7 @@ def run_ours(args):
             with open(peaks_path) as f:
                 peak, peak_src = float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         else:
-            peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+            peak, peak_src = 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not a measurement"
         kind = WORKLOADS[args.workload][2]
         roofline = roofline_object(prof, prof_times, ms_total, args.steps, launches, kind, m_local,
                                    alg_bytes, peak, peak_src, args.workload, flushed,
@@ -539,7 +544,7 @@ def run_ours(args):
                                              {0: "direct 8-byte push (1 hop)" if world <= 4 else "LL two-shot",
                                               3: "direct 8-byte push (1 hop)",
                                               1: "LL one-shot", 2: "LL two-shot"}[args.protocol]),
-                       "l2": "inputs larger than L2 (320 MB algorithmic, 240-320 MB streamed per launch per GPU > 126 MB)" if alg_bytes > 126e6
+                       "l2": f"inputs larger than L2 ({alg_bytes / 1e6:.0f} MB algorithmic > {l2_bytes / 1e6:.0f} MB L2)" if alg_bytes > l2_bytes
                              else ("L2 flushed (256 MB written, then 256 MB read so that no dirty lines remain) before every timed step; the warm figure is in l2_warm"
                                    if flushed else "L2-WARM: working set fits in L2, no flush between steps")},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": 8 * n,
@@ -771,7 +776,7 @@ def roofline_object(prof, prof_times, ms_total, steps, launches, kind, m_local, 
 
 
 def read_traffic(workload, kernel_key):
-    """dram bytes (read+write) per launch of the dominant kernel from the committed
+    """dram bytes (read+write) per launch of the dominant kernel from an
     ncu --set full capture (profiles/traffic.json) -- only when that capture was taken on THIS
     workload and kernel; otherwise null (a constant from another run is not a measurement)."""
     p = os.path.join(ROOT, "profiles", "traffic.json")

@@ -1,6 +1,6 @@
-"""cfmmrouter.jl_b200 -- B200-native dual-decomposition inner loop of
+"""cfmmrouter.jl_b200 -- GPU-native dual-decomposition inner loop of
 CFMMRouter.jl: the per-pool find_arb! sweep and the Ψ/acc folds of route!'s
-L-BFGS-B callback run as hand-written sm_100a CUDA kernels behind the C ABI of
+L-BFGS-B callback run as hand-written sm_90a (H100) CUDA kernels behind the C ABI of
 include/cfmm_b200.h; this package is the Python host-side mirror of the
 reference's Router / route! / CFMM / Objective interface.
 

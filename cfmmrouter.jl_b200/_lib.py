@@ -99,7 +99,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; "
-            "g.build()'` (nvcc, sm_100a).  There is no CPU fallback for the sweep.")
+            "g.build()'` (nvcc, sm_90a).  There is no CPU fallback for the sweep.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SYMBOLS.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export it

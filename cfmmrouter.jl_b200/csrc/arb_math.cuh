@@ -261,7 +261,7 @@ constexpr int kTickStride = 8;
 // The tick a walk STARTS in (the current tick) is additionally stored per pool, in pool order,
 // as four coalesced double2 streams (Univ3First): (k, R_1+α), (R_2+β, current_price),
 // (δmax↑, R_2), (δmax↓, R_1) -- 64 bytes per pool, every byte of which a trading pool uses.
-// ncu on the CSR-only form: 170 MB of DRAM reads against 48 MB algorithmic on config 4,
+// On the CSR-only form the DRAM reads are several times the 48 MB algorithmic of config 4,
 // because one touched 32-byte sector of a 128-byte tick costs a 128-byte fetch, behind a
 // dependent load (tick_off -> record).  Most walks end in the tick they start in: they now read
 // pool-indexed streams only, and the CSR is touched by the walks that cross a boundary.
@@ -321,10 +321,10 @@ __device__ __forceinline__ Trade univ3_arb(const double* __restrict__ td, int n_
   const auto record = [&](int i) { return reinterpret_cast<const double2*>(rec0 + (size_t)(i - 1) * 4); };
   // The walk is a chain of dependent record loads (tick i+1 is only visited once tick i is fully
   // consumed): the NEXT tick's first sector is requested before this tick's sqrt / div chain
-  // starts, so its latency overlaps the arithmetic (ncu: 60 % of the stall samples sat on these
-  // loads).  A prefetched record that is never visited costs one 32-byte sector.  (Requesting it
-  // only when a two-multiply estimate says the first tick will be consumed was measured: fewer
-  // bytes, 40.9 us against 36.1 us on config 4 -- the latency matters, the bytes do not.)
+  // starts, so its latency overlaps the arithmetic (most stall samples sat on these loads).  A
+  // prefetched record that is never visited costs one 32-byte sector.  (Requesting it only when a
+  // two-multiply estimate says the first tick will be consumed was slower despite fewer bytes:
+  // the latency matters, the bytes do not.)
   double2 a_next = make_double2(0.0, 0.0), b_next = a_next;
   const auto prefetch = [&](int i) {
     if (in_range(i)) {

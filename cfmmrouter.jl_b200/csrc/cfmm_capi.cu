@@ -1,4 +1,4 @@
-// cfmm_capi.cu -- libcfmm_b200.so: C ABI (include/cfmm_b200.h) over the sm_100a
+// cfmm_capi.cu -- libcfmm_b200.so: C ABI (include/cfmm_b200.h) over the sm_90a
 // sweep kernels.  Host side of the drop-in boundary: pool ingest, token sort,
 // SoA upload, sweep orchestration, trade read-back, multi-GPU exchange set-up.
 //
@@ -154,7 +154,7 @@ struct cfmm_ctx {
   // buffers and copied from there (DMA at link rate, overlapped with the next block's gather)
   void* h_bounce[2] = {nullptr, nullptr};
   cudaEvent_t ev_bounce[2] = {nullptr, nullptr};
-  int sm_count = 148;
+  int sm_count = 132;  // (H100 SXM; cfmm_create reads the device's own count)
   // options
   int exact = 0;
   int debug_skip = 0;  // measurement only (tools/explore.py)
@@ -174,7 +174,7 @@ struct cfmm_ctx {
   int fused_exchange = 1;         // product-only sets: run the peer exchange in the sweep kernel's tail
   int grid_waves = -1;            // first-generation kernel: waves of CTAs (-1 = 1; 0 = one CTA per 512 pools; see launch_sweep)
   int exchange_protocol = 0;      // 0 = by world size, 1 = LL one-shot, 2 = LL two-shot, 3 = direct 8-byte push (peer_exchange.cuh)
-  int coop_launch = 0;            // fused exchange: launch the sweep kernel cooperatively (measured at N = 2: +4 to +8 us per step)
+  int coop_launch = 0;            // fused exchange: launch the sweep kernel cooperatively
   int exchange_bypass = 0;        // 1 = sweeps return this rank's partial [Ψ; acc] (no exchange); every rank must agree
   cfmm::FusedExchange fx_pending; // set by enqueue_sweep when the next TMA launch must carry the exchange
   int blocks_per_sm = 0;  // 0 = occupancy-derived
@@ -603,7 +603,7 @@ int launch_sweep(cfmm_ctx* ctx, int ptype, const P& pools, PoolSet& s,
   const int64_t per_block = (int64_t)cfmm::kSweepThreads * U;
   const int64_t m_all = s.m_padded;  // includes the zero-trade padding pools, if any
   int64_t blocks = (m_all + per_block - 1) / per_block;
-  // persistent-style grid: one wave of resident CTAs (148 SMs x occupancy)
+  // persistent-style grid: one wave of resident CTAs (SM count x occupancy)
   int& occ = ctx->occupancy[mat ? reinterpret_cast<const void*>(&cfmm::sweep_kernel<P, true, U>)
                                  : reinterpret_cast<const void*>(&cfmm::sweep_kernel<P, false, U>)];
   if (occ == 0) {
@@ -617,8 +617,8 @@ int launch_sweep(cfmm_ctx* ctx, int ptype, const P& pools, PoolSet& s,
   }
   const int per_sm = ctx->blocks_per_sm > 0 && ctx->blocks_per_sm < occ ? ctx->blocks_per_sm : occ;
   // grid_waves: 1 (default) = one wave of resident CTAs striding over the pools; 0 = one CTA per
-  // 512 pools, handed out by the hardware block scheduler (measured on UniV3, whose tick walks
-  // make the work per pool uneven: 47.0 us against 45.2 us for the strided wave -- kept as a knob)
+  // 512 pools, handed out by the hardware block scheduler (an alternative for UniV3, whose tick
+  // walks make the work per pool uneven -- kept as a knob)
   const int waves = ctx->grid_waves >= 0 ? ctx->grid_waves : 1;
   const int64_t cap = (int64_t)ctx->sm_count * per_sm * (waves > 0 ? waves : 1);
   if (waves > 0 && blocks > cap) blocks = cap;

@@ -18,8 +18,7 @@
 // replicated L-BFGS-B drivers stay in lock-step).
 //
 // The first version of this file (flag + pull over peer loads, system fences)
-// measured 24 us per exchange at 2 GPUs against ~15 us for ncclAllReduce; see
-// DESIGN.md for the numbers of this one.
+// was slower than ncclAllReduce; the push protocols below replaced it.
 //
 // Receive areas are double-buffered by epoch parity.  A rank pushes epoch e+2
 // only after finishing exchange e+1, i.e. after receiving every peer's e+1
@@ -232,7 +231,7 @@ __global__ void __launch_bounds__(kExchangeThreads)
 // slot is written again two exchanges later, which the writer cannot start before this rank
 // has finished the next exchange (it needs this rank's contribution), i.e. after this kernel:
 // the reset is never overtaken.  Per rank (W-1)·len·8 bytes leave over NVLink (2.8 MB at W = 8,
-// n = 50k: ~3 us of wire time) against two dependent hops of the two-shot LL form.
+// n = 50k) against two dependent hops of the two-shot LL form.
 constexpr unsigned long long kDirectEmpty = ~0ull;
 __device__ __forceinline__ void st_u64_sys(unsigned long long* p, unsigned long long v) {
   asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
@@ -323,9 +322,9 @@ class PeerExchange {
   const std::string& error() const { return err_; }
   int launches_per_reduce() const { return 1; }
   // protocol: 1 = LL one-shot, 2 = LL two-shot, 3 = direct; anything else = by world size: the
-  // direct push up to 4 ranks, LL two-shot beyond (measured on B200 / NVSwitch, 10M pools per GPU,
-  // us per step: N=2 60.6 / 61.5 (LL1) / 62.3 (LL2); N=4 63.1 / - / 64.3; N=8 68.9 / 74.9 / 66.1 --
-  // the bytes a rank sends cost ~2.5 us per MB here, more than the second hop beyond 4 ranks)
+  // direct push up to 4 ranks, LL two-shot beyond: the one-hop push sends (W-1)x the bytes of the
+  // two-shot form, and beyond 4 ranks those bytes cost more than the second hop on an NVSwitch
+  // system.  The crossover has not been re-measured on H100; exchange_protocol overrides it.
   void force_mode(int mode) { mode_ = mode >= 1 && mode <= 3 ? mode : (world_ <= 4 ? 3 : 2); }
   int mode() const { return mode_; }
   // fused use: the sweep kernel itself runs the exchange body; returns the epoch to tag with

@@ -181,7 +181,7 @@ inline PoolLayout build_pool_layout(const int64_t* Ai, int64_t m, int64_t n_toke
   if (symmetric && orient != 0) {
     deg = token_degrees(Ai, m, n_tokens);
     // hub detection: some token sits in far more pools than the average token.
-    // On uniform graphs orientation only perturbs the layout (measured -2.6 %),
+    // On uniform graphs orientation only perturbs the layout (it was slightly slower),
     // so in auto mode it is applied to skewed graphs only.
     int64_t max_deg = 0;
     for (int64_t d : deg) max_deg = d > max_deg ? d : max_deg;

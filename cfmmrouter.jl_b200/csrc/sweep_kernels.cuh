@@ -1,4 +1,4 @@
-// sweep_kernels.cuh -- the dual-gradient sweep kernels (sm_100a).
+// sweep_kernels.cuh -- the dual-gradient sweep kernels (sm_90a).
 //
 // One launch per pool type evaluates find_arb! for every pool of that type at
 // the current dual price ν (src/router.jl:38-42) and folds the result into

@@ -1,5 +1,5 @@
 /*
- * cfmm_b200.h -- C ABI of libcfmm_b200.so: the B200-native replacement for the
+ * cfmm_b200.h -- C ABI of libcfmm_b200.so: the H100-native replacement for the
  * dual-decomposition inner loop of CFMMRouter.jl (reference @ 5932e42).
  *
  * The reference has no FFI; the seam this ABI fills is INSIDE route!
@@ -219,8 +219,7 @@ int cfmm_solve(cfmm_ctx *ctx, const double *lin, const double *lower, const doub
  *                      grid barrier is resident, or fails the launch); 0 (default) = plain launch,
  *                      residency follows from the occupancy query that sizes the persistent grid,
  *                      and a barrier that cannot complete ends in CFMM_ERR_COMM after the poll
- *                      bound instead of hanging.  Measured at N = 2 on B200: the cooperative
- *                      launch costs +4 to +8 us per step.
+ *                      bound instead of hanging.
  *   "exchange_bypass"  multi-GPU: 1 = sweeps skip the exchange and return this rank's partial
  *                      [psi ; acc] (verification; every rank must set it alike).
  *   "exchange_protocol" multi-GPU: how [psi ; acc] is summed over NVLink peer memory: 3 = direct
@@ -245,8 +244,9 @@ int cfmm_solve(cfmm_ctx *ctx, const double *lin, const double *lower, const doub
  *                      kernel too (48-byte records, same fixed-point slice); 0 = first-generation
  *                      kernel.
  *   "balance"          TMA kernel: 1 (default) = every CTA's chunk range is sized by its measured
- *                      speed (SMs differ by ~15 %; durations are fed back through mapped pinned
- *                      memory and the range table is re-derived between launches); 0 = even split.
+ *                      speed (durations are fed back through device memory and an occasional
+ *                      asynchronous copy, and the range table is re-derived between launches);
+ *                      0 = even split.
  *   "trace"            1 = TMA sweeps record per-CTA phase timestamps (cfmm_debug_read_trace).
  *   "profile"          N = time the next N kernel launches (cfmm_profile_read). */
 int cfmm_set_option(cfmm_ctx *ctx, const char *key, int64_t value);

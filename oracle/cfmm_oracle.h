@@ -3,7 +3,7 @@
  *
  * A plain-C restatement of the arithmetic on CFMMRouter.jl's dual-decomposition
  * hot path (reference @ 5932e42, v0.3.1).  Every function cites the reference
- * file:line it follows (paths relative to /root/reference).
+ * file:line it follows (paths relative to the reference tree).
  *
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl
  * reference legs may load this library; the product path (libcfmm_b200.so)

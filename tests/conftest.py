@@ -10,13 +10,13 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     _ensure_built()
 
 
 def _ensure_built():
     """A fresh checkout has no build artefacts (they are git-ignored): build the
-    product library (nvcc cross-compiles for sm_100a without a GPU) and the oracle
+    product library (nvcc cross-compiles for sm_90a without a GPU) and the oracle
     once, exactly as __graft_entry__.build() does."""
     import shutil
     import subprocess

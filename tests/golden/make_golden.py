@@ -2,7 +2,7 @@
 closed forms on the hot path, used to pin the CPU oracle independently of any
 floating-point evaluation order.
 
-Formulas restated from the reference (paths relative to /root/reference):
+Formulas restated from the reference (paths relative to the reference tree):
   ProductTwoCoin        src/cfmms.jl:125-126, 130-140
   GeometricMeanTwoCoin  src/cfmms.jl:180-181, 185-196
   UniV3                 src/cfmms.jl:251-259, 294-313, 321-337, 339-395

@@ -27,7 +27,7 @@ def test_roofline_object_single_kernel_step():
     r = bench.roofline_object(prof, pt, 67.5, 1000, 1000, "product", 10_000_000, 320e6, 6576.1,
                               "measured", "config5_10M_product_50k_tokens", False)
     assert r["bound"] == "hbm" and r["unit"] == "GB/s" and r["kernel"].startswith("product_sweep_tma")
-    # traffic: only from an ncu capture of THIS kernel on THIS workload (profiles/traffic.json), else null
+    # traffic: only from an ncu capture of THIS kernel on THIS workload (profiles/traffic.json, if present), else null
     assert r["traffic"] == bench.read_traffic("config5_10M_product_50k_tokens", "product_sweep_tma")
     assert bench.read_traffic("config2_100k_product_1k_tokens", "sweep_kernel_univ3") is None
     assert r["l2_state"] == "inputs larger than L2"

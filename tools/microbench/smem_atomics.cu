@@ -1,6 +1,6 @@
 // Microbenchmark: cost of accumulating one value per "pool" into a 1600-slot shared slice
 // with random slots, for the candidate primitives of the Ψ[b] accumulation.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o smem_atomics smem_atomics.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o smem_atomics smem_atomics.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>
@@ -70,14 +70,16 @@ __global__ void __launch_bounds__(THREADS, 2) bench(int iters, double* out, doub
   if (t == 123.456) out[0] = t;
 }
 
+static int g_grid = 0;  // two CTAs per SM, as the sweep kernel runs
+
 template <int MODE>
 float run(int iters, double* out, double* gpsi, int n_tokens) {
   cudaEvent_t a, b;
   cudaEventCreate(&a); cudaEventCreate(&b);
-  bench<MODE><<<296, THREADS>>>(iters / 10, out, gpsi, n_tokens);
+  bench<MODE><<<g_grid, THREADS>>>(iters / 10, out, gpsi, n_tokens);
   cudaDeviceSynchronize();
   cudaEventRecord(a);
-  bench<MODE><<<296, THREADS>>>(iters, out, gpsi, n_tokens);
+  bench<MODE><<<g_grid, THREADS>>>(iters, out, gpsi, n_tokens);
   cudaEventRecord(b);
   cudaEventSynchronize(b);
   float ms; cudaEventElapsedTime(&ms, a, b);
@@ -87,8 +89,12 @@ float run(int iters, double* out, double* gpsi, int n_tokens) {
 int main() {
   double *out, *gpsi; const int n_tokens = 50000;
   cudaMalloc(&out, 8); cudaMalloc(&gpsi, 8 * n_tokens); cudaMemset(gpsi, 0, 8 * n_tokens);
+  int sms = 0, khz = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);  // maximum SM clock
+  g_grid = 2 * sms;
   const int iters = 2000;
-  const double ops = 296.0 * THREADS * iters;
+  const double ops = (double)g_grid * THREADS * iters;
   const char* names[] = {"0 LDS only", "1 fp64 atomicAdd (CAS loop) random", "2 3x RED.32 limbs", "3 ATOMS.ADD.32 ret + RED.32 carry",
                          "4 2x RED.32", "5 fp64 CAS conflict-free lanes", "6 global RED.F64 spread 50k", "7 carry scheme conflict-free",
                          "8 2x RED.F32", "9 1x RED.32"};
@@ -99,8 +105,8 @@ int main() {
   ms[6] = run<6>(iters, out, gpsi, n_tokens); ms[7] = run<7>(iters, out, gpsi, n_tokens);
   ms[8] = run<8>(iters, out, gpsi, n_tokens); ms[9] = run<9>(iters, out, gpsi, n_tokens);
   for (int m = 0; m < 10; ++m) {
-    // cycles per warp-op per SM at 1.965 GHz: (ms*1e-3*1.965e9) / (ops/32/148)
-    const double cyc = ms[m] * 1e-3 * 1.965e9 / (ops / 32.0 / 148.0);
+    // cycles per warp-op per SM at the maximum SM clock: (ms*1e-3*clock) / (ops/32/SMs)
+    const double cyc = ms[m] * 1e-3 * (khz * 1e3) / (ops / 32.0 / sms);
     printf("%-40s %8.3f ms  %7.2f cyc/warp-op/SM  (%.1f us per 10M ops)\n", names[m], ms[m], cyc, ms[m] * 1e3 * 1e7 / ops);
   }
   return 0;
