@@ -99,7 +99,8 @@ struct PoolSet {
   // the fixed-point Ψ[b] slice
   DevBuf<unsigned char> d_packed;
   int packed_mode = -1;        // -1 = stale; else (econ ? 1 : 0) | (fixed ? 2 : 0) | (compact ? 4 : 0)
-  // compact stream: γ dictionary (<= 256 distinct fees) and the per-pool codes (device order)
+  // compact stream: γ dictionary (<= 256 distinct fees) and the per-pool codes (device order);
+  // compact_ok also needs every chunk's first tokens to span less than 2^13
   DevBuf<unsigned short> d_gcode;
   DevBuf<double> d_gtab;       // [256] 1/γ by code, then [256] γ by code
   bool compact_ok = false;
@@ -200,7 +201,7 @@ struct cfmm_ctx {
   const void* pinned_ok[2] = {nullptr, nullptr};  // host pointers already verified as pinned
   int balance = 1;              // 1 = TMA kernel: CTA ranges sized by measured CTA speed (feedback), 0 = even split
   int geomean_tma = 1;          // gradient-only GeometricMean sweeps on the TMA kernel (0: first-generation kernel)
-  int compact_stream = 1;       // ProductTwoCoin, economized math: 24-byte pool records (γ dictionary) when the set allows it
+  int compact_stream = 1;       // ProductTwoCoin, economized math: 20-byte pool records (γ dictionary, chunk-relative a) when the set allows it
   // resident CTAs per SM of every kernel instantiation this context has launched.
   // Per context, not per process: cudaFuncSetAttribute (the > 48 KB dynamic shared
   // memory opt-in) acts on the current device only, and contexts of one process
@@ -407,6 +408,15 @@ int upload_set(cfmm_ctx* ctx, int type) {
   clock.mark("gather + upload gamma, Ai, gidx");
   s.compact_ok = false;
   if (type == CFMM_POOL_PRODUCT && s.tma_ok) {
+    // the compact stream stores a as an offset from its chunk's first a: every chunk's span must
+    // fit the field.  The layout is fixed here and reserve updates do not move a.
+    int64_t max_span = 0;
+#pragma omp parallel for schedule(static) reduction(max : max_span) if (s.n_chunks > (1 << 12))
+    for (int64_t c = 0; c < s.n_chunks; ++c) {
+      const int64_t first = real_before(c * cfmm::kTmaChunk), last = real_before((c + 1) * cfmm::kTmaChunk - 1);
+      const int64_t span = (first < 0 || last < 0) ? 0 : (int64_t)oa[(size_t)last] - (int64_t)oa[(size_t)first];
+      max_span = std::max(max_span, span);
+    }
     // γ dictionary of the compact stream: fees are categorical in practice.  Pass 1 (serial,
     // cheap): the distinct values, through a 1024-slot open-addressing table on the bit pattern;
     // pass 2 (the upload's gather): the codes
@@ -431,7 +441,7 @@ int upload_set(cfmm_ctx* ctx, int type) {
         h = (h + 1) & (kSlots - 1);
       }
     };
-    bool ok = slot_of(1.0, true) >= 0;  // (the padding pools' fee)
+    bool ok = max_span <= cfmm::kMetaMaxSpan && slot_of(1.0, true) >= 0;  // (the padding pools' fee)
     double last = 1.0;
     for (int64_t i = 0; i < m && ok; ++i) {
       const double g = s.gamma[(size_t)i];
@@ -676,7 +686,7 @@ template <int POOL>
 int ensure_packed(cfmm_ctx* ctx, PoolSet& s, bool econ, bool fixed, bool compact, cudaStream_t st) {
   const int mode = (econ ? 1 : 0) | (fixed ? 2 : 0) | (compact ? 4 : 0);
   if (s.packed_mode == mode) return CFMM_OK;
-  const size_t bytes = (size_t)s.n_chunks * (compact ? cfmm::kTmaChunk * cfmm::kTmaCompactPoolBytes : cfmm::tma_chunk_bytes<POOL>());
+  const size_t bytes = (size_t)s.n_chunks * (compact ? cfmm::tma_chunk_bytes_c<POOL, true>() : cfmm::tma_chunk_bytes<POOL>());
   if (s.d_packed.n < bytes) CU_TRY(ctx, s.d_packed.alloc((size_t)s.n_chunks * cfmm::tma_chunk_bytes<POOL>()));
   const int threads = 256;
   if (compact) {

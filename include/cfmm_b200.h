@@ -237,9 +237,11 @@ int cfmm_solve(cfmm_ctx *ctx, const double *lin, const double *lower, const doub
  *   "geomean_log2"     gradient-only GeometricMean sweeps take the power as exp2(e*log2 t)
  *                      (1, default; <= 12 ulp over the admitted range, validated against
  *                      pow on hardware) or as pow (0).
- *   "compact_stream"   1 (default) = economized ProductTwoCoin sweeps stream 24-byte pool records
- *                      (fee through a dictionary of <= 256 distinct values, second token relative
- *                      to its bucket) when the pool set allows it; 0 = 32-byte records.
+ *   "compact_stream"   1 (default) = economized ProductTwoCoin sweeps stream 20-byte pool records
+ *                      (fee through a dictionary of <= 256 distinct values, first token relative
+ *                      to its 96-pool chunk's first, second token relative to its bucket) when the
+ *                      pool set allows it (<= 256 fees, every chunk's first tokens spanning < 8192);
+ *                      0 = 32-byte records.
  *   "geomean_tma"      1 (default) = gradient-only GeometricMeanTwoCoin sweeps run on the TMA
  *                      kernel too (48-byte records, same fixed-point slice); 0 = first-generation
  *                      kernel.
