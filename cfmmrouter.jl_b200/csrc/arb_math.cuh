@@ -189,11 +189,11 @@ __device__ __forceinline__ Trade geomean_arb(double R1, double R2, double w1,
 //     Δ_tendered = r2·(u − 1)/γ ,   Λ_received = r1·(1 − u/t)
 // which is src/cfmms.jl:180-181 with r2 and r1 factored out of the powers
 // (1/(e+1) = w_received/(w1+w2)).  One pow instead of four.
-// LOG2EXP2: u = exp2(ex·log2(ratio)) instead of pow(ratio, ex).  Checked on the CPU
-// against 40-digit arithmetic over the whole admitted range (|log2 ratio| <= 64,
-// ex in (0.04, 0.96)): <= 0.8 ulp for |log2 ratio| <= 1, <= 12 ulp at the extremes
-// (the absolute error of the product ex·log2 grows with |log2 ratio|).  Staged for the
-// next round: not yet run on hardware, reachable only through option "geomean_log2".
+// LOG2EXP2: u = exp2(ex·log2(ratio)) instead of pow(ratio, ex); the default of gradient-only
+// sweeps (option "geomean_log2" = 1, on this kernel and on the TMA kernel).  The absolute error
+// of ex·log2(ratio) grows with |log2 ratio| (<= 64 in the admitted range) and becomes a relative
+// error of u.  Measured per flow on an H100 80GB HBM3 against extended precision, in units of
+// eps·(R + γ|flow|)/γ: <= 1.4 + 2·|ex·log2 ratio|, 38.4 at most (tests/test_gpu_pool_readout.py).
 template <bool LOG2EXP2 = false>
 __device__ __forceinline__ Trade geomean_arb_econ(double R1, double R2, double w1,
                                                   double w2, double g, double v1,
