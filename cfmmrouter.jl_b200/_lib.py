@@ -59,6 +59,7 @@ SYMBOLS = {
     "cfmm_get_trades": (C.c_int, [_ctx, _dp, _dp]),
     "cfmm_solve": (C.c_int, [_ctx, _dp, _dp, _dp, _dp, C.POINTER(SolveOpts), _dp, C.POINTER(SolveInfo)]),
     "cfmm_update_reserves": (C.c_int, [_ctx, C.c_int, C.c_int64, C.c_int64, _dp]),
+    "cfmm_update_univ3": (C.c_int, [_ctx, C.c_int64, C.c_int64, _dp, _dp]),
     "cfmm_apply_trades": (C.c_int, [_ctx]),
     "cfmm_set_option": (C.c_int, [_ctx, C.c_char_p, C.c_int64]),
     "cfmm_last_sweep_ms": (C.c_int, [_ctx, C.POINTER(C.c_float)]),

@@ -244,8 +244,9 @@ __device__ __forceinline__ Trade geomean_arb_econ(double R1, double R2, double w
 
 // Every tick's BoundedProduct (src/cfmms.jl:272-278, built by compute_at_tick
 // :294-313) depends only on pool state (liquidity, tick prices, current price),
-// never on ν.  It is therefore evaluated ONCE at cfmm_finalize, on the host,
-// with the same IEEE operations in the same order, and stored per pool as two
+// never on ν.  It is therefore evaluated only when that state changes (cfmm_finalize,
+// cfmm_update_univ3, cfmm_apply_trades: the rebuild kernels of univ3_state.cuh), with
+// the same IEEE operations in the same order, and stored per pool as two
 // DIRECTION BLOCKS of one 32-byte record per tick (kTickStride doubles per tick in all):
 //   "upper" walk (towards lower prices), block 0, tick i:  [k, R_1+α, δmax↑ = k/β − (R_1+α), R_2]
 //   "lower" walk (the flipped pool, :289), block 1, tick i: [k, R_2+β, δmax↓ = k/α − (R_2+β), R_1]

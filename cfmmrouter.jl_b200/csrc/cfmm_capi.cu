@@ -28,6 +28,7 @@
 #include "sweep_kernels.cuh"
 #include "product_tma.cuh"
 #include "solver.cuh"
+#include "univ3_state.cuh"
 
 namespace {
 
@@ -87,6 +88,9 @@ struct PoolSet {
   DevBuf<double2> d_first[4];             // univ3: the current tick of every pool, four streams (arb_math.cuh)
   DevBuf<int2> d_Ai, d_tick;
   DevBuf<int64_t> d_gidx;                 // sorted position -> global insertion index
+  DevBuf<double> d_lower, d_liq;          // univ3: raw tick data, CSR in device order (univ3_state.cuh)
+  std::vector<double> first_lower;        // univ3: T₁ = lower_ticks[1] per pool (insertion order)
+  std::vector<int64_t> n_ticks;           // univ3: tick count per pool (insertion order)
   int64_t total_ticks = 0;
   int64_t m_padded = 0;        // product: arrays padded to whole 96-pool chunks, per b-bucket
   bool in_fast_range = false;  // every R, γ in [2^-100, 2^100] and γ <= 1
@@ -127,6 +131,7 @@ struct PoolSet {
     d_gam.release(); d_tickdata.release();
     for (auto& f : d_first) f.release();
     d_Ai.release(); d_tick.release(); d_gidx.release();
+    d_lower.release(); d_liq.release();
     d_packed.release(); d_inv_scale.release(); d_tok_sum.release(); d_gcode.release(); d_gtab.release();
     if (h_dur) cudaFreeHost(h_dur);
     h_dur = nullptr;
@@ -150,6 +155,7 @@ struct cfmm_ctx {
   cudaEvent_t ev_order = nullptr;      // orders work across a change of stream
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   DevBuf<double> d_nu;  // n
+  DevBuf<double> d_nu_mat;  // n, UniV3 sets only: ν of the last materialising sweep (cfmm_apply_trades)
   double* h_stage = nullptr;   // pinned, n+1
   // finalize uploads: device-order arrays are gathered block by block into two pinned bounce
   // buffers and copied from there (DMA at link rate, overlapped with the next block's gather)
@@ -354,6 +360,41 @@ cudaError_t upload_streamed(cfmm_ctx* ctx, DevBuf<T>& dst, int64_t count, Fill f
   return cudaSuccess;
 }
 
+cfmm::Univ3State univ3_state(PoolSet& s) {
+  cfmm::Univ3State u;
+  u.f0 = s.d_first[0].p;
+  u.f1 = s.d_first[1].p;
+  u.f2 = s.d_first[2].p;
+  u.f3 = s.d_first[3].p;
+  u.tick = s.d_tick.p;
+  u.tickdata = s.d_tickdata.p;
+  u.lower = s.d_lower.p;
+  u.liq = s.d_liq.p;
+  u.m = s.m;
+  u.total_ticks = s.total_ticks;
+  return u;
+}
+
+// Rebuild the derived UniV3 state (univ3_state.cuh) of the pools d_pos[0..count) (d_pos ==
+// nullptr: all pools), whose ticks d_cum lists (n_ticks in all), after storing the optional new
+// prices / liquidities (device arrays in listing order).  Enqueued on the context stream.
+cudaError_t univ3_rebuild(cfmm_ctx* ctx, PoolSet& s, const int64_t* d_pos, const int64_t* d_cum, int64_t count,
+                          int64_t n_ticks, const double* d_price, const double* d_liq, bool new_tick) {
+  const cfmm::Univ3State u = univ3_state(s);
+  const int threads = 256;
+  if (count > 0 && (new_tick || d_price)) {
+    cfmm::univ3_current_tick_kernel<<<(unsigned)((count + threads - 1) / threads), threads, 0, ctx->stream>>>(
+        u, d_pos, d_price, count);
+    ctx->launches++;
+  }
+  if (n_ticks > 0) {
+    cfmm::univ3_ticks_kernel<<<(unsigned)((n_ticks + threads - 1) / threads), threads, 0, ctx->stream>>>(
+        u, d_pos, d_cum, count, n_ticks, d_liq);
+    ctx->launches++;
+  }
+  return cudaGetLastError();
+}
+
 int upload_set(cfmm_ctx* ctx, int type) {
   PoolSet& s = ctx->sets[type];
   if (s.m == 0) return CFMM_OK;
@@ -495,58 +536,41 @@ int upload_set(cfmm_ctx* ctx, int type) {
     }));
   }
   if (type == CFMM_POOL_UNIV3) {
-    // compute_at_tick (src/cfmms.jl:294-313) for every tick, once, on the host:
-    // IEEE sqrt / div / mul / sub in the reference's order (see arb_math.cuh)
-    std::vector<double> td;
-    std::vector<double2> first[4];
-    for (auto& f : first) f.assign((size_t)m, make_double2(0.0, 0.0));
-    std::vector<int2> tick((size_t)m);
-    td.assign(s.lower.size() * cfmm::kTickStride, 0.0);
-    int64_t n_ticks_total = 0;
+    // the raw tick data goes to the device in device pool order; the tick records and the
+    // current-tick streams are computed there (univ3_state.cuh)
+    std::vector<int64_t> dev_off((size_t)m + 1, 0);
     for (int64_t p = 0; p < m; ++p) {
-      const int64_t i = s.order[(size_t)p];
-      const int64_t b = s.tick_off[(size_t)i], e = s.tick_off[(size_t)i + 1];
-      const double price = s.cp[(size_t)i];
-      first[1][(size_t)p].y = price;
-      // current_tick = searchsortedlast(lower_ticks, current_price; rev=true)
-      // (src/cfmms.jl:235): number of leading ticks >= current_price
-      int cur = 0;
-      while (b + cur < e && s.lower[(size_t)(b + cur)] >= price) ++cur;
-      tick[(size_t)p] = make_int2((int)n_ticks_total, cur);
-      for (int64_t q = b; q < e; ++q) {
-        const int idx = (int)(q - b) + 1;  // 1-based
-        volatile double k = s.liq[(size_t)q];
-        volatile double pplus = s.lower[(size_t)q];                      // tick_high_price :252
-        volatile double pminus = (q + 1 < e) ? s.lower[(size_t)q + 1] : 0.0;  // tick_low_price :255-259
-        volatile double alpha = std::sqrt(k / pplus);
-        volatile double beta = std::sqrt(k * pminus);
-        volatile double pp = idx > cur ? pplus : (idx < cur ? pminus : price);
-        volatile double R1 = std::sqrt(k / pp) - alpha;
-        volatile double R2 = std::sqrt(k * pp) - beta;
-        volatile double ra = R1 + alpha;
-        volatile double rb = R2 + beta;
-        volatile double dmax_up = k / beta - ra;
-        volatile double dmax_dn = k / alpha - rb;
-        // two direction blocks per pool, one 32-byte record per tick in each (arb_math.cuh)
-        const size_t base = (size_t)n_ticks_total * cfmm::kTickStride, nt = (size_t)(e - b), ti = (size_t)(q - b);
-        const double up_rec[4] = {k, ra, dmax_up, R2}, dn_rec[4] = {k, rb, dmax_dn, R1};
-        for (int c = 0; c < 4; ++c) {
-          td[base + ti * 4 + c] = up_rec[c];
-          td[base + nt * 4 + ti * 4 + c] = dn_rec[c];
-        }
-        if (idx == cur) {  // the tick a walk starts in: also per pool, in pool order
-          first[0][(size_t)p] = make_double2(k, ra);
-          first[1][(size_t)p].x = rb;
-          first[2][(size_t)p] = make_double2(dmax_up, R2);
-          first[3][(size_t)p] = make_double2(dmax_dn, R1);
-        }
-      }
-      n_ticks_total += e - b;
+      const int64_t i = order[p];
+      dev_off[(size_t)p + 1] = dev_off[(size_t)p] + (s.tick_off[(size_t)i + 1] - s.tick_off[(size_t)i]);
     }
-    s.total_ticks = n_ticks_total;
-    for (int f = 0; f < 4; ++f) CU_TRY(ctx, s.d_first[f].upload(first[f]));
-    CU_TRY(ctx, s.d_tick.upload(tick));
-    CU_TRY(ctx, s.d_tickdata.upload(td));
+    s.total_ticks = dev_off[(size_t)m];
+    s.first_lower.resize((size_t)m);
+    s.n_ticks.resize((size_t)m);
+    for (int64_t i = 0; i < m; ++i) {
+      s.first_lower[(size_t)i] = s.lower[(size_t)s.tick_off[(size_t)i]];
+      s.n_ticks[(size_t)i] = s.tick_off[(size_t)i + 1] - s.tick_off[(size_t)i];
+    }
+    std::vector<double> lower((size_t)s.total_ticks), liq((size_t)s.total_ticks);
+#pragma omp parallel for schedule(static) if (m > (1 << 14))
+    for (int64_t p = 0; p < m; ++p) {
+      const int64_t i = order[p], b = s.tick_off[(size_t)i], nt = s.n_ticks[(size_t)i];
+      std::copy(s.lower.begin() + b, s.lower.begin() + b + nt, lower.begin() + dev_off[(size_t)p]);
+      std::copy(s.liq.begin() + b, s.liq.begin() + b + nt, liq.begin() + dev_off[(size_t)p]);
+    }
+    CU_TRY(ctx, s.d_lower.upload(lower));
+    CU_TRY(ctx, s.d_liq.upload(liq));
+    CU_TRY(ctx, upload_streamed(ctx, s.d_tick, m, [&](int64_t p) { return make_int2((int)dev_off[(size_t)p], 0); }));
+    CU_TRY(ctx, upload_streamed(ctx, s.d_first[1], m, [&](int64_t p) {
+      return make_double2(0.0, s.cp[(size_t)order[p]]);
+    }));
+    for (int f : {0, 2, 3}) {
+      CU_TRY(ctx, s.d_first[f].alloc((size_t)m));
+      CU_TRY(ctx, cudaMemsetAsync(s.d_first[f].p, 0, (size_t)m * sizeof(double2), ctx->stream));
+    }
+    CU_TRY(ctx, s.d_tickdata.alloc((size_t)s.total_ticks * cfmm::kTickStride));
+    CU_TRY(ctx, univ3_rebuild(ctx, s, nullptr, nullptr, m, s.total_ticks, nullptr, nullptr, true));
+    CU_TRY(ctx, ctx->d_nu_mat.alloc((size_t)ctx->n_tokens));
+    clock.mark("univ3 tick data: upload + device rebuild");
   }
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // the bounce copies read the staging below
   clock.mark("other arrays, drain");
@@ -939,6 +963,10 @@ int enqueue_sweep(cfmm_ctx* ctx, const double* d_v, double* d_dst, bool mat,
       cfmm::Univ3Pools p{s.d_first[0].p, s.d_first[1].p, s.d_first[2].p, s.d_first[3].p, s.d_gam.p, s.d_Ai.p, s.d_tick.p,
                          s.d_tickdata.p, s.m_padded, (int)s.total_ticks};
       if ((rc = launch_sweep(ctx, PT, p, s, d_v, d_psi, mat, st)) != CFMM_OK) return rc;
+      // cfmm_apply_trades moves UniV3 prices by the ν of the last materialising sweep: keep it,
+      // since the caller's d_v (and the context's own ν buffer) may be overwritten before then
+      if (mat) CU_TRY(ctx, cudaMemcpyAsync(ctx->d_nu_mat.p, d_v, (size_t)ctx->n_tokens * sizeof(double),
+                                           cudaMemcpyDeviceToDevice, st));
     }
   }
   if (ctx->zero_pending) {  // no kernel ran (empty pool set): clear the other accumulator here
@@ -1049,6 +1077,7 @@ void cfmm_destroy(cfmm_ctx* ctx) {
     if (e) cudaEventDestroy(e);
   for (auto& s : ctx->sets) s.release();
   ctx->d_nu.release();
+  ctx->d_nu_mat.release();
   ctx->d_grid_done.release();
   ctx->d_trace.release();
   ctx->d_accum[0].release();
@@ -1739,16 +1768,71 @@ int cfmm_update_reserves(cfmm_ctx* ctx, int type, int64_t first, int64_t count,
   return CFMM_OK;
 }
 
+namespace {
+
+// Store new prices / liquidities (host arrays in listing order, either may be NULL) of the UniV3
+// pools at device positions pos and rebuild their derived state on the device; synchronous.
+int univ3_update_listed(cfmm_ctx* ctx, PoolSet& s, const std::vector<int64_t>& pos, const double* price,
+                        const double* liq, bool new_tick) {
+  const int64_t count = (int64_t)pos.size();
+  std::vector<int64_t> cum((size_t)count + 1, 0);
+  for (int64_t j = 0; j < count; ++j)
+    cum[(size_t)j + 1] = cum[(size_t)j] + s.n_ticks[(size_t)s.order[(size_t)pos[(size_t)j]]];
+  const int64_t n_ticks = cum[(size_t)count];
+  DevBuf<int64_t> d_pos, d_cum;
+  DevBuf<double> d_price, d_liq;
+  CU_TRY(ctx, d_pos.upload(pos));
+  CU_TRY(ctx, d_cum.upload(cum));
+  if (price) {
+    CU_TRY(ctx, d_price.alloc((size_t)count));
+    CU_TRY(ctx, DevBuf<double>::copy_in(d_price.p, price, (size_t)count * sizeof(double)));
+  }
+  if (liq && n_ticks > 0) {
+    CU_TRY(ctx, d_liq.alloc((size_t)n_ticks));
+    CU_TRY(ctx, DevBuf<double>::copy_in(d_liq.p, liq, (size_t)n_ticks * sizeof(double)));
+  }
+  CU_TRY(ctx, univ3_rebuild(ctx, s, d_pos.p, d_cum.p, count, n_ticks, d_price.p, d_liq.p, new_tick));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return CFMM_OK;
+}
+
+}  // namespace
+
+int cfmm_update_univ3(cfmm_ctx* ctx, int64_t first, int64_t count, const double* current_price,
+                      const double* liquidity) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  PoolSet& s = ctx->sets[CFMM_POOL_UNIV3];
+  if (first < 0 || count < 0 || first + count > s.m)
+    return fail(ctx, CFMM_ERR_INVALID, "update_univ3: range [%lld, %lld) outside 0..%lld",
+                (long long)first, (long long)(first + count), (long long)s.m);
+  if (count == 0 || (!current_price && !liquidity)) return CFMM_OK;
+  // validated like cfmm_add_univ3, all before any change: a rejected call changes no pool
+  if (current_price)
+    for (int64_t j = 0; j < count; ++j)
+      if (!(s.first_lower[(size_t)(first + j)] >= current_price[j]))
+        return fail(ctx, CFMM_ERR_INVALID,
+                    "univ3 pool %lld: current_price above the first lower tick "
+                    "(current_tick == 0; BoundsError in the reference)",
+                    (long long)(first + j));
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  ctx->state_version++;
+  if (s.pos_of.empty()) {
+    s.pos_of.resize((size_t)s.m);
+    for (int64_t p = 0; p < s.m_padded; ++p)
+      if (s.order[(size_t)p] >= 0) s.pos_of[(size_t)s.order[(size_t)p]] = p;
+  }
+  std::vector<int64_t> pos(s.pos_of.begin() + first, s.pos_of.begin() + first + count);
+  return univ3_update_listed(ctx, s, pos, current_price, liquidity, current_price != nullptr);
+}
+
 int cfmm_apply_trades(cfmm_ctx* ctx) {
   int rc = ready(ctx);
   if (rc != CFMM_OK) return rc;
   if (!ctx->has_trades)
     return fail(ctx, CFMM_ERR_STATE,
                 "no materialising sweep has run (call cfmm_sweep with materialize=1)");
-  if (ctx->sets[CFMM_POOL_UNIV3].m > 0)
-    return fail(ctx, CFMM_ERR_INVALID,
-                "cfmm_apply_trades: UniV3 pools have no explicit reserves (R + γΔ − Λ is defined for "
-                "ProductTwoCoin / GeometricMeanTwoCoin only)");
   CU_TRY(ctx, cudaSetDevice(ctx->device));
   ctx->state_version++;
   if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
@@ -1773,6 +1857,28 @@ int cfmm_apply_trades(cfmm_ctx* ctx) {
     if (s.tma_ok) {
       int rc2 = refresh_scale(ctx, s);
       if (rc2 != CFMM_OK) return rc2;
+    }
+  }
+  PoolSet& u = ctx->sets[CFMM_POOL_UNIV3];
+  if (u.m > 0) {
+    // new prices from the kept ν (univ3_move_kernel), then the state of the pools that moved
+    DevBuf<int64_t> moved;
+    DevBuf<unsigned long long> n_moved;
+    CU_TRY(ctx, moved.alloc((size_t)u.m));
+    CU_TRY(ctx, n_moved.alloc(1));
+    CU_TRY(ctx, cudaMemsetAsync(n_moved.p, 0, sizeof(unsigned long long), ctx->stream));
+    const int threads = 256;
+    cfmm::univ3_move_kernel<<<(unsigned)((u.m + threads - 1) / threads), threads, 0, ctx->stream>>>(
+        univ3_state(u), u.d_gam.p, u.d_Ai.p, ctx->d_nu_mat.p, moved.p, n_moved.p);
+    ctx->launches++;
+    unsigned long long h = 0;
+    CU_TRY(ctx, cudaMemcpyAsync(&h, n_moved.p, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    if (h > 0) {
+      std::vector<int64_t> pos((size_t)h);
+      CU_TRY(ctx, cudaMemcpy(pos.data(), moved.p, (size_t)h * sizeof(int64_t), cudaMemcpyDeviceToHost));
+      std::sort(pos.begin(), pos.end());  // (the list order is the atomics'; sorted, the rebuild reads in device order)
+      if ((rc = univ3_update_listed(ctx, u, pos, nullptr, nullptr, true)) != CFMM_OK) return rc;
     }
   }
   return CFMM_OK;

@@ -1,0 +1,170 @@
+// univ3_state.cuh -- the device-resident state of UniV3 pools (sm_90a): the per-tick
+// BoundedProduct records the sweep walks read, rebuilt from the raw tick data (lower tick
+// prices, liquidity, current price) at cfmm_finalize, on cfmm_update_univ3 and on
+// cfmm_apply_trades.  This is the library's only implementation of compute_at_tick
+// (src/cfmms.jl:294-313).
+//
+// Raw state, kept on the device in the CSR order of the tick records (device pool order):
+//   lower, liq : double[total_ticks]      16 B per tick
+//   f1[p].y    : the pool's current price (the same word the sweep reads it from)
+//   tick[p]    : (tick_off, current_tick 1-based)
+// Derived state, rewritten in place (sweep graphs captured earlier keep valid pointers):
+//   tickdata   : two 32-byte direction records per tick (arb_math.cuh, kTickStride)
+//   f0..f3     : the current tick's records per pool (Univ3First)
+//   tick[p].y  : current_tick
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "arb_math.cuh"
+
+namespace cfmm {
+
+struct Univ3State {
+  double2* f0;          // (k, R_1+α) of the current tick
+  double2* f1;          // (R_2+β, current_price)
+  double2* f2;          // (δmax↑, R_2)
+  double2* f3;          // (δmax↓, R_1)
+  int2* tick;           // (tick_off, current_tick)
+  double* tickdata;     // kTickStride doubles per tick
+  const double* lower;  // CSR, strictly decreasing within a pool
+  double* liq;          // CSR
+  int64_t m;
+  int64_t total_ticks;
+};
+
+__device__ __forceinline__ double univ3_price(const Univ3State& s, int64_t p) {
+  return reinterpret_cast<const double*>(s.f1 + p)[1];
+}
+
+__device__ __forceinline__ int univ3_tick_end(const Univ3State& s, int64_t p) {
+  return p + 1 < s.m ? s.tick[p + 1].x : (int)s.total_ticks;
+}
+
+// current_tick of pools pos[j] (pos == nullptr: pool j), j < count, after an optional price
+// push new_price[j]: searchsortedlast(lower_ticks, price, rev=true) (src/cfmms.jl:235), i.e. the
+// number of leading ticks >= price.  The ticks are strictly decreasing, so the leading run is
+// found by bisection; ties count as >=, a NaN price gives 0 (both as the linear count).
+__global__ void univ3_current_tick_kernel(Univ3State s, const int64_t* __restrict__ pos,
+                                          const double* __restrict__ new_price, int64_t count) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= count) return;
+  const int64_t p = pos ? pos[j] : j;
+  double price;
+  if (new_price) {
+    price = new_price[j];
+    reinterpret_cast<double*>(s.f1 + p)[1] = price;
+  } else {
+    price = univ3_price(s, p);
+  }
+  const int off = s.tick[p].x, nt = univ3_tick_end(s, p) - off;
+  int lo = 0, hi = nt;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (s.lower[off + mid] >= price)
+      lo = mid + 1;
+    else
+      hi = mid;
+  }
+  reinterpret_cast<int*>(s.tick + p)[1] = lo;
+}
+
+// compute_at_tick (src/cfmms.jl:294-313) for every tick of pools pos[j] (pos == nullptr: of all
+// pools), one thread per tick: cum[j] .. cum[j+1]-1 are the listed pools' ticks in listing order
+// (cum == nullptr: the device CSR itself).  new_liq (optional, indexed like the listing) is
+// stored first.  IEEE operations in the reference's order, written as intrinsics because nvcc
+// contracts a*b+c to an FMA by default: the records are bit-identical to compute_at_tick's.
+__global__ void univ3_ticks_kernel(Univ3State s, const int64_t* __restrict__ pos,
+                                   const int64_t* __restrict__ cum, int64_t count, int64_t n_ticks,
+                                   const double* __restrict__ new_liq) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_ticks) return;
+  int64_t p, ti;
+  int off, nt;
+  if (pos) {
+    int64_t lo = 0, hi = count - 1;  // last j with cum[j] <= t
+    while (lo < hi) {
+      const int64_t mid = (lo + hi + 1) >> 1;
+      if (cum[mid] <= t)
+        lo = mid;
+      else
+        hi = mid - 1;
+    }
+    p = pos[lo];
+    ti = t - cum[lo];
+    off = s.tick[p].x;
+    nt = (int)(cum[lo + 1] - cum[lo]);
+  } else {
+    int64_t lo = 0, hi = s.m - 1;  // last pool whose first tick is <= t (every pool has a tick)
+    while (lo < hi) {
+      const int64_t mid = (lo + hi + 1) >> 1;
+      if (s.tick[mid].x <= t)
+        lo = mid;
+      else
+        hi = mid - 1;
+    }
+    p = lo;
+    off = s.tick[p].x;
+    ti = t - off;
+    nt = univ3_tick_end(s, p) - off;
+  }
+  const int64_t q = off + ti;
+  double k;
+  if (new_liq) {
+    k = new_liq[t];
+    s.liq[q] = k;
+  } else {
+    k = s.liq[q];
+  }
+  const double price = univ3_price(s, p);
+  const int cur = s.tick[p].y;
+  const int idx = (int)ti + 1;  // 1-based
+  const double pplus = s.lower[q];                            // tick_high_price :252
+  const double pminus = ti + 1 < nt ? s.lower[q + 1] : 0.0;   // tick_low_price :255-259
+  const double alpha = __dsqrt_rn(__ddiv_rn(k, pplus));
+  const double beta = __dsqrt_rn(__dmul_rn(k, pminus));
+  const double pp = idx > cur ? pplus : (idx < cur ? pminus : price);
+  const double R1 = __dsub_rn(__dsqrt_rn(__ddiv_rn(k, pp)), alpha);
+  const double R2 = __dsub_rn(__dsqrt_rn(__dmul_rn(k, pp)), beta);
+  const double ra = __dadd_rn(R1, alpha);
+  const double rb = __dadd_rn(R2, beta);
+  const double dmax_up = __dsub_rn(__ddiv_rn(k, beta), ra);
+  const double dmax_dn = __dsub_rn(__ddiv_rn(k, alpha), rb);
+  double2* up = reinterpret_cast<double2*>(s.tickdata + (size_t)off * kTickStride + (size_t)ti * 4);
+  double2* dn = reinterpret_cast<double2*>(s.tickdata + (size_t)off * kTickStride + (size_t)(nt + ti) * 4);
+  up[0] = make_double2(k, ra);
+  up[1] = make_double2(dmax_up, R2);
+  dn[0] = make_double2(k, rb);
+  dn[1] = make_double2(dmax_dn, R1);
+  if (idx == cur) {  // the tick a walk starts in: also per pool (the price word of f1 stays)
+    s.f0[p] = make_double2(k, ra);
+    reinterpret_cast<double*>(s.f1 + p)[0] = rb;
+    s.f2[p] = make_double2(dmax_up, R2);
+    s.f3[p] = make_double2(dmax_dn, R1);
+  }
+}
+
+// The post-trade price of every pool (include/cfmm_b200.h, cfmm_apply_trades), from the ν of the
+// last materialising sweep: p = ν[a]/ν[b] and the no-trade band exactly as univ3_arb computes
+// them; the target p/γ (upper walk) or γ·p (lower walk), unchanged if it is NaN or not > 0, else
+// clamped to the first lower tick.  Pools whose price changes get it stored in f1 and are listed.
+__global__ void univ3_move_kernel(Univ3State s, const double* __restrict__ gam, const int2* __restrict__ Ai,
+                                  const double* __restrict__ nu, int64_t* __restrict__ moved,
+                                  unsigned long long* __restrict__ n_moved) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= s.m) return;
+  const double q = univ3_price(s, p), g = gam[p];
+  const int2 ai = Ai[p];
+  const double pr = __ddiv_rn(nu[ai.x], nu[ai.y]);
+  const double lo = __dmul_rn(g, q);
+  if (lo <= pr && pr <= __ddiv_rn(q, g)) return;
+  const double target = pr < lo ? __ddiv_rn(pr, g) : __dmul_rn(g, pr);
+  if (!(target > 0.0)) return;
+  const double t1 = s.lower[s.tick[p].x];
+  const double qn = target < t1 ? target : t1;
+  if (qn == q) return;
+  reinterpret_cast<double*>(s.f1 + p)[1] = qn;
+  moved[atomicAdd(n_moved, 1ull)] = p;
+}
+
+}  // namespace cfmm

@@ -52,6 +52,7 @@ mutable struct B200Router{O,T}
     ctxs::Vector{Ptr{Cvoid}}        # one context per device (multi-GPU: pools sharded in list order)
     shard::Vector{UnitRange{Int}}   # positions of `order` each context holds
     pin::Ptr{Float64}               # pinned staging: ν [n] | ψ [n] | acc [1], per context (n_ctx blocks)
+    vmat::Vector{T}                 # ν of the last materialising sweep (update_reserves! moves UniV3 pools by it)
 end
 
 # One device context holding the pools cfmms[ids] (positions in the caller's list); returns
@@ -135,7 +136,7 @@ function B200Router(objective::O, cfmms::Vector{C}, n_tokens; device::Integer=0,
     Δs = AbstractVector{T}[zeros(T, 2) for _ in cfmms]     # zerotrade, router.jl:23-26
     Λs = AbstractVector{T}[zeros(T, 2) for _ in cfmms]
     r = B200Router{O,T}(objective, convert(Vector{CFMM{T}}, cfmms), Δs, Λs, zeros(T, n_tokens),
-                        ctxs[1], order, ψ, Ref(zero(T)), ctxs, shard, pin)
+                        ctxs[1], order, ψ, Ref(zero(T)), ctxs, shard, pin, zeros(T, n_tokens))
     finalizer(r) do x
         foreach(c -> ccall((:cfmm_destroy, LIB), Cvoid, (Ptr{Cvoid},), c), x.ctxs)
         ccall((:cfmm_host_free, LIB), Cvoid, (Ptr{Cvoid},), x.pin)
@@ -165,6 +166,7 @@ function sweep!(r::B200Router{O,T}, v::AbstractVector{T}; materialize::Bool=fals
     foreach(k -> chk(r.ctxs[k], rcs[k]), 1:W)
     r.acc[] = unsafe_load(r.pin, 2n + 1)            # every context holds the bitwise-identical sum
     if materialize
+        r.vmat .= v
         for k in 1:W
             mk = length(r.shard[k])
             D = Vector{Float64}(undef, 2mk); L = Vector{Float64}(undef, 2mk)
@@ -200,6 +202,7 @@ function route!(r::B200Router; v=nothing, verbose=false, m=5, factr=1e1, pgtol=1
         GC.@preserve lin lo up v chk(r.ctx, ccall((:cfmm_solve, LIB), Cint,
             (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ref{SolveOpts}, Ptr{Float64}, Ref{SolveInfo}),
             r.ctx, lin, lo, up, v0, opts, r.v, info))
+        r.vmat .= r.v
         mk = length(r.order); D = Vector{Float64}(undef, 2mk); L = Vector{Float64}(undef, 2mk)
         chk(r.ctx, ccall((:cfmm_get_trades, LIB), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}), r.ctx, D, L))
         for (j, i) in enumerate(r.order)
@@ -253,30 +256,54 @@ function netflows!(ψ, r::B200Router)
 end
 netflows(r::B200Router) = (ψ = zero(r.v); netflows!(ψ, r); ψ)
 
+# The price a UniV3 pool moves to when it trades at ν (cfmm_b200.h, cfmm_apply_trades): the
+# same IEEE operations as the device, so the host objects follow the device bit for bit.
+function univ3_moved_price(c::UniV3, v)
+    q, g = c.current_price, c.γ
+    p = v[c.Ai[1]] / v[c.Ai[2]]
+    lo = g * q
+    (lo <= p && p <= q / g) && return q             # no trade, src/cfmms.jl:347
+    target = p < lo ? p / g : g * p                 # upper walk :361 / lower walk :381 (pool price γ·p)
+    target > 0 || return q                          # NaN or not > 0: unchanged
+    t1 = c.lower_ticks[1]
+    return target < t1 ? target : t1
+end
+
 # A working update_reserves!(r) (the reference's, src/router.jl:127-132, calls a per-CFMM
-# method that is defined nowhere): R <- R + γΔ − Λ (test/cfmms.jl:10) applied on the device
-# from the materialised trades, and mirrored on the host objects with the same expression.
+# method that is defined nowhere), applied on the device from the materialised trades and
+# mirrored on the host objects with the same expressions: R <- R + γΔ − Λ (test/cfmms.jl:10)
+# for the two-coin pools; a UniV3 pool moves to the price its walk traded it to.
 function update_reserves!(r::B200Router)
     for (Δ, Λ, c) in zip(r.Δs, r.Λs, r.cfmms)
-        (c isa ProductTwoCoin || c isa GeometricMeanTwoCoin) || continue
-        c.R .= c.R .+ c.γ .* Δ .- Λ
+        if c isa ProductTwoCoin || c isa GeometricMeanTwoCoin
+            c.R .= c.R .+ c.γ .* Δ .- Λ
+        elseif c isa UniV3
+            c.current_price = univ3_moved_price(c, r.vmat)
+            c.current_tick = searchsortedlast(c.lower_ticks, c.current_price, rev=true)   # cfmms.jl:235
+        end
     end
-    if any(c -> c isa UniV3, r.cfmms)
-        sync_reserves!(r)                       # mixed set: push the two-coin reserves
-    else
-        foreach(c -> chk(c, ccall((:cfmm_apply_trades, LIB), Cint, (Ptr{Cvoid},), c)), r.ctxs)
-    end
+    foreach(c -> chk(c, ccall((:cfmm_apply_trades, LIB), Cint, (Ptr{Cvoid},), c)), r.ctxs)
     return nothing
 end
 
-# The reference reads cfmm.R live on every sweep; push mutated reserves explicitly.
+# The reference reads the pool objects live on every sweep; push mutated state explicitly:
+# cfmm.R of the two-coin pools, current_price and liquidity of the UniV3 pools (their tick
+# prices are fixed at construction).
 function sync_reserves!(r::B200Router)
-    for (k, ctx) in enumerate(r.ctxs), (ptype, T) in ((0, ProductTwoCoin), (1, GeometricMeanTwoCoin))
-        ids = [i for i in r.order[r.shard[k]] if r.cfmms[i] isa T]
+    for (k, ctx) in enumerate(r.ctxs)
+        for (ptype, T) in ((0, ProductTwoCoin), (1, GeometricMeanTwoCoin))
+            ids = [i for i in r.order[r.shard[k]] if r.cfmms[i] isa T]
+            isempty(ids) && continue
+            R = Float64[r.cfmms[i].R[j] for i in ids for j in 1:2]
+            chk(ctx, ccall((:cfmm_update_reserves, LIB), Cint,
+                (Ptr{Cvoid}, Cint, Int64, Int64, Ptr{Float64}), ctx, ptype, 0, length(ids), R))
+        end
+        ids = [i for i in r.order[r.shard[k]] if r.cfmms[i] isa UniV3]
         isempty(ids) && continue
-        R = Float64[r.cfmms[i].R[j] for i in ids for j in 1:2]
-        chk(ctx, ccall((:cfmm_update_reserves, LIB), Cint,
-            (Ptr{Cvoid}, Cint, Int64, Int64, Ptr{Float64}), ctx, ptype, 0, length(ids), R))
+        cp = Float64[r.cfmms[i].current_price for i in ids]
+        lq = reduce(vcat, (Float64.(r.cfmms[i].liquidity) for i in ids))
+        chk(ctx, ccall((:cfmm_update_univ3, LIB), Cint,
+            (Ptr{Cvoid}, Int64, Int64, Ptr{Float64}, Ptr{Float64}), ctx, 0, length(ids), cp, lq))
     end
 end
 

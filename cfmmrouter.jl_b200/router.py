@@ -73,6 +73,7 @@ class DevicePools:
         self.n_tokens = int(n_tokens)
         self.device = int(device)
         self.peer_attached = False
+        self._univ3_ticks = np.zeros(0, dtype=np.int64)  # tick count per UniV3 pool (update_univ3 checks)
         self._psi = np.zeros(self.n_tokens)
         self._acc = C.c_double(0.0)
         # pinned staging for sweep(): ν in, [Ψ; acc] out (contiguous) -- the buffers the library
@@ -119,6 +120,7 @@ class DevicePools:
             raise ValueError("inconsistent UniV3 CSR arrays")
         self._chk(self._lib.cfmm_add_univ3(self._ctx, len(cp), _dp(cp), _dp(gamma), _ip(Ai),
                                            _ip(off), _dp(lt), _dp(lq)))
+        self._univ3_ticks = np.concatenate([self._univ3_ticks, np.diff(off)])
 
     def add_file(self, path: str):
         """Add the pools of a flat pool file (write_pool_file / cfmm_pool_file_write)."""
@@ -233,12 +235,35 @@ class DevicePools:
         return out, {k: getattr(info, k) for k, _ in _lib.SolveInfo._fields_}
 
     def apply_trades(self):
-        """R <- R + γΔ − Λ on the device, from the last materialising sweep."""
+        """Apply the trades of the last materialising sweep on the device: R <- R + γΔ − Λ for the
+        two-coin pools, UniV3 pools move to the price their walk traded them to (univ3_moved_price)."""
         self._chk(self._lib.cfmm_apply_trades(self._ctx))
 
     def update_reserves(self, pool_type: int, first: int, R):
         R = np.ascontiguousarray(R, dtype=np.float64).reshape(-1, 2)
         self._chk(self._lib.cfmm_update_reserves(self._ctx, int(pool_type), int(first), len(R), _dp(R)))
+
+    def update_univ3(self, first: int, current_price=None, liquidity=None, count: int = None):
+        """cfmm_update_univ3: new current prices and/or tick liquidities of the UniV3 pools
+        [first, first + count) (UniV3 insertion order).  current_price: [count]; liquidity: the
+        concatenated ticks of the same pools in ingest CSR order.  count defaults to
+        len(current_price); a liquidity-only push must give it."""
+        first = int(first)
+        cp = None if current_price is None else np.ascontiguousarray(current_price, dtype=np.float64).reshape(-1)
+        lq = None if liquidity is None else np.ascontiguousarray(liquidity, dtype=np.float64).reshape(-1)
+        if count is None:
+            if cp is None:
+                raise ValueError("update_univ3: count is required when no prices are given")
+            count = len(cp)
+        count = int(count)
+        if cp is not None and len(cp) != count:
+            raise ValueError(f"update_univ3: {len(cp)} prices for {count} pools")
+        if lq is not None:
+            nt = self._univ3_ticks[first:first + count] if 0 <= first <= len(self._univ3_ticks) else []
+            if len(nt) == count and len(lq) != int(np.sum(nt)):
+                raise ValueError(f"update_univ3: {len(lq)} liquidities for {int(np.sum(nt))} ticks")
+        self._chk(self._lib.cfmm_update_univ3(self._ctx, first, count, None if cp is None else _dp(cp),
+                                              None if lq is None else _dp(lq)))
 
     # -- multi-GPU --------------------------------------------------------------
     def detach_group(self):
@@ -418,6 +443,7 @@ class Router:
             psi, acc = out[:-1].copy(), float(out[-1])
         self._psi, self._acc = psi, acc
         if materialize:
+            self._v_mat = np.array(v, dtype=np.float64)
             self._fetch_trades()
 
     def _fetch_trades(self):
@@ -441,13 +467,20 @@ class Router:
             self.Λs[:] = Ll[:n]
 
     def sync_reserves(self):
-        """Push cfmm.R of every Product/GeoMean pool to the device (the reference
-        reads cfmm.R live on each sweep; call this after mutating reserves)."""
+        """Push the state of every pool to the device: cfmm.R of the Product/GeoMean pools,
+        current_price and liquidity of the UniV3 pools (the reference reads the pool objects
+        live on each sweep; call this after mutating them).  A UniV3 pool's tick prices are
+        fixed at construction."""
         shard = self.cfmms[self._lo:self._hi]
         for t in (0, 1):
             ids = self._type_lists[t]
             if ids:
                 self._pools.update_reserves(t, 0, np.array([shard[i].R for i in ids]))
+        ids = self._type_lists[2]
+        if ids:
+            cs = [shard[i] for i in ids]
+            self._pools.update_univ3(0, np.array([c.current_price for c in cs]),
+                                     np.concatenate([c.liquidity for c in cs]))
 
 
 def find_arb(*args):
@@ -500,6 +533,7 @@ def route(r: Router, v=None, verbose=False, m=5, factr=1e1, pgtol=1e-5,
                                  v0=None if v is None else np.asarray(v, dtype=np.float64),
                                  pgtol=pgtol, factr=factr, maxfun=maxfun, maxiter=maxiter)
         r.v[:] = x
+        r._v_mat = x.copy()
         r._fetch_trades()
         r.last_result = info
         return None
@@ -557,18 +591,39 @@ def netflows(r: Router):
     return psi
 
 
+def univ3_moved_price(c: UniV3, v):
+    """The price a UniV3 pool moves to when it trades at ν = v (include/cfmm_b200.h,
+    cfmm_apply_trades): p = v[a]/v[b]; unchanged inside the no-trade band γq <= p <= q/γ,
+    else min(p/γ, T₁) (upper walk, p < γq) or min(γp, T₁) (lower walk), unchanged if that
+    target is NaN or not > 0.  The same IEEE operations as the device kernel: bit-identical."""
+    with np.errstate(all="ignore"):
+        q, g = np.float64(c.current_price), np.float64(c.gamma)
+        p = np.float64(v[c.Ai[0] - 1]) / np.float64(v[c.Ai[1] - 1])
+        lo = g * q
+        if lo <= p and p <= q / g:
+            return float(q)
+        target = p / g if p < lo else g * p
+        if not target > 0.0:
+            return float(q)
+        t1 = np.float64(c.lower_ticks[0])
+        return float(target if target < t1 else t1)
+
+
 def update_reserves(r: Router):
     """A working update_reserves!(r) (the reference's, src/router.jl:127-132,
-    calls a per-CFMM method that is defined nowhere): R ← R + γΔ − Λ for the
-    two-coin pools, on the host objects and on the device."""
+    calls a per-CFMM method that is defined nowhere), on the host objects and on
+    the device: R ← R + γΔ − Λ for the two-coin pools (test/cfmms.jl:10); a UniV3
+    pool moves to the price its arbitrage walk traded it to (univ3_moved_price, at
+    the ν of the last materialising sweep), with current_tick re-derived as the
+    constructor does."""
+    v = getattr(r, "_v_mat", None)
+    if v is None:
+        v = r.v
     for D, L, c in zip(r.Δs, r.Λs, r.cfmms):
         if isinstance(c, (ProductTwoCoin, GeometricMeanTwoCoin)):
             c.R = c.R + c.gamma * D - L  # same operation order as the device kernel: bit-identical
-    if any(isinstance(c, UniV3) for c in r.cfmms):
-        import warnings
-        warnings.warn("update_reserves: UniV3 pools keep their state (current_price / ticks are not advanced: "
-                      "the reference defines no reserve update for them)", stacklevel=2)
-        r.sync_reserves()  # mixed set: push the two-coin reserves from the host objects
-    else:
-        r._pools.apply_trades()  # on the device, from the materialised trades: no upload
+        elif isinstance(c, UniV3):
+            c.current_price = univ3_moved_price(c, v)
+            c.current_tick = int(np.sum(c.lower_ticks >= c.current_price))
+    r._pools.apply_trades()  # on the device, from the materialised trades: no upload
     return None

@@ -155,12 +155,42 @@ int cfmm_get_trades(cfmm_ctx *ctx, double *Delta, double *Lambda);
 int cfmm_update_reserves(cfmm_ctx *ctx, int type, int64_t first, int64_t count,
                          const double *R);
 
-/* Apply the trades of the last materialising sweep to the device-resident
- * reserves: R <- R + γΔ − Λ for every ProductTwoCoin / GeometricMeanTwoCoin pool
- * (the update the reference intends with update_reserves!(r), src/router.jl:127-132,
- * whose per-CFMM method is defined nowhere; formula from test/cfmms.jl:10).
- * Lets a caller route repeatedly on evolving state without re-uploading pools.
- * Fails with CFMM_ERR_INVALID if the context holds UniV3 pools. */
+/* Overwrite the state of UniV3 pools [first, first+count), counted in UniV3
+ * insertion order.  current_price: [count], or NULL to keep the prices.
+ * liquidity: the concatenated tick liquidities of those pools in their ingested
+ * CSR order, or NULL to keep them.  The tick grid (lower_ticks, tick counts) is
+ * fixed at cfmm_finalize.  Prices are validated as in cfmm_add_univ3 (a price
+ * above the pool's first lower tick, or NaN, is rejected with CFMM_ERR_INVALID);
+ * a rejected call changes no pool.  current_tick and every tick's BoundedProduct
+ * (compute_at_tick, src/cfmms.jl:294-313) are recomputed on the device.
+ * Synchronous. */
+int cfmm_update_univ3(cfmm_ctx *ctx, int64_t first, int64_t count,
+                      const double *current_price, const double *liquidity);
+
+/* Apply the trades of the last materialising sweep to the device-resident pool
+ * state (the update the reference intends with update_reserves!(r),
+ * src/router.jl:127-132, whose per-CFMM method is defined nowhere).  Lets a
+ * caller route repeatedly on evolving state without re-uploading pools.
+ *
+ * ProductTwoCoin / GeometricMeanTwoCoin: R <- R + γΔ − Λ (test/cfmms.jl:10).
+ *
+ * UniV3: the pool moves to the price its arbitrage walk (find_arb_pos,
+ * src/cfmms.jl:321-337) trades it to.  With fee γ, current price q, first lower
+ * tick T₁ = lower_ticks[1] and p = ν[a]/ν[b] at the ν of the last materialising
+ * sweep (whichever entry point ran it; the library keeps a copy of that ν):
+ *
+ *   case (as src/cfmms.jl:347, 351)            new price q′
+ *   γ·q <= p <= q/γ  (no trade)                q
+ *   p < γ·q          (upper walk, :361)         min(p/γ, T₁)
+ *   otherwise        (lower walk, :381)         min(γ·p, T₁)
+ *   p/γ resp. γ·p is NaN or not > 0            q
+ *
+ * γ·q, q/γ, p/γ and γ·p are single IEEE operations, so q′ is bit-reproducible on
+ * any host.  The clamp to T₁ covers a lower walk that drains tick 1 (no tick is
+ * defined above T₁) and the case where p/γ rounds above q = T₁.  Then
+ * current_tick′ = searchsortedlast(lower_ticks, q′, rev=true) (:235) and every
+ * tick's BoundedProduct is compute_at_tick at (q′, current_tick′), recomputed on
+ * the device for the pools whose price changed. */
 int cfmm_apply_trades(cfmm_ctx *ctx);
 
 /* ---- the outer iteration on the device (SURVEY §8f rank 2) ---------------------------
