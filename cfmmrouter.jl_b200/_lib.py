@@ -61,6 +61,13 @@ SYMBOLS = {
     "cfmm_update_reserves": (C.c_int, [_ctx, C.c_int, C.c_int64, C.c_int64, _dp]),
     "cfmm_update_univ3": (C.c_int, [_ctx, C.c_int64, C.c_int64, _dp, _dp]),
     "cfmm_apply_trades": (C.c_int, [_ctx]),
+    "cfmm_append_product": (C.c_int, [_ctx, C.c_int64, _dp, _dp, _ip]),
+    "cfmm_append_geomean": (C.c_int, [_ctx, C.c_int64, _dp, _dp, _ip, _dp]),
+    "cfmm_append_univ3": (C.c_int, [_ctx, C.c_int64, _dp, _dp, _ip, _ip, _dp, _dp]),
+    "cfmm_set_active": (C.c_int, [_ctx, C.c_int, C.c_int64, C.c_int64, C.POINTER(C.c_uint8)]),
+    "cfmm_get_pool_state": (C.c_int, [_ctx, C.c_int, C.c_int64, C.c_int64, _dp, C.POINTER(C.c_uint8)]),
+    "cfmm_compact": (C.c_int, [_ctx]),
+    "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),
     "cfmm_set_option": (C.c_int, [_ctx, C.c_char_p, C.c_int64]),
     "cfmm_last_sweep_ms": (C.c_int, [_ctx, C.POINTER(C.c_float)]),
     "cfmm_launch_count": (C.c_int64, [_ctx]),

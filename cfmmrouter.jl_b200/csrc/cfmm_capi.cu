@@ -17,6 +17,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
+#include <memory>
 #include <new>
 #include <string>
 #include <unordered_map>
@@ -41,6 +43,15 @@ struct DevBuf {
   DevBuf() = default;
   DevBuf(const DevBuf&) = delete;  // owns its allocation: freed on every exit path
   DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), n(o.n) {
+    o.p = nullptr;
+    o.n = 0;
+  }
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    std::swap(p, o.p);
+    std::swap(n, o.n);
+    return *this;
+  }
   ~DevBuf() { release(); }
   cudaError_t alloc(size_t count) {
     release();
@@ -70,7 +81,10 @@ struct DevBuf {
   }
 };
 
-// One pool type's shard: host staging until finalize, device SoA afterwards.
+// One pool type's shard: host staging until finalize, device SoA afterwards.  Each type has a
+// main set (laid out at cfmm_finalize / cfmm_compact) and a tail set (the pools appended since,
+// cfmm_append_*: a-sorted layout, first-generation kernel).  A set is movable (std::swap), so a
+// new layout is built beside the live one and swapped in.
 struct PoolSet {
   int64_t m = 0;
   // host staging (insertion order)
@@ -126,6 +140,12 @@ struct PoolSet {
   int64_t tma_launches = 0;
   cfmm::HVec<uint8_t> swapped;  // product: pool stored with its two tokens exchanged (insertion index)
   bool skewed = false;          // product: hub tokens detected at finalize
+  // retired pools (cfmm_set_active): the host flags (insertion order; empty = none retired), the
+  // device-order mask the off-path kernels read (1 = active; allocated on the first retire) and,
+  // for the two-coin types, the parked reserves of the retired pools (R itself holds (0, 0))
+  std::vector<uint8_t> retired;
+  DevBuf<uint8_t> d_active;
+  DevBuf<double2> d_park;
   void release() {
     d_R.release(); d_w.release(); d_outD.release(); d_outL.release();
     d_gam.release(); d_tickdata.release();
@@ -133,6 +153,7 @@ struct PoolSet {
     d_Ai.release(); d_tick.release(); d_gidx.release();
     d_lower.release(); d_liq.release();
     d_packed.release(); d_inv_scale.release(); d_tok_sum.release(); d_gcode.release(); d_gtab.release();
+    d_active.release(); d_park.release();
     if (h_dur) cudaFreeHost(h_dur);
     h_dur = nullptr;
     if (ev_dur) cudaEventDestroy(ev_dur);
@@ -150,6 +171,7 @@ struct cfmm_ctx {
   bool finalized = false;
   bool has_trades = false;
   PoolSet sets[3];
+  PoolSet tails[3];  // pools appended after finalize (cfmm_append_*), folded into sets by cfmm_compact
   cudaStream_t stream = nullptr;
   cudaStream_t last_stream = nullptr;  // stream of the last sweep (cfmm_sweep_device* may use the caller's)
   cudaEvent_t ev_order = nullptr;      // orders work across a change of stream
@@ -248,9 +270,11 @@ int fail(cfmm_ctx* ctx, int code, const char* fmt, ...) {
   } while (0)
 
 int check_common(cfmm_ctx* ctx, int64_t m, const double* R, const double* gamma,
-                 const int64_t* Ai) {
+                 const int64_t* Ai, bool append = false) {
   if (!ctx) return CFMM_ERR_INVALID;
-  if (ctx->finalized)
+  if (append && !ctx->finalized)
+    return fail(ctx, CFMM_ERR_STATE, "pools are appended after cfmm_finalize (cfmm_add_* before it)");
+  if (!append && ctx->finalized)
     return fail(ctx, CFMM_ERR_STATE, "pools cannot be added after cfmm_finalize");
   if (m < 0) return fail(ctx, CFMM_ERR_INVALID, "negative pool count");
   if (m > 0 && (!gamma || !Ai || !R))
@@ -300,11 +324,12 @@ inline bool fast_range_ok(double v) { return v >= cfmm::kFastLo && v <= cfmm::kF
 
 // layout of one pool type (pool_layout.hpp): ProductTwoCoin gets the b-bucketed,
 // chunk-padded layout of the TMA kernel; the other types are a-sorted only.
-cfmm::PoolLayout layout_for(const cfmm_ctx* ctx, int type, const int64_t* Ai, int64_t m,
+// Tail sets (bucketed = false) always get the a-sorted layout of tma_variant -1.
+cfmm::PoolLayout layout_for(const cfmm_ctx* ctx, int type, const int64_t* Ai, int64_t m, bool bucketed,
                             void (*mark)(const char*) = nullptr) {
   const bool product = type == CFMM_POOL_PRODUCT;
   cfmm::TileShape shape;
-  if ((product || type == CFMM_POOL_GEOMEAN) && ctx->tma_variant >= 0) {
+  if ((product || type == CFMM_POOL_GEOMEAN) && bucketed && ctx->tma_variant >= 0) {
     shape.tile = cfmm::kTmaChunk;
     shape.nbmax = cfmm::kTmaNbMax;
   }
@@ -370,6 +395,7 @@ cfmm::Univ3State univ3_state(PoolSet& s) {
   u.tickdata = s.d_tickdata.p;
   u.lower = s.d_lower.p;
   u.liq = s.d_liq.p;
+  u.active = s.d_active.p;
   u.m = s.m;
   u.total_ticks = s.total_ticks;
   return u;
@@ -395,13 +421,13 @@ cudaError_t univ3_rebuild(cfmm_ctx* ctx, PoolSet& s, const int64_t* d_pos, const
   return cudaGetLastError();
 }
 
-int upload_set(cfmm_ctx* ctx, int type) {
-  PoolSet& s = ctx->sets[type];
+// Lay out the staged pools of s (a main set, or a tail: tail = true) and upload them.
+int upload_set(cfmm_ctx* ctx, int type, PoolSet& s, bool tail) {
   if (s.m == 0) return CFMM_OK;
   const int64_t m = s.m;
   PhaseClock clock;
   g_layout_clock = clock.on ? &clock : nullptr;
-  cfmm::PoolLayout lay = layout_for(ctx, type, s.Ai.data(), m, clock.on ? layout_mark : nullptr);
+  cfmm::PoolLayout lay = layout_for(ctx, type, s.Ai.data(), m, !tail, clock.on ? layout_mark : nullptr);
   g_layout_clock = nullptr;
   const cfmm::HVec<int>&oa = lay.oa, &ob = lay.ob;
   s.swapped.swap(lay.swapped);
@@ -569,7 +595,7 @@ int upload_set(cfmm_ctx* ctx, int type) {
     }
     CU_TRY(ctx, s.d_tickdata.alloc((size_t)s.total_ticks * cfmm::kTickStride));
     CU_TRY(ctx, univ3_rebuild(ctx, s, nullptr, nullptr, m, s.total_ticks, nullptr, nullptr, true));
-    CU_TRY(ctx, ctx->d_nu_mat.alloc((size_t)ctx->n_tokens));
+    if (ctx->d_nu_mat.n != (size_t)ctx->n_tokens) CU_TRY(ctx, ctx->d_nu_mat.alloc((size_t)ctx->n_tokens));
     clock.mark("univ3 tick data: upload + device rebuild");
   }
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // the bounce copies read the staging below
@@ -919,8 +945,9 @@ int enqueue_sweep(cfmm_ctx* ctx, const double* d_v, double* d_dst, bool mat,
   bool fused = false;
   {
     const PoolSet& ps = ctx->sets[CFMM_POOL_PRODUCT];
+    const bool no_tails = ctx->tails[0].m == 0 && ctx->tails[1].m == 0 && ctx->tails[2].m == 0;
     if (ctx->comm.attached() && !ctx->exchange_bypass && ctx->fused_exchange && !mat && ps.m > 0 && ps.tma_ok && ctx->use_tma &&
-        ctx->debug_skip == 0 && ctx->sets[CFMM_POOL_GEOMEAN].m == 0 && ctx->sets[CFMM_POOL_UNIV3].m == 0) {
+        ctx->debug_skip == 0 && ctx->sets[CFMM_POOL_GEOMEAN].m == 0 && ctx->sets[CFMM_POOL_UNIV3].m == 0 && no_tails) {
       fused = true;
       ctx->fx_pending.view = ctx->comm.view();
       ctx->fx_pending.dst = d_dst ? d_dst : d_psi;
@@ -939,6 +966,11 @@ int enqueue_sweep(cfmm_ctx* ctx, const double* d_v, double* d_dst, bool mat,
         if ((rc = launch_sweep(ctx, PT, p, s, d_v, d_psi, mat, st)) != CFMM_OK) return rc;
       }
     }
+    PoolSet& t = ctx->tails[PT];  // appended pools: first-generation kernel, same accumulator
+    if (t.m > 0) {
+      cfmm::ProductPools p{t.d_R.p, t.d_gam.p, t.d_Ai.p};
+      if ((rc = launch_sweep(ctx, PT, p, t, d_v, d_psi, mat, st)) != CFMM_OK) return rc;
+    }
   }
   {
     PoolSet& s = ctx->sets[CFMM_POOL_GEOMEAN];
@@ -955,19 +987,32 @@ int enqueue_sweep(cfmm_ctx* ctx, const double* d_v, double* d_dst, bool mat,
         return rc;
       }
     }
+    PoolSet& t = ctx->tails[PT];
+    if (t.m > 0) {
+      cfmm::GeomeanPools p{t.d_R.p, t.d_gam.p, t.d_Ai.p, t.d_w.p};
+      if (ctx->geomean_log2 && !mat) {
+        cfmm::GeomeanPoolsLog2 q;
+        static_cast<cfmm::GeomeanPools&>(q) = p;
+        if ((rc = launch_sweep(ctx, PT, q, t, d_v, d_psi, mat, st)) != CFMM_OK) return rc;
+      } else if ((rc = launch_sweep(ctx, PT, p, t, d_v, d_psi, mat, st)) != CFMM_OK) {
+        return rc;
+      }
+    }
   }
   {
-    PoolSet& s = ctx->sets[CFMM_POOL_UNIV3];
     constexpr int PT = CFMM_POOL_UNIV3;
-    if (s.m > 0) {
+    for (PoolSet* ps : {&ctx->sets[PT], &ctx->tails[PT]}) {
+      PoolSet& s = *ps;
+      if (s.m == 0) continue;
       cfmm::Univ3Pools p{s.d_first[0].p, s.d_first[1].p, s.d_first[2].p, s.d_first[3].p, s.d_gam.p, s.d_Ai.p, s.d_tick.p,
                          s.d_tickdata.p, s.m_padded, (int)s.total_ticks};
       if ((rc = launch_sweep(ctx, PT, p, s, d_v, d_psi, mat, st)) != CFMM_OK) return rc;
-      // cfmm_apply_trades moves UniV3 prices by the ν of the last materialising sweep: keep it,
-      // since the caller's d_v (and the context's own ν buffer) may be overwritten before then
-      if (mat) CU_TRY(ctx, cudaMemcpyAsync(ctx->d_nu_mat.p, d_v, (size_t)ctx->n_tokens * sizeof(double),
-                                           cudaMemcpyDeviceToDevice, st));
     }
+    // cfmm_apply_trades moves UniV3 prices by the ν of the last materialising sweep: keep it,
+    // since the caller's d_v (and the context's own ν buffer) may be overwritten before then
+    if (mat && (ctx->sets[PT].m > 0 || ctx->tails[PT].m > 0))
+      CU_TRY(ctx, cudaMemcpyAsync(ctx->d_nu_mat.p, d_v, (size_t)ctx->n_tokens * sizeof(double),
+                                  cudaMemcpyDeviceToDevice, st));
   }
   if (ctx->zero_pending) {  // no kernel ran (empty pool set): clear the other accumulator here
     CU_TRY(ctx, cudaMemsetAsync(take_zero_pending(ctx), 0, acc_bytes, st));
@@ -998,6 +1043,27 @@ int ready(cfmm_ctx* ctx) {
   if (!ctx->finalized)
     return fail(ctx, CFMM_ERR_STATE, "cfmm_finalize has not been called");
   return CFMM_OK;
+}
+
+// Calibration (cfmm_finalize, cfmm_compact): a dozen gradient sweeps at ν = 1 settle the
+// speed-weighted CTA ranges of the TMA kernels (and pay the one-time costs of the first launch:
+// function attributes, stream packing) here rather than in the caller's first sweeps.  ~1 ms.
+int calibrate(cfmm_ctx* ctx) {
+  bool any = false;
+  for (int t : {CFMM_POOL_PRODUCT, CFMM_POOL_GEOMEAN}) any = any || (ctx->sets[t].m > 0 && ctx->sets[t].tma_ok);
+  if (!any || !ctx->balance) return CFMM_OK;
+  std::vector<double> ones((size_t)ctx->n_tokens, 1.0);
+  CU_TRY(ctx, DevBuf<double>::copy_in(ctx->d_nu.p, ones.data(), ones.size() * sizeof(double)));
+  ctx->calibrating = true;
+  int rc = CFMM_OK;
+  for (int it = 0; it < 12 && rc == CFMM_OK; ++it) {
+    const double* view = nullptr;
+    rc = enqueue_sweep(ctx, ctx->d_nu.p, nullptr, false, ctx->stream, &view);
+    if (rc == CFMM_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess)
+      rc = fail(ctx, CFMM_ERR_CUDA, "calibration sweep failed: %s", cudaGetErrorString(cudaGetLastError()));
+  }
+  ctx->calibrating = false;
+  return rc;
 }
 
 }  // namespace
@@ -1076,6 +1142,7 @@ void cfmm_destroy(cfmm_ctx* ctx) {
   for (auto e : ctx->prof.ev)
     if (e) cudaEventDestroy(e);
   for (auto& s : ctx->sets) s.release();
+  for (auto& s : ctx->tails) s.release();
   ctx->d_nu.release();
   ctx->d_nu_mat.release();
   ctx->d_grid_done.release();
@@ -1113,19 +1180,16 @@ int cfmm_add_geomean(cfmm_ctx* ctx, int64_t m, const double* R,
   return CFMM_OK;
 }
 
-int cfmm_add_univ3(cfmm_ctx* ctx, int64_t m, const double* current_price,
-                   const double* gamma, const int64_t* Ai,
-                   const int64_t* tick_off, const double* lower_ticks,
-                   const double* liquidity) {
-  static const double dummy = 0.0;
-  int rc = check_common(ctx, m, m > 0 ? &dummy : nullptr, gamma, Ai);
-  if (rc != CFMM_OK) return rc;
-  if (m == 0) return CFMM_OK;
+namespace {
+
+// cfmm_add_univ3's checks of the CSR arrays (the pools are checked by check_common); ticks_before:
+// the ticks already staged in the set the pools go to
+int check_univ3(cfmm_ctx* ctx, int64_t m, const double* current_price, const int64_t* tick_off,
+                const double* lower_ticks, const double* liquidity, int64_t ticks_before) {
   if (!current_price || !tick_off || !lower_ticks || !liquidity)
     return fail(ctx, CFMM_ERR_INVALID, "null array argument");
   if (tick_off[0] != 0)
     return fail(ctx, CFMM_ERR_INVALID, "tick_off[0] must be 0");
-  PoolSet& s = ctx->sets[CFMM_POOL_UNIV3];
   for (int64_t i = 0; i < m; ++i) {
     const int64_t b = tick_off[i], e = tick_off[i + 1];
     if (e <= b)
@@ -1141,9 +1205,14 @@ int cfmm_add_univ3(cfmm_ctx* ctx, int64_t m, const double* current_price,
                   "(current_tick == 0; BoundsError in the reference)",
                   (long long)i);
   }
-  const int64_t n_ticks = tick_off[m];
-  if ((int64_t)s.lower.size() + n_ticks > (int64_t)0x7fffffff)
+  if (ticks_before + tick_off[m] > (int64_t)0x7fffffff)
     return fail(ctx, CFMM_ERR_INVALID, "more than 2^31-1 ticks in one context");
+  return CFMM_OK;
+}
+
+void stage_univ3(cfmm_ctx* ctx, PoolSet& s, int64_t m, const double* current_price, const double* gamma,
+                 const int64_t* Ai, const int64_t* tick_off, const double* lower_ticks, const double* liquidity) {
+  const int64_t n_ticks = tick_off[m];
   const int64_t base = (int64_t)s.lower.size();
   if (s.tick_off.empty()) s.tick_off.push_back(0);
   for (int64_t i = 1; i <= m; ++i) s.tick_off.push_back(base + tick_off[i]);
@@ -1151,6 +1220,22 @@ int cfmm_add_univ3(cfmm_ctx* ctx, int64_t m, const double* current_price,
   s.lower.insert(s.lower.end(), lower_ticks, lower_ticks + n_ticks);
   s.liq.insert(s.liq.end(), liquidity, liquidity + n_ticks);
   append_common(ctx, s, m, nullptr, gamma, Ai);
+}
+
+}  // namespace
+
+int cfmm_add_univ3(cfmm_ctx* ctx, int64_t m, const double* current_price,
+                   const double* gamma, const int64_t* Ai,
+                   const int64_t* tick_off, const double* lower_ticks,
+                   const double* liquidity) {
+  static const double dummy = 0.0;
+  int rc = check_common(ctx, m, m > 0 ? &dummy : nullptr, gamma, Ai);
+  if (rc != CFMM_OK) return rc;
+  if (m == 0) return CFMM_OK;
+  PoolSet& s = ctx->sets[CFMM_POOL_UNIV3];
+  if ((rc = check_univ3(ctx, m, current_price, tick_off, lower_ticks, liquidity, (int64_t)s.lower.size())) != CFMM_OK)
+    return rc;
+  stage_univ3(ctx, s, m, current_price, gamma, Ai, tick_off, lower_ticks, liquidity);
   return CFMM_OK;
 }
 
@@ -1248,7 +1333,7 @@ int cfmm_finalize(cfmm_ctx* ctx) {
   const bool timing = getenv("CFMM_TIMING") != nullptr;
   auto t0 = std::chrono::steady_clock::now();
   for (int t = 0; t < 3; ++t) {
-    int rc = upload_set(ctx, t);
+    int rc = upload_set(ctx, t, ctx->sets[t], false);
     if (rc != CFMM_OK) return rc;
     if (timing) {
       const auto t1 = std::chrono::steady_clock::now();
@@ -1258,31 +1343,11 @@ int cfmm_finalize(cfmm_ctx* ctx) {
     }
   }
   ctx->finalized = true;
-  // Calibration: a dozen gradient sweeps at ν = 1 settle the speed-weighted CTA ranges of the TMA
-  // kernels (and pay the one-time costs of the first launch: function attributes, stream packing)
-  // here rather than in the caller's first sweeps.  ~1 ms.
-  {
-    bool any = false;
-    for (int t : {CFMM_POOL_PRODUCT, CFMM_POOL_GEOMEAN}) any = any || (ctx->sets[t].m > 0 && ctx->sets[t].tma_ok);
-    if (any && ctx->balance) {
-      std::vector<double> ones((size_t)ctx->n_tokens, 1.0);
-      CU_TRY(ctx, DevBuf<double>::copy_in(ctx->d_nu.p, ones.data(), ones.size() * sizeof(double)));
-      ctx->calibrating = true;
-      int rc = CFMM_OK;
-      for (int it = 0; it < 12 && rc == CFMM_OK; ++it) {
-        const double* view = nullptr;
-        rc = enqueue_sweep(ctx, ctx->d_nu.p, nullptr, false, ctx->stream, &view);
-        if (rc == CFMM_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess)
-          rc = fail(ctx, CFMM_ERR_CUDA, "calibration sweep failed: %s", cudaGetErrorString(cudaGetLastError()));
-      }
-      ctx->calibrating = false;
-      if (rc != CFMM_OK) return rc;
-      if (timing)
-        fprintf(stderr, "[cfmm] finalize: calibration %.3f s\n",
-                std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count());
-    }
-  }
-  return CFMM_OK;
+  const int rc = calibrate(ctx);
+  if (rc == CFMM_OK && timing)
+    fprintf(stderr, "[cfmm] finalize: calibration %.3f s\n",
+            std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count());
+  return rc;
 }
 
 int64_t cfmm_num_pools(const cfmm_ctx* ctx) { return ctx ? ctx->n_pools : -1; }
@@ -1684,13 +1749,53 @@ int cfmm_last_sweep_ms(cfmm_ctx* ctx, float* ms_out) {
   return CFMM_OK;
 }
 
+namespace {
+
+int64_t type_pools(const cfmm_ctx* ctx, int type) { return ctx->sets[type].m + ctx->tails[type].m; }
+
+// Part of a type-local pool range [first, first + count) that falls in one set: pools
+// [0, sets[t].m) of a type are its main set's, the rest its tail's.  `offset`: where the part
+// starts within the caller's range.
+struct Span {
+  PoolSet* s;
+  int64_t first, count, offset;
+};
+std::vector<Span> split_range(cfmm_ctx* ctx, int type, int64_t first, int64_t count) {
+  std::vector<Span> out;
+  PoolSet& a = ctx->sets[type];
+  const int64_t hi = first + count;
+  if (count <= 0) return out;
+  if (first < a.m) out.push_back({&a, first, std::min(hi, a.m) - first, 0});
+  if (hi > a.m) {
+    const int64_t lo = std::max(first, a.m);
+    out.push_back({&ctx->tails[type], lo - a.m, hi - lo, lo - first});
+  }
+  return out;
+}
+
+void ensure_pos_of(PoolSet& s) {
+  if (!s.pos_of.empty() || s.m == 0) return;
+  s.pos_of.resize((size_t)s.m);
+  for (int64_t p = 0; p < s.m_padded; ++p)
+    if (s.order[(size_t)p] >= 0) s.pos_of[(size_t)s.order[(size_t)p]] = p;
+}
+
+// A change of the pool set (append, retire / restore, compact): captured sweep graphs are stale,
+// and the materialised trades no longer describe the set.
+void membership_changed(cfmm_ctx* ctx) {
+  ctx->state_version++;
+  ctx->has_trades = false;
+}
+
+}  // namespace
+
 int cfmm_get_trades(cfmm_ctx* ctx, double* Delta, double* Lambda) {
   int rc = ready(ctx);
   if (rc != CFMM_OK) return rc;
   if (!Delta || !Lambda) return fail(ctx, CFMM_ERR_INVALID, "null host pointer");
   if (!ctx->has_trades)
     return fail(ctx, CFMM_ERR_STATE,
-                "no materialising sweep has run (call cfmm_sweep with materialize=1)");
+                "no materialising sweep has run since the last change of the pool set (call cfmm_sweep with materialize=1)");
   CU_TRY(ctx, cudaSetDevice(ctx->device));
   if (ctx->n_pools == 0) return CFMM_OK;
   if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
@@ -1701,14 +1806,16 @@ int cfmm_get_trades(cfmm_ctx* ctx, double* Delta, double* Lambda) {
     allD.release();
     return fail(ctx, CFMM_ERR_CUDA, "cudaMalloc failed: %s", cudaGetErrorString(e));
   }
-  for (auto& s : ctx->sets) {
-    if (s.m == 0) continue;
-    const int threads = 256;
-    const int64_t blocks = (s.m_padded + threads - 1) / threads;
-    cfmm::scatter_trades_kernel<<<(unsigned)blocks, threads, 0, ctx->stream>>>(
-        s.d_outD.p, s.d_outL.p, s.d_gidx.p, allD.p, allL.p, s.m_padded);
-    ctx->launches++;
-  }
+  for (PoolSet* group : {ctx->sets, ctx->tails})
+    for (int t = 0; t < 3; ++t) {
+      PoolSet& s = group[t];
+      if (s.m == 0) continue;
+      const int threads = 256;
+      const int64_t blocks = (s.m_padded + threads - 1) / threads;
+      cfmm::scatter_trades_kernel<<<(unsigned)blocks, threads, 0, ctx->stream>>>(
+          s.d_outD.p, s.d_outL.p, s.d_gidx.p, allD.p, allL.p, s.m_padded);
+      ctx->launches++;
+    }
   const size_t bytes = (size_t)ctx->n_pools * sizeof(double2);
   cudaError_t e1 = cudaMemcpyAsync(Delta, allD.p, bytes, cudaMemcpyDeviceToHost, ctx->stream);
   cudaError_t e2 = cudaMemcpyAsync(Lambda, allL.p, bytes, cudaMemcpyDeviceToHost, ctx->stream);
@@ -1721,26 +1828,11 @@ int cfmm_get_trades(cfmm_ctx* ctx, double* Delta, double* Lambda) {
   return CFMM_OK;
 }
 
-int cfmm_update_reserves(cfmm_ctx* ctx, int type, int64_t first, int64_t count,
-                         const double* R) {
-  int rc = ready(ctx);
-  if (rc != CFMM_OK) return rc;
-  if (type != CFMM_POOL_PRODUCT && type != CFMM_POOL_GEOMEAN)
-    return fail(ctx, CFMM_ERR_INVALID, "update_reserves: type must be PRODUCT or GEOMEAN");
-  PoolSet& s = ctx->sets[type];
-  ctx->state_version++;
-  if (first < 0 || count < 0 || first + count > s.m)
-    return fail(ctx, CFMM_ERR_INVALID, "update_reserves: range [%lld, %lld) outside 0..%lld",
-                (long long)first, (long long)(first + count), (long long)s.m);
-  if (count == 0) return CFMM_OK;
-  if (!R) return fail(ctx, CFMM_ERR_INVALID, "null reserve array");
-  CU_TRY(ctx, cudaSetDevice(ctx->device));
-  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
-  if (s.pos_of.empty()) {
-    s.pos_of.resize((size_t)s.m);
-    for (int64_t p = 0; p < s.m_padded; ++p)
-      if (s.order[(size_t)p] >= 0) s.pos_of[(size_t)s.order[(size_t)p]] = p;
-  }
+namespace {
+
+// new reserves of the pools [first, first + count) of one set (insertion order within the set)
+int update_reserves_set(cfmm_ctx* ctx, PoolSet& s, int64_t first, int64_t count, const double* R) {
+  ensure_pos_of(s);
   std::vector<double2> newR((size_t)count);
   for (int64_t j = 0; j < count; ++j) {
     newR[(size_t)j] = s.swapped[(size_t)(first + j)] ? make_double2(R[2 * j + 1], R[2 * j])
@@ -1756,7 +1848,7 @@ int cfmm_update_reserves(cfmm_ctx* ctx, int type, int64_t first, int64_t count,
   if (e == cudaSuccess) {
     const int threads = 256;
     cfmm::update_reserves_kernel<<<(unsigned)((count + threads - 1) / threads), threads, 0,
-                                   ctx->stream>>>(s.d_R.p, d_pos.p, d_new.p, count);
+                                   ctx->stream>>>(s.d_R.p, d_pos.p, d_new.p, count, s.d_active.p, s.d_park.p);
     ctx->launches++;
     e = cudaStreamSynchronize(ctx->stream);
   }
@@ -1765,6 +1857,28 @@ int cfmm_update_reserves(cfmm_ctx* ctx, int type, int64_t first, int64_t count,
   if (e != cudaSuccess)
     return fail(ctx, CFMM_ERR_CUDA, "update_reserves failed: %s", cudaGetErrorString(e));
   if (s.tma_ok) return refresh_scale(ctx, s);
+  return CFMM_OK;
+}
+
+}  // namespace
+
+int cfmm_update_reserves(cfmm_ctx* ctx, int type, int64_t first, int64_t count,
+                         const double* R) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if (type != CFMM_POOL_PRODUCT && type != CFMM_POOL_GEOMEAN)
+    return fail(ctx, CFMM_ERR_INVALID, "update_reserves: type must be PRODUCT or GEOMEAN");
+  const int64_t m = type_pools(ctx, type);
+  ctx->state_version++;
+  if (first < 0 || count < 0 || first + count > m)
+    return fail(ctx, CFMM_ERR_INVALID, "update_reserves: range [%lld, %lld) outside 0..%lld",
+                (long long)first, (long long)(first + count), (long long)m);
+  if (count == 0) return CFMM_OK;
+  if (!R) return fail(ctx, CFMM_ERR_INVALID, "null reserve array");
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  for (const Span& sp : split_range(ctx, type, first, count))
+    if ((rc = update_reserves_set(ctx, *sp.s, sp.first, sp.count, R + 2 * sp.offset)) != CFMM_OK) return rc;
   return CFMM_OK;
 }
 
@@ -1802,29 +1916,35 @@ int cfmm_update_univ3(cfmm_ctx* ctx, int64_t first, int64_t count, const double*
                       const double* liquidity) {
   int rc = ready(ctx);
   if (rc != CFMM_OK) return rc;
-  PoolSet& s = ctx->sets[CFMM_POOL_UNIV3];
-  if (first < 0 || count < 0 || first + count > s.m)
+  const int64_t m = type_pools(ctx, CFMM_POOL_UNIV3);
+  if (first < 0 || count < 0 || first + count > m)
     return fail(ctx, CFMM_ERR_INVALID, "update_univ3: range [%lld, %lld) outside 0..%lld",
-                (long long)first, (long long)(first + count), (long long)s.m);
+                (long long)first, (long long)(first + count), (long long)m);
   if (count == 0 || (!current_price && !liquidity)) return CFMM_OK;
+  const std::vector<Span> spans = split_range(ctx, CFMM_POOL_UNIV3, first, count);
   // validated like cfmm_add_univ3, all before any change: a rejected call changes no pool
   if (current_price)
-    for (int64_t j = 0; j < count; ++j)
-      if (!(s.first_lower[(size_t)(first + j)] >= current_price[j]))
-        return fail(ctx, CFMM_ERR_INVALID,
-                    "univ3 pool %lld: current_price above the first lower tick "
-                    "(current_tick == 0; BoundsError in the reference)",
-                    (long long)(first + j));
+    for (const Span& sp : spans)
+      for (int64_t j = 0; j < sp.count; ++j)
+        if (!(sp.s->first_lower[(size_t)(sp.first + j)] >= current_price[sp.offset + j]))
+          return fail(ctx, CFMM_ERR_INVALID,
+                      "univ3 pool %lld: current_price above the first lower tick "
+                      "(current_tick == 0; BoundsError in the reference)",
+                      (long long)(first + sp.offset + j));
   CU_TRY(ctx, cudaSetDevice(ctx->device));
   if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
   ctx->state_version++;
-  if (s.pos_of.empty()) {
-    s.pos_of.resize((size_t)s.m);
-    for (int64_t p = 0; p < s.m_padded; ++p)
-      if (s.order[(size_t)p] >= 0) s.pos_of[(size_t)s.order[(size_t)p]] = p;
+  int64_t tick_base = 0;  // liquidities of the parts before this one
+  for (const Span& sp : spans) {
+    PoolSet& s = *sp.s;
+    ensure_pos_of(s);
+    std::vector<int64_t> pos(s.pos_of.begin() + sp.first, s.pos_of.begin() + sp.first + sp.count);
+    rc = univ3_update_listed(ctx, s, pos, current_price ? current_price + sp.offset : nullptr,
+                             liquidity ? liquidity + tick_base : nullptr, current_price != nullptr);
+    if (rc != CFMM_OK) return rc;
+    for (int64_t j = 0; j < sp.count; ++j) tick_base += s.n_ticks[(size_t)(sp.first + j)];
   }
-  std::vector<int64_t> pos(s.pos_of.begin() + first, s.pos_of.begin() + first + count);
-  return univ3_update_listed(ctx, s, pos, current_price, liquidity, current_price != nullptr);
+  return CFMM_OK;
 }
 
 int cfmm_apply_trades(cfmm_ctx* ctx) {
@@ -1832,35 +1952,37 @@ int cfmm_apply_trades(cfmm_ctx* ctx) {
   if (rc != CFMM_OK) return rc;
   if (!ctx->has_trades)
     return fail(ctx, CFMM_ERR_STATE,
-                "no materialising sweep has run (call cfmm_sweep with materialize=1)");
+                "no materialising sweep has run since the last change of the pool set (call cfmm_sweep with materialize=1)");
   CU_TRY(ctx, cudaSetDevice(ctx->device));
   ctx->state_version++;
   if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
   DevBuf<int> flag;
   std::vector<int> zero(1, 0);
-  for (int t : {CFMM_POOL_PRODUCT, CFMM_POOL_GEOMEAN}) {
-    PoolSet& s = ctx->sets[t];
-    if (s.m == 0) continue;
-    if (s.d_outD.n != (size_t)s.m_padded)
-      return fail(ctx, CFMM_ERR_STATE, "trades of this pool type were never materialised");
-    CU_TRY(ctx, flag.upload(zero));
-    const int threads = 256;
-    cfmm::apply_trades_kernel<<<(unsigned)((s.m_padded + threads - 1) / threads), threads, 0, ctx->stream>>>(
-        s.d_R.p, s.d_gam.p, s.d_outD.p, s.d_outL.p, s.d_gidx.p, s.m_padded, flag.p);
-    ctx->launches++;
-    int h = 0;
-    cudaError_t e = cudaMemcpyAsync(&h, flag.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    flag.release();
-    if (e != cudaSuccess) return fail(ctx, CFMM_ERR_CUDA, "apply_trades failed: %s", cudaGetErrorString(e));
-    if (h) s.in_fast_range = false;  // later sweeps take the generic (guarded) form
-    if (s.tma_ok) {
-      int rc2 = refresh_scale(ctx, s);
-      if (rc2 != CFMM_OK) return rc2;
+  for (int t : {CFMM_POOL_PRODUCT, CFMM_POOL_GEOMEAN})
+    for (PoolSet* ps : {&ctx->sets[t], &ctx->tails[t]}) {
+      PoolSet& s = *ps;
+      if (s.m == 0) continue;
+      if (s.d_outD.n != (size_t)s.m_padded)
+        return fail(ctx, CFMM_ERR_STATE, "trades of this pool type were never materialised");
+      CU_TRY(ctx, flag.upload(zero));
+      const int threads = 256;
+      cfmm::apply_trades_kernel<<<(unsigned)((s.m_padded + threads - 1) / threads), threads, 0, ctx->stream>>>(
+          s.d_R.p, s.d_gam.p, s.d_outD.p, s.d_outL.p, s.d_gidx.p, s.m_padded, s.d_active.p, flag.p);
+      ctx->launches++;
+      int h = 0;
+      cudaError_t e = cudaMemcpyAsync(&h, flag.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+      flag.release();
+      if (e != cudaSuccess) return fail(ctx, CFMM_ERR_CUDA, "apply_trades failed: %s", cudaGetErrorString(e));
+      if (h) s.in_fast_range = false;  // later sweeps take the generic (guarded) form
+      if (s.tma_ok) {
+        int rc2 = refresh_scale(ctx, s);
+        if (rc2 != CFMM_OK) return rc2;
+      }
     }
-  }
-  PoolSet& u = ctx->sets[CFMM_POOL_UNIV3];
-  if (u.m > 0) {
+  for (PoolSet* ps : {&ctx->sets[CFMM_POOL_UNIV3], &ctx->tails[CFMM_POOL_UNIV3]}) {
+    PoolSet& u = *ps;
+    if (u.m == 0) continue;
     // new prices from the kept ν (univ3_move_kernel), then the state of the pools that moved
     DevBuf<int64_t> moved;
     DevBuf<unsigned long long> n_moved;
@@ -1883,6 +2005,319 @@ int cfmm_apply_trades(cfmm_ctx* ctx) {
   }
   return CFMM_OK;
 }
+
+// ---- pool membership after finalize: append, retire / restore, read back, compact ----------
+namespace {
+
+// Retire (active[j] == 0) or restore the pools [first, first + count) of one set.  Only pools
+// whose flag changes are touched; *changed counts them.
+int set_active_set(cfmm_ctx* ctx, int type, PoolSet& s, int64_t first, int64_t count, const uint8_t* active,
+                   int64_t* changed) {
+  ensure_pos_of(s);
+  if (s.retired.empty()) s.retired.assign((size_t)s.m, 0);
+  std::vector<int64_t> pos[2];
+  for (int64_t j = 0; j < count; ++j) {
+    const int want = active[j] ? 1 : 0;
+    if (want != (s.retired[(size_t)(first + j)] ? 0 : 1)) pos[want].push_back(s.pos_of[(size_t)(first + j)]);
+  }
+  *changed = (int64_t)(pos[0].size() + pos[1].size());
+  if (*changed == 0) return CFMM_OK;
+  const bool two_coin = type != CFMM_POOL_UNIV3;
+  if (!s.d_active.n) {
+    CU_TRY(ctx, s.d_active.alloc((size_t)s.m_padded));
+    CU_TRY(ctx, cudaMemsetAsync(s.d_active.p, 1, (size_t)s.m_padded, ctx->stream));
+    if (two_coin) CU_TRY(ctx, s.d_park.alloc((size_t)s.m_padded));
+  }
+  const int threads = 256;
+  for (int flag : {0, 1}) {
+    const int64_t n = (int64_t)pos[flag].size();
+    if (n == 0) continue;
+    DevBuf<int64_t> d_pos;
+    CU_TRY(ctx, d_pos.upload(pos[flag]));
+    cfmm::set_active_kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, ctx->stream>>>(
+        two_coin ? s.d_R.p : nullptr, s.d_park.p, s.d_active.p, d_pos.p, n, flag);
+    ctx->launches++;
+    CU_TRY(ctx, cudaGetLastError());
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  }
+  for (int64_t j = 0; j < count; ++j) s.retired[(size_t)(first + j)] = active[j] ? 0 : 1;
+  if (!two_coin) {  // tick records of the changed pools: zero liquidity while retired (univ3_state.cuh)
+    std::vector<int64_t> all(pos[0]);
+    all.insert(all.end(), pos[1].begin(), pos[1].end());
+    std::sort(all.begin(), all.end());
+    return univ3_update_listed(ctx, s, all, nullptr, nullptr, false);
+  }
+  return s.tma_ok ? refresh_scale(ctx, s) : CFMM_OK;
+}
+
+// After a new layout of s is uploaded (every pool active on the device), retire again the pools
+// s.retired lists.
+int reapply_retired(cfmm_ctx* ctx, int type, PoolSet& s) {
+  if (s.retired.empty()) return CFMM_OK;
+  std::vector<uint8_t> active((size_t)s.m);
+  for (int64_t i = 0; i < s.m; ++i) active[(size_t)i] = s.retired[(size_t)i] ? 0 : 1;
+  s.retired.clear();
+  int64_t changed = 0;
+  return set_active_set(ctx, type, s, 0, s.m, active.data(), &changed);
+}
+
+// Append the current state of every pool of src, in src's insertion order, to the host staging of
+// dst (and its retired flags): what cfmm_add_* would have staged for a pool set built afresh from
+// the device state.  Retired two-coin pools give their parked reserves.
+int read_back(cfmm_ctx* ctx, int type, PoolSet& src, PoolSet& dst) {
+  const int64_t m = src.m, mp = src.m_padded;
+  if (m == 0) return CFMM_OK;
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  auto d2h = [](void* dst_p, const void* src_p, size_t bytes) {
+    return cudaMemcpy(dst_p, src_p, bytes, cudaMemcpyDeviceToHost);
+  };
+  std::vector<double> gam((size_t)mp);
+  std::vector<int2> ai((size_t)mp);
+  std::vector<int64_t> gidx((size_t)mp);
+  CU_TRY(ctx, d2h(gam.data(), src.d_gam.p, (size_t)mp * sizeof(double)));
+  CU_TRY(ctx, d2h(ai.data(), src.d_Ai.p, (size_t)mp * sizeof(int2)));
+  CU_TRY(ctx, d2h(gidx.data(), src.d_gidx.p, (size_t)mp * sizeof(int64_t)));
+  std::vector<double2> R, park, w, f1;
+  std::vector<int2> tick;
+  std::vector<double> lower, liq;
+  if (type != CFMM_POOL_UNIV3) {
+    R.resize((size_t)mp);
+    CU_TRY(ctx, d2h(R.data(), src.d_R.p, (size_t)mp * sizeof(double2)));
+    if (src.d_park.n) {
+      park.resize((size_t)mp);
+      CU_TRY(ctx, d2h(park.data(), src.d_park.p, (size_t)mp * sizeof(double2)));
+    }
+  }
+  if (type == CFMM_POOL_GEOMEAN) {
+    w.resize((size_t)mp);
+    CU_TRY(ctx, d2h(w.data(), src.d_w.p, (size_t)mp * sizeof(double2)));
+  }
+  if (type == CFMM_POOL_UNIV3) {
+    f1.resize((size_t)m);
+    tick.resize((size_t)m);
+    lower.resize((size_t)src.total_ticks);
+    liq.resize((size_t)src.total_ticks);
+    CU_TRY(ctx, d2h(f1.data(), src.d_first[1].p, (size_t)m * sizeof(double2)));
+    CU_TRY(ctx, d2h(tick.data(), src.d_tick.p, (size_t)m * sizeof(int2)));
+    CU_TRY(ctx, d2h(lower.data(), src.d_lower.p, lower.size() * sizeof(double)));
+    CU_TRY(ctx, d2h(liq.data(), src.d_liq.p, liq.size() * sizeof(double)));
+  }
+  const size_t b = (size_t)dst.m, n = b + (size_t)m;
+  dst.gamma.resize(n);
+  dst.Ai.resize(2 * n);
+  dst.gidx.resize(n);
+  if (type != CFMM_POOL_UNIV3) dst.R.resize(2 * n);
+  if (type == CFMM_POOL_GEOMEAN) dst.w.resize(2 * n);
+  if (type == CFMM_POOL_UNIV3) dst.cp.resize(n);
+  if (!src.retired.empty() || !dst.retired.empty()) {
+    dst.retired.resize(n, 0);
+    if (!src.retired.empty()) std::copy(src.retired.begin(), src.retired.end(), dst.retired.begin() + b);
+  }
+  for (int64_t p = 0; p < mp; ++p) {
+    const int64_t i = src.order[(size_t)p];
+    if (i < 0) continue;  // padding
+    const size_t k = b + (size_t)i;
+    const bool sw = (gidx[(size_t)p] >> 62) & 1;
+    const int64_t ta = ai[(size_t)p].x + 1, tb = ai[(size_t)p].y + 1;
+    dst.gamma[k] = gam[(size_t)p];
+    dst.Ai[2 * k] = sw ? tb : ta;
+    dst.Ai[2 * k + 1] = sw ? ta : tb;
+    dst.gidx[k] = gidx[(size_t)p] & ~(1ll << 62);
+    if (type != CFMM_POOL_UNIV3) {
+      const bool parked = !park.empty() && !src.retired.empty() && src.retired[(size_t)i];
+      const double2 r = parked ? park[(size_t)p] : R[(size_t)p];
+      dst.R[2 * k] = sw ? r.y : r.x;
+      dst.R[2 * k + 1] = sw ? r.x : r.y;
+    }
+    if (type == CFMM_POOL_GEOMEAN) {
+      dst.w[2 * k] = w[(size_t)p].x;
+      dst.w[2 * k + 1] = w[(size_t)p].y;
+    }
+    if (type == CFMM_POOL_UNIV3) dst.cp[k] = f1[(size_t)p].y;
+  }
+  if (type == CFMM_POOL_UNIV3) {  // tick CSR in insertion order
+    ensure_pos_of(src);
+    if (dst.tick_off.empty()) dst.tick_off.push_back(0);
+    for (int64_t i = 0; i < m; ++i) {
+      const int64_t off = tick[(size_t)src.pos_of[(size_t)i]].x, nt = src.n_ticks[(size_t)i];
+      dst.lower.insert(dst.lower.end(), lower.begin() + off, lower.begin() + off + nt);
+      dst.liq.insert(dst.liq.end(), liq.begin() + off, liq.begin() + off + nt);
+      dst.tick_off.push_back((int64_t)dst.lower.size());
+    }
+  }
+  dst.m += m;
+  return CFMM_OK;
+}
+
+// Lay out the staged pools of `next` where `live` was, retire again what was retired, and swap
+// the new set in (the old one is released).
+int install_set(cfmm_ctx* ctx, int type, PoolSet& live, PoolSet& next, bool tail) {
+  int rc = upload_set(ctx, type, next, tail);
+  if (rc == CFMM_OK) rc = reapply_retired(ctx, type, next);
+  if (rc != CFMM_OK) {
+    next.release();
+    return rc;
+  }
+  std::swap(live, next);
+  next.release();
+  return CFMM_OK;
+}
+
+// cfmm_append_*: a new tail of one type = the current tail (its device state) + the new pools,
+// staged by `stage` after the arguments were checked.  O(tail), never touches the main set.
+int append_to_tail(cfmm_ctx* ctx, int type, const std::function<void(PoolSet&)>& stage) {
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  int rc = use_stream(ctx, ctx->stream);
+  if (rc != CFMM_OK) return rc;
+  PoolSet& tail = ctx->tails[type];
+  auto next = std::make_unique<PoolSet>();
+  if ((rc = read_back(ctx, type, tail, *next)) != CFMM_OK) return rc;
+  stage(*next);
+  if (!next->retired.empty()) next->retired.resize((size_t)next->m, 0);
+  if ((rc = install_set(ctx, type, tail, *next, true)) != CFMM_OK) return rc;
+  membership_changed(ctx);
+  return CFMM_OK;
+}
+
+int check_type(cfmm_ctx* ctx, int type) {
+  if (type != CFMM_POOL_PRODUCT && type != CFMM_POOL_GEOMEAN && type != CFMM_POOL_UNIV3)
+    return fail(ctx, CFMM_ERR_INVALID, "unknown pool type %d", type);
+  return CFMM_OK;
+}
+
+int check_range(cfmm_ctx* ctx, int type, int64_t first, int64_t count, const char* what) {
+  const int64_t m = type_pools(ctx, type);
+  if (first < 0 || count < 0 || first + count > m)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: range [%lld, %lld) outside 0..%lld", what, (long long)first,
+                (long long)(first + count), (long long)m);
+  return CFMM_OK;
+}
+
+}  // namespace
+
+int cfmm_append_product(cfmm_ctx* ctx, int64_t m, const double* R, const double* gamma, const int64_t* Ai) {
+  int rc = check_common(ctx, m, R, gamma, Ai, true);
+  if (rc != CFMM_OK || m == 0) return rc;
+  return append_to_tail(ctx, CFMM_POOL_PRODUCT, [&](PoolSet& s) { append_common(ctx, s, m, R, gamma, Ai); });
+}
+
+int cfmm_append_geomean(cfmm_ctx* ctx, int64_t m, const double* R, const double* gamma, const int64_t* Ai,
+                        const double* w) {
+  int rc = check_common(ctx, m, R, gamma, Ai, true);
+  if (rc != CFMM_OK) return rc;
+  if (m > 0 && !w) return fail(ctx, CFMM_ERR_INVALID, "null weight array");
+  if (m == 0) return CFMM_OK;
+  return append_to_tail(ctx, CFMM_POOL_GEOMEAN, [&](PoolSet& s) {
+    append_common(ctx, s, m, R, gamma, Ai);
+    s.w.insert(s.w.end(), w, w + 2 * m);
+  });
+}
+
+int cfmm_append_univ3(cfmm_ctx* ctx, int64_t m, const double* current_price, const double* gamma,
+                      const int64_t* Ai, const int64_t* tick_off, const double* lower_ticks,
+                      const double* liquidity) {
+  static const double dummy = 0.0;
+  int rc = check_common(ctx, m, m > 0 ? &dummy : nullptr, gamma, Ai, true);
+  if (rc != CFMM_OK || m == 0) return rc;
+  PoolSet& tail = ctx->tails[CFMM_POOL_UNIV3];
+  if ((rc = check_univ3(ctx, m, current_price, tick_off, lower_ticks, liquidity, tail.total_ticks)) != CFMM_OK)
+    return rc;
+  return append_to_tail(ctx, CFMM_POOL_UNIV3, [&](PoolSet& s) {
+    stage_univ3(ctx, s, m, current_price, gamma, Ai, tick_off, lower_ticks, liquidity);
+  });
+}
+
+int cfmm_set_active(cfmm_ctx* ctx, int type, int64_t first, int64_t count, const uint8_t* active) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if ((rc = check_type(ctx, type)) != CFMM_OK) return rc;
+  if ((rc = check_range(ctx, type, first, count, "set_active")) != CFMM_OK) return rc;
+  if (count == 0) return CFMM_OK;
+  if (!active) return fail(ctx, CFMM_ERR_INVALID, "null active array");
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  int64_t changed = 0;
+  for (const Span& sp : split_range(ctx, type, first, count)) {
+    int64_t c = 0;
+    rc = set_active_set(ctx, type, *sp.s, sp.first, sp.count, active + sp.offset, &c);
+    changed += c;
+    if (rc != CFMM_OK) break;
+  }
+  if (changed > 0) membership_changed(ctx);
+  return rc;
+}
+
+int cfmm_get_pool_state(cfmm_ctx* ctx, int type, int64_t first, int64_t count, double* state, uint8_t* active) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if ((rc = check_type(ctx, type)) != CFMM_OK) return rc;
+  if ((rc = check_range(ctx, type, first, count, "get_pool_state")) != CFMM_OK) return rc;
+  if (count == 0) return CFMM_OK;
+  if (!state) return fail(ctx, CFMM_ERR_INVALID, "null state array");
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  const int width = type == CFMM_POOL_UNIV3 ? 1 : 2;
+  for (const Span& sp : split_range(ctx, type, first, count)) {
+    PoolSet& s = *sp.s;
+    ensure_pos_of(s);
+    std::vector<int64_t> pos(s.pos_of.begin() + sp.first, s.pos_of.begin() + sp.first + sp.count);
+    DevBuf<int64_t> d_pos;
+    DevBuf<double> d_out;
+    CU_TRY(ctx, d_pos.upload(pos));
+    CU_TRY(ctx, d_out.alloc((size_t)(width * sp.count)));
+    const int threads = 256;
+    cfmm::gather_state_kernel<<<(unsigned)((sp.count + threads - 1) / threads), threads, 0, ctx->stream>>>(
+        s.d_R.p, s.d_park.p, s.d_active.p, type == CFMM_POOL_UNIV3 ? s.d_first[1].p : nullptr, s.d_gidx.p, d_pos.p,
+        sp.count, d_out.p);
+    ctx->launches++;
+    CU_TRY(ctx, cudaGetLastError());
+    CU_TRY(ctx, cudaMemcpyAsync(state + width * sp.offset, d_out.p, (size_t)(width * sp.count) * sizeof(double),
+                                cudaMemcpyDeviceToHost, ctx->stream));
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    if (active)
+      for (int64_t j = 0; j < sp.count; ++j)
+        active[sp.offset + j] = (s.retired.empty() || !s.retired[(size_t)(sp.first + j)]) ? 1 : 0;
+  }
+  return CFMM_OK;
+}
+
+int cfmm_compact(cfmm_ctx* ctx) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  for (int t = 0; t < 3; ++t) {
+    PoolSet &live = ctx->sets[t], &tail = ctx->tails[t];
+    if (live.m + tail.m == 0) continue;
+    auto next = std::make_unique<PoolSet>();
+    if ((rc = read_back(ctx, t, live, *next)) != CFMM_OK) return rc;
+    if ((rc = read_back(ctx, t, tail, *next)) != CFMM_OK) return rc;
+    if ((rc = install_set(ctx, t, live, *next, false)) != CFMM_OK) return rc;
+    auto empty = std::make_unique<PoolSet>();
+    tail.release();
+    std::swap(tail, *empty);
+  }
+  membership_changed(ctx);
+  return calibrate(ctx);
+}
+
+// Test hook: info[8] = {main-set pools, tail pools, main-set padded length, TMA layout built,
+// fixed-point Ψ slice allowed, compact stream allowed, every reserve in the guard-free range,
+// retired pools} of one pool type.
+int cfmm_debug_pool_set_info(cfmm_ctx* ctx, int type, int64_t* info) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if ((rc = check_type(ctx, type)) != CFMM_OK) return rc;
+  if (!info) return fail(ctx, CFMM_ERR_INVALID, "null info array");
+  const PoolSet &s = ctx->sets[type], &t = ctx->tails[type];
+  int64_t retired = 0;
+  for (const PoolSet* p : {&s, &t})
+    for (uint8_t r : p->retired) retired += r;
+  const int64_t v[8] = {s.m, t.m, s.m_padded, s.tma_ok, s.fixed_ok, s.compact_ok, s.in_fast_range, retired};
+  memcpy(info, v, sizeof(v));
+  return CFMM_OK;
+}
+
 
 int cfmm_set_option(cfmm_ctx* ctx, const char* key, int64_t value) {
   if (!ctx || !key) return CFMM_ERR_INVALID;
@@ -2031,7 +2466,7 @@ int cfmm_debug_product_layout(int64_t n_tokens, int64_t m, const int64_t* Ai, in
   fake.n_tokens = n_tokens;
   fake.tma_variant = variant;
   fake.orient_by_degree = orient;
-  const cfmm::PoolLayout lay = layout_for(&fake, CFMM_POOL_PRODUCT, Ai, m);
+  const cfmm::PoolLayout lay = layout_for(&fake, CFMM_POOL_PRODUCT, Ai, m, true);
   info[0] = lay.m_padded;
   info[1] = lay.nb;
   info[2] = lay.bucketed;

@@ -292,14 +292,16 @@ __global__ void scatter_trades_kernel(const double2* __restrict__ D,
 
 // R <- (R + γ·Δ) − Λ from the materialised trades of the same device order
 // (the update the reference's tests use, test/cfmms.jl:10: R⁺ = R + γ*Δ - Λ);
-// *out_of_range is raised when a new reserve leaves the guard-free range.
+// *out_of_range is raised when a new reserve leaves the guard-free range.  active (device order,
+// 0 = retired; null = all active) skips retired pools.
 __global__ void apply_trades_kernel(double2* __restrict__ R, const double* __restrict__ gam,
                                     const double2* __restrict__ D, const double2* __restrict__ L,
                                     const int64_t* __restrict__ gidx, int64_t m,
-                                    int* __restrict__ out_of_range) {
+                                    const uint8_t* __restrict__ active, int* __restrict__ out_of_range) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= m) return;
   if (gidx[i] < 0) return;  // padding pool
+  if (active && !active[i]) return;  // retired pool: its zeroed reserves stay, its state is parked
   const double g = gam[i];
   const double2 r = R[i], d = D[i], l = L[i];
   double2 n;
@@ -309,14 +311,61 @@ __global__ void apply_trades_kernel(double2* __restrict__ R, const double* __res
   if (!in_fast_range(n.x) || !in_fast_range(n.y)) atomicOr(out_of_range, 1);
 }
 
-// R[pos[j]] = newR[j]
+// R[pos[j]] = newR[j]; a retired pool (active[p] == 0; active may be null) gets it in its parked
+// state instead, which becomes live when the pool is restored
 __global__ void update_reserves_kernel(double2* __restrict__ R,
                                        const int64_t* __restrict__ pos,
                                        const double2* __restrict__ newR,
-                                       int64_t count) {
+                                       int64_t count, const uint8_t* __restrict__ active,
+                                       double2* __restrict__ park) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= count) return;
-  R[pos[j]] = newR[j];
+  const int64_t p = pos[j];
+  if (active && !active[p])
+    park[p] = newR[j];
+  else
+    R[p] = newR[j];
+}
+
+// Retire (flag 0) or restore (flag 1) the two-coin pools at device positions pos[j]: a retired
+// pool's reserves move to park and R becomes (0, 0), the no-trade state of the padding pools.
+// The host lists only pools whose flag changes.
+__global__ void set_active_kernel(double2* __restrict__ R, double2* __restrict__ park,
+                                  uint8_t* __restrict__ active, const int64_t* __restrict__ pos,
+                                  int64_t count, int flag) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= count) return;
+  const int64_t p = pos[j];
+  if (R) {
+    if (flag) {
+      R[p] = park[p];
+    } else {
+      park[p] = R[p];
+      R[p] = make_double2(0.0, 0.0);
+    }
+  }
+  active[p] = (uint8_t)flag;
+}
+
+// Pool state in listing order (cfmm_get_pool_state): the pools at device positions pos[j].  Two-coin
+// (R non-null): out[2j..2j+1] = the reserves as ingested (a pool stored with its tokens exchanged,
+// bit 62 of gidx, is swapped back), the parked ones for a retired pool.  UniV3 (price non-null,
+// the price word of f1): out[j] = the current price.
+__global__ void gather_state_kernel(const double2* __restrict__ R, const double2* __restrict__ park,
+                                    const uint8_t* __restrict__ active, const double2* __restrict__ price,
+                                    const int64_t* __restrict__ gidx, const int64_t* __restrict__ pos,
+                                    int64_t count, double* __restrict__ out) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= count) return;
+  const int64_t p = pos[j];
+  if (price) {
+    out[j] = price[p].y;
+    return;
+  }
+  const double2 r = (active && !active[p]) ? park[p] : R[p];
+  const bool swapped = (gidx[p] >> 62) & 1;
+  out[2 * j] = swapped ? r.y : r.x;
+  out[2 * j + 1] = swapped ? r.x : r.y;
 }
 
 }  // namespace cfmm

@@ -12,6 +12,8 @@
 //   tickdata   : two 32-byte direction records per tick (arb_math.cuh, kTickStride)
 //   f0..f3     : the current tick's records per pool (Univ3First)
 //   tick[p].y  : current_tick
+// A retired pool (cfmm_set_active; active[p] == 0) keeps its raw state; its derived records are
+// built with zero liquidity, so every tick is is_empty_pool and the sweep trades nothing.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -29,6 +31,7 @@ struct Univ3State {
   double* tickdata;     // kTickStride doubles per tick
   const double* lower;  // CSR, strictly decreasing within a pool
   double* liq;          // CSR
+  const uint8_t* active;  // device order, 0 = retired; null = every pool active
   int64_t m;
   int64_t total_ticks;
 };
@@ -116,6 +119,7 @@ __global__ void univ3_ticks_kernel(Univ3State s, const int64_t* __restrict__ pos
   } else {
     k = s.liq[q];
   }
+  if (s.active && !s.active[p]) k = 0.0;  // retired: empty ticks (the raw liquidity stays)
   const double price = univ3_price(s, p);
   const int cur = s.tick[p].y;
   const int idx = (int)ti + 1;  // 1-based
@@ -153,6 +157,7 @@ __global__ void univ3_move_kernel(Univ3State s, const double* __restrict__ gam, 
                                   unsigned long long* __restrict__ n_moved) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= s.m) return;
+  if (s.active && !s.active[p]) return;  // retired pools do not trade and do not move
   const double q = univ3_price(s, p), g = gam[p];
   const int2 ai = Ai[p];
   const double pr = __ddiv_rn(nu[ai.x], nu[ai.y]);

@@ -307,4 +307,30 @@ function sync_reserves!(r::B200Router)
     end
 end
 
+# Changing the pool set of one context after cfmm_finalize (cfmm_b200.h): pools appended with the
+# next insertion indices, pools retired and restored, the current state read back, the appended
+# pools folded into the main layout.  R, w: [2m] pool-major; Ai: [2m] 1-based; ptype: 0 / 1 / 2.
+append_product!(ctx, R::Vector{Float64}, γ::Vector{Float64}, Ai::Vector{Int64}) =
+    chk(ctx, ccall((:cfmm_append_product, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Float64}, Ptr{Float64}, Ptr{Int64}), ctx, length(γ), R, γ, Ai))
+append_geomean!(ctx, R::Vector{Float64}, γ::Vector{Float64}, Ai::Vector{Int64}, w::Vector{Float64}) =
+    chk(ctx, ccall((:cfmm_append_geomean, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Float64}, Ptr{Float64}, Ptr{Int64}, Ptr{Float64}), ctx, length(γ), R, γ, Ai, w))
+append_univ3!(ctx, cp::Vector{Float64}, γ::Vector{Float64}, Ai::Vector{Int64}, tick_off::Vector{Int64},
+              lower::Vector{Float64}, liq::Vector{Float64}) =
+    chk(ctx, ccall((:cfmm_append_univ3, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Float64}, Ptr{Float64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}),
+        ctx, length(cp), cp, γ, Ai, tick_off, lower, liq))
+set_active!(ctx, ptype::Integer, first::Integer, active::AbstractVector{Bool}) =
+    chk(ctx, ccall((:cfmm_set_active, LIB), Cint, (Ptr{Cvoid}, Cint, Int64, Int64, Ptr{UInt8}),
+        ctx, ptype, first, length(active), UInt8.(active)))
+function pool_state(ctx, ptype::Integer, first::Integer, count::Integer)
+    state = zeros(Float64, ptype == 2 ? count : 2count)
+    active = zeros(UInt8, count)
+    chk(ctx, ccall((:cfmm_get_pool_state, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Int64, Int64, Ptr{Float64}, Ptr{UInt8}), ctx, ptype, first, count, state, active))
+    return state, active .!= 0
+end
+compact!(ctx) = chk(ctx, ccall((:cfmm_compact, LIB), Cint, (Ptr{Cvoid},), ctx))
+
 end # module

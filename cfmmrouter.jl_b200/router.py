@@ -92,23 +92,32 @@ class DevicePools:
         _lib.check(self._lib, self._ctx, rc)
 
     def add_product(self, R, gamma, Ai):
+        self._product(self._lib.cfmm_add_product, R, gamma, Ai)
+
+    def add_geomean(self, R, gamma, Ai, w):
+        self._geomean(self._lib.cfmm_add_geomean, R, gamma, Ai, w)
+
+    def add_univ3(self, current_price, gamma, Ai, tick_off, lower_ticks, liquidity):
+        self._univ3(self._lib.cfmm_add_univ3, current_price, gamma, Ai, tick_off, lower_ticks, liquidity)
+
+    def _product(self, fn, R, gamma, Ai):
         R = np.ascontiguousarray(R, dtype=np.float64).reshape(-1, 2)
         gamma = np.ascontiguousarray(gamma, dtype=np.float64).reshape(-1)
         Ai = np.ascontiguousarray(Ai, dtype=np.int64).reshape(-1, 2)
         if not (len(R) == len(gamma) == len(Ai)):
             raise ValueError("R, gamma, Ai must describe the same number of pools")
-        self._chk(self._lib.cfmm_add_product(self._ctx, len(gamma), _dp(R), _dp(gamma), _ip(Ai)))
+        self._chk(fn(self._ctx, len(gamma), _dp(R), _dp(gamma), _ip(Ai)))
 
-    def add_geomean(self, R, gamma, Ai, w):
+    def _geomean(self, fn, R, gamma, Ai, w):
         R = np.ascontiguousarray(R, dtype=np.float64).reshape(-1, 2)
         w = np.ascontiguousarray(w, dtype=np.float64).reshape(-1, 2)
         gamma = np.ascontiguousarray(gamma, dtype=np.float64).reshape(-1)
         Ai = np.ascontiguousarray(Ai, dtype=np.int64).reshape(-1, 2)
         if not (len(R) == len(gamma) == len(Ai) == len(w)):
             raise ValueError("R, gamma, Ai, w must describe the same number of pools")
-        self._chk(self._lib.cfmm_add_geomean(self._ctx, len(gamma), _dp(R), _dp(gamma), _ip(Ai), _dp(w)))
+        self._chk(fn(self._ctx, len(gamma), _dp(R), _dp(gamma), _ip(Ai), _dp(w)))
 
-    def add_univ3(self, current_price, gamma, Ai, tick_off, lower_ticks, liquidity):
+    def _univ3(self, fn, current_price, gamma, Ai, tick_off, lower_ticks, liquidity):
         cp = np.ascontiguousarray(current_price, dtype=np.float64).reshape(-1)
         gamma = np.ascontiguousarray(gamma, dtype=np.float64).reshape(-1)
         Ai = np.ascontiguousarray(Ai, dtype=np.int64).reshape(-1, 2)
@@ -118,8 +127,7 @@ class DevicePools:
         if not (len(cp) == len(gamma) == len(Ai) == len(off) - 1) or len(lt) != len(lq) \
                 or (len(off) and off[-1] != len(lt)):
             raise ValueError("inconsistent UniV3 CSR arrays")
-        self._chk(self._lib.cfmm_add_univ3(self._ctx, len(cp), _dp(cp), _dp(gamma), _ip(Ai),
-                                           _ip(off), _dp(lt), _dp(lq)))
+        self._chk(fn(self._ctx, len(cp), _dp(cp), _dp(gamma), _ip(Ai), _ip(off), _dp(lt), _dp(lq)))
         self._univ3_ticks = np.concatenate([self._univ3_ticks, np.diff(off)])
 
     def add_file(self, path: str):
@@ -265,6 +273,50 @@ class DevicePools:
         self._chk(self._lib.cfmm_update_univ3(self._ctx, first, count, None if cp is None else _dp(cp),
                                               None if lq is None else _dp(lq)))
 
+    # -- changing the pool set after finalize (include/cfmm_b200.h) ---------------
+    def append_product(self, R, gamma, Ai):
+        """cfmm_append_product: ProductTwoCoin pools added after finalize (next insertion indices)."""
+        self._product(self._lib.cfmm_append_product, R, gamma, Ai)
+
+    def append_geomean(self, R, gamma, Ai, w):
+        self._geomean(self._lib.cfmm_append_geomean, R, gamma, Ai, w)
+
+    def append_univ3(self, current_price, gamma, Ai, tick_off, lower_ticks, liquidity):
+        self._univ3(self._lib.cfmm_append_univ3, current_price, gamma, Ai, tick_off, lower_ticks, liquidity)
+
+    def set_active(self, pool_type: int, first: int, active):
+        """cfmm_set_active: retire (False) or restore (True) the pools [first, first + len(active))
+        of one type, counted in that type's insertion order."""
+        a = np.ascontiguousarray(np.asarray(active).reshape(-1) != 0, dtype=np.uint8)
+        self._chk(self._lib.cfmm_set_active(self._ctx, int(pool_type), int(first), len(a),
+                                            a.ctypes.data_as(C.POINTER(C.c_uint8))))
+
+    def pool_state(self, pool_type: int, first: int = 0, count: int = None):
+        """cfmm_get_pool_state: (state, active) of the pools [first, first + count) of one type.
+        state: reserves (count, 2) for the two-coin types, current prices (count,) for UniV3;
+        active: bool (count,).  count defaults to the rest of the type's pools."""
+        if count is None:
+            info = self.pool_set_info(pool_type)
+            count = info["main"] + info["tail"] - int(first)
+        count = int(count)
+        width = 1 if pool_type == _lib.POOL_UNIV3 else 2
+        state = np.zeros(max(count, 0) * width)
+        active = np.zeros(max(count, 0), dtype=np.uint8)
+        self._chk(self._lib.cfmm_get_pool_state(self._ctx, int(pool_type), int(first), count, _dp(state),
+                                                active.ctypes.data_as(C.POINTER(C.c_uint8))))
+        return (state if width == 1 else state.reshape(-1, 2)), active.astype(bool)
+
+    def compact(self):
+        """cfmm_compact: fold the appended pools into the main layout (finalize's layout path)."""
+        self._chk(self._lib.cfmm_compact(self._ctx))
+
+    def pool_set_info(self, pool_type: int) -> dict:
+        """Layout facts of one pool type (cfmm_debug_pool_set_info; read-only)."""
+        info = np.zeros(8, dtype=np.int64)
+        self._chk(self._lib.cfmm_debug_pool_set_info(self._ctx, int(pool_type), _ip(info)))
+        keys = ("main", "tail", "padded", "tma", "fixed_point", "compact_stream", "fast_range", "retired")
+        return {k: int(x) for k, x in zip(keys, info)}
+
     # -- multi-GPU --------------------------------------------------------------
     def detach_group(self):
         self._chk(self._lib.cfmm_comm_detach(self._ctx))
@@ -338,7 +390,8 @@ class Router:
     Fields as in the reference: objective, cfmms, Δs, Λs, v.  Δs / Λs are
     (m, 2) arrays; Δs[i] / Λs[i] are the trade vectors of cfmms[i].  As in the
     reference (router.jl:39, loop bound length(r.Δs)), pools appended to
-    r.cfmms after construction are ignored.
+    r.cfmms after construction are ignored; add_cfmms adds pools to a built
+    router, and set_active retires and restores pools (single GPU).
 
     Multi-GPU: with `group` (a torch.distributed process group, one process per
     GPU) every rank holds the full Python pool list but uploads only its
@@ -367,6 +420,7 @@ class Router:
         self._exchange = exchange
         factory = _pools_factory or DevicePools
         self._pools = factory(int(n_tokens), device)
+        self._retired = np.zeros(m, dtype=bool)
         self._upload()
         if self._world > 1 and exchange == "peer":
             self._attach_with_agreement(group)
@@ -405,29 +459,76 @@ class Router:
     def _upload(self):
         shard = self.cfmms[self._lo:self._hi]
         idx = _pack(shard)
-        p = self._pools
-        order = []  # library global order -> shard-local list position
-        if idx[0]:
-            cs = [shard[i] for i in idx[0]]
-            p.add_product(np.array([c.R for c in cs]), np.array([c.gamma for c in cs]),
-                          np.array([c.Ai for c in cs]))
-            order += idx[0]
-        if idx[1]:
-            cs = [shard[i] for i in idx[1]]
-            p.add_geomean(np.array([c.R for c in cs]), np.array([c.gamma for c in cs]),
-                          np.array([c.Ai for c in cs]), np.array([c.w for c in cs]))
-            order += idx[1]
-        if idx[2]:
-            cs = [shard[i] for i in idx[2]]
-            off = np.concatenate([[0], np.cumsum([len(c.lower_ticks) for c in cs])]).astype(np.int64)
-            p.add_univ3(np.array([c.current_price for c in cs]), np.array([c.gamma for c in cs]),
-                        np.array([c.Ai for c in cs]), off,
-                        np.concatenate([c.lower_ticks for c in cs]),
-                        np.concatenate([c.liquidity for c in cs]))
-            order += idx[2]
-        p.finalize()
+        order = self._add(shard, idx, append=False)  # library global order -> shard-local list position
+        self._pools.finalize()
         self._order = np.asarray(order, dtype=np.int64)
         self._type_lists = idx
+
+    def _add(self, cs_all, idx, append):
+        """Hand the pools cs_all[idx[t]] to the library type by type (cfmm_add_* before finalize,
+        cfmm_append_* after); returns the positions in cs_all in the library's global order."""
+        p = self._pools
+        order = []
+        if idx[0]:
+            cs = [cs_all[i] for i in idx[0]]
+            (p.append_product if append else p.add_product)(
+                np.array([c.R for c in cs]), np.array([c.gamma for c in cs]), np.array([c.Ai for c in cs]))
+            order += idx[0]
+        if idx[1]:
+            cs = [cs_all[i] for i in idx[1]]
+            (p.append_geomean if append else p.add_geomean)(
+                np.array([c.R for c in cs]), np.array([c.gamma for c in cs]),
+                np.array([c.Ai for c in cs]), np.array([c.w for c in cs]))
+            order += idx[1]
+        if idx[2]:
+            cs = [cs_all[i] for i in idx[2]]
+            off = np.concatenate([[0], np.cumsum([len(c.lower_ticks) for c in cs])]).astype(np.int64)
+            (p.append_univ3 if append else p.add_univ3)(
+                np.array([c.current_price for c in cs]), np.array([c.gamma for c in cs]),
+                np.array([c.Ai for c in cs]), off, np.concatenate([c.lower_ticks for c in cs]),
+                np.concatenate([c.liquidity for c in cs]))
+            order += idx[2]
+        return order
+
+    def add_cfmms(self, cfmms):
+        """Add pools to a built router without rebuilding it (cfmm_append_*): they extend r.cfmms,
+        r.Δs and r.Λs, and trade from the next route on.  Single GPU."""
+        if self._world > 1:
+            raise NotImplementedError("add_cfmms drives one GPU")
+        new = list(cfmms)
+        if not new:
+            return
+        idx = _pack(new)
+        base = len(self.cfmms)
+        order = self._add(new, idx, append=True)
+        self.cfmms += new
+        self.Δs = np.concatenate([self.Δs, np.zeros((len(new), 2))])
+        self.Λs = np.concatenate([self.Λs, np.zeros((len(new), 2))])
+        self._retired = np.concatenate([self._retired, np.zeros(len(new), dtype=bool)])
+        self._order = np.concatenate([self._order, base + np.asarray(order, dtype=np.int64)])
+        self._hi = len(self.cfmms)
+        for t in (0, 1, 2):
+            self._type_lists[t] = self._type_lists[t] + [base + i for i in idx[t]]
+
+    def set_active(self, list_indices, flag: bool):
+        """Retire (flag False) or restore (True) the pools r.cfmms[i] for i in list_indices
+        (cfmm_set_active).  A retired pool trades nothing and update_reserves(r) leaves it as it
+        is; its trades read back as zero.  Single GPU."""
+        if self._world > 1:
+            raise NotImplementedError("set_active drives one GPU")
+        ids = np.unique(np.asarray(list_indices, dtype=np.int64).reshape(-1))
+        if len(ids) and (ids[0] < 0 or ids[-1] >= len(self.cfmms)):
+            raise IndexError("set_active: pool index out of range")
+        for t in (0, 1, 2):
+            local = {i: k for k, i in enumerate(self._type_lists[t])}
+            ks = sorted(local[i] for i in ids if i in local)
+            if not ks:
+                continue
+            span = np.array(self._type_lists[t][ks[0]:ks[-1] + 1])
+            active = ~self._retired[span]
+            active[np.asarray(ks) - ks[0]] = bool(flag)
+            self._pools.set_active(t, ks[0], active)
+            self._retired[span] = ~active
 
     # one find_arb!(r, v) + folds; caches Ψ and acc like the reference caches Δs/Λs
     def _sweep(self, v, materialize=False):
@@ -615,11 +716,13 @@ def update_reserves(r: Router):
     the device: R ← R + γΔ − Λ for the two-coin pools (test/cfmms.jl:10); a UniV3
     pool moves to the price its arbitrage walk traded it to (univ3_moved_price, at
     the ν of the last materialising sweep), with current_tick re-derived as the
-    constructor does."""
+    constructor does.  Retired pools (Router.set_active) are left unchanged."""
     v = getattr(r, "_v_mat", None)
     if v is None:
         v = r.v
-    for D, L, c in zip(r.Δs, r.Λs, r.cfmms):
+    for D, L, c, retired in zip(r.Δs, r.Λs, r.cfmms, r._retired):
+        if retired:  # retired pools keep their state (cfmm_set_active)
+            continue
         if isinstance(c, (ProductTwoCoin, GeometricMeanTwoCoin)):
             c.R = c.R + c.gamma * D - L  # same operation order as the device kernel: bit-identical
         elif isinstance(c, UniV3):

@@ -193,6 +193,51 @@ int cfmm_update_univ3(cfmm_ctx *ctx, int64_t first, int64_t count,
  * the device for the pools whose price changed. */
 int cfmm_apply_trades(cfmm_ctx *ctx);
 
+/* ---- changing the pool set after cfmm_finalize ------------------------------------------
+ * Pools are listed, drained and delisted while a caller routes block after block.  These
+ * entry points change the set without a rebuild (cfmm_destroy, cfmm_add_*, cfmm_finalize).
+ * Every change that alters the set (an append, a pool retired or restored, a compact) makes
+ * cfmm_get_trades and cfmm_apply_trades return CFMM_ERR_STATE until the next materialising
+ * sweep, and makes cfmm_sweep re-capture its graph.
+ *
+ * cfmm_append_*: the arguments and checks of the matching cfmm_add_*, valid only after
+ * cfmm_finalize (before it: CFMM_ERR_STATE); a rejected call changes nothing.  The new pools take
+ * the next global insertion indices (cfmm_num_pools grows) and the next indices of their type,
+ * so cfmm_update_reserves, cfmm_update_univ3, cfmm_get_trades and the calls below address them
+ * like ingested pools.  They live in a per-type tail, laid out like "tma_variant" -1 and swept
+ * by the first-generation kernel after the type's main set; an append re-lays out only the tail
+ * (from its current device state).  cfmm_compact folds the tails into the main layout. */
+int cfmm_append_product(cfmm_ctx *ctx, int64_t m, const double *R,
+                        const double *gamma, const int64_t *Ai);
+int cfmm_append_geomean(cfmm_ctx *ctx, int64_t m, const double *R,
+                        const double *gamma, const int64_t *Ai, const double *w);
+int cfmm_append_univ3(cfmm_ctx *ctx, int64_t m, const double *current_price,
+                      const double *gamma, const int64_t *Ai,
+                      const int64_t *tick_off, const double *lower_ticks,
+                      const double *liquidity);
+
+/* Retire (active[j] == 0) or restore (active[j] != 0) the pools [first, first+count) of one
+ * type, counted in that type's insertion order (appended pools included).  A retired pool
+ * trades exactly zero and adds nothing to psi or acc; cfmm_apply_trades leaves it unchanged
+ * (a UniV3 pool does not move).  Its state is kept: cfmm_update_reserves / cfmm_update_univ3
+ * on a retired pool store the pushed state, which becomes live when it is restored.  Retiring
+ * a retired pool or restoring an active one does nothing. */
+int cfmm_set_active(cfmm_ctx *ctx, int type, int64_t first, int64_t count,
+                    const uint8_t *active);
+
+/* The current state of the pools [first, first+count) of one type, in that type's insertion
+ * order: PRODUCT / GEOMEAN: the reserves, state [2*count] pool-major as cfmm_add_* takes them;
+ * UNIV3: the current price, state [count].  Retired pools report the state they keep.
+ * active (may be NULL): [count], 1 = active, 0 = retired. */
+int cfmm_get_pool_state(cfmm_ctx *ctx, int type, int64_t first, int64_t count,
+                        double *state, uint8_t *active);
+
+/* Fold every type's appended pools into its main layout: the current state of all pools is
+ * read back and laid out as cfmm_finalize does, with the same insertion indices (retired pools
+ * stay retired), and the finalize calibration sweeps run again.  Afterwards a gradient sweep is
+ * one launch per pool type again.  Costs about what cfmm_finalize costs. */
+int cfmm_compact(cfmm_ctx *ctx);
+
 /* ---- the outer iteration on the device (SURVEY §8f rank 2) ---------------------------
  * Minimises the dual g(nu) = lin' nu + sum_i arb_i(nu) over the box lower <= nu <= upper
  * -- route! (src/router.jl:58-108) for objectives of the form f(nu) = lin' nu on a box,
@@ -315,6 +360,10 @@ int cfmm_selftest_inrange_math(cfmm_ctx *ctx, const double *a, const double *b,
 int cfmm_debug_product_layout(int64_t n_tokens, int64_t m, const int64_t *Ai, int orient,
                               int variant, int64_t cap, int64_t *order_out,
                               int32_t *chunk_bucket_out, uint8_t *swapped_out, int64_t *info);
+/* Test hook: info[8] = {main-set pools, appended (tail) pools, main-set padded length, TMA
+ * layout built, fixed-point psi slice allowed, compact stream allowed, every reserve in the
+ * guard-free range, retired pools} of one pool type. */
+int cfmm_debug_pool_set_info(cfmm_ctx *ctx, int type, int64_t *info);
 /* Measurement hook (option "trace" = 1): per-CTA phase timestamps of the last TMA gradient
  * sweep, ns of %globaltimer: out[8 * grid] = {entry, price slice ready, own range done,
  * all chunks done, partials flushed, exit, grid barrier passed (fused exchange, else 0),
