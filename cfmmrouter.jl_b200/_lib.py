@@ -67,6 +67,8 @@ SYMBOLS = {
     "cfmm_set_active": (C.c_int, [_ctx, C.c_int, C.c_int64, C.c_int64, C.POINTER(C.c_uint8)]),
     "cfmm_get_pool_state": (C.c_int, [_ctx, C.c_int, C.c_int64, C.c_int64, _dp, C.POINTER(C.c_uint8)]),
     "cfmm_compact": (C.c_int, [_ctx]),
+    "cfmm_quote_swaps": (C.c_int, [_ctx, C.c_int, C.c_int64, _ip, _dp, _dp]),
+    "cfmm_execute_swaps": (C.c_int, [_ctx, C.c_int, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),
     "cfmm_set_option": (C.c_int, [_ctx, C.c_char_p, C.c_int64]),
     "cfmm_last_sweep_ms": (C.c_int, [_ctx, C.POINTER(C.c_float)]),

@@ -30,6 +30,7 @@
 #include "sweep_kernels.cuh"
 #include "product_tma.cuh"
 #include "solver.cuh"
+#include "swap_kernels.cuh"
 #include "univ3_state.cuh"
 
 namespace {
@@ -241,7 +242,7 @@ struct cfmm_ctx {
   // optional per-kernel timing (option "profile"): event pairs per launch
   struct Prof {
     std::vector<cudaEvent_t> ev;  // 2 per recorded launch
-    std::vector<int> type;        // pool type (3 = peer exchange)
+    std::vector<int> type;        // pool type (3 = peer exchange, 4 = swap kernels)
     size_t used = 0;              // launches recorded
   } prof;
 };
@@ -2278,6 +2279,197 @@ int cfmm_get_pool_state(cfmm_ctx* ctx, int type, int64_t first, int64_t count, d
       for (int64_t j = 0; j < sp.count; ++j)
         active[sp.offset + j] = (s.retired.empty() || !s.retired[(size_t)(sp.first + j)]) ? 1 : 0;
   }
+  return CFMM_OK;
+}
+
+// ---- swaps: quotes and in-order execution (swap_kernels.cuh) ----------------------------
+namespace {
+
+// Every argument of cfmm_quote_swaps / cfmm_execute_swaps, checked on the host before any launch.
+int check_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const double* tender,
+                const double* received, bool need_received, const char* what) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if ((rc = check_type(ctx, type)) != CFMM_OK) return rc;
+  if (q < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: negative row count", what);
+  if (q > 0 && (!pool || !tender || (need_received && !received)))
+    return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
+  const int64_t m = type_pools(ctx, type);
+  for (int64_t j = 0; j < q; ++j) {
+    if (pool[j] < 0 || pool[j] >= m)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: pool %lld outside 0..%lld", what, (long long)j,
+                  (long long)pool[j], (long long)m);
+    const double x1 = tender[2 * j], x2 = tender[2 * j + 1];
+    if (!std::isfinite(x1) || !std::isfinite(x2) || x1 < 0.0 || x2 < 0.0)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: tender (%g, %g) must be finite and >= 0", what,
+                  (long long)j, x1, x2);
+    if (x1 > 0.0 && x2 > 0.0)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: tender (%g, %g) has both sides > 0", what, (long long)j,
+                  x1, x2);
+  }
+  return CFMM_OK;
+}
+
+constexpr int kProfSwaps = 4;  // cfmm_profile_read: the swap kernels' slot
+
+cfmm::SwapSet swap_set(PoolSet& s) {
+  cfmm::SwapSet w;
+  w.R = s.d_R.p;
+  w.gam = s.d_gam.p;
+  w.w = s.d_w.p;
+  w.gidx = s.d_gidx.p;
+  w.active = s.d_active.p;
+  w.u = univ3_state(s);
+  return w;
+}
+
+// The rows of one call that fall in one set (main or tail): row index and device position.
+struct SetRows {
+  PoolSet* s;
+  std::vector<int64_t> row, pos;
+};
+
+std::vector<SetRows> rows_by_set(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool) {
+  std::vector<SetRows> out{{&ctx->sets[type], {}, {}}, {&ctx->tails[type], {}, {}}};
+  const int64_t m_main = ctx->sets[type].m;
+  for (SetRows& r : out) ensure_pos_of(*r.s);
+  for (int64_t j = 0; j < q; ++j) {
+    SetRows& r = out[pool[j] < m_main ? 0 : 1];
+    r.row.push_back(j);
+    r.pos.push_back(r.s->pos_of[(size_t)(pool[j] < m_main ? pool[j] : pool[j] - m_main)]);
+  }
+  return out;
+}
+
+}  // namespace
+
+// launch KERNEL<type> (the pool type as a template argument) with the arguments that follow
+#define CFMM_SWAP_LAUNCH(type, KERNEL, blocks, st, ...)                                      \
+  do {                                                                                        \
+    if ((type) == CFMM_POOL_PRODUCT) KERNEL<0><<<(blocks), 256, 0, (st)>>>(__VA_ARGS__);      \
+    else if ((type) == CFMM_POOL_GEOMEAN) KERNEL<1><<<(blocks), 256, 0, (st)>>>(__VA_ARGS__); \
+    else KERNEL<2><<<(blocks), 256, 0, (st)>>>(__VA_ARGS__);                                  \
+  } while (0)
+
+int cfmm_quote_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const double* tender,
+                     double* received) {
+  int rc = check_swaps(ctx, type, q, pool, tender, received, true, "quote_swaps");
+  if (rc != CFMM_OK || q == 0) return rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  DevBuf<double> d_tender, d_recv;
+  CU_TRY(ctx, d_tender.alloc((size_t)(2 * q)));
+  CU_TRY(ctx, DevBuf<double>::copy_in(d_tender.p, tender, (size_t)(2 * q) * sizeof(double)));
+  CU_TRY(ctx, d_recv.alloc((size_t)(2 * q)));
+  for (SetRows& r : rows_by_set(ctx, type, q, pool)) {
+    const int64_t n = (int64_t)r.row.size();
+    if (n == 0) continue;
+    DevBuf<int64_t> d_row, d_pos;
+    CU_TRY(ctx, d_row.upload(r.row));
+    CU_TRY(ctx, d_pos.upload(r.pos));
+    const cfmm::SwapSet ss = swap_set(*r.s);
+    const unsigned blocks = (unsigned)((n + 255) / 256);
+    {
+      ProfScope prof(ctx, kProfSwaps, ctx->stream);
+      CFMM_SWAP_LAUNCH(type, cfmm::swap_quote_kernel, blocks, ctx->stream, ss, d_row.p, d_pos.p, n, d_tender.p,
+                       d_recv.p);
+    }
+    ctx->launches++;
+    CU_TRY(ctx, cudaGetLastError());
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // (d_row, d_pos are freed at the end of the block)
+  }
+  CU_TRY(ctx, cudaMemcpyAsync(received, d_recv.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
+                              ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return CFMM_OK;
+}
+
+int cfmm_execute_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const double* tender,
+                       double* received) {
+  int rc = check_swaps(ctx, type, q, pool, tender, received, false, "execute_swaps");
+  if (rc != CFMM_OK || q == 0) return rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  ctx->state_version++;
+  DevBuf<double> d_tender, d_recv;
+  CU_TRY(ctx, d_tender.alloc((size_t)(2 * q)));
+  CU_TRY(ctx, DevBuf<double>::copy_in(d_tender.p, tender, (size_t)(2 * q) * sizeof(double)));
+  CU_TRY(ctx, d_recv.alloc((size_t)(2 * q)));
+  for (SetRows& r : rows_by_set(ctx, type, q, pool)) {
+    PoolSet& s = *r.s;
+    const int64_t n = (int64_t)r.row.size();
+    if (n == 0) continue;
+    // group the rows by pool, batch order kept inside each pool: a stable counting sort on the
+    // device position (a stable comparison sort when the batch is small against the set)
+    std::vector<int64_t> seg_rows((size_t)n), seg_pos, seg_off;
+    if (n * 8 >= s.m_padded) {
+      std::vector<int64_t> start((size_t)s.m_padded + 1, 0);
+      for (int64_t j = 0; j < n; ++j) start[(size_t)r.pos[(size_t)j] + 1]++;
+      for (int64_t p = 0; p < s.m_padded; ++p) {
+        if (start[(size_t)p + 1] > 0) {
+          seg_pos.push_back(p);
+          seg_off.push_back(start[(size_t)p]);
+        }
+        start[(size_t)p + 1] += start[(size_t)p];
+      }
+      for (int64_t j = 0; j < n; ++j) seg_rows[(size_t)start[(size_t)r.pos[(size_t)j]]++] = r.row[(size_t)j];
+    } else {
+      std::vector<int64_t> idx((size_t)n);
+      for (int64_t j = 0; j < n; ++j) idx[(size_t)j] = j;
+      std::stable_sort(idx.begin(), idx.end(),
+                       [&](int64_t a, int64_t b) { return r.pos[(size_t)a] < r.pos[(size_t)b]; });
+      for (int64_t j = 0; j < n; ++j) {
+        const int64_t p = r.pos[(size_t)idx[(size_t)j]];
+        if (seg_pos.empty() || seg_pos.back() != p) {
+          seg_pos.push_back(p);
+          seg_off.push_back(j);
+        }
+        seg_rows[(size_t)j] = r.row[(size_t)idx[(size_t)j]];
+      }
+    }
+    seg_off.push_back(n);
+    const int64_t n_seg = (int64_t)seg_pos.size();
+    DevBuf<int64_t> d_seg_pos, d_seg_off, d_seg_rows, d_moved;
+    DevBuf<unsigned long long> d_n_moved;
+    DevBuf<int> d_flag;
+    CU_TRY(ctx, d_seg_pos.upload(seg_pos));
+    CU_TRY(ctx, d_seg_off.upload(seg_off));
+    CU_TRY(ctx, d_seg_rows.upload(seg_rows));
+    CU_TRY(ctx, d_n_moved.alloc(1));
+    CU_TRY(ctx, d_flag.alloc(1));
+    if (type == CFMM_POOL_UNIV3) CU_TRY(ctx, d_moved.alloc((size_t)n_seg));
+    CU_TRY(ctx, cudaMemsetAsync(d_n_moved.p, 0, sizeof(unsigned long long), ctx->stream));
+    CU_TRY(ctx, cudaMemsetAsync(d_flag.p, 0, sizeof(int), ctx->stream));
+    const cfmm::SwapSet ss = swap_set(s);
+    const unsigned blocks = (unsigned)((n_seg + 255) / 256);
+    {
+      ProfScope prof(ctx, kProfSwaps, ctx->stream);
+      CFMM_SWAP_LAUNCH(type, cfmm::swap_execute_kernel, blocks, ctx->stream, ss, d_seg_pos.p, d_seg_off.p,
+                       d_seg_rows.p, n_seg, d_tender.p, d_recv.p, d_moved.p, d_n_moved.p, d_flag.p);
+    }
+    ctx->launches++;
+    CU_TRY(ctx, cudaGetLastError());
+    unsigned long long h_moved = 0;
+    int h_flag = 0;
+    CU_TRY(ctx, cudaMemcpyAsync(&h_moved, d_n_moved.p, sizeof(h_moved), cudaMemcpyDeviceToHost, ctx->stream));
+    CU_TRY(ctx, cudaMemcpyAsync(&h_flag, d_flag.p, sizeof(h_flag), cudaMemcpyDeviceToHost, ctx->stream));
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    if (type == CFMM_POOL_UNIV3) {
+      if (h_moved > 0) {  // the derived state of the pools that moved, as after cfmm_apply_trades
+        std::vector<int64_t> moved((size_t)h_moved);
+        CU_TRY(ctx, cudaMemcpy(moved.data(), d_moved.p, (size_t)h_moved * sizeof(int64_t), cudaMemcpyDeviceToHost));
+        std::sort(moved.begin(), moved.end());
+        if ((rc = univ3_update_listed(ctx, s, moved, nullptr, nullptr, true)) != CFMM_OK) return rc;
+      }
+    } else {
+      if (h_flag) s.in_fast_range = false;  // later sweeps take the generic (guarded) form
+      if (s.tma_ok && (rc = refresh_scale(ctx, s)) != CFMM_OK) return rc;
+    }
+  }
+  if (received)
+    CU_TRY(ctx, cudaMemcpyAsync(received, d_recv.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
+                                ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return CFMM_OK;
 }
 

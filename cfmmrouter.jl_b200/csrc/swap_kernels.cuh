@@ -1,0 +1,219 @@
+// swap_kernels.cuh -- quotes and in-order execution of swaps against the device-resident pools
+// (sm_90a; cfmm_quote_swaps / cfmm_execute_swaps, include/cfmm_b200.h).  Off the sweep path:
+// no sweep kernel reads anything these kernels add.
+//
+// A row is a tender (x1, x2) of one pool, at most one side > 0.  With δ = γ·x (forward_trade's
+// γ*Δ[1], src/cfmms.jl:445) the amount received on the other side is
+//   ProductTwoCoin        forward_amount of the BoundedProduct (R₁R₂, 0, 0, R₁, R₂) (:411-414):
+//                         λ₂ = min(R₂, R₂ − k/(R₁ + δ)), k = R₁·R₂
+//   GeometricMeanTwoCoin  from the invariant R₁^w₁·R₂^w₂: λ₂ = R₂·(1 − (R₁/(R₁+δ))^η), η = w₁/w₂,
+//                         evaluated as −R₂·expm1(−η·log1p(δ/R₁)) and clamped to [0, R₂]
+//   UniV3                 forward_trade (:436-449): the tick walk of trade_through_pools over the
+//                         upper ticks (token 1) or the flipped lower ticks (token 2)
+// and symmetrically for a token-2 tender.  Execute moves a two-coin pool to (R + γΔ) − Λ (the
+// operations of apply_trades_kernel) and a UniV3 pool to the price its walk ended at
+// (univ3_walk).  Tender and received are in the pool's ingest token order; a ProductTwoCoin pool
+// stored with its tokens exchanged (bit 62 of gidx) is exchanged on the way in and out.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "arb_math.cuh"
+#include "univ3_state.cuh"
+
+namespace cfmm {
+
+// The arrays of one pool set (main or tail) the swap kernels read and write, in device order.
+struct SwapSet {
+  double2* R;             // two-coin reserves, stored order
+  const double* gam;
+  const double2* w;       // GeometricMeanTwoCoin weights (null for the other types)
+  const int64_t* gidx;    // global insertion index; bit 62 = stored with its tokens exchanged
+  const uint8_t* active;  // 0 = retired; null = every pool active
+  Univ3State u;           // UniV3 only
+};
+
+// λ out of a two-coin pool for a net tender d of the token whose reserve is r_in (weights: w_in
+// of the tendered token, w_out of the other; GeometricMeanTwoCoin only).
+template <int TYPE>
+__device__ __forceinline__ double two_coin_out(double r_in, double r_out, double d, double w_in, double w_out) {
+  if constexpr (TYPE == 0) {
+    const double k = __dmul_rn(r_in, r_out);
+    const double l = __dsub_rn(r_out, __ddiv_rn(k, __dadd_rn(r_in, d)));
+    return r_out < l ? r_out : l;  // min(R₂, λ) of forward_amount (NaN propagates as there)
+  } else {
+    const double eta = __ddiv_rn(w_in, w_out);
+    const double u = __dmul_rn(eta, log1p(__ddiv_rn(d, r_in)));
+    const double l = __dmul_rn(r_out, -expm1(-u));
+    return l < 0.0 ? 0.0 : (l > r_out ? r_out : l);
+  }
+}
+
+// Λ of the tender (x1, x2), both in stored order, against reserves r (stored order).
+template <int TYPE>
+__device__ __forceinline__ double2 two_coin_quote(double2 r, double g, double2 w, double x1, double x2) {
+  if (x1 > 0.0) return make_double2(0.0, two_coin_out<TYPE>(r.x, r.y, __dmul_rn(g, x1), w.x, w.y));
+  if (x2 > 0.0) return make_double2(two_coin_out<TYPE>(r.y, r.x, __dmul_rn(g, x2), w.y, w.x), 0.0);
+  return make_double2(0.0, 0.0);
+}
+
+struct Univ3Walk {
+  double lambda;  // received
+  double price;   // q′ (== the start price when !moved)
+  bool moved;
+};
+
+// forward_trade of one UniV3 pool (src/cfmms.jl:401-449) from the raw state: ticks lower[0..nt),
+// liquidities liq[0..nt), at `price` with current tick cur (1-based), for the net tender d of
+// token 1 (tok1) or token 2.  The walk visits cur, cur+1, .. nt (token 1) or cur, cur-1, .. 1
+// (token 2, on the flipped ticks), each tick through univ3_compute_at_tick, and stops in the
+// first tick whose max_amount_pos exceeds what is left of d.  max_amount_pos follows the
+// reference's branch: an empty tick (k = 0) gives 0 rather than k/β − (R₁+α) = NaN.
+// The new price (include/cfmm_b200.h, cfmm_execute_swaps): inside the ending tick idx with δ′
+// left, y = (R₁+α) + δ′ and q′ = (k/y)/y (token 1) or y = (R₂+β) + δ′ and q′ = (y/k)·y (token 2),
+// clamped to [lo(idx), hi(idx)]; after the walk exhausted every non-empty tick it reached, the
+// far boundary of the last one (lo for token 1, hi for token 2); unchanged if it walked none.
+__device__ __forceinline__ Univ3Walk univ3_walk(const double* lower, const double* liq, int nt, double price,
+                                                int cur, double d, bool tok1) {
+  Univ3Walk r;
+  r.price = price;
+  r.moved = false;
+  double lam = 0.0;
+  int last = 0;  // last non-empty tick walked (0 = none)
+  const int step = tok1 ? 1 : -1;
+  for (int idx = cur; tok1 ? idx <= nt : idx >= 1; idx += step) {
+    const double hi = lower[idx - 1], lo = idx < nt ? lower[idx] : 0.0;
+    const Univ3Tick t = univ3_compute_at_tick(liq[idx - 1], hi, lo, price, idx, cur);
+    // flip_sides (src/cfmms.jl:289) for a token-2 tender
+    const double a = tok1 ? t.alpha : t.beta, b = tok1 ? t.beta : t.alpha;
+    const double r_in = tok1 ? t.R1 : t.R2, r_out = tok1 ? t.R2 : t.R1;
+    const double ra = __dadd_rn(r_in, a);
+    const double mx = b > 0.0 ? __dsub_rn(__ddiv_rn(t.k, b), ra) : (a > 0.0 ? __longlong_as_double(0x7ff0000000000000ll) : 0.0);
+    if (mx > d) {
+      const double y = __dadd_rn(ra, d);
+      double l = __dsub_rn(__dadd_rn(r_out, b), __ddiv_rn(t.k, y));
+      l = r_out < l ? r_out : l;
+      r.lambda = __dadd_rn(lam, l);
+      double q = tok1 ? __ddiv_rn(__ddiv_rn(t.k, y), y) : __dmul_rn(__ddiv_rn(y, t.k), y);
+      q = q < lo ? lo : (q > hi ? hi : q);
+      r.price = q;
+      r.moved = true;
+      return r;
+    }
+    lam = __dadd_rn(lam, r_out);
+    d = __dsub_rn(d, mx);
+    if (t.k != 0.0) last = idx;
+  }
+  r.lambda = lam;
+  if (last > 0) {
+    r.price = tok1 ? (last < nt ? lower[last] : 0.0) : lower[last - 1];
+    r.moved = true;
+  }
+  return r;
+}
+
+// Quotes: one thread per row.  rows[j] is the row's index in the call (tender / received
+// [2·row, 2·row+1], ingest order), pos[j] its pool's device position in this set.
+template <int TYPE>
+__global__ void swap_quote_kernel(SwapSet s, const int64_t* __restrict__ rows, const int64_t* __restrict__ pos,
+                                  int64_t n, const double* __restrict__ tender, double* __restrict__ received) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const int64_t row = rows[j], p = pos[j];
+  double2 out = make_double2(0.0, 0.0);
+  if (!s.active || s.active[p]) {
+    const double x1 = tender[2 * row], x2 = tender[2 * row + 1];
+    if constexpr (TYPE == 2) {
+      if (x1 > 0.0 || x2 > 0.0) {
+        const int off = s.u.tick[p].x, nt = univ3_tick_end(s.u, p) - off;
+        const bool tok1 = x1 > 0.0;
+        const Univ3Walk wk = univ3_walk(s.u.lower + off, s.u.liq + off, nt, univ3_price(s.u, p), s.u.tick[p].y,
+                                        __dmul_rn(s.gam[p], tok1 ? x1 : x2), tok1);
+        out = tok1 ? make_double2(0.0, wk.lambda) : make_double2(wk.lambda, 0.0);
+      }
+    } else {
+      const bool sw = (s.gidx[p] >> 62) & 1;
+      const double2 w = TYPE == 1 ? s.w[p] : make_double2(0.0, 0.0);
+      const double2 l = two_coin_quote<TYPE>(s.R[p], s.gam[p], w, sw ? x2 : x1, sw ? x1 : x2);
+      out = sw ? make_double2(l.y, l.x) : l;
+    }
+  }
+  received[2 * row] = out.x;
+  received[2 * row + 1] = out.y;
+}
+
+// Execution: one thread per distinct pool.  seg_pos[k] is the k-th pool's device position, its
+// rows are seg_rows[seg_off[k] .. seg_off[k+1]) in batch order.  The thread reads the pool's
+// state once, applies the rows in order (each sees the ones before it), writes every row's
+// received and the final state once.  Two-coin: *out_of_range is raised when a new reserve
+// leaves the guard-free range.  UniV3: the new price goes to the price word of f1, and pools
+// whose price changed are listed in moved (their derived state is rebuilt afterwards by
+// univ3_current_tick_kernel / univ3_ticks_kernel, as after cfmm_apply_trades).
+template <int TYPE>
+__global__ void swap_execute_kernel(SwapSet s, const int64_t* __restrict__ seg_pos,
+                                    const int64_t* __restrict__ seg_off, const int64_t* __restrict__ seg_rows,
+                                    int64_t n_seg, const double* __restrict__ tender,
+                                    double* __restrict__ received, int64_t* __restrict__ moved,
+                                    unsigned long long* __restrict__ n_moved, int* __restrict__ out_of_range) {
+  const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n_seg) return;
+  const int64_t p = seg_pos[k], r0 = seg_off[k], r1 = seg_off[k + 1];
+  if (s.active && !s.active[p]) {  // retired: receives nothing, its parked state stays
+    for (int64_t r = r0; r < r1; ++r) {
+      const int64_t row = seg_rows[r];
+      received[2 * row] = 0.0;
+      received[2 * row + 1] = 0.0;
+    }
+    return;
+  }
+  const double g = s.gam[p];
+  if constexpr (TYPE == 2) {
+    const int off = s.u.tick[p].x, nt = univ3_tick_end(s.u, p) - off;
+    const double* lower = s.u.lower + off;
+    const double q0 = univ3_price(s.u, p);
+    double q = q0;
+    int cur = s.u.tick[p].y;
+    for (int64_t r = r0; r < r1; ++r) {
+      const int64_t row = seg_rows[r];
+      const double x1 = tender[2 * row], x2 = tender[2 * row + 1];
+      double2 out = make_double2(0.0, 0.0);
+      if (x1 > 0.0 || x2 > 0.0) {
+        const bool tok1 = x1 > 0.0;
+        const Univ3Walk wk = univ3_walk(lower, s.u.liq + off, nt, q, cur, __dmul_rn(g, tok1 ? x1 : x2), tok1);
+        out = tok1 ? make_double2(0.0, wk.lambda) : make_double2(wk.lambda, 0.0);
+        if (wk.moved) {
+          q = wk.price;
+          cur = univ3_tick_of(lower, nt, q);
+        }
+      }
+      received[2 * row] = out.x;
+      received[2 * row + 1] = out.y;
+    }
+    if (q != q0) {
+      reinterpret_cast<double*>(s.u.f1 + p)[1] = q;
+      moved[atomicAdd(n_moved, 1ull)] = p;
+    }
+  } else {
+    const bool sw = (s.gidx[p] >> 62) & 1;
+    const double2 w = TYPE == 1 ? s.w[p] : make_double2(0.0, 0.0);
+    double2 R = s.R[p];
+    for (int64_t r = r0; r < r1; ++r) {
+      const int64_t row = seg_rows[r];
+      const double x1 = tender[2 * row], x2 = tender[2 * row + 1];
+      double2 out = make_double2(0.0, 0.0);
+      if (x1 > 0.0 || x2 > 0.0) {
+        const double d1 = sw ? x2 : x1, d2 = sw ? x1 : x2;
+        const double2 l = two_coin_quote<TYPE>(R, g, w, d1, d2);
+        R.x = __dsub_rn(__dadd_rn(R.x, __dmul_rn(g, d1)), l.x);  // (R + γΔ) − Λ, as apply_trades_kernel
+        R.y = __dsub_rn(__dadd_rn(R.y, __dmul_rn(g, d2)), l.y);
+        out = sw ? make_double2(l.y, l.x) : l;
+      }
+      received[2 * row] = out.x;
+      received[2 * row + 1] = out.y;
+    }
+    s.R[p] = R;
+    if (!in_fast_range(R.x) || !in_fast_range(R.y)) atomicOr(out_of_range, 1);
+  }
+}
+
+}  // namespace cfmm

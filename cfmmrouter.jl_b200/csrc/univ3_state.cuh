@@ -44,10 +44,23 @@ __device__ __forceinline__ int univ3_tick_end(const Univ3State& s, int64_t p) {
   return p + 1 < s.m ? s.tick[p + 1].x : (int)s.total_ticks;
 }
 
+// searchsortedlast(lower_ticks, price, rev=true) (src/cfmms.jl:235) over one pool's nt ticks,
+// i.e. the number of leading ticks >= price.  The ticks are strictly decreasing, so the leading
+// run is found by bisection; ties count as >=, a NaN price gives 0 (both as the linear count).
+__device__ __forceinline__ int univ3_tick_of(const double* lower, int nt, double price) {
+  int lo = 0, hi = nt;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (lower[mid] >= price)
+      lo = mid + 1;
+    else
+      hi = mid;
+  }
+  return lo;
+}
+
 // current_tick of pools pos[j] (pos == nullptr: pool j), j < count, after an optional price
-// push new_price[j]: searchsortedlast(lower_ticks, price, rev=true) (src/cfmms.jl:235), i.e. the
-// number of leading ticks >= price.  The ticks are strictly decreasing, so the leading run is
-// found by bisection; ties count as >=, a NaN price gives 0 (both as the linear count).
+// push new_price[j] (univ3_tick_of).
 __global__ void univ3_current_tick_kernel(Univ3State s, const int64_t* __restrict__ pos,
                                           const double* __restrict__ new_price, int64_t count) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -61,22 +74,35 @@ __global__ void univ3_current_tick_kernel(Univ3State s, const int64_t* __restric
     price = univ3_price(s, p);
   }
   const int off = s.tick[p].x, nt = univ3_tick_end(s, p) - off;
-  int lo = 0, hi = nt;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (s.lower[off + mid] >= price)
-      lo = mid + 1;
-    else
-      hi = mid;
-  }
-  reinterpret_cast<int*>(s.tick + p)[1] = lo;
+  reinterpret_cast<int*>(s.tick + p)[1] = univ3_tick_of(s.lower + off, nt, price);
+}
+
+// One tick's BoundedProduct (src/cfmms.jl:272-278) from the raw state.
+struct Univ3Tick {
+  double k, alpha, beta, R1, R2;
+};
+
+// compute_at_tick (src/cfmms.jl:294-313): tick idx (1-based) of a pool at `price` whose current
+// tick is cur, with liquidity k and bounds pplus = lower_ticks[idx], pminus = lower_ticks[idx+1]
+// (0 for the last tick).  IEEE operations in the reference's order, written as intrinsics because
+// nvcc contracts a*b+c to an FMA by default.  The library's only copy of this arithmetic: the
+// tick records (univ3_ticks_kernel) and the swap walks (swap_kernels.cuh) both call it.
+__device__ __forceinline__ Univ3Tick univ3_compute_at_tick(double k, double pplus, double pminus, double price,
+                                                           int idx, int cur) {
+  Univ3Tick t;
+  t.k = k;
+  t.alpha = __dsqrt_rn(__ddiv_rn(k, pplus));
+  t.beta = __dsqrt_rn(__dmul_rn(k, pminus));
+  const double pp = idx > cur ? pplus : (idx < cur ? pminus : price);
+  t.R1 = __dsub_rn(__dsqrt_rn(__ddiv_rn(k, pp)), t.alpha);
+  t.R2 = __dsub_rn(__dsqrt_rn(__dmul_rn(k, pp)), t.beta);
+  return t;
 }
 
 // compute_at_tick (src/cfmms.jl:294-313) for every tick of pools pos[j] (pos == nullptr: of all
 // pools), one thread per tick: cum[j] .. cum[j+1]-1 are the listed pools' ticks in listing order
 // (cum == nullptr: the device CSR itself).  new_liq (optional, indexed like the listing) is
-// stored first.  IEEE operations in the reference's order, written as intrinsics because nvcc
-// contracts a*b+c to an FMA by default: the records are bit-identical to compute_at_tick's.
+// stored first.  The records are bit-identical to compute_at_tick's (univ3_compute_at_tick).
 __global__ void univ3_ticks_kernel(Univ3State s, const int64_t* __restrict__ pos,
                                    const int64_t* __restrict__ cum, int64_t count, int64_t n_ticks,
                                    const double* __restrict__ new_liq) {
@@ -125,11 +151,8 @@ __global__ void univ3_ticks_kernel(Univ3State s, const int64_t* __restrict__ pos
   const int idx = (int)ti + 1;  // 1-based
   const double pplus = s.lower[q];                            // tick_high_price :252
   const double pminus = ti + 1 < nt ? s.lower[q + 1] : 0.0;   // tick_low_price :255-259
-  const double alpha = __dsqrt_rn(__ddiv_rn(k, pplus));
-  const double beta = __dsqrt_rn(__dmul_rn(k, pminus));
-  const double pp = idx > cur ? pplus : (idx < cur ? pminus : price);
-  const double R1 = __dsub_rn(__dsqrt_rn(__ddiv_rn(k, pp)), alpha);
-  const double R2 = __dsub_rn(__dsqrt_rn(__dmul_rn(k, pp)), beta);
+  const Univ3Tick tk = univ3_compute_at_tick(k, pplus, pminus, price, idx, cur);
+  const double alpha = tk.alpha, beta = tk.beta, R1 = tk.R1, R2 = tk.R2;
   const double ra = __dadd_rn(R1, alpha);
   const double rb = __dadd_rn(R2, beta);
   const double dmax_up = __dsub_rn(__ddiv_rn(k, beta), ra);

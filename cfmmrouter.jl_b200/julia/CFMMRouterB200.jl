@@ -333,4 +333,24 @@ function pool_state(ctx, ptype::Integer, first::Integer, count::Integer)
 end
 compact!(ctx) = chk(ctx, ccall((:cfmm_compact, LIB), Cint, (Ptr{Cvoid},), ctx))
 
+# Swaps against the device-resident pools (cfmm_quote_swaps / cfmm_execute_swaps).  pools are
+# 0-based indices in the type's insertion order; tender is 2 x q (column j = row j's Δ in the
+# pool's token order); both return received as 2 x q.  Like the rest of this file, never executed.
+function quote_swaps(ctx, ptype::Integer, pools::Vector{Int64}, tender::Matrix{Float64})
+    size(tender) == (2, length(pools)) || throw(ArgumentError("tender must be 2 x length(pools)"))
+    received = zeros(Float64, 2, length(pools))
+    chk(ctx, ccall((:cfmm_quote_swaps, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Int64, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}),
+        ctx, ptype, length(pools), pools, tender, received))
+    return received
+end
+function execute_swaps!(ctx, ptype::Integer, pools::Vector{Int64}, tender::Matrix{Float64})
+    size(tender) == (2, length(pools)) || throw(ArgumentError("tender must be 2 x length(pools)"))
+    received = zeros(Float64, 2, length(pools))
+    chk(ctx, ccall((:cfmm_execute_swaps, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Int64, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}),
+        ctx, ptype, length(pools), pools, tender, received))
+    return received
+end
+
 end # module

@@ -310,6 +310,34 @@ class DevicePools:
         """cfmm_compact: fold the appended pools into the main layout (finalize's layout path)."""
         self._chk(self._lib.cfmm_compact(self._ctx))
 
+    # -- swaps (include/cfmm_b200.h, cfmm_quote_swaps / cfmm_execute_swaps) ---------------
+    @staticmethod
+    def _swap_args(pools, tender):
+        pools = np.ascontiguousarray(pools, dtype=np.int64).reshape(-1)
+        tender = np.ascontiguousarray(tender, dtype=np.float64)
+        if tender.ndim != 2 or tender.shape[1] != 2 or len(tender) != len(pools):
+            raise ValueError(f"tender must have shape ({len(pools)}, 2), one row per pool index")
+        return pools, tender
+
+    def quote_swaps(self, pool_type: int, pools, tender):
+        """cfmm_quote_swaps: what each row (pools[j], tender[j]) would receive, every row priced on
+        the current state on its own; no state changes.  pools: indices in the type's insertion
+        order; tender: (q, 2) in each pool's token order.  Returns received (q, 2)."""
+        pools, tender = self._swap_args(pools, tender)
+        out = np.zeros((len(pools), 2))
+        self._chk(self._lib.cfmm_quote_swaps(self._ctx, int(pool_type), len(pools), _ip(pools), _dp(tender),
+                                             _dp(out)))
+        return out
+
+    def execute_swaps(self, pool_type: int, pools, tender):
+        """cfmm_execute_swaps: apply the rows in batch order (a row sees every earlier row on the same
+        pool) and return what each row received, (q, 2)."""
+        pools, tender = self._swap_args(pools, tender)
+        out = np.zeros((len(pools), 2))
+        self._chk(self._lib.cfmm_execute_swaps(self._ctx, int(pool_type), len(pools), _ip(pools), _dp(tender),
+                                               _dp(out)))
+        return out
+
     def pool_set_info(self, pool_type: int) -> dict:
         """Layout facts of one pool type (cfmm_debug_pool_set_info; read-only)."""
         info = np.zeros(8, dtype=np.int64)
@@ -529,6 +557,61 @@ class Router:
             active[np.asarray(ks) - ks[0]] = bool(flag)
             self._pools.set_active(t, ks[0], active)
             self._retired[span] = ~active
+
+    def _swap_rows(self, list_indices, tenders, what):
+        """Per pool type: (rows of the call, type-local pool indices) of the pools r.cfmms[i]."""
+        if self._world > 1:
+            raise NotImplementedError(f"{what} drives one GPU")
+        ids = np.asarray(list_indices, dtype=np.int64).reshape(-1)
+        tenders = np.ascontiguousarray(tenders, dtype=np.float64)
+        if tenders.shape != (len(ids), 2):
+            raise ValueError(f"{what}: tenders must have shape ({len(ids)}, 2)")
+        if len(ids) and (ids.min() < 0 or ids.max() >= len(self.cfmms)):
+            raise IndexError(f"{what}: pool index out of range")
+        kind = np.full(len(self.cfmms), -1, dtype=np.int64)
+        local = np.zeros(len(self.cfmms), dtype=np.int64)
+        for t in (0, 1, 2):
+            lst = np.asarray(self._type_lists[t], dtype=np.int64)
+            kind[lst] = t
+            local[lst] = np.arange(len(lst))
+        groups = []
+        for t in (0, 1, 2):
+            rows = np.flatnonzero(kind[ids] == t)
+            if len(rows):
+                groups.append((t, rows, local[ids[rows]]))
+        return ids, tenders, groups
+
+    def quote_swaps(self, list_indices, tenders):
+        """What tendering tenders[j] (in the pool's token order) to r.cfmms[list_indices[j]] pays
+        out, every row on the current state on its own (cfmm_quote_swaps); no state changes.
+        Returns received (q, 2) in the caller's order.  Single GPU."""
+        ids, tenders, groups = self._swap_rows(list_indices, tenders, "quote_swaps")
+        out = np.zeros((len(ids), 2))
+        for t, rows, loc in groups:
+            out[rows] = self._pools.quote_swaps(t, loc, tenders[rows])
+        return out
+
+    def execute_swaps(self, list_indices, tenders):
+        """Execute the swaps in order (cfmm_execute_swaps): each row sees every earlier row on the
+        same pool.  Returns received (q, 2) in the caller's order and refreshes the touched pool
+        objects (R, or current_price / current_tick) from the device state.  Single GPU."""
+        ids, tenders, groups = self._swap_rows(list_indices, tenders, "execute_swaps")
+        out = np.zeros((len(ids), 2))
+        for t, rows, loc in groups:
+            out[rows] = self._pools.execute_swaps(t, loc, tenders[rows])
+        for t, rows, loc in groups:
+            touched = np.unique(loc)
+            lo, hi = int(touched[0]), int(touched[-1]) + 1
+            state, _ = self._pools.pool_state(t, lo, hi - lo)
+            lst = self._type_lists[t]
+            for k in touched:
+                c = self.cfmms[lst[k]]
+                if t == _lib.POOL_UNIV3:
+                    c.current_price = float(state[k - lo])
+                    c.current_tick = int(np.sum(c.lower_ticks >= c.current_price))
+                else:
+                    c.R = state[k - lo].copy()
+        return out
 
     # one find_arb!(r, v) + folds; caches Ψ and acc like the reference caches Δs/Λs
     def _sweep(self, v, materialize=False):

@@ -238,6 +238,52 @@ int cfmm_get_pool_state(cfmm_ctx *ctx, int type, int64_t first, int64_t count,
  * one launch per pool type again.  Costs about what cfmm_finalize costs. */
 int cfmm_compact(cfmm_ctx *ctx);
 
+/* ---- swaps against the device-resident pools ------------------------------------------
+ * q swaps on pools of one type.  pool: [q] indices in that type's insertion order (appended
+ * pools included).  tender: [2q] pool-major Δ, in the pool's ingest token order (Ai as given to
+ * cfmm_add_*): each row (x, 0), (0, x) or (0, 0) with x finite and >= 0.  received: [2q] Λ,
+ * nonzero only on the side opposite the tender.
+ *
+ * cfmm_quote_swaps prices every row against the current state on its own (rows on the same pool
+ * do not see each other) and changes no state.  cfmm_execute_swaps applies the rows in batch
+ * order: a row sees the effect of every earlier row on the same pool, and received holds what
+ * each row actually got (the semantics of replaying a block).  Afterwards the state version
+ * moves (captured sweep graphs see the new state), the guard-free range flag and the fixed-point
+ * scale follow the new reserves, and the materialised trades (cfmm_get_trades) stay as they are.
+ *
+ * Both are synchronous.  Before cfmm_finalize they return CFMM_ERR_STATE; a bad type, an index
+ * outside the type's pools, a NaN / Inf / negative tender or a row with both sides > 0 gives
+ * CFMM_ERR_INVALID.  Every argument is checked before anything runs: a rejected call changes no
+ * pool.  Retired pools (cfmm_set_active) receive (0, 0) and keep their state, parked or not.
+ *
+ * Trade rules, with δ = γ·x the tender net of the fee (forward_trade's γ*Δ[1], src/cfmms.jl:445),
+ * for a tender of token 1 (token 2 is symmetric):
+ *   ProductTwoCoin        λ₂ = min(R₂, R₂ − k/(R₁ + δ)), k = R₁·R₂: forward_amount of the
+ *                         BoundedProduct (k, 0, 0, R₁, R₂) in the reference's operation order (bit
+ *                         for bit; a tender below about eps·R₁ can give a λ a few ulp below zero,
+ *                         as there).
+ *   GeometricMeanTwoCoin  λ₂ = R₂·(1 − (R₁/(R₁ + δ))^η), η = w₁/w₂, clamped to [0, R₂]; evaluated as
+ *                         −R₂·expm1(−η·log1p(δ/R₁)), within (4 + 2η)·eps·R₂ of the exact value.
+ *   UniV3                 received = forward_trade(Δ, cfmm) (src/cfmms.jl:436-449), bit for bit: the
+ *                         tick walk from the current tick through the upper ticks (token 1) or the
+ *                         flipped lower ticks (token 2); empty ticks are walked through.
+ * Execute, two-coin: R <- (R + γΔ) − Λ, the IEEE operations of cfmm_apply_trades.
+ * Execute, UniV3: liquidity and ticks stay, the price moves to q′ (each step one IEEE operation):
+ *   walk ended inside tick idx with δ′ left:  token 1: y = (R₁+α) + δ′, q′ = (k/y)/y
+ *                                             token 2: y = (R₂+β) + δ′, q′ = (y/k)·y
+ *                                             clamped to [lo(idx), hi(idx)], hi(idx) =
+ *                                             lower_ticks[idx], lo(idx) = lower_ticks[idx+1] (0 for
+ *                                             the last tick)
+ *   walk exhausted every non-empty tick it reached: the far boundary of the last non-empty tick
+ *                                             walked, lo(j) (token 1) or hi(j) (token 2)
+ *   tender (0, 0), or no non-empty tick walked: unchanged
+ *   then current_tick = searchsortedlast(lower_ticks, q′, rev=true) and the tick records are
+ *   rebuilt as after cfmm_update_univ3. */
+int cfmm_quote_swaps(cfmm_ctx *ctx, int type, int64_t q, const int64_t *pool,
+                     const double *tender, double *received);
+int cfmm_execute_swaps(cfmm_ctx *ctx, int type, int64_t q, const int64_t *pool,
+                       const double *tender, double *received /* may be NULL */);
+
 /* ---- the outer iteration on the device (SURVEY §8f rank 2) ---------------------------
  * Minimises the dual g(nu) = lin' nu + sum_i arb_i(nu) over the box lower <= nu <= upper
  * -- route! (src/router.jl:58-108) for objectives of the form f(nu) = lin' nu on a box,
@@ -337,8 +383,9 @@ int64_t cfmm_launch_count(const cfmm_ctx *ctx);
 /* Per-kernel device timing.  cfmm_set_option(ctx, "profile", N) arms CUDA-event
  * pairs for the next N kernel launches (recorded on the launching stream,
  * around each sweep kernel / the peer exchange).  cfmm_profile_read sums the
- * durations recorded so far for one pool type (cfmm_pool_type, or 3 = the
- * multi-GPU exchange kernel); it synchronises on the recorded events.
+ * durations recorded so far for one pool type (cfmm_pool_type, 3 = the multi-GPU
+ * exchange kernel, or 4 = the kernels of cfmm_quote_swaps / cfmm_execute_swaps); it
+ * synchronises on the recorded events.
  * cfmm_profile_reset re-arms the same N pairs. */
 int cfmm_profile_read(cfmm_ctx *ctx, int type, double *total_ms, int64_t *launches);
 /* The individual durations (ms) behind cfmm_profile_read, in launch order: fills
