@@ -69,6 +69,8 @@ SYMBOLS = {
     "cfmm_compact": (C.c_int, [_ctx]),
     "cfmm_quote_swaps": (C.c_int, [_ctx, C.c_int, C.c_int64, _ip, _dp, _dp]),
     "cfmm_execute_swaps": (C.c_int, [_ctx, C.c_int, C.c_int64, _ip, _dp, _dp]),
+    "cfmm_modify_univ3_liquidity": (C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
+    "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),
     "cfmm_set_option": (C.c_int, [_ctx, C.c_char_p, C.c_int64]),
     "cfmm_last_sweep_ms": (C.c_int, [_ctx, C.POINTER(C.c_float)]),

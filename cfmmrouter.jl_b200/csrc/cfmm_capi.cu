@@ -2341,6 +2341,46 @@ std::vector<SetRows> rows_by_set(cfmm_ctx* ctx, int type, int64_t q, const int64
   return out;
 }
 
+// The rows of one set grouped by pool, batch order kept inside each pool: pos[j] is the j-th
+// touched device position (ascending), rows[off[j] .. off[j+1]) its row indices.  A stable
+// counting sort on the device position (a stable comparison sort when the batch is small against
+// the set).
+struct PoolGroups {
+  std::vector<int64_t> pos, off, rows;
+};
+
+PoolGroups group_by_pool(const SetRows& r, int64_t m_padded) {
+  const int64_t n = (int64_t)r.row.size();
+  PoolGroups g;
+  g.rows.resize((size_t)n);
+  if (n * 8 >= m_padded) {
+    std::vector<int64_t> start((size_t)m_padded + 1, 0);
+    for (int64_t j = 0; j < n; ++j) start[(size_t)r.pos[(size_t)j] + 1]++;
+    for (int64_t p = 0; p < m_padded; ++p) {
+      if (start[(size_t)p + 1] > 0) {
+        g.pos.push_back(p);
+        g.off.push_back(start[(size_t)p]);
+      }
+      start[(size_t)p + 1] += start[(size_t)p];
+    }
+    for (int64_t j = 0; j < n; ++j) g.rows[(size_t)start[(size_t)r.pos[(size_t)j]]++] = r.row[(size_t)j];
+  } else {
+    std::vector<int64_t> idx((size_t)n);
+    for (int64_t j = 0; j < n; ++j) idx[(size_t)j] = j;
+    std::stable_sort(idx.begin(), idx.end(), [&](int64_t a, int64_t b) { return r.pos[(size_t)a] < r.pos[(size_t)b]; });
+    for (int64_t j = 0; j < n; ++j) {
+      const int64_t p = r.pos[(size_t)idx[(size_t)j]];
+      if (g.pos.empty() || g.pos.back() != p) {
+        g.pos.push_back(p);
+        g.off.push_back(j);
+      }
+      g.rows[(size_t)j] = r.row[(size_t)idx[(size_t)j]];
+    }
+  }
+  g.off.push_back(n);
+  return g;
+}
+
 }  // namespace
 
 // launch KERNEL<type> (the pool type as a template argument) with the arguments that follow
@@ -2399,42 +2439,14 @@ int cfmm_execute_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, 
     PoolSet& s = *r.s;
     const int64_t n = (int64_t)r.row.size();
     if (n == 0) continue;
-    // group the rows by pool, batch order kept inside each pool: a stable counting sort on the
-    // device position (a stable comparison sort when the batch is small against the set)
-    std::vector<int64_t> seg_rows((size_t)n), seg_pos, seg_off;
-    if (n * 8 >= s.m_padded) {
-      std::vector<int64_t> start((size_t)s.m_padded + 1, 0);
-      for (int64_t j = 0; j < n; ++j) start[(size_t)r.pos[(size_t)j] + 1]++;
-      for (int64_t p = 0; p < s.m_padded; ++p) {
-        if (start[(size_t)p + 1] > 0) {
-          seg_pos.push_back(p);
-          seg_off.push_back(start[(size_t)p]);
-        }
-        start[(size_t)p + 1] += start[(size_t)p];
-      }
-      for (int64_t j = 0; j < n; ++j) seg_rows[(size_t)start[(size_t)r.pos[(size_t)j]]++] = r.row[(size_t)j];
-    } else {
-      std::vector<int64_t> idx((size_t)n);
-      for (int64_t j = 0; j < n; ++j) idx[(size_t)j] = j;
-      std::stable_sort(idx.begin(), idx.end(),
-                       [&](int64_t a, int64_t b) { return r.pos[(size_t)a] < r.pos[(size_t)b]; });
-      for (int64_t j = 0; j < n; ++j) {
-        const int64_t p = r.pos[(size_t)idx[(size_t)j]];
-        if (seg_pos.empty() || seg_pos.back() != p) {
-          seg_pos.push_back(p);
-          seg_off.push_back(j);
-        }
-        seg_rows[(size_t)j] = r.row[(size_t)idx[(size_t)j]];
-      }
-    }
-    seg_off.push_back(n);
-    const int64_t n_seg = (int64_t)seg_pos.size();
+    const PoolGroups seg = group_by_pool(r, s.m_padded);
+    const int64_t n_seg = (int64_t)seg.pos.size();
     DevBuf<int64_t> d_seg_pos, d_seg_off, d_seg_rows, d_moved;
     DevBuf<unsigned long long> d_n_moved;
     DevBuf<int> d_flag;
-    CU_TRY(ctx, d_seg_pos.upload(seg_pos));
-    CU_TRY(ctx, d_seg_off.upload(seg_off));
-    CU_TRY(ctx, d_seg_rows.upload(seg_rows));
+    CU_TRY(ctx, d_seg_pos.upload(seg.pos));
+    CU_TRY(ctx, d_seg_off.upload(seg.off));
+    CU_TRY(ctx, d_seg_rows.upload(seg.rows));
     CU_TRY(ctx, d_n_moved.alloc(1));
     CU_TRY(ctx, d_flag.alloc(1));
     if (type == CFMM_POOL_UNIV3) CU_TRY(ctx, d_moved.alloc((size_t)n_seg));
@@ -2470,6 +2482,247 @@ int cfmm_execute_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, 
     CU_TRY(ctx, cudaMemcpyAsync(received, d_recv.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
                                 ctx->stream));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return CFMM_OK;
+}
+
+// ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------
+namespace {
+
+int check_liquidity_rows(cfmm_ctx* ctx, int64_t q, const int64_t* pool, const double* range, const double* dL) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if (q < 0) return fail(ctx, CFMM_ERR_INVALID, "modify_univ3_liquidity: negative row count");
+  if (q > 0 && (!pool || !range || !dL)) return fail(ctx, CFMM_ERR_INVALID, "modify_univ3_liquidity: null array argument");
+  const int64_t m = type_pools(ctx, CFMM_POOL_UNIV3);
+  for (int64_t j = 0; j < q; ++j) {
+    if (pool[j] < 0 || pool[j] >= m)
+      return fail(ctx, CFMM_ERR_INVALID, "modify_univ3_liquidity: row %lld: pool %lld outside 0..%lld", (long long)j,
+                  (long long)pool[j], (long long)m);
+    const double lo = range[2 * j], hi = range[2 * j + 1];
+    if (!std::isfinite(lo) || !std::isfinite(hi) || !(lo > 0.0) || !(lo < hi))
+      return fail(ctx, CFMM_ERR_INVALID, "modify_univ3_liquidity: row %lld: range (%g, %g) needs 0 < lo < hi, both finite",
+                  (long long)j, lo, hi);
+    if (!std::isfinite(dL[j]) || dL[j] == 0.0)
+      return fail(ctx, CFMM_ERR_INVALID, "modify_univ3_liquidity: row %lld: dL %g must be finite and != 0", (long long)j,
+                  dL[j]);
+  }
+  return CFMM_OK;
+}
+
+// One set's part of a cfmm_modify_univ3_liquidity call: the touched pools' new ladders (stage A,
+// listing order) and, when tick counts change, the set's new CSR arrays (stage B).
+struct LiquidityStage {
+  PoolSet* s = nullptr;
+  PoolGroups g;
+  std::vector<int64_t> new_nt, cum;   // per touched pool: new tick count, listing offsets [n + 1]
+  std::vector<double> top;            // per touched pool: its highest candidate boundary
+  int64_t growth = 0;                 // ticks added to the set
+  DevBuf<int64_t> d_pos, d_row_off, d_rows, d_cum;
+  DevBuf<double> d_lower, d_liq;      // stage-A ladders
+  DevBuf<double> n_lower, n_liq, n_tickdata;  // stage B, growth > 0 only
+  DevBuf<int2> n_tick;
+};
+
+// Stage A of one set: merge, inherit, apply; nothing of the set is written.
+int liquidity_stage(cfmm_ctx* ctx, LiquidityStage& st, const SetRows& r, const double* range,
+                    const double* d_range, const double* d_dL, unsigned long long* d_bad) {
+  PoolSet& s = *st.s;
+  st.g = group_by_pool(r, s.m_padded);
+  const int64_t n = (int64_t)st.g.pos.size();
+  std::vector<int64_t> cand_off(1, 0);
+  std::vector<double> cand;
+  st.top.resize((size_t)n);
+  for (int64_t j = 0; j < n; ++j) {
+    const size_t b = cand.size();
+    for (int64_t k = st.g.off[(size_t)j]; k < st.g.off[(size_t)j + 1]; ++k) {
+      const int64_t row = st.g.rows[(size_t)k];
+      cand.push_back(range[2 * row]);
+      cand.push_back(range[2 * row + 1]);
+    }
+    std::sort(cand.begin() + b, cand.end(), std::greater<double>());
+    cand.erase(std::unique(cand.begin() + b, cand.end()), cand.end());
+    st.top[(size_t)j] = cand[b];
+    cand_off.push_back((int64_t)cand.size());
+  }
+  DevBuf<int64_t> d_cand_off, d_nt;
+  DevBuf<double> d_cand;
+  CU_TRY(ctx, st.d_pos.upload(st.g.pos));
+  CU_TRY(ctx, st.d_row_off.upload(st.g.off));
+  CU_TRY(ctx, st.d_rows.upload(st.g.rows));
+  CU_TRY(ctx, d_cand_off.upload(cand_off));
+  CU_TRY(ctx, d_cand.upload(cand));
+  CU_TRY(ctx, d_nt.alloc((size_t)n));
+  const cfmm::Univ3State u = univ3_state(s);
+  const int threads = 256;
+  const unsigned pool_blocks = (unsigned)((n + threads - 1) / threads);
+  cfmm::univ3_liq_ladder_kernel<<<pool_blocks, threads, 0, ctx->stream>>>(u, st.d_pos.p, d_cand_off.p, d_cand.p, n,
+                                                                          d_nt.p, nullptr, nullptr, nullptr);
+  ctx->launches++;
+  CU_TRY(ctx, cudaGetLastError());
+  st.new_nt.resize((size_t)n);
+  CU_TRY(ctx, cudaMemcpyAsync(st.new_nt.data(), d_nt.p, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost,
+                              ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  st.cum.assign((size_t)n + 1, 0);
+  for (int64_t j = 0; j < n; ++j) {
+    st.cum[(size_t)j + 1] = st.cum[(size_t)j] + st.new_nt[(size_t)j];
+    st.growth += st.new_nt[(size_t)j] - s.n_ticks[(size_t)s.order[(size_t)st.g.pos[(size_t)j]]];
+  }
+  if (s.total_ticks + st.growth > (int64_t)0x7fffffff)
+    return fail(ctx, CFMM_ERR_INVALID, "modify_univ3_liquidity: more than 2^31-1 ticks in one pool set");
+  const int64_t n_ticks = st.cum[(size_t)n];
+  CU_TRY(ctx, st.d_cum.upload(st.cum));
+  CU_TRY(ctx, st.d_lower.alloc((size_t)n_ticks));
+  CU_TRY(ctx, st.d_liq.alloc((size_t)n_ticks));
+  cfmm::univ3_liq_ladder_kernel<<<pool_blocks, threads, 0, ctx->stream>>>(u, st.d_pos.p, d_cand_off.p, d_cand.p, n,
+                                                                          nullptr, st.d_cum.p, st.d_lower.p, st.d_liq.p);
+  cfmm::univ3_liq_apply_kernel<<<(unsigned)((n_ticks + threads - 1) / threads), threads, 0, ctx->stream>>>(
+      st.d_cum.p, n, n_ticks, st.d_row_off.p, st.d_rows.p, d_range, d_dL, st.d_lower.p, st.d_liq.p, d_bad);
+  ctx->launches += 2;
+  CU_TRY(ctx, cudaGetLastError());
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // (the candidate arrays are freed on return)
+  return CFMM_OK;
+}
+
+// Stage B allocations of one set whose tick counts change: all of them before anything is
+// released or written, so that a failure leaves the set as it was.
+cudaError_t liquidity_alloc(LiquidityStage& st) {
+  const PoolSet& s = *st.s;
+  const size_t total = (size_t)(s.total_ticks + st.growth);
+  cudaError_t e = st.n_lower.alloc(total);
+  if (e == cudaSuccess) e = st.n_liq.alloc(total);
+  if (e == cudaSuccess) e = st.n_tick.alloc((size_t)s.m);
+  if (e == cudaSuccess) e = st.n_tickdata.alloc(total * cfmm::kTickStride);
+  return e;
+}
+
+// Stage B of one set: commit the new ladders and rebuild the tick records.
+int liquidity_commit(cfmm_ctx* ctx, LiquidityStage& st) {
+  PoolSet& s = *st.s;
+  const int64_t n = (int64_t)st.g.pos.size();
+  const int threads = 256;
+  if (st.growth == 0) {  // same tick counts: the new liquidities go through the update path
+    CU_TRY(ctx, univ3_rebuild(ctx, s, st.d_pos.p, st.d_cum.p, n, st.cum[(size_t)n], nullptr, st.d_liq.p, false));
+  } else {
+    std::vector<int64_t> shift((size_t)n + 1, 0);
+    for (int64_t j = 0; j < n; ++j)
+      shift[(size_t)j + 1] = shift[(size_t)j] + st.new_nt[(size_t)j] - s.n_ticks[(size_t)s.order[(size_t)st.g.pos[(size_t)j]]];
+    DevBuf<int64_t> d_shift;
+    CU_TRY(ctx, d_shift.upload(shift));
+    const int64_t total = s.total_ticks + st.growth;
+    cfmm::univ3_splice_offsets_kernel<<<(unsigned)((s.m + threads - 1) / threads), threads, 0, ctx->stream>>>(
+        s.d_tick.p, st.n_tick.p, s.m, st.d_pos.p, d_shift.p, n);
+    cfmm::univ3_splice_ticks_kernel<<<(unsigned)((total + threads - 1) / threads), threads, 0, ctx->stream>>>(
+        s.d_tick.p, st.n_tick.p, s.m, total, st.d_pos.p, st.d_cum.p, n, st.d_lower.p, st.d_liq.p, s.d_lower.p,
+        s.d_liq.p, st.n_lower.p, st.n_liq.p);
+    ctx->launches += 2;
+    CU_TRY(ctx, cudaGetLastError());
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    std::swap(s.d_lower, st.n_lower);
+    std::swap(s.d_liq, st.n_liq);
+    std::swap(s.d_tick, st.n_tick);
+    std::swap(s.d_tickdata, st.n_tickdata);
+    s.total_ticks = total;
+    CU_TRY(ctx, univ3_rebuild(ctx, s, nullptr, nullptr, s.m, s.total_ticks, nullptr, nullptr, true));
+  }
+  for (int64_t j = 0; j < n; ++j) {
+    const int64_t i = s.order[(size_t)st.g.pos[(size_t)j]];
+    s.n_ticks[(size_t)i] = st.new_nt[(size_t)j];
+    s.first_lower[(size_t)i] = std::max(s.first_lower[(size_t)i], st.top[(size_t)j]);
+  }
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return CFMM_OK;
+}
+
+}  // namespace
+
+int cfmm_modify_univ3_liquidity(cfmm_ctx* ctx, int64_t q, const int64_t* pool, const double* range,
+                                const double* dL) {
+  int rc = check_liquidity_rows(ctx, q, pool, range, dL);
+  if (rc != CFMM_OK || q == 0) return rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  DevBuf<double> d_range, d_dL;
+  DevBuf<unsigned long long> d_bad;
+  CU_TRY(ctx, d_range.alloc((size_t)(2 * q)));
+  CU_TRY(ctx, DevBuf<double>::copy_in(d_range.p, range, (size_t)(2 * q) * sizeof(double)));
+  CU_TRY(ctx, d_dL.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<double>::copy_in(d_dL.p, dL, (size_t)q * sizeof(double)));
+  CU_TRY(ctx, d_bad.alloc(1));
+  CU_TRY(ctx, cudaMemsetAsync(d_bad.p, 0xff, sizeof(unsigned long long), ctx->stream));
+  // stage A for every set first: a row that fails anywhere rejects the whole call
+  std::vector<std::unique_ptr<LiquidityStage>> stages;
+  for (SetRows& r : rows_by_set(ctx, CFMM_POOL_UNIV3, q, pool)) {
+    if (r.row.empty()) continue;
+    stages.push_back(std::make_unique<LiquidityStage>());
+    stages.back()->s = r.s;
+    if ((rc = liquidity_stage(ctx, *stages.back(), r, range, d_range.p, d_dL.p, d_bad.p)) != CFMM_OK) return rc;
+  }
+  unsigned long long bad = 0;
+  CU_TRY(ctx, cudaMemcpyAsync(&bad, d_bad.p, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (bad != ~0ull)
+    return fail(ctx, CFMM_ERR_INVALID,
+                "modify_univ3_liquidity: row %lld leaves a tick it adds to with liquidity < 0 or not finite",
+                (long long)bad);
+  for (auto& st : stages) {
+    if (st->growth == 0) continue;
+    const cudaError_t e = liquidity_alloc(*st);
+    if (e != cudaSuccess) {
+      (void)cudaGetLastError();  // (an allocation failure is not sticky: clear it for later calls)
+      return fail(ctx, e == cudaErrorMemoryAllocation ? CFMM_ERR_NOMEM : CFMM_ERR_CUDA,
+                  "modify_univ3_liquidity: allocating the grown tick arrays failed: %s", cudaGetErrorString(e));
+    }
+  }
+  ctx->state_version++;
+  for (auto& st : stages)
+    if ((rc = liquidity_commit(ctx, *st)) != CFMM_OK) return rc;
+  return CFMM_OK;
+}
+
+int cfmm_get_univ3_ticks(cfmm_ctx* ctx, int64_t first, int64_t count, int64_t* tick_off, double* lower_ticks,
+                         double* liquidity) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if ((rc = check_range(ctx, CFMM_POOL_UNIV3, first, count, "get_univ3_ticks")) != CFMM_OK) return rc;
+  if (!tick_off) return fail(ctx, CFMM_ERR_INVALID, "get_univ3_ticks: null tick_off");
+  tick_off[0] = 0;
+  if (count == 0) return CFMM_OK;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  int64_t base = 0;
+  for (const Span& sp : split_range(ctx, CFMM_POOL_UNIV3, first, count)) {
+    PoolSet& s = *sp.s;
+    ensure_pos_of(s);
+    std::vector<int64_t> pos(s.pos_of.begin() + sp.first, s.pos_of.begin() + sp.first + sp.count);
+    std::vector<int64_t> cum((size_t)sp.count + 1, 0);
+    for (int64_t j = 0; j < sp.count; ++j) {
+      cum[(size_t)j + 1] = cum[(size_t)j] + s.n_ticks[(size_t)(sp.first + j)];
+      tick_off[sp.offset + j + 1] = base + cum[(size_t)j + 1];
+    }
+    const int64_t n_ticks = cum[(size_t)sp.count];
+    if (lower_ticks || liquidity) {
+      DevBuf<int64_t> d_pos, d_cum;
+      DevBuf<double> d_lo, d_lq;
+      CU_TRY(ctx, d_pos.upload(pos));
+      CU_TRY(ctx, d_cum.upload(cum));
+      CU_TRY(ctx, d_lo.alloc((size_t)n_ticks));
+      CU_TRY(ctx, d_lq.alloc((size_t)n_ticks));
+      const int threads = 256;
+      cfmm::univ3_gather_ticks_kernel<<<(unsigned)((n_ticks + threads - 1) / threads), threads, 0, ctx->stream>>>(
+          univ3_state(s), d_pos.p, d_cum.p, sp.count, n_ticks, d_lo.p, d_lq.p);
+      ctx->launches++;
+      CU_TRY(ctx, cudaGetLastError());
+      if (lower_ticks)
+        CU_TRY(ctx, cudaMemcpyAsync(lower_ticks + base, d_lo.p, (size_t)n_ticks * sizeof(double),
+                                    cudaMemcpyDeviceToHost, ctx->stream));
+      if (liquidity)
+        CU_TRY(ctx, cudaMemcpyAsync(liquidity + base, d_lq.p, (size_t)n_ticks * sizeof(double),
+                                    cudaMemcpyDeviceToHost, ctx->stream));
+      CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    }
+    base += n_ticks;
+  }
   return CFMM_OK;
 }
 

@@ -1,7 +1,8 @@
 // univ3_state.cuh -- the device-resident state of UniV3 pools (sm_90a): the per-tick
 // BoundedProduct records the sweep walks read, rebuilt from the raw tick data (lower tick
-// prices, liquidity, current price) at cfmm_finalize, on cfmm_update_univ3 and on
-// cfmm_apply_trades.  This is the library's only implementation of compute_at_tick
+// prices, liquidity, current price) at cfmm_finalize, on cfmm_update_univ3, on
+// cfmm_apply_trades and on cfmm_modify_univ3_liquidity, whose ladder merge, row replay and CSR
+// splice kernels are here too.  This is the library's only implementation of compute_at_tick
 // (src/cfmms.jl:294-313).
 //
 // Raw state, kept on the device in the CSR order of the tick records (device pool order):
@@ -52,6 +53,32 @@ __device__ __forceinline__ int univ3_tick_of(const double* lower, int nt, double
   while (lo < hi) {
     const int mid = (lo + hi) >> 1;
     if (lower[mid] >= price)
+      lo = mid + 1;
+    else
+      hi = mid;
+  }
+  return lo;
+}
+
+// The listed pool a listing-order tick t belongs to: the last j < count with cum[j] <= t.
+__device__ __forceinline__ int64_t univ3_listed(const int64_t* cum, int64_t count, int64_t t) {
+  int64_t lo = 0, hi = count - 1;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi + 1) >> 1;
+    if (cum[mid] <= t)
+      lo = mid;
+    else
+      hi = mid - 1;
+  }
+  return lo;
+}
+
+// The number of entries of the ascending pos[0..count) that are < p.
+__device__ __forceinline__ int64_t univ3_rank(const int64_t* pos, int64_t count, int64_t p) {
+  int64_t lo = 0, hi = count;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (pos[mid] < p)
       lo = mid + 1;
     else
       hi = mid;
@@ -111,14 +138,7 @@ __global__ void univ3_ticks_kernel(Univ3State s, const int64_t* __restrict__ pos
   int64_t p, ti;
   int off, nt;
   if (pos) {
-    int64_t lo = 0, hi = count - 1;  // last j with cum[j] <= t
-    while (lo < hi) {
-      const int64_t mid = (lo + hi + 1) >> 1;
-      if (cum[mid] <= t)
-        lo = mid;
-      else
-        hi = mid - 1;
-    }
+    const int64_t lo = univ3_listed(cum, count, t);
     p = pos[lo];
     ti = t - cum[lo];
     off = s.tick[p].x;
@@ -193,6 +213,134 @@ __global__ void univ3_move_kernel(Univ3State s, const double* __restrict__ gam, 
   if (qn == q) return;
   reinterpret_cast<double*>(s.f1 + p)[1] = qn;
   moved[atomicAdd(n_moved, 1ull)] = p;
+}
+
+// ---- liquidity changes (cfmm_modify_univ3_liquidity; include/cfmm_b200.h) ---------------------
+// The touched pools are listed in ascending device position: pos[j], their rows (indices into the
+// call's range / dL, batch order) rows[row_off[j] .. row_off[j+1]), and their distinct candidate
+// boundaries cand[cand_off[j] .. cand_off[j+1]), strictly decreasing.
+
+// One pool's ladder merged with its candidates (out_lower == nullptr: counted only).  A candidate
+// equal to a ladder boundary bit for bit adds nothing; any other one splits the tick it falls in
+// and inherits that tick's liquidity, or 0 above T₁.  Returns the new tick count.
+__device__ __forceinline__ int64_t univ3_merge_ladder(const double* lower, const double* liq, int nt,
+                                                      const double* cand, int64_t nc, double* out_lower,
+                                                      double* out_liq) {
+  int a = 0;
+  int64_t b = 0, n = 0;
+  double inherit = 0.0;
+  while (a < nt || b < nc) {
+    double x, l;
+    if (b == nc || (a < nt && lower[a] >= cand[b])) {
+      if (b < nc && lower[a] == cand[b]) ++b;
+      x = lower[a];
+      l = inherit = liq[a];
+      ++a;
+    } else {
+      x = cand[b];
+      l = inherit;
+      ++b;
+    }
+    if (out_lower) {
+      out_lower[n] = x;
+      out_liq[n] = l;
+    }
+    ++n;
+  }
+  return n;
+}
+
+// Stage A, one thread per touched pool: its new tick count (cum == nullptr) or its new ladder with
+// inherited liquidities, written to out_lower / out_liq from cum[j] on (listing order).
+__global__ void univ3_liq_ladder_kernel(Univ3State s, const int64_t* __restrict__ pos,
+                                        const int64_t* __restrict__ cand_off, const double* __restrict__ cand,
+                                        int64_t count, int64_t* __restrict__ new_nt, const int64_t* __restrict__ cum,
+                                        double* __restrict__ out_lower, double* __restrict__ out_liq) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= count) return;
+  const int64_t p = pos[j];
+  const int off = s.tick[p].x, nt = univ3_tick_end(s, p) - off;
+  const int64_t c0 = cand_off[j], nc = cand_off[j + 1] - c0;
+  if (cum)
+    univ3_merge_ladder(s.lower + off, s.liq + off, nt, cand + c0, nc, out_lower + cum[j], out_liq + cum[j]);
+  else
+    new_nt[j] = univ3_merge_ladder(s.lower + off, s.liq + off, nt, cand + c0, nc, nullptr, nullptr);
+}
+
+// Stage A, one thread per new tick: the pool's rows in batch order, each adding dL (one IEEE
+// addition) when lo < T <= hi for the tick's upper bound T.  A tick left < 0 or not finite
+// records its row in *first_bad (atomicMin: the call reports the lowest such row).
+__global__ void univ3_liq_apply_kernel(const int64_t* __restrict__ cum, int64_t count, int64_t n_ticks,
+                                       const int64_t* __restrict__ row_off, const int64_t* __restrict__ rows,
+                                       const double* __restrict__ range, const double* __restrict__ dL,
+                                       const double* __restrict__ new_lower, double* __restrict__ new_liq,
+                                       unsigned long long* __restrict__ first_bad) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_ticks) return;
+  const int64_t j = univ3_listed(cum, count, t);
+  const double T = new_lower[t];
+  double L = new_liq[t];
+  for (int64_t k = row_off[j]; k < row_off[j + 1]; ++k) {
+    const int64_t r = rows[k];
+    if (range[2 * r] < T && T <= range[2 * r + 1]) {
+      L = __dadd_rn(L, dL[r]);
+      if (!(L >= 0.0 && isfinite(L))) {
+        atomicMin(first_bad, (unsigned long long)r);
+        return;
+      }
+    }
+  }
+  new_liq[t] = L;
+}
+
+// Stage B (tick counts changed), one thread per pool: its first tick in the new CSR, shifted by
+// the growth of the touched pools before it (shift[k]: of the first k listed pools).
+__global__ void univ3_splice_offsets_kernel(const int2* __restrict__ old_tick, int2* __restrict__ new_tick, int64_t m,
+                                            const int64_t* __restrict__ pos, const int64_t* __restrict__ shift,
+                                            int64_t count) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= m) return;
+  new_tick[p] = make_int2((int)(old_tick[p].x + shift[univ3_rank(pos, count, p)]), 0);
+}
+
+// Stage B, one thread per tick of the new CSR: a touched pool's tick from the stage-A ladders
+// (listing order, cum), any other pool's from the old CSR.
+__global__ void univ3_splice_ticks_kernel(const int2* __restrict__ old_tick, const int2* __restrict__ new_tick,
+                                          int64_t m, int64_t new_total, const int64_t* __restrict__ pos,
+                                          const int64_t* __restrict__ cum, int64_t count,
+                                          const double* __restrict__ scr_lower, const double* __restrict__ scr_liq,
+                                          const double* __restrict__ old_lower, const double* __restrict__ old_liq,
+                                          double* __restrict__ out_lower, double* __restrict__ out_liq) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= new_total) return;
+  int64_t lo = 0, hi = m - 1;  // last pool whose first tick is <= t (every pool has a tick)
+  while (lo < hi) {
+    const int64_t mid = (lo + hi + 1) >> 1;
+    if (new_tick[mid].x <= t)
+      lo = mid;
+    else
+      hi = mid - 1;
+  }
+  const int64_t p = lo, ti = t - new_tick[p].x, k = univ3_rank(pos, count, p);
+  if (k < count && pos[k] == p) {
+    out_lower[t] = scr_lower[cum[k] + ti];
+    out_liq[t] = scr_liq[cum[k] + ti];
+  } else {
+    out_lower[t] = old_lower[old_tick[p].x + ti];
+    out_liq[t] = old_liq[old_tick[p].x + ti];
+  }
+}
+
+// cfmm_get_univ3_ticks, one thread per listed tick: the ladders of pools pos[j] in listing order.
+__global__ void univ3_gather_ticks_kernel(Univ3State s, const int64_t* __restrict__ pos,
+                                          const int64_t* __restrict__ cum, int64_t count, int64_t n_ticks,
+                                          double* __restrict__ lower_out, double* __restrict__ liq_out) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_ticks) return;
+  const int64_t j = univ3_listed(cum, count, t);
+  const int64_t q = s.tick[pos[j]].x + (t - cum[j]);
+  lower_out[t] = s.lower[q];
+  liq_out[t] = s.liq[q];
 }
 
 }  // namespace cfmm

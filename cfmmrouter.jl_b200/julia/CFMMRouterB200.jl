@@ -353,4 +353,27 @@ function execute_swaps!(ctx, ptype::Integer, pools::Vector{Int64}, tender::Matri
     return received
 end
 
+# UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
+# UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
+# current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never
+# executed.
+function modify_univ3_liquidity!(ctx, pools::Vector{Int64}, range::Matrix{Float64}, dL::Vector{Float64})
+    size(range) == (2, length(pools)) == (2, length(dL)) ||
+        throw(ArgumentError("range must be 2 x length(pools), dL of length(pools)"))
+    chk(ctx, ccall((:cfmm_modify_univ3_liquidity, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}),
+        ctx, length(pools), pools, range, dL))
+end
+function univ3_ticks(ctx, first::Integer, count::Integer)
+    off = zeros(Int64, count + 1)
+    chk(ctx, ccall((:cfmm_get_univ3_ticks, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Int64, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}),
+        ctx, first, count, off, C_NULL, C_NULL))
+    lower, liq = zeros(Float64, off[end]), zeros(Float64, off[end])
+    chk(ctx, ccall((:cfmm_get_univ3_ticks, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Int64, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}),
+        ctx, first, count, off, lower, liq))
+    return off, lower, liq
+end
+
 end # module

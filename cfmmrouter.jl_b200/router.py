@@ -338,6 +338,42 @@ class DevicePools:
                                                _dp(out)))
         return out
 
+    # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
+    def modify_univ3_liquidity(self, pools, lo, hi, dL):
+        """cfmm_modify_univ3_liquidity: row j adds dL[j] (> 0 mints, < 0 burns) to the ticks of UniV3
+        pool pools[j] (insertion order) on the price range (lo[j], hi[j]], inserting lo and hi into its
+        ladder when they are not boundaries yet.  Rows apply in batch order; a row that would leave a
+        tick below zero rejects the whole call and changes nothing."""
+        pools = np.ascontiguousarray(pools, dtype=np.int64).reshape(-1)
+        rng = np.ascontiguousarray(np.stack([np.asarray(lo, dtype=np.float64).reshape(-1),
+                                             np.asarray(hi, dtype=np.float64).reshape(-1)], axis=1))
+        dL = np.ascontiguousarray(dL, dtype=np.float64).reshape(-1)
+        if not (len(pools) == len(rng) == len(dL)):
+            raise ValueError("modify_univ3_liquidity: pools, lo, hi, dL must have one entry per row")
+        self._chk(self._lib.cfmm_modify_univ3_liquidity(self._ctx, len(pools), _ip(pools), _dp(rng), _dp(dL)))
+        if len(pools):
+            first = int(pools.min())
+            self.univ3_ticks(first, int(pools.max()) + 1 - first, ladders=False)
+
+    def univ3_ticks(self, first: int = 0, count: int = None, ladders: bool = True):
+        """cfmm_get_univ3_ticks: (tick_off [count + 1], lower_ticks, liquidity) of the UniV3 pools
+        [first, first + count), the current ladders in CSR form (lower_ticks / liquidity are None
+        with ladders=False).  count defaults to the rest of the UniV3 pools."""
+        first = int(first)
+        if count is None:
+            info = self.pool_set_info(_lib.POOL_UNIV3)
+            count = info["main"] + info["tail"] - first
+        count = int(count)
+        off = np.zeros(max(count, 0) + 1, dtype=np.int64)
+        self._chk(self._lib.cfmm_get_univ3_ticks(self._ctx, first, count, _ip(off), None, None))
+        lt = lq = None
+        if ladders:
+            lt, lq = np.zeros(int(off[-1])), np.zeros(int(off[-1]))
+            self._chk(self._lib.cfmm_get_univ3_ticks(self._ctx, first, count, _ip(off), _dp(lt), _dp(lq)))
+        if len(self._univ3_ticks) >= first + count:
+            self._univ3_ticks[first:first + count] = np.diff(off)
+        return off, lt, lq
+
     def pool_set_info(self, pool_type: int) -> dict:
         """Layout facts of one pool type (cfmm_debug_pool_set_info; read-only)."""
         info = np.zeros(8, dtype=np.int64)
@@ -613,6 +649,38 @@ class Router:
                     c.R = state[k - lo].copy()
         return out
 
+    def modify_liquidity(self, list_indices, lo, hi, dL):
+        """Mint (dL > 0) or burn (dL < 0) liquidity on the price range (lo[j], hi[j]] of the UniV3
+        pool r.cfmms[list_indices[j]], rows in order (cfmm_modify_univ3_liquidity): boundaries that
+        are new to a pool's ladder are inserted, and a row that would leave a tick below zero
+        rejects the whole call.  Refreshes the touched pool objects (lower_ticks, liquidity,
+        current_tick) from the device state.  Single GPU."""
+        if self._world > 1:
+            raise NotImplementedError("modify_liquidity drives one GPU")
+        ids = np.asarray(list_indices, dtype=np.int64).reshape(-1)
+        lo, hi, dL = (np.asarray(x, dtype=np.float64).reshape(-1) for x in (lo, hi, dL))
+        if not (len(ids) == len(lo) == len(hi) == len(dL)):
+            raise ValueError("modify_liquidity: list_indices, lo, hi, dL must have one entry per row")
+        if len(ids) and (ids.min() < 0 or ids.max() >= len(self.cfmms)):
+            raise IndexError("modify_liquidity: pool index out of range")
+        lst = np.asarray(self._type_lists[2], dtype=np.int64)
+        local = np.full(len(self.cfmms), -1, dtype=np.int64)
+        local[lst] = np.arange(len(lst))
+        loc = local[ids]
+        if np.any(loc < 0):
+            raise TypeError(f"modify_liquidity: r.cfmms[{int(ids[np.argmax(loc < 0)])}] is not a UniV3 pool")
+        self._pools.modify_univ3_liquidity(loc, lo, hi, dL)
+        if not len(ids):
+            return
+        touched = np.unique(loc)
+        first = int(touched[0])
+        off, lt, lq = self._pools.univ3_ticks(first, int(touched[-1]) + 1 - first)
+        for k in touched:
+            c = self.cfmms[lst[k]]
+            s = slice(off[k - first], off[k - first + 1])
+            c.lower_ticks, c.liquidity = lt[s].copy(), lq[s].copy()
+            c.current_tick = int(np.sum(c.lower_ticks >= c.current_price))
+
     # one find_arb!(r, v) + folds; caches Ψ and acc like the reference caches Δs/Λs
     def _sweep(self, v, materialize=False):
         psi, acc = self._pools.sweep(v, materialize)
@@ -653,8 +721,10 @@ class Router:
     def sync_reserves(self):
         """Push the state of every pool to the device: cfmm.R of the Product/GeoMean pools,
         current_price and liquidity of the UniV3 pools (the reference reads the pool objects
-        live on each sweep; call this after mutating them).  A UniV3 pool's tick prices are
-        fixed at construction."""
+        live on each sweep; call this after mutating them).  A UniV3 pool's tick prices are the
+        device's current ladder: those of construction, grown by modify_liquidity (which keeps the
+        pool objects in step).  Assigning other lower_ticks to a pool object does not move the
+        device's boundaries; use modify_liquidity for that."""
         shard = self.cfmms[self._lo:self._hi]
         for t in (0, 1):
             ids = self._type_lists[t]

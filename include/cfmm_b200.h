@@ -157,9 +157,11 @@ int cfmm_update_reserves(cfmm_ctx *ctx, int type, int64_t first, int64_t count,
 
 /* Overwrite the state of UniV3 pools [first, first+count), counted in UniV3
  * insertion order.  current_price: [count], or NULL to keep the prices.
- * liquidity: the concatenated tick liquidities of those pools in their ingested
+ * liquidity: the concatenated tick liquidities of those pools in their current
  * CSR order, or NULL to keep them.  The tick grid (lower_ticks, tick counts) is
- * fixed at cfmm_finalize.  Prices are validated as in cfmm_add_univ3 (a price
+ * the one of cfmm_add_univ3 / cfmm_append_univ3 until cfmm_modify_univ3_liquidity
+ * inserts boundaries (cfmm_get_univ3_ticks reads the current one).  Prices are
+ * validated as in cfmm_add_univ3 against the current first lower tick (a price
  * above the pool's first lower tick, or NaN, is rejected with CFMM_ERR_INVALID);
  * a rejected call changes no pool.  current_tick and every tick's BoundedProduct
  * (compute_at_tick, src/cfmms.jl:294-313) are recomputed on the device.
@@ -283,6 +285,46 @@ int cfmm_quote_swaps(cfmm_ctx *ctx, int type, int64_t q, const int64_t *pool,
                      const double *tender, double *received);
 int cfmm_execute_swaps(cfmm_ctx *ctx, int type, int64_t q, const int64_t *pool,
                        const double *tender, double *received /* may be NULL */);
+
+/* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
+ * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
+ * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
+ * src/cfmms.jl:251-259).  A row (pool, lo, hi, dL) needs 0 < lo < hi, both finite, and dL finite
+ * and != 0 (dL > 0 mints, dL < 0 burns).  The rows are applied in batch order, with the result of
+ * applying them one at a time:
+ *   boundaries  hi and lo are inserted unless some Tᵢ equals them bit for bit.  A boundary inside
+ *               tick i splits it; both parts carry Lᵢ (copied).  A boundary above T₁ adds a new
+ *               first tick (T₁, b] with liquidity 0 (b is the new T₁); one below Tₙ splits the
+ *               last tick.
+ *   liquidity   every tick whose upper bound Tᵢ satisfies lo < Tᵢ <= hi gets Lᵢ <- Lᵢ + dL, one
+ *               IEEE addition (round to nearest), in batch order per tick.
+ *   rejection   a row that leaves a tick it added to with L < 0 or L not finite rejects the whole
+ *               call with CFMM_ERR_INVALID; the message names the first such row, and no pool
+ *               changes.  Burning exactly x from a tick that an earlier mint of x raised from
+ *               L >= 0, with only mints on that tick in between, never fails: rounding is
+ *               monotonic, so the tick holds at least x and the difference is >= 0.
+ *   unchanged   the current price q.  current_tick is re-derived (searchsortedlast, :235) and
+ *               every tick's compute_at_tick record rebuilt on the device.  Boundaries are never
+ *               removed: a range burned to zero stays as an empty tick, which walks pass through.
+ * Retired pools (cfmm_set_active) take the change in the state they keep; their records stay
+ * empty until they are restored.  Afterwards the state version moves (captured sweep graphs
+ * re-capture; the tick arrays may have been reallocated), the materialised trades stay (as after
+ * cfmm_execute_swaps), cfmm_apply_trades clamps to the current T₁, cfmm_update_univ3 validates
+ * prices against the current T₁ and takes liquidity in the current CSR order.
+ *
+ * Before cfmm_finalize: CFMM_ERR_STATE.  A pool outside the UniV3 pools, a NaN or Inf, lo <= 0,
+ * lo >= hi or dL == 0: CFMM_ERR_INVALID before anything runs.  q == 0 does nothing.  A call that
+ * would take a main or appended set past 2^31-1 ticks is rejected (CFMM_ERR_INVALID) before
+ * anything changes; CFMM_ERR_NOMEM if the grown tick arrays cannot be allocated, with no pool
+ * changed. */
+/* q rows on UniV3 pools; pool: [q] UniV3 insertion order (tails included);
+ * range: [2q] pool-major (lo, hi); dL: [q].  Synchronous. */
+int cfmm_modify_univ3_liquidity(cfmm_ctx *ctx, int64_t q, const int64_t *pool,
+                                const double *range, const double *dL);
+/* The current ladders of UniV3 pools [first, first+count): tick_off [count+1] always;
+ * lower_ticks / liquidity (may be NULL) [tick_off[count]].  Retired pools report their kept state. */
+int cfmm_get_univ3_ticks(cfmm_ctx *ctx, int64_t first, int64_t count, int64_t *tick_off,
+                         double *lower_ticks, double *liquidity);
 
 /* ---- the outer iteration on the device (SURVEY §8f rank 2) ---------------------------
  * Minimises the dual g(nu) = lin' nu + sum_i arb_i(nu) over the box lower <= nu <= upper
