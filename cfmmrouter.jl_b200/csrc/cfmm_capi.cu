@@ -123,6 +123,13 @@ struct PoolSet {
   DevBuf<unsigned short> d_gcode;
   DevBuf<double> d_gtab;       // [256] 1/γ by code, then [256] γ by code
   bool compact_ok = false;
+  // the 192-pool compact records pair consecutive chunks of one bucket: their count, the first
+  // record of every bucket, and per chunk its record << 2 | (second of its record) << 1 | (alone in
+  // its record: the last chunk of a bucket with an odd chunk count)
+  int64_t n_recs = 0;
+  cfmm::BucketTable rec_buckets;
+  DevBuf<int> d_chunk_rec;
+  int range_pools = 0;         // pools per unit of the range table (96-pool chunks or 192-pool records)
   DevBuf<double> d_inv_scale, d_tok_sum;
   bool fixed_ok = false;       // every token fits the fixed-point rules (range, totals)
   // speed-weighted CTA ranges of the TMA kernel (product_tma.cuh): the table passed to the next
@@ -154,6 +161,7 @@ struct PoolSet {
     d_Ai.release(); d_tick.release(); d_gidx.release();
     d_lower.release(); d_liq.release();
     d_packed.release(); d_inv_scale.release(); d_tok_sum.release(); d_gcode.release(); d_gtab.release();
+    d_chunk_rec.release();
     d_active.release(); d_park.release();
     if (h_dur) cudaFreeHost(h_dur);
     h_dur = nullptr;
@@ -231,6 +239,7 @@ struct cfmm_ctx {
   int balance = 1;              // 1 = TMA kernel: CTA ranges sized by measured CTA speed (feedback), 0 = even split
   int geomean_tma = 1;          // gradient-only GeometricMean sweeps on the TMA kernel (0: first-generation kernel)
   int compact_stream = 1;       // ProductTwoCoin, economized math: 20-byte pool records (γ dictionary, chunk-relative a) when the set allows it
+  int compact_record = 0;       // pools per compact record: 96 or 192; 0 = 192 on sets with at least 4 records per resident warp
   // resident CTAs per SM of every kernel instantiation this context has launched.
   // Per context, not per process: cudaFuncSetAttribute (the > 48 KB dynamic shared
   // memory opt-in) acts on the current device only, and contexts of one process
@@ -476,12 +485,30 @@ int upload_set(cfmm_ctx* ctx, int type, PoolSet& s, bool tail) {
   clock.mark("gather + upload gamma, Ai, gidx");
   s.compact_ok = false;
   if (type == CFMM_POOL_PRODUCT && s.tma_ok) {
-    // the compact stream stores a as an offset from its chunk's first a: every chunk's span must
-    // fit the field.  The layout is fixed here and reserve updates do not move a.
+    // 192-pool records: consecutive chunks of a bucket in pairs
+    std::vector<int> chunk_rec((size_t)s.n_chunks);
+    s.n_recs = 0;
+    for (int b = 0; b < s.buckets.n_buckets; ++b) {
+      const int c0 = s.buckets.first_chunk[b], c1 = s.buckets.first_chunk[b + 1];
+      s.rec_buckets.first_chunk[b] = (int)s.n_recs;
+      for (int c = c0; c < c1; ++c) {
+        const int k = c - c0;
+        chunk_rec[(size_t)c] = (int)((s.n_recs + k / 2) << 2) | ((k & 1) << 1) | ((k & 1) == 0 && c + 1 == c1 ? 1 : 0);
+      }
+      s.n_recs += (c1 - c0 + 1) / 2;
+    }
+    s.rec_buckets.n_buckets = s.buckets.n_buckets;
+    s.rec_buckets.first_chunk[s.buckets.n_buckets] = (int)s.n_recs;
+    // the compact stream stores a as an offset from its record's first a: the span of every
+    // 192-pool record must fit the field (the 96-pool records are its halves).  The layout is fixed
+    // here and reserve updates do not move a.
     int64_t max_span = 0;
 #pragma omp parallel for schedule(static) reduction(max : max_span) if (s.n_chunks > (1 << 12))
     for (int64_t c = 0; c < s.n_chunks; ++c) {
-      const int64_t first = real_before(c * cfmm::kTmaChunk), last = real_before((c + 1) * cfmm::kTmaChunk - 1);
+      const int v = chunk_rec[(size_t)c];
+      if (v & 2) continue;  // second chunk of a record
+      const int64_t end = (v & 1) ? c + 1 : c + 2;
+      const int64_t first = real_before(c * cfmm::kTmaChunk), last = real_before(end * cfmm::kTmaChunk - 1);
       const int64_t span = (first < 0 || last < 0) ? 0 : (int64_t)oa[(size_t)last] - (int64_t)oa[(size_t)first];
       max_span = std::max(max_span, span);
     }
@@ -509,7 +536,8 @@ int upload_set(cfmm_ctx* ctx, int type, PoolSet& s, bool tail) {
         h = (h + 1) & (kSlots - 1);
       }
     };
-    bool ok = max_span <= cfmm::kMetaMaxSpan && slot_of(1.0, true) >= 0;  // (the padding pools' fee)
+    // (the padding pools' fee, inserted first: code 0, which pack_chunks_compact_kernel relies on)
+    bool ok = max_span <= cfmm::kMetaMaxSpan && slot_of(1.0, true) >= 0;
     double last = 1.0;
     for (int64_t i = 0; i < m && ok; ++i) {
       const double g = s.gamma[(size_t)i];
@@ -530,6 +558,7 @@ int upload_set(cfmm_ctx* ctx, int type, PoolSet& s, bool tail) {
         return (unsigned short)slot_of(i < 0 ? 1.0 : s.gamma[(size_t)i], false);
       }));
       CU_TRY(ctx, s.d_gtab.upload(tab));
+      CU_TRY(ctx, s.d_chunk_rec.upload(chunk_rec));
       s.compact_ok = true;
     }
     clock.mark("fee dictionary + codes");
@@ -733,16 +762,20 @@ int refresh_scale(cfmm_ctx* ctx, PoolSet& s) {
 }
 
 // the packed stream of the mode this sweep runs in (rebuilt when the mode or the reserves changed)
-template <int POOL>
+template <int POOL, int L = cfmm::kTmaL>
 int ensure_packed(cfmm_ctx* ctx, PoolSet& s, bool econ, bool fixed, bool compact, cudaStream_t st) {
-  const int mode = (econ ? 1 : 0) | (fixed ? 2 : 0) | (compact ? 4 : 0);
+  const int mode = (econ ? 1 : 0) | (fixed ? 2 : 0) | (compact ? 4 : 0) | (L != cfmm::kTmaL ? 8 : 0);
   if (s.packed_mode == mode) return CFMM_OK;
-  const size_t bytes = (size_t)s.n_chunks * (compact ? cfmm::tma_chunk_bytes_c<POOL, true>() : cfmm::tma_chunk_bytes<POOL>());
-  if (s.d_packed.n < bytes) CU_TRY(ctx, s.d_packed.alloc((size_t)s.n_chunks * cfmm::tma_chunk_bytes<POOL>()));
+  const size_t wide = (size_t)s.n_chunks * cfmm::tma_chunk_bytes<POOL>();
+  const size_t bytes = !compact ? wide
+                       : L == cfmm::kTmaL ? (size_t)s.n_chunks * cfmm::tma_chunk_bytes_c<POOL, true>()
+                                          : (size_t)s.n_recs * cfmm::tma_chunk_bytes_c<POOL, true, L>();
+  if (s.d_packed.n < bytes) CU_TRY(ctx, s.d_packed.alloc(std::max(bytes, wide)));
   const int threads = 256;
   if (compact) {
-    cfmm::pack_chunks_compact_kernel<<<(unsigned)((s.m_padded + threads - 1) / threads), threads, 0, st>>>(
-        s.d_R.p, s.d_Ai.p, s.d_gcode.p, s.m_padded, s.nb, fixed ? s.d_inv_scale.p : nullptr, s.d_packed.p);
+    cfmm::pack_chunks_compact_kernel<L><<<(unsigned)((s.m_padded + threads - 1) / threads), threads, 0, st>>>(
+        s.d_R.p, s.d_Ai.p, s.d_gcode.p, s.m_padded, s.nb, fixed ? s.d_inv_scale.p : nullptr, s.d_chunk_rec.p,
+        s.d_packed.p);
     ctx->launches++;
     CU_TRY(ctx, cudaGetLastError());
     s.packed_mode = mode;
@@ -758,31 +791,38 @@ int ensure_packed(cfmm_ctx* ctx, PoolSet& s, bool econ, bool fixed, bool compact
   return CFMM_OK;
 }
 
-template <int POOL, bool ECON, bool SKEW, bool FIXED, bool COMPACT = false>
+template <int POOL, bool ECON, bool SKEW, bool FIXED, bool COMPACT = false, int L = cfmm::kTmaL>
 int launch_tma_cfg(cfmm_ctx* ctx, PoolSet& s, const double* d_v, double* d_psi, cudaStream_t st) {
-  auto kern = cfmm::product_sweep_tma<POOL, ECON, SKEW, FIXED, COMPACT>;
-  constexpr int kThreads = cfmm::tma_threads<POOL>(), kSmem = cfmm::tma_smem_bytes_c<POOL, COMPACT>();
+  auto kern = cfmm::product_sweep_tma<POOL, ECON, SKEW, FIXED, COMPACT, L>;
+  constexpr int kThreads = cfmm::tma_threads<POOL, L>(), kSmem = cfmm::tma_smem_bytes_c<POOL, COMPACT, L>();
   int& occ = ctx->occupancy[reinterpret_cast<const void*>(kern)];
   if (occ == 0) {
     CU_TRY(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
     CU_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, kSmem));
     if (occ < 1) return fail(ctx, CFMM_ERR_CUDA, "product_sweep_tma does not fit on an SM");
   }
-  int rc = ensure_packed<POOL>(ctx, s, ECON, FIXED, COMPACT, st);
+  int rc = ensure_packed<POOL, L>(ctx, s, ECON, FIXED, COMPACT, st);
   if (rc != CFMM_OK) return rc;
+  // the unit of the bucket and range tables: 96-pool chunks, or the 192-pool records
+  const int64_t n_units = L == cfmm::kTmaL ? s.n_chunks : s.n_recs;
+  const cfmm::BucketTable& tab = L == cfmm::kTmaL ? s.buckets : s.rec_buckets;
+  if (s.range_pools != 32 * L) {  // a table in the other unit: start over
+    s.range_pools = 32 * L;
+    s.ranges.n = -1;
+  }
   // (grid and range table)
   const int per_sm = ctx->blocks_per_sm > 0 && ctx->blocks_per_sm < occ ? ctx->blocks_per_sm : occ;
   int grid = ctx->sm_count * per_sm;
-  if (grid > s.n_chunks) grid = (int)s.n_chunks;
+  if (grid > n_units) grid = (int)n_units;
   // ---- speed-weighted ranges (see product_tma.cuh) ---------------------------------------
   unsigned* d_dur = nullptr;
   const bool tabled = grid <= cfmm::kTmaMaxRanges;
-  const bool balancing = ctx->balance && tabled && s.n_chunks >= (int64_t)grid * 32;
+  const bool balancing = ctx->balance && tabled && n_units >= (int64_t)grid * 32;
   auto set_buckets = [&]() {  // b-bucket of every range's first chunk
     int b = 0;
     for (int g = 0; g <= grid; ++g) {
-      const int c = g < grid ? s.ranges.first[g] : (int)s.n_chunks - 1;
-      while (b + 1 < s.buckets.n_buckets && s.buckets.first_chunk[b + 1] <= c) ++b;
+      const int c = g < grid ? s.ranges.first[g] : (int)n_units - 1;
+      while (b + 1 < tab.n_buckets && tab.first_chunk[b + 1] <= c) ++b;
       s.ranges.bucket[g] = (short)b;
     }
   };
@@ -791,7 +831,7 @@ int launch_tma_cfg(cfmm_ctx* ctx, PoolSet& s, const double* d_v, double* d_psi, 
   } else if (s.ranges.n != grid || !balancing) {
     if (s.ranges.n != grid || s.range_updates != 0) {  // (first launch with this grid, or balancing switched off)
       s.ranges.n = grid;
-      for (int g = 0; g <= grid; ++g) s.ranges.first[g] = (int)(s.n_chunks * g / grid);
+      for (int g = 0; g <= grid; ++g) s.ranges.first[g] = (int)(n_units * g / grid);
       set_buckets();
       s.speed.assign((size_t)grid, 1.0);
       s.range_version = (s.range_version % 250) + 1;
@@ -840,9 +880,9 @@ int launch_tma_cfg(cfmm_ctx* ctx, PoolSet& s, const double* d_v, double* d_psi, 
         double acc_len = 0.0;
         int prev = 0;
         for (int g = 0; g < grid; ++g) {
-          acc_len += (double)s.n_chunks * s.speed[(size_t)g] / total;
-          int end = g + 1 == grid ? (int)s.n_chunks : (int)(acc_len + 0.5);
-          const int min_end = prev + 1, max_end = (int)s.n_chunks - (grid - 1 - g);
+          acc_len += (double)n_units * s.speed[(size_t)g] / total;
+          int end = g + 1 == grid ? (int)n_units : (int)(acc_len + 0.5);
+          const int min_end = prev + 1, max_end = (int)n_units - (grid - 1 - g);
           end = end < min_end ? min_end : (end > max_end ? max_end : end);
           s.ranges.first[g + 1] = end;
           prev = end;
@@ -872,12 +912,12 @@ int launch_tma_cfg(cfmm_ctx* ctx, PoolSet& s, const double* d_v, double* d_psi, 
   if (fx.mode != 0 && ctx->coop_launch) {
     // the fused exchange meets at a grid-wide barrier: a COOPERATIVE launch makes the driver
     // guarantee that every CTA is resident (or fail the launch) instead of inferring it
-    void* args[] = {&a_packed, &a_gam, &s.buckets, &a_nb, &d_v, &a_scale, &d_psi, &a_n, &a_zero,
+    void* args[] = {&a_packed, &a_gam, const_cast<cfmm::BucketTable*>(&tab), &a_nb, &d_v, &a_scale, &d_psi, &a_n, &a_zero,
                     &a_range, &a_flags, &fx, &s.ranges, &d_dur, &a_trace};
     CU_TRY(ctx, cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(kern), dim3(grid), dim3(kThreads),
                                             args, kSmem, st));
   } else {
-    kern<<<grid, kThreads, kSmem, st>>>(a_packed, a_gam, s.buckets, a_nb, d_v, a_scale, d_psi, a_n, a_zero,
+    kern<<<grid, kThreads, kSmem, st>>>(a_packed, a_gam, tab, a_nb, d_v, a_scale, d_psi, a_n, a_zero,
                                         a_range, a_flags, fx, s.ranges, d_dur, a_trace);
   }
   if (ctx->d_trace.n) ctx->trace_grid = grid;
@@ -902,6 +942,17 @@ int launch_tma(cfmm_ctx* ctx, PoolSet& s, const double* d_v, double* d_psi, cuda
   const bool fixed = ctx->psi_fixed_point && s.fixed_ok;
   if constexpr (POOL == 0) {
     if (econ && ctx->compact_stream && s.compact_ok && !ctx->exact) {
+      // 192-pool records halve the per-record work (wait, counter, re-arm) and combine Ψ[a] over
+      // the warp, but leave warps idle on small sets: taken when every resident warp gets several
+      constexpr int L6 = cfmm::kTmaL6;
+      const int64_t warps = (int64_t)ctx->sm_count * cfmm::tma_ctas_per_sm<0, L6>() * cfmm::tma_warps<0, L6>();
+      const bool rec192 = ctx->compact_record == 192 || (ctx->compact_record == 0 && s.n_recs >= 4 * warps);
+      if (rec192) {
+        if (!s.skewed && fixed) return launch_tma_cfg<0, true, false, true, true, L6>(ctx, s, d_v, d_psi, st);
+        if (!s.skewed && !fixed) return launch_tma_cfg<0, true, false, false, true, L6>(ctx, s, d_v, d_psi, st);
+        if (s.skewed && fixed) return launch_tma_cfg<0, true, true, true, true, L6>(ctx, s, d_v, d_psi, st);
+        return launch_tma_cfg<0, true, true, false, true, L6>(ctx, s, d_v, d_psi, st);
+      }
       if (!s.skewed && fixed) return launch_tma_cfg<0, true, false, true, true>(ctx, s, d_v, d_psi, st);
       if (!s.skewed && !fixed) return launch_tma_cfg<0, true, false, false, true>(ctx, s, d_v, d_psi, st);
       if (s.skewed && fixed) return launch_tma_cfg<0, true, true, true, true>(ctx, s, d_v, d_psi, st);
@@ -2789,6 +2840,9 @@ int cfmm_set_option(cfmm_ctx* ctx, const char* key, int64_t value) {
     ctx->psi_fixed_point = value != 0;
   } else if (!strcmp(key, "compact_stream")) {
     ctx->compact_stream = value != 0;
+  } else if (!strcmp(key, "compact_record")) {
+    if (value != 0 && value != 96 && value != 192) return fail(ctx, CFMM_ERR_INVALID, "compact_record: 0 (by set size), 96 or 192");
+    ctx->compact_record = (int)value;
   } else if (!strcmp(key, "geomean_tma")) {
     ctx->geomean_tma = value != 0;
   } else if (!strcmp(key, "balance")) {

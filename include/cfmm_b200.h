@@ -402,9 +402,13 @@ int cfmm_solve(cfmm_ctx *ctx, const double *lin, const double *lower, const doub
  *                      pow on hardware) or as pow (0).
  *   "compact_stream"   1 (default) = economized ProductTwoCoin sweeps stream 20-byte pool records
  *                      (fee through a dictionary of <= 256 distinct values, first token relative
- *                      to its 96-pool chunk's first, second token relative to its bucket) when the
- *                      pool set allows it (<= 256 fees, every chunk's first tokens spanning < 8192);
+ *                      to its record's first, second token relative to its bucket) when the
+ *                      pool set allows it (<= 256 fees, the first tokens of every pair of
+ *                      consecutive 96-pool chunks of a bucket spanning < 8192);
  *                      0 = 32-byte records.
+ *   "compact_record"   pools per record of that stream: 192 (two chunks of a bucket, one bulk
+ *                      copy, six pools per thread), 96, or 0 (default) = 192 when the set has at
+ *                      least 4 such records per resident warp, else 96.
  *   "geomean_tma"      1 (default) = gradient-only GeometricMeanTwoCoin sweeps run on the TMA
  *                      kernel too (48-byte records, same fixed-point slice); 0 = first-generation
  *                      kernel.

@@ -149,7 +149,8 @@ def main():
     for name, _ in cfgs:
         t = np.concatenate(res[name])
         row = {"cfg": name, "type": a.type, "flushed": bool(a.flush), "m": a.m, "n": a.n, "median_us": float(np.median(t)), "mean_us": float(t.mean()),
-               "min_us": float(t.min()), "p95_us": float(np.quantile(t, 0.95)), "launches": len(t)}
+               "min_us": float(t.min()), "p95_us": float(np.quantile(t, 0.95)), "launches": len(t),
+               "round_medians_us": [round(float(np.median(x)), 3) for x in res[name]]}
         print(json.dumps(row), flush=True)
         out.append(row)
     if a.out:
