@@ -24,6 +24,14 @@ POOL_PRODUCT = 0
 POOL_GEOMEAN = 1
 POOL_UNIV3 = 2
 
+# cfmm_execute_swap_orders: row kinds and per-row status
+SWAP_EXACT_IN = 0
+SWAP_EXACT_OUT = 1
+ORDER_FILLED = 0
+ORDER_LIMIT = 1
+ORDER_UNREACHABLE = 2
+ORDER_RETIRED = 3
+
 COMM_HANDLE_BYTES = 128
 
 class SolveOpts(C.Structure):
@@ -69,6 +77,9 @@ SYMBOLS = {
     "cfmm_compact": (C.c_int, [_ctx]),
     "cfmm_quote_swaps": (C.c_int, [_ctx, C.c_int, C.c_int64, _ip, _dp, _dp]),
     "cfmm_execute_swaps": (C.c_int, [_ctx, C.c_int, C.c_int64, _ip, _dp, _dp]),
+    "cfmm_quote_swaps_exact_out": (C.c_int, [_ctx, C.c_int, C.c_int64, _ip, _dp, _dp]),
+    "cfmm_execute_swap_orders": (C.c_int, [_ctx, C.c_int, C.c_int64, _ip, C.POINTER(C.c_uint8), _dp, _dp, _dp, _dp,
+                                           C.POINTER(C.c_uint8)]),
     "cfmm_modify_univ3_liquidity": (C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),

@@ -2432,6 +2432,31 @@ PoolGroups group_by_pool(const SetRows& r, int64_t m_padded) {
   return g;
 }
 
+// After an execute kernel on set s: the derived state of the UniV3 pools it listed in d_moved
+// (d_n_moved of them) is rebuilt as after cfmm_apply_trades; for two-coin sets a raised d_flag
+// (a reserve left the guard-free range) clears in_fast_range, and the fixed-point scale follows.
+int swap_bookkeeping(cfmm_ctx* ctx, PoolSet& s, int type, const int64_t* d_moved,
+                     const unsigned long long* d_n_moved, const int* d_flag) {
+  int rc = CFMM_OK;
+  unsigned long long h_moved = 0;
+  int h_flag = 0;
+  CU_TRY(ctx, cudaMemcpyAsync(&h_moved, d_n_moved, sizeof(h_moved), cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, cudaMemcpyAsync(&h_flag, d_flag, sizeof(h_flag), cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (type == CFMM_POOL_UNIV3) {
+    if (h_moved > 0) {  // the derived state of the pools that moved, as after cfmm_apply_trades
+      std::vector<int64_t> moved((size_t)h_moved);
+      CU_TRY(ctx, cudaMemcpy(moved.data(), d_moved, (size_t)h_moved * sizeof(int64_t), cudaMemcpyDeviceToHost));
+      std::sort(moved.begin(), moved.end());
+      if ((rc = univ3_update_listed(ctx, s, moved, nullptr, nullptr, true)) != CFMM_OK) return rc;
+    }
+  } else {
+    if (h_flag) s.in_fast_range = false;  // later sweeps take the generic (guarded) form
+    if (s.tma_ok && (rc = refresh_scale(ctx, s)) != CFMM_OK) return rc;
+  }
+  return CFMM_OK;
+}
+
 }  // namespace
 
 // launch KERNEL<type> (the pool type as a template argument) with the arguments that follow
@@ -2512,26 +2537,129 @@ int cfmm_execute_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, 
     }
     ctx->launches++;
     CU_TRY(ctx, cudaGetLastError());
-    unsigned long long h_moved = 0;
-    int h_flag = 0;
-    CU_TRY(ctx, cudaMemcpyAsync(&h_moved, d_n_moved.p, sizeof(h_moved), cudaMemcpyDeviceToHost, ctx->stream));
-    CU_TRY(ctx, cudaMemcpyAsync(&h_flag, d_flag.p, sizeof(h_flag), cudaMemcpyDeviceToHost, ctx->stream));
-    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    if (type == CFMM_POOL_UNIV3) {
-      if (h_moved > 0) {  // the derived state of the pools that moved, as after cfmm_apply_trades
-        std::vector<int64_t> moved((size_t)h_moved);
-        CU_TRY(ctx, cudaMemcpy(moved.data(), d_moved.p, (size_t)h_moved * sizeof(int64_t), cudaMemcpyDeviceToHost));
-        std::sort(moved.begin(), moved.end());
-        if ((rc = univ3_update_listed(ctx, s, moved, nullptr, nullptr, true)) != CFMM_OK) return rc;
-      }
-    } else {
-      if (h_flag) s.in_fast_range = false;  // later sweeps take the generic (guarded) form
-      if (s.tma_ok && (rc = refresh_scale(ctx, s)) != CFMM_OK) return rc;
-    }
+    if ((rc = swap_bookkeeping(ctx, s, type, d_moved.p, d_n_moved.p, d_flag.p)) != CFMM_OK) return rc;
   }
   if (received)
     CU_TRY(ctx, cudaMemcpyAsync(received, d_recv.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
                                 ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return CFMM_OK;
+}
+
+// ---- exact-output rows and slippage limits (swap_kernels.cuh) -----------------------------------
+namespace {
+
+// The kinds and limits of cfmm_execute_swap_orders (the amounts are checked by check_swaps).
+int check_orders(cfmm_ctx* ctx, int64_t q, const uint8_t* kind, const double* limit) {
+  if (q > 0 && !kind) return fail(ctx, CFMM_ERR_INVALID, "execute_swap_orders: null kind array");
+  for (int64_t j = 0; j < q; ++j) {
+    if (kind[j] != CFMM_SWAP_EXACT_IN && kind[j] != CFMM_SWAP_EXACT_OUT)
+      return fail(ctx, CFMM_ERR_INVALID, "execute_swap_orders: row %lld: kind %d is neither exact-in (0) nor exact-out (1)",
+                  (long long)j, (int)kind[j]);
+    if (!limit) continue;
+    const double l = limit[j];
+    if (std::isnan(l) || l < 0.0)
+      return fail(ctx, CFMM_ERR_INVALID, "execute_swap_orders: row %lld: limit %g must be >= 0", (long long)j, l);
+    if (std::isinf(l) && kind[j] == CFMM_SWAP_EXACT_IN)
+      return fail(ctx, CFMM_ERR_INVALID, "execute_swap_orders: row %lld: an exact-in row's minimum received must be finite",
+                  (long long)j);
+  }
+  return CFMM_OK;
+}
+
+}  // namespace
+
+int cfmm_quote_swaps_exact_out(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const double* want,
+                               double* tender) {
+  int rc = check_swaps(ctx, type, q, pool, want, tender, true, "quote_swaps_exact_out");
+  if (rc != CFMM_OK || q == 0) return rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  DevBuf<double> d_want, d_tender;
+  CU_TRY(ctx, d_want.alloc((size_t)(2 * q)));
+  CU_TRY(ctx, DevBuf<double>::copy_in(d_want.p, want, (size_t)(2 * q) * sizeof(double)));
+  CU_TRY(ctx, d_tender.alloc((size_t)(2 * q)));
+  for (SetRows& r : rows_by_set(ctx, type, q, pool)) {
+    const int64_t n = (int64_t)r.row.size();
+    if (n == 0) continue;
+    DevBuf<int64_t> d_row, d_pos;
+    CU_TRY(ctx, d_row.upload(r.row));
+    CU_TRY(ctx, d_pos.upload(r.pos));
+    const cfmm::SwapSet ss = swap_set(*r.s);
+    const unsigned blocks = (unsigned)((n + 255) / 256);
+    {
+      ProfScope prof(ctx, kProfSwaps, ctx->stream);
+      CFMM_SWAP_LAUNCH(type, cfmm::swap_quote_exact_out_kernel, blocks, ctx->stream, ss, d_row.p, d_pos.p, n,
+                       d_want.p, d_tender.p);
+    }
+    ctx->launches++;
+    CU_TRY(ctx, cudaGetLastError());
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // (d_row, d_pos are freed at the end of the block)
+  }
+  CU_TRY(ctx, cudaMemcpyAsync(tender, d_tender.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
+                              ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return CFMM_OK;
+}
+
+int cfmm_execute_swap_orders(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const uint8_t* kind,
+                             const double* amount, const double* limit, double* paid, double* received,
+                             uint8_t* status) {
+  int rc = check_swaps(ctx, type, q, pool, amount, nullptr, false, "execute_swap_orders");
+  if (rc != CFMM_OK) return rc;
+  if ((rc = check_orders(ctx, q, kind, limit)) != CFMM_OK || q == 0) return rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  ctx->state_version++;
+  DevBuf<double> d_amount, d_limit, d_paid, d_recv;
+  DevBuf<uint8_t> d_kind, d_status;
+  CU_TRY(ctx, d_amount.alloc((size_t)(2 * q)));
+  CU_TRY(ctx, DevBuf<double>::copy_in(d_amount.p, amount, (size_t)(2 * q) * sizeof(double)));
+  CU_TRY(ctx, d_kind.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<uint8_t>::copy_in(d_kind.p, kind, (size_t)q));
+  if (limit) {
+    CU_TRY(ctx, d_limit.alloc((size_t)q));
+    CU_TRY(ctx, DevBuf<double>::copy_in(d_limit.p, limit, (size_t)q * sizeof(double)));
+  }
+  CU_TRY(ctx, d_paid.alloc((size_t)(2 * q)));
+  CU_TRY(ctx, d_recv.alloc((size_t)(2 * q)));
+  CU_TRY(ctx, d_status.alloc((size_t)q));
+  for (SetRows& r : rows_by_set(ctx, type, q, pool)) {
+    PoolSet& s = *r.s;
+    const int64_t n = (int64_t)r.row.size();
+    if (n == 0) continue;
+    const PoolGroups seg = group_by_pool(r, s.m_padded);
+    const int64_t n_seg = (int64_t)seg.pos.size();
+    DevBuf<int64_t> d_seg_pos, d_seg_off, d_seg_rows, d_moved;
+    DevBuf<unsigned long long> d_n_moved;
+    DevBuf<int> d_flag;
+    CU_TRY(ctx, d_seg_pos.upload(seg.pos));
+    CU_TRY(ctx, d_seg_off.upload(seg.off));
+    CU_TRY(ctx, d_seg_rows.upload(seg.rows));
+    CU_TRY(ctx, d_n_moved.alloc(1));
+    CU_TRY(ctx, d_flag.alloc(1));
+    if (type == CFMM_POOL_UNIV3) CU_TRY(ctx, d_moved.alloc((size_t)n_seg));
+    CU_TRY(ctx, cudaMemsetAsync(d_n_moved.p, 0, sizeof(unsigned long long), ctx->stream));
+    CU_TRY(ctx, cudaMemsetAsync(d_flag.p, 0, sizeof(int), ctx->stream));
+    const cfmm::SwapSet ss = swap_set(s);
+    const unsigned blocks = (unsigned)((n_seg + 255) / 256);
+    {
+      ProfScope prof(ctx, kProfSwaps, ctx->stream);
+      CFMM_SWAP_LAUNCH(type, cfmm::swap_execute_orders_kernel, blocks, ctx->stream, ss, d_seg_pos.p, d_seg_off.p,
+                       d_seg_rows.p, n_seg, d_kind.p, d_amount.p, d_limit.p, d_paid.p, d_recv.p, d_status.p,
+                       d_moved.p, d_n_moved.p, d_flag.p);
+    }
+    ctx->launches++;
+    CU_TRY(ctx, cudaGetLastError());
+    if ((rc = swap_bookkeeping(ctx, s, type, d_moved.p, d_n_moved.p, d_flag.p)) != CFMM_OK) return rc;
+  }
+  if (paid)
+    CU_TRY(ctx, cudaMemcpyAsync(paid, d_paid.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
+                                ctx->stream));
+  if (received)
+    CU_TRY(ctx, cudaMemcpyAsync(received, d_recv.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
+                                ctx->stream));
+  if (status) CU_TRY(ctx, cudaMemcpyAsync(status, d_status.p, (size_t)q, cudaMemcpyDeviceToHost, ctx->stream));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return CFMM_OK;
 }

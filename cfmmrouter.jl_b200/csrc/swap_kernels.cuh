@@ -216,4 +216,273 @@ __global__ void swap_execute_kernel(SwapSet s, const int64_t* __restrict__ seg_p
   }
 }
 
+// ---- exact-output rows and slippage limits (cfmm_quote_swaps_exact_out / cfmm_execute_swap_orders)
+// f(x) is the exact-input quote of a tender x on one side at the pool's current state: two_coin_out
+// with δ = γ·x, or univ3_walk(..., γ·x, ...).lambda, the operations swap_quote_kernel runs, so f is
+// cfmm_quote_swaps bit for bit (f(0) = 0, as for a zero tender).  The old kernels are unchanged: the
+// helpers they call are the ones the new kernels call.
+//
+// An exact-output row wanting y > 0 takes x* with f(x*) >= y and f(pred(x*)) < y (or x* = 0),
+// searched on the ordinals of the doubles in [0, DBL_MAX] (a double >= 0 read as an int64 is
+// monotone in the double): from the closed-form estimate e, gallop 1, 2, 4, .. ordinals away from
+// e until f brackets y, then bisect the bracket to adjacent doubles.  Every loop is bounded by the
+// 63-bit ordinal range: at most 1 + 63 + 62 evaluations of f (include/cfmm_b200.h).
+
+constexpr int64_t kSwapOrdMax = 0x7fefffffffffffffll;  // the ordinal of DBL_MAX
+
+// The ordinal the search starts from: a NaN or non-positive estimate starts at the least
+// subnormal, an infinite one at DBL_MAX.
+__device__ __forceinline__ int64_t swap_start_ord(double e) {
+  if (!(e > 0.0)) return 1;
+  const int64_t o = __double_as_longlong(e);
+  return o > kSwapOrdMax ? kSwapOrdMax : o;
+}
+
+// The ordinal of the crossing x* of f through y > 0 found from the estimate e; -1 when
+// f(DBL_MAX) < y (unreachable).  f(0) = 0 < y is known and never evaluated.
+template <class F>
+__device__ __forceinline__ int64_t swap_crossing(const F& f, double y, double e) {
+  const int64_t o = swap_start_ord(e);
+  int64_t lo = 0, hi = o;
+  if (f(__longlong_as_double(o)) >= y) {  // gallop down: hi stays a tender that reaches y
+    for (int64_t step = 1; hi > 1; step <<= 1) {
+      const int64_t c = hi - step;
+      if (c <= 0) break;  // lo = 0
+      if (f(__longlong_as_double(c)) >= y) {
+        hi = c;
+      } else {
+        lo = c;
+        break;
+      }
+    }
+  } else {  // gallop up: lo stays a tender that falls short
+    lo = o;
+    for (int64_t step = 1;; step <<= 1) {
+      if (lo == kSwapOrdMax) return -1;
+      const int64_t c = kSwapOrdMax - lo <= step ? kSwapOrdMax : lo + step;
+      if (f(__longlong_as_double(c)) >= y) {
+        hi = c;
+        break;
+      }
+      lo = c;
+    }
+  }
+  while (hi - lo > 1) {
+    const int64_t mid = lo + ((hi - lo) >> 1);
+    if (f(__longlong_as_double(mid)) >= y)
+      hi = mid;
+    else
+      lo = mid;
+  }
+  return hi;
+}
+
+// The two-coin estimate of the tender that receives y from (r_in, r_out), fee γ (+inf when
+// y >= r_out):  ProductTwoCoin        e = ((r_in·r_out)/(r_out − y) − r_in)/γ
+//               GeometricMeanTwoCoin  e = (r_in·expm1(−log1p(−(y/r_out))/η))/γ, η = w_in/w_out
+template <int TYPE>
+__device__ __forceinline__ double two_coin_estimate(double r_in, double r_out, double g, double y, double w_in,
+                                                    double w_out) {
+  if (!(y < r_out)) return __longlong_as_double(0x7ff0000000000000ll);
+  double d;
+  if constexpr (TYPE == 0) {
+    d = __dsub_rn(__ddiv_rn(__dmul_rn(r_in, r_out), __dsub_rn(r_out, y)), r_in);
+  } else {
+    const double eta = __ddiv_rn(w_in, w_out);
+    d = __dmul_rn(r_in, expm1(__ddiv_rn(-log1p(-__ddiv_rn(y, r_out)), eta)));
+  }
+  return __ddiv_rn(d, g);
+}
+
+// The UniV3 estimate: the reverse of univ3_walk.  Walking the same ticks in the same direction,
+// a tick whose R_out covers what is still wanted (y′ <= R_out) is inverted,
+// δ′ = k/((R_out + β) − y′) − (R_in + α), and e = (s + δ′)/γ, where s sums the max_amount_pos of
+// the ticks before it; any other tick adds its max_amount_pos to s and takes R_out off y′.  +inf
+// when the ticks run out first.
+__device__ __forceinline__ double univ3_estimate(const double* lower, const double* liq, int nt, double price,
+                                                 int cur, double g, double y, bool tok1) {
+  double s = 0.0;
+  const int step = tok1 ? 1 : -1;
+  for (int idx = cur; tok1 ? idx <= nt : idx >= 1; idx += step) {
+    const double hi = lower[idx - 1], lo = idx < nt ? lower[idx] : 0.0;
+    const Univ3Tick t = univ3_compute_at_tick(liq[idx - 1], hi, lo, price, idx, cur);
+    const double a = tok1 ? t.alpha : t.beta, b = tok1 ? t.beta : t.alpha;
+    const double r_in = tok1 ? t.R1 : t.R2, r_out = tok1 ? t.R2 : t.R1;
+    const double ra = __dadd_rn(r_in, a);
+    if (y <= r_out) {
+      const double d = __dsub_rn(__ddiv_rn(t.k, __dsub_rn(__dadd_rn(r_out, b), y)), ra);
+      return __ddiv_rn(__dadd_rn(s, d), g);
+    }
+    const double mx = b > 0.0 ? __dsub_rn(__ddiv_rn(t.k, b), ra) : (a > 0.0 ? __longlong_as_double(0x7ff0000000000000ll) : 0.0);
+    s = __dadd_rn(s, mx);
+    y = __dsub_rn(y, r_out);
+  }
+  return __longlong_as_double(0x7ff0000000000000ll);
+}
+
+// One pool at its current state, for the exact-output search and the order rows: a tender of the
+// ingest token tok1 (token 1) or token 2.  f, estimate and the transition of one filled row.
+template <int TYPE>
+struct SwapPool {
+  // two-coin
+  double2 R, w;
+  bool sw;
+  // UniV3
+  const double* lower;
+  const double* liq;
+  int nt, cur;
+  double q;
+  double g;
+
+  __device__ __forceinline__ double f(double x, bool tok1) const {
+    if constexpr (TYPE == 2) {
+      return univ3_walk(lower, liq, nt, q, cur, __dmul_rn(g, x), tok1).lambda;
+    } else {
+      const bool in_x = tok1 != sw;  // the tender's reserve is R.x
+      return two_coin_out<TYPE>(in_x ? R.x : R.y, in_x ? R.y : R.x, __dmul_rn(g, x), in_x ? w.x : w.y,
+                                in_x ? w.y : w.x);
+    }
+  }
+
+  __device__ __forceinline__ double estimate(double y, bool tok1) const {
+    if constexpr (TYPE == 2) {
+      return univ3_estimate(lower, liq, nt, q, cur, g, y, tok1);
+    } else {
+      const bool in_x = tok1 != sw;
+      return two_coin_estimate<TYPE>(in_x ? R.x : R.y, in_x ? R.y : R.x, g, y, in_x ? w.x : w.y, in_x ? w.y : w.x);
+    }
+  }
+
+  // x* for y > 0; +inf when unreachable
+  __device__ __forceinline__ double exact_out(double y, bool tok1) const {
+    const int64_t o = swap_crossing([&](double x) { return f(x, tok1); }, y, estimate(y, tok1));
+    return o < 0 ? __longlong_as_double(0x7ff0000000000000ll) : __longlong_as_double(o);
+  }
+
+  // Execute a tender x > 0 as swap_execute_kernel does; returns what it received.
+  __device__ __forceinline__ double execute(double x, bool tok1) {
+    if constexpr (TYPE == 2) {
+      const Univ3Walk wk = univ3_walk(lower, liq, nt, q, cur, __dmul_rn(g, x), tok1);
+      if (wk.moved) {
+        q = wk.price;
+        cur = univ3_tick_of(lower, nt, q);
+      }
+      return wk.lambda;
+    } else {
+      const double d1 = tok1 != sw ? x : 0.0, d2 = tok1 != sw ? 0.0 : x;
+      const double2 l = two_coin_quote<TYPE>(R, g, w, d1, d2);
+      R.x = __dsub_rn(__dadd_rn(R.x, __dmul_rn(g, d1)), l.x);  // (R + γΔ) − Λ, as apply_trades_kernel
+      R.y = __dsub_rn(__dadd_rn(R.y, __dmul_rn(g, d2)), l.y);
+      return tok1 != sw ? l.y : l.x;
+    }
+  }
+};
+
+template <int TYPE>
+__device__ __forceinline__ SwapPool<TYPE> swap_pool(const SwapSet& s, int64_t p) {
+  SwapPool<TYPE> P;
+  P.g = s.gam[p];
+  if constexpr (TYPE == 2) {
+    const int off = s.u.tick[p].x;
+    P.nt = univ3_tick_end(s.u, p) - off;
+    P.lower = s.u.lower + off;
+    P.liq = s.u.liq + off;
+    P.q = univ3_price(s.u, p);
+    P.cur = s.u.tick[p].y;
+  } else {
+    P.R = s.R[p];
+    P.w = TYPE == 1 ? s.w[p] : make_double2(0.0, 0.0);
+    P.sw = (s.gidx[p] >> 62) & 1;
+  }
+  return P;
+}
+
+// Exact-output quotes: one thread per row, addressed as in swap_quote_kernel.  want (0, y) tenders
+// token 1, (y, 0) token 2; tender gets (x*, 0) or (0, x*), +inf for x* when y cannot be reached
+// or the pool is retired, (0, 0) for y = 0.
+template <int TYPE>
+__global__ void swap_quote_exact_out_kernel(SwapSet s, const int64_t* __restrict__ rows,
+                                            const int64_t* __restrict__ pos, int64_t n,
+                                            const double* __restrict__ want, double* __restrict__ tender) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const int64_t row = rows[j], p = pos[j];
+  const double y1 = want[2 * row], y2 = want[2 * row + 1];
+  double x = 0.0;
+  const bool tok1 = y2 > 0.0;
+  if (y1 > 0.0 || y2 > 0.0) {
+    if (s.active && !s.active[p])
+      x = __longlong_as_double(0x7ff0000000000000ll);
+    else
+      x = swap_pool<TYPE>(s, p).exact_out(tok1 ? y2 : y1, tok1);
+  }
+  tender[2 * row] = tok1 ? x : 0.0;
+  tender[2 * row + 1] = tok1 ? 0.0 : x;
+}
+
+// Order rows: one thread per distinct pool, grouped as for swap_execute_kernel.  Each row, in
+// batch order against the running state: kind 0 tenders its amount and reverts when it receives
+// less than limit (0 without limits); kind 1 tenders x* for its wanted amount and reverts when y
+// is unreachable or x* > limit (+inf without limits).  Only filled rows move the running state;
+// the state and the moved list / out-of-range flag are written as swap_execute_kernel writes them.
+template <int TYPE>
+__global__ void swap_execute_orders_kernel(SwapSet s, const int64_t* __restrict__ seg_pos,
+                                           const int64_t* __restrict__ seg_off, const int64_t* __restrict__ seg_rows,
+                                           int64_t n_seg, const uint8_t* __restrict__ kind,
+                                           const double* __restrict__ amount, const double* __restrict__ limit,
+                                           double* __restrict__ paid, double* __restrict__ received,
+                                           uint8_t* __restrict__ status, int64_t* __restrict__ moved,
+                                           unsigned long long* __restrict__ n_moved, int* __restrict__ out_of_range) {
+  const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n_seg) return;
+  const int64_t p = seg_pos[k], r0 = seg_off[k], r1 = seg_off[k + 1];
+  const bool retired = s.active && !s.active[p];
+  SwapPool<TYPE> P;
+  if (!retired) P = swap_pool<TYPE>(s, p);
+  const double q0 = TYPE == 2 && !retired ? P.q : 0.0;
+  for (int64_t r = r0; r < r1; ++r) {
+    const int64_t row = seg_rows[r];
+    const double a1 = amount[2 * row], a2 = amount[2 * row + 1];
+    const bool out = kind[row] == 1;
+    const double inf = __longlong_as_double(0x7ff0000000000000ll);
+    const double lim = limit ? limit[row] : (out ? inf : 0.0);
+    const bool tok1 = out ? a2 > 0.0 : a1 > 0.0;  // the tender is token 1
+    const double amt = a1 > 0.0 ? a1 : a2;
+    double x = 0.0, lam = 0.0;
+    uint8_t st = 0;  // CFMM_ORDER_FILLED
+    if (retired) {
+      st = 3;  // CFMM_ORDER_RETIRED
+    } else if (!out) {
+      x = amt;
+      lam = x > 0.0 ? P.f(x, tok1) : 0.0;
+      if (lam < lim) st = 1;  // CFMM_ORDER_LIMIT
+    } else if (amt > 0.0) {
+      x = P.exact_out(amt, tok1);
+      if (x == inf) st = 2;  // CFMM_ORDER_UNREACHABLE
+      else if (x > lim) st = 1;
+    }
+    if (st == 0) {
+      if (x > 0.0) lam = P.execute(x, tok1);
+    } else {
+      x = 0.0;
+      lam = 0.0;
+    }
+    paid[2 * row] = tok1 ? x : 0.0;
+    paid[2 * row + 1] = tok1 ? 0.0 : x;
+    received[2 * row] = tok1 ? 0.0 : lam;
+    received[2 * row + 1] = tok1 ? lam : 0.0;
+    status[row] = st;
+  }
+  if (retired) return;
+  if constexpr (TYPE == 2) {
+    if (P.q != q0) {
+      reinterpret_cast<double*>(s.u.f1 + p)[1] = P.q;
+      moved[atomicAdd(n_moved, 1ull)] = p;
+    }
+  } else {
+    s.R[p] = P.R;
+    if (!in_fast_range(P.R.x) || !in_fast_range(P.R.y)) atomicOr(out_of_range, 1);
+  }
+}
+
 }  // namespace cfmm

@@ -353,6 +353,35 @@ function execute_swaps!(ctx, ptype::Integer, pools::Vector{Int64}, tender::Matri
     return received
 end
 
+# Exact-output quotes and order rows with slippage limits (cfmm_quote_swaps_exact_out /
+# cfmm_execute_swap_orders).  want / amount are 2 x q as tender above; kind is 0 (exact-in) or 1
+# (exact-out) per row; limit is nothing or a length-q vector.  execute_swap_orders! returns
+# (paid, received, status).  Like the rest of this file, never executed.
+const SWAP_EXACT_IN = 0
+const SWAP_EXACT_OUT = 1
+const ORDER_FILLED, ORDER_LIMIT, ORDER_UNREACHABLE, ORDER_RETIRED = 0, 1, 2, 3
+function quote_swaps_exact_out(ctx, ptype::Integer, pools::Vector{Int64}, want::Matrix{Float64})
+    size(want) == (2, length(pools)) || throw(ArgumentError("want must be 2 x length(pools)"))
+    tender = zeros(Float64, 2, length(pools))
+    chk(ctx, ccall((:cfmm_quote_swaps_exact_out, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Int64, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}),
+        ctx, ptype, length(pools), pools, want, tender))
+    return tender
+end
+function execute_swap_orders!(ctx, ptype::Integer, pools::Vector{Int64}, kind::Vector{UInt8},
+                              amount::Matrix{Float64}, limit::Union{Nothing,Vector{Float64}}=nothing)
+    q = length(pools)
+    size(amount) == (2, q) || throw(ArgumentError("amount must be 2 x length(pools)"))
+    length(kind) == q || throw(ArgumentError("kind must have length(pools) entries"))
+    limit === nothing || length(limit) == q || throw(ArgumentError("limit must have length(pools) entries"))
+    paid, received, status = zeros(Float64, 2, q), zeros(Float64, 2, q), zeros(UInt8, q)
+    chk(ctx, ccall((:cfmm_execute_swap_orders, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Int64, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+         Ptr{Float64}, Ptr{UInt8}),
+        ctx, ptype, q, pools, kind, amount, limit === nothing ? C_NULL : limit, paid, received, status))
+    return paid, received, status
+end
+
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
 # current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never

@@ -338,6 +338,38 @@ class DevicePools:
                                                _dp(out)))
         return out
 
+    def quote_swaps_exact_out(self, pool_type: int, pools, want):
+        """cfmm_quote_swaps_exact_out: the tender x* each row needs to receive want[j] ((0, y):
+        receive token 2 for token 1; (y, 0) the reverse), every row on the current state on its own;
+        no state changes.  Returns tender (q, 2); +inf where y cannot be reached."""
+        pools, want = self._swap_args(pools, want)
+        out = np.zeros((len(pools), 2))
+        self._chk(self._lib.cfmm_quote_swaps_exact_out(self._ctx, int(pool_type), len(pools), _ip(pools),
+                                                       _dp(want), _dp(out)))
+        return out
+
+    def execute_swap_orders(self, pool_type: int, pools, kind, amount, limit=None):
+        """cfmm_execute_swap_orders: rows of kind 0 (exact-in: amount is the tender, limit the
+        minimum received) or 1 (exact-out: amount the wanted output, limit the maximum tender), in
+        batch order; a row whose limit fails reverts.  limit=None: no limits.  Returns
+        (paid (q, 2), received (q, 2), status (q,) uint8; 0 filled, 1 limit, 2 unreachable,
+        3 retired)."""
+        pools, amount = self._swap_args(pools, amount)
+        kind = np.ascontiguousarray(kind, dtype=np.uint8).reshape(-1)
+        if len(kind) != len(pools):
+            raise ValueError(f"kind must have {len(pools)} entries, one per row")
+        if limit is not None:
+            limit = np.ascontiguousarray(limit, dtype=np.float64).reshape(-1)
+            if len(limit) != len(pools):
+                raise ValueError(f"limit must have {len(pools)} entries, one per row")
+        paid, received = np.zeros((len(pools), 2)), np.zeros((len(pools), 2))
+        status = np.zeros(len(pools), dtype=np.uint8)
+        u8 = C.POINTER(C.c_uint8)
+        self._chk(self._lib.cfmm_execute_swap_orders(
+            self._ctx, int(pool_type), len(pools), _ip(pools), kind.ctypes.data_as(u8), _dp(amount),
+            None if limit is None else _dp(limit), _dp(paid), _dp(received), status.ctypes.data_as(u8)))
+        return paid, received, status
+
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
         """cfmm_modify_univ3_liquidity: row j adds dL[j] (> 0 mints, < 0 burns) to the ticks of UniV3
@@ -635,6 +667,43 @@ class Router:
         out = np.zeros((len(ids), 2))
         for t, rows, loc in groups:
             out[rows] = self._pools.execute_swaps(t, loc, tenders[rows])
+        self._refresh_swapped(groups)
+        return out
+
+    def quote_swaps_exact_out(self, list_indices, wants):
+        """The tender each row needs to receive wants[j] ((0, y): y of the pool's token 2 for its
+        token 1; (y, 0) the reverse) from r.cfmms[list_indices[j]], every row on the current state on
+        its own (cfmm_quote_swaps_exact_out); no state changes.  Returns tender (q, 2) in the
+        caller's order, +inf where y cannot be reached.  Single GPU."""
+        ids, wants, groups = self._swap_rows(list_indices, wants, "quote_swaps_exact_out")
+        out = np.zeros((len(ids), 2))
+        for t, rows, loc in groups:
+            out[rows] = self._pools.quote_swaps_exact_out(t, loc, wants[rows])
+        return out
+
+    def execute_swap_orders(self, list_indices, kinds, amounts, limits=None):
+        """Execute exact-in (kind 0) and exact-out (kind 1) rows in order with optional limits
+        (cfmm_execute_swap_orders): a row whose limit fails reverts and later rows see the state
+        without it.  Returns (paid, received, status) in the caller's order and refreshes the
+        touched pool objects from the device state, as execute_swaps does.  Single GPU."""
+        ids, amounts, groups = self._swap_rows(list_indices, amounts, "execute_swap_orders")
+        kinds = np.asarray(kinds, dtype=np.uint8).reshape(-1)
+        if len(kinds) != len(ids):
+            raise ValueError(f"execute_swap_orders: kinds must have {len(ids)} entries")
+        if limits is not None:
+            limits = np.asarray(limits, dtype=np.float64).reshape(-1)
+            if len(limits) != len(ids):
+                raise ValueError(f"execute_swap_orders: limits must have {len(ids)} entries")
+        paid, received = np.zeros((len(ids), 2)), np.zeros((len(ids), 2))
+        status = np.zeros(len(ids), dtype=np.uint8)
+        for t, rows, loc in groups:
+            paid[rows], received[rows], status[rows] = self._pools.execute_swap_orders(
+                t, loc, kinds[rows], amounts[rows], None if limits is None else limits[rows])
+        self._refresh_swapped(groups)
+        return paid, received, status
+
+    def _refresh_swapped(self, groups):
+        """The touched pool objects' R, or current_price / current_tick, from the device state."""
         for t, rows, loc in groups:
             touched = np.unique(loc)
             lo, hi = int(touched[0]), int(touched[-1]) + 1
@@ -647,7 +716,6 @@ class Router:
                     c.current_tick = int(np.sum(c.lower_ticks >= c.current_price))
                 else:
                     c.R = state[k - lo].copy()
-        return out
 
     def modify_liquidity(self, list_indices, lo, hi, dL):
         """Mint (dL > 0) or burn (dL < 0) liquidity on the price range (lo[j], hi[j]] of the UniV3

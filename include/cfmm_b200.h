@@ -286,6 +286,75 @@ int cfmm_quote_swaps(cfmm_ctx *ctx, int type, int64_t q, const int64_t *pool,
 int cfmm_execute_swaps(cfmm_ctx *ctx, int type, int64_t q, const int64_t *pool,
                        const double *tender, double *received /* may be NULL */);
 
+/* ---- exact-output swaps and slippage limits ----------------------------------------------
+ * f(x) below is the exact-input quote of one pool at its current state as a function of the gross
+ * tender x on one side: what cfmm_quote_swaps returns for that tender, bit for bit (f(0) = 0).
+ *
+ * Exact-output quote.  For a wanted output y > 0 on the side opposite the tender, the tender x* is
+ * a crossing of f through y on the ordered doubles of [0, DBL_MAX]:
+ *     f(x*) >= y, and x* = 0 or f(pred(x*)) < y        (pred: the next smaller double).
+ * y = 0 gives x* = 0; x* = +inf when f(DBL_MAX) < y (unreachable) or the pool is retired.
+ * The search is deterministic and bounded.  It starts from the estimate e (each step one IEEE
+ * operation, round to nearest; log1p / expm1 are CUDA's), for a tender of the token with reserve
+ * R_in and fee γ, wanting y of the other (R_out):
+ *   ProductTwoCoin        e = ((R_in·R_out)/(R_out − y) − R_in)/γ, +inf if y >= R_out
+ *   GeometricMeanTwoCoin  e = (R_in·expm1(−log1p(−(y/R_out))/η))/γ, η = w_in/w_out, +inf if y >= R_out
+ *   UniV3                 the ticks of the forward walk in its order, each from compute_at_tick
+ *                         with α, β, R_in, R_out flipped for a token-2 tender; s = 0, y′ = y:
+ *                         a tick with y′ <= R_out ends the walk with
+ *                           e = (s + (k/((R_out + β) − y′) − (R_in + α)))/γ,
+ *                         any other tick does s = s + max_amount_pos, y′ = y′ − R_out; +inf if the
+ *                         ticks run out.
+ * Let o(x) be the bit pattern of a double x >= 0 read as an int64 (monotone in x), and
+ * o_e = o(e) clamped to [1, o(DBL_MAX)] (1 for a NaN or e <= 0).  If f(e) >= y the search gallops
+ * down: hi = o_e, then c = hi − 1, hi − 2, hi − 4, … (each step from the last c that still
+ * reached y) until f(c) < y (lo = c) or c <= 0 (lo = 0).  Otherwise it gallops up: lo = o_e, then
+ * c = lo + 1, lo + 2, lo + 4, … capped at o(DBL_MAX), until f(c) >= y (hi = c); unreachable
+ * when o(DBL_MAX) falls short.  It then bisects, mid = lo + (hi − lo)/2, keeping f(lo) < y <=
+ * f(hi), until hi = lo + 1, and x* = hi.  At most 1 + 63 + 62 evaluations of f.
+ *   ProductTwoCoin: f is non-decreasing in x.  γ·x, R_in + δ, k/·, R_out − · and min(R_out, ·)
+ *   are each correctly rounded monotone functions (non-decreasing, or non-increasing for k/·
+ *   with the subtraction reversing it), so their composition is monotone; the crossing is unique
+ *   and x* is the least double that receives at least y.
+ *   UniV3 and GeometricMeanTwoCoin: f can step back by a few ulp (where a UniV3 walk enters a new
+ *   tick, whose first output can round slightly below zero; through CUDA's log1p and expm1), so
+ *   several crossings can lie within a few ulp.  x* is the one this search finds.
+ *
+ * cfmm_quote_swaps_exact_out: want [2q] pool-major, (0, y) receives token 2 for a tender of token
+ * 1 and (y, 0) the reverse (ingest token order, as cfmm_quote_swaps); tender [2q] gets (x*, 0) or
+ * (0, x*).  Rows are priced on the current state on their own; no state changes.
+ *
+ * cfmm_execute_swap_orders: rows of kind CFMM_SWAP_EXACT_IN (amount = the tender, as
+ * cfmm_execute_swaps; limit = the minimum received, NULL means 0) or CFMM_SWAP_EXACT_OUT (amount =
+ * the wanted output, as above; limit = the maximum tender, NULL or +inf means none), applied in
+ * batch order per pool.  An exact-out row's x* is computed against the pool's state after the
+ * earlier rows of the batch.  A row reverts, changing nothing, when its pool is retired
+ * (CFMM_ORDER_RETIRED), an exact-in row receives less than its limit or an exact-out row's x*
+ * exceeds its limit (CFMM_ORDER_LIMIT), or y is unreachable (CFMM_ORDER_UNREACHABLE); later rows
+ * see the state without it.  An equal limit fills.  A filled row (CFMM_ORDER_FILLED) runs the
+ * transition of cfmm_execute_swaps with its tender, so the filled rows of a batch leave exactly
+ * the state, and receive exactly what, cfmm_execute_swaps with their paid tenders gives.  Per row:
+ * paid [2q] the gross tender on the tender side, received [2q] (an exact-out row receives f(x*) >=
+ * y), status [q]; a reverted row pays and receives (0, 0).  The bookkeeping afterwards is that of
+ * cfmm_execute_swaps.
+ *
+ * Both are synchronous.  Before cfmm_finalize: CFMM_ERR_STATE.  CFMM_ERR_INVALID before anything
+ * runs, so no pool changes, for a bad type, a pool outside the type's pools, a kind other than 0
+ * or 1, an amount that is NaN, Inf, negative or has both sides > 0, a limit that is NaN or
+ * negative, or a limit of +inf on an exact-in row.  q == 0 does nothing. */
+#define CFMM_SWAP_EXACT_IN 0
+#define CFMM_SWAP_EXACT_OUT 1
+#define CFMM_ORDER_FILLED 0
+#define CFMM_ORDER_LIMIT 1
+#define CFMM_ORDER_UNREACHABLE 2
+#define CFMM_ORDER_RETIRED 3
+int cfmm_quote_swaps_exact_out(cfmm_ctx *ctx, int type, int64_t q, const int64_t *pool,
+                               const double *want /* [2q] */, double *tender /* [2q], +inf unreachable */);
+int cfmm_execute_swap_orders(cfmm_ctx *ctx, int type, int64_t q, const int64_t *pool,
+                             const uint8_t *kind /* [q] */, const double *amount /* [2q] */,
+                             const double *limit /* [q] or NULL */, double *paid /* [2q] or NULL */,
+                             double *received /* [2q] or NULL */, uint8_t *status /* [q] or NULL */);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
@@ -430,7 +499,8 @@ int64_t cfmm_launch_count(const cfmm_ctx *ctx);
  * pairs for the next N kernel launches (recorded on the launching stream,
  * around each sweep kernel / the peer exchange).  cfmm_profile_read sums the
  * durations recorded so far for one pool type (cfmm_pool_type, 3 = the multi-GPU
- * exchange kernel, or 4 = the kernels of cfmm_quote_swaps / cfmm_execute_swaps); it
+ * exchange kernel, or 4 = the kernels of cfmm_quote_swaps / cfmm_execute_swaps /
+ * cfmm_quote_swaps_exact_out / cfmm_execute_swap_orders); it
  * synchronises on the recorded events.
  * cfmm_profile_reset re-arms the same N pairs. */
 int cfmm_profile_read(cfmm_ctx *ctx, int type, double *total_ms, int64_t *launches);
