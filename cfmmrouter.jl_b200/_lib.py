@@ -31,6 +31,8 @@ ORDER_FILLED = 0
 ORDER_LIMIT = 1
 ORDER_UNREACHABLE = 2
 ORDER_RETIRED = 3
+# cfmm_quote_paths / cfmm_execute_paths
+PATH_MAX_HOPS = 8
 
 COMM_HANDLE_BYTES = 128
 
@@ -80,7 +82,11 @@ SYMBOLS = {
     "cfmm_quote_swaps_exact_out": (C.c_int, [_ctx, C.c_int, C.c_int64, _ip, _dp, _dp]),
     "cfmm_execute_swap_orders": (C.c_int, [_ctx, C.c_int, C.c_int64, _ip, C.POINTER(C.c_uint8), _dp, _dp, _dp, _dp,
                                            C.POINTER(C.c_uint8)]),
-    "cfmm_modify_univ3_liquidity": (C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
+    "cfmm_quote_paths": (C.c_int, [_ctx, C.c_int64, _ip, C.POINTER(C.c_int), _ip, _ip, C.POINTER(C.c_uint8), _dp,
+                                   _dp, _dp, C.POINTER(C.c_uint8)]),
+    "cfmm_execute_paths": (C.c_int, [_ctx, C.c_int64, _ip, C.POINTER(C.c_int), _ip, _ip, C.POINTER(C.c_uint8), _dp,
+                                     _dp, _dp, _dp, C.POINTER(C.c_uint8)]),
+    "cfmm_modify_univ3_liquidity":(C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),
     "cfmm_set_option": (C.c_int, [_ctx, C.c_char_p, C.c_int64]),

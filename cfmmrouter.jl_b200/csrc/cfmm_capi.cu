@@ -31,6 +31,7 @@
 #include "product_tma.cuh"
 #include "solver.cuh"
 #include "swap_kernels.cuh"
+#include "path_kernels.cuh"
 #include "univ3_state.cuh"
 
 namespace {
@@ -2448,6 +2449,7 @@ int swap_bookkeeping(cfmm_ctx* ctx, PoolSet& s, int type, const int64_t* d_moved
       std::vector<int64_t> moved((size_t)h_moved);
       CU_TRY(ctx, cudaMemcpy(moved.data(), d_moved, (size_t)h_moved * sizeof(int64_t), cudaMemcpyDeviceToHost));
       std::sort(moved.begin(), moved.end());
+      moved.erase(std::unique(moved.begin(), moved.end()), moved.end());  // (a pool crossed by several paths)
       if ((rc = univ3_update_listed(ctx, s, moved, nullptr, nullptr, true)) != CFMM_OK) return rc;
     }
   } else {
@@ -2662,6 +2664,280 @@ int cfmm_execute_swap_orders(cfmm_ctx* ctx, int type, int64_t q, const int64_t* 
   if (status) CU_TRY(ctx, cudaMemcpyAsync(status, d_status.p, (size_t)q, cudaMemcpyDeviceToHost, ctx->stream));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return CFMM_OK;
+}
+
+// ---- multi-hop swap paths (path_kernels.cuh) ---------------------------------------------------
+namespace {
+
+// Set k of the path kernels: 2·type, + 1 for the type's appended pools.
+PoolSet& path_set(cfmm_ctx* ctx, int k) { return (k & 1) ? ctx->tails[k >> 1] : ctx->sets[k >> 1]; }
+
+// Every host-side argument of cfmm_quote_paths / cfmm_execute_paths, checked before any launch
+// (the token walk is checked on the device, path_check_kernel).
+int check_paths(cfmm_ctx* ctx, int64_t q, const int64_t* hop_off, const int* hop_type, const int64_t* hop_pool,
+                const int64_t* token_in, const uint8_t* kind, const double* amount, const double* limit,
+                const char* what) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if (q < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: negative path count", what);
+  if (q == 0) return CFMM_OK;
+  if (!hop_off || !hop_type || !hop_pool || !token_in || !kind || !amount)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
+  if (hop_off[0] != 0) return fail(ctx, CFMM_ERR_INVALID, "%s: hop_off[0] must be 0", what);
+  for (int64_t j = 0; j < q; ++j) {
+    const int64_t n = hop_off[j + 1] - hop_off[j];
+    if (n < 1 || n > CFMM_PATH_MAX_HOPS)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld has %lld hops (hop_off must rise by 1..%d per path)", what,
+                  (long long)j, (long long)n, CFMM_PATH_MAX_HOPS);
+  }
+  for (int64_t j = 0; j < q; ++j) {
+    for (int64_t h = hop_off[j]; h < hop_off[j + 1]; ++h) {
+      const int t = hop_type[h];
+      if (t != CFMM_POOL_PRODUCT && t != CFMM_POOL_GEOMEAN && t != CFMM_POOL_UNIV3)
+        return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld hop %lld: unknown pool type %d", what, (long long)j,
+                    (long long)(h - hop_off[j]), t);
+      if (hop_pool[h] < 0 || hop_pool[h] >= type_pools(ctx, t))
+        return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld hop %lld: pool %lld outside 0..%lld", what, (long long)j,
+                    (long long)(h - hop_off[j]), (long long)hop_pool[h], (long long)type_pools(ctx, t));
+      for (int64_t g = hop_off[j]; g < h; ++g)
+        if (hop_type[g] == t && hop_pool[g] == hop_pool[h])
+          return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld: hops %lld and %lld are the same pool", what, (long long)j,
+                      (long long)(g - hop_off[j]), (long long)(h - hop_off[j]));
+    }
+    if (token_in[j] < 1 || token_in[j] > ctx->n_tokens)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld: token_in %lld outside 1..%lld", what, (long long)j,
+                  (long long)token_in[j], (long long)ctx->n_tokens);
+    if (kind[j] != CFMM_SWAP_EXACT_IN && kind[j] != CFMM_SWAP_EXACT_OUT)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld: kind %d is neither exact-in (0) nor exact-out (1)", what,
+                  (long long)j, (int)kind[j]);
+    if (!std::isfinite(amount[j]) || amount[j] < 0.0)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld: amount %g must be finite and >= 0", what, (long long)j,
+                  amount[j]);
+    if (!limit) continue;
+    if (std::isnan(limit[j]) || limit[j] < 0.0)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld: limit %g must be >= 0", what, (long long)j, limit[j]);
+    if (std::isinf(limit[j]) && kind[j] == CFMM_SWAP_EXACT_IN)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld: an exact-in path's minimum received must be finite", what,
+                  (long long)j);
+  }
+  return CFMM_OK;
+}
+
+// One path call on the device: the hops resolved to (set, device position) as rows_by_set
+// resolves rows, the path arrays, the six sets (PathSets, in device memory) and the per-hop outputs.
+struct PathCall {
+  int64_t q = 0, H = 0;
+  std::vector<uint8_t> set;
+  std::vector<int64_t> pos;
+  DevBuf<int64_t> d_off, d_pos, d_token;
+  DevBuf<uint8_t> d_set, d_tok1, d_kind, d_status;
+  DevBuf<double> d_amount, d_tender, d_recv;
+  DevBuf<cfmm::PathSets> d_P;
+  cfmm::PathSets P{};
+};
+
+// Upload a checked call, walk its tokens on the device (path_check_kernel) and reject it, before
+// anything is written, when some hop's pool does not hold the token that reaches it.
+int path_prepare(cfmm_ctx* ctx, PathCall& c, int64_t q, const int64_t* hop_off, const int* hop_type,
+                 const int64_t* hop_pool, const int64_t* token_in, const uint8_t* kind, const double* amount,
+                 const char* what) {
+  int rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  c.q = q;
+  c.H = hop_off[q];
+  for (int k = 0; k < cfmm::kPathSets; ++k) ensure_pos_of(path_set(ctx, k));
+  c.set.resize((size_t)c.H);
+  c.pos.resize((size_t)c.H);
+  for (int64_t h = 0; h < c.H; ++h) {
+    const int t = hop_type[h];
+    const int64_t m_main = ctx->sets[t].m;
+    const bool tail = hop_pool[h] >= m_main;
+    c.set[(size_t)h] = (uint8_t)(2 * t + (tail ? 1 : 0));
+    c.pos[(size_t)h] = path_set(ctx, 2 * t + (tail ? 1 : 0)).pos_of[(size_t)(tail ? hop_pool[h] - m_main : hop_pool[h])];
+  }
+  for (int k = 0; k < cfmm::kPathSets; ++k) {
+    PoolSet& s = path_set(ctx, k);
+    c.P.s[k] = swap_set(s);
+    c.P.Ai[k] = s.d_Ai.p;
+  }
+  CU_TRY(ctx, c.d_off.alloc((size_t)q + 1));
+  CU_TRY(ctx, DevBuf<int64_t>::copy_in(c.d_off.p, hop_off, (size_t)(q + 1) * sizeof(int64_t)));
+  CU_TRY(ctx, c.d_token.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<int64_t>::copy_in(c.d_token.p, token_in, (size_t)q * sizeof(int64_t)));
+  CU_TRY(ctx, c.d_kind.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<uint8_t>::copy_in(c.d_kind.p, kind, (size_t)q));
+  CU_TRY(ctx, c.d_amount.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<double>::copy_in(c.d_amount.p, amount, (size_t)q * sizeof(double)));
+  CU_TRY(ctx, c.d_set.upload(c.set));
+  CU_TRY(ctx, c.d_pos.upload(c.pos));
+  CU_TRY(ctx, c.d_tok1.alloc((size_t)c.H));
+  CU_TRY(ctx, c.d_tender.alloc((size_t)c.H));
+  CU_TRY(ctx, c.d_recv.alloc((size_t)c.H));
+  CU_TRY(ctx, c.d_status.alloc((size_t)q));
+  CU_TRY(ctx, c.d_P.alloc(1));
+  CU_TRY(ctx, DevBuf<cfmm::PathSets>::copy_in(c.d_P.p, &c.P, sizeof(cfmm::PathSets)));
+  DevBuf<unsigned long long> d_bad;
+  CU_TRY(ctx, d_bad.alloc(1));
+  CU_TRY(ctx, cudaMemsetAsync(d_bad.p, 0xff, sizeof(unsigned long long), ctx->stream));
+  {
+    ProfScope prof(ctx, kProfSwaps, ctx->stream);
+    cfmm::path_check_kernel<<<(unsigned)((q + 255) / 256), 256, 0, ctx->stream>>>(
+        c.d_P.p, q, c.d_off.p, c.d_set.p, c.d_pos.p, c.d_token.p, c.d_tok1.p, d_bad.p);
+  }
+  ctx->launches++;
+  CU_TRY(ctx, cudaGetLastError());
+  unsigned long long bad = 0;
+  CU_TRY(ctx, cudaMemcpyAsync(&bad, d_bad.p, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  if (bad != ~0ull) {
+    const int64_t j = (int64_t)(std::upper_bound(hop_off, hop_off + q + 1, (int64_t)bad) - hop_off) - 1;
+    int64_t t = token_in[j];
+    for (int64_t h = hop_off[j]; h < (int64_t)bad; ++h) {  // the token that reached the bad hop
+      int2 ai;
+      CU_TRY(ctx, cudaMemcpy(&ai, path_set(ctx, c.set[(size_t)h]).d_Ai.p + c.pos[(size_t)h], sizeof(int2),
+                             cudaMemcpyDeviceToHost));
+      t = (t - 1 == ai.x ? ai.y : ai.x) + 1;
+    }
+    return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld hop %lld: pool %lld of type %d does not hold token %lld", what,
+                (long long)j, (long long)(bad - hop_off[j]), (long long)hop_pool[bad], hop_type[bad], (long long)t);
+  }
+  return CFMM_OK;
+}
+
+int path_outputs(cfmm_ctx* ctx, const PathCall& c, double* hop_tender, double* hop_received, uint8_t* status) {
+  if (hop_tender)
+    CU_TRY(ctx, cudaMemcpyAsync(hop_tender, c.d_tender.p, (size_t)c.H * sizeof(double), cudaMemcpyDeviceToHost,
+                                ctx->stream));
+  if (hop_received)
+    CU_TRY(ctx, cudaMemcpyAsync(hop_received, c.d_recv.p, (size_t)c.H * sizeof(double), cudaMemcpyDeviceToHost,
+                                ctx->stream));
+  if (status) CU_TRY(ctx, cudaMemcpyAsync(status, c.d_status.p, (size_t)c.q, cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return CFMM_OK;
+}
+
+// The last level a pool of one set was given in this call (0 = none yet): a dense array when the
+// call's hops on the set are many against its size, a hash otherwise (group_by_pool's rule).
+struct LevelTable {
+  std::vector<int> dense;
+  std::unordered_map<int64_t, int> sparse;
+  int& at(int64_t p) { return dense.empty() ? sparse[p] : dense[(size_t)p]; }
+};
+
+// Execution order of cfmm_execute_paths: path j's level is 1 + the largest level of an earlier
+// path sharing one of its pools, so the paths of one level touch disjoint pools and every pool sees
+// its paths in batch order.  order: the paths sorted stably by (level, batch index); the paths of
+// level L (1-based) are order[level_off[L-1] .. level_off[L]).
+void path_levels(cfmm_ctx* ctx, const PathCall& c, const int64_t* hop_off, std::vector<int64_t>& order,
+                 std::vector<int64_t>& level_off) {
+  LevelTable tab[cfmm::kPathSets];
+  int64_t count[cfmm::kPathSets] = {};
+  for (int64_t h = 0; h < c.H; ++h) count[c.set[(size_t)h]]++;
+  for (int k = 0; k < cfmm::kPathSets; ++k) {
+    const int64_t mp = path_set(ctx, k).m_padded;
+    if (count[k] > 0 && count[k] * 8 >= mp)
+      tab[k].dense.assign((size_t)mp, 0);
+    else
+      tab[k].sparse.reserve((size_t)count[k]);
+  }
+  std::vector<int> lev((size_t)c.q);
+  int n_levels = 0;
+  for (int64_t j = 0; j < c.q; ++j) {
+    int L = 0;
+    for (int64_t h = hop_off[j]; h < hop_off[j + 1]; ++h) L = std::max(L, tab[c.set[(size_t)h]].at(c.pos[(size_t)h]));
+    ++L;
+    for (int64_t h = hop_off[j]; h < hop_off[j + 1]; ++h) tab[c.set[(size_t)h]].at(c.pos[(size_t)h]) = L;
+    lev[(size_t)j] = L;
+    n_levels = std::max(n_levels, L);
+  }
+  level_off.assign((size_t)n_levels + 1, 0);
+  for (int64_t j = 0; j < c.q; ++j) level_off[(size_t)lev[(size_t)j]]++;
+  for (int L = 1; L <= n_levels; ++L) level_off[(size_t)L] += level_off[(size_t)L - 1];
+  std::vector<int64_t> next(level_off.begin(), level_off.end() - 1);
+  order.resize((size_t)c.q);
+  for (int64_t j = 0; j < c.q; ++j) order[(size_t)next[(size_t)lev[(size_t)j] - 1]++] = j;
+}
+
+}  // namespace
+
+int cfmm_quote_paths(cfmm_ctx* ctx, int64_t q, const int64_t* hop_off, const int* hop_type, const int64_t* hop_pool,
+                     const int64_t* token_in, const uint8_t* kind, const double* amount, double* hop_tender,
+                     double* hop_received, uint8_t* status) {
+  int rc = check_paths(ctx, q, hop_off, hop_type, hop_pool, token_in, kind, amount, nullptr, "quote_paths");
+  if (rc != CFMM_OK || q == 0) return rc;
+  if (!hop_tender || !hop_received || !status) return fail(ctx, CFMM_ERR_INVALID, "quote_paths: null array argument");
+  PathCall c;
+  if ((rc = path_prepare(ctx, c, q, hop_off, hop_type, hop_pool, token_in, kind, amount, "quote_paths")) != CFMM_OK)
+    return rc;
+  {
+    ProfScope prof(ctx, kProfSwaps, ctx->stream);
+    cfmm::path_quote_kernel<<<(unsigned)((q + 255) / 256), 256, 0, ctx->stream>>>(
+        c.d_P.p, q, c.d_off.p, c.d_set.p, c.d_pos.p, c.d_tok1.p, c.d_kind.p, c.d_amount.p, c.d_tender.p, c.d_recv.p,
+        c.d_status.p);
+  }
+  ctx->launches++;
+  CU_TRY(ctx, cudaGetLastError());
+  return path_outputs(ctx, c, hop_tender, hop_received, status);
+}
+
+int cfmm_execute_paths(cfmm_ctx* ctx, int64_t q, const int64_t* hop_off, const int* hop_type, const int64_t* hop_pool,
+                       const int64_t* token_in, const uint8_t* kind, const double* amount, const double* limit,
+                       double* hop_tender, double* hop_received, uint8_t* status) {
+  int rc = check_paths(ctx, q, hop_off, hop_type, hop_pool, token_in, kind, amount, limit, "execute_paths");
+  if (rc != CFMM_OK || q == 0) return rc;
+  PathCall c;
+  if ((rc = path_prepare(ctx, c, q, hop_off, hop_type, hop_pool, token_in, kind, amount, "execute_paths")) != CFMM_OK)
+    return rc;
+  ctx->state_version++;
+  DevBuf<double> d_limit;
+  if (limit) {
+    CU_TRY(ctx, d_limit.alloc((size_t)q));
+    CU_TRY(ctx, DevBuf<double>::copy_in(d_limit.p, limit, (size_t)q * sizeof(double)));
+  }
+  // bookkeeping words: out_of_range [6], touched [6]; the moved lists of the two UniV3 sets
+  DevBuf<int> d_flags;
+  DevBuf<unsigned long long> d_n_moved;
+  DevBuf<int64_t> d_moved[2];
+  CU_TRY(ctx, d_flags.alloc(2 * cfmm::kPathSets));
+  CU_TRY(ctx, d_n_moved.alloc(2));
+  CU_TRY(ctx, cudaMemsetAsync(d_flags.p, 0, 2 * cfmm::kPathSets * sizeof(int), ctx->stream));
+  CU_TRY(ctx, cudaMemsetAsync(d_n_moved.p, 0, 2 * sizeof(unsigned long long), ctx->stream));
+  for (int u = 0; u < 2; ++u) {
+    const int64_t n = std::count(c.set.begin(), c.set.end(), (uint8_t)(2 * CFMM_POOL_UNIV3 + u));
+    CU_TRY(ctx, d_moved[u].alloc((size_t)n));
+    c.P.moved[u] = d_moved[u].p;
+  }
+  c.P.out_of_range = d_flags.p;
+  c.P.touched = d_flags.p + cfmm::kPathSets;
+  c.P.n_moved = d_n_moved.p;
+  CU_TRY(ctx, DevBuf<cfmm::PathSets>::copy_in(c.d_P.p, &c.P, sizeof(cfmm::PathSets)));
+  std::vector<int64_t> order, level_off;
+  path_levels(ctx, c, hop_off, order, level_off);
+  DevBuf<int64_t> d_order;
+  CU_TRY(ctx, d_order.upload(order));
+  for (size_t L = 1; L < level_off.size(); ++L) {
+    const int64_t n = level_off[L] - level_off[L - 1];
+    {
+      ProfScope prof(ctx, kProfSwaps, ctx->stream);
+      cfmm::path_execute_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(
+          c.d_P.p, d_order.p + level_off[L - 1], n, c.d_off.p, c.d_set.p, c.d_pos.p, c.d_tok1.p, c.d_kind.p,
+          c.d_amount.p, d_limit.p, c.d_tender.p, c.d_recv.p, c.d_status.p);
+    }
+    ctx->launches++;
+    CU_TRY(ctx, cudaGetLastError());
+  }
+  int touched[cfmm::kPathSets];
+  CU_TRY(ctx, cudaMemcpyAsync(touched, c.P.touched, sizeof(touched), cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  for (int k = 0; k < cfmm::kPathSets; ++k) {
+    if (!touched[k]) continue;
+    const int t = k >> 1;
+    if ((rc = swap_bookkeeping(ctx, path_set(ctx, k), t, t == CFMM_POOL_UNIV3 ? d_moved[k & 1].p : nullptr,
+                               d_n_moved.p + (k & 1), d_flags.p + k)) != CFMM_OK)
+      return rc;
+  }
+  return path_outputs(ctx, c, hop_tender, hop_received, status);
 }
 
 // ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------

@@ -382,6 +382,43 @@ function execute_swap_orders!(ctx, ptype::Integer, pools::Vector{Int64}, kind::V
     return paid, received, status
 end
 
+# Multi-hop swap paths (cfmm_quote_paths / cfmm_execute_paths).  Path j is the hops
+# hop_off[j]+1 .. hop_off[j+1] of hop_type / hop_pool (hop_off is the 0-based CSR offset vector of
+# length q+1; pools are 0-based insertion indices of their type); token_in is 1-based.  Both
+# return (hop_tender, hop_received, status).  Like the rest of this file, never executed.
+const PATH_MAX_HOPS = 8
+function _check_paths(hop_off, hop_type, hop_pool, token_in, kind, amount)
+    q = length(hop_off) - 1
+    q >= 0 && length(token_in) == length(kind) == length(amount) == q ||
+        throw(ArgumentError("hop_off needs q+1 entries, token_in / kind / amount q each"))
+    length(hop_type) == length(hop_pool) == hop_off[end] ||
+        throw(ArgumentError("hop_type / hop_pool need hop_off[end] entries"))
+    return q, Int(hop_off[end])
+end
+function quote_paths(ctx, hop_off::Vector{Int64}, hop_type::Vector{Cint}, hop_pool::Vector{Int64},
+                     token_in::Vector{Int64}, kind::Vector{UInt8}, amount::Vector{Float64})
+    q, H = _check_paths(hop_off, hop_type, hop_pool, token_in, kind, amount)
+    tender, received, status = zeros(Float64, H), zeros(Float64, H), zeros(UInt8, q)
+    chk(ctx, ccall((:cfmm_quote_paths, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Cint}, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64},
+         Ptr{Float64}, Ptr{Float64}, Ptr{UInt8}),
+        ctx, q, hop_off, hop_type, hop_pool, token_in, kind, amount, tender, received, status))
+    return tender, received, status
+end
+function execute_paths!(ctx, hop_off::Vector{Int64}, hop_type::Vector{Cint}, hop_pool::Vector{Int64},
+                        token_in::Vector{Int64}, kind::Vector{UInt8}, amount::Vector{Float64},
+                        limit::Union{Nothing,Vector{Float64}}=nothing)
+    q, H = _check_paths(hop_off, hop_type, hop_pool, token_in, kind, amount)
+    limit === nothing || length(limit) == q || throw(ArgumentError("limit must have q entries"))
+    tender, received, status = zeros(Float64, H), zeros(Float64, H), zeros(UInt8, q)
+    chk(ctx, ccall((:cfmm_execute_paths, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Cint}, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64},
+         Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8}),
+        ctx, q, hop_off, hop_type, hop_pool, token_in, kind, amount, limit === nothing ? C_NULL : limit,
+        tender, received, status))
+    return tender, received, status
+end
+
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
 # current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never

@@ -370,6 +370,54 @@ class DevicePools:
             None if limit is None else _dp(limit), _dp(paid), _dp(received), status.ctypes.data_as(u8)))
         return paid, received, status
 
+    # -- multi-hop paths (include/cfmm_b200.h, cfmm_quote_paths / cfmm_execute_paths) ------------
+    @staticmethod
+    def _path_args(hop_off, hop_type, hop_pool, token_in, kind, amount):
+        hop_off = np.ascontiguousarray(hop_off, dtype=np.int64).reshape(-1)
+        hop_type = np.ascontiguousarray(hop_type, dtype=np.int32).reshape(-1)
+        hop_pool = np.ascontiguousarray(hop_pool, dtype=np.int64).reshape(-1)
+        token_in = np.ascontiguousarray(token_in, dtype=np.int64).reshape(-1)
+        kind = np.ascontiguousarray(kind, dtype=np.uint8).reshape(-1)
+        amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
+        q = len(hop_off) - 1
+        if q < 0 or not (len(token_in) == len(kind) == len(amount) == q):
+            raise ValueError("paths: hop_off needs q + 1 entries and token_in, kind, amount q each")
+        H = int(hop_off[-1])
+        if not (len(hop_type) == len(hop_pool) == H):
+            raise ValueError(f"paths: hop_type and hop_pool need hop_off[-1] = {H} entries")
+        return q, H, hop_off, hop_type, hop_pool, token_in, kind, amount
+
+    def quote_paths(self, hop_off, hop_type, hop_pool, token_in, kind, amount):
+        """cfmm_quote_paths: path j is the hops hop_off[j] .. hop_off[j+1] (pool hop_pool[h] of type
+        hop_type[h]), starting with token token_in[j] (1-based); kind 0 tenders amount[j] to the first
+        hop, kind 1 wants amount[j] out of the last.  Every path on the current state on its own; no
+        state changes.  Returns (hop_tender [H], hop_received [H], status [q] uint8)."""
+        q, H, off, typ, pool, tok, kind, amount = self._path_args(hop_off, hop_type, hop_pool, token_in, kind, amount)
+        tender, received, status = np.zeros(H), np.zeros(H), np.zeros(q, dtype=np.uint8)
+        u8, i32 = C.POINTER(C.c_uint8), C.POINTER(C.c_int)
+        self._chk(self._lib.cfmm_quote_paths(self._ctx, q, _ip(off), typ.ctypes.data_as(i32), _ip(pool), _ip(tok),
+                                             kind.ctypes.data_as(u8), _dp(amount), _dp(tender), _dp(received),
+                                             status.ctypes.data_as(u8)))
+        return tender, received, status
+
+    def execute_paths(self, hop_off, hop_type, hop_pool, token_in, kind, amount, limit=None):
+        """cfmm_execute_paths: the paths of quote_paths in batch order, each with its limit (kind 0:
+        the minimum final output; kind 1: the maximum first tender; None: no limits).  A path whose
+        limit fails reverts every hop, and later paths see the state without it.  Returns
+        (hop_tender [H], hop_received [H], status [q] uint8)."""
+        q, H, off, typ, pool, tok, kind, amount = self._path_args(hop_off, hop_type, hop_pool, token_in, kind, amount)
+        if limit is not None:
+            limit = np.ascontiguousarray(limit, dtype=np.float64).reshape(-1)
+            if len(limit) != q:
+                raise ValueError(f"limit must have {q} entries, one per path")
+        tender, received, status = np.zeros(H), np.zeros(H), np.zeros(q, dtype=np.uint8)
+        u8, i32 = C.POINTER(C.c_uint8), C.POINTER(C.c_int)
+        self._chk(self._lib.cfmm_execute_paths(self._ctx, q, _ip(off), typ.ctypes.data_as(i32), _ip(pool), _ip(tok),
+                                               kind.ctypes.data_as(u8), _dp(amount),
+                                               None if limit is None else _dp(limit), _dp(tender), _dp(received),
+                                               status.ctypes.data_as(u8)))
+        return tender, received, status
+
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
         """cfmm_modify_univ3_liquidity: row j adds dL[j] (> 0 mints, < 0 burns) to the ticks of UniV3
@@ -626,6 +674,16 @@ class Router:
             self._pools.set_active(t, ks[0], active)
             self._retired[span] = ~active
 
+    def _locate(self):
+        """Per list position: the pool's type and its index in the type's insertion order."""
+        kind = np.full(len(self.cfmms), -1, dtype=np.int64)
+        local = np.zeros(len(self.cfmms), dtype=np.int64)
+        for t in (0, 1, 2):
+            lst = np.asarray(self._type_lists[t], dtype=np.int64)
+            kind[lst] = t
+            local[lst] = np.arange(len(lst))
+        return kind, local
+
     def _swap_rows(self, list_indices, tenders, what):
         """Per pool type: (rows of the call, type-local pool indices) of the pools r.cfmms[i]."""
         if self._world > 1:
@@ -636,12 +694,7 @@ class Router:
             raise ValueError(f"{what}: tenders must have shape ({len(ids)}, 2)")
         if len(ids) and (ids.min() < 0 or ids.max() >= len(self.cfmms)):
             raise IndexError(f"{what}: pool index out of range")
-        kind = np.full(len(self.cfmms), -1, dtype=np.int64)
-        local = np.zeros(len(self.cfmms), dtype=np.int64)
-        for t in (0, 1, 2):
-            lst = np.asarray(self._type_lists[t], dtype=np.int64)
-            kind[lst] = t
-            local[lst] = np.arange(len(lst))
+        kind, local = self._locate()
         groups = []
         for t in (0, 1, 2):
             rows = np.flatnonzero(kind[ids] == t)
@@ -701,6 +754,57 @@ class Router:
                 t, loc, kinds[rows], amounts[rows], None if limits is None else limits[rows])
         self._refresh_swapped(groups)
         return paid, received, status
+
+    def _path_args(self, paths, token_in, kinds, amounts, what):
+        """The CSR form of cfmm_quote_paths of paths (lists of r.cfmms positions), and the per-type
+        groups of the hops' pools (for _refresh_swapped)."""
+        if self._world > 1:
+            raise NotImplementedError(f"{what} drives one GPU")
+        paths = [np.asarray(p, dtype=np.int64).reshape(-1) for p in paths]
+        q = len(paths)
+        token_in, kinds, amounts = (np.asarray(a).reshape(-1) for a in (token_in, kinds, amounts))
+        if not (len(token_in) == len(kinds) == len(amounts) == q):
+            raise ValueError(f"{what}: token_in, kinds and amounts need one entry per path ({q})")
+        off = np.zeros(q + 1, dtype=np.int64)
+        off[1:] = np.cumsum([len(p) for p in paths])
+        ids = np.concatenate(paths) if q else np.zeros(0, dtype=np.int64)
+        if len(ids) and (ids.min() < 0 or ids.max() >= len(self.cfmms)):
+            raise IndexError(f"{what}: pool index out of range")
+        kind, local = self._locate()
+        hop_type, hop_pool = kind[ids], local[ids]
+        groups = [(t, None, hop_pool[hop_type == t]) for t in (0, 1, 2) if np.any(hop_type == t)]
+        return off, hop_type, hop_pool, token_in, kinds, amounts, groups
+
+    def quote_paths(self, paths, token_in, kinds, amounts):
+        """Price multi-hop paths (cfmm_quote_paths): paths[j] lists r.cfmms positions, token_in[j]
+        (1-based, as Ai) is tendered to the first pool, and each pool's output goes to the next.  Kind
+        0 tenders amounts[j]; kind 1 wants amounts[j] out of the last pool.  Every path on the current
+        state on its own; no state changes.  Returns (paid [q], received [q], status [q], hop_tender
+        [H], hop_received [H]) with the hops flattened in path order.  Single GPU."""
+        off, ht, hp, tok, kinds, amounts, _ = self._path_args(paths, token_in, kinds, amounts, "quote_paths")
+        tender, received, status = self._pools.quote_paths(off, ht, hp, tok, kinds, amounts)
+        return self._path_result(off, tender, received, status)
+
+    def execute_paths(self, paths, token_in, kinds, amounts, limits=None):
+        """Execute multi-hop paths in order (cfmm_execute_paths), each with an optional limit (kind 0:
+        the minimum final output; kind 1: the maximum tender): a path whose limit fails reverts every
+        hop and later paths see the state without it.  Returns what quote_paths returns and refreshes
+        the touched pool objects from the device state, as execute_swaps does.  Single GPU."""
+        off, ht, hp, tok, kinds, amounts, groups = self._path_args(paths, token_in, kinds, amounts, "execute_paths")
+        if limits is not None:
+            limits = np.asarray(limits, dtype=np.float64).reshape(-1)
+            if len(limits) != len(off) - 1:
+                raise ValueError(f"execute_paths: limits must have {len(off) - 1} entries")
+        tender, received, status = self._pools.execute_paths(off, ht, hp, tok, kinds, amounts, limits)
+        self._refresh_swapped(groups)
+        return self._path_result(off, tender, received, status)
+
+    @staticmethod
+    def _path_result(off, tender, received, status):
+        q = len(off) - 1
+        paid = tender[off[:-1]] if q else np.zeros(0)
+        got = received[off[1:] - 1] if q else np.zeros(0)
+        return paid, got, status, tender, received
 
     def _refresh_swapped(self, groups):
         """The touched pool objects' R, or current_price / current_tick, from the device state."""

@@ -355,6 +355,62 @@ int cfmm_execute_swap_orders(cfmm_ctx *ctx, int type, int64_t q, const int64_t *
                              const double *limit /* [q] or NULL */, double *paid /* [2q] or NULL */,
                              double *received /* [2q] or NULL */, uint8_t *status /* [q] or NULL */);
 
+/* ---- multi-hop swap paths ----------------------------------------------------------------
+ * A path tenders token t₀ to its first pool, tenders what that pool pays out to the next, and so
+ * on; one limit covers the whole path, and a path whose limit fails reverts every hop.  Path j is
+ * the hops hop_off[j] .. hop_off[j+1]) (hop_off [q+1], hop_off[0] = 0, 1..CFMM_PATH_MAX_HOPS hops
+ * per path; H = hop_off[q]).  Hop h is pool hop_pool[h] of type hop_type[h], addressed as
+ * cfmm_quote_swaps addresses a pool (the type's insertion order, appended pools included).  The
+ * pools of one path are distinct, so its hops never see each other.
+ *
+ * Tokens.  t₀ = token_in[j] (1-based).  Hop h's pool must hold t_{h−1}, and t_h is its other token.
+ * The hop tenders token 1 of the pool's ingest order (Ai as given to cfmm_add_* / cfmm_append_*)
+ * when t_{h−1} is that token, token 2 otherwise.
+ *
+ * f_h(x) is the exact-input quote of hop h's pool at its state before the path: what
+ * cfmm_quote_swaps returns for that tender, bit for bit (f_h(0) = 0).
+ *   Exact-in (kind CFMM_SWAP_EXACT_IN).  x₁ = amount; λ_h = f_h(x_h); x_{h+1} = λ_h if λ_h > 0,
+ *     else 0 (a ProductTwoCoin output can be a few ulp below zero, see the swaps section: it is
+ *     passed on as 0, the reported λ_h keeps its value).  The limit is the minimum λ_n (NULL: 0).
+ *   Exact-out (kind CFMM_SWAP_EXACT_OUT).  y_n = amount; for h = n … 1, x_h is the crossing of f_h
+ *     through y_h found by the search of cfmm_quote_swaps_exact_out, bit for bit (0 for y_h = 0), and
+ *     y_{h−1} = x_h.  λ_h = f_h(x_h) >= y_h: the surplus λ_h − x_{h+1} >= 0 stays with the trader.
+ *     The limit is the maximum x₁ (NULL or +inf: none).
+ * Status (CFMM_ORDER_*), first match: RETIRED when a hop's pool is retired; UNREACHABLE when some
+ * x_h = +inf; LIMIT (execute only) when λ_n < limit (exact-in) or x₁ > limit (exact-out), so an
+ * equal limit fills; otherwise FILLED.  A path that does not fill reports 0 as every hop's tender
+ * and received.  Per hop, hop_tender [H] = x_h (gross, in the tendered token) and hop_received
+ * [H] = λ_h; the path paid hop_tender[hop_off[j]] and received hop_received[hop_off[j+1] − 1].
+ *
+ * cfmm_quote_paths prices every path on the current state on its own; no state changes.
+ * cfmm_execute_paths runs the paths in batch order: path j is priced on the state every earlier
+ * filled path left, and a filled path runs the transition of cfmm_execute_swaps on each hop with
+ * tender x_h.  So the final state and every hop amount are bit-identical to running, path by path,
+ * each hop of each filled path as a one-row cfmm_execute_swaps call with that tender.  A reverted
+ * path changes nothing.  Afterwards every set a filled path touched gets the bookkeeping of
+ * cfmm_execute_swaps (state version, guard-free range flag, fixed-point scale, UniV3 tick records);
+ * the materialised trades stay.  Paths that share no pool run in parallel: path j's level is 1 +
+ * the largest level of an earlier path sharing one of its pools, and each level is one launch.
+ *
+ * Both are synchronous.  Before cfmm_finalize: CFMM_ERR_STATE.  q == 0 does nothing.
+ * CFMM_ERR_INVALID, before anything changes, for: q < 0 or a null array; hop_off not starting at 0,
+ * decreasing, or a path of 0 or more than CFMM_PATH_MAX_HOPS hops; a bad type or a pool outside the
+ * type's pools; the same pool twice in one path; token_in outside 1..n_tokens; a hop whose pool
+ * does not hold the token that reaches it (the message names the first such path and hop); a kind
+ * other than 0 or 1; an amount that is NaN, Inf or negative; a limit that is NaN or negative, or
+ * +inf on an exact-in path. */
+#define CFMM_PATH_MAX_HOPS 8
+int cfmm_quote_paths(cfmm_ctx *ctx, int64_t q, const int64_t *hop_off /* [q+1] */,
+                     const int *hop_type /* [H] */, const int64_t *hop_pool /* [H] */,
+                     const int64_t *token_in /* [q], 1-based */, const uint8_t *kind /* [q] */,
+                     const double *amount /* [q] */, double *hop_tender /* [H] */,
+                     double *hop_received /* [H] */, uint8_t *status /* [q] */);
+int cfmm_execute_paths(cfmm_ctx *ctx, int64_t q, const int64_t *hop_off, const int *hop_type,
+                       const int64_t *hop_pool, const int64_t *token_in, const uint8_t *kind,
+                       const double *amount, const double *limit /* [q] or NULL */,
+                       double *hop_tender /* [H] or NULL */, double *hop_received /* [H] or NULL */,
+                       uint8_t *status /* [q] or NULL */);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
@@ -500,7 +556,8 @@ int64_t cfmm_launch_count(const cfmm_ctx *ctx);
  * around each sweep kernel / the peer exchange).  cfmm_profile_read sums the
  * durations recorded so far for one pool type (cfmm_pool_type, 3 = the multi-GPU
  * exchange kernel, or 4 = the kernels of cfmm_quote_swaps / cfmm_execute_swaps /
- * cfmm_quote_swaps_exact_out / cfmm_execute_swap_orders); it
+ * cfmm_quote_swaps_exact_out / cfmm_execute_swap_orders / cfmm_quote_paths /
+ * cfmm_execute_paths); it
  * synchronises on the recorded events.
  * cfmm_profile_reset re-arms the same N pairs. */
 int cfmm_profile_read(cfmm_ctx *ctx, int type, double *total_ms, int64_t *launches);
