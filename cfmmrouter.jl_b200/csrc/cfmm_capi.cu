@@ -130,6 +130,10 @@ struct PoolSet {
   int64_t n_recs = 0;
   cfmm::BucketTable rec_buckets;
   DevBuf<int> d_chunk_rec;
+  // ... which take the 18-byte pool record when every record's lanes, lane offsets and fees fit its
+  // fields (else the set runs the 96-pool records), with the records' 64-byte headers
+  bool rec18_ok = false;
+  DevBuf<unsigned> d_rec_hdr;
   int range_pools = 0;         // pools per unit of the range table (96-pool chunks or 192-pool records)
   DevBuf<double> d_inv_scale, d_tok_sum;
   bool fixed_ok = false;       // every token fits the fixed-point rules (range, totals)
@@ -162,7 +166,7 @@ struct PoolSet {
     d_Ai.release(); d_tick.release(); d_gidx.release();
     d_lower.release(); d_liq.release();
     d_packed.release(); d_inv_scale.release(); d_tok_sum.release(); d_gcode.release(); d_gtab.release();
-    d_chunk_rec.release();
+    d_chunk_rec.release(); d_rec_hdr.release();
     d_active.release(); d_park.release();
     if (h_dur) cudaFreeHost(h_dur);
     h_dur = nullptr;
@@ -485,6 +489,7 @@ int upload_set(cfmm_ctx* ctx, int type, PoolSet& s, bool tail) {
   }));
   clock.mark("gather + upload gamma, Ai, gidx");
   s.compact_ok = false;
+  s.rec18_ok = false;
   if (type == CFMM_POOL_PRODUCT && s.tma_ok) {
     // 192-pool records: consecutive chunks of a bucket in pairs
     std::vector<int> chunk_rec((size_t)s.n_chunks);
@@ -561,6 +566,52 @@ int upload_set(cfmm_ctx* ctx, int type, PoolSet& s, bool tail) {
       CU_TRY(ctx, s.d_gtab.upload(tab));
       CU_TRY(ctx, s.d_chunk_rec.upload(chunk_rec));
       s.compact_ok = true;
+      // the 192-pool record's 64-byte headers (product_tma.cuh, kTmaRec18PoolBytes): a_base, the
+      // record's γ codes (at most four among its real pools), the a of every lane's first pool
+      // relative to a_base (<= 255); and every lane's first tokens must span at most 7
+      constexpr int kHdrWords = cfmm::kTmaRec18HeaderBytes / 4;
+      std::vector<unsigned> hdr((size_t)s.n_recs * kHdrWords, 0u);
+      int rec18_bad = 0;
+#pragma omp parallel for schedule(static) reduction(| : rec18_bad) if (s.n_chunks > (1 << 12))
+      for (int64_t c = 0; c < s.n_chunks; ++c) {
+        const int v = chunk_rec[(size_t)c];
+        if (v & 2) continue;  // second chunk of a record
+        unsigned* h = hdr.data() + (size_t)(v >> 2) * kHdrWords;
+        // logical pool q of the record: device position c·96 + q; the second half of a record
+        // without a second chunk repeats the first half's last a (pack_chunks_compact_kernel)
+        auto a_at = [&](int q) {
+          const int64_t i = real_before(c * cfmm::kTmaChunk + ((v & 1) ? std::min(q, cfmm::kTmaChunk - 1) : q));
+          return i < 0 ? (int64_t)0 : (int64_t)oa[(size_t)i];
+        };
+        const int64_t a_base = a_at(0);
+        h[0] = (unsigned)a_base;
+        int n_fees = 0;
+        unsigned fees[cfmm::kRec18Fees] = {};
+        bool ok18 = true;
+        for (int l = 0; l < 32 && ok18; ++l) {
+          const int64_t a_lane = a_at(l * cfmm::kTmaL6);
+          ok18 = a_lane - a_base <= cfmm::kRec18MaxLaneOff &&
+                 a_at(l * cfmm::kTmaL6 + cfmm::kTmaL6 - 1) - a_lane < (1 << cfmm::kRec18ABits);
+          h[2 + l / 4] |= (unsigned)(a_lane - a_base) << (8 * (l % 4));
+          for (int j = 0; j < cfmm::kTmaL6 && ok18; ++j) {
+            const int q = l * cfmm::kTmaL6 + j;
+            if ((v & 1) && q >= cfmm::kTmaChunk) break;
+            const int64_t i = order[c * cfmm::kTmaChunk + q];
+            if (i < 0) continue;  // padding: fee slot 0, whatever its code
+            const unsigned code = (unsigned)slot_of(s.gamma[(size_t)i], false);
+            int k = 0;
+            while (k < n_fees && fees[k] != code) ++k;
+            if (k == n_fees) {
+              if (n_fees == cfmm::kRec18Fees) ok18 = false;
+              else fees[n_fees++] = code;
+            }
+          }
+        }
+        for (int k = 0; k < cfmm::kRec18Fees; ++k) h[1] |= fees[k < n_fees ? k : 0] << (8 * k);
+        rec18_bad |= ok18 ? 0 : 1;
+      }
+      s.rec18_ok = rec18_bad == 0;
+      if (s.rec18_ok) CU_TRY(ctx, s.d_rec_hdr.upload(hdr));
     }
     clock.mark("fee dictionary + codes");
   }
@@ -776,7 +827,7 @@ int ensure_packed(cfmm_ctx* ctx, PoolSet& s, bool econ, bool fixed, bool compact
   if (compact) {
     cfmm::pack_chunks_compact_kernel<L><<<(unsigned)((s.m_padded + threads - 1) / threads), threads, 0, st>>>(
         s.d_R.p, s.d_Ai.p, s.d_gcode.p, s.m_padded, s.nb, fixed ? s.d_inv_scale.p : nullptr, s.d_chunk_rec.p,
-        s.d_packed.p);
+        s.d_packed.p, s.d_rec_hdr.p);
     ctx->launches++;
     CU_TRY(ctx, cudaGetLastError());
     s.packed_mode = mode;
@@ -937,18 +988,27 @@ int launch_tma_cfg(cfmm_ctx* ctx, PoolSet& s, const double* d_v, double* d_psi, 
   return CFMM_OK;
 }
 
+// Pools per compact record a gradient-only ProductTwoCoin sweep of the main set s streams under the
+// current options: 192 (18-byte pool records), 96 (20-byte pool records), 0 (the 32-byte stream).
+int compact_record_of(const cfmm_ctx* ctx, const PoolSet& s) {
+  if (!(ctx->gradient_math != 0 && ctx->compact_stream && s.compact_ok && !ctx->exact)) return 0;
+  // 192-pool records halve the per-record work (wait, counter, re-arm) and combine Ψ[a] over
+  // the warp, but leave warps idle on small sets: taken when every resident warp gets several
+  constexpr int L6 = cfmm::kTmaL6;
+  const int64_t warps = (int64_t)ctx->sm_count * cfmm::tma_ctas_per_sm<0, L6>() * cfmm::tma_warps<0, L6>();
+  const bool rec192 = s.rec18_ok && (ctx->compact_record == 192 || (ctx->compact_record == 0 && s.n_recs >= 4 * warps));
+  return rec192 ? 192 : 96;
+}
+
 template <int POOL>
 int launch_tma(cfmm_ctx* ctx, PoolSet& s, const double* d_v, double* d_psi, cudaStream_t st) {
   const bool econ = ctx->gradient_math != 0;
   const bool fixed = ctx->psi_fixed_point && s.fixed_ok;
   if constexpr (POOL == 0) {
-    if (econ && ctx->compact_stream && s.compact_ok && !ctx->exact) {
-      // 192-pool records halve the per-record work (wait, counter, re-arm) and combine Ψ[a] over
-      // the warp, but leave warps idle on small sets: taken when every resident warp gets several
+    const int rec = compact_record_of(ctx, s);
+    if (rec != 0) {
       constexpr int L6 = cfmm::kTmaL6;
-      const int64_t warps = (int64_t)ctx->sm_count * cfmm::tma_ctas_per_sm<0, L6>() * cfmm::tma_warps<0, L6>();
-      const bool rec192 = ctx->compact_record == 192 || (ctx->compact_record == 0 && s.n_recs >= 4 * warps);
-      if (rec192) {
+      if (rec == 192) {
         if (!s.skewed && fixed) return launch_tma_cfg<0, true, false, true, true, L6>(ctx, s, d_v, d_psi, st);
         if (!s.skewed && !fixed) return launch_tma_cfg<0, true, false, false, true, L6>(ctx, s, d_v, d_psi, st);
         if (s.skewed && fixed) return launch_tma_cfg<0, true, true, true, true, L6>(ctx, s, d_v, d_psi, st);
@@ -3199,6 +3259,18 @@ int cfmm_compact(cfmm_ctx* ctx) {
   }
   membership_changed(ctx);
   return calibrate(ctx);
+}
+
+// Test hook: pools per compact record of the next gradient-only sweep of the main set (see
+// compact_record_of; ProductTwoCoin only, 0 for the other types).
+int cfmm_debug_compact_record(cfmm_ctx* ctx, int type, int64_t* pools_per_record) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if ((rc = check_type(ctx, type)) != CFMM_OK) return rc;
+  if (!pools_per_record) return fail(ctx, CFMM_ERR_INVALID, "null output");
+  const PoolSet& s = ctx->sets[type];
+  *pools_per_record = type == CFMM_POOL_PRODUCT && s.tma_ok && ctx->use_tma ? compact_record_of(ctx, s) : 0;
+  return CFMM_OK;
 }
 
 // Test hook: info[8] = {main-set pools, tail pools, main-set padded length, TMA layout built,

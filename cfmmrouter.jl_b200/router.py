@@ -461,6 +461,13 @@ class DevicePools:
         keys = ("main", "tail", "padded", "tma", "fixed_point", "compact_stream", "fast_range", "retired")
         return {k: int(x) for k, x in zip(keys, info)}
 
+    def compact_record(self, pool_type: int) -> int:
+        """Pools per compact record the next gradient-only sweep of the main set streams: 192
+        (18-byte pool records), 96 (20-byte pool records) or 0 (cfmm_debug_compact_record; read-only)."""
+        out = np.zeros(1, dtype=np.int64)
+        self._chk(self._lib.cfmm_debug_compact_record(self._ctx, int(pool_type), _ip(out)))
+        return int(out[0])
+
     # -- multi-GPU --------------------------------------------------------------
     def detach_group(self):
         self._chk(self._lib.cfmm_comm_detach(self._ctx))

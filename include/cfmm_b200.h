@@ -584,6 +584,11 @@ int cfmm_debug_product_layout(int64_t n_tokens, int64_t m, const int64_t *Ai, in
  * layout built, fixed-point psi slice allowed, compact stream allowed, every reserve in the
  * guard-free range, retired pools} of one pool type. */
 int cfmm_debug_pool_set_info(cfmm_ctx *ctx, int type, int64_t *info);
+/* Test hook: pools per compact record the next gradient-only sweep of the main set of
+ * `type` streams under the current options: 192 (18-byte pool records), 96 (20-byte
+ * pool records) or 0 (no compact stream: other pool types, exact or reference-order
+ * math, or a set that does not fit it). */
+int cfmm_debug_compact_record(cfmm_ctx *ctx, int type, int64_t *pools_per_record);
 /* Measurement hook (option "trace" = 1): per-CTA phase timestamps of the last TMA gradient
  * sweep, ns of %globaltimer: out[8 * grid] = {entry, price slice ready, own range done,
  * all chunks done, partials flushed, exit, grid barrier passed (fused exchange, else 0),

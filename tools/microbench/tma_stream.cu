@@ -5,7 +5,9 @@
 // dependent read of the stage per lane and record, so the loop costs next to nothing besides the
 // copies, the waits, the counter and the re-arm.  201.7 MB per pass (the headline set's 20-byte
 // stream); GB/s from CUDA events (median of the timed launches), with the GPU name, its power
-// limit and the median SM clock sampled while the timed launches ran.
+// limit and the median SM clock sampled while the timed launches ran.  Then the headline set's
+// record count (52,099 192-pool records) at 3872 B (201.7 MB, 20 B per pool) and at 3520 B
+// (183.4 MB, 18 B per pool), 2 x 10 warps, interleaved over several rounds.
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tma_stream tma_stream.cu -lnvidia-ml
 //        (-L/usr/local/cuda/lib64/stubs where the driver's libnvidia-ml is not on the link path)
 #include <cuda_runtime.h>
@@ -17,6 +19,8 @@
 #include <vector>
 
 constexpr size_t kStreamBytes = 201700000;  // 104,167 records x 1936 B
+constexpr int kHeadlineRecords = 52099;     // 192-pool records of the headline set
+constexpr size_t kBufBytes = (size_t)kHeadlineRecords * 3872 > kStreamBytes ? (size_t)kHeadlineRecords * 3872 : kStreamBytes;
 constexpr int kStages = 2;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -84,18 +88,19 @@ __global__ void __launch_bounds__(WARPS * 32, CTAS) stream(const unsigned char* 
 static nvmlDevice_t g_nvml;
 static bool g_have_nvml = false;
 
+// returns the median launch time in µs (0 when the shape does not fit); n_rec <= 0: kStreamBytes / REC
 template <int REC, int WARPS, int CTAS>
-void run(const unsigned char* d_src, unsigned* d_out, int sms, std::vector<unsigned>& clocks) {
+double run(const unsigned char* d_src, unsigned* d_out, int sms, std::vector<unsigned>& clocks, int n_rec = 0) {
   constexpr int smem = WARPS * kStages * REC;
   auto k = stream<REC, WARPS, CTAS>;
   cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   int occ = 0;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, WARPS * 32, smem);
-  const int n_rec = (int)(kStreamBytes / REC);
+  if (n_rec <= 0) n_rec = (int)(kStreamBytes / REC);
   const int grid = sms * CTAS;
   if (occ < CTAS) {
     printf("%5d B  %d x %2d warps: does not fit (%d CTAs/SM)\n", REC, CTAS, WARPS, occ);
-    return;
+    return 0.0;
   }
   constexpr int kLaunches = 200;
   std::vector<cudaEvent_t> ev(kLaunches + 1);
@@ -122,6 +127,7 @@ void run(const unsigned char* d_src, unsigned* d_out, int sms, std::vector<unsig
   printf("%5d B  %d x %2d warps  %7d records  %2d KB ring/SM  median %7.2f us  min %7.2f us  %7.1f GB/s (median)\n", REC,
          CTAS, WARPS, n_rec, CTAS * smem / 1024, med_us, min_us, bytes / (med_us * 1e3));
   for (auto& e : ev) cudaEventDestroy(e);
+  return med_us;
 }
 
 int main() {
@@ -137,9 +143,9 @@ int main() {
   printf("GPU %s, %d SMs, power limit %.0f W\n", prop.name, sms, power_mw / 1000.0);
   unsigned char* d_src;
   unsigned* d_out;
-  cudaMalloc(&d_src, kStreamBytes + 4096);
+  cudaMalloc(&d_src, kBufBytes + 4096);
   cudaMalloc(&d_out, 4);
-  cudaMemset(d_src, 1, kStreamBytes + 4096);
+  cudaMemset(d_src, 1, kBufBytes + 4096);
   std::vector<unsigned> clocks;
   run<1936, 14, 2>(d_src, d_out, sms, clocks);
   run<1936, 10, 2>(d_src, d_out, sms, clocks);
@@ -151,6 +157,19 @@ int main() {
   run<3872, 10, 2>(d_src, d_out, sms, clocks);
   run<3872, 24, 1>(d_src, d_out, sms, clocks);
   run<1936, 14, 2>(d_src, d_out, sms, clocks);  // the first shape again: drift check
+  // the headline record count at both 192-pool record sizes, alternated
+  constexpr int kRounds = 7;
+  double t20[kRounds], t18[kRounds];
+  for (int r = 0; r < kRounds; ++r) {
+    t20[r] = run<3872, 10, 2>(d_src, d_out, sms, clocks, kHeadlineRecords);
+    t18[r] = run<3520, 10, 2>(d_src, d_out, sms, clocks, kHeadlineRecords);
+  }
+  std::sort(t20, t20 + kRounds);
+  std::sort(t18, t18 + kRounds);
+  printf("headline records, %d rounds of medians: 3872 B %.2f..%.2f us (median %.2f), 3520 B %.2f..%.2f us (median %.2f), "
+         "%.1f %% less time\n",
+         kRounds, t20[0], t20[kRounds - 1], t20[kRounds / 2], t18[0], t18[kRounds - 1], t18[kRounds / 2],
+         100.0 * (1.0 - t18[kRounds / 2] / t20[kRounds / 2]));
   if (!clocks.empty()) {
     std::sort(clocks.begin(), clocks.end());
     printf("SM clock during the timed launches: median %u MHz (min %u, max %u, %zu samples)\n", clocks[clocks.size() / 2],
