@@ -86,6 +86,12 @@ SYMBOLS = {
                                    _dp, _dp, C.POINTER(C.c_uint8)]),
     "cfmm_execute_paths": (C.c_int, [_ctx, C.c_int64, _ip, C.POINTER(C.c_int), _ip, _ip, C.POINTER(C.c_uint8), _dp,
                                      _dp, _dp, _dp, C.POINTER(C.c_uint8)]),
+    "cfmm_pair_pools": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, C.c_int64, C.POINTER(C.c_int), _ip,
+                                  C.POINTER(C.c_uint8)]),
+    "cfmm_quote_split_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, _dp, _dp, _dp,
+                                          C.POINTER(C.c_uint8), _dp, _dp]),
+    "cfmm_execute_split_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, _dp, _dp, _dp,
+                                            _dp, C.POINTER(C.c_uint8), _dp, _dp]),
     "cfmm_modify_univ3_liquidity":(C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),

@@ -32,7 +32,10 @@
 #include "solver.cuh"
 #include "swap_kernels.cuh"
 #include "path_kernels.cuh"
+#include "split_kernels.cuh"
 #include "univ3_state.cuh"
+
+#include <cub/cub.cuh>
 
 namespace {
 
@@ -250,6 +253,14 @@ struct cfmm_ctx {
   // memory opt-in) acts on the current device only, and contexts of one process
   // may sit on different devices and be driven from different host threads.
   std::unordered_map<const void*, int> occupancy;
+  // the pair index of cfmm_pair_pools and the split orders (split_kernels.cuh): built on first use
+  // after cfmm_finalize, cfmm_append_* or cfmm_compact (which move pools); retiring or restoring a
+  // pool keeps it, activity is read when a row is priced
+  struct PairIndex {
+    bool built = false;
+    int64_t n_pairs = 0;
+    DevBuf<int64_t> keys, off, pool;  // distinct keys ascending; CSR [n_pairs + 1]; entries by key
+  } pairs;
   int64_t launches = 0;
   std::string err;
   cfmm::PeerExchange comm;
@@ -2265,6 +2276,7 @@ int read_back(cfmm_ctx* ctx, int type, PoolSet& src, PoolSet& dst) {
 // Lay out the staged pools of `next` where `live` was, retire again what was retired, and swap
 // the new set in (the old one is released).
 int install_set(cfmm_ctx* ctx, int type, PoolSet& live, PoolSet& next, bool tail) {
+  ctx->pairs.built = false;  // device positions change
   int rc = upload_set(ctx, type, next, tail);
   if (rc == CFMM_OK) rc = reapply_retired(ctx, type, next);
   if (rc != CFMM_OK) {
@@ -2998,6 +3010,345 @@ int cfmm_execute_paths(cfmm_ctx* ctx, int64_t q, const int64_t* hop_off, const i
       return rc;
   }
   return path_outputs(ctx, c, hop_tender, hop_received, status);
+}
+
+// ---- orders split across the pools of their token pair (split_kernels.cuh) --------------------
+namespace {
+
+// The pair index on the device: keys per pool in global insertion order (pair_key_kernel), a stable
+// radix sort, a run-length pass and the CSR offsets.  Kept until the pools move.
+int ensure_pair_index(cfmm_ctx* ctx) {
+  auto& ix = ctx->pairs;
+  if (ix.built) return CFMM_OK;
+  const int64_t n = ctx->n_pools, nt = ctx->n_tokens;
+  if (n > INT32_MAX) return fail(ctx, CFMM_ERR_INVALID, "pair index: more than 2^31 - 1 pools");
+  ix.keys.release();
+  ix.off.release();
+  ix.pool.release();
+  ix.n_pairs = 0;
+  if (n > 0) {
+    cudaStream_t st = ctx->stream;
+    DevBuf<int64_t> keys_in, ent_in, keys_sorted, run_len;
+    DevBuf<int> d_runs;
+    DevBuf<unsigned char> temp;
+    CU_TRY(ctx, keys_in.alloc((size_t)n));
+    CU_TRY(ctx, ent_in.alloc((size_t)n));
+    CU_TRY(ctx, keys_sorted.alloc((size_t)n));
+    CU_TRY(ctx, run_len.alloc((size_t)n + 1));
+    CU_TRY(ctx, d_runs.alloc(1));
+    CU_TRY(ctx, ix.pool.alloc((size_t)n));
+    CU_TRY(ctx, ix.keys.alloc((size_t)n));
+    CU_TRY(ctx, ix.off.alloc((size_t)n + 1));
+    int end_bit = 1;  // keys < n_tokens²
+    while (end_bit < 63 && (1ll << end_bit) < nt * nt) ++end_bit;
+    const int items = (int)n;
+    size_t b1 = 0, b2 = 0, b3 = 0;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(nullptr, b1, keys_in.p, keys_sorted.p, ent_in.p, ix.pool.p, items, 0,
+                                                end_bit, st));
+    CU_TRY(ctx, cub::DeviceRunLengthEncode::Encode(nullptr, b2, keys_sorted.p, ix.keys.p, run_len.p, d_runs.p, items, st));
+    CU_TRY(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b3, run_len.p, ix.off.p, items + 1, st));
+    CU_TRY(ctx, temp.alloc(std::max(b1, std::max(b2, b3))));
+    size_t bytes = temp.n;
+    {
+      ProfScope prof(ctx, kProfSwaps, st);
+      for (int k = 0; k < cfmm::kPathSets; ++k) {
+        PoolSet& s = path_set(ctx, k);
+        if (s.m == 0) continue;
+        cfmm::pair_key_kernel<<<(unsigned)((s.m_padded + 255) / 256), 256, 0, st>>>(s.d_Ai.p, s.d_gidx.p, s.m_padded, k,
+                                                                                   nt, keys_in.p, ent_in.p);
+        ctx->launches++;
+      }
+      CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(temp.p, bytes, keys_in.p, keys_sorted.p, ent_in.p, ix.pool.p, items, 0,
+                                                  end_bit, st));
+      CU_TRY(ctx, cudaMemsetAsync(run_len.p, 0, ((size_t)n + 1) * sizeof(int64_t), st));
+      bytes = temp.n;
+      CU_TRY(ctx, cub::DeviceRunLengthEncode::Encode(temp.p, bytes, keys_sorted.p, ix.keys.p, run_len.p, d_runs.p, items,
+                                                     st));
+      bytes = temp.n;
+      CU_TRY(ctx, cub::DeviceScan::ExclusiveSum(temp.p, bytes, run_len.p, ix.off.p, items + 1, st));
+      ctx->launches += 3;
+    }
+    CU_TRY(ctx, cudaGetLastError());
+    int runs = 0;
+    CU_TRY(ctx, cudaMemcpyAsync(&runs, d_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU_TRY(ctx, cudaStreamSynchronize(st));
+    ix.n_pairs = runs;
+  }
+  ix.built = true;
+  return CFMM_OK;
+}
+
+// Tokens of rows naming a pair: 1-based, in range, distinct.
+int check_pair_tokens(cfmm_ctx* ctx, int64_t q, const int64_t* a, const int64_t* b, const char* what) {
+  for (int64_t j = 0; j < q; ++j) {
+    if (a[j] < 1 || a[j] > ctx->n_tokens || b[j] < 1 || b[j] > ctx->n_tokens)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: tokens (%lld, %lld) outside 1..%lld", what, (long long)j,
+                  (long long)a[j], (long long)b[j], (long long)ctx->n_tokens);
+    if (a[j] == b[j])
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: the two tokens are both %lld", what, (long long)j,
+                  (long long)a[j]);
+  }
+  return CFMM_OK;
+}
+
+// The rows' pairs on the device (index into the pair index, -1 = none) and their pool counts on
+// the host; the tokens are uploaded to d_a / d_b.
+int pair_lookup(cfmm_ctx* ctx, int64_t q, const int64_t* a, const int64_t* b, DevBuf<int64_t>& d_a,
+                DevBuf<int64_t>& d_b, DevBuf<int64_t>& d_pair, std::vector<int64_t>& count) {
+  int rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  if ((rc = ensure_pair_index(ctx)) != CFMM_OK) return rc;
+  DevBuf<int64_t> d_count;
+  CU_TRY(ctx, d_a.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_a.p, a, (size_t)q * sizeof(int64_t)));
+  CU_TRY(ctx, d_b.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_b.p, b, (size_t)q * sizeof(int64_t)));
+  CU_TRY(ctx, d_pair.alloc((size_t)q));
+  CU_TRY(ctx, d_count.alloc((size_t)q));
+  {
+    ProfScope prof(ctx, kProfSwaps, ctx->stream);
+    cfmm::pair_lookup_kernel<<<(unsigned)((q + 255) / 256), 256, 0, ctx->stream>>>(
+        ctx->pairs.keys.p, ctx->pairs.n_pairs, ctx->pairs.off.p, d_a.p, d_b.p, q, ctx->n_tokens, d_pair.p, d_count.p);
+  }
+  ctx->launches++;
+  CU_TRY(ctx, cudaGetLastError());
+  count.resize((size_t)q);
+  CU_TRY(ctx, cudaMemcpyAsync(count.data(), d_count.p, (size_t)q * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return CFMM_OK;
+}
+
+// Every argument of cfmm_quote_split_orders / cfmm_execute_split_orders, before anything runs.
+int check_split(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const uint8_t* kind,
+                const double* amount, const double* limit, const char* what) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if (q < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: negative row count", what);
+  if (q == 0) return CFMM_OK;
+  if (!token_in || !token_out || !kind || !amount) return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
+  if ((rc = check_pair_tokens(ctx, q, token_in, token_out, what)) != CFMM_OK) return rc;
+  for (int64_t j = 0; j < q; ++j) {
+    if (kind[j] != CFMM_SWAP_EXACT_IN && kind[j] != CFMM_SWAP_EXACT_OUT)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: kind %d is neither exact-in (0) nor exact-out (1)", what,
+                  (long long)j, (int)kind[j]);
+    if (!std::isfinite(amount[j]) || amount[j] < 0.0)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: amount %g must be finite and >= 0", what, (long long)j,
+                  amount[j]);
+    if (!limit) continue;
+    if (std::isnan(limit[j]) || limit[j] < 0.0)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: limit %g must be >= 0", what, (long long)j, limit[j]);
+    if (std::isinf(limit[j]) && kind[j] == CFMM_SWAP_EXACT_IN)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: an exact-in row's minimum received must be finite", what,
+                  (long long)j);
+  }
+  return CFMM_OK;
+}
+
+// Execution order: the rows grouped by pair, batch order kept inside each pair; a row whose pair no
+// pool holds is a group of its own.  A counting sort on the pair when the batch is large against the
+// index, a stable comparison sort otherwise (group_by_pool's rule).
+void group_by_pair(const std::vector<int64_t>& pair, int64_t n_pairs, std::vector<int64_t>& off,
+                   std::vector<int64_t>& rows) {
+  const int64_t q = (int64_t)pair.size();
+  rows.resize((size_t)q);
+  if (q * 8 >= n_pairs) {
+    std::vector<int64_t> start((size_t)n_pairs + 2, 0);
+    for (int64_t j = 0; j < q; ++j) start[(size_t)(pair[(size_t)j] + 2)]++;
+    for (int64_t k = 0; k <= n_pairs; ++k) start[(size_t)k + 1] += start[(size_t)k];
+    for (int64_t j = 0; j < q; ++j) rows[(size_t)start[(size_t)(pair[(size_t)j] + 1)]++] = j;
+  } else {
+    for (int64_t j = 0; j < q; ++j) rows[(size_t)j] = j;
+    std::stable_sort(rows.begin(), rows.end(), [&](int64_t a, int64_t b) { return pair[(size_t)a] < pair[(size_t)b]; });
+  }
+  off.clear();
+  for (int64_t j = 0; j < q; ++j) {
+    const int64_t p = pair[(size_t)rows[(size_t)j]];
+    if (j == 0 || p < 0 || p != pair[(size_t)rows[(size_t)j - 1]]) off.push_back(j);
+  }
+  off.push_back(q);
+}
+
+int split_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                 const uint8_t* kind, const double* amount, const double* limit, double* paid, double* received,
+                 double* price, uint8_t* status, double* leg_delta, double* leg_lambda) {
+  int rc;
+  DevBuf<int64_t> d_in, d_out, d_pair;
+  std::vector<int64_t> count;
+  if ((rc = pair_lookup(ctx, q, token_in, token_out, d_in, d_out, d_pair, count)) != CFMM_OK) return rc;
+  std::vector<int64_t> leg_off((size_t)q + 1, 0);
+  for (int64_t j = 0; j < q; ++j) leg_off[(size_t)j + 1] = leg_off[(size_t)j] + count[(size_t)j];
+  const int64_t L = leg_off[(size_t)q];
+  const bool legs = (leg_delta || leg_lambda) && L > 0;
+  DevBuf<int64_t> d_leg_off;
+  DevBuf<uint8_t> d_kind, d_status;
+  DevBuf<double> d_amount, d_limit, d_paid, d_recv, d_price, d_ld, d_ll;
+  CU_TRY(ctx, d_leg_off.upload(leg_off));
+  CU_TRY(ctx, d_kind.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<uint8_t>::copy_in(d_kind.p, kind, (size_t)q));
+  CU_TRY(ctx, d_amount.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<double>::copy_in(d_amount.p, amount, (size_t)q * sizeof(double)));
+  if (limit) {
+    CU_TRY(ctx, d_limit.alloc((size_t)q));
+    CU_TRY(ctx, DevBuf<double>::copy_in(d_limit.p, limit, (size_t)q * sizeof(double)));
+  }
+  CU_TRY(ctx, d_paid.alloc((size_t)q));
+  CU_TRY(ctx, d_recv.alloc((size_t)q));
+  CU_TRY(ctx, d_price.alloc((size_t)q));
+  CU_TRY(ctx, d_status.alloc((size_t)q));
+  if (legs) {
+    CU_TRY(ctx, d_ld.alloc((size_t)(2 * L)));
+    CU_TRY(ctx, d_ll.alloc((size_t)(2 * L)));
+  }
+  cfmm::PathSets P{};
+  for (int k = 0; k < cfmm::kPathSets; ++k) {
+    PoolSet& s = path_set(ctx, k);
+    P.s[k] = swap_set(s);
+    P.Ai[k] = s.d_Ai.p;
+  }
+  // execute: out_of_range [6], touched [6]; per UniV3 set the moved list and its listed flags
+  DevBuf<int> d_flags;
+  DevBuf<unsigned long long> d_n_moved;
+  DevBuf<int64_t> d_moved[2];
+  DevBuf<uint8_t> d_listed[2];
+  cfmm::SplitMoved mv{};
+  if (exec) {
+    CU_TRY(ctx, d_flags.alloc(2 * cfmm::kPathSets));
+    CU_TRY(ctx, d_n_moved.alloc(2));
+    CU_TRY(ctx, cudaMemsetAsync(d_flags.p, 0, 2 * cfmm::kPathSets * sizeof(int), ctx->stream));
+    CU_TRY(ctx, cudaMemsetAsync(d_n_moved.p, 0, 2 * sizeof(unsigned long long), ctx->stream));
+    for (int u = 0; u < 2; ++u) {
+      const size_t m = (size_t)path_set(ctx, 2 * CFMM_POOL_UNIV3 + u).m_padded;
+      CU_TRY(ctx, d_moved[u].alloc(m));
+      CU_TRY(ctx, d_listed[u].alloc(m));
+      if (m) CU_TRY(ctx, cudaMemsetAsync(d_listed[u].p, 0, m, ctx->stream));
+      P.moved[u] = d_moved[u].p;
+      mv.flag[u] = d_listed[u].p;
+    }
+    P.out_of_range = d_flags.p;
+    P.touched = d_flags.p + cfmm::kPathSets;
+    P.n_moved = d_n_moved.p;
+  }
+  DevBuf<cfmm::PathSets> d_P;
+  CU_TRY(ctx, d_P.alloc(1));
+  CU_TRY(ctx, DevBuf<cfmm::PathSets>::copy_in(d_P.p, &P, sizeof(cfmm::PathSets)));
+  cfmm::SplitRows R{d_in.p,    d_out.p,  d_kind.p,  d_amount.p, d_limit.p, d_pair.p, d_leg_off.p,
+                    d_paid.p,  d_recv.p, d_price.p, d_status.p, d_ld.p,    d_ll.p};
+  const cfmm::PairIndexView ix{ctx->pairs.off.p, ctx->pairs.pool.p};
+  const int per_block = cfmm::kSplitThreads / 32;
+  if (!exec) {
+    ProfScope prof(ctx, kProfSwaps, ctx->stream);
+    cfmm::split_quote_kernel<<<(unsigned)((q + per_block - 1) / per_block), cfmm::kSplitThreads, 0, ctx->stream>>>(
+        d_P.p, ix, R, q);
+    ctx->launches++;
+    CU_TRY(ctx, cudaGetLastError());
+  } else {
+    ctx->state_version++;
+    std::vector<int64_t> pair((size_t)q), seg_off, seg_rows;
+    CU_TRY(ctx, cudaMemcpyAsync(pair.data(), d_pair.p, (size_t)q * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    group_by_pair(pair, ctx->pairs.n_pairs, seg_off, seg_rows);
+    const int64_t n_seg = (int64_t)seg_off.size() - 1;
+    DevBuf<int64_t> d_seg_off, d_seg_rows;
+    CU_TRY(ctx, d_seg_off.upload(seg_off));
+    CU_TRY(ctx, d_seg_rows.upload(seg_rows));
+    {
+      ProfScope prof(ctx, kProfSwaps, ctx->stream);
+      cfmm::split_execute_kernel<<<(unsigned)((n_seg + per_block - 1) / per_block), cfmm::kSplitThreads, 0,
+                                   ctx->stream>>>(d_P.p, ix, R, d_seg_off.p, d_seg_rows.p, n_seg, mv);
+    }
+    ctx->launches++;
+    CU_TRY(ctx, cudaGetLastError());
+    int touched[cfmm::kPathSets];
+    CU_TRY(ctx, cudaMemcpyAsync(touched, P.touched, sizeof(touched), cudaMemcpyDeviceToHost, ctx->stream));
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    for (int k = 0; k < cfmm::kPathSets; ++k) {
+      if (!touched[k]) continue;
+      const int t = k >> 1;
+      if ((rc = swap_bookkeeping(ctx, path_set(ctx, k), t, t == CFMM_POOL_UNIV3 ? d_moved[k & 1].p : nullptr,
+                                 d_n_moved.p + (k & 1), d_flags.p + k)) != CFMM_OK)
+        return rc;
+    }
+  }
+  const auto d2h = [&](void* dst, const void* src, size_t bytes) {
+    return dst ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream) : cudaSuccess;
+  };
+  CU_TRY(ctx, d2h(paid, d_paid.p, (size_t)q * sizeof(double)));
+  CU_TRY(ctx, d2h(received, d_recv.p, (size_t)q * sizeof(double)));
+  CU_TRY(ctx, d2h(price, d_price.p, (size_t)q * sizeof(double)));
+  CU_TRY(ctx, d2h(status, d_status.p, (size_t)q));
+  if (legs) {
+    CU_TRY(ctx, d2h(leg_delta, d_ld.p, (size_t)(2 * L) * sizeof(double)));
+    CU_TRY(ctx, d2h(leg_lambda, d_ll.p, (size_t)(2 * L) * sizeof(double)));
+  }
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return CFMM_OK;
+}
+
+}  // namespace
+
+int cfmm_pair_pools(cfmm_ctx* ctx, int64_t q, const int64_t* token_a, const int64_t* token_b, int64_t* count,
+                    int64_t cap, int* type_out, int64_t* pool_out, uint8_t* active_out) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if (q < 0) return fail(ctx, CFMM_ERR_INVALID, "pair_pools: negative row count");
+  if (q == 0) return CFMM_OK;
+  if (!token_a || !token_b || !count) return fail(ctx, CFMM_ERR_INVALID, "pair_pools: null array argument");
+  if ((rc = check_pair_tokens(ctx, q, token_a, token_b, "pair_pools")) != CFMM_OK) return rc;
+  DevBuf<int64_t> d_a, d_b, d_pair;
+  std::vector<int64_t> cnt;
+  if ((rc = pair_lookup(ctx, q, token_a, token_b, d_a, d_b, d_pair, cnt)) != CFMM_OK) return rc;
+  std::vector<int64_t> cum((size_t)q, 0);
+  int64_t total = 0;
+  for (int64_t j = 0; j < q; ++j) {
+    count[j] = cnt[(size_t)j];
+    cum[(size_t)j] = total;
+    total += cnt[(size_t)j];
+  }
+  if (total == 0 || total > cap || (!type_out && !pool_out && !active_out)) return CFMM_OK;
+  DevBuf<int64_t> d_cum, d_ent;
+  CU_TRY(ctx, d_cum.upload(cum));
+  CU_TRY(ctx, d_ent.alloc((size_t)total));
+  {
+    ProfScope prof(ctx, kProfSwaps, ctx->stream);
+    cfmm::pair_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(
+        ctx->pairs.off.p, ctx->pairs.pool.p, d_pair.p, d_cum.p, q, total, d_ent.p);
+  }
+  ctx->launches++;
+  CU_TRY(ctx, cudaGetLastError());
+  std::vector<int64_t> ent((size_t)total);
+  CU_TRY(ctx, cudaMemcpyAsync(ent.data(), d_ent.p, (size_t)total * sizeof(int64_t), cudaMemcpyDeviceToHost,
+                              ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  for (int64_t t = 0; t < total; ++t) {  // (set, device position) -> (type, index in the type's insertion order)
+    const int k = (int)(ent[(size_t)t] >> cfmm::kPairSetShift);
+    const int64_t p = ent[(size_t)t] & cfmm::kPairPosMask;
+    PoolSet& s = path_set(ctx, k);
+    const int64_t i = s.order[(size_t)p];
+    if (type_out) type_out[t] = k >> 1;
+    if (pool_out) pool_out[t] = i + ((k & 1) ? ctx->sets[k >> 1].m : 0);
+    if (active_out) active_out[t] = (s.retired.empty() || !s.retired[(size_t)i]) ? 1 : 0;
+  }
+  return CFMM_OK;
+}
+
+int cfmm_quote_split_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                            const uint8_t* kind, const double* amount, double* paid, double* received, double* price,
+                            uint8_t* status, double* leg_delta, double* leg_lambda) {
+  int rc = check_split(ctx, q, token_in, token_out, kind, amount, nullptr, "quote_split_orders");
+  if (rc != CFMM_OK || q == 0) return rc;
+  return split_orders(ctx, false, q, token_in, token_out, kind, amount, nullptr, paid, received, price, status,
+                      leg_delta, leg_lambda);
+}
+
+int cfmm_execute_split_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                              const uint8_t* kind, const double* amount, const double* limit, double* paid,
+                              double* received, double* price, uint8_t* status, double* leg_delta,
+                              double* leg_lambda) {
+  int rc = check_split(ctx, q, token_in, token_out, kind, amount, limit, "execute_split_orders");
+  if (rc != CFMM_OK || q == 0) return rc;
+  return split_orders(ctx, true, q, token_in, token_out, kind, amount, limit, paid, received, price, status,
+                      leg_delta, leg_lambda);
 }
 
 // ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------

@@ -290,10 +290,17 @@ __global__ void scatter_trades_kernel(const double2* __restrict__ D,
   outL[o] = swapped ? make_double2(l.y, l.x) : l;
 }
 
-// R <- (R + γ·Δ) − Λ from the materialised trades of the same device order
-// (the update the reference's tests use, test/cfmms.jl:10: R⁺ = R + γ*Δ - Λ);
-// *out_of_range is raised when a new reserve leaves the guard-free range.  active (device order,
-// 0 = retired; null = all active) skips retired pools.
+// R <- (R + γ·Δ) − Λ (the update the reference's tests use, test/cfmms.jl:10: R⁺ = R + γ*Δ - Λ)
+__device__ __forceinline__ double2 apply_trade(double2 r, double g, double2 d, double2 l) {
+  double2 n;
+  n.x = __dsub_rn(__dadd_rn(r.x, __dmul_rn(g, d.x)), l.x);
+  n.y = __dsub_rn(__dadd_rn(r.y, __dmul_rn(g, d.y)), l.y);
+  return n;
+}
+
+// apply_trade from the materialised trades of the same device order; *out_of_range is raised when
+// a new reserve leaves the guard-free range.  active (device order, 0 = retired; null = all active)
+// skips retired pools.
 __global__ void apply_trades_kernel(double2* __restrict__ R, const double* __restrict__ gam,
                                     const double2* __restrict__ D, const double2* __restrict__ L,
                                     const int64_t* __restrict__ gidx, int64_t m,
@@ -304,9 +311,7 @@ __global__ void apply_trades_kernel(double2* __restrict__ R, const double* __res
   if (active && !active[i]) return;  // retired pool: its zeroed reserves stay, its state is parked
   const double g = gam[i];
   const double2 r = R[i], d = D[i], l = L[i];
-  double2 n;
-  n.x = __dsub_rn(__dadd_rn(r.x, __dmul_rn(g, d.x)), l.x);
-  n.y = __dsub_rn(__dadd_rn(r.y, __dmul_rn(g, d.y)), l.y);
+  const double2 n = apply_trade(r, g, d, l);
   R[i] = n;
   if (!in_fast_range(n.x) || !in_fast_range(n.y)) atomicOr(out_of_range, 1);
 }

@@ -419,6 +419,54 @@ function execute_paths!(ctx, hop_off::Vector{Int64}, hop_type::Vector{Cint}, hop
     return tender, received, status
 end
 
+# Orders split across every pool of their token pair (cfmm_pair_pools / cfmm_quote_split_orders /
+# cfmm_execute_split_orders).  Tokens are 1-based.  pair_pools returns (count, type, pool, active),
+# pools 0-based insertion indices of their type, each row's pools after the previous row's.  The
+# split calls return (paid, received, price, status, leg_delta, leg_lambda); the legs are 2 x L
+# (column = one pool's (Δ, Λ) side), rows after one another in pair_pools order.  Like the rest of
+# this file, never executed.
+function pair_pools(ctx, token_a::Vector{Int64}, token_b::Vector{Int64})
+    q = length(token_a)
+    length(token_b) == q || throw(ArgumentError("token_a and token_b need one entry per row"))
+    count = zeros(Int64, q)
+    chk(ctx, ccall((:cfmm_pair_pools, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Int64, Ptr{Cint}, Ptr{Int64}, Ptr{UInt8}),
+        ctx, q, token_a, token_b, count, 0, C_NULL, C_NULL, C_NULL))
+    L = sum(count; init=0)
+    typ, pool, active = zeros(Cint, L), zeros(Int64, L), zeros(UInt8, L)
+    L > 0 && chk(ctx, ccall((:cfmm_pair_pools, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Int64, Ptr{Cint}, Ptr{Int64}, Ptr{UInt8}),
+        ctx, q, token_a, token_b, count, L, typ, pool, active))
+    return count, typ, pool, active
+end
+function _split_orders(fn, ctx, token_in, token_out, kind, amount, limit)
+    q = length(token_in)
+    length(token_out) == length(kind) == length(amount) == q ||
+        throw(ArgumentError("token_in / token_out / kind / amount need one entry per row"))
+    limit === nothing || length(limit) == q || throw(ArgumentError("limit must have q entries"))
+    L = sum(pair_pools(ctx, token_in, token_out)[1]; init=0)
+    paid, received, price, status = zeros(q), zeros(q), zeros(q), zeros(UInt8, q)
+    ld, ll = zeros(2, L), zeros(2, L)
+    if fn === :quote
+        chk(ctx, ccall((:cfmm_quote_split_orders, LIB), Cint,
+            (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+             Ptr{Float64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64}),
+            ctx, q, token_in, token_out, kind, amount, paid, received, price, status, ld, ll))
+    else
+        chk(ctx, ccall((:cfmm_execute_split_orders, LIB), Cint,
+            (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+             Ptr{Float64}, Ptr{Float64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64}),
+            ctx, q, token_in, token_out, kind, amount, limit === nothing ? C_NULL : limit, paid, received,
+            price, status, ld, ll))
+    end
+    return paid, received, price, status, ld, ll
+end
+quote_split_orders(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}, kind::Vector{UInt8},
+                   amount::Vector{Float64}) = _split_orders(:quote, ctx, token_in, token_out, kind, amount, nothing)
+execute_split_orders!(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}, kind::Vector{UInt8},
+                      amount::Vector{Float64}, limit::Union{Nothing,Vector{Float64}}=nothing) =
+    _split_orders(:execute, ctx, token_in, token_out, kind, amount, limit)
+
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
 # current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never

@@ -418,6 +418,70 @@ class DevicePools:
                                                status.ctypes.data_as(u8)))
         return tender, received, status
 
+    # -- orders split across the pools of their pair (include/cfmm_b200.h, cfmm_pair_pools /
+    #    cfmm_quote_split_orders / cfmm_execute_split_orders) ------------------------------------
+    def pair_pools(self, token_a, token_b):
+        """cfmm_pair_pools: the pools holding each unordered pair {token_a[j], token_b[j]} (1-based),
+        in global insertion order.  Returns (off [q + 1], type [L], index [L] in the type's insertion
+        order, active [L] bool); row j's pools are off[j] .. off[j + 1]."""
+        a = np.ascontiguousarray(token_a, dtype=np.int64).reshape(-1)
+        b = np.ascontiguousarray(token_b, dtype=np.int64).reshape(-1)
+        if len(a) != len(b):
+            raise ValueError("pair_pools: token_a and token_b need one entry per row")
+        count = np.zeros(len(a), dtype=np.int64)
+        self._chk(self._lib.cfmm_pair_pools(self._ctx, len(a), _ip(a), _ip(b), _ip(count), 0, None, None, None))
+        off = np.concatenate([[0], np.cumsum(count)]).astype(np.int64)
+        L = int(off[-1])
+        typ, idx, act = np.zeros(L, dtype=np.int32), np.zeros(L, dtype=np.int64), np.zeros(L, dtype=np.uint8)
+        if L:
+            self._chk(self._lib.cfmm_pair_pools(self._ctx, len(a), _ip(a), _ip(b), _ip(count), L,
+                                                typ.ctypes.data_as(C.POINTER(C.c_int)), _ip(idx),
+                                                act.ctypes.data_as(C.POINTER(C.c_uint8))))
+        return off, typ, idx, act.astype(bool)
+
+    def _split(self, execute, token_in, token_out, kind, amount, limit, legs):
+        tin = np.ascontiguousarray(token_in, dtype=np.int64).reshape(-1)
+        tout = np.ascontiguousarray(token_out, dtype=np.int64).reshape(-1)
+        kind = np.ascontiguousarray(kind, dtype=np.uint8).reshape(-1)
+        amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
+        q = len(tin)
+        if not (len(tout) == len(kind) == len(amount) == q):
+            raise ValueError("split orders: token_in, token_out, kind and amount need one entry per row")
+        if limit is not None:
+            limit = np.ascontiguousarray(limit, dtype=np.float64).reshape(-1)
+            if len(limit) != q:
+                raise ValueError(f"limit must have {q} entries, one per row")
+        paid, received, price = np.zeros(q), np.zeros(q), np.zeros(q)
+        status = np.zeros(q, dtype=np.uint8)
+        off = ld = ll = None
+        if legs:
+            off = self.pair_pools(tin, tout)[0] if q else np.zeros(1, dtype=np.int64)
+            ld, ll = np.zeros((int(off[-1]), 2)), np.zeros((int(off[-1]), 2))
+        u8 = C.POINTER(C.c_uint8)
+        args = [self._ctx, q, _ip(tin), _ip(tout), kind.ctypes.data_as(u8), _dp(amount)]
+        if execute:
+            args.append(None if limit is None else _dp(limit))
+        args += [_dp(paid), _dp(received), _dp(price), status.ctypes.data_as(u8),
+                 _dp(ld) if legs else None, _dp(ll) if legs else None]
+        fn = self._lib.cfmm_execute_split_orders if execute else self._lib.cfmm_quote_split_orders
+        self._chk(fn(*args))
+        out = (paid, received, price, status)
+        return out + ((off, ld, ll),) if legs else out
+
+    def quote_split_orders(self, token_in, token_out, kind, amount, legs: bool = False):
+        """cfmm_quote_split_orders: row j sells token_in[j] for token_out[j] (1-based) over every pool
+        of the pair, split where the pools' marginal prices meet; kind 0 tenders amount[j], kind 1
+        wants amount[j].  Every row on the current state on its own; no state changes.  Returns
+        (paid [q], received [q], price [q] = s*, status [q] uint8) and, with legs=True, also
+        (off [q + 1], leg_delta [L, 2], leg_lambda [L, 2]) in pair_pools order."""
+        return self._split(False, token_in, token_out, kind, amount, None, legs)
+
+    def execute_split_orders(self, token_in, token_out, kind, amount, limit=None, legs: bool = False):
+        """cfmm_execute_split_orders: the rows of quote_split_orders in batch order, each on the state
+        the earlier filled rows left, with optional limits (kind 0: minimum received; kind 1: maximum
+        paid); a row whose limit fails reverts.  Returns what quote_split_orders returns."""
+        return self._split(True, token_in, token_out, kind, amount, limit, legs)
+
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
         """cfmm_modify_univ3_liquidity: row j adds dL[j] (> 0 mints, < 0 burns) to the ticks of UniV3
@@ -812,6 +876,49 @@ class Router:
         paid = tender[off[:-1]] if q else np.zeros(0)
         got = received[off[1:] - 1] if q else np.zeros(0)
         return paid, got, status, tender, received
+
+    def pair_pools(self, a, b):
+        """The r.cfmms positions of the pools that hold the token pair {a, b} (1-based), in the
+        library's global insertion order, retired ones included (cfmm_pair_pools).  Single GPU."""
+        if self._world > 1:
+            raise NotImplementedError("pair_pools drives one GPU")
+        _, typ, idx, _ = self._pools.pair_pools([int(a)], [int(b)])
+        return np.array([self._type_lists[int(t)][int(i)] for t, i in zip(typ, idx)], dtype=np.int64)
+
+    def _split_args(self, token_in, token_out, kinds, amounts, limits, what):
+        if self._world > 1:
+            raise NotImplementedError(f"{what} drives one GPU")
+        tin, tout, kinds, amounts = (np.asarray(x).reshape(-1) for x in (token_in, token_out, kinds, amounts))
+        if not (len(tin) == len(tout) == len(kinds) == len(amounts)):
+            raise ValueError(f"{what}: token_in, token_out, kinds and amounts need one entry per row")
+        if limits is not None:
+            limits = np.asarray(limits, dtype=np.float64).reshape(-1)
+            if len(limits) != len(tin):
+                raise ValueError(f"{what}: limits must have {len(tin)} entries")
+        return tin, tout, kinds, amounts, limits
+
+    def quote_split_orders(self, token_in, token_out, kinds, amounts):
+        """Sell token_in[j] for token_out[j] (1-based) over every pool of the pair, split so that the
+        pools' marginal prices meet (cfmm_quote_split_orders): kind 0 tenders amounts[j], kind 1 wants
+        amounts[j] out.  Every row on the current state on its own; no state changes.  Returns
+        (paid [q], received [q], price [q], status [q]); price is s* = ν_in/ν_out.  Single GPU."""
+        tin, tout, kinds, amounts, _ = self._split_args(token_in, token_out, kinds, amounts, None,
+                                                        "quote_split_orders")
+        return self._pools.quote_split_orders(tin, tout, kinds, amounts)
+
+    def execute_split_orders(self, token_in, token_out, kinds, amounts, limits=None):
+        """Execute split orders in order (cfmm_execute_split_orders), each with an optional limit (kind
+        0: the minimum received; kind 1: the maximum paid): a row whose limit fails reverts and later
+        rows see the state without it.  Returns what quote_split_orders returns and refreshes the pool
+        objects of the filled rows' pairs from the device state, as execute_swaps does.  Single GPU."""
+        tin, tout, kinds, amounts, limits = self._split_args(token_in, token_out, kinds, amounts, limits,
+                                                             "execute_split_orders")
+        out = self._pools.execute_split_orders(tin, tout, kinds, amounts, limits)
+        filled = out[3] == _lib.ORDER_FILLED
+        if np.any(filled):
+            _, typ, idx, _ = self._pools.pair_pools(tin[filled], tout[filled])
+            self._refresh_swapped([(t, None, idx[typ == t]) for t in (0, 1, 2) if np.any(typ == t)])
+        return out
 
     def _refresh_swapped(self, groups):
         """The touched pool objects' R, or current_price / current_tick, from the device state."""

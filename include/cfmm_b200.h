@@ -411,6 +411,100 @@ int cfmm_execute_paths(cfmm_ctx *ctx, int64_t q, const int64_t *hop_off, const i
                        double *hop_tender /* [H] or NULL */, double *hop_received /* [H] or NULL */,
                        uint8_t *status /* [q] or NULL */);
 
+/* ---- the pools of a token pair -----------------------------------------------------------
+ * For each row, the pools that hold the unordered token pair {token_a[j], token_b[j]} (1-based,
+ * distinct): all three types, main sets and appended pools, in global insertion order (the
+ * cfmm_num_pools numbering).  count [q] is always written.  When cap >= Σ count, the rows' lists
+ * follow one another in row order: type_out [Σ count] (cfmm_pool_type), pool_out [Σ count] (the
+ * index in the type's insertion order, as cfmm_quote_swaps addresses a pool) and active_out
+ * [Σ count] (0 = retired); any of them may be NULL.  So a first call with cap = 0 sizes the
+ * outputs.  The index behind it is built on the device on the first call that needs it after
+ * cfmm_finalize, cfmm_append_* or cfmm_compact (a key min(a,b)·n_tokens + max(a,b) per pool, a
+ * stable radix sort, a run-length pass; lookups bisect the distinct keys) and kept; retiring or
+ * restoring a pool does not rebuild it.  Synchronous.  Before cfmm_finalize: CFMM_ERR_STATE;
+ * tokens outside 1..n_tokens or equal, q < 0 or a null token / count array: CFMM_ERR_INVALID. */
+int cfmm_pair_pools(cfmm_ctx *ctx, int64_t q, const int64_t *token_a /* [q] */,
+                    const int64_t *token_b /* [q] */, int64_t *count /* [q] */, int64_t cap,
+                    int *type_out, int64_t *pool_out, uint8_t *active_out);
+
+/* ---- orders split optimally across every pool of their token pair ------------------------
+ * A row sells token j = token_in[r] for token i = token_out[r] (1-based, distinct) over every pool
+ * that holds {i, j} (cfmm_pair_pools order).  This is route! with Swap(i, j, δ, 2) over those pools
+ * only (src/objectives.jl:92-146, src/router.jl:58-108): with ν_i = 1 its dual has one variable,
+ * s = ν_j/ν_i, and the optimal split is the pools' response at the s* where their net intake of j
+ * matches the order (dual decomposition, docs/src/method.md).
+ *
+ * Pool response at s.  ν[i] = 1.0, ν[j] = s.  Pool k's legs (Δ_k, Λ_k) are the materialising
+ * find_arb! at ν[Ai] (src/cfmms.jl:125-140 ProductTwoCoin, :180-196 GeometricMeanTwoCoin,
+ * :339-395 UniV3, the UniV3 walk from the pool's current price and ladder): what cfmm_sweep with
+ * materialize = 1 reads back through cfmm_get_trades, bit for bit.  Retired pools give (0, 0).
+ * Legs are in the pool's ingest token order (a ProductTwoCoin pool stored with its tokens exchanged
+ * is mapped back).
+ *
+ * Sums.  N(s) = Σ_k (Δ_j,k − Λ_j,k), the pools' net intake of j, non-increasing in s, and
+ * O(s) = Σ_k (Λ_i,k − Δ_i,k), their output of i; each term one IEEE subtraction.  k runs over the
+ * pair's pools in order, and the sum has one fixed shape: partial l (l = 0 … 31) adds the terms
+ * k ≡ l (mod 32) in increasing k, starting from +0.0; then for m = 16, 8, 4, 2, 1 every partial
+ * becomes p_l + p_(l xor m).  The result is p_0 (every p_l ends equal).  No atomics.
+ *
+ * Search, on o(s), the bit pattern of s > 0 read as an int64, over [o(DBL_MIN), o(DBL_MAX)].
+ * enough(s) is N(s) > δ (a NaN counts as true) for exact-in (kind CFMM_SWAP_EXACT_IN, amount δ
+ * tendered), O(s) >= y for exact-out (CFMM_SWAP_EXACT_OUT, amount y wanted); true at small s.
+ *   start   e = the largest no-trade boundary over the pair's active pools (NaNs ignored), the s
+ *           below which pool k starts to take j, each step one IEEE operation:
+ *             ProductTwoCoin        (γ·R_i)/R_j
+ *             GeometricMeanTwoCoin  ((γ·w_j)·R_i)/(w_i·R_j)
+ *             UniV3                 γ·q when its token 1 is j, γ/q when it is i (q: current price)
+ *           o_e = o(e) clamped to [o(DBL_MIN), o(DBL_MAX)] (o(DBL_MIN) when e is NaN or < DBL_MIN).
+ *   gallop  if enough(o_e): lo = o_e, then c = lo + 1, lo + 2, lo + 4, … capped at o(DBL_MAX),
+ *           lo = c while enough(c), until !enough(c) (hi = c); unreachable when lo = o(DBL_MAX).
+ *           Otherwise hi = o_e, then c = hi − 1, hi − 2, hi − 4, … capped at o(DBL_MIN), hi = c
+ *           while !enough(c), until enough(c) (lo = c); unreachable when hi = o(DBL_MIN).
+ *   bisect  mid = lo + (hi − lo)/2 replaces lo (enough) or hi (not) until hi = lo + 1.
+ *   result  s* = hi for exact-in (N(s*) <= δ), s* = lo for exact-out (O(s*) >= y).
+ * Every row costs at most 1 + 63 + 62 evaluations of the pair's pools in the search and one more at
+ * s*, which writes the legs: 127.  A row with amount 0 fills with zeros and runs no search (the
+ * split never hands out free arbitrage to an empty order).  A pair no active pool holds, and a
+ * gallop that reaches either end without a bracket (the pools cannot absorb δ, or cannot deliver
+ * y, e.g. a UniV3 pool whose last tick is empty), give CFMM_ORDER_UNREACHABLE.
+ *
+ * What a fill means.  paid = N(s*) of j, received = O(s*) of i, price = s* (0 for an unreachable
+ * row or amount 0), and each pool trades its legs at s*.  When the pair's pools disagree on the
+ * price by more than their fees, the optimal split also arbitrages between them, as route! would:
+ * some legs then pay out j or take in i, and the legs show it.
+ *
+ * cfmm_quote_split_orders prices every row on the current state on its own; no state changes.
+ * cfmm_execute_split_orders runs the rows in batch order, each priced on the state the earlier
+ * filled rows left.  limit (NULL: none) is the minimum received for exact-in and the maximum paid
+ * for exact-out; a row whose limit fails reverts with CFMM_ORDER_LIMIT (its price is still
+ * reported), and an equal limit fills.  A filled row applies to each of its pair's active pools the
+ * transition of cfmm_apply_trades at its ν: two-coin R <- (R + γΔ) − Λ; UniV3 the q′ rule there
+ * with p = ν[a]/ν[b] (current tick updated with it).  Rows of one pair run in order in one warp;
+ * pairs share no pool and run in parallel.  Afterwards the bookkeeping of cfmm_execute_swaps
+ * (state version, guard-free range flag, fixed-point scale, UniV3 tick records); the materialised
+ * trades stay.  Reverted and unreachable rows change nothing and pay and receive 0.
+ *
+ * Per row: paid, received, price [q], status [q] (CFMM_ORDER_*); legs (optional): leg_delta,
+ * leg_lambda [2L], L = the sum of the rows' pool counts (cfmm_pair_pools), row after row, each
+ * pool's (Δ, Λ) pool-major in the pair's order as cfmm_get_trades lays them out; 0 for a row that
+ * does not fill.  Every output may be NULL.
+ *
+ * Both are synchronous.  Before cfmm_finalize: CFMM_ERR_STATE.  q == 0 does nothing.
+ * CFMM_ERR_INVALID before anything changes for: q < 0 or a null input array; tokens outside
+ * 1..n_tokens or token_in == token_out; a kind other than 0 or 1; an amount that is NaN, Inf or
+ * negative; a limit that is NaN or negative, or +inf on an exact-in row. */
+int cfmm_quote_split_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [q] */,
+                            const int64_t *token_out /* [q] */, const uint8_t *kind /* [q] */,
+                            const double *amount /* [q] */, double *paid /* [q] */,
+                            double *received /* [q] */, double *price /* [q] */,
+                            uint8_t *status /* [q] */, double *leg_delta /* [2L] or NULL */,
+                            double *leg_lambda /* [2L] or NULL */);
+int cfmm_execute_split_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_in,
+                              const int64_t *token_out, const uint8_t *kind, const double *amount,
+                              const double *limit /* [q] or NULL */, double *paid, double *received,
+                              double *price, uint8_t *status, double *leg_delta,
+                              double *leg_lambda);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
@@ -557,7 +651,8 @@ int64_t cfmm_launch_count(const cfmm_ctx *ctx);
  * durations recorded so far for one pool type (cfmm_pool_type, 3 = the multi-GPU
  * exchange kernel, or 4 = the kernels of cfmm_quote_swaps / cfmm_execute_swaps /
  * cfmm_quote_swaps_exact_out / cfmm_execute_swap_orders / cfmm_quote_paths /
- * cfmm_execute_paths); it
+ * cfmm_execute_paths / cfmm_pair_pools / cfmm_quote_split_orders /
+ * cfmm_execute_split_orders, the pair-index build counted as one launch); it
  * synchronises on the recorded events.
  * cfmm_profile_reset re-arms the same N pairs. */
 int cfmm_profile_read(cfmm_ctx *ctx, int type, double *total_ms, int64_t *launches);
