@@ -33,6 +33,7 @@ ORDER_UNREACHABLE = 2
 ORDER_RETIRED = 3
 # cfmm_quote_paths / cfmm_execute_paths
 PATH_MAX_HOPS = 8
+ROUTE_MAX_HUBS = 7  # CFMM_ROUTE_MAX_HUBS
 
 COMM_HANDLE_BYTES = 128
 
@@ -92,6 +93,10 @@ SYMBOLS = {
                                           C.POINTER(C.c_uint8), _dp, _dp]),
     "cfmm_execute_split_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, _dp, _dp, _dp,
                                             _dp, C.POINTER(C.c_uint8), _dp, _dp]),
+    "cfmm_quote_routed_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, _ip, _ip, _dp, _dp,
+                                           _dp, C.POINTER(C.c_uint8), _dp, _dp, _dp, _dp]),
+    "cfmm_execute_routed_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, _dp, _ip, _ip, _dp,
+                                             _dp, _dp, C.POINTER(C.c_uint8), _dp, _dp, _dp, _dp]),
     "cfmm_modify_univ3_liquidity":(C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),

@@ -33,6 +33,7 @@
 #include "swap_kernels.cuh"
 #include "path_kernels.cuh"
 #include "split_kernels.cuh"
+#include "route_kernels.cuh"
 #include "univ3_state.cuh"
 
 #include <cub/cub.cuh>
@@ -3169,6 +3170,63 @@ void group_by_pair(const std::vector<int64_t>& pair, int64_t n_pairs, std::vecto
   off.push_back(q);
 }
 
+// The pool sets the order kernels see (on the device), and on execute the flags they raise:
+// out_of_range [6], touched [6], and per UniV3 set the moved list and its listed flags.
+struct OrderSets {
+  cfmm::PathSets P{};
+  cfmm::SplitMoved mv{};
+  DevBuf<int> flags;
+  DevBuf<unsigned long long> n_moved;
+  DevBuf<int64_t> moved[2];
+  DevBuf<uint8_t> listed[2];
+  DevBuf<cfmm::PathSets> d_P;
+};
+
+int order_sets(cfmm_ctx* ctx, bool exec, OrderSets& os) {
+  cfmm::PathSets& P = os.P;
+  for (int k = 0; k < cfmm::kPathSets; ++k) {
+    PoolSet& s = path_set(ctx, k);
+    P.s[k] = swap_set(s);
+    P.Ai[k] = s.d_Ai.p;
+  }
+  if (exec) {
+    CU_TRY(ctx, os.flags.alloc(2 * cfmm::kPathSets));
+    CU_TRY(ctx, os.n_moved.alloc(2));
+    CU_TRY(ctx, cudaMemsetAsync(os.flags.p, 0, 2 * cfmm::kPathSets * sizeof(int), ctx->stream));
+    CU_TRY(ctx, cudaMemsetAsync(os.n_moved.p, 0, 2 * sizeof(unsigned long long), ctx->stream));
+    for (int u = 0; u < 2; ++u) {
+      const size_t m = (size_t)path_set(ctx, 2 * CFMM_POOL_UNIV3 + u).m_padded;
+      CU_TRY(ctx, os.moved[u].alloc(m));
+      CU_TRY(ctx, os.listed[u].alloc(m));
+      if (m) CU_TRY(ctx, cudaMemsetAsync(os.listed[u].p, 0, m, ctx->stream));
+      P.moved[u] = os.moved[u].p;
+      os.mv.flag[u] = os.listed[u].p;
+    }
+    P.out_of_range = os.flags.p;
+    P.touched = os.flags.p + cfmm::kPathSets;
+    P.n_moved = os.n_moved.p;
+  }
+  CU_TRY(ctx, os.d_P.alloc(1));
+  CU_TRY(ctx, DevBuf<cfmm::PathSets>::copy_in(os.d_P.p, &P, sizeof(cfmm::PathSets)));
+  return CFMM_OK;
+}
+
+// After an execute: the bookkeeping of cfmm_execute_swaps on every set a filled row touched.
+int order_bookkeeping(cfmm_ctx* ctx, OrderSets& os) {
+  int rc;
+  int touched[cfmm::kPathSets];
+  CU_TRY(ctx, cudaMemcpyAsync(touched, os.P.touched, sizeof(touched), cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  for (int k = 0; k < cfmm::kPathSets; ++k) {
+    if (!touched[k]) continue;
+    const int t = k >> 1;
+    if ((rc = swap_bookkeeping(ctx, path_set(ctx, k), t, t == CFMM_POOL_UNIV3 ? os.moved[k & 1].p : nullptr,
+                               os.n_moved.p + (k & 1), os.flags.p + k)) != CFMM_OK)
+      return rc;
+  }
+  return CFMM_OK;
+}
+
 int split_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, const int64_t* token_out,
                  const uint8_t* kind, const double* amount, const double* limit, double* paid, double* received,
                  double* price, uint8_t* status, double* leg_delta, double* leg_lambda) {
@@ -3200,38 +3258,8 @@ int split_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, c
     CU_TRY(ctx, d_ld.alloc((size_t)(2 * L)));
     CU_TRY(ctx, d_ll.alloc((size_t)(2 * L)));
   }
-  cfmm::PathSets P{};
-  for (int k = 0; k < cfmm::kPathSets; ++k) {
-    PoolSet& s = path_set(ctx, k);
-    P.s[k] = swap_set(s);
-    P.Ai[k] = s.d_Ai.p;
-  }
-  // execute: out_of_range [6], touched [6]; per UniV3 set the moved list and its listed flags
-  DevBuf<int> d_flags;
-  DevBuf<unsigned long long> d_n_moved;
-  DevBuf<int64_t> d_moved[2];
-  DevBuf<uint8_t> d_listed[2];
-  cfmm::SplitMoved mv{};
-  if (exec) {
-    CU_TRY(ctx, d_flags.alloc(2 * cfmm::kPathSets));
-    CU_TRY(ctx, d_n_moved.alloc(2));
-    CU_TRY(ctx, cudaMemsetAsync(d_flags.p, 0, 2 * cfmm::kPathSets * sizeof(int), ctx->stream));
-    CU_TRY(ctx, cudaMemsetAsync(d_n_moved.p, 0, 2 * sizeof(unsigned long long), ctx->stream));
-    for (int u = 0; u < 2; ++u) {
-      const size_t m = (size_t)path_set(ctx, 2 * CFMM_POOL_UNIV3 + u).m_padded;
-      CU_TRY(ctx, d_moved[u].alloc(m));
-      CU_TRY(ctx, d_listed[u].alloc(m));
-      if (m) CU_TRY(ctx, cudaMemsetAsync(d_listed[u].p, 0, m, ctx->stream));
-      P.moved[u] = d_moved[u].p;
-      mv.flag[u] = d_listed[u].p;
-    }
-    P.out_of_range = d_flags.p;
-    P.touched = d_flags.p + cfmm::kPathSets;
-    P.n_moved = d_n_moved.p;
-  }
-  DevBuf<cfmm::PathSets> d_P;
-  CU_TRY(ctx, d_P.alloc(1));
-  CU_TRY(ctx, DevBuf<cfmm::PathSets>::copy_in(d_P.p, &P, sizeof(cfmm::PathSets)));
+  OrderSets os;
+  if ((rc = order_sets(ctx, exec, os)) != CFMM_OK) return rc;
   cfmm::SplitRows R{d_in.p,    d_out.p,  d_kind.p,  d_amount.p, d_limit.p, d_pair.p, d_leg_off.p,
                     d_paid.p,  d_recv.p, d_price.p, d_status.p, d_ld.p,    d_ll.p};
   const cfmm::PairIndexView ix{ctx->pairs.off.p, ctx->pairs.pool.p};
@@ -3239,7 +3267,7 @@ int split_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, c
   if (!exec) {
     ProfScope prof(ctx, kProfSwaps, ctx->stream);
     cfmm::split_quote_kernel<<<(unsigned)((q + per_block - 1) / per_block), cfmm::kSplitThreads, 0, ctx->stream>>>(
-        d_P.p, ix, R, q);
+        os.d_P.p, ix, R, q);
     ctx->launches++;
     CU_TRY(ctx, cudaGetLastError());
   } else {
@@ -3255,20 +3283,11 @@ int split_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, c
     {
       ProfScope prof(ctx, kProfSwaps, ctx->stream);
       cfmm::split_execute_kernel<<<(unsigned)((n_seg + per_block - 1) / per_block), cfmm::kSplitThreads, 0,
-                                   ctx->stream>>>(d_P.p, ix, R, d_seg_off.p, d_seg_rows.p, n_seg, mv);
+                                   ctx->stream>>>(os.d_P.p, ix, R, d_seg_off.p, d_seg_rows.p, n_seg, os.mv);
     }
     ctx->launches++;
     CU_TRY(ctx, cudaGetLastError());
-    int touched[cfmm::kPathSets];
-    CU_TRY(ctx, cudaMemcpyAsync(touched, P.touched, sizeof(touched), cudaMemcpyDeviceToHost, ctx->stream));
-    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    for (int k = 0; k < cfmm::kPathSets; ++k) {
-      if (!touched[k]) continue;
-      const int t = k >> 1;
-      if ((rc = swap_bookkeeping(ctx, path_set(ctx, k), t, t == CFMM_POOL_UNIV3 ? d_moved[k & 1].p : nullptr,
-                                 d_n_moved.p + (k & 1), d_flags.p + k)) != CFMM_OK)
-        return rc;
-    }
+    if ((rc = order_bookkeeping(ctx, os)) != CFMM_OK) return rc;
   }
   const auto d2h = [&](void* dst, const void* src, size_t bytes) {
     return dst ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream) : cudaSuccess;
@@ -3277,6 +3296,174 @@ int split_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, c
   CU_TRY(ctx, d2h(received, d_recv.p, (size_t)q * sizeof(double)));
   CU_TRY(ctx, d2h(price, d_price.p, (size_t)q * sizeof(double)));
   CU_TRY(ctx, d2h(status, d_status.p, (size_t)q));
+  if (legs) {
+    CU_TRY(ctx, d2h(leg_delta, d_ld.p, (size_t)(2 * L) * sizeof(double)));
+    CU_TRY(ctx, d2h(leg_lambda, d_ll.p, (size_t)(2 * L) * sizeof(double)));
+  }
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return CFMM_OK;
+}
+
+// ---- orders routed over their pair and two-hop routes through hubs (route_kernels.cuh) ----------
+
+// Every argument of cfmm_quote_routed_orders / cfmm_execute_routed_orders, before anything runs.
+int check_routed(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const uint8_t* kind,
+                 const double* amount, const double* limit, const int64_t* hub_off, const int64_t* hubs,
+                 const char* what) {
+  int rc = check_split(ctx, q, token_in, token_out, kind, amount, limit, what);
+  if (rc != CFMM_OK || q == 0) return rc;
+  if (!hub_off) return fail(ctx, CFMM_ERR_INVALID, "%s: null hub_off", what);
+  if (hub_off[0] != 0) return fail(ctx, CFMM_ERR_INVALID, "%s: hub_off[0] = %lld, not 0", what, (long long)hub_off[0]);
+  for (int64_t r = 0; r < q; ++r) {
+    const int64_t c = hub_off[r + 1] - hub_off[r];
+    if (c < 0 || c > CFMM_ROUTE_MAX_HUBS)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: %lld hubs, not 0..%d", what, (long long)r, (long long)c,
+                  CFMM_ROUTE_MAX_HUBS);
+  }
+  if (hub_off[q] > 0 && !hubs) return fail(ctx, CFMM_ERR_INVALID, "%s: null hubs", what);
+  for (int64_t r = 0; r < q; ++r) {
+    for (int64_t g = hub_off[r]; g < hub_off[r + 1]; ++g) {
+      const int64_t h = hubs[g];
+      if (h < 1 || h > ctx->n_tokens)
+        return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: hub %lld outside 1..%lld", what, (long long)r, (long long)h,
+                    (long long)ctx->n_tokens);
+      if (h == token_in[r] || h == token_out[r])
+        return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: hub %lld is one of the row's tokens", what, (long long)r,
+                    (long long)h);
+      for (int64_t f = hub_off[r]; f < g; ++f)
+        if (hubs[f] == h)
+          return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: hub %lld listed twice", what, (long long)r, (long long)h);
+    }
+  }
+  return CFMM_OK;
+}
+
+int routed_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                  const uint8_t* kind, const double* amount, const double* limit, const int64_t* hub_off,
+                  const int64_t* hubs, double* paid, double* received, double* price, uint8_t* status,
+                  double* hub_price, double* hub_surplus, double* leg_delta, double* leg_lambda) {
+  int rc;
+  const int64_t nh = hub_off[q];
+  // the rows' pair lists: (j, i), then (j, h), (h, i) per hub; row r's start at r + 2·hub_off[r]
+  const int64_t n_lists = q + 2 * nh;
+  std::vector<int64_t> la((size_t)n_lists), lb((size_t)n_lists);
+  int max_hubs = 0;
+  for (int64_t r = 0; r < q; ++r) {
+    const int64_t base = r + 2 * hub_off[r];
+    la[(size_t)base] = token_in[r];
+    lb[(size_t)base] = token_out[r];
+    for (int64_t g = hub_off[r]; g < hub_off[r + 1]; ++g) {
+      const int64_t x = base + 1 + 2 * (g - hub_off[r]);
+      la[(size_t)x] = token_in[r];
+      lb[(size_t)x] = hubs[g];
+      la[(size_t)x + 1] = hubs[g];
+      lb[(size_t)x + 1] = token_out[r];
+    }
+    max_hubs = std::max(max_hubs, (int)(hub_off[r + 1] - hub_off[r]));
+  }
+  DevBuf<int64_t> d_a, d_b, d_pair;
+  std::vector<int64_t> count;
+  if ((rc = pair_lookup(ctx, n_lists, la.data(), lb.data(), d_a, d_b, d_pair, count)) != CFMM_OK) return rc;
+  std::vector<int64_t> leg_off((size_t)n_lists + 1, 0);
+  for (int64_t j = 0; j < n_lists; ++j) leg_off[(size_t)j + 1] = leg_off[(size_t)j] + count[(size_t)j];
+  const int64_t L = leg_off[(size_t)n_lists];
+  const bool legs = (leg_delta || leg_lambda) && L > 0;
+  DevBuf<int64_t> d_in, d_out, d_leg_off, d_hub_off, d_hubs;
+  DevBuf<uint8_t> d_kind, d_status;
+  DevBuf<double> d_amount, d_limit, d_paid, d_recv, d_price, d_hp, d_hs, d_ld, d_ll;
+  CU_TRY(ctx, d_in.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_in.p, token_in, (size_t)q * sizeof(int64_t)));
+  CU_TRY(ctx, d_out.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_out.p, token_out, (size_t)q * sizeof(int64_t)));
+  CU_TRY(ctx, d_hub_off.alloc((size_t)q + 1));
+  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_hub_off.p, hub_off, ((size_t)q + 1) * sizeof(int64_t)));
+  if (nh > 0) {
+    CU_TRY(ctx, d_hubs.alloc((size_t)nh));
+    CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_hubs.p, hubs, (size_t)nh * sizeof(int64_t)));
+  }
+  CU_TRY(ctx, d_leg_off.upload(leg_off));
+  CU_TRY(ctx, d_kind.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<uint8_t>::copy_in(d_kind.p, kind, (size_t)q));
+  CU_TRY(ctx, d_amount.alloc((size_t)q));
+  CU_TRY(ctx, DevBuf<double>::copy_in(d_amount.p, amount, (size_t)q * sizeof(double)));
+  if (limit) {
+    CU_TRY(ctx, d_limit.alloc((size_t)q));
+    CU_TRY(ctx, DevBuf<double>::copy_in(d_limit.p, limit, (size_t)q * sizeof(double)));
+  }
+  CU_TRY(ctx, d_paid.alloc((size_t)q));
+  CU_TRY(ctx, d_recv.alloc((size_t)q));
+  CU_TRY(ctx, d_price.alloc((size_t)q));
+  CU_TRY(ctx, d_status.alloc((size_t)q));
+  if (nh > 0) {
+    CU_TRY(ctx, d_hp.alloc((size_t)nh));
+    CU_TRY(ctx, d_hs.alloc((size_t)nh));
+  }
+  if (legs) {
+    CU_TRY(ctx, d_ld.alloc((size_t)(2 * L)));
+    CU_TRY(ctx, d_ll.alloc((size_t)(2 * L)));
+  }
+  OrderSets os;
+  if ((rc = order_sets(ctx, exec, os)) != CFMM_OK) return rc;
+  cfmm::RouteRows R{d_in.p,    d_out.p,   d_kind.p,  d_amount.p, d_limit.p, d_hub_off.p, d_hubs.p, d_pair.p, d_leg_off.p,
+                    d_paid.p,  d_recv.p,  d_price.p, d_status.p, d_hp.p,    d_hs.p,      d_ld.p,   d_ll.p};
+  const cfmm::PairIndexView ix{ctx->pairs.off.p, ctx->pairs.pool.p};
+  const unsigned threads = 32u * (1u + (unsigned)max_hubs);  // warp 0: the direct pools, warp 1 + h: hub h
+  if (!exec) {
+    ProfScope prof(ctx, kProfSwaps, ctx->stream);
+    cfmm::route_quote_kernel<<<(unsigned)q, threads, 0, ctx->stream>>>(os.d_P.p, ix, R);
+    ctx->launches++;
+    CU_TRY(ctx, cudaGetLastError());
+  } else {
+    ctx->state_version++;
+    // levels: a row's level is 1 + the highest level of an earlier row sharing one of its pairs (a
+    // pool belongs to one pair); pairs no pool holds conflict with nothing
+    std::vector<int64_t> pair((size_t)n_lists);
+    CU_TRY(ctx, cudaMemcpyAsync(pair.data(), d_pair.p, (size_t)n_lists * sizeof(int64_t), cudaMemcpyDeviceToHost,
+                                ctx->stream));
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    std::vector<int32_t> pair_level((size_t)ctx->pairs.n_pairs, 0);
+    std::vector<int32_t> level((size_t)q);
+    int32_t n_levels = 0;
+    for (int64_t r = 0; r < q; ++r) {
+      const int64_t b = r + 2 * hub_off[r], e = r + 1 + 2 * hub_off[r + 1];
+      int32_t lv = 0;
+      for (int64_t x = b; x < e; ++x)
+        if (pair[(size_t)x] >= 0) lv = std::max(lv, pair_level[(size_t)pair[(size_t)x]]);
+      ++lv;
+      for (int64_t x = b; x < e; ++x)
+        if (pair[(size_t)x] >= 0) pair_level[(size_t)pair[(size_t)x]] = lv;
+      level[(size_t)r] = lv;
+      n_levels = std::max(n_levels, lv);
+    }
+    std::vector<int64_t> start((size_t)n_levels + 2, 0), rows((size_t)q);  // rows by level, batch order kept
+    for (int64_t r = 0; r < q; ++r) start[(size_t)level[(size_t)r] + 1]++;
+    for (int32_t l = 0; l <= n_levels; ++l) start[(size_t)l + 1] += start[(size_t)l];
+    std::vector<int64_t> fill(start);
+    for (int64_t r = 0; r < q; ++r) rows[(size_t)fill[(size_t)level[(size_t)r]]++] = r;
+    DevBuf<int64_t> d_rows;
+    CU_TRY(ctx, d_rows.upload(rows));
+    for (int32_t l = 1; l <= n_levels; ++l) {
+      const int64_t n = start[(size_t)l + 1] - start[(size_t)l];
+      if (n == 0) continue;
+      {
+        ProfScope prof(ctx, kProfSwaps, ctx->stream);
+        cfmm::route_execute_kernel<<<(unsigned)n, threads, 0, ctx->stream>>>(os.d_P.p, ix, R,
+                                                                              d_rows.p + start[(size_t)l], os.mv);
+      }
+      ctx->launches++;
+      CU_TRY(ctx, cudaGetLastError());
+    }
+    if ((rc = order_bookkeeping(ctx, os)) != CFMM_OK) return rc;
+  }
+  const auto d2h = [&](void* dst, const void* src, size_t bytes) {
+    return dst && bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream) : cudaSuccess;
+  };
+  CU_TRY(ctx, d2h(paid, d_paid.p, (size_t)q * sizeof(double)));
+  CU_TRY(ctx, d2h(received, d_recv.p, (size_t)q * sizeof(double)));
+  CU_TRY(ctx, d2h(price, d_price.p, (size_t)q * sizeof(double)));
+  CU_TRY(ctx, d2h(status, d_status.p, (size_t)q));
+  CU_TRY(ctx, d2h(hub_price, d_hp.p, (size_t)nh * sizeof(double)));
+  CU_TRY(ctx, d2h(hub_surplus, d_hs.p, (size_t)nh * sizeof(double)));
   if (legs) {
     CU_TRY(ctx, d2h(leg_delta, d_ld.p, (size_t)(2 * L) * sizeof(double)));
     CU_TRY(ctx, d2h(leg_lambda, d_ll.p, (size_t)(2 * L) * sizeof(double)));
@@ -3349,6 +3536,26 @@ int cfmm_execute_split_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in,
   if (rc != CFMM_OK || q == 0) return rc;
   return split_orders(ctx, true, q, token_in, token_out, kind, amount, limit, paid, received, price, status,
                       leg_delta, leg_lambda);
+}
+
+int cfmm_quote_routed_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                             const uint8_t* kind, const double* amount, const int64_t* hub_off, const int64_t* hubs,
+                             double* paid, double* received, double* price, uint8_t* status, double* hub_price,
+                             double* hub_surplus, double* leg_delta, double* leg_lambda) {
+  int rc = check_routed(ctx, q, token_in, token_out, kind, amount, nullptr, hub_off, hubs, "quote_routed_orders");
+  if (rc != CFMM_OK || q == 0) return rc;
+  return routed_orders(ctx, false, q, token_in, token_out, kind, amount, nullptr, hub_off, hubs, paid, received, price,
+                       status, hub_price, hub_surplus, leg_delta, leg_lambda);
+}
+
+int cfmm_execute_routed_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                               const uint8_t* kind, const double* amount, const double* limit, const int64_t* hub_off,
+                               const int64_t* hubs, double* paid, double* received, double* price, uint8_t* status,
+                               double* hub_price, double* hub_surplus, double* leg_delta, double* leg_lambda) {
+  int rc = check_routed(ctx, q, token_in, token_out, kind, amount, limit, hub_off, hubs, "execute_routed_orders");
+  if (rc != CFMM_OK || q == 0) return rc;
+  return routed_orders(ctx, true, q, token_in, token_out, kind, amount, limit, hub_off, hubs, paid, received, price,
+                       status, hub_price, hub_surplus, leg_delta, leg_lambda);
 }
 
 // ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------

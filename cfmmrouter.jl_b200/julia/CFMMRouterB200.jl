@@ -467,6 +467,51 @@ execute_split_orders!(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}, ki
                       amount::Vector{Float64}, limit::Union{Nothing,Vector{Float64}}=nothing) =
     _split_orders(:execute, ctx, token_in, token_out, kind, amount, limit)
 
+# Orders routed over their pair and the two-hop routes through hub tokens (cfmm_quote_routed_orders /
+# cfmm_execute_routed_orders).  Row r's hubs are hubs[hub_off[r]+1 : hub_off[r+1]] (1-based tokens,
+# hub_off 0-based offsets, at most 7 per row).  Returns (paid, received, price, status, hub_price,
+# hub_surplus, leg_delta, leg_lambda); each row's legs are its pairs' pools in the order (j, i),
+# (j, h₁), (h₁, i), (j, h₂), …, in pair_pools order.  Never executed, like the rest of this file.
+function _routed_orders(fn, ctx, token_in, token_out, kind, amount, hub_off, hubs, limit)
+    q = length(token_in)
+    length(token_out) == length(kind) == length(amount) == q && length(hub_off) == q + 1 ||
+        throw(ArgumentError("token_in / token_out / kind / amount need q entries, hub_off q + 1"))
+    limit === nothing || length(limit) == q || throw(ArgumentError("limit must have q entries"))
+    a, b = Int64[], Int64[]
+    for r in 1:q
+        push!(a, token_in[r]); push!(b, token_out[r])
+        for h in hubs[hub_off[r]+1:hub_off[r+1]]
+            push!(a, token_in[r], h); push!(b, h, token_out[r])
+        end
+    end
+    L = sum(pair_pools(ctx, a, b)[1]; init=0)
+    nh = length(hubs)
+    paid, received, price, status = zeros(q), zeros(q), zeros(q), zeros(UInt8, q)
+    hp, hs, ld, ll = zeros(nh), zeros(nh), zeros(2, L), zeros(2, L)
+    if fn === :quote
+        chk(ctx, ccall((:cfmm_quote_routed_orders, LIB), Cint,
+            (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Int64}, Ptr{Int64},
+             Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+             Ptr{Float64}),
+            ctx, q, token_in, token_out, kind, amount, hub_off, hubs, paid, received, price, status, hp, hs, ld, ll))
+    else
+        chk(ctx, ccall((:cfmm_execute_routed_orders, LIB), Cint,
+            (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64}, Ptr{Int64},
+             Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64},
+             Ptr{Float64}, Ptr{Float64}),
+            ctx, q, token_in, token_out, kind, amount, limit === nothing ? C_NULL : limit, hub_off, hubs, paid,
+            received, price, status, hp, hs, ld, ll))
+    end
+    return paid, received, price, status, hp, hs, ld, ll
+end
+quote_routed_orders(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}, kind::Vector{UInt8},
+                    amount::Vector{Float64}, hub_off::Vector{Int64}, hubs::Vector{Int64}) =
+    _routed_orders(:quote, ctx, token_in, token_out, kind, amount, hub_off, hubs, nothing)
+execute_routed_orders!(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}, kind::Vector{UInt8},
+                       amount::Vector{Float64}, hub_off::Vector{Int64}, hubs::Vector{Int64},
+                       limit::Union{Nothing,Vector{Float64}}=nothing) =
+    _routed_orders(:execute, ctx, token_in, token_out, kind, amount, hub_off, hubs, limit)
+
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
 # current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never

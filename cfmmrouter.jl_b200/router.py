@@ -482,6 +482,80 @@ class DevicePools:
         paid); a row whose limit fails reverts.  Returns what quote_split_orders returns."""
         return self._split(True, token_in, token_out, kind, amount, limit, legs)
 
+    # -- orders routed over their pair and two-hop routes through hubs (include/cfmm_b200.h,
+    #    cfmm_quote_routed_orders / cfmm_execute_routed_orders) -----------------------------------
+    @staticmethod
+    def route_pairs(token_in, token_out, hub_off, hubs):
+        """The pair lists of routed rows, as cfmm_pair_pools rows: per row (j, i), then (j, h), (h, i)
+        for each of its hubs.  Returns (token_a, token_b, first list of each row [q + 1])."""
+        a, b, first = [], [], [0]
+        for r in range(len(token_in)):
+            j, i = int(token_in[r]), int(token_out[r])
+            a.append(j)
+            b.append(i)
+            for h in hubs[int(hub_off[r]):int(hub_off[r + 1])]:
+                a += [j, int(h)]
+                b += [int(h), i]
+            first.append(len(a))
+        return np.array(a, dtype=np.int64), np.array(b, dtype=np.int64), np.array(first, dtype=np.int64)
+
+    def _routed(self, execute, token_in, token_out, kind, amount, hub_off, hubs, limit, legs):
+        tin = np.ascontiguousarray(token_in, dtype=np.int64).reshape(-1)
+        tout = np.ascontiguousarray(token_out, dtype=np.int64).reshape(-1)
+        kind = np.ascontiguousarray(kind, dtype=np.uint8).reshape(-1)
+        amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
+        hub_off = np.ascontiguousarray(hub_off, dtype=np.int64).reshape(-1)
+        hubs = np.ascontiguousarray(hubs, dtype=np.int64).reshape(-1)
+        q = len(tin)
+        if not (len(tout) == len(kind) == len(amount) == q) or len(hub_off) != q + 1:
+            raise ValueError("routed orders: token_in, token_out, kind and amount need one entry per row, "
+                             "hub_off q + 1")
+        if limit is not None:
+            limit = np.ascontiguousarray(limit, dtype=np.float64).reshape(-1)
+            if len(limit) != q:
+                raise ValueError(f"limit must have {q} entries, one per row")
+        nh = int(hub_off[-1]) if q else 0
+        if q and (hub_off[0] != 0 or np.any(np.diff(hub_off) < 0) or len(hubs) != nh):
+            raise ValueError("routed orders: hub_off must rise from 0 to len(hubs)")
+        paid, received, price = np.zeros(q), np.zeros(q), np.zeros(q)
+        status = np.zeros(q, dtype=np.uint8)
+        hp, hs = np.zeros(nh), np.zeros(nh)
+        off = ld = ll = None
+        if legs:
+            off = np.zeros(1, dtype=np.int64)
+            if q:
+                a, b, first = self.route_pairs(tin, tout, hub_off, hubs)
+                off = self.pair_pools(a, b)[0][first]
+            ld, ll = np.zeros((int(off[-1]), 2)), np.zeros((int(off[-1]), 2))
+        u8 = C.POINTER(C.c_uint8)
+        args = [self._ctx, q, _ip(tin), _ip(tout), kind.ctypes.data_as(u8), _dp(amount)]
+        if execute:
+            args.append(None if limit is None else _dp(limit))
+        args += [_ip(hub_off) if q else None, _ip(hubs) if nh else None, _dp(paid), _dp(received), _dp(price),
+                 status.ctypes.data_as(u8), _dp(hp) if nh else None, _dp(hs) if nh else None,
+                 _dp(ld) if legs else None, _dp(ll) if legs else None]
+        fn = self._lib.cfmm_execute_routed_orders if execute else self._lib.cfmm_quote_routed_orders
+        self._chk(fn(*args))
+        out = (paid, received, price, status, hp, hs)
+        return out + ((off, ld, ll),) if legs else out
+
+    def quote_routed_orders(self, token_in, token_out, kind, amount, hub_off, hubs, legs: bool = False):
+        """cfmm_quote_routed_orders: row j sells token_in[j] for token_out[j] (1-based) over the pools of
+        the pair and, for each hub h of hubs[hub_off[j] .. hub_off[j+1]] (at most ROUTE_MAX_HUBS), the
+        pools of (token_in, h) and (h, token_out), split optimally; kind 0 tenders amount[j], kind 1
+        wants amount[j].  Every row on the current state on its own; no state changes.  Returns (paid
+        [q], received [q], price [q] = s*, status [q] uint8, hub_price [Σ] = t_h*, hub_surplus [Σ]) and,
+        with legs=True, also (off [q + 1], leg_delta [L, 2], leg_lambda [L, 2]), each row's legs in the
+        pair_pools order of route_pairs."""
+        return self._routed(False, token_in, token_out, kind, amount, hub_off, hubs, None, legs)
+
+    def execute_routed_orders(self, token_in, token_out, kind, amount, hub_off, hubs, limit=None,
+                              legs: bool = False):
+        """cfmm_execute_routed_orders: the rows of quote_routed_orders in batch order, each on the state
+        the earlier filled rows left, with optional limits (kind 0: minimum received; kind 1: maximum
+        paid); a row whose limit fails reverts.  Returns what quote_routed_orders returns."""
+        return self._routed(True, token_in, token_out, kind, amount, hub_off, hubs, limit, legs)
+
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
         """cfmm_modify_univ3_liquidity: row j adds dL[j] (> 0 mints, < 0 burns) to the ticks of UniV3
@@ -917,6 +991,47 @@ class Router:
         filled = out[3] == _lib.ORDER_FILLED
         if np.any(filled):
             _, typ, idx, _ = self._pools.pair_pools(tin[filled], tout[filled])
+            self._refresh_swapped([(t, None, idx[typ == t]) for t in (0, 1, 2) if np.any(typ == t)])
+        return out
+
+    def _routed_args(self, token_in, token_out, kinds, amounts, hubs, limits, what):
+        tin, tout, kinds, amounts, limits = self._split_args(token_in, token_out, kinds, amounts, limits, what)
+        q = len(tin)
+        if all(np.ndim(h) == 0 for h in hubs):  # one list shared by every row
+            per_row = [list(hubs)] * q
+        else:
+            per_row = [list(h) for h in hubs]
+            if len(per_row) != q:
+                raise ValueError(f"{what}: hubs must be one list, or one list per row ({q})")
+        hub_off = np.concatenate([[0], np.cumsum([len(h) for h in per_row])]).astype(np.int64)
+        flat = np.array([int(x) for h in per_row for x in h], dtype=np.int64)
+        return tin, tout, kinds, amounts, hub_off, flat, limits
+
+    def quote_routed_orders(self, token_in, token_out, kinds, amounts, hubs):
+        """Sell token_in[j] for token_out[j] (1-based) over the pools of the pair and the two-hop routes
+        through the hub tokens `hubs` (one list for every row, or one list per row; at most
+        ROUTE_MAX_HUBS each), split optimally (cfmm_quote_routed_orders): kind 0 tenders amounts[j],
+        kind 1 wants amounts[j] out.  Pools between two hubs are not used.  Every row on the current
+        state on its own; no state changes.  Returns (paid [q], received [q], price [q], status [q]);
+        price is s* = ν_in/ν_out.  Single GPU."""
+        tin, tout, kinds, amounts, off, flat, _ = self._routed_args(token_in, token_out, kinds, amounts, hubs, None,
+                                                                    "quote_routed_orders")
+        return self._pools.quote_routed_orders(tin, tout, kinds, amounts, off, flat)[:4]
+
+    def execute_routed_orders(self, token_in, token_out, kinds, amounts, hubs, limits=None):
+        """Execute routed orders in order (cfmm_execute_routed_orders), each with an optional limit (kind
+        0: the minimum received; kind 1: the maximum paid): a row whose limit fails reverts and later
+        rows see the state without it.  Returns what quote_routed_orders returns and refreshes the pool
+        objects of the filled rows' pairs from the device state, as execute_swaps does.  Single GPU."""
+        tin, tout, kinds, amounts, off, flat, limits = self._routed_args(token_in, token_out, kinds, amounts, hubs,
+                                                                         limits, "execute_routed_orders")
+        out = self._pools.execute_routed_orders(tin, tout, kinds, amounts, off, flat, limits)[:4]
+        filled = np.flatnonzero(out[3] == _lib.ORDER_FILLED)
+        if len(filled):
+            sub = np.concatenate([[0], np.cumsum(np.diff(off)[filled])]).astype(np.int64)
+            fh = np.concatenate([flat[off[r]:off[r + 1]] for r in filled]).astype(np.int64)
+            a, b, _ = DevicePools.route_pairs(tin[filled], tout[filled], sub, fh)
+            _, typ, idx, _ = self._pools.pair_pools(a, b)
             self._refresh_swapped([(t, None, idx[typ == t]) for t in (0, 1, 2) if np.any(typ == t)])
         return out
 

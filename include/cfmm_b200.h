@@ -505,6 +505,86 @@ int cfmm_execute_split_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_in,
                               double *price, uint8_t *status, double *leg_delta,
                               double *leg_lambda);
 
+/* ---- orders routed over their pair and two-hop routes through hub tokens -----------------
+ * A row sells j = token_in[r] for i = token_out[r] (1-based, distinct) over the pools of {j, i}
+ * (the direct pools) and, for each of its hubs h = hubs[hub_off[r] .. hub_off[r+1]) (1-based,
+ * 0..CFMM_ROUTE_MAX_HUBS per row, distinct, neither i nor j), the pools of {j, h} and of {h, i}
+ * (hub h's pools), each list in cfmm_pair_pools order.  Pools between two hubs are not used.  This
+ * is route! with Swap(i, j, δ) over exactly these pools (src/objectives.jl:92-146,
+ * docs/src/method.md).  With ν_i = 1, ν_j = s and ν_h = t_h, hub h's price only enters hub h's pools,
+ * so the dual separates: for each s, t_h solves "hub h's pools net to zero in h" (monotone in t_h),
+ * and what is left is the split's convex problem in s, whose slope is δ − N(s).  General pool
+ * graphs, with pools between hubs, remain cfmm_solve's.
+ *
+ * Pool response at (s, t).  A pool's legs are split orders' (the materialising find_arb! at ν[Ai],
+ * mapped back to the ingest token order; retired pools give (0, 0)) at ν_i = 1, ν_j = s, ν_h = t_h.
+ *
+ * Sums, each with split orders' warp tree over one list of pools (partial l adds the terms of
+ * pools k ≡ l (mod 32) in increasing k from +0.0, then the xor butterfly 16 … 1):
+ *   direct    over the direct pools: N_d = Σ (Δ_j − Λ_j), O_d = Σ (Λ_i − Δ_i), split orders' bits;
+ *   hub h     over its {j, h} pools followed by its {h, i} pools: N_h = Σ (Δ_j − Λ_j),
+ *             O_h = Σ (Λ_i − Δ_i) and H_h = Σ (Λ_h − Δ_h), a pool adding nothing to a sum whose
+ *             token it does not hold (each term one IEEE subtraction);
+ *   N(s) = ((N_d + N_h₁) + N_h₂) + … and O(s) likewise, in the row's hub order, each hub's sums
+ *   taken at its t_h(s).  With no hubs, or hubs that hold no pools, N and O are split orders'.
+ *
+ * Search.  Both searches are split orders' gallop and bisection on the ordinals o(x) of the doubles
+ * in [DBL_MIN, DBL_MAX], from a start o(e) clamped to that range (o(DBL_MIN) for a NaN e):
+ *   inner (hub h, at one s)  enough(t) is !(H_h(t) >= 0) (a NaN counts as true).  t_h(s) = hi, the
+ *           smallest ordinal the search finds with H_h >= 0, so the hub surplus is never negative;
+ *           when H_h(DBL_MIN) >= 0 already (the gallop down reaches o(DBL_MIN)), t_h = DBL_MIN.
+ *           The first inner search of a row starts from the largest no-trade boundary of the hub's
+ *           active {h, i} pools (split orders' boundary with h in j's role); every later one starts
+ *           from the t_h the row's previous outer evaluation found.  H_h < 0 at t = DBL_MAX (the
+ *           gallop up reaches o(DBL_MAX)) makes the row CFMM_ORDER_UNREACHABLE.
+ *   outer   split orders' search on s with their enough (exact-in N(s) > δ, exact-out O(s) >= y),
+ *           each evaluation running every hub's inner search.  Its start e is the largest of the
+ *           direct pools' boundaries (split orders') and, for each hub with an active pool on both
+ *           sides, b_jh · b_hi (one IEEE multiply; b_jh the largest boundary of its active {j, h}
+ *           pools with j in j's role, b_hi that of its {h, i} pools with h in j's role).
+ *           s* = hi for exact-in, lo for exact-out; t_h* = the t_h found at s* by that evaluation.
+ * The legs pass at s* reuses t_h* and runs no inner search.  So a row costs at most 127 evaluations
+ * of the direct pools and, for each hub, 126·126 + 1 of its pools.  A row with no hubs is split
+ * orders' row bit for bit (legs, status and price included).  A row none of whose pools is active
+ * is UNREACHABLE, and amount 0 fills with zeros and runs no search.
+ *
+ * Outputs, each optional (NULL): paid = N(s*), received = O(s*), price = s* (0 when unreachable or
+ * amount 0), status [q] (CFMM_ORDER_*); hub_price [Σ] = t_h* (0 when price is 0); hub_surplus [Σ]
+ * = H_h(t_h*) >= 0, the hub token left with the trader (0 unless filled); legs leg_delta,
+ * leg_lambda [2L], row after row, each row's lists concatenated in the order {j, i}, {j, h₁},
+ * {h₁, i}, {j, h₂}, …, so that one cfmm_pair_pools call on those pairs identifies them; 0 for a row
+ * that does not fill.
+ *
+ * cfmm_quote_routed_orders prices every row on the current state on its own; no state changes.
+ * cfmm_execute_routed_orders runs the rows in batch order with split orders' limits and revert rule.
+ * A filled row applies cfmm_apply_trades' transition at its ν to each of its active pools (two-coin
+ * R <- (R + γΔ) − Λ; UniV3 the q′ rule with p = ν[a]/ν[b], current tick updated).  Two rows
+ * conflict when they share a token pair (a pool belongs to one pair): a row's level is 1 + the
+ * highest level of an earlier row sharing one of its pairs, and each level is one launch of one CTA
+ * per row (warp 0 the direct pools, warp 1 + h hub h).  Afterwards the bookkeeping of
+ * cfmm_execute_swaps.  Reverted and unreachable rows change nothing.
+ *
+ * Both are synchronous.  Before cfmm_finalize: CFMM_ERR_STATE.  q == 0 does nothing.
+ * CFMM_ERR_INVALID before anything changes for every argument split orders reject, and for: a null
+ * hub_off, hub_off[0] != 0, a row with fewer than 0 or more than CFMM_ROUTE_MAX_HUBS hubs, a null
+ * hubs with hub_off[q] > 0, a hub outside 1..n_tokens, equal to the row's i or j, or listed twice in
+ * the row. */
+#define CFMM_ROUTE_MAX_HUBS 7
+int cfmm_quote_routed_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [q] */,
+                             const int64_t *token_out /* [q] */, const uint8_t *kind /* [q] */,
+                             const double *amount /* [q] */, const int64_t *hub_off /* [q+1] */,
+                             const int64_t *hubs /* [Σ] */, double *paid /* [q] */,
+                             double *received /* [q] */, double *price /* [q] */,
+                             uint8_t *status /* [q] */, double *hub_price /* [Σ] */,
+                             double *hub_surplus /* [Σ] */, double *leg_delta /* [2L] */,
+                             double *leg_lambda /* [2L] */);
+int cfmm_execute_routed_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_in,
+                               const int64_t *token_out, const uint8_t *kind, const double *amount,
+                               const double *limit /* [q] or NULL */, const int64_t *hub_off,
+                               const int64_t *hubs, double *paid, double *received, double *price,
+                               uint8_t *status, double *hub_price, double *hub_surplus,
+                               double *leg_delta, double *leg_lambda);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
@@ -652,7 +732,8 @@ int64_t cfmm_launch_count(const cfmm_ctx *ctx);
  * exchange kernel, or 4 = the kernels of cfmm_quote_swaps / cfmm_execute_swaps /
  * cfmm_quote_swaps_exact_out / cfmm_execute_swap_orders / cfmm_quote_paths /
  * cfmm_execute_paths / cfmm_pair_pools / cfmm_quote_split_orders /
- * cfmm_execute_split_orders, the pair-index build counted as one launch); it
+ * cfmm_execute_split_orders / cfmm_quote_routed_orders / cfmm_execute_routed_orders,
+ * the pair-index build counted as one launch); it
  * synchronises on the recorded events.
  * cfmm_profile_reset re-arms the same N pairs. */
 int cfmm_profile_read(cfmm_ctx *ctx, int type, double *total_ms, int64_t *launches);
