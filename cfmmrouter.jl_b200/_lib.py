@@ -97,6 +97,12 @@ SYMBOLS = {
                                            _dp, C.POINTER(C.c_uint8), _dp, _dp, _dp, _dp]),
     "cfmm_execute_routed_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, _dp, _ip, _ip, _dp,
                                              _dp, _dp, C.POINTER(C.c_uint8), _dp, _dp, _dp, _dp]),
+    "cfmm_quote_arbitrage": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, _ip, _dp, _dp, _dp, C.POINTER(C.c_uint8), _dp,
+                                       _dp, _dp, _dp]),
+    "cfmm_execute_arbitrage": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _dp, _ip, _ip, _dp, _dp, _dp, C.POINTER(C.c_uint8),
+                                         _dp, _dp, _dp, _dp]),
+    "cfmm_scan_arbitrage": (C.c_int, [_ctx, C.c_int64, _ip, _dp, C.c_int, C.c_int64, _ip, _ip, _ip, _ip, _ip, _dp,
+                                      _dp]),
     "cfmm_modify_univ3_liquidity":(C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),

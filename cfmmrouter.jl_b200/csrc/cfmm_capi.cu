@@ -34,6 +34,7 @@
 #include "path_kernels.cuh"
 #include "split_kernels.cuh"
 #include "route_kernels.cuh"
+#include "arb_scan_kernels.cuh"
 #include "univ3_state.cuh"
 
 #include <cub/cub.cuh>
@@ -261,6 +262,12 @@ struct cfmm_ctx {
     bool built = false;
     int64_t n_pairs = 0;
     DevBuf<int64_t> keys, off, pool;  // distinct keys ascending; CSR [n_pairs + 1]; entries by key
+    // the token adjacency of cfmm_scan_arbitrage (arb_scan_kernels.cuh): built on first use after
+    // the index, kept with it
+    bool adj_built = false;
+    DevBuf<int64_t> adj_off;             // [n_tokens + 1]
+    DevBuf<int32_t> adj_nbr, adj_pair;   // [2·n_pairs]
+    std::vector<int64_t> adj_off_host;
   } pairs;
   int64_t launches = 0;
   std::string err;
@@ -3023,6 +3030,11 @@ int ensure_pair_index(cfmm_ctx* ctx) {
   if (ix.built) return CFMM_OK;
   const int64_t n = ctx->n_pools, nt = ctx->n_tokens;
   if (n > INT32_MAX) return fail(ctx, CFMM_ERR_INVALID, "pair index: more than 2^31 - 1 pools");
+  ix.adj_built = false;
+  ix.adj_off.release();
+  ix.adj_nbr.release();
+  ix.adj_pair.release();
+  ix.adj_off_host.clear();
   ix.keys.release();
   ix.off.release();
   ix.pool.release();
@@ -3307,11 +3319,37 @@ int split_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, c
 // ---- orders routed over their pair and two-hop routes through hubs (route_kernels.cuh) ----------
 
 // Every argument of cfmm_quote_routed_orders / cfmm_execute_routed_orders, before anything runs.
+int check_hubs(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const int64_t* hub_off,
+               const int64_t* hubs, const char* what);
+
 int check_routed(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const uint8_t* kind,
                  const double* amount, const double* limit, const int64_t* hub_off, const int64_t* hubs,
                  const char* what) {
   int rc = check_split(ctx, q, token_in, token_out, kind, amount, limit, what);
   if (rc != CFMM_OK || q == 0) return rc;
+  return check_hubs(ctx, q, token_in, token_out, hub_off, hubs, what);
+}
+
+// Every argument of cfmm_quote_arbitrage / cfmm_execute_arbitrage: routed rows' tokens and hubs, and
+// min_profit (NULL: 0) neither NaN, negative nor +inf (an exact-in row's minimum received).
+int check_arbitrage(cfmm_ctx* ctx, int64_t q, const int64_t* base, const int64_t* other, const double* min_profit,
+                    const int64_t* hub_off, const int64_t* hubs, const char* what) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if (q < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: negative row count", what);
+  if (q == 0) return CFMM_OK;
+  if (!base || !other) return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
+  if ((rc = check_pair_tokens(ctx, q, other, base, what)) != CFMM_OK) return rc;
+  for (int64_t r = 0; min_profit && r < q; ++r)
+    if (!(min_profit[r] >= 0.0) || std::isinf(min_profit[r]))
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: min_profit %g must be finite and >= 0", what, (long long)r,
+                  min_profit[r]);
+  return check_hubs(ctx, q, other, base, hub_off, hubs, what);
+}
+
+// Routed and arbitrage rows' hub lists.
+int check_hubs(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const int64_t* hub_off,
+               const int64_t* hubs, const char* what) {
   if (!hub_off) return fail(ctx, CFMM_ERR_INVALID, "%s: null hub_off", what);
   if (hub_off[0] != 0) return fail(ctx, CFMM_ERR_INVALID, "%s: hub_off[0] = %lld, not 0", what, (long long)hub_off[0]);
   for (int64_t r = 0; r < q; ++r) {
@@ -3338,7 +3376,9 @@ int check_routed(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_
   return CFMM_OK;
 }
 
-int routed_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, const int64_t* token_out,
+// Routed rows, or with arb arbitrage rows (token_in = the other token, token_out = the base token,
+// kind and amount null, limit = min_profit, paid = the surplus of the other token, received = profit).
+int routed_orders(cfmm_ctx* ctx, bool exec, bool arb, int64_t q, const int64_t* token_in, const int64_t* token_out,
                   const uint8_t* kind, const double* amount, const double* limit, const int64_t* hub_off,
                   const int64_t* hubs, double* paid, double* received, double* price, uint8_t* status,
                   double* hub_price, double* hub_surplus, double* leg_delta, double* leg_lambda) {
@@ -3382,10 +3422,12 @@ int routed_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, 
     CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_hubs.p, hubs, (size_t)nh * sizeof(int64_t)));
   }
   CU_TRY(ctx, d_leg_off.upload(leg_off));
-  CU_TRY(ctx, d_kind.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<uint8_t>::copy_in(d_kind.p, kind, (size_t)q));
-  CU_TRY(ctx, d_amount.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<double>::copy_in(d_amount.p, amount, (size_t)q * sizeof(double)));
+  if (!arb) {
+    CU_TRY(ctx, d_kind.alloc((size_t)q));
+    CU_TRY(ctx, DevBuf<uint8_t>::copy_in(d_kind.p, kind, (size_t)q));
+    CU_TRY(ctx, d_amount.alloc((size_t)q));
+    CU_TRY(ctx, DevBuf<double>::copy_in(d_amount.p, amount, (size_t)q * sizeof(double)));
+  }
   if (limit) {
     CU_TRY(ctx, d_limit.alloc((size_t)q));
     CU_TRY(ctx, DevBuf<double>::copy_in(d_limit.p, limit, (size_t)q * sizeof(double)));
@@ -3410,7 +3452,10 @@ int routed_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, 
   const unsigned threads = 32u * (1u + (unsigned)max_hubs);  // warp 0: the direct pools, warp 1 + h: hub h
   if (!exec) {
     ProfScope prof(ctx, kProfSwaps, ctx->stream);
-    cfmm::route_quote_kernel<<<(unsigned)q, threads, 0, ctx->stream>>>(os.d_P.p, ix, R);
+    if (arb)
+      cfmm::arb_quote_kernel<<<(unsigned)q, threads, 0, ctx->stream>>>(os.d_P.p, ix, R);
+    else
+      cfmm::route_quote_kernel<<<(unsigned)q, threads, 0, ctx->stream>>>(os.d_P.p, ix, R);
     ctx->launches++;
     CU_TRY(ctx, cudaGetLastError());
   } else {
@@ -3447,8 +3492,12 @@ int routed_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, 
       if (n == 0) continue;
       {
         ProfScope prof(ctx, kProfSwaps, ctx->stream);
-        cfmm::route_execute_kernel<<<(unsigned)n, threads, 0, ctx->stream>>>(os.d_P.p, ix, R,
+        if (arb)
+          cfmm::arb_execute_kernel<<<(unsigned)n, threads, 0, ctx->stream>>>(os.d_P.p, ix, R,
                                                                               d_rows.p + start[(size_t)l], os.mv);
+        else
+          cfmm::route_execute_kernel<<<(unsigned)n, threads, 0, ctx->stream>>>(os.d_P.p, ix, R,
+                                                                                d_rows.p + start[(size_t)l], os.mv);
       }
       ctx->launches++;
       CU_TRY(ctx, cudaGetLastError());
@@ -3469,6 +3518,260 @@ int routed_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, 
     CU_TRY(ctx, d2h(leg_lambda, d_ll.p, (size_t)(2 * L) * sizeof(double)));
   }
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return CFMM_OK;
+}
+
+// ---- arbitrage cycles through base tokens (arb_scan_kernels.cuh) --------------------------------
+
+// Every argument of cfmm_scan_arbitrage, before anything runs.
+int check_scan(cfmm_ctx* ctx, int64_t nb, const int64_t* base, const double* min_profit, int max_hubs, int64_t cap,
+               const int64_t* found, const int64_t* row_base, const int64_t* row_other, const int64_t* hub_count,
+               const int64_t* hubs, const double* profit, const double* price) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if (nb < 0) return fail(ctx, CFMM_ERR_INVALID, "scan_arbitrage: negative base count");
+  if (cap < 0) return fail(ctx, CFMM_ERR_INVALID, "scan_arbitrage: negative cap");
+  if (!found) return fail(ctx, CFMM_ERR_INVALID, "scan_arbitrage: null found");
+  if (max_hubs < 0 || max_hubs > CFMM_ROUTE_MAX_HUBS)
+    return fail(ctx, CFMM_ERR_INVALID, "scan_arbitrage: max_hubs %d, not 0..%d", max_hubs, CFMM_ROUTE_MAX_HUBS);
+  if (cap > 0 && (!row_base || !row_other || !hub_count || !hubs || !profit || !price))
+    return fail(ctx, CFMM_ERR_INVALID, "scan_arbitrage: null output with cap > 0");
+  if (nb == 0) return CFMM_OK;
+  if (!base || !min_profit) return fail(ctx, CFMM_ERR_INVALID, "scan_arbitrage: null array argument");
+  for (int64_t b = 0; b < nb; ++b) {
+    if (base[b] < 1 || base[b] > ctx->n_tokens)
+      return fail(ctx, CFMM_ERR_INVALID, "scan_arbitrage: base %lld: token %lld outside 1..%lld", (long long)b,
+                  (long long)base[b], (long long)ctx->n_tokens);
+    if (!(min_profit[b] > 0.0) || std::isinf(min_profit[b]))
+      return fail(ctx, CFMM_ERR_INVALID, "scan_arbitrage: base %lld: min_profit %g must be finite and > 0",
+                  (long long)b, min_profit[b]);
+  }
+  std::vector<int64_t> sorted(base, base + nb);
+  std::sort(sorted.begin(), sorted.end());
+  for (int64_t b = 1; b < nb; ++b)
+    if (sorted[(size_t)b] == sorted[(size_t)b - 1])
+      return fail(ctx, CFMM_ERR_INVALID, "scan_arbitrage: base token %lld listed twice", (long long)sorted[(size_t)b]);
+  return CFMM_OK;
+}
+
+// The token adjacency (arb_scan_kernels.cuh), built from the pair index's keys and kept with it.
+int ensure_adjacency(cfmm_ctx* ctx) {
+  int rc;
+  if ((rc = ensure_pair_index(ctx)) != CFMM_OK) return rc;
+  auto& ix = ctx->pairs;
+  if (ix.adj_built) return CFMM_OK;
+  const int64_t nt = ctx->n_tokens, np = ix.n_pairs, m = 2 * np;
+  if (nt >= INT32_MAX || m > INT32_MAX)
+    return fail(ctx, CFMM_ERR_INVALID, "token adjacency: more than 2^31 - 1 tokens or entries");
+  cudaStream_t st = ctx->stream;
+  CU_TRY(ctx, ix.adj_off.alloc((size_t)nt + 1));
+  CU_TRY(ctx, ix.adj_nbr.alloc((size_t)m));
+  CU_TRY(ctx, ix.adj_pair.alloc((size_t)m));
+  DevBuf<int64_t> kin, kout;
+  DevBuf<int32_t> vin;
+  DevBuf<unsigned char> temp;
+  size_t bytes = 0;
+  int end_bit = 1;  // keys < n_tokens²
+  while (end_bit < 63 && (1ll << end_bit) < nt * nt) ++end_bit;
+  if (m > 0) {
+    CU_TRY(ctx, kin.alloc((size_t)m));
+    CU_TRY(ctx, kout.alloc((size_t)m));
+    CU_TRY(ctx, vin.alloc((size_t)m));
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(nullptr, bytes, kin.p, kout.p, vin.p, ix.adj_pair.p, (int)m, 0, end_bit,
+                                                st));
+    CU_TRY(ctx, temp.alloc(bytes));
+  }
+  {
+    ProfScope prof(ctx, kProfSwaps, st);
+    if (m > 0) {
+      cfmm::adj_entries_kernel<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(ix.keys.p, np, nt, kin.p, vin.p);
+      CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(temp.p, bytes, kin.p, kout.p, vin.p, ix.adj_pair.p, (int)m, 0,
+                                                  end_bit, st));
+      ctx->launches += 2;
+    }
+    const int64_t th = std::max(m, nt + 1);
+    cfmm::adj_finish_kernel<<<(unsigned)((th + 255) / 256), 256, 0, st>>>(kout.p, m, nt, ix.adj_nbr.p, ix.adj_off.p);
+    ctx->launches++;
+  }
+  CU_TRY(ctx, cudaGetLastError());
+  ix.adj_off_host.resize((size_t)nt + 1);
+  CU_TRY(ctx, cudaMemcpyAsync(ix.adj_off_host.data(), ix.adj_off.p, ((size_t)nt + 1) * sizeof(int64_t),
+                              cudaMemcpyDeviceToHost, st));
+  CU_TRY(ctx, cudaStreamSynchronize(st));
+  ix.adj_built = true;
+  return CFMM_OK;
+}
+
+int scan_arbitrage(cfmm_ctx* ctx, int64_t nb, const int64_t* base, const double* min_profit, int max_hubs, int64_t cap,
+                   int64_t* found, int64_t* row_base, int64_t* row_other, int64_t* hub_count, int64_t* hubs,
+                   double* profit, double* price) {
+  int rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  if ((rc = ensure_adjacency(ctx)) != CFMM_OK) return rc;
+  auto& ix = ctx->pairs;
+  cudaStream_t st = ctx->stream;
+  const int64_t np = ix.n_pairs;
+  // slots: (base b, its e-th neighbour), base after base
+  std::vector<int64_t> slot_off((size_t)nb + 1, 0);
+  for (int64_t b = 0; b < nb; ++b)
+    slot_off[(size_t)b + 1] =
+        slot_off[(size_t)b] + ix.adj_off_host[(size_t)base[b]] - ix.adj_off_host[(size_t)base[b] - 1];
+  const int64_t ns = slot_off[(size_t)nb];
+  if (ns == 0) return CFMM_OK;
+  DevBuf<unsigned char> temp;
+  const auto cub_scan = [&](const int64_t* in, int64_t* out, int64_t n) {
+    size_t b = 0;
+    cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, b, in, out, (int)n, st);
+    if (e == cudaSuccess && b > temp.n) e = temp.alloc(b);
+    return e == cudaSuccess ? cub::DeviceScan::ExclusiveSum(temp.p, b, in, out, (int)n, st) : e;
+  };
+  const auto d2h_now = [&](void* dst, const void* src, size_t bytes) {
+    cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st);
+    return e == cudaSuccess ? cudaStreamSynchronize(st) : e;
+  };
+  const auto blocks = [](int64_t threads) { return (unsigned)((threads + 255) / 256); };
+  OrderSets os;
+  if ((rc = order_sets(ctx, false, os)) != CFMM_OK) return rc;
+  // rates
+  DevBuf<long long> rate;
+  CU_TRY(ctx, rate.alloc((size_t)(2 * np)));
+  CU_TRY(ctx, cudaMemsetAsync(rate.p, 0, (size_t)(2 * np) * sizeof(long long), st));
+  {
+    ProfScope prof(ctx, kProfSwaps, st);
+    cfmm::arb_rates_kernel<<<blocks(ctx->n_pools), 256, 0, st>>>(os.d_P.p, ix.off.p, ix.pool.p, ix.keys.p, np,
+                                                                 ctx->n_tokens, rate.p);
+  }
+  ctx->launches++;
+  CU_TRY(ctx, cudaGetLastError());
+  // candidates, one warp per slot, then their rows in slot order
+  DevBuf<int64_t> d_base, d_slot_off, flag, nhub, row_pos, hub_pos;
+  DevBuf<int32_t> slot_hub, slot_lists;
+  DevBuf<double> d_min;
+  CU_TRY(ctx, d_base.alloc((size_t)nb));
+  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_base.p, base, (size_t)nb * sizeof(int64_t)));
+  CU_TRY(ctx, d_min.alloc((size_t)nb));
+  CU_TRY(ctx, DevBuf<double>::copy_in(d_min.p, min_profit, (size_t)nb * sizeof(double)));
+  CU_TRY(ctx, d_slot_off.upload(slot_off));
+  CU_TRY(ctx, flag.alloc((size_t)ns + 1));
+  CU_TRY(ctx, nhub.alloc((size_t)ns + 1));
+  CU_TRY(ctx, row_pos.alloc((size_t)ns + 1));
+  CU_TRY(ctx, hub_pos.alloc((size_t)ns + 1));
+  CU_TRY(ctx, slot_hub.alloc((size_t)(cfmm::kRouteMaxHubs * ns)));
+  CU_TRY(ctx, slot_lists.alloc((size_t)((1 + 2 * cfmm::kRouteMaxHubs) * ns)));
+  CU_TRY(ctx, cudaMemsetAsync(flag.p, 0, ((size_t)ns + 1) * sizeof(int64_t), st));
+  CU_TRY(ctx, cudaMemsetAsync(nhub.p, 0, ((size_t)ns + 1) * sizeof(int64_t), st));
+  const cfmm::AdjView A{ix.adj_off.p, ix.adj_nbr.p, ix.adj_pair.p};
+  {
+    ProfScope prof(ctx, kProfSwaps, st);
+    cfmm::arb_candidates_kernel<<<blocks(32 * ns), 256, 0, st>>>(A, reinterpret_cast<const double*>(rate.p), d_base.p,
+                                                                  d_slot_off.p, nb, max_hubs, flag.p, nhub.p,
+                                                                  slot_hub.p, slot_lists.p);
+    CU_TRY(ctx, cub_scan(flag.p, row_pos.p, ns + 1));
+    CU_TRY(ctx, cub_scan(nhub.p, hub_pos.p, ns + 1));
+  }
+  ctx->launches += 3;
+  CU_TRY(ctx, cudaGetLastError());
+  int64_t q = 0, nh = 0;
+  CU_TRY(ctx, d2h_now(&q, row_pos.p + ns, sizeof(int64_t)));
+  CU_TRY(ctx, d2h_now(&nh, hub_pos.p + ns, sizeof(int64_t)));
+  if (q == 0) return CFMM_OK;
+  DevBuf<int64_t> tin, tout, row_b, hub_off, d_hubs, pair;
+  DevBuf<double> surplus, d_profit, d_price;
+  DevBuf<uint8_t> status;
+  CU_TRY(ctx, tin.alloc((size_t)q));
+  CU_TRY(ctx, tout.alloc((size_t)q));
+  CU_TRY(ctx, row_b.alloc((size_t)q));
+  CU_TRY(ctx, hub_off.alloc((size_t)q + 1));
+  CU_TRY(ctx, d_hubs.alloc((size_t)nh));
+  CU_TRY(ctx, pair.alloc((size_t)(q + 2 * nh)));
+  CU_TRY(ctx, surplus.alloc((size_t)q));
+  CU_TRY(ctx, d_profit.alloc((size_t)q));
+  CU_TRY(ctx, d_price.alloc((size_t)q));
+  CU_TRY(ctx, status.alloc((size_t)q));
+  {
+    ProfScope prof(ctx, kProfSwaps, st);
+    cfmm::arb_rows_kernel<<<blocks(ns + 1), 256, 0, st>>>(A, d_base.p, d_slot_off.p, nb, flag.p, nhub.p, slot_hub.p,
+                                                          slot_lists.p, row_pos.p, hub_pos.p, tin.p, tout.p, row_b.p,
+                                                          hub_off.p, d_hubs.p, pair.p);
+  }
+  ctx->launches++;
+  CU_TRY(ctx, cudaGetLastError());
+  // solve: every candidate as an arbitrage row on the current state
+  const cfmm::PairIndexView pv{ix.off.p, ix.pool.p};
+  cfmm::RouteRows R{tin.p,     tout.p,  nullptr,    nullptr,     nullptr, hub_off.p, d_hubs.p, pair.p, nullptr,
+                    surplus.p, d_profit.p, d_price.p, status.p, nullptr, nullptr,   nullptr,  nullptr};
+  {
+    ProfScope prof(ctx, kProfSwaps, st);
+    cfmm::arb_quote_kernel<<<(unsigned)q, 32u * (1u + (unsigned)max_hubs), 0, st>>>(os.d_P.p, pv, R);
+  }
+  ctx->launches++;
+  CU_TRY(ctx, cudaGetLastError());
+  // select: filled rows with profit >= their base's minimum, then (base index, profit desc, x asc) by
+  // two stable sorts of the (base index, x)-ordered rows: on the complemented profit bits, then the base
+  DevBuf<int64_t> keep, keep_pos;
+  DevBuf<uint64_t> key;
+  CU_TRY(ctx, keep.alloc((size_t)q + 1));
+  CU_TRY(ctx, keep_pos.alloc((size_t)q + 1));
+  CU_TRY(ctx, key.alloc((size_t)q));
+  {
+    ProfScope prof(ctx, kProfSwaps, st);
+    cfmm::arb_keep_kernel<<<blocks(q + 1), 256, 0, st>>>(status.p, d_profit.p, row_b.p, d_min.p, q, keep.p, key.p);
+    CU_TRY(ctx, cub_scan(keep.p, keep_pos.p, q + 1));
+  }
+  ctx->launches += 2;
+  CU_TRY(ctx, cudaGetLastError());
+  int64_t n_sel = 0;
+  CU_TRY(ctx, d2h_now(&n_sel, keep_pos.p + q, sizeof(int64_t)));
+  *found = n_sel;
+  const int64_t n_out = std::min(n_sel, cap);
+  if (n_out == 0) return CFMM_OK;
+  DevBuf<int64_t> sel, v1, v2;
+  DevBuf<uint64_t> sel_key, key_s;
+  DevBuf<uint32_t> b1, b_s;
+  CU_TRY(ctx, sel.alloc((size_t)n_sel));
+  CU_TRY(ctx, v1.alloc((size_t)n_sel));
+  CU_TRY(ctx, v2.alloc((size_t)n_sel));
+  CU_TRY(ctx, sel_key.alloc((size_t)n_sel));
+  CU_TRY(ctx, key_s.alloc((size_t)n_sel));
+  CU_TRY(ctx, b1.alloc((size_t)n_sel));
+  CU_TRY(ctx, b_s.alloc((size_t)n_sel));
+  int b_bits = 1;
+  while (b_bits < 32 && (1ll << b_bits) < nb) ++b_bits;
+  size_t s1 = 0, s2 = 0;
+  CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(nullptr, s1, sel_key.p, key_s.p, sel.p, v1.p, (int)n_sel, 0, 64, st));
+  CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(nullptr, s2, b1.p, b_s.p, v1.p, v2.p, (int)n_sel, 0, b_bits, st));
+  if (std::max(s1, s2) > temp.n) CU_TRY(ctx, temp.alloc(std::max(s1, s2)));
+  DevBuf<int64_t> o_base, o_other, o_count, o_hubs;
+  DevBuf<double> o_profit, o_price;
+  CU_TRY(ctx, o_base.alloc((size_t)n_out));
+  CU_TRY(ctx, o_other.alloc((size_t)n_out));
+  CU_TRY(ctx, o_count.alloc((size_t)n_out));
+  CU_TRY(ctx, o_hubs.alloc((size_t)(cfmm::kRouteMaxHubs * n_out)));
+  CU_TRY(ctx, o_profit.alloc((size_t)n_out));
+  CU_TRY(ctx, o_price.alloc((size_t)n_out));
+  {
+    ProfScope prof(ctx, kProfSwaps, st);
+    cfmm::arb_select_kernel<<<blocks(q), 256, 0, st>>>(keep_pos.p, key.p, q, sel.p, sel_key.p);
+    s1 = temp.n;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(temp.p, s1, sel_key.p, key_s.p, sel.p, v1.p, (int)n_sel, 0, 64, st));
+    cfmm::arb_base_key_kernel<<<blocks(n_sel), 256, 0, st>>>(v1.p, n_sel, row_b.p, b1.p);
+    s2 = temp.n;
+    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(temp.p, s2, b1.p, b_s.p, v1.p, v2.p, (int)n_sel, 0, b_bits, st));
+    cfmm::arb_output_kernel<<<blocks(n_out), 256, 0, st>>>(v2.p, n_out, tin.p, tout.p, hub_off.p, d_hubs.p,
+                                                           d_profit.p, d_price.p, o_base.p, o_other.p, o_count.p,
+                                                           o_hubs.p, o_profit.p, o_price.p);
+  }
+  ctx->launches += 5;
+  CU_TRY(ctx, cudaGetLastError());
+  const size_t n8 = (size_t)n_out * sizeof(int64_t);
+  CU_TRY(ctx, cudaMemcpyAsync(row_base, o_base.p, n8, cudaMemcpyDeviceToHost, st));
+  CU_TRY(ctx, cudaMemcpyAsync(row_other, o_other.p, n8, cudaMemcpyDeviceToHost, st));
+  CU_TRY(ctx, cudaMemcpyAsync(hub_count, o_count.p, n8, cudaMemcpyDeviceToHost, st));
+  CU_TRY(ctx, cudaMemcpyAsync(hubs, o_hubs.p, n8 * cfmm::kRouteMaxHubs, cudaMemcpyDeviceToHost, st));
+  CU_TRY(ctx, cudaMemcpyAsync(profit, o_profit.p, (size_t)n_out * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU_TRY(ctx, cudaMemcpyAsync(price, o_price.p, (size_t)n_out * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CU_TRY(ctx, cudaStreamSynchronize(st));
   return CFMM_OK;
 }
 
@@ -3544,7 +3847,7 @@ int cfmm_quote_routed_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, 
                              double* hub_surplus, double* leg_delta, double* leg_lambda) {
   int rc = check_routed(ctx, q, token_in, token_out, kind, amount, nullptr, hub_off, hubs, "quote_routed_orders");
   if (rc != CFMM_OK || q == 0) return rc;
-  return routed_orders(ctx, false, q, token_in, token_out, kind, amount, nullptr, hub_off, hubs, paid, received, price,
+  return routed_orders(ctx, false, false, q, token_in, token_out, kind, amount, nullptr, hub_off, hubs, paid, received, price,
                        status, hub_price, hub_surplus, leg_delta, leg_lambda);
 }
 
@@ -3554,8 +3857,39 @@ int cfmm_execute_routed_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in
                                double* hub_price, double* hub_surplus, double* leg_delta, double* leg_lambda) {
   int rc = check_routed(ctx, q, token_in, token_out, kind, amount, limit, hub_off, hubs, "execute_routed_orders");
   if (rc != CFMM_OK || q == 0) return rc;
-  return routed_orders(ctx, true, q, token_in, token_out, kind, amount, limit, hub_off, hubs, paid, received, price,
-                       status, hub_price, hub_surplus, leg_delta, leg_lambda);
+  return routed_orders(ctx, true, false, q, token_in, token_out, kind, amount, limit, hub_off, hubs, paid, received,
+                       price, status, hub_price, hub_surplus, leg_delta, leg_lambda);
+}
+
+int cfmm_quote_arbitrage(cfmm_ctx* ctx, int64_t q, const int64_t* base, const int64_t* other, const int64_t* hub_off,
+                         const int64_t* hubs, double* profit, double* surplus_in, double* price, uint8_t* status,
+                         double* hub_price, double* hub_surplus, double* leg_delta, double* leg_lambda) {
+  int rc = check_arbitrage(ctx, q, base, other, nullptr, hub_off, hubs, "quote_arbitrage");
+  if (rc != CFMM_OK || q == 0) return rc;
+  return routed_orders(ctx, false, true, q, other, base, nullptr, nullptr, nullptr, hub_off, hubs, surplus_in, profit,
+                       price, status, hub_price, hub_surplus, leg_delta, leg_lambda);
+}
+
+int cfmm_execute_arbitrage(cfmm_ctx* ctx, int64_t q, const int64_t* base, const int64_t* other,
+                           const double* min_profit, const int64_t* hub_off, const int64_t* hubs, double* profit,
+                           double* surplus_in, double* price, uint8_t* status, double* hub_price, double* hub_surplus,
+                           double* leg_delta, double* leg_lambda) {
+  int rc = check_arbitrage(ctx, q, base, other, min_profit, hub_off, hubs, "execute_arbitrage");
+  if (rc != CFMM_OK || q == 0) return rc;
+  return routed_orders(ctx, true, true, q, other, base, nullptr, nullptr, min_profit, hub_off, hubs, surplus_in,
+                       profit, price, status, hub_price, hub_surplus, leg_delta, leg_lambda);
+}
+
+int cfmm_scan_arbitrage(cfmm_ctx* ctx, int64_t nb, const int64_t* base, const double* min_profit, int max_hubs,
+                        int64_t cap, int64_t* found, int64_t* row_base, int64_t* row_other, int64_t* hub_count,
+                        int64_t* hubs, double* profit, double* price) {
+  int rc = check_scan(ctx, nb, base, min_profit, max_hubs, cap, found, row_base, row_other, hub_count, hubs, profit,
+                      price);
+  if (rc != CFMM_OK) return rc;
+  *found = 0;
+  if (nb == 0) return CFMM_OK;
+  return scan_arbitrage(ctx, nb, base, min_profit, max_hubs, cap, found, row_base, row_other, hub_count, hubs, profit,
+                        price);
 }
 
 // ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------

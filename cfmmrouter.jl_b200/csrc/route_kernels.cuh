@@ -177,8 +177,11 @@ __device__ __forceinline__ RouteSums route_sums(const PathSets* P, const RouteWa
 
 // Row `row`, CTA-wide (blockDim.x = 32·(1 + the call's largest hub count); every thread takes every
 // CTA-level branch).  EXEC: the limit decides, and a filled row applies cfmm_apply_trades' transition
-// at its ν to each of its pools.
-template <bool EXEC>
+// at its ν to each of its pools.  ARB: an arbitrage row (cfmm_quote_arbitrage), the exact-in row with
+// δ = 0 that runs its search: j = the other token x, i = the base token p, kind and amount unread,
+// the limit is the minimum profit, paid reports the surplus 0 − N(s*) and received the profit O(s*);
+// a row whose pair {x, p} no pool holds is unreachable, and leg_off may be null when there are no legs.
+template <bool EXEC, bool ARB = false>
 __device__ __forceinline__ void route_row(const PathSets* P, const PairIndexView& ix, const RouteRows& R, int64_t row,
                                           const SplitMoved& mv) {
   __shared__ double sh_n[1 + kRouteMaxHubs], sh_o[1 + kRouteMaxHubs], sh_b1[1 + kRouteMaxHubs],
@@ -188,18 +191,19 @@ __device__ __forceinline__ void route_row(const PathSets* P, const PairIndexView
   const int nh = (int)(R.hub_off[row + 1] - R.hub_off[row]);
   const bool mine = w <= nh;  // this warp owns the direct pools or a hub's
   const int64_t tj = R.token_in[row] - 1;
-  const bool out = R.kind[row] == 1;
-  const double amt = R.amount[row];
+  const bool out = !ARB && R.kind[row] == 1;
+  const double amt = ARB ? 0.0 : R.amount[row];
   const double inf = __longlong_as_double(0x7ff0000000000000ll);
   const double lim = R.limit ? R.limit[row] : (out ? inf : 0.0);
   RouteWarp W{};
   if (mine) W = route_warp(ix, R, row, w, tj);
   uint8_t st = 0;  // CFMM_ORDER_FILLED
+  if (ARB && R.pair[row + 2 * R.hub_off[row]] < 0) st = 2;
   double s = 0.0;
   double N = 0.0, O = 0.0;
   int64_t th = kSplitOrdMin;  // this hub warp's t_h at s*, as an ordinal
   double hs = 0.0;            // and its surplus there
-  if (amt > 0.0) {
+  if (ARB ? st == 0 : amt > 0.0) {  // a routed row with amount 0 fills with zeros and runs no search
     // start: the largest no-trade boundary per list, and whether the list has an active pool
     if (mine) {
       double b1 = -inf, b2 = -inf;
@@ -322,12 +326,12 @@ __device__ __forceinline__ void route_row(const PathSets* P, const PairIndexView
       }
     }
   }
-  const bool filled = st == 0 && amt > 0.0;
+  const bool filled = st == 0 && (ARB || amt > 0.0);
   // legs (list order) and, on execute, the transition of each pool at (s*, t_h*)
   if (mine) {
     const double tv = __longlong_as_double(th);
     const int64_t base = row + 2 * R.hub_off[row];
-    const int64_t l0 = R.leg_off[w == 0 ? base : base + 2 * w - 1];
+    const int64_t l0 = (ARB && !R.leg_off) ? 0 : R.leg_off[w == 0 ? base : base + 2 * w - 1];
     for (int64_t t = lane; t < W.ca + W.cb; t += 32) {
       Trade tr;
       tr.d1 = tr.d2 = tr.l1 = tr.l2 = 0.0;
@@ -376,12 +380,12 @@ __device__ __forceinline__ void route_row(const PathSets* P, const PairIndexView
     }
     if (lane == 0 && W.hub) {
       const int64_t g = R.hub_off[row] + w - 1;
-      if (R.hub_price) R.hub_price[g] = (st == 2 || !(amt > 0.0)) ? 0.0 : tv;
+      if (R.hub_price) R.hub_price[g] = (st == 2 || !(ARB || amt > 0.0)) ? 0.0 : tv;
       if (R.hub_surplus) R.hub_surplus[g] = filled ? hs : 0.0;
     }
   }
   if (threadIdx.x == 0) {
-    R.paid[row] = filled ? N : 0.0;
+    R.paid[row] = filled ? (ARB ? __dsub_rn(0.0, N) : N) : 0.0;
     R.received[row] = filled ? O : 0.0;
     R.price[row] = st == 2 ? 0.0 : s;
     R.status[row] = st;
@@ -400,6 +404,19 @@ __global__ void __launch_bounds__(kRouteThreads, 1) route_execute_kernel(const P
                                                                       RouteRows R, const int64_t* __restrict__ rows,
                                                                       SplitMoved mv) {
   route_row<true>(P, ix, R, rows[blockIdx.x], mv);
+}
+
+// Arbitrage rows (cfmm_quote_arbitrage / cfmm_execute_arbitrage, and the solve of
+// cfmm_scan_arbitrage): route_row's ARB mode, launched as the routed kernels are.
+__global__ void __launch_bounds__(kRouteThreads, 1) arb_quote_kernel(const PathSets* __restrict__ P, PairIndexView ix,
+                                                                  RouteRows R) {
+  route_row<false, true>(P, ix, R, blockIdx.x, SplitMoved{});
+}
+
+__global__ void __launch_bounds__(kRouteThreads, 1) arb_execute_kernel(const PathSets* __restrict__ P, PairIndexView ix,
+                                                                    RouteRows R, const int64_t* __restrict__ rows,
+                                                                    SplitMoved mv) {
+  route_row<true, true>(P, ix, R, rows[blockIdx.x], mv);
 }
 
 }  // namespace cfmm

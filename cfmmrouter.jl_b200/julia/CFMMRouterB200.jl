@@ -512,6 +512,63 @@ execute_routed_orders!(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}, k
                        limit::Union{Nothing,Vector{Float64}}=nothing) =
     _routed_orders(:execute, ctx, token_in, token_out, kind, amount, hub_off, hubs, limit)
 
+# Arbitrage cycles through base tokens (cfmm_quote_arbitrage / cfmm_execute_arbitrage /
+# cfmm_scan_arbitrage).  Row r runs the cycles from base[r] through other[r] and back, directly and
+# through the hubs hubs[hub_off[r]+1 : hub_off[r+1]].  Returns (profit, surplus_in, price, status,
+# hub_price, hub_surplus, leg_delta, leg_lambda), legs in the pair order (other, base), (other, h₁),
+# (h₁, base), ….  scan_arbitrage returns (found, base, other, hub_off, hubs, profit, price) of the first
+# min(found, cap) rows.  Never executed, like the rest of this file.
+function _arbitrage(fn, ctx, base, other, hub_off, hubs, min_profit)
+    q = length(base)
+    length(other) == q && length(hub_off) == q + 1 ||
+        throw(ArgumentError("base / other need q entries, hub_off q + 1"))
+    min_profit === nothing || length(min_profit) == q || throw(ArgumentError("min_profit must have q entries"))
+    a, b = Int64[], Int64[]
+    for r in 1:q
+        push!(a, other[r]); push!(b, base[r])
+        for h in hubs[hub_off[r]+1:hub_off[r+1]]
+            push!(a, other[r], h); push!(b, h, base[r])
+        end
+    end
+    L = sum(pair_pools(ctx, a, b)[1]; init=0)
+    nh = length(hubs)
+    profit, surplus, price, status = zeros(q), zeros(q), zeros(q), zeros(UInt8, q)
+    hp, hs, ld, ll = zeros(nh), zeros(nh), zeros(2, L), zeros(2, L)
+    if fn === :quote
+        chk(ctx, ccall((:cfmm_quote_arbitrage, LIB), Cint,
+            (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64},
+             Ptr{Float64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+            ctx, q, base, other, hub_off, hubs, profit, surplus, price, status, hp, hs, ld, ll))
+    else
+        chk(ctx, ccall((:cfmm_execute_arbitrage, LIB), Cint,
+            (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64},
+             Ptr{Float64}, Ptr{Float64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+            ctx, q, base, other, min_profit === nothing ? C_NULL : min_profit, hub_off, hubs, profit, surplus,
+            price, status, hp, hs, ld, ll))
+    end
+    return profit, surplus, price, status, hp, hs, ld, ll
+end
+quote_arbitrage(ctx, base::Vector{Int64}, other::Vector{Int64}, hub_off::Vector{Int64}, hubs::Vector{Int64}) =
+    _arbitrage(:quote, ctx, base, other, hub_off, hubs, nothing)
+execute_arbitrage!(ctx, base::Vector{Int64}, other::Vector{Int64}, hub_off::Vector{Int64}, hubs::Vector{Int64},
+                   min_profit::Union{Nothing,Vector{Float64}}=nothing) =
+    _arbitrage(:execute, ctx, base, other, hub_off, hubs, min_profit)
+
+function scan_arbitrage(ctx, base::Vector{Int64}, min_profit::Vector{Float64}, max_hubs::Integer, cap::Integer)
+    length(min_profit) == length(base) || throw(ArgumentError("min_profit must have one entry per base token"))
+    found = Ref{Int64}(0)
+    rb, ro, hc = zeros(Int64, cap), zeros(Int64, cap), zeros(Int64, cap)
+    hb, pr, px = zeros(Int64, 7, cap), zeros(cap), zeros(cap)
+    chk(ctx, ccall((:cfmm_scan_arbitrage, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Float64}, Cint, Int64, Ref{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Int64},
+         Ptr{Int64}, Ptr{Float64}, Ptr{Float64}),
+        ctx, length(base), base, min_profit, max_hubs, cap, found, rb, ro, hc, hb, pr, px))
+    n = min(found[], cap)
+    hub_off = vcat(0, cumsum(hc[1:n]))
+    hubs = reduce(vcat, [hb[1:hc[r], r] for r in 1:n]; init=Int64[])
+    return found[], rb[1:n], ro[1:n], hub_off, hubs, pr[1:n], px[1:n]
+end
+
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
 # current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never

@@ -556,6 +556,89 @@ class DevicePools:
         paid); a row whose limit fails reverts.  Returns what quote_routed_orders returns."""
         return self._routed(True, token_in, token_out, kind, amount, hub_off, hubs, limit, legs)
 
+    # -- arbitrage cycles through base tokens (include/cfmm_b200.h, cfmm_quote_arbitrage /
+    #    cfmm_execute_arbitrage / cfmm_scan_arbitrage) -------------------------------------------
+    def _arbitrage(self, execute, base, other, hub_off, hubs, min_profit, legs):
+        base = np.ascontiguousarray(base, dtype=np.int64).reshape(-1)
+        other = np.ascontiguousarray(other, dtype=np.int64).reshape(-1)
+        hub_off = np.ascontiguousarray(hub_off, dtype=np.int64).reshape(-1)
+        hubs = np.ascontiguousarray(hubs, dtype=np.int64).reshape(-1)
+        q = len(base)
+        if len(other) != q or len(hub_off) != q + 1:
+            raise ValueError("arbitrage rows: base and other need one entry per row, hub_off q + 1")
+        if min_profit is not None:
+            min_profit = np.ascontiguousarray(min_profit, dtype=np.float64).reshape(-1)
+            if len(min_profit) != q:
+                raise ValueError(f"min_profit must have {q} entries, one per row")
+        nh = int(hub_off[-1]) if q else 0
+        if q and (hub_off[0] != 0 or np.any(np.diff(hub_off) < 0) or len(hubs) != nh):
+            raise ValueError("arbitrage rows: hub_off must rise from 0 to len(hubs)")
+        profit, surplus, price = np.zeros(q), np.zeros(q), np.zeros(q)
+        status = np.zeros(q, dtype=np.uint8)
+        hp, hs = np.zeros(nh), np.zeros(nh)
+        off = ld = ll = None
+        if legs:
+            off = np.zeros(1, dtype=np.int64)
+            if q:
+                a, b, first = self.route_pairs(other, base, hub_off, hubs)
+                off = self.pair_pools(a, b)[0][first]
+            ld, ll = np.zeros((int(off[-1]), 2)), np.zeros((int(off[-1]), 2))
+        u8 = C.POINTER(C.c_uint8)
+        args = [self._ctx, q, _ip(base), _ip(other)]
+        if execute:
+            args.append(None if min_profit is None else _dp(min_profit))
+        args += [_ip(hub_off) if q else None, _ip(hubs) if nh else None, _dp(profit), _dp(surplus), _dp(price),
+                 status.ctypes.data_as(u8), _dp(hp) if nh else None, _dp(hs) if nh else None,
+                 _dp(ld) if legs else None, _dp(ll) if legs else None]
+        fn = self._lib.cfmm_execute_arbitrage if execute else self._lib.cfmm_quote_arbitrage
+        self._chk(fn(*args))
+        out = (profit, surplus, price, status, hp, hs)
+        return out + ((off, ld, ll),) if legs else out
+
+    def quote_arbitrage(self, base, other, hub_off, hubs, legs: bool = False):
+        """cfmm_quote_arbitrage: row j runs the cycles from base[j] (1-based) through other[j] and back,
+        directly and through each hub of hubs[hub_off[j] .. hub_off[j+1]] (at most ROUTE_MAX_HUBS),
+        sized optimally (route! with BasketLiquidation(base, 0) over the row's pools).  Every row on
+        the current state on its own; no state changes.  Returns (profit [q] in the base token,
+        surplus_in [q] of other, price [q] = s*, status [q] uint8, hub_price [Σ], hub_surplus [Σ]) and,
+        with legs=True, also (off [q + 1], leg_delta [L, 2], leg_lambda [L, 2]) in the pair_pools order
+        of route_pairs(other, base, hub_off, hubs)."""
+        return self._arbitrage(False, base, other, hub_off, hubs, None, legs)
+
+    def execute_arbitrage(self, base, other, hub_off, hubs, min_profit=None, legs: bool = False):
+        """cfmm_execute_arbitrage: the rows of quote_arbitrage in batch order, each re-solved on the state
+        the earlier filled rows left; a row whose profit is below min_profit[j] (None: 0) reverts.
+        Returns what quote_arbitrage returns."""
+        return self._arbitrage(True, base, other, hub_off, hubs, min_profit, legs)
+
+    def scan_arbitrage(self, base, min_profit, max_hubs: int = _lib.ROUTE_MAX_HUBS, cap: int = None):
+        """cfmm_scan_arbitrage: the pair cycles and triangles through the distinct base tokens `base`
+        (1-based) that yield at least min_profit[b] (> 0, in base b's token) on the current state,
+        with up to max_hubs hubs per row, ordered by (base index, profit descending, other
+        ascending).  No state changes.  cap (None: every row found) bounds the rows returned.
+        Returns (found, row_base [n], row_other [n], hub_off [n + 1], hubs [Σ], profit [n],
+        price [n]) with n = min(found, cap); the rows go to execute_arbitrage as they are.  With
+        cap=None the scan runs twice: once to count, once to fetch."""
+        base = np.ascontiguousarray(base, dtype=np.int64).reshape(-1)
+        min_profit = np.ascontiguousarray(np.broadcast_to(np.asarray(min_profit, dtype=np.float64), base.shape))
+        found = np.zeros(1, dtype=np.int64)
+
+        def call(c):
+            rb, ro, hc = np.zeros(c, dtype=np.int64), np.zeros(c, dtype=np.int64), np.zeros(c, dtype=np.int64)
+            hb, pr, px = np.zeros((c, _lib.ROUTE_MAX_HUBS), dtype=np.int64), np.zeros(c), np.zeros(c)
+            self._chk(self._lib.cfmm_scan_arbitrage(self._ctx, len(base), _ip(base), _dp(min_profit), int(max_hubs), c,
+                                                    _ip(found), _ip(rb), _ip(ro), _ip(hc), _ip(hb), _dp(pr), _dp(px)))
+            return rb, ro, hc, hb, pr, px
+
+        out = call(max(0, int(cap)) if cap is not None else 0)
+        if cap is None and found[0] > 0:
+            out = call(int(found[0]))
+        n = min(int(found[0]), len(out[0]))
+        rb, ro, hc, hb, pr, px = (x[:n] for x in out)
+        hub_off = np.concatenate([[0], np.cumsum(hc)]).astype(np.int64)
+        hubs = np.concatenate([hb[r, :hc[r]] for r in range(n)]).astype(np.int64) if n else np.zeros(0, np.int64)
+        return int(found[0]), rb, ro, hub_off, hubs, pr, px
+
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
         """cfmm_modify_univ3_liquidity: row j adds dL[j] (> 0 mints, < 0 burns) to the ticks of UniV3
@@ -1031,6 +1114,65 @@ class Router:
             sub = np.concatenate([[0], np.cumsum(np.diff(off)[filled])]).astype(np.int64)
             fh = np.concatenate([flat[off[r]:off[r + 1]] for r in filled]).astype(np.int64)
             a, b, _ = DevicePools.route_pairs(tin[filled], tout[filled], sub, fh)
+            _, typ, idx, _ = self._pools.pair_pools(a, b)
+            self._refresh_swapped([(t, None, idx[typ == t]) for t in (0, 1, 2) if np.any(typ == t)])
+        return out
+
+    def _arbitrage_args(self, base, other, hubs, min_profit, what):
+        if self._world > 1:
+            raise NotImplementedError(f"{what} drives one GPU")
+        base, other = np.asarray(base).reshape(-1), np.asarray(other).reshape(-1)
+        if len(base) != len(other):
+            raise ValueError(f"{what}: base and other need one entry per row")
+        q = len(base)
+        if isinstance(hubs, tuple) and len(hubs) == 2:  # (hub_off, hubs) as scan_arbitrage returns them
+            hub_off, flat = (np.asarray(x, dtype=np.int64).reshape(-1) for x in hubs)
+        else:
+            per_row = [list(hubs)] * q if all(np.ndim(h) == 0 for h in hubs) else [list(h) for h in hubs]
+            if len(per_row) != q:
+                raise ValueError(f"{what}: hubs must be one list, or one list per row ({q})")
+            hub_off = np.concatenate([[0], np.cumsum([len(h) for h in per_row])]).astype(np.int64)
+            flat = np.array([int(x) for h in per_row for x in h], dtype=np.int64)
+        if min_profit is not None:
+            min_profit = np.asarray(min_profit, dtype=np.float64).reshape(-1)
+            if len(min_profit) != q:
+                raise ValueError(f"{what}: min_profit must have {q} entries")
+        return base, other, hub_off, flat, min_profit
+
+    def scan_arbitrage(self, base, min_profit, max_hubs: int = _lib.ROUTE_MAX_HUBS):
+        """Find the arbitrage cycles that start and end in one of the base tokens (1-based, distinct):
+        two pools of one pair that disagree (p → x → p) and triangles (p → x → y → p), each row (p, x)
+        sized optimally over its pair's pools and up to max_hubs triangles (cfmm_scan_arbitrage).  Keeps
+        the rows whose profit reaches min_profit (one value, or one per base token, in units of that
+        base token), ordered by (base, profit descending, x).  No state changes.  Returns (row_base [n],
+        row_other [n], (hub_off [n + 1], hubs [Σ]), profit [n], price [n]); pass the first three to
+        execute_arbitrage with the minimum profits to close them.  Single GPU."""
+        if self._world > 1:
+            raise NotImplementedError("scan_arbitrage drives one GPU")
+        _, rb, ro, hub_off, hubs, profit, price = self._pools.scan_arbitrage(base, min_profit, max_hubs)
+        return rb, ro, (hub_off, hubs), profit, price
+
+    def quote_arbitrage(self, base, other, hubs):
+        """Size the cycles from base[j] through other[j] and back, directly and through each hub of
+        `hubs` (one list for every row, one list per row, or (hub_off, hubs) as scan_arbitrage returns
+        them), as route! with BasketLiquidation(base, 0) over the row's pools (cfmm_quote_arbitrage).
+        Every row on the current state on its own.  Returns (profit [q], surplus_in [q], price [q],
+        status [q]).  Single GPU."""
+        base, other, off, flat, _ = self._arbitrage_args(base, other, hubs, None, "quote_arbitrage")
+        return self._pools.quote_arbitrage(base, other, off, flat)[:4]
+
+    def execute_arbitrage(self, base, other, hubs, min_profit=None):
+        """Run arbitrage rows in order (cfmm_execute_arbitrage), each re-solved on the state the earlier
+        rows left; a row whose profit is below min_profit[j] (None: 0) reverts.  Returns what
+        quote_arbitrage returns and refreshes the pool objects of the filled rows' pairs from the
+        device state, as execute_routed_orders does.  Single GPU."""
+        base, other, off, flat, min_profit = self._arbitrage_args(base, other, hubs, min_profit, "execute_arbitrage")
+        out = self._pools.execute_arbitrage(base, other, off, flat, min_profit)[:4]
+        filled = np.flatnonzero(out[3] == _lib.ORDER_FILLED)
+        if len(filled):
+            sub = np.concatenate([[0], np.cumsum(np.diff(off)[filled])]).astype(np.int64)
+            fh = np.concatenate([flat[off[r]:off[r + 1]] for r in filled]).astype(np.int64)
+            a, b, _ = DevicePools.route_pairs(other[filled], base[filled], sub, fh)
             _, typ, idx, _ = self._pools.pair_pools(a, b)
             self._refresh_swapped([(t, None, idx[typ == t]) for t in (0, 1, 2) if np.any(typ == t)])
         return out

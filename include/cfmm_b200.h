@@ -585,6 +585,81 @@ int cfmm_execute_routed_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_in
                                uint8_t *status, double *hub_price, double *hub_surplus,
                                double *leg_delta, double *leg_lambda);
 
+/* ---- arbitrage: pair cycles and triangles through base tokens --------------------------------
+ * An arbitrage row names a base token p = base[r] (the profit token), another token x = other[r]
+ * (1-based, distinct) and hubs y = hubs[hub_off[r] .. hub_off[r+1]) with routed rows' rules (at most
+ * CFMM_ROUTE_MAX_HUBS, distinct, neither p nor x).  Its pools are those of {x, p}, {x, y} and {y, p}:
+ * the pair cycle p → x → p and one triangle p → x → y → p (either direction) per hub.  The row is
+ * route! with BasketLiquidation(p, 0) over these pools: maximise the output of p while x and every y
+ * end non-negative.  That is the routed exact-in row j = x, i = p with δ = 0, and its dual separates
+ * in the same way, so the row runs routed rows' searches (start, gallop, bisection, inner hub
+ * searches, sums and their order, UNREACHABLE rules) with enough(s) = N(s) > 0 (a NaN counts as
+ * true) and s* = hi.  It runs the search where a routed row with amount 0 does not, and a row whose
+ * pair {x, p} no pool holds is CFMM_ORDER_UNREACHABLE.
+ *
+ * Outputs, each optional (NULL), per row: profit = O(s*), the p the cycle yields; surplus_in =
+ * 0.0 − N(s*) >= 0 (one IEEE subtraction), the x left with the trader; price = s* (0 when
+ * unreachable); status; hub_price [Σ] = t_h*, hub_surplus [Σ] = H_h(t_h*) >= 0; legs leg_delta,
+ * leg_lambda [2L] in routed rows' list order ({x, p}, {x, y₁}, {y₁, p}, …).  Rows that do not fill
+ * report 0 for profit, surplus and the legs.  With no arbitrage left, the row fills with profit 0.
+ * By weak duality O >= s·N − Σ t_h·H_h, so rounding can leave a filled profit a few ulps below 0.
+ *
+ * cfmm_quote_arbitrage prices every row on the current state on its own; no state changes.
+ * cfmm_execute_arbitrage runs the rows in batch order, each on the state the earlier filled rows
+ * left, with routed rows' levels, transitions and bookkeeping.  min_profit [q] (NULL: 0) is each
+ * row's limit: a row with profit < min_profit reverts with CFMM_ORDER_LIMIT (an equal value fills).
+ *
+ * cfmm_scan_arbitrage finds the rows worth running for distinct base tokens base[nb], each with
+ * min_profit[b] (finite, > 0, in units of that base token), with up to max_hubs (0..7) hubs per row.
+ * It changes no state and is synchronous.  Its steps:
+ *   adjacency  for every distinct token pair {a, b} of the pools (retired included), the entries
+ *            a → b and b → a sorted by (token, neighbour); built on the device with the pair index
+ *            (first use after cfmm_finalize, cfmm_append_* or cfmm_compact; kept across retire and
+ *            restore).  2·n_pairs entries of 8 bytes.
+ *   rates    r(a → b) = the largest, over the active pools of {a, b}, of the start boundary of
+ *            routed rows with a in j's role (ProductTwoCoin (γ·R_b)/R_a, GeometricMeanTwoCoin
+ *            ((γ·w_a)·R_b)/(w_b·R_a), UniV3 γ·q when a is its token 1, γ/q otherwise); NaNs are
+ *            ignored; 0 when no pool of the pair is active.  Per call: rates depend on the state.
+ *   screen   for each base p and each neighbour x of p: the pair score fl(r(p→x)·r(x→p)), and for
+ *            every common neighbour y of p and x the triangle score, the larger of those of
+ *            fl(fl(r(p→x)·r(x→y))·r(y→p)) and fl(fl(r(p→y)·r(y→x))·r(x→p)) that pass.  A score
+ *            passes when > 1 − 2⁻⁴⁰.  The row's hubs are the first max_hubs passing triangles in
+ *            (score descending, y ascending) order.  A row (p, x, hubs) is a candidate when its
+ *            pair score or at least one triangle passes; candidates are ordered by (base index, x).
+ *   solve    every candidate is quoted as cfmm_quote_arbitrage would quote it.
+ *   select   the candidates that fill with profit >= min_profit[base], ordered by (base index,
+ *            profit descending, x ascending); *found is their number.
+ * The first min(*found, cap) rows are written: row_base, row_other, hub_count [cap], hubs
+ * [cap × CFMM_ROUTE_MAX_HUBS] (1-based, best first, zero-padded), profit and price [cap].  The screen
+ * is conservative: a profitable cycle's exact rate product exceeds 1, and the bests of a pool's two
+ * directions multiply to γ² <= 1.  Passing rows to cfmm_execute_arbitrage with their minimum profits
+ * closes the opportunities; each row is re-solved on the state the rows before it left, so rows that
+ * share pools shrink or revert instead of spending twice.
+ *
+ * Before cfmm_finalize: CFMM_ERR_STATE.  q == 0 / nb == 0 do nothing (*found = 0).
+ * CFMM_ERR_INVALID before anything runs for: rows: q < 0, a null base or other, tokens outside
+ * 1..n_tokens or base == other, routed rows' hub rejections, a min_profit that is NaN, negative or
+ * +inf.  Scan: nb < 0, cap < 0, a null found, base tokens outside 1..n_tokens or repeated, a
+ * min_profit that is <= 0, NaN or Inf, max_hubs outside 0..CFMM_ROUTE_MAX_HUBS, a null base or
+ * min_profit with nb > 0, a null output with cap > 0. */
+int cfmm_quote_arbitrage(cfmm_ctx *ctx, int64_t q, const int64_t *base /* [q] */,
+                         const int64_t *other /* [q] */, const int64_t *hub_off /* [q+1] */,
+                         const int64_t *hubs /* [Σ] */, double *profit /* [q] */,
+                         double *surplus_in /* [q] */, double *price /* [q] */,
+                         uint8_t *status /* [q] */, double *hub_price /* [Σ] */,
+                         double *hub_surplus /* [Σ] */, double *leg_delta /* [2L] */,
+                         double *leg_lambda /* [2L] */);
+int cfmm_execute_arbitrage(cfmm_ctx *ctx, int64_t q, const int64_t *base, const int64_t *other,
+                           const double *min_profit /* [q] or NULL */, const int64_t *hub_off,
+                           const int64_t *hubs, double *profit, double *surplus_in, double *price,
+                           uint8_t *status, double *hub_price, double *hub_surplus,
+                           double *leg_delta, double *leg_lambda);
+int cfmm_scan_arbitrage(cfmm_ctx *ctx, int64_t nb, const int64_t *base /* [nb] */,
+                        const double *min_profit /* [nb] */, int max_hubs, int64_t cap,
+                        int64_t *found, int64_t *row_base /* [cap] */, int64_t *row_other /* [cap] */,
+                        int64_t *hub_count /* [cap] */, int64_t *hubs /* [cap × 7] */,
+                        double *profit /* [cap] */, double *price /* [cap] */);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
