@@ -20,7 +20,10 @@
 #include <functional>
 #include <memory>
 #include <new>
+#include <numeric>
+#include <optional>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -67,11 +70,14 @@ struct DevBuf {
     if (e == cudaSuccess) n = count;
     return e;
   }
-  cudaError_t upload(const std::vector<T>& h) {
-    cudaError_t e = alloc(h.size());
-    if (e != cudaSuccess || h.empty()) return e;
-    return copy_in(p, h.data(), h.size() * sizeof(T));
+  // alloc + copy_in of count host elements; a null h or count == 0 leaves the buffer empty (an
+  // optional argument not given)
+  cudaError_t upload(const T* h, size_t count) {
+    cudaError_t e = alloc(h ? count : 0);
+    if (e != cudaSuccess || !h || count == 0) return e;
+    return copy_in(p, h, count * sizeof(T));
   }
+  cudaError_t upload(const std::vector<T>& h) { return upload(h.data(), h.size()); }
   // H2D from pageable memory, COMPLETE on return.  cudaMemcpy alone is not: for pageable sources
   // it returns once the data sits in the driver's staging buffer, the DMA may still be in flight --
   // and the contexts' streams are non-blocking, so a kernel launched on them right afterwards does
@@ -756,6 +762,37 @@ struct ProfScope {
     }
   }
 };
+
+constexpr int kProfSwaps = 4;  // cfmm_profile_read: the slot of the swap, path, order and arbitrage kernels
+constexpr int kNoProf = -1;    // launch: not timed
+
+// One launch site on ctx->stream: enqueue() enqueues the site's n kernels, timed as one profile
+// entry of slot prof (kNoProf: not timed).  enqueue returns void, or an int status when it also
+// makes library calls that can fail (cub).
+template <class F>
+int launch(cfmm_ctx* ctx, int prof, int64_t n, F&& enqueue) {
+  int rc = CFMM_OK;
+  {
+    std::optional<ProfScope> scope;
+    if (prof != kNoProf) scope.emplace(ctx, prof, ctx->stream);
+    if constexpr (std::is_void_v<decltype(enqueue())>)
+      enqueue();
+    else
+      rc = enqueue();
+  }
+  if (rc != CFMM_OK) return rc;
+  ctx->launches += n;
+  CU_TRY(ctx, cudaGetLastError());
+  return CFMM_OK;
+}
+
+// Async D2H copy of n elements on ctx->stream, skipped when dst is null (an output not asked for)
+// or n == 0.
+template <class T>
+cudaError_t read_back(cfmm_ctx* ctx, T* dst, const T* src, size_t n) {
+  if (!dst || n == 0) return cudaSuccess;
+  return cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream);
+}
 
 template <class P>
 int launch_sweep(cfmm_ctx* ctx, int ptype, const P& pools, PoolSet& s,
@@ -1974,9 +2011,7 @@ int update_reserves_set(cfmm_ctx* ctx, PoolSet& s, int64_t first, int64_t count,
   DevBuf<double2> d_new;
   DevBuf<int64_t> d_pos;
   CU_TRY(ctx, d_new.upload(newR));
-  cudaError_t e = d_pos.alloc((size_t)count);
-  if (e == cudaSuccess)
-    e = DevBuf<int64_t>::copy_in(d_pos.p, s.pos_of.data() + first, (size_t)count * sizeof(int64_t));
+  cudaError_t e = d_pos.upload(s.pos_of.data() + first, (size_t)count);
   if (e == cudaSuccess) {
     const int threads = 256;
     cfmm::update_reserves_kernel<<<(unsigned)((count + threads - 1) / threads), threads, 0,
@@ -2029,14 +2064,8 @@ int univ3_update_listed(cfmm_ctx* ctx, PoolSet& s, const std::vector<int64_t>& p
   DevBuf<double> d_price, d_liq;
   CU_TRY(ctx, d_pos.upload(pos));
   CU_TRY(ctx, d_cum.upload(cum));
-  if (price) {
-    CU_TRY(ctx, d_price.alloc((size_t)count));
-    CU_TRY(ctx, DevBuf<double>::copy_in(d_price.p, price, (size_t)count * sizeof(double)));
-  }
-  if (liq && n_ticks > 0) {
-    CU_TRY(ctx, d_liq.alloc((size_t)n_ticks));
-    CU_TRY(ctx, DevBuf<double>::copy_in(d_liq.p, liq, (size_t)n_ticks * sizeof(double)));
-  }
+  CU_TRY(ctx, d_price.upload(price, (size_t)count));
+  CU_TRY(ctx, d_liq.upload(liq, (size_t)n_ticks));
   CU_TRY(ctx, univ3_rebuild(ctx, s, d_pos.p, d_cum.p, count, n_ticks, d_price.p, d_liq.p, new_tick));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return CFMM_OK;
@@ -2399,13 +2428,13 @@ int cfmm_get_pool_state(cfmm_ctx* ctx, int type, int64_t first, int64_t count, d
     CU_TRY(ctx, d_pos.upload(pos));
     CU_TRY(ctx, d_out.alloc((size_t)(width * sp.count)));
     const int threads = 256;
-    cfmm::gather_state_kernel<<<(unsigned)((sp.count + threads - 1) / threads), threads, 0, ctx->stream>>>(
-        s.d_R.p, s.d_park.p, s.d_active.p, type == CFMM_POOL_UNIV3 ? s.d_first[1].p : nullptr, s.d_gidx.p, d_pos.p,
-        sp.count, d_out.p);
-    ctx->launches++;
-    CU_TRY(ctx, cudaGetLastError());
-    CU_TRY(ctx, cudaMemcpyAsync(state + width * sp.offset, d_out.p, (size_t)(width * sp.count) * sizeof(double),
-                                cudaMemcpyDeviceToHost, ctx->stream));
+    if ((rc = launch(ctx, kNoProf, 1, [&] {
+           cfmm::gather_state_kernel<<<(unsigned)((sp.count + threads - 1) / threads), threads, 0, ctx->stream>>>(
+               s.d_R.p, s.d_park.p, s.d_active.p, type == CFMM_POOL_UNIV3 ? s.d_first[1].p : nullptr, s.d_gidx.p,
+               d_pos.p, sp.count, d_out.p);
+         })) != CFMM_OK)
+      return rc;
+    CU_TRY(ctx, read_back(ctx, state + width * sp.offset, d_out.p, (size_t)(width * sp.count)));
     CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     if (active)
       for (int64_t j = 0; j < sp.count; ++j)
@@ -2442,8 +2471,6 @@ int check_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const d
   return CFMM_OK;
 }
 
-constexpr int kProfSwaps = 4;  // cfmm_profile_read: the swap kernels' slot
-
 cfmm::SwapSet swap_set(PoolSet& s) {
   cfmm::SwapSet w;
   w.R = s.d_R.p;
@@ -2473,45 +2500,52 @@ std::vector<SetRows> rows_by_set(cfmm_ctx* ctx, int type, int64_t q, const int64
   return out;
 }
 
-// The rows of one set grouped by pool, batch order kept inside each pool: pos[j] is the j-th
-// touched device position (ascending), rows[off[j] .. off[j+1]) its row indices.  A stable
-// counting sort on the device position (a stable comparison sort when the batch is small against
-// the set).
-struct PoolGroups {
-  std::vector<int64_t> pos, off, rows;
+// A stable group by key: key[g] is the g-th distinct key (ascending), rows[off[g] .. off[g+1]) the
+// values of its entries in batch order: val[j] for entry j (j itself when val is null).  Keys lie in
+// -1 .. n_keys - 1, and every entry of key -1 is a group of its own.  A counting sort on the key
+// when the batch is large against the key range, a stable comparison sort otherwise.
+struct Groups {
+  std::vector<int64_t> key, off, rows;
 };
 
-PoolGroups group_by_pool(const SetRows& r, int64_t m_padded) {
-  const int64_t n = (int64_t)r.row.size();
-  PoolGroups g;
+Groups group_by_key(const std::vector<int64_t>& key, int64_t n_keys, const std::vector<int64_t>* val = nullptr) {
+  const int64_t n = (int64_t)key.size();
+  const auto value = [&](int64_t j) { return val ? (*val)[(size_t)j] : j; };
+  Groups g;
   g.rows.resize((size_t)n);
-  if (n * 8 >= m_padded) {
-    std::vector<int64_t> start((size_t)m_padded + 1, 0);
-    for (int64_t j = 0; j < n; ++j) start[(size_t)r.pos[(size_t)j] + 1]++;
-    for (int64_t p = 0; p < m_padded; ++p) {
-      if (start[(size_t)p + 1] > 0) {
-        g.pos.push_back(p);
-        g.off.push_back(start[(size_t)p]);
+  if (n * 8 >= n_keys) {
+    // slot s = key + 1; start[s + 1] counts the slot's entries, then start[s] is its first row
+    std::vector<int64_t> start((size_t)n_keys + 2, 0);
+    for (int64_t j = 0; j < n; ++j) start[(size_t)(key[(size_t)j] + 2)]++;
+    for (int64_t s = 0; s <= n_keys; ++s) {
+      const int64_t c = start[(size_t)s + 1];
+      for (int64_t i = 0; i < c; i += s == 0 ? 1 : c) {
+        g.key.push_back(s - 1);
+        g.off.push_back(start[(size_t)s] + i);
       }
-      start[(size_t)p + 1] += start[(size_t)p];
+      start[(size_t)s + 1] += start[(size_t)s];
     }
-    for (int64_t j = 0; j < n; ++j) g.rows[(size_t)start[(size_t)r.pos[(size_t)j]]++] = r.row[(size_t)j];
+    for (int64_t j = 0; j < n; ++j) g.rows[(size_t)start[(size_t)(key[(size_t)j] + 1)]++] = value(j);
   } else {
     std::vector<int64_t> idx((size_t)n);
-    for (int64_t j = 0; j < n; ++j) idx[(size_t)j] = j;
-    std::stable_sort(idx.begin(), idx.end(), [&](int64_t a, int64_t b) { return r.pos[(size_t)a] < r.pos[(size_t)b]; });
+    std::iota(idx.begin(), idx.end(), (int64_t)0);
+    std::stable_sort(idx.begin(), idx.end(), [&](int64_t a, int64_t b) { return key[(size_t)a] < key[(size_t)b]; });
     for (int64_t j = 0; j < n; ++j) {
-      const int64_t p = r.pos[(size_t)idx[(size_t)j]];
-      if (g.pos.empty() || g.pos.back() != p) {
-        g.pos.push_back(p);
+      const int64_t k = key[(size_t)idx[(size_t)j]];
+      if (j == 0 || k < 0 || k != g.key.back()) {
+        g.key.push_back(k);
         g.off.push_back(j);
       }
-      g.rows[(size_t)j] = r.row[(size_t)idx[(size_t)j]];
+      g.rows[(size_t)j] = value(idx[(size_t)j]);
     }
   }
   g.off.push_back(n);
   return g;
 }
+
+// The rows of one set grouped by pool: key[g] is the g-th touched device position, rows the call's
+// row indices.
+Groups group_by_pool(const SetRows& r, int64_t m_padded) { return group_by_key(r.pos, m_padded, &r.row); }
 
 // After an execute kernel on set s: the derived state of the UniV3 pools it listed in d_moved
 // (d_n_moved of them) is rebuilt as after cfmm_apply_trades; for two-coin sets a raised d_flag
@@ -2521,8 +2555,8 @@ int swap_bookkeeping(cfmm_ctx* ctx, PoolSet& s, int type, const int64_t* d_moved
   int rc = CFMM_OK;
   unsigned long long h_moved = 0;
   int h_flag = 0;
-  CU_TRY(ctx, cudaMemcpyAsync(&h_moved, d_n_moved, sizeof(h_moved), cudaMemcpyDeviceToHost, ctx->stream));
-  CU_TRY(ctx, cudaMemcpyAsync(&h_flag, d_flag, sizeof(h_flag), cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, read_back(ctx, &h_moved, d_n_moved, 1));
+  CU_TRY(ctx, read_back(ctx, &h_flag, d_flag, 1));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   if (type == CFMM_POOL_UNIV3) {
     if (h_moved > 0) {  // the derived state of the pools that moved, as after cfmm_apply_trades
@@ -2539,26 +2573,48 @@ int swap_bookkeeping(cfmm_ctx* ctx, PoolSet& s, int type, const int64_t* d_moved
   return CFMM_OK;
 }
 
-}  // namespace
+// The kinds, amounts and limits of order rows (noun: "row" or "path"); amount and limit may be null
+// (amounts checked elsewhere; no limits).
+int check_order_row(cfmm_ctx* ctx, const char* what, const char* noun, int64_t j, const uint8_t* kind,
+                    const double* amount, const double* limit) {
+  if (kind[j] != CFMM_SWAP_EXACT_IN && kind[j] != CFMM_SWAP_EXACT_OUT)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: %s %lld: kind %d is neither exact-in (0) nor exact-out (1)", what, noun,
+                (long long)j, (int)kind[j]);
+  if (amount && (!std::isfinite(amount[j]) || amount[j] < 0.0))
+    return fail(ctx, CFMM_ERR_INVALID, "%s: %s %lld: amount %g must be finite and >= 0", what, noun, (long long)j,
+                amount[j]);
+  if (!limit) return CFMM_OK;
+  if (std::isnan(limit[j]) || limit[j] < 0.0)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: %s %lld: limit %g must be >= 0", what, noun, (long long)j, limit[j]);
+  if (std::isinf(limit[j]) && kind[j] == CFMM_SWAP_EXACT_IN)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: %s %lld: an exact-in %s's minimum received must be finite", what, noun,
+                (long long)j, noun);
+  return CFMM_OK;
+}
 
-// launch KERNEL<type> (the pool type as a template argument) with the arguments that follow
-#define CFMM_SWAP_LAUNCH(type, KERNEL, blocks, st, ...)                                      \
-  do {                                                                                        \
-    if ((type) == CFMM_POOL_PRODUCT) KERNEL<0><<<(blocks), 256, 0, (st)>>>(__VA_ARGS__);      \
-    else if ((type) == CFMM_POOL_GEOMEAN) KERNEL<1><<<(blocks), 256, 0, (st)>>>(__VA_ARGS__); \
-    else KERNEL<2><<<(blocks), 256, 0, (st)>>>(__VA_ARGS__);                                  \
-  } while (0)
+extern "C++" {  // (templates, inside the file's extern "C" block)
 
-int cfmm_quote_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const double* tender,
-                     double* received) {
-  int rc = check_swaps(ctx, type, q, pool, tender, received, true, "quote_swaps");
-  if (rc != CFMM_OK || q == 0) return rc;
+// Launch the swap kernel of the given pool type on `blocks` blocks of 256 threads: kernel(T) is its
+// instantiation for pool type T (a std::integral_constant).
+template <class Kernel, class... Args>
+void swap_launch(int type, Kernel kernel, unsigned blocks, cudaStream_t st, Args... args) {
+  const auto k = type == CFMM_POOL_PRODUCT   ? kernel(std::integral_constant<int, 0>{})
+                 : type == CFMM_POOL_GEOMEAN ? kernel(std::integral_constant<int, 1>{})
+                                             : kernel(std::integral_constant<int, 2>{});
+  k<<<blocks, 256, 0, st>>>(args...);
+}
+
+// cfmm_quote_swaps and cfmm_quote_swaps_exact_out: rows (pool, in [2]) priced on the current state on
+// their own, out [2] per row; one launch per set.
+template <class Kernel>
+int quote_swap_rows(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const double* in, double* out,
+                    Kernel kernel) {
+  int rc;
   CU_TRY(ctx, cudaSetDevice(ctx->device));
   if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
-  DevBuf<double> d_tender, d_recv;
-  CU_TRY(ctx, d_tender.alloc((size_t)(2 * q)));
-  CU_TRY(ctx, DevBuf<double>::copy_in(d_tender.p, tender, (size_t)(2 * q) * sizeof(double)));
-  CU_TRY(ctx, d_recv.alloc((size_t)(2 * q)));
+  DevBuf<double> d_in, d_out;
+  CU_TRY(ctx, d_in.upload(in, (size_t)(2 * q)));
+  CU_TRY(ctx, d_out.alloc((size_t)(2 * q)));
   for (SetRows& r : rows_by_set(ctx, type, q, pool)) {
     const int64_t n = (int64_t)r.row.size();
     if (n == 0) continue;
@@ -2566,20 +2622,69 @@ int cfmm_quote_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, co
     CU_TRY(ctx, d_row.upload(r.row));
     CU_TRY(ctx, d_pos.upload(r.pos));
     const cfmm::SwapSet ss = swap_set(*r.s);
-    const unsigned blocks = (unsigned)((n + 255) / 256);
-    {
-      ProfScope prof(ctx, kProfSwaps, ctx->stream);
-      CFMM_SWAP_LAUNCH(type, cfmm::swap_quote_kernel, blocks, ctx->stream, ss, d_row.p, d_pos.p, n, d_tender.p,
-                       d_recv.p);
-    }
-    ctx->launches++;
-    CU_TRY(ctx, cudaGetLastError());
+    if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+           swap_launch(type, kernel, (unsigned)((n + 255) / 256), ctx->stream, ss, d_row.p, d_pos.p, n, d_in.p,
+                       d_out.p);
+         })) != CFMM_OK)
+      return rc;
     CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // (d_row, d_pos are freed at the end of the block)
   }
-  CU_TRY(ctx, cudaMemcpyAsync(received, d_recv.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
-                              ctx->stream));
+  CU_TRY(ctx, read_back(ctx, out, d_out.p, (size_t)(2 * q)));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return CFMM_OK;
+}
+
+// cfmm_execute_swaps and cfmm_execute_swap_orders: per set, the rows grouped by pool (a thread per
+// touched pool runs its rows in batch order), one launch with the row arrays `rows`, then
+// swap_bookkeeping.
+template <class Kernel, class... Rows>
+int execute_swap_rows(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, Kernel kernel, Rows... rows) {
+  int rc;
+  for (SetRows& r : rows_by_set(ctx, type, q, pool)) {
+    PoolSet& s = *r.s;
+    if (r.row.empty()) continue;
+    const Groups seg = group_by_pool(r, s.m_padded);
+    const int64_t n_seg = (int64_t)seg.key.size();
+    DevBuf<int64_t> d_seg_pos, d_seg_off, d_seg_rows, d_moved;
+    DevBuf<unsigned long long> d_n_moved;
+    DevBuf<int> d_flag;
+    CU_TRY(ctx, d_seg_pos.upload(seg.key));
+    CU_TRY(ctx, d_seg_off.upload(seg.off));
+    CU_TRY(ctx, d_seg_rows.upload(seg.rows));
+    CU_TRY(ctx, d_n_moved.alloc(1));
+    CU_TRY(ctx, d_flag.alloc(1));
+    if (type == CFMM_POOL_UNIV3) CU_TRY(ctx, d_moved.alloc((size_t)n_seg));
+    CU_TRY(ctx, cudaMemsetAsync(d_n_moved.p, 0, sizeof(unsigned long long), ctx->stream));
+    CU_TRY(ctx, cudaMemsetAsync(d_flag.p, 0, sizeof(int), ctx->stream));
+    const cfmm::SwapSet ss = swap_set(s);
+    if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+           swap_launch(type, kernel, (unsigned)((n_seg + 255) / 256), ctx->stream, ss, d_seg_pos.p, d_seg_off.p,
+                       d_seg_rows.p, n_seg, rows..., d_moved.p, d_n_moved.p, d_flag.p);
+         })) != CFMM_OK)
+      return rc;
+    if ((rc = swap_bookkeeping(ctx, s, type, d_moved.p, d_n_moved.p, d_flag.p)) != CFMM_OK) return rc;
+  }
+  return CFMM_OK;
+}
+
+}  // extern "C++"
+
+}  // namespace
+
+int cfmm_quote_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const double* tender,
+                     double* received) {
+  int rc = check_swaps(ctx, type, q, pool, tender, received, true, "quote_swaps");
+  if (rc != CFMM_OK || q == 0) return rc;
+  return quote_swap_rows(ctx, type, q, pool, tender, received,
+                         [](auto t) { return cfmm::swap_quote_kernel<decltype(t)::value>; });
+}
+
+int cfmm_quote_swaps_exact_out(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const double* want,
+                               double* tender) {
+  int rc = check_swaps(ctx, type, q, pool, want, tender, true, "quote_swaps_exact_out");
+  if (rc != CFMM_OK || q == 0) return rc;
+  return quote_swap_rows(ctx, type, q, pool, want, tender,
+                         [](auto t) { return cfmm::swap_quote_exact_out_kernel<decltype(t)::value>; });
 }
 
 int cfmm_execute_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const double* tender,
@@ -2590,40 +2695,13 @@ int cfmm_execute_swaps(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, 
   if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
   ctx->state_version++;
   DevBuf<double> d_tender, d_recv;
-  CU_TRY(ctx, d_tender.alloc((size_t)(2 * q)));
-  CU_TRY(ctx, DevBuf<double>::copy_in(d_tender.p, tender, (size_t)(2 * q) * sizeof(double)));
+  CU_TRY(ctx, d_tender.upload(tender, (size_t)(2 * q)));
   CU_TRY(ctx, d_recv.alloc((size_t)(2 * q)));
-  for (SetRows& r : rows_by_set(ctx, type, q, pool)) {
-    PoolSet& s = *r.s;
-    const int64_t n = (int64_t)r.row.size();
-    if (n == 0) continue;
-    const PoolGroups seg = group_by_pool(r, s.m_padded);
-    const int64_t n_seg = (int64_t)seg.pos.size();
-    DevBuf<int64_t> d_seg_pos, d_seg_off, d_seg_rows, d_moved;
-    DevBuf<unsigned long long> d_n_moved;
-    DevBuf<int> d_flag;
-    CU_TRY(ctx, d_seg_pos.upload(seg.pos));
-    CU_TRY(ctx, d_seg_off.upload(seg.off));
-    CU_TRY(ctx, d_seg_rows.upload(seg.rows));
-    CU_TRY(ctx, d_n_moved.alloc(1));
-    CU_TRY(ctx, d_flag.alloc(1));
-    if (type == CFMM_POOL_UNIV3) CU_TRY(ctx, d_moved.alloc((size_t)n_seg));
-    CU_TRY(ctx, cudaMemsetAsync(d_n_moved.p, 0, sizeof(unsigned long long), ctx->stream));
-    CU_TRY(ctx, cudaMemsetAsync(d_flag.p, 0, sizeof(int), ctx->stream));
-    const cfmm::SwapSet ss = swap_set(s);
-    const unsigned blocks = (unsigned)((n_seg + 255) / 256);
-    {
-      ProfScope prof(ctx, kProfSwaps, ctx->stream);
-      CFMM_SWAP_LAUNCH(type, cfmm::swap_execute_kernel, blocks, ctx->stream, ss, d_seg_pos.p, d_seg_off.p,
-                       d_seg_rows.p, n_seg, d_tender.p, d_recv.p, d_moved.p, d_n_moved.p, d_flag.p);
-    }
-    ctx->launches++;
-    CU_TRY(ctx, cudaGetLastError());
-    if ((rc = swap_bookkeeping(ctx, s, type, d_moved.p, d_n_moved.p, d_flag.p)) != CFMM_OK) return rc;
-  }
-  if (received)
-    CU_TRY(ctx, cudaMemcpyAsync(received, d_recv.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
-                                ctx->stream));
+  if ((rc = execute_swap_rows(ctx, type, q, pool,
+                              [](auto t) { return cfmm::swap_execute_kernel<decltype(t)::value>; }, d_tender.p,
+                              d_recv.p)) != CFMM_OK)
+    return rc;
+  CU_TRY(ctx, read_back(ctx, received, d_recv.p, (size_t)(2 * q)));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return CFMM_OK;
 }
@@ -2635,54 +2713,13 @@ namespace {
 int check_orders(cfmm_ctx* ctx, int64_t q, const uint8_t* kind, const double* limit) {
   if (q > 0 && !kind) return fail(ctx, CFMM_ERR_INVALID, "execute_swap_orders: null kind array");
   for (int64_t j = 0; j < q; ++j) {
-    if (kind[j] != CFMM_SWAP_EXACT_IN && kind[j] != CFMM_SWAP_EXACT_OUT)
-      return fail(ctx, CFMM_ERR_INVALID, "execute_swap_orders: row %lld: kind %d is neither exact-in (0) nor exact-out (1)",
-                  (long long)j, (int)kind[j]);
-    if (!limit) continue;
-    const double l = limit[j];
-    if (std::isnan(l) || l < 0.0)
-      return fail(ctx, CFMM_ERR_INVALID, "execute_swap_orders: row %lld: limit %g must be >= 0", (long long)j, l);
-    if (std::isinf(l) && kind[j] == CFMM_SWAP_EXACT_IN)
-      return fail(ctx, CFMM_ERR_INVALID, "execute_swap_orders: row %lld: an exact-in row's minimum received must be finite",
-                  (long long)j);
+    const int rc = check_order_row(ctx, "execute_swap_orders", "row", j, kind, nullptr, limit);
+    if (rc != CFMM_OK) return rc;
   }
   return CFMM_OK;
 }
 
 }  // namespace
-
-int cfmm_quote_swaps_exact_out(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const double* want,
-                               double* tender) {
-  int rc = check_swaps(ctx, type, q, pool, want, tender, true, "quote_swaps_exact_out");
-  if (rc != CFMM_OK || q == 0) return rc;
-  CU_TRY(ctx, cudaSetDevice(ctx->device));
-  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
-  DevBuf<double> d_want, d_tender;
-  CU_TRY(ctx, d_want.alloc((size_t)(2 * q)));
-  CU_TRY(ctx, DevBuf<double>::copy_in(d_want.p, want, (size_t)(2 * q) * sizeof(double)));
-  CU_TRY(ctx, d_tender.alloc((size_t)(2 * q)));
-  for (SetRows& r : rows_by_set(ctx, type, q, pool)) {
-    const int64_t n = (int64_t)r.row.size();
-    if (n == 0) continue;
-    DevBuf<int64_t> d_row, d_pos;
-    CU_TRY(ctx, d_row.upload(r.row));
-    CU_TRY(ctx, d_pos.upload(r.pos));
-    const cfmm::SwapSet ss = swap_set(*r.s);
-    const unsigned blocks = (unsigned)((n + 255) / 256);
-    {
-      ProfScope prof(ctx, kProfSwaps, ctx->stream);
-      CFMM_SWAP_LAUNCH(type, cfmm::swap_quote_exact_out_kernel, blocks, ctx->stream, ss, d_row.p, d_pos.p, n,
-                       d_want.p, d_tender.p);
-    }
-    ctx->launches++;
-    CU_TRY(ctx, cudaGetLastError());
-    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // (d_row, d_pos are freed at the end of the block)
-  }
-  CU_TRY(ctx, cudaMemcpyAsync(tender, d_tender.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
-                              ctx->stream));
-  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  return CFMM_OK;
-}
 
 int cfmm_execute_swap_orders(cfmm_ctx* ctx, int type, int64_t q, const int64_t* pool, const uint8_t* kind,
                              const double* amount, const double* limit, double* paid, double* received,
@@ -2695,53 +2732,19 @@ int cfmm_execute_swap_orders(cfmm_ctx* ctx, int type, int64_t q, const int64_t* 
   ctx->state_version++;
   DevBuf<double> d_amount, d_limit, d_paid, d_recv;
   DevBuf<uint8_t> d_kind, d_status;
-  CU_TRY(ctx, d_amount.alloc((size_t)(2 * q)));
-  CU_TRY(ctx, DevBuf<double>::copy_in(d_amount.p, amount, (size_t)(2 * q) * sizeof(double)));
-  CU_TRY(ctx, d_kind.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<uint8_t>::copy_in(d_kind.p, kind, (size_t)q));
-  if (limit) {
-    CU_TRY(ctx, d_limit.alloc((size_t)q));
-    CU_TRY(ctx, DevBuf<double>::copy_in(d_limit.p, limit, (size_t)q * sizeof(double)));
-  }
+  CU_TRY(ctx, d_amount.upload(amount, (size_t)(2 * q)));
+  CU_TRY(ctx, d_kind.upload(kind, (size_t)q));
+  CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
   CU_TRY(ctx, d_paid.alloc((size_t)(2 * q)));
   CU_TRY(ctx, d_recv.alloc((size_t)(2 * q)));
   CU_TRY(ctx, d_status.alloc((size_t)q));
-  for (SetRows& r : rows_by_set(ctx, type, q, pool)) {
-    PoolSet& s = *r.s;
-    const int64_t n = (int64_t)r.row.size();
-    if (n == 0) continue;
-    const PoolGroups seg = group_by_pool(r, s.m_padded);
-    const int64_t n_seg = (int64_t)seg.pos.size();
-    DevBuf<int64_t> d_seg_pos, d_seg_off, d_seg_rows, d_moved;
-    DevBuf<unsigned long long> d_n_moved;
-    DevBuf<int> d_flag;
-    CU_TRY(ctx, d_seg_pos.upload(seg.pos));
-    CU_TRY(ctx, d_seg_off.upload(seg.off));
-    CU_TRY(ctx, d_seg_rows.upload(seg.rows));
-    CU_TRY(ctx, d_n_moved.alloc(1));
-    CU_TRY(ctx, d_flag.alloc(1));
-    if (type == CFMM_POOL_UNIV3) CU_TRY(ctx, d_moved.alloc((size_t)n_seg));
-    CU_TRY(ctx, cudaMemsetAsync(d_n_moved.p, 0, sizeof(unsigned long long), ctx->stream));
-    CU_TRY(ctx, cudaMemsetAsync(d_flag.p, 0, sizeof(int), ctx->stream));
-    const cfmm::SwapSet ss = swap_set(s);
-    const unsigned blocks = (unsigned)((n_seg + 255) / 256);
-    {
-      ProfScope prof(ctx, kProfSwaps, ctx->stream);
-      CFMM_SWAP_LAUNCH(type, cfmm::swap_execute_orders_kernel, blocks, ctx->stream, ss, d_seg_pos.p, d_seg_off.p,
-                       d_seg_rows.p, n_seg, d_kind.p, d_amount.p, d_limit.p, d_paid.p, d_recv.p, d_status.p,
-                       d_moved.p, d_n_moved.p, d_flag.p);
-    }
-    ctx->launches++;
-    CU_TRY(ctx, cudaGetLastError());
-    if ((rc = swap_bookkeeping(ctx, s, type, d_moved.p, d_n_moved.p, d_flag.p)) != CFMM_OK) return rc;
-  }
-  if (paid)
-    CU_TRY(ctx, cudaMemcpyAsync(paid, d_paid.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
-                                ctx->stream));
-  if (received)
-    CU_TRY(ctx, cudaMemcpyAsync(received, d_recv.p, (size_t)(2 * q) * sizeof(double), cudaMemcpyDeviceToHost,
-                                ctx->stream));
-  if (status) CU_TRY(ctx, cudaMemcpyAsync(status, d_status.p, (size_t)q, cudaMemcpyDeviceToHost, ctx->stream));
+  if ((rc = execute_swap_rows(ctx, type, q, pool,
+                              [](auto t) { return cfmm::swap_execute_orders_kernel<decltype(t)::value>; },
+                              d_kind.p, d_amount.p, d_limit.p, d_paid.p, d_recv.p, d_status.p)) != CFMM_OK)
+    return rc;
+  CU_TRY(ctx, read_back(ctx, paid, d_paid.p, (size_t)(2 * q)));
+  CU_TRY(ctx, read_back(ctx, received, d_recv.p, (size_t)(2 * q)));
+  CU_TRY(ctx, read_back(ctx, status, d_status.p, (size_t)q));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return CFMM_OK;
 }
@@ -2787,24 +2790,75 @@ int check_paths(cfmm_ctx* ctx, int64_t q, const int64_t* hop_off, const int* hop
     if (token_in[j] < 1 || token_in[j] > ctx->n_tokens)
       return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld: token_in %lld outside 1..%lld", what, (long long)j,
                   (long long)token_in[j], (long long)ctx->n_tokens);
-    if (kind[j] != CFMM_SWAP_EXACT_IN && kind[j] != CFMM_SWAP_EXACT_OUT)
-      return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld: kind %d is neither exact-in (0) nor exact-out (1)", what,
-                  (long long)j, (int)kind[j]);
-    if (!std::isfinite(amount[j]) || amount[j] < 0.0)
-      return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld: amount %g must be finite and >= 0", what, (long long)j,
-                  amount[j]);
-    if (!limit) continue;
-    if (std::isnan(limit[j]) || limit[j] < 0.0)
-      return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld: limit %g must be >= 0", what, (long long)j, limit[j]);
-    if (std::isinf(limit[j]) && kind[j] == CFMM_SWAP_EXACT_IN)
-      return fail(ctx, CFMM_ERR_INVALID, "%s: path %lld: an exact-in path's minimum received must be finite", what,
-                  (long long)j);
+    if ((rc = check_order_row(ctx, what, "path", j, kind, amount, limit)) != CFMM_OK) return rc;
+  }
+  return CFMM_OK;
+}
+
+// The pool sets the path and order kernels see (on the device), and on execute the flags they
+// raise: out_of_range [6], touched [6], and per UniV3 set the moved list.  The order kernels list a
+// pool once (listed flags; the lists hold m_padded entries), the path kernels once per hop that
+// crossed it (moved_len: the lists' lengths, no listed flags).
+struct OrderSets {
+  cfmm::PathSets P{};
+  cfmm::SplitMoved mv{};
+  DevBuf<int> flags;
+  DevBuf<unsigned long long> n_moved;
+  DevBuf<int64_t> moved[2];
+  DevBuf<uint8_t> listed[2];
+  DevBuf<cfmm::PathSets> d_P;
+};
+
+int order_sets(cfmm_ctx* ctx, bool exec, OrderSets& os, const int64_t* moved_len = nullptr) {
+  cfmm::PathSets& P = os.P;
+  for (int k = 0; k < cfmm::kPathSets; ++k) {
+    PoolSet& s = path_set(ctx, k);
+    P.s[k] = swap_set(s);
+    P.Ai[k] = s.d_Ai.p;
+  }
+  if (exec) {
+    CU_TRY(ctx, os.flags.alloc(2 * cfmm::kPathSets));
+    CU_TRY(ctx, os.n_moved.alloc(2));
+    CU_TRY(ctx, cudaMemsetAsync(os.flags.p, 0, 2 * cfmm::kPathSets * sizeof(int), ctx->stream));
+    CU_TRY(ctx, cudaMemsetAsync(os.n_moved.p, 0, 2 * sizeof(unsigned long long), ctx->stream));
+    for (int u = 0; u < 2; ++u) {
+      if (moved_len) {
+        CU_TRY(ctx, os.moved[u].alloc((size_t)moved_len[u]));
+      } else {
+        const size_t m = (size_t)path_set(ctx, 2 * CFMM_POOL_UNIV3 + u).m_padded;
+        CU_TRY(ctx, os.moved[u].alloc(m));
+        CU_TRY(ctx, os.listed[u].alloc(m));
+        if (m) CU_TRY(ctx, cudaMemsetAsync(os.listed[u].p, 0, m, ctx->stream));
+        os.mv.flag[u] = os.listed[u].p;
+      }
+      P.moved[u] = os.moved[u].p;
+    }
+    P.out_of_range = os.flags.p;
+    P.touched = os.flags.p + cfmm::kPathSets;
+    P.n_moved = os.n_moved.p;
+  }
+  CU_TRY(ctx, os.d_P.upload(&P, 1));
+  return CFMM_OK;
+}
+
+// After an execute: the bookkeeping of cfmm_execute_swaps on every set a filled row touched.
+int order_bookkeeping(cfmm_ctx* ctx, OrderSets& os) {
+  int rc;
+  int touched[cfmm::kPathSets];
+  CU_TRY(ctx, read_back(ctx, touched, os.P.touched, cfmm::kPathSets));
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  for (int k = 0; k < cfmm::kPathSets; ++k) {
+    if (!touched[k]) continue;
+    const int t = k >> 1;
+    if ((rc = swap_bookkeeping(ctx, path_set(ctx, k), t, t == CFMM_POOL_UNIV3 ? os.moved[k & 1].p : nullptr,
+                               os.n_moved.p + (k & 1), os.flags.p + k)) != CFMM_OK)
+      return rc;
   }
   return CFMM_OK;
 }
 
 // One path call on the device: the hops resolved to (set, device position) as rows_by_set
-// resolves rows, the path arrays, the six sets (PathSets, in device memory) and the per-hop outputs.
+// resolves rows, the path arrays, the pool sets and the per-hop outputs.
 struct PathCall {
   int64_t q = 0, H = 0;
   std::vector<uint8_t> set;
@@ -2812,13 +2866,12 @@ struct PathCall {
   DevBuf<int64_t> d_off, d_pos, d_token;
   DevBuf<uint8_t> d_set, d_tok1, d_kind, d_status;
   DevBuf<double> d_amount, d_tender, d_recv;
-  DevBuf<cfmm::PathSets> d_P;
-  cfmm::PathSets P{};
+  OrderSets os;
 };
 
 // Upload a checked call, walk its tokens on the device (path_check_kernel) and reject it, before
 // anything is written, when some hop's pool does not hold the token that reaches it.
-int path_prepare(cfmm_ctx* ctx, PathCall& c, int64_t q, const int64_t* hop_off, const int* hop_type,
+int path_prepare(cfmm_ctx* ctx, PathCall& c, bool exec, int64_t q, const int64_t* hop_off, const int* hop_type,
                  const int64_t* hop_pool, const int64_t* token_in, const uint8_t* kind, const double* amount,
                  const char* what) {
   int rc;
@@ -2829,46 +2882,36 @@ int path_prepare(cfmm_ctx* ctx, PathCall& c, int64_t q, const int64_t* hop_off, 
   for (int k = 0; k < cfmm::kPathSets; ++k) ensure_pos_of(path_set(ctx, k));
   c.set.resize((size_t)c.H);
   c.pos.resize((size_t)c.H);
+  int64_t univ3_hops[2] = {0, 0};
   for (int64_t h = 0; h < c.H; ++h) {
     const int t = hop_type[h];
     const int64_t m_main = ctx->sets[t].m;
     const bool tail = hop_pool[h] >= m_main;
     c.set[(size_t)h] = (uint8_t)(2 * t + (tail ? 1 : 0));
     c.pos[(size_t)h] = path_set(ctx, 2 * t + (tail ? 1 : 0)).pos_of[(size_t)(tail ? hop_pool[h] - m_main : hop_pool[h])];
+    if (t == CFMM_POOL_UNIV3) univ3_hops[tail ? 1 : 0]++;
   }
-  for (int k = 0; k < cfmm::kPathSets; ++k) {
-    PoolSet& s = path_set(ctx, k);
-    c.P.s[k] = swap_set(s);
-    c.P.Ai[k] = s.d_Ai.p;
-  }
-  CU_TRY(ctx, c.d_off.alloc((size_t)q + 1));
-  CU_TRY(ctx, DevBuf<int64_t>::copy_in(c.d_off.p, hop_off, (size_t)(q + 1) * sizeof(int64_t)));
-  CU_TRY(ctx, c.d_token.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<int64_t>::copy_in(c.d_token.p, token_in, (size_t)q * sizeof(int64_t)));
-  CU_TRY(ctx, c.d_kind.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<uint8_t>::copy_in(c.d_kind.p, kind, (size_t)q));
-  CU_TRY(ctx, c.d_amount.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<double>::copy_in(c.d_amount.p, amount, (size_t)q * sizeof(double)));
+  CU_TRY(ctx, c.d_off.upload(hop_off, (size_t)q + 1));
+  CU_TRY(ctx, c.d_token.upload(token_in, (size_t)q));
+  CU_TRY(ctx, c.d_kind.upload(kind, (size_t)q));
+  CU_TRY(ctx, c.d_amount.upload(amount, (size_t)q));
   CU_TRY(ctx, c.d_set.upload(c.set));
   CU_TRY(ctx, c.d_pos.upload(c.pos));
   CU_TRY(ctx, c.d_tok1.alloc((size_t)c.H));
   CU_TRY(ctx, c.d_tender.alloc((size_t)c.H));
   CU_TRY(ctx, c.d_recv.alloc((size_t)c.H));
   CU_TRY(ctx, c.d_status.alloc((size_t)q));
-  CU_TRY(ctx, c.d_P.alloc(1));
-  CU_TRY(ctx, DevBuf<cfmm::PathSets>::copy_in(c.d_P.p, &c.P, sizeof(cfmm::PathSets)));
+  if ((rc = order_sets(ctx, exec, c.os, univ3_hops)) != CFMM_OK) return rc;
   DevBuf<unsigned long long> d_bad;
   CU_TRY(ctx, d_bad.alloc(1));
   CU_TRY(ctx, cudaMemsetAsync(d_bad.p, 0xff, sizeof(unsigned long long), ctx->stream));
-  {
-    ProfScope prof(ctx, kProfSwaps, ctx->stream);
-    cfmm::path_check_kernel<<<(unsigned)((q + 255) / 256), 256, 0, ctx->stream>>>(
-        c.d_P.p, q, c.d_off.p, c.d_set.p, c.d_pos.p, c.d_token.p, c.d_tok1.p, d_bad.p);
-  }
-  ctx->launches++;
-  CU_TRY(ctx, cudaGetLastError());
+  if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+         cfmm::path_check_kernel<<<(unsigned)((q + 255) / 256), 256, 0, ctx->stream>>>(
+             c.os.d_P.p, q, c.d_off.p, c.d_set.p, c.d_pos.p, c.d_token.p, c.d_tok1.p, d_bad.p);
+       })) != CFMM_OK)
+    return rc;
   unsigned long long bad = 0;
-  CU_TRY(ctx, cudaMemcpyAsync(&bad, d_bad.p, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, read_back(ctx, &bad, d_bad.p, 1));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   if (bad != ~0ull) {
     const int64_t j = (int64_t)(std::upper_bound(hop_off, hop_off + q + 1, (int64_t)bad) - hop_off) - 1;
@@ -2886,57 +2929,53 @@ int path_prepare(cfmm_ctx* ctx, PathCall& c, int64_t q, const int64_t* hop_off, 
 }
 
 int path_outputs(cfmm_ctx* ctx, const PathCall& c, double* hop_tender, double* hop_received, uint8_t* status) {
-  if (hop_tender)
-    CU_TRY(ctx, cudaMemcpyAsync(hop_tender, c.d_tender.p, (size_t)c.H * sizeof(double), cudaMemcpyDeviceToHost,
-                                ctx->stream));
-  if (hop_received)
-    CU_TRY(ctx, cudaMemcpyAsync(hop_received, c.d_recv.p, (size_t)c.H * sizeof(double), cudaMemcpyDeviceToHost,
-                                ctx->stream));
-  if (status) CU_TRY(ctx, cudaMemcpyAsync(status, c.d_status.p, (size_t)c.q, cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, read_back(ctx, hop_tender, c.d_tender.p, (size_t)c.H));
+  CU_TRY(ctx, read_back(ctx, hop_received, c.d_recv.p, (size_t)c.H));
+  CU_TRY(ctx, read_back(ctx, status, c.d_status.p, (size_t)c.q));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return CFMM_OK;
 }
 
-// The last level a pool of one set was given in this call (0 = none yet): a dense array when the
-// call's hops on the set are many against its size, a hash otherwise (group_by_pool's rule).
+// The last level a resource of one table was given in this call (0 = none yet): a dense array when
+// the call's uses of the table are many against its size, a hash otherwise (group_by_key's rule).
 struct LevelTable {
   std::vector<int> dense;
   std::unordered_map<int64_t, int> sparse;
   int& at(int64_t p) { return dense.empty() ? sparse[p] : dense[(size_t)p]; }
 };
 
-// Execution order of cfmm_execute_paths: path j's level is 1 + the largest level of an earlier
-// path sharing one of its pools, so the paths of one level touch disjoint pools and every pool sees
-// its paths in batch order.  order: the paths sorted stably by (level, batch index); the paths of
-// level L (1-based) are order[level_off[L-1] .. level_off[L]).
-void path_levels(cfmm_ctx* ctx, const PathCall& c, const int64_t* hop_off, std::vector<int64_t>& order,
-                 std::vector<int64_t>& level_off) {
-  LevelTable tab[cfmm::kPathSets];
-  int64_t count[cfmm::kPathSets] = {};
-  for (int64_t h = 0; h < c.H; ++h) count[c.set[(size_t)h]]++;
-  for (int k = 0; k < cfmm::kPathSets; ++k) {
-    const int64_t mp = path_set(ctx, k).m_padded;
-    if (count[k] > 0 && count[k] * 8 >= mp)
-      tab[k].dense.assign((size_t)mp, 0);
+// Execution order of the execute calls that run conflicting rows apart (paths, routed orders): row
+// j's level is 1 + the largest level of an earlier row sharing one of its resources, so the rows of
+// one level touch disjoint resources and every resource sees its rows in batch order.  A resource is
+// an index into one of the tables (size[k] entries, uses[k] of them named by the call);
+// for_each(j, visit) calls visit(k, index) on every resource of row j.  order: the rows sorted stably
+// by (level, batch index); the rows of level L (1-based) are order[level_off[L-1] .. level_off[L]).
+extern "C++" template <class ForEach>
+void conflict_levels(int64_t q, int n_tables, const int64_t* size, const int64_t* uses, ForEach for_each,
+                     std::vector<int64_t>& order, std::vector<int64_t>& level_off) {
+  std::vector<LevelTable> tab((size_t)n_tables);
+  for (int k = 0; k < n_tables; ++k) {
+    if (uses[k] > 0 && uses[k] * 8 >= size[k])
+      tab[(size_t)k].dense.assign((size_t)size[k], 0);
     else
-      tab[k].sparse.reserve((size_t)count[k]);
+      tab[(size_t)k].sparse.reserve((size_t)uses[k]);
   }
-  std::vector<int> lev((size_t)c.q);
+  std::vector<int> lev((size_t)q);
   int n_levels = 0;
-  for (int64_t j = 0; j < c.q; ++j) {
+  for (int64_t j = 0; j < q; ++j) {
     int L = 0;
-    for (int64_t h = hop_off[j]; h < hop_off[j + 1]; ++h) L = std::max(L, tab[c.set[(size_t)h]].at(c.pos[(size_t)h]));
+    for_each(j, [&](int k, int64_t p) { L = std::max(L, tab[(size_t)k].at(p)); });
     ++L;
-    for (int64_t h = hop_off[j]; h < hop_off[j + 1]; ++h) tab[c.set[(size_t)h]].at(c.pos[(size_t)h]) = L;
+    for_each(j, [&](int k, int64_t p) { tab[(size_t)k].at(p) = L; });
     lev[(size_t)j] = L;
     n_levels = std::max(n_levels, L);
   }
   level_off.assign((size_t)n_levels + 1, 0);
-  for (int64_t j = 0; j < c.q; ++j) level_off[(size_t)lev[(size_t)j]]++;
+  for (int64_t j = 0; j < q; ++j) level_off[(size_t)lev[(size_t)j]]++;
   for (int L = 1; L <= n_levels; ++L) level_off[(size_t)L] += level_off[(size_t)L - 1];
   std::vector<int64_t> next(level_off.begin(), level_off.end() - 1);
-  order.resize((size_t)c.q);
-  for (int64_t j = 0; j < c.q; ++j) order[(size_t)next[(size_t)lev[(size_t)j] - 1]++] = j;
+  order.resize((size_t)q);
+  for (int64_t j = 0; j < q; ++j) order[(size_t)next[(size_t)lev[(size_t)j] - 1]++] = j;
 }
 
 }  // namespace
@@ -2948,16 +2987,15 @@ int cfmm_quote_paths(cfmm_ctx* ctx, int64_t q, const int64_t* hop_off, const int
   if (rc != CFMM_OK || q == 0) return rc;
   if (!hop_tender || !hop_received || !status) return fail(ctx, CFMM_ERR_INVALID, "quote_paths: null array argument");
   PathCall c;
-  if ((rc = path_prepare(ctx, c, q, hop_off, hop_type, hop_pool, token_in, kind, amount, "quote_paths")) != CFMM_OK)
+  if ((rc = path_prepare(ctx, c, false, q, hop_off, hop_type, hop_pool, token_in, kind, amount, "quote_paths")) !=
+      CFMM_OK)
     return rc;
-  {
-    ProfScope prof(ctx, kProfSwaps, ctx->stream);
-    cfmm::path_quote_kernel<<<(unsigned)((q + 255) / 256), 256, 0, ctx->stream>>>(
-        c.d_P.p, q, c.d_off.p, c.d_set.p, c.d_pos.p, c.d_tok1.p, c.d_kind.p, c.d_amount.p, c.d_tender.p, c.d_recv.p,
-        c.d_status.p);
-  }
-  ctx->launches++;
-  CU_TRY(ctx, cudaGetLastError());
+  if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+         cfmm::path_quote_kernel<<<(unsigned)((q + 255) / 256), 256, 0, ctx->stream>>>(
+             c.os.d_P.p, q, c.d_off.p, c.d_set.p, c.d_pos.p, c.d_tok1.p, c.d_kind.p, c.d_amount.p, c.d_tender.p,
+             c.d_recv.p, c.d_status.p);
+       })) != CFMM_OK)
+    return rc;
   return path_outputs(ctx, c, hop_tender, hop_received, status);
 }
 
@@ -2967,56 +3005,35 @@ int cfmm_execute_paths(cfmm_ctx* ctx, int64_t q, const int64_t* hop_off, const i
   int rc = check_paths(ctx, q, hop_off, hop_type, hop_pool, token_in, kind, amount, limit, "execute_paths");
   if (rc != CFMM_OK || q == 0) return rc;
   PathCall c;
-  if ((rc = path_prepare(ctx, c, q, hop_off, hop_type, hop_pool, token_in, kind, amount, "execute_paths")) != CFMM_OK)
+  if ((rc = path_prepare(ctx, c, true, q, hop_off, hop_type, hop_pool, token_in, kind, amount, "execute_paths")) !=
+      CFMM_OK)
     return rc;
   ctx->state_version++;
   DevBuf<double> d_limit;
-  if (limit) {
-    CU_TRY(ctx, d_limit.alloc((size_t)q));
-    CU_TRY(ctx, DevBuf<double>::copy_in(d_limit.p, limit, (size_t)q * sizeof(double)));
-  }
-  // bookkeeping words: out_of_range [6], touched [6]; the moved lists of the two UniV3 sets
-  DevBuf<int> d_flags;
-  DevBuf<unsigned long long> d_n_moved;
-  DevBuf<int64_t> d_moved[2];
-  CU_TRY(ctx, d_flags.alloc(2 * cfmm::kPathSets));
-  CU_TRY(ctx, d_n_moved.alloc(2));
-  CU_TRY(ctx, cudaMemsetAsync(d_flags.p, 0, 2 * cfmm::kPathSets * sizeof(int), ctx->stream));
-  CU_TRY(ctx, cudaMemsetAsync(d_n_moved.p, 0, 2 * sizeof(unsigned long long), ctx->stream));
-  for (int u = 0; u < 2; ++u) {
-    const int64_t n = std::count(c.set.begin(), c.set.end(), (uint8_t)(2 * CFMM_POOL_UNIV3 + u));
-    CU_TRY(ctx, d_moved[u].alloc((size_t)n));
-    c.P.moved[u] = d_moved[u].p;
-  }
-  c.P.out_of_range = d_flags.p;
-  c.P.touched = d_flags.p + cfmm::kPathSets;
-  c.P.n_moved = d_n_moved.p;
-  CU_TRY(ctx, DevBuf<cfmm::PathSets>::copy_in(c.d_P.p, &c.P, sizeof(cfmm::PathSets)));
+  CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
+  // levels over the hops' pools: one table per set
+  int64_t size[cfmm::kPathSets], uses[cfmm::kPathSets] = {};
+  for (int k = 0; k < cfmm::kPathSets; ++k) size[k] = path_set(ctx, k).m_padded;
+  for (int64_t h = 0; h < c.H; ++h) uses[c.set[(size_t)h]]++;
   std::vector<int64_t> order, level_off;
-  path_levels(ctx, c, hop_off, order, level_off);
+  conflict_levels(
+      q, cfmm::kPathSets, size, uses,
+      [&](int64_t j, auto&& visit) {
+        for (int64_t h = hop_off[j]; h < hop_off[j + 1]; ++h) visit(c.set[(size_t)h], c.pos[(size_t)h]);
+      },
+      order, level_off);
   DevBuf<int64_t> d_order;
   CU_TRY(ctx, d_order.upload(order));
   for (size_t L = 1; L < level_off.size(); ++L) {
     const int64_t n = level_off[L] - level_off[L - 1];
-    {
-      ProfScope prof(ctx, kProfSwaps, ctx->stream);
-      cfmm::path_execute_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(
-          c.d_P.p, d_order.p + level_off[L - 1], n, c.d_off.p, c.d_set.p, c.d_pos.p, c.d_tok1.p, c.d_kind.p,
-          c.d_amount.p, d_limit.p, c.d_tender.p, c.d_recv.p, c.d_status.p);
-    }
-    ctx->launches++;
-    CU_TRY(ctx, cudaGetLastError());
-  }
-  int touched[cfmm::kPathSets];
-  CU_TRY(ctx, cudaMemcpyAsync(touched, c.P.touched, sizeof(touched), cudaMemcpyDeviceToHost, ctx->stream));
-  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  for (int k = 0; k < cfmm::kPathSets; ++k) {
-    if (!touched[k]) continue;
-    const int t = k >> 1;
-    if ((rc = swap_bookkeeping(ctx, path_set(ctx, k), t, t == CFMM_POOL_UNIV3 ? d_moved[k & 1].p : nullptr,
-                               d_n_moved.p + (k & 1), d_flags.p + k)) != CFMM_OK)
+    if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+           cfmm::path_execute_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(
+               c.os.d_P.p, d_order.p + level_off[L - 1], n, c.d_off.p, c.d_set.p, c.d_pos.p, c.d_tok1.p, c.d_kind.p,
+               c.d_amount.p, d_limit.p, c.d_tender.p, c.d_recv.p, c.d_status.p);
+         })) != CFMM_OK)
       return rc;
   }
+  if ((rc = order_bookkeeping(ctx, c.os)) != CFMM_OK) return rc;
   return path_outputs(ctx, c, hop_tender, hop_received, status);
 }
 
@@ -3061,16 +3078,16 @@ int ensure_pair_index(cfmm_ctx* ctx) {
     CU_TRY(ctx, cub::DeviceRunLengthEncode::Encode(nullptr, b2, keys_sorted.p, ix.keys.p, run_len.p, d_runs.p, items, st));
     CU_TRY(ctx, cub::DeviceScan::ExclusiveSum(nullptr, b3, run_len.p, ix.off.p, items + 1, st));
     CU_TRY(ctx, temp.alloc(std::max(b1, std::max(b2, b3))));
-    size_t bytes = temp.n;
-    {
-      ProfScope prof(ctx, kProfSwaps, st);
+    int n_sets = 0;
+    for (int k = 0; k < cfmm::kPathSets; ++k) n_sets += path_set(ctx, k).m > 0;
+    int rc = launch(ctx, kProfSwaps, n_sets + 3, [&]() -> int {
       for (int k = 0; k < cfmm::kPathSets; ++k) {
         PoolSet& s = path_set(ctx, k);
         if (s.m == 0) continue;
         cfmm::pair_key_kernel<<<(unsigned)((s.m_padded + 255) / 256), 256, 0, st>>>(s.d_Ai.p, s.d_gidx.p, s.m_padded, k,
                                                                                    nt, keys_in.p, ent_in.p);
-        ctx->launches++;
       }
+      size_t bytes = temp.n;
       CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(temp.p, bytes, keys_in.p, keys_sorted.p, ent_in.p, ix.pool.p, items, 0,
                                                   end_bit, st));
       CU_TRY(ctx, cudaMemsetAsync(run_len.p, 0, ((size_t)n + 1) * sizeof(int64_t), st));
@@ -3079,11 +3096,11 @@ int ensure_pair_index(cfmm_ctx* ctx) {
                                                      st));
       bytes = temp.n;
       CU_TRY(ctx, cub::DeviceScan::ExclusiveSum(temp.p, bytes, run_len.p, ix.off.p, items + 1, st));
-      ctx->launches += 3;
-    }
-    CU_TRY(ctx, cudaGetLastError());
+      return CFMM_OK;
+    });
+    if (rc != CFMM_OK) return rc;
     int runs = 0;
-    CU_TRY(ctx, cudaMemcpyAsync(&runs, d_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU_TRY(ctx, read_back(ctx, &runs, d_runs.p, 1));
     CU_TRY(ctx, cudaStreamSynchronize(st));
     ix.n_pairs = runs;
   }
@@ -3113,21 +3130,18 @@ int pair_lookup(cfmm_ctx* ctx, int64_t q, const int64_t* a, const int64_t* b, De
   if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
   if ((rc = ensure_pair_index(ctx)) != CFMM_OK) return rc;
   DevBuf<int64_t> d_count;
-  CU_TRY(ctx, d_a.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_a.p, a, (size_t)q * sizeof(int64_t)));
-  CU_TRY(ctx, d_b.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_b.p, b, (size_t)q * sizeof(int64_t)));
+  CU_TRY(ctx, d_a.upload(a, (size_t)q));
+  CU_TRY(ctx, d_b.upload(b, (size_t)q));
   CU_TRY(ctx, d_pair.alloc((size_t)q));
   CU_TRY(ctx, d_count.alloc((size_t)q));
-  {
-    ProfScope prof(ctx, kProfSwaps, ctx->stream);
-    cfmm::pair_lookup_kernel<<<(unsigned)((q + 255) / 256), 256, 0, ctx->stream>>>(
-        ctx->pairs.keys.p, ctx->pairs.n_pairs, ctx->pairs.off.p, d_a.p, d_b.p, q, ctx->n_tokens, d_pair.p, d_count.p);
-  }
-  ctx->launches++;
-  CU_TRY(ctx, cudaGetLastError());
+  if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+         cfmm::pair_lookup_kernel<<<(unsigned)((q + 255) / 256), 256, 0, ctx->stream>>>(
+             ctx->pairs.keys.p, ctx->pairs.n_pairs, ctx->pairs.off.p, d_a.p, d_b.p, q, ctx->n_tokens, d_pair.p,
+             d_count.p);
+       })) != CFMM_OK)
+    return rc;
   count.resize((size_t)q);
-  CU_TRY(ctx, cudaMemcpyAsync(count.data(), d_count.p, (size_t)q * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, read_back(ctx, count.data(), d_count.p, (size_t)q));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return CFMM_OK;
 }
@@ -3141,101 +3155,69 @@ int check_split(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t
   if (q == 0) return CFMM_OK;
   if (!token_in || !token_out || !kind || !amount) return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
   if ((rc = check_pair_tokens(ctx, q, token_in, token_out, what)) != CFMM_OK) return rc;
-  for (int64_t j = 0; j < q; ++j) {
-    if (kind[j] != CFMM_SWAP_EXACT_IN && kind[j] != CFMM_SWAP_EXACT_OUT)
-      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: kind %d is neither exact-in (0) nor exact-out (1)", what,
-                  (long long)j, (int)kind[j]);
-    if (!std::isfinite(amount[j]) || amount[j] < 0.0)
-      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: amount %g must be finite and >= 0", what, (long long)j,
-                  amount[j]);
-    if (!limit) continue;
-    if (std::isnan(limit[j]) || limit[j] < 0.0)
-      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: limit %g must be >= 0", what, (long long)j, limit[j]);
-    if (std::isinf(limit[j]) && kind[j] == CFMM_SWAP_EXACT_IN)
-      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: an exact-in row's minimum received must be finite", what,
-                  (long long)j);
-  }
+  for (int64_t j = 0; j < q; ++j)
+    if ((rc = check_order_row(ctx, what, "row", j, kind, amount, limit)) != CFMM_OK) return rc;
   return CFMM_OK;
 }
 
-// Execution order: the rows grouped by pair, batch order kept inside each pair; a row whose pair no
-// pool holds is a group of its own.  A counting sort on the pair when the batch is large against the
-// index, a stable comparison sort otherwise (group_by_pool's rule).
-void group_by_pair(const std::vector<int64_t>& pair, int64_t n_pairs, std::vector<int64_t>& off,
-                   std::vector<int64_t>& rows) {
-  const int64_t q = (int64_t)pair.size();
-  rows.resize((size_t)q);
-  if (q * 8 >= n_pairs) {
-    std::vector<int64_t> start((size_t)n_pairs + 2, 0);
-    for (int64_t j = 0; j < q; ++j) start[(size_t)(pair[(size_t)j] + 2)]++;
-    for (int64_t k = 0; k <= n_pairs; ++k) start[(size_t)k + 1] += start[(size_t)k];
-    for (int64_t j = 0; j < q; ++j) rows[(size_t)start[(size_t)(pair[(size_t)j] + 1)]++] = j;
-  } else {
-    for (int64_t j = 0; j < q; ++j) rows[(size_t)j] = j;
-    std::stable_sort(rows.begin(), rows.end(), [&](int64_t a, int64_t b) { return pair[(size_t)a] < pair[(size_t)b]; });
-  }
-  off.clear();
-  for (int64_t j = 0; j < q; ++j) {
-    const int64_t p = pair[(size_t)rows[(size_t)j]];
-    if (j == 0 || p < 0 || p != pair[(size_t)rows[(size_t)j - 1]]) off.push_back(j);
-  }
-  off.push_back(q);
-}
-
-// The pool sets the order kernels see (on the device), and on execute the flags they raise:
-// out_of_range [6], touched [6], and per UniV3 set the moved list and its listed flags.
-struct OrderSets {
-  cfmm::PathSets P{};
-  cfmm::SplitMoved mv{};
-  DevBuf<int> flags;
-  DevBuf<unsigned long long> n_moved;
-  DevBuf<int64_t> moved[2];
-  DevBuf<uint8_t> listed[2];
-  DevBuf<cfmm::PathSets> d_P;
+// One split, routed or arbitrage call on the device: the rows' pair lists looked up in the pair
+// index (d_a, d_b, d_pair; one list per split row), the legs of every list (leg_off), the row
+// arrays, the per-row outputs and the pool sets.  On execute, pair holds the lists' pairs on the
+// host.
+struct OrderCall {
+  int64_t q = 0, L = 0;
+  bool legs = false;  // leg outputs asked for, and some list has a pool
+  std::vector<int64_t> pair;
+  DevBuf<int64_t> d_a, d_b, d_pair, d_leg_off;
+  DevBuf<uint8_t> d_kind, d_status;
+  DevBuf<double> d_amount, d_limit, d_paid, d_recv, d_price, d_ld, d_ll;
+  OrderSets os;
 };
 
-int order_sets(cfmm_ctx* ctx, bool exec, OrderSets& os) {
-  cfmm::PathSets& P = os.P;
-  for (int k = 0; k < cfmm::kPathSets; ++k) {
-    PoolSet& s = path_set(ctx, k);
-    P.s[k] = swap_set(s);
-    P.Ai[k] = s.d_Ai.p;
+// kind and amount are null for arbitrage rows, limit when there are no limits.
+int order_prepare(cfmm_ctx* ctx, OrderCall& c, bool exec, int64_t q, int64_t n_lists, const int64_t* a,
+                  const int64_t* b, const uint8_t* kind, const double* amount, const double* limit, bool legs) {
+  int rc;
+  std::vector<int64_t> count;
+  if ((rc = pair_lookup(ctx, n_lists, a, b, c.d_a, c.d_b, c.d_pair, count)) != CFMM_OK) return rc;
+  std::vector<int64_t> leg_off((size_t)n_lists + 1, 0);
+  for (int64_t j = 0; j < n_lists; ++j) leg_off[(size_t)j + 1] = leg_off[(size_t)j] + count[(size_t)j];
+  c.q = q;
+  c.L = leg_off[(size_t)n_lists];
+  c.legs = legs && c.L > 0;
+  CU_TRY(ctx, c.d_leg_off.upload(leg_off));
+  CU_TRY(ctx, c.d_kind.upload(kind, (size_t)q));
+  CU_TRY(ctx, c.d_amount.upload(amount, (size_t)q));
+  CU_TRY(ctx, c.d_limit.upload(limit, (size_t)q));
+  CU_TRY(ctx, c.d_paid.alloc((size_t)q));
+  CU_TRY(ctx, c.d_recv.alloc((size_t)q));
+  CU_TRY(ctx, c.d_price.alloc((size_t)q));
+  CU_TRY(ctx, c.d_status.alloc((size_t)q));
+  if (c.legs) {
+    CU_TRY(ctx, c.d_ld.alloc((size_t)(2 * c.L)));
+    CU_TRY(ctx, c.d_ll.alloc((size_t)(2 * c.L)));
   }
+  if ((rc = order_sets(ctx, exec, c.os)) != CFMM_OK) return rc;
   if (exec) {
-    CU_TRY(ctx, os.flags.alloc(2 * cfmm::kPathSets));
-    CU_TRY(ctx, os.n_moved.alloc(2));
-    CU_TRY(ctx, cudaMemsetAsync(os.flags.p, 0, 2 * cfmm::kPathSets * sizeof(int), ctx->stream));
-    CU_TRY(ctx, cudaMemsetAsync(os.n_moved.p, 0, 2 * sizeof(unsigned long long), ctx->stream));
-    for (int u = 0; u < 2; ++u) {
-      const size_t m = (size_t)path_set(ctx, 2 * CFMM_POOL_UNIV3 + u).m_padded;
-      CU_TRY(ctx, os.moved[u].alloc(m));
-      CU_TRY(ctx, os.listed[u].alloc(m));
-      if (m) CU_TRY(ctx, cudaMemsetAsync(os.listed[u].p, 0, m, ctx->stream));
-      P.moved[u] = os.moved[u].p;
-      os.mv.flag[u] = os.listed[u].p;
-    }
-    P.out_of_range = os.flags.p;
-    P.touched = os.flags.p + cfmm::kPathSets;
-    P.n_moved = os.n_moved.p;
+    ctx->state_version++;
+    c.pair.resize((size_t)n_lists);
+    CU_TRY(ctx, read_back(ctx, c.pair.data(), c.d_pair.p, (size_t)n_lists));
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   }
-  CU_TRY(ctx, os.d_P.alloc(1));
-  CU_TRY(ctx, DevBuf<cfmm::PathSets>::copy_in(os.d_P.p, &P, sizeof(cfmm::PathSets)));
   return CFMM_OK;
 }
 
-// After an execute: the bookkeeping of cfmm_execute_swaps on every set a filled row touched.
-int order_bookkeeping(cfmm_ctx* ctx, OrderSets& os) {
-  int rc;
-  int touched[cfmm::kPathSets];
-  CU_TRY(ctx, cudaMemcpyAsync(touched, os.P.touched, sizeof(touched), cudaMemcpyDeviceToHost, ctx->stream));
-  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  for (int k = 0; k < cfmm::kPathSets; ++k) {
-    if (!touched[k]) continue;
-    const int t = k >> 1;
-    if ((rc = swap_bookkeeping(ctx, path_set(ctx, k), t, t == CFMM_POOL_UNIV3 ? os.moved[k & 1].p : nullptr,
-                               os.n_moved.p + (k & 1), os.flags.p + k)) != CFMM_OK)
-      return rc;
+int order_outputs(cfmm_ctx* ctx, const OrderCall& c, double* paid, double* received, double* price, uint8_t* status,
+                  double* leg_delta, double* leg_lambda) {
+  CU_TRY(ctx, read_back(ctx, paid, c.d_paid.p, (size_t)c.q));
+  CU_TRY(ctx, read_back(ctx, received, c.d_recv.p, (size_t)c.q));
+  CU_TRY(ctx, read_back(ctx, price, c.d_price.p, (size_t)c.q));
+  CU_TRY(ctx, read_back(ctx, status, c.d_status.p, (size_t)c.q));
+  if (c.legs) {
+    CU_TRY(ctx, read_back(ctx, leg_delta, c.d_ld.p, (size_t)(2 * c.L)));
+    CU_TRY(ctx, read_back(ctx, leg_lambda, c.d_ll.p, (size_t)(2 * c.L)));
   }
+  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return CFMM_OK;
 }
 
@@ -3243,77 +3225,36 @@ int split_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, c
                  const uint8_t* kind, const double* amount, const double* limit, double* paid, double* received,
                  double* price, uint8_t* status, double* leg_delta, double* leg_lambda) {
   int rc;
-  DevBuf<int64_t> d_in, d_out, d_pair;
-  std::vector<int64_t> count;
-  if ((rc = pair_lookup(ctx, q, token_in, token_out, d_in, d_out, d_pair, count)) != CFMM_OK) return rc;
-  std::vector<int64_t> leg_off((size_t)q + 1, 0);
-  for (int64_t j = 0; j < q; ++j) leg_off[(size_t)j + 1] = leg_off[(size_t)j] + count[(size_t)j];
-  const int64_t L = leg_off[(size_t)q];
-  const bool legs = (leg_delta || leg_lambda) && L > 0;
-  DevBuf<int64_t> d_leg_off;
-  DevBuf<uint8_t> d_kind, d_status;
-  DevBuf<double> d_amount, d_limit, d_paid, d_recv, d_price, d_ld, d_ll;
-  CU_TRY(ctx, d_leg_off.upload(leg_off));
-  CU_TRY(ctx, d_kind.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<uint8_t>::copy_in(d_kind.p, kind, (size_t)q));
-  CU_TRY(ctx, d_amount.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<double>::copy_in(d_amount.p, amount, (size_t)q * sizeof(double)));
-  if (limit) {
-    CU_TRY(ctx, d_limit.alloc((size_t)q));
-    CU_TRY(ctx, DevBuf<double>::copy_in(d_limit.p, limit, (size_t)q * sizeof(double)));
-  }
-  CU_TRY(ctx, d_paid.alloc((size_t)q));
-  CU_TRY(ctx, d_recv.alloc((size_t)q));
-  CU_TRY(ctx, d_price.alloc((size_t)q));
-  CU_TRY(ctx, d_status.alloc((size_t)q));
-  if (legs) {
-    CU_TRY(ctx, d_ld.alloc((size_t)(2 * L)));
-    CU_TRY(ctx, d_ll.alloc((size_t)(2 * L)));
-  }
-  OrderSets os;
-  if ((rc = order_sets(ctx, exec, os)) != CFMM_OK) return rc;
-  cfmm::SplitRows R{d_in.p,    d_out.p,  d_kind.p,  d_amount.p, d_limit.p, d_pair.p, d_leg_off.p,
-                    d_paid.p,  d_recv.p, d_price.p, d_status.p, d_ld.p,    d_ll.p};
+  OrderCall c;
+  if ((rc = order_prepare(ctx, c, exec, q, q, token_in, token_out, kind, amount, limit, leg_delta || leg_lambda)) !=
+      CFMM_OK)
+    return rc;
+  cfmm::SplitRows R{c.d_a.p,    c.d_b.p,    c.d_kind.p,  c.d_amount.p, c.d_limit.p, c.d_pair.p, c.d_leg_off.p,
+                    c.d_paid.p, c.d_recv.p, c.d_price.p, c.d_status.p, c.d_ld.p,    c.d_ll.p};
   const cfmm::PairIndexView ix{ctx->pairs.off.p, ctx->pairs.pool.p};
-  const int per_block = cfmm::kSplitThreads / 32;
+  const int per_block = cfmm::kSplitThreads / 32;  // a warp per row (quote) or per pair (execute)
   if (!exec) {
-    ProfScope prof(ctx, kProfSwaps, ctx->stream);
-    cfmm::split_quote_kernel<<<(unsigned)((q + per_block - 1) / per_block), cfmm::kSplitThreads, 0, ctx->stream>>>(
-        os.d_P.p, ix, R, q);
-    ctx->launches++;
-    CU_TRY(ctx, cudaGetLastError());
+    rc = launch(ctx, kProfSwaps, 1, [&] {
+      cfmm::split_quote_kernel<<<(unsigned)((q + per_block - 1) / per_block), cfmm::kSplitThreads, 0, ctx->stream>>>(
+          c.os.d_P.p, ix, R, q);
+    });
+    if (rc != CFMM_OK) return rc;
   } else {
-    ctx->state_version++;
-    std::vector<int64_t> pair((size_t)q), seg_off, seg_rows;
-    CU_TRY(ctx, cudaMemcpyAsync(pair.data(), d_pair.p, (size_t)q * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    group_by_pair(pair, ctx->pairs.n_pairs, seg_off, seg_rows);
-    const int64_t n_seg = (int64_t)seg_off.size() - 1;
+    // the rows grouped by pair, batch order kept inside each pair; a row whose pair no pool holds is a
+    // group of its own
+    const Groups seg = group_by_key(c.pair, ctx->pairs.n_pairs);
+    const int64_t n_seg = (int64_t)seg.key.size();
     DevBuf<int64_t> d_seg_off, d_seg_rows;
-    CU_TRY(ctx, d_seg_off.upload(seg_off));
-    CU_TRY(ctx, d_seg_rows.upload(seg_rows));
-    {
-      ProfScope prof(ctx, kProfSwaps, ctx->stream);
+    CU_TRY(ctx, d_seg_off.upload(seg.off));
+    CU_TRY(ctx, d_seg_rows.upload(seg.rows));
+    rc = launch(ctx, kProfSwaps, 1, [&] {
       cfmm::split_execute_kernel<<<(unsigned)((n_seg + per_block - 1) / per_block), cfmm::kSplitThreads, 0,
-                                   ctx->stream>>>(os.d_P.p, ix, R, d_seg_off.p, d_seg_rows.p, n_seg, os.mv);
-    }
-    ctx->launches++;
-    CU_TRY(ctx, cudaGetLastError());
-    if ((rc = order_bookkeeping(ctx, os)) != CFMM_OK) return rc;
+                                   ctx->stream>>>(c.os.d_P.p, ix, R, d_seg_off.p, d_seg_rows.p, n_seg, c.os.mv);
+    });
+    if (rc != CFMM_OK) return rc;
+    if ((rc = order_bookkeeping(ctx, c.os)) != CFMM_OK) return rc;
   }
-  const auto d2h = [&](void* dst, const void* src, size_t bytes) {
-    return dst ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream) : cudaSuccess;
-  };
-  CU_TRY(ctx, d2h(paid, d_paid.p, (size_t)q * sizeof(double)));
-  CU_TRY(ctx, d2h(received, d_recv.p, (size_t)q * sizeof(double)));
-  CU_TRY(ctx, d2h(price, d_price.p, (size_t)q * sizeof(double)));
-  CU_TRY(ctx, d2h(status, d_status.p, (size_t)q));
-  if (legs) {
-    CU_TRY(ctx, d2h(leg_delta, d_ld.p, (size_t)(2 * L) * sizeof(double)));
-    CU_TRY(ctx, d2h(leg_lambda, d_ll.p, (size_t)(2 * L) * sizeof(double)));
-  }
-  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  return CFMM_OK;
+  return order_outputs(ctx, c, paid, received, price, status, leg_delta, leg_lambda);
 }
 
 // ---- orders routed over their pair and two-hop routes through hubs (route_kernels.cuh) ----------
@@ -3401,124 +3342,61 @@ int routed_orders(cfmm_ctx* ctx, bool exec, bool arb, int64_t q, const int64_t* 
     }
     max_hubs = std::max(max_hubs, (int)(hub_off[r + 1] - hub_off[r]));
   }
-  DevBuf<int64_t> d_a, d_b, d_pair;
-  std::vector<int64_t> count;
-  if ((rc = pair_lookup(ctx, n_lists, la.data(), lb.data(), d_a, d_b, d_pair, count)) != CFMM_OK) return rc;
-  std::vector<int64_t> leg_off((size_t)n_lists + 1, 0);
-  for (int64_t j = 0; j < n_lists; ++j) leg_off[(size_t)j + 1] = leg_off[(size_t)j] + count[(size_t)j];
-  const int64_t L = leg_off[(size_t)n_lists];
-  const bool legs = (leg_delta || leg_lambda) && L > 0;
-  DevBuf<int64_t> d_in, d_out, d_leg_off, d_hub_off, d_hubs;
-  DevBuf<uint8_t> d_kind, d_status;
-  DevBuf<double> d_amount, d_limit, d_paid, d_recv, d_price, d_hp, d_hs, d_ld, d_ll;
-  CU_TRY(ctx, d_in.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_in.p, token_in, (size_t)q * sizeof(int64_t)));
-  CU_TRY(ctx, d_out.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_out.p, token_out, (size_t)q * sizeof(int64_t)));
-  CU_TRY(ctx, d_hub_off.alloc((size_t)q + 1));
-  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_hub_off.p, hub_off, ((size_t)q + 1) * sizeof(int64_t)));
-  if (nh > 0) {
-    CU_TRY(ctx, d_hubs.alloc((size_t)nh));
-    CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_hubs.p, hubs, (size_t)nh * sizeof(int64_t)));
-  }
-  CU_TRY(ctx, d_leg_off.upload(leg_off));
-  if (!arb) {
-    CU_TRY(ctx, d_kind.alloc((size_t)q));
-    CU_TRY(ctx, DevBuf<uint8_t>::copy_in(d_kind.p, kind, (size_t)q));
-    CU_TRY(ctx, d_amount.alloc((size_t)q));
-    CU_TRY(ctx, DevBuf<double>::copy_in(d_amount.p, amount, (size_t)q * sizeof(double)));
-  }
-  if (limit) {
-    CU_TRY(ctx, d_limit.alloc((size_t)q));
-    CU_TRY(ctx, DevBuf<double>::copy_in(d_limit.p, limit, (size_t)q * sizeof(double)));
-  }
-  CU_TRY(ctx, d_paid.alloc((size_t)q));
-  CU_TRY(ctx, d_recv.alloc((size_t)q));
-  CU_TRY(ctx, d_price.alloc((size_t)q));
-  CU_TRY(ctx, d_status.alloc((size_t)q));
-  if (nh > 0) {
-    CU_TRY(ctx, d_hp.alloc((size_t)nh));
-    CU_TRY(ctx, d_hs.alloc((size_t)nh));
-  }
-  if (legs) {
-    CU_TRY(ctx, d_ld.alloc((size_t)(2 * L)));
-    CU_TRY(ctx, d_ll.alloc((size_t)(2 * L)));
-  }
-  OrderSets os;
-  if ((rc = order_sets(ctx, exec, os)) != CFMM_OK) return rc;
-  cfmm::RouteRows R{d_in.p,    d_out.p,   d_kind.p,  d_amount.p, d_limit.p, d_hub_off.p, d_hubs.p, d_pair.p, d_leg_off.p,
-                    d_paid.p,  d_recv.p,  d_price.p, d_status.p, d_hp.p,    d_hs.p,      d_ld.p,   d_ll.p};
+  OrderCall c;
+  if ((rc = order_prepare(ctx, c, exec, q, n_lists, la.data(), lb.data(), kind, amount, limit,
+                          leg_delta || leg_lambda)) != CFMM_OK)
+    return rc;
+  DevBuf<int64_t> d_in, d_out, d_hub_off, d_hubs;
+  DevBuf<double> d_hp, d_hs;
+  CU_TRY(ctx, d_in.upload(token_in, (size_t)q));
+  CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
+  CU_TRY(ctx, d_hub_off.upload(hub_off, (size_t)q + 1));
+  CU_TRY(ctx, d_hubs.upload(hubs, (size_t)nh));
+  CU_TRY(ctx, d_hp.alloc((size_t)nh));
+  CU_TRY(ctx, d_hs.alloc((size_t)nh));
+  cfmm::RouteRows R{d_in.p,     d_out.p,    c.d_kind.p,  c.d_amount.p, c.d_limit.p, d_hub_off.p,
+                    d_hubs.p,   c.d_pair.p, c.d_leg_off.p, c.d_paid.p, c.d_recv.p,  c.d_price.p,
+                    c.d_status.p, d_hp.p,   d_hs.p,      c.d_ld.p,     c.d_ll.p};
   const cfmm::PairIndexView ix{ctx->pairs.off.p, ctx->pairs.pool.p};
   const unsigned threads = 32u * (1u + (unsigned)max_hubs);  // warp 0: the direct pools, warp 1 + h: hub h
   if (!exec) {
-    ProfScope prof(ctx, kProfSwaps, ctx->stream);
-    if (arb)
-      cfmm::arb_quote_kernel<<<(unsigned)q, threads, 0, ctx->stream>>>(os.d_P.p, ix, R);
-    else
-      cfmm::route_quote_kernel<<<(unsigned)q, threads, 0, ctx->stream>>>(os.d_P.p, ix, R);
-    ctx->launches++;
-    CU_TRY(ctx, cudaGetLastError());
+    rc = launch(ctx, kProfSwaps, 1, [&] {
+      if (arb)
+        cfmm::arb_quote_kernel<<<(unsigned)q, threads, 0, ctx->stream>>>(c.os.d_P.p, ix, R);
+      else
+        cfmm::route_quote_kernel<<<(unsigned)q, threads, 0, ctx->stream>>>(c.os.d_P.p, ix, R);
+    });
+    if (rc != CFMM_OK) return rc;
   } else {
-    ctx->state_version++;
-    // levels: a row's level is 1 + the highest level of an earlier row sharing one of its pairs (a
-    // pool belongs to one pair); pairs no pool holds conflict with nothing
-    std::vector<int64_t> pair((size_t)n_lists);
-    CU_TRY(ctx, cudaMemcpyAsync(pair.data(), d_pair.p, (size_t)n_lists * sizeof(int64_t), cudaMemcpyDeviceToHost,
-                                ctx->stream));
-    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    std::vector<int32_t> pair_level((size_t)ctx->pairs.n_pairs, 0);
-    std::vector<int32_t> level((size_t)q);
-    int32_t n_levels = 0;
-    for (int64_t r = 0; r < q; ++r) {
-      const int64_t b = r + 2 * hub_off[r], e = r + 1 + 2 * hub_off[r + 1];
-      int32_t lv = 0;
-      for (int64_t x = b; x < e; ++x)
-        if (pair[(size_t)x] >= 0) lv = std::max(lv, pair_level[(size_t)pair[(size_t)x]]);
-      ++lv;
-      for (int64_t x = b; x < e; ++x)
-        if (pair[(size_t)x] >= 0) pair_level[(size_t)pair[(size_t)x]] = lv;
-      level[(size_t)r] = lv;
-      n_levels = std::max(n_levels, lv);
-    }
-    std::vector<int64_t> start((size_t)n_levels + 2, 0), rows((size_t)q);  // rows by level, batch order kept
-    for (int64_t r = 0; r < q; ++r) start[(size_t)level[(size_t)r] + 1]++;
-    for (int32_t l = 0; l <= n_levels; ++l) start[(size_t)l + 1] += start[(size_t)l];
-    std::vector<int64_t> fill(start);
-    for (int64_t r = 0; r < q; ++r) rows[(size_t)fill[(size_t)level[(size_t)r]]++] = r;
+    // levels over the rows' pairs (a pool belongs to one pair); pairs no pool holds conflict with
+    // nothing
+    const int64_t n_pairs = ctx->pairs.n_pairs;
+    std::vector<int64_t> order, level_off;
+    conflict_levels(
+        q, 1, &n_pairs, &n_lists,
+        [&](int64_t r, auto&& visit) {
+          for (int64_t x = r + 2 * hub_off[r]; x < r + 1 + 2 * hub_off[r + 1]; ++x)
+            if (c.pair[(size_t)x] >= 0) visit(0, c.pair[(size_t)x]);
+        },
+        order, level_off);
     DevBuf<int64_t> d_rows;
-    CU_TRY(ctx, d_rows.upload(rows));
-    for (int32_t l = 1; l <= n_levels; ++l) {
-      const int64_t n = start[(size_t)l + 1] - start[(size_t)l];
-      if (n == 0) continue;
-      {
-        ProfScope prof(ctx, kProfSwaps, ctx->stream);
+    CU_TRY(ctx, d_rows.upload(order));
+    for (size_t l = 1; l < level_off.size(); ++l) {
+      const int64_t n = level_off[l] - level_off[l - 1];
+      const int64_t* rows = d_rows.p + level_off[l - 1];
+      rc = launch(ctx, kProfSwaps, 1, [&] {
         if (arb)
-          cfmm::arb_execute_kernel<<<(unsigned)n, threads, 0, ctx->stream>>>(os.d_P.p, ix, R,
-                                                                              d_rows.p + start[(size_t)l], os.mv);
+          cfmm::arb_execute_kernel<<<(unsigned)n, threads, 0, ctx->stream>>>(c.os.d_P.p, ix, R, rows, c.os.mv);
         else
-          cfmm::route_execute_kernel<<<(unsigned)n, threads, 0, ctx->stream>>>(os.d_P.p, ix, R,
-                                                                                d_rows.p + start[(size_t)l], os.mv);
-      }
-      ctx->launches++;
-      CU_TRY(ctx, cudaGetLastError());
+          cfmm::route_execute_kernel<<<(unsigned)n, threads, 0, ctx->stream>>>(c.os.d_P.p, ix, R, rows, c.os.mv);
+      });
+      if (rc != CFMM_OK) return rc;
     }
-    if ((rc = order_bookkeeping(ctx, os)) != CFMM_OK) return rc;
+    if ((rc = order_bookkeeping(ctx, c.os)) != CFMM_OK) return rc;
   }
-  const auto d2h = [&](void* dst, const void* src, size_t bytes) {
-    return dst && bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream) : cudaSuccess;
-  };
-  CU_TRY(ctx, d2h(paid, d_paid.p, (size_t)q * sizeof(double)));
-  CU_TRY(ctx, d2h(received, d_recv.p, (size_t)q * sizeof(double)));
-  CU_TRY(ctx, d2h(price, d_price.p, (size_t)q * sizeof(double)));
-  CU_TRY(ctx, d2h(status, d_status.p, (size_t)q));
-  CU_TRY(ctx, d2h(hub_price, d_hp.p, (size_t)nh * sizeof(double)));
-  CU_TRY(ctx, d2h(hub_surplus, d_hs.p, (size_t)nh * sizeof(double)));
-  if (legs) {
-    CU_TRY(ctx, d2h(leg_delta, d_ld.p, (size_t)(2 * L) * sizeof(double)));
-    CU_TRY(ctx, d2h(leg_lambda, d_ll.p, (size_t)(2 * L) * sizeof(double)));
-  }
-  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  return CFMM_OK;
+  CU_TRY(ctx, read_back(ctx, hub_price, d_hp.p, (size_t)nh));
+  CU_TRY(ctx, read_back(ctx, hub_surplus, d_hs.p, (size_t)nh));
+  return order_outputs(ctx, c, paid, received, price, status, leg_delta, leg_lambda);
 }
 
 // ---- arbitrage cycles through base tokens (arb_scan_kernels.cuh) --------------------------------
@@ -3581,22 +3459,19 @@ int ensure_adjacency(cfmm_ctx* ctx) {
                                                 st));
     CU_TRY(ctx, temp.alloc(bytes));
   }
-  {
-    ProfScope prof(ctx, kProfSwaps, st);
+  int rc2 = launch(ctx, kProfSwaps, m > 0 ? 3 : 1, [&]() -> int {
     if (m > 0) {
       cfmm::adj_entries_kernel<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(ix.keys.p, np, nt, kin.p, vin.p);
       CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(temp.p, bytes, kin.p, kout.p, vin.p, ix.adj_pair.p, (int)m, 0,
                                                   end_bit, st));
-      ctx->launches += 2;
     }
     const int64_t th = std::max(m, nt + 1);
     cfmm::adj_finish_kernel<<<(unsigned)((th + 255) / 256), 256, 0, st>>>(kout.p, m, nt, ix.adj_nbr.p, ix.adj_off.p);
-    ctx->launches++;
-  }
-  CU_TRY(ctx, cudaGetLastError());
+    return CFMM_OK;
+  });
+  if (rc2 != CFMM_OK) return rc2;
   ix.adj_off_host.resize((size_t)nt + 1);
-  CU_TRY(ctx, cudaMemcpyAsync(ix.adj_off_host.data(), ix.adj_off.p, ((size_t)nt + 1) * sizeof(int64_t),
-                              cudaMemcpyDeviceToHost, st));
+  CU_TRY(ctx, read_back(ctx, ix.adj_off_host.data(), ix.adj_off.p, (size_t)nt + 1));
   CU_TRY(ctx, cudaStreamSynchronize(st));
   ix.adj_built = true;
   return CFMM_OK;
@@ -3626,10 +3501,6 @@ int scan_arbitrage(cfmm_ctx* ctx, int64_t nb, const int64_t* base, const double*
     if (e == cudaSuccess && b > temp.n) e = temp.alloc(b);
     return e == cudaSuccess ? cub::DeviceScan::ExclusiveSum(temp.p, b, in, out, (int)n, st) : e;
   };
-  const auto d2h_now = [&](void* dst, const void* src, size_t bytes) {
-    cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st);
-    return e == cudaSuccess ? cudaStreamSynchronize(st) : e;
-  };
   const auto blocks = [](int64_t threads) { return (unsigned)((threads + 255) / 256); };
   OrderSets os;
   if ((rc = order_sets(ctx, false, os)) != CFMM_OK) return rc;
@@ -3637,21 +3508,17 @@ int scan_arbitrage(cfmm_ctx* ctx, int64_t nb, const int64_t* base, const double*
   DevBuf<long long> rate;
   CU_TRY(ctx, rate.alloc((size_t)(2 * np)));
   CU_TRY(ctx, cudaMemsetAsync(rate.p, 0, (size_t)(2 * np) * sizeof(long long), st));
-  {
-    ProfScope prof(ctx, kProfSwaps, st);
-    cfmm::arb_rates_kernel<<<blocks(ctx->n_pools), 256, 0, st>>>(os.d_P.p, ix.off.p, ix.pool.p, ix.keys.p, np,
-                                                                 ctx->n_tokens, rate.p);
-  }
-  ctx->launches++;
-  CU_TRY(ctx, cudaGetLastError());
+  if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+         cfmm::arb_rates_kernel<<<blocks(ctx->n_pools), 256, 0, st>>>(os.d_P.p, ix.off.p, ix.pool.p, ix.keys.p, np,
+                                                                      ctx->n_tokens, rate.p);
+       })) != CFMM_OK)
+    return rc;
   // candidates, one warp per slot, then their rows in slot order
   DevBuf<int64_t> d_base, d_slot_off, flag, nhub, row_pos, hub_pos;
   DevBuf<int32_t> slot_hub, slot_lists;
   DevBuf<double> d_min;
-  CU_TRY(ctx, d_base.alloc((size_t)nb));
-  CU_TRY(ctx, DevBuf<int64_t>::copy_in(d_base.p, base, (size_t)nb * sizeof(int64_t)));
-  CU_TRY(ctx, d_min.alloc((size_t)nb));
-  CU_TRY(ctx, DevBuf<double>::copy_in(d_min.p, min_profit, (size_t)nb * sizeof(double)));
+  CU_TRY(ctx, d_base.upload(base, (size_t)nb));
+  CU_TRY(ctx, d_min.upload(min_profit, (size_t)nb));
   CU_TRY(ctx, d_slot_off.upload(slot_off));
   CU_TRY(ctx, flag.alloc((size_t)ns + 1));
   CU_TRY(ctx, nhub.alloc((size_t)ns + 1));
@@ -3662,19 +3529,19 @@ int scan_arbitrage(cfmm_ctx* ctx, int64_t nb, const int64_t* base, const double*
   CU_TRY(ctx, cudaMemsetAsync(flag.p, 0, ((size_t)ns + 1) * sizeof(int64_t), st));
   CU_TRY(ctx, cudaMemsetAsync(nhub.p, 0, ((size_t)ns + 1) * sizeof(int64_t), st));
   const cfmm::AdjView A{ix.adj_off.p, ix.adj_nbr.p, ix.adj_pair.p};
-  {
-    ProfScope prof(ctx, kProfSwaps, st);
-    cfmm::arb_candidates_kernel<<<blocks(32 * ns), 256, 0, st>>>(A, reinterpret_cast<const double*>(rate.p), d_base.p,
-                                                                  d_slot_off.p, nb, max_hubs, flag.p, nhub.p,
-                                                                  slot_hub.p, slot_lists.p);
-    CU_TRY(ctx, cub_scan(flag.p, row_pos.p, ns + 1));
-    CU_TRY(ctx, cub_scan(nhub.p, hub_pos.p, ns + 1));
-  }
-  ctx->launches += 3;
-  CU_TRY(ctx, cudaGetLastError());
+  if ((rc = launch(ctx, kProfSwaps, 3, [&]() -> int {
+         cfmm::arb_candidates_kernel<<<blocks(32 * ns), 256, 0, st>>>(A, reinterpret_cast<const double*>(rate.p),
+                                                                       d_base.p, d_slot_off.p, nb, max_hubs, flag.p,
+                                                                       nhub.p, slot_hub.p, slot_lists.p);
+         CU_TRY(ctx, cub_scan(flag.p, row_pos.p, ns + 1));
+         CU_TRY(ctx, cub_scan(nhub.p, hub_pos.p, ns + 1));
+         return CFMM_OK;
+       })) != CFMM_OK)
+    return rc;
   int64_t q = 0, nh = 0;
-  CU_TRY(ctx, d2h_now(&q, row_pos.p + ns, sizeof(int64_t)));
-  CU_TRY(ctx, d2h_now(&nh, hub_pos.p + ns, sizeof(int64_t)));
+  CU_TRY(ctx, read_back(ctx, &q, row_pos.p + ns, 1));
+  CU_TRY(ctx, read_back(ctx, &nh, hub_pos.p + ns, 1));
+  CU_TRY(ctx, cudaStreamSynchronize(st));
   if (q == 0) return CFMM_OK;
   DevBuf<int64_t> tin, tout, row_b, hub_off, d_hubs, pair;
   DevBuf<double> surplus, d_profit, d_price;
@@ -3689,24 +3556,20 @@ int scan_arbitrage(cfmm_ctx* ctx, int64_t nb, const int64_t* base, const double*
   CU_TRY(ctx, d_profit.alloc((size_t)q));
   CU_TRY(ctx, d_price.alloc((size_t)q));
   CU_TRY(ctx, status.alloc((size_t)q));
-  {
-    ProfScope prof(ctx, kProfSwaps, st);
-    cfmm::arb_rows_kernel<<<blocks(ns + 1), 256, 0, st>>>(A, d_base.p, d_slot_off.p, nb, flag.p, nhub.p, slot_hub.p,
-                                                          slot_lists.p, row_pos.p, hub_pos.p, tin.p, tout.p, row_b.p,
-                                                          hub_off.p, d_hubs.p, pair.p);
-  }
-  ctx->launches++;
-  CU_TRY(ctx, cudaGetLastError());
+  if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+         cfmm::arb_rows_kernel<<<blocks(ns + 1), 256, 0, st>>>(A, d_base.p, d_slot_off.p, nb, flag.p, nhub.p,
+                                                               slot_hub.p, slot_lists.p, row_pos.p, hub_pos.p, tin.p,
+                                                               tout.p, row_b.p, hub_off.p, d_hubs.p, pair.p);
+       })) != CFMM_OK)
+    return rc;
   // solve: every candidate as an arbitrage row on the current state
   const cfmm::PairIndexView pv{ix.off.p, ix.pool.p};
   cfmm::RouteRows R{tin.p,     tout.p,  nullptr,    nullptr,     nullptr, hub_off.p, d_hubs.p, pair.p, nullptr,
                     surplus.p, d_profit.p, d_price.p, status.p, nullptr, nullptr,   nullptr,  nullptr};
-  {
-    ProfScope prof(ctx, kProfSwaps, st);
-    cfmm::arb_quote_kernel<<<(unsigned)q, 32u * (1u + (unsigned)max_hubs), 0, st>>>(os.d_P.p, pv, R);
-  }
-  ctx->launches++;
-  CU_TRY(ctx, cudaGetLastError());
+  if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+         cfmm::arb_quote_kernel<<<(unsigned)q, 32u * (1u + (unsigned)max_hubs), 0, st>>>(os.d_P.p, pv, R);
+       })) != CFMM_OK)
+    return rc;
   // select: filled rows with profit >= their base's minimum, then (base index, profit desc, x asc) by
   // two stable sorts of the (base index, x)-ordered rows: on the complemented profit bits, then the base
   DevBuf<int64_t> keep, keep_pos;
@@ -3714,15 +3577,16 @@ int scan_arbitrage(cfmm_ctx* ctx, int64_t nb, const int64_t* base, const double*
   CU_TRY(ctx, keep.alloc((size_t)q + 1));
   CU_TRY(ctx, keep_pos.alloc((size_t)q + 1));
   CU_TRY(ctx, key.alloc((size_t)q));
-  {
-    ProfScope prof(ctx, kProfSwaps, st);
-    cfmm::arb_keep_kernel<<<blocks(q + 1), 256, 0, st>>>(status.p, d_profit.p, row_b.p, d_min.p, q, keep.p, key.p);
-    CU_TRY(ctx, cub_scan(keep.p, keep_pos.p, q + 1));
-  }
-  ctx->launches += 2;
-  CU_TRY(ctx, cudaGetLastError());
+  if ((rc = launch(ctx, kProfSwaps, 2, [&]() -> int {
+         cfmm::arb_keep_kernel<<<blocks(q + 1), 256, 0, st>>>(status.p, d_profit.p, row_b.p, d_min.p, q, keep.p,
+                                                              key.p);
+         CU_TRY(ctx, cub_scan(keep.p, keep_pos.p, q + 1));
+         return CFMM_OK;
+       })) != CFMM_OK)
+    return rc;
   int64_t n_sel = 0;
-  CU_TRY(ctx, d2h_now(&n_sel, keep_pos.p + q, sizeof(int64_t)));
+  CU_TRY(ctx, read_back(ctx, &n_sel, keep_pos.p + q, 1));
+  CU_TRY(ctx, cudaStreamSynchronize(st));
   *found = n_sel;
   const int64_t n_out = std::min(n_sel, cap);
   if (n_out == 0) return CFMM_OK;
@@ -3750,27 +3614,27 @@ int scan_arbitrage(cfmm_ctx* ctx, int64_t nb, const int64_t* base, const double*
   CU_TRY(ctx, o_hubs.alloc((size_t)(cfmm::kRouteMaxHubs * n_out)));
   CU_TRY(ctx, o_profit.alloc((size_t)n_out));
   CU_TRY(ctx, o_price.alloc((size_t)n_out));
-  {
-    ProfScope prof(ctx, kProfSwaps, st);
-    cfmm::arb_select_kernel<<<blocks(q), 256, 0, st>>>(keep_pos.p, key.p, q, sel.p, sel_key.p);
-    s1 = temp.n;
-    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(temp.p, s1, sel_key.p, key_s.p, sel.p, v1.p, (int)n_sel, 0, 64, st));
-    cfmm::arb_base_key_kernel<<<blocks(n_sel), 256, 0, st>>>(v1.p, n_sel, row_b.p, b1.p);
-    s2 = temp.n;
-    CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(temp.p, s2, b1.p, b_s.p, v1.p, v2.p, (int)n_sel, 0, b_bits, st));
-    cfmm::arb_output_kernel<<<blocks(n_out), 256, 0, st>>>(v2.p, n_out, tin.p, tout.p, hub_off.p, d_hubs.p,
-                                                           d_profit.p, d_price.p, o_base.p, o_other.p, o_count.p,
-                                                           o_hubs.p, o_profit.p, o_price.p);
-  }
-  ctx->launches += 5;
-  CU_TRY(ctx, cudaGetLastError());
-  const size_t n8 = (size_t)n_out * sizeof(int64_t);
-  CU_TRY(ctx, cudaMemcpyAsync(row_base, o_base.p, n8, cudaMemcpyDeviceToHost, st));
-  CU_TRY(ctx, cudaMemcpyAsync(row_other, o_other.p, n8, cudaMemcpyDeviceToHost, st));
-  CU_TRY(ctx, cudaMemcpyAsync(hub_count, o_count.p, n8, cudaMemcpyDeviceToHost, st));
-  CU_TRY(ctx, cudaMemcpyAsync(hubs, o_hubs.p, n8 * cfmm::kRouteMaxHubs, cudaMemcpyDeviceToHost, st));
-  CU_TRY(ctx, cudaMemcpyAsync(profit, o_profit.p, (size_t)n_out * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CU_TRY(ctx, cudaMemcpyAsync(price, o_price.p, (size_t)n_out * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if ((rc = launch(ctx, kProfSwaps, 5, [&]() -> int {
+         cfmm::arb_select_kernel<<<blocks(q), 256, 0, st>>>(keep_pos.p, key.p, q, sel.p, sel_key.p);
+         s1 = temp.n;
+         CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(temp.p, s1, sel_key.p, key_s.p, sel.p, v1.p, (int)n_sel, 0, 64,
+                                                     st));
+         cfmm::arb_base_key_kernel<<<blocks(n_sel), 256, 0, st>>>(v1.p, n_sel, row_b.p, b1.p);
+         s2 = temp.n;
+         CU_TRY(ctx, cub::DeviceRadixSort::SortPairs(temp.p, s2, b1.p, b_s.p, v1.p, v2.p, (int)n_sel, 0, b_bits, st));
+         cfmm::arb_output_kernel<<<blocks(n_out), 256, 0, st>>>(v2.p, n_out, tin.p, tout.p, hub_off.p, d_hubs.p,
+                                                                d_profit.p, d_price.p, o_base.p, o_other.p,
+                                                                o_count.p, o_hubs.p, o_profit.p, o_price.p);
+         return CFMM_OK;
+       })) != CFMM_OK)
+    return rc;
+  const size_t n = (size_t)n_out;
+  CU_TRY(ctx, read_back(ctx, row_base, o_base.p, n));
+  CU_TRY(ctx, read_back(ctx, row_other, o_other.p, n));
+  CU_TRY(ctx, read_back(ctx, hub_count, o_count.p, n));
+  CU_TRY(ctx, read_back(ctx, hubs, o_hubs.p, n * cfmm::kRouteMaxHubs));
+  CU_TRY(ctx, read_back(ctx, profit, o_profit.p, n));
+  CU_TRY(ctx, read_back(ctx, price, o_price.p, n));
   CU_TRY(ctx, cudaStreamSynchronize(st));
   return CFMM_OK;
 }
@@ -3799,16 +3663,13 @@ int cfmm_pair_pools(cfmm_ctx* ctx, int64_t q, const int64_t* token_a, const int6
   DevBuf<int64_t> d_cum, d_ent;
   CU_TRY(ctx, d_cum.upload(cum));
   CU_TRY(ctx, d_ent.alloc((size_t)total));
-  {
-    ProfScope prof(ctx, kProfSwaps, ctx->stream);
-    cfmm::pair_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(
-        ctx->pairs.off.p, ctx->pairs.pool.p, d_pair.p, d_cum.p, q, total, d_ent.p);
-  }
-  ctx->launches++;
-  CU_TRY(ctx, cudaGetLastError());
+  if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+         cfmm::pair_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(
+             ctx->pairs.off.p, ctx->pairs.pool.p, d_pair.p, d_cum.p, q, total, d_ent.p);
+       })) != CFMM_OK)
+    return rc;
   std::vector<int64_t> ent((size_t)total);
-  CU_TRY(ctx, cudaMemcpyAsync(ent.data(), d_ent.p, (size_t)total * sizeof(int64_t), cudaMemcpyDeviceToHost,
-                              ctx->stream));
+  CU_TRY(ctx, read_back(ctx, ent.data(), d_ent.p, (size_t)total));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   for (int64_t t = 0; t < total; ++t) {  // (set, device position) -> (type, index in the type's insertion order)
     const int k = (int)(ent[(size_t)t] >> cfmm::kPairSetShift);
@@ -3920,7 +3781,7 @@ int check_liquidity_rows(cfmm_ctx* ctx, int64_t q, const int64_t* pool, const do
 // listing order) and, when tick counts change, the set's new CSR arrays (stage B).
 struct LiquidityStage {
   PoolSet* s = nullptr;
-  PoolGroups g;
+  Groups g;
   std::vector<int64_t> new_nt, cum;   // per touched pool: new tick count, listing offsets [n + 1]
   std::vector<double> top;            // per touched pool: its highest candidate boundary
   int64_t growth = 0;                 // ticks added to the set
@@ -3935,7 +3796,7 @@ int liquidity_stage(cfmm_ctx* ctx, LiquidityStage& st, const SetRows& r, const d
                     const double* d_range, const double* d_dL, unsigned long long* d_bad) {
   PoolSet& s = *st.s;
   st.g = group_by_pool(r, s.m_padded);
-  const int64_t n = (int64_t)st.g.pos.size();
+  const int64_t n = (int64_t)st.g.key.size();
   std::vector<int64_t> cand_off(1, 0);
   std::vector<double> cand;
   st.top.resize((size_t)n);
@@ -3953,7 +3814,7 @@ int liquidity_stage(cfmm_ctx* ctx, LiquidityStage& st, const SetRows& r, const d
   }
   DevBuf<int64_t> d_cand_off, d_nt;
   DevBuf<double> d_cand;
-  CU_TRY(ctx, st.d_pos.upload(st.g.pos));
+  CU_TRY(ctx, st.d_pos.upload(st.g.key));
   CU_TRY(ctx, st.d_row_off.upload(st.g.off));
   CU_TRY(ctx, st.d_rows.upload(st.g.rows));
   CU_TRY(ctx, d_cand_off.upload(cand_off));
@@ -3962,18 +3823,19 @@ int liquidity_stage(cfmm_ctx* ctx, LiquidityStage& st, const SetRows& r, const d
   const cfmm::Univ3State u = univ3_state(s);
   const int threads = 256;
   const unsigned pool_blocks = (unsigned)((n + threads - 1) / threads);
-  cfmm::univ3_liq_ladder_kernel<<<pool_blocks, threads, 0, ctx->stream>>>(u, st.d_pos.p, d_cand_off.p, d_cand.p, n,
-                                                                          d_nt.p, nullptr, nullptr, nullptr);
-  ctx->launches++;
-  CU_TRY(ctx, cudaGetLastError());
+  int rc;
+  if ((rc = launch(ctx, kNoProf, 1, [&] {
+         cfmm::univ3_liq_ladder_kernel<<<pool_blocks, threads, 0, ctx->stream>>>(u, st.d_pos.p, d_cand_off.p, d_cand.p,
+                                                                               n, d_nt.p, nullptr, nullptr, nullptr);
+       })) != CFMM_OK)
+    return rc;
   st.new_nt.resize((size_t)n);
-  CU_TRY(ctx, cudaMemcpyAsync(st.new_nt.data(), d_nt.p, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost,
-                              ctx->stream));
+  CU_TRY(ctx, read_back(ctx, st.new_nt.data(), d_nt.p, (size_t)n));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   st.cum.assign((size_t)n + 1, 0);
   for (int64_t j = 0; j < n; ++j) {
     st.cum[(size_t)j + 1] = st.cum[(size_t)j] + st.new_nt[(size_t)j];
-    st.growth += st.new_nt[(size_t)j] - s.n_ticks[(size_t)s.order[(size_t)st.g.pos[(size_t)j]]];
+    st.growth += st.new_nt[(size_t)j] - s.n_ticks[(size_t)s.order[(size_t)st.g.key[(size_t)j]]];
   }
   if (s.total_ticks + st.growth > (int64_t)0x7fffffff)
     return fail(ctx, CFMM_ERR_INVALID, "modify_univ3_liquidity: more than 2^31-1 ticks in one pool set");
@@ -3981,12 +3843,13 @@ int liquidity_stage(cfmm_ctx* ctx, LiquidityStage& st, const SetRows& r, const d
   CU_TRY(ctx, st.d_cum.upload(st.cum));
   CU_TRY(ctx, st.d_lower.alloc((size_t)n_ticks));
   CU_TRY(ctx, st.d_liq.alloc((size_t)n_ticks));
-  cfmm::univ3_liq_ladder_kernel<<<pool_blocks, threads, 0, ctx->stream>>>(u, st.d_pos.p, d_cand_off.p, d_cand.p, n,
-                                                                          nullptr, st.d_cum.p, st.d_lower.p, st.d_liq.p);
-  cfmm::univ3_liq_apply_kernel<<<(unsigned)((n_ticks + threads - 1) / threads), threads, 0, ctx->stream>>>(
-      st.d_cum.p, n, n_ticks, st.d_row_off.p, st.d_rows.p, d_range, d_dL, st.d_lower.p, st.d_liq.p, d_bad);
-  ctx->launches += 2;
-  CU_TRY(ctx, cudaGetLastError());
+  if ((rc = launch(ctx, kNoProf, 2, [&] {
+         cfmm::univ3_liq_ladder_kernel<<<pool_blocks, threads, 0, ctx->stream>>>(
+             u, st.d_pos.p, d_cand_off.p, d_cand.p, n, nullptr, st.d_cum.p, st.d_lower.p, st.d_liq.p);
+         cfmm::univ3_liq_apply_kernel<<<(unsigned)((n_ticks + threads - 1) / threads), threads, 0, ctx->stream>>>(
+             st.d_cum.p, n, n_ticks, st.d_row_off.p, st.d_rows.p, d_range, d_dL, st.d_lower.p, st.d_liq.p, d_bad);
+       })) != CFMM_OK)
+    return rc;
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // (the candidate arrays are freed on return)
   return CFMM_OK;
 }
@@ -4006,24 +3869,25 @@ cudaError_t liquidity_alloc(LiquidityStage& st) {
 // Stage B of one set: commit the new ladders and rebuild the tick records.
 int liquidity_commit(cfmm_ctx* ctx, LiquidityStage& st) {
   PoolSet& s = *st.s;
-  const int64_t n = (int64_t)st.g.pos.size();
+  const int64_t n = (int64_t)st.g.key.size();
   const int threads = 256;
   if (st.growth == 0) {  // same tick counts: the new liquidities go through the update path
     CU_TRY(ctx, univ3_rebuild(ctx, s, st.d_pos.p, st.d_cum.p, n, st.cum[(size_t)n], nullptr, st.d_liq.p, false));
   } else {
     std::vector<int64_t> shift((size_t)n + 1, 0);
     for (int64_t j = 0; j < n; ++j)
-      shift[(size_t)j + 1] = shift[(size_t)j] + st.new_nt[(size_t)j] - s.n_ticks[(size_t)s.order[(size_t)st.g.pos[(size_t)j]]];
+      shift[(size_t)j + 1] = shift[(size_t)j] + st.new_nt[(size_t)j] - s.n_ticks[(size_t)s.order[(size_t)st.g.key[(size_t)j]]];
     DevBuf<int64_t> d_shift;
     CU_TRY(ctx, d_shift.upload(shift));
     const int64_t total = s.total_ticks + st.growth;
-    cfmm::univ3_splice_offsets_kernel<<<(unsigned)((s.m + threads - 1) / threads), threads, 0, ctx->stream>>>(
-        s.d_tick.p, st.n_tick.p, s.m, st.d_pos.p, d_shift.p, n);
-    cfmm::univ3_splice_ticks_kernel<<<(unsigned)((total + threads - 1) / threads), threads, 0, ctx->stream>>>(
-        s.d_tick.p, st.n_tick.p, s.m, total, st.d_pos.p, st.d_cum.p, n, st.d_lower.p, st.d_liq.p, s.d_lower.p,
-        s.d_liq.p, st.n_lower.p, st.n_liq.p);
-    ctx->launches += 2;
-    CU_TRY(ctx, cudaGetLastError());
+    const int rc = launch(ctx, kNoProf, 2, [&] {
+      cfmm::univ3_splice_offsets_kernel<<<(unsigned)((s.m + threads - 1) / threads), threads, 0, ctx->stream>>>(
+          s.d_tick.p, st.n_tick.p, s.m, st.d_pos.p, d_shift.p, n);
+      cfmm::univ3_splice_ticks_kernel<<<(unsigned)((total + threads - 1) / threads), threads, 0, ctx->stream>>>(
+          s.d_tick.p, st.n_tick.p, s.m, total, st.d_pos.p, st.d_cum.p, n, st.d_lower.p, st.d_liq.p, s.d_lower.p,
+          s.d_liq.p, st.n_lower.p, st.n_liq.p);
+    });
+    if (rc != CFMM_OK) return rc;
     CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     std::swap(s.d_lower, st.n_lower);
     std::swap(s.d_liq, st.n_liq);
@@ -4033,7 +3897,7 @@ int liquidity_commit(cfmm_ctx* ctx, LiquidityStage& st) {
     CU_TRY(ctx, univ3_rebuild(ctx, s, nullptr, nullptr, s.m, s.total_ticks, nullptr, nullptr, true));
   }
   for (int64_t j = 0; j < n; ++j) {
-    const int64_t i = s.order[(size_t)st.g.pos[(size_t)j]];
+    const int64_t i = s.order[(size_t)st.g.key[(size_t)j]];
     s.n_ticks[(size_t)i] = st.new_nt[(size_t)j];
     s.first_lower[(size_t)i] = std::max(s.first_lower[(size_t)i], st.top[(size_t)j]);
   }
@@ -4051,10 +3915,8 @@ int cfmm_modify_univ3_liquidity(cfmm_ctx* ctx, int64_t q, const int64_t* pool, c
   if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
   DevBuf<double> d_range, d_dL;
   DevBuf<unsigned long long> d_bad;
-  CU_TRY(ctx, d_range.alloc((size_t)(2 * q)));
-  CU_TRY(ctx, DevBuf<double>::copy_in(d_range.p, range, (size_t)(2 * q) * sizeof(double)));
-  CU_TRY(ctx, d_dL.alloc((size_t)q));
-  CU_TRY(ctx, DevBuf<double>::copy_in(d_dL.p, dL, (size_t)q * sizeof(double)));
+  CU_TRY(ctx, d_range.upload(range, (size_t)(2 * q)));
+  CU_TRY(ctx, d_dL.upload(dL, (size_t)q));
   CU_TRY(ctx, d_bad.alloc(1));
   CU_TRY(ctx, cudaMemsetAsync(d_bad.p, 0xff, sizeof(unsigned long long), ctx->stream));
   // stage A for every set first: a row that fails anywhere rejects the whole call
@@ -4066,7 +3928,7 @@ int cfmm_modify_univ3_liquidity(cfmm_ctx* ctx, int64_t q, const int64_t* pool, c
     if ((rc = liquidity_stage(ctx, *stages.back(), r, range, d_range.p, d_dL.p, d_bad.p)) != CFMM_OK) return rc;
   }
   unsigned long long bad = 0;
-  CU_TRY(ctx, cudaMemcpyAsync(&bad, d_bad.p, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
+  CU_TRY(ctx, read_back(ctx, &bad, d_bad.p, 1));
   CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   if (bad != ~0ull)
     return fail(ctx, CFMM_ERR_INVALID,
@@ -4116,16 +3978,14 @@ int cfmm_get_univ3_ticks(cfmm_ctx* ctx, int64_t first, int64_t count, int64_t* t
       CU_TRY(ctx, d_lo.alloc((size_t)n_ticks));
       CU_TRY(ctx, d_lq.alloc((size_t)n_ticks));
       const int threads = 256;
-      cfmm::univ3_gather_ticks_kernel<<<(unsigned)((n_ticks + threads - 1) / threads), threads, 0, ctx->stream>>>(
-          univ3_state(s), d_pos.p, d_cum.p, sp.count, n_ticks, d_lo.p, d_lq.p);
-      ctx->launches++;
-      CU_TRY(ctx, cudaGetLastError());
-      if (lower_ticks)
-        CU_TRY(ctx, cudaMemcpyAsync(lower_ticks + base, d_lo.p, (size_t)n_ticks * sizeof(double),
-                                    cudaMemcpyDeviceToHost, ctx->stream));
-      if (liquidity)
-        CU_TRY(ctx, cudaMemcpyAsync(liquidity + base, d_lq.p, (size_t)n_ticks * sizeof(double),
-                                    cudaMemcpyDeviceToHost, ctx->stream));
+      if ((rc = launch(ctx, kNoProf, 1, [&] {
+             cfmm::univ3_gather_ticks_kernel<<<(unsigned)((n_ticks + threads - 1) / threads), threads, 0,
+                                               ctx->stream>>>(univ3_state(s), d_pos.p, d_cum.p, sp.count, n_ticks,
+                                                              d_lo.p, d_lq.p);
+           })) != CFMM_OK)
+        return rc;
+      CU_TRY(ctx, read_back(ctx, lower_ticks ? lower_ticks + base : nullptr, d_lo.p, (size_t)n_ticks));
+      CU_TRY(ctx, read_back(ctx, liquidity ? liquidity + base : nullptr, d_lq.p, (size_t)n_ticks));
       CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     }
     base += n_ticks;
@@ -4376,11 +4236,10 @@ int cfmm_selftest_inrange_math(cfmm_ctx* ctx, const double* a, const double* b, 
   CU_TRY(ctx, cudaSetDevice(ctx->device));
   DevBuf<double> da, db;
   DevBuf<unsigned long long> dm;
-  std::vector<double> ha(a, a + n), hb(b, b + n);
-  std::vector<unsigned long long> hz(1, 0);
-  CU_TRY(ctx, da.upload(ha));
-  CU_TRY(ctx, db.upload(hb));
-  CU_TRY(ctx, dm.upload(hz));
+  const unsigned long long zero = 0;
+  CU_TRY(ctx, da.upload(a, (size_t)n));
+  CU_TRY(ctx, db.upload(b, (size_t)n));
+  CU_TRY(ctx, dm.upload(&zero, 1));
   if (n > 0) {
     cfmm::inrange_math_selftest_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(
         da.p, db.p, n, dm.p);
