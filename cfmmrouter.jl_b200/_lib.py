@@ -103,6 +103,8 @@ SYMBOLS = {
                                          _dp, _dp, _dp, _dp]),
     "cfmm_scan_arbitrage": (C.c_int, [_ctx, C.c_int64, _ip, _dp, C.c_int, C.c_int64, _ip, _ip, _ip, _ip, _ip, _dp,
                                       _dp]),
+    "cfmm_choose_order_hubs": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, C.c_int,
+                                         C.POINTER(C.c_uint8), _ip, _ip, _dp, _ip]),
     "cfmm_modify_univ3_liquidity":(C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),

@@ -38,6 +38,7 @@
 #include "split_kernels.cuh"
 #include "route_kernels.cuh"
 #include "arb_scan_kernels.cuh"
+#include "hub_kernels.cuh"
 #include "univ3_state.cuh"
 
 #include <cub/cub.cuh>
@@ -3639,6 +3640,73 @@ int scan_arbitrage(cfmm_ctx* ctx, int64_t nb, const int64_t* base, const double*
   return CFMM_OK;
 }
 
+// ---- hubs chosen for order rows (hub_kernels.cuh) -----------------------------------------------
+
+// Every argument of cfmm_choose_order_hubs, before anything runs: split orders' rows, max_hubs, and
+// the two CSR outputs.
+int check_choose_hubs(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                      const uint8_t* kind, const double* amount, int max_hubs, const int64_t* hub_off,
+                      const int64_t* hubs) {
+  int rc = check_split(ctx, q, token_in, token_out, kind, amount, nullptr, "choose_order_hubs");
+  if (rc != CFMM_OK) return rc;
+  if (max_hubs < 0 || max_hubs > CFMM_ROUTE_MAX_HUBS)
+    return fail(ctx, CFMM_ERR_INVALID, "choose_order_hubs: max_hubs %d, not 0..%d", max_hubs, CFMM_ROUTE_MAX_HUBS);
+  if (q > 0 && (!hub_off || !hubs)) return fail(ctx, CFMM_ERR_INVALID, "choose_order_hubs: null hub_off or hubs");
+  return CFMM_OK;
+}
+
+int choose_order_hubs(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                      const uint8_t* kind, const double* amount, int max_hubs, const uint8_t* allowed,
+                      int64_t* hub_off, int64_t* hubs, double* hub_score, int64_t* n_eligible) {
+  int rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  if ((rc = ensure_adjacency(ctx)) != CFMM_OK) return rc;
+  auto& ix = ctx->pairs;
+  cudaStream_t st = ctx->stream;
+  OrderSets os;
+  if ((rc = order_sets(ctx, false, os)) != CFMM_OK) return rc;
+  const size_t slots = (size_t)q * (size_t)max_hubs;
+  DevBuf<int64_t> d_in, d_out, d_nhub, d_hub, d_elig;
+  DevBuf<uint8_t> d_kind, d_allowed;
+  DevBuf<double> d_amount, d_score;
+  CU_TRY(ctx, d_in.upload(token_in, (size_t)q));
+  CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
+  CU_TRY(ctx, d_kind.upload(kind, (size_t)q));
+  CU_TRY(ctx, d_amount.upload(amount, (size_t)q));
+  CU_TRY(ctx, d_allowed.upload(allowed, (size_t)ctx->n_tokens));
+  CU_TRY(ctx, d_nhub.alloc((size_t)q));
+  CU_TRY(ctx, d_elig.alloc((size_t)q));
+  CU_TRY(ctx, d_hub.alloc(slots));
+  CU_TRY(ctx, d_score.alloc(slots));
+  const cfmm::PairIndexView pv{ix.off.p, ix.pool.p};
+  const cfmm::AdjView A{ix.adj_off.p, ix.adj_nbr.p, ix.adj_pair.p};
+  if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+         cfmm::hub_choice_kernel<<<(unsigned)((32 * q + 255) / 256), 256, 0, st>>>(
+             os.d_P.p, pv, A, d_in.p, d_out.p, d_kind.p, d_amount.p, q, max_hubs, d_allowed.p, d_nhub.p, d_hub.p,
+             d_score.p, d_elig.p);
+       })) != CFMM_OK)
+    return rc;
+  std::vector<int64_t> nhub((size_t)q), hub(slots);
+  std::vector<double> score(hub_score ? slots : 0);
+  CU_TRY(ctx, read_back(ctx, nhub.data(), d_nhub.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, hub.data(), d_hub.p, slots));
+  CU_TRY(ctx, read_back(ctx, hub_score ? score.data() : nullptr, d_score.p, slots));
+  CU_TRY(ctx, read_back(ctx, n_eligible, d_elig.p, (size_t)q));
+  CU_TRY(ctx, cudaStreamSynchronize(st));
+  // pack each row's first nhub[r] slots
+  hub_off[0] = 0;
+  for (int64_t r = 0; r < q; ++r) {
+    const int64_t g = hub_off[r];
+    for (int64_t h = 0; h < nhub[(size_t)r]; ++h) {
+      hubs[g + h] = hub[(size_t)(max_hubs * r + h)];
+      if (hub_score) hub_score[g + h] = score[(size_t)(max_hubs * r + h)];
+    }
+    hub_off[r + 1] = g + nhub[(size_t)r];
+  }
+  return CFMM_OK;
+}
+
 }  // namespace
 
 int cfmm_pair_pools(cfmm_ctx* ctx, int64_t q, const int64_t* token_a, const int64_t* token_b, int64_t* count,
@@ -3751,6 +3819,19 @@ int cfmm_scan_arbitrage(cfmm_ctx* ctx, int64_t nb, const int64_t* base, const do
   if (nb == 0) return CFMM_OK;
   return scan_arbitrage(ctx, nb, base, min_profit, max_hubs, cap, found, row_base, row_other, hub_count, hubs, profit,
                         price);
+}
+
+int cfmm_choose_order_hubs(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                           const uint8_t* kind, const double* amount, int max_hubs, const uint8_t* allowed,
+                           int64_t* hub_off, int64_t* hubs, double* hub_score, int64_t* n_eligible) {
+  int rc = check_choose_hubs(ctx, q, token_in, token_out, kind, amount, max_hubs, hub_off, hubs);
+  if (rc != CFMM_OK) return rc;
+  if (q == 0) {
+    if (hub_off) hub_off[0] = 0;
+    return CFMM_OK;
+  }
+  return choose_order_hubs(ctx, q, token_in, token_out, kind, amount, max_hubs, allowed, hub_off, hubs, hub_score,
+                           n_eligible);
 }
 
 // ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------

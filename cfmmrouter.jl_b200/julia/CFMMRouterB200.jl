@@ -569,6 +569,28 @@ function scan_arbitrage(ctx, base::Vector{Int64}, min_profit::Vector{Float64}, m
     return found[], rb[1:n], ro[1:n], hub_off, hubs, pr[1:n], px[1:n]
 end
 
+# Hub tokens chosen for order rows (cfmm_choose_order_hubs): up to max_hubs (0..7) common neighbours of
+# token_in[r] and token_out[r] per row, ranked by their best single two-hop route; allowed (nothing:
+# every token) is a mask over the tokens.  Returns (hub_off, hubs, score, n_eligible); hub_off and hubs
+# go to quote_routed_orders / execute_routed_orders! as they are.  Never executed, like the rest of
+# this file.
+function choose_order_hubs(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}, kind::Vector{UInt8},
+                           amount::Vector{Float64}, max_hubs::Integer,
+                           allowed::Union{Nothing,Vector{UInt8}}=nothing)
+    q = length(token_in)
+    length(token_out) == length(kind) == length(amount) == q ||
+        throw(ArgumentError("token_in / token_out / kind / amount need q entries"))
+    cap = max(q * max_hubs, 1)
+    hub_off, hubs, score, n_elig = zeros(Int64, q + 1), zeros(Int64, cap), zeros(cap), zeros(Int64, q)
+    chk(ctx, ccall((:cfmm_choose_order_hubs, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Cint, Ptr{UInt8}, Ptr{Int64},
+         Ptr{Int64}, Ptr{Float64}, Ptr{Int64}),
+        ctx, q, token_in, token_out, kind, amount, max_hubs, allowed === nothing ? C_NULL : allowed, hub_off,
+        hubs, score, n_elig))
+    n = hub_off[end]
+    return hub_off, hubs[1:n], score[1:n], n_elig
+end
+
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
 # current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never

@@ -639,6 +639,38 @@ class DevicePools:
         hubs = np.concatenate([hb[r, :hc[r]] for r in range(n)]).astype(np.int64) if n else np.zeros(0, np.int64)
         return int(found[0]), rb, ro, hub_off, hubs, pr, px
 
+    # -- hub tokens chosen for order rows (include/cfmm_b200.h, cfmm_choose_order_hubs) ------------
+    def choose_order_hubs(self, token_in, token_out, kind, amount, max_hubs: int = _lib.ROUTE_MAX_HUBS,
+                          allowed=None):
+        """cfmm_choose_order_hubs: for row j (sell token_in[j] for token_out[j], 1-based; kind 0
+        tenders amount[j], kind 1 wants amount[j]) the common neighbours h of the two tokens (with
+        allowed[h - 1] when a mask [n_tokens] is given), ranked by their best single two-hop route: the
+        most received (kind 0) or the least paid (kind 1) through the best pool of each hop.  No state
+        changes.  Returns (hub_off [q + 1], hubs [Σ] best first, score [Σ], n_eligible [q]); hub_off
+        and hubs go to quote_routed_orders / execute_routed_orders as they are."""
+        tin = np.ascontiguousarray(token_in, dtype=np.int64).reshape(-1)
+        tout = np.ascontiguousarray(token_out, dtype=np.int64).reshape(-1)
+        kind = np.ascontiguousarray(kind, dtype=np.uint8).reshape(-1)
+        amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
+        q = len(tin)
+        if not (len(tout) == len(kind) == len(amount) == q):
+            raise ValueError("choose_order_hubs: token_in, token_out, kind and amount need one entry per row")
+        u8 = C.POINTER(C.c_uint8)
+        mask = None
+        if allowed is not None:
+            mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
+            if len(mask) != self.n_tokens:
+                raise ValueError(f"choose_order_hubs: allowed must have {self.n_tokens} entries, one per token")
+        cap = q * max(int(max_hubs), 0)
+        hub_off, hubs = np.zeros(q + 1, dtype=np.int64), np.zeros(max(cap, 1), dtype=np.int64)
+        score, n_elig = np.zeros(max(cap, 1)), np.zeros(q, dtype=np.int64)
+        self._chk(self._lib.cfmm_choose_order_hubs(self._ctx, q, _ip(tin), _ip(tout), kind.ctypes.data_as(u8),
+                                                   _dp(amount), int(max_hubs),
+                                                   None if mask is None else mask.ctypes.data_as(u8), _ip(hub_off),
+                                                   _ip(hubs), _dp(score), _ip(n_elig)))
+        n = int(hub_off[-1])
+        return hub_off, hubs[:n].copy(), score[:n].copy(), n_elig
+
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
         """cfmm_modify_univ3_liquidity: row j adds dL[j] (> 0 mints, < 0 burns) to the ticks of UniV3
@@ -1117,6 +1149,45 @@ class Router:
             _, typ, idx, _ = self._pools.pair_pools(a, b)
             self._refresh_swapped([(t, None, idx[typ == t]) for t in (0, 1, 2) if np.any(typ == t)])
         return out
+
+    def _choose(self, token_in, token_out, kinds, amounts, max_hubs, allowed, what):
+        tin, tout, kinds, amounts, _ = self._split_args(token_in, token_out, kinds, amounts, None, what)
+        if not 0 <= int(max_hubs) <= _lib.ROUTE_MAX_HUBS:
+            raise ValueError(f"{what}: max_hubs must be 0..{_lib.ROUTE_MAX_HUBS}")
+        off, flat, _, _ = self._pools.choose_order_hubs(tin, tout, kinds, amounts, int(max_hubs), allowed)
+        return tin, tout, kinds, amounts, off, flat
+
+    def choose_hubs(self, token_in, token_out, kinds, amounts, max_hubs: int = _lib.ROUTE_MAX_HUBS, allowed=None):
+        """Choose each order row's hub tokens on the device (cfmm_choose_order_hubs): the common
+        neighbours h of token_in[j] and token_out[j] (1-based; with allowed[h - 1] when a mask over the
+        tokens is given) that carry a two-hop route on active pools, ranked by that route's best single
+        quote (kind 0: most received for amounts[j]; kind 1: least paid for amounts[j] out), at most
+        max_hubs per row.  No state changes.  Returns one list of hubs per row, best first, ready for
+        quote_routed_orders / execute_routed_orders.  Single GPU."""
+        _, _, _, _, off, flat = self._choose(token_in, token_out, kinds, amounts, max_hubs, allowed, "choose_hubs")
+        return [flat[off[r]:off[r + 1]].tolist() for r in range(len(off) - 1)]
+
+    def quote_auto_routed_orders(self, token_in, token_out, kinds, amounts, max_hubs: int = _lib.ROUTE_MAX_HUBS,
+                                 allowed=None):
+        """choose_hubs, then quote_routed_orders with the chosen hubs: each row split optimally over its
+        pair's pools and the two-hop routes through its chosen hubs.  No state changes.  Returns
+        (paid [q], received [q], price [q], status [q], hubs), hubs one list per row.  Single GPU."""
+        tin, tout, kinds, amounts, off, flat = self._choose(token_in, token_out, kinds, amounts, max_hubs, allowed,
+                                                            "quote_auto_routed_orders")
+        out = self._pools.quote_routed_orders(tin, tout, kinds, amounts, off, flat)[:4]
+        return out + ([flat[off[r]:off[r + 1]].tolist() for r in range(len(tin))],)
+
+    def execute_auto_routed_orders(self, token_in, token_out, kinds, amounts, limits=None,
+                                   max_hubs: int = _lib.ROUTE_MAX_HUBS, allowed=None):
+        """choose_hubs, then execute_routed_orders with the chosen hubs and the optional limits (kind 0:
+        the minimum received; kind 1: the maximum paid).  Every row's hubs are chosen once, on the state
+        at entry; the execute then re-solves each row, over those hubs, on the state the earlier rows
+        left.  Returns what quote_auto_routed_orders returns and refreshes the touched pool objects, as
+        execute_routed_orders does.  Single GPU."""
+        tin, tout, kinds, amounts, off, flat = self._choose(token_in, token_out, kinds, amounts, max_hubs, allowed,
+                                                            "execute_auto_routed_orders")
+        hubs = [flat[off[r]:off[r + 1]].tolist() for r in range(len(tin))]
+        return self.execute_routed_orders(tin, tout, kinds, amounts, hubs, limits) + (hubs,)
 
     def _arbitrage_args(self, base, other, hubs, min_profit, what):
         if self._world > 1:

@@ -660,6 +660,47 @@ int cfmm_scan_arbitrage(cfmm_ctx *ctx, int64_t nb, const int64_t *base /* [nb] *
                         int64_t *hub_count /* [cap] */, int64_t *hubs /* [cap × 7] */,
                         double *profit /* [cap] */, double *price /* [cap] */);
 
+/* ---- hub tokens chosen for order rows ----------------------------------------------------
+ * For each order row (j = token_in[r], i = token_out[r], kind[r], amount[r], split orders' rules),
+ * up to max_hubs (0..CFMM_ROUTE_MAX_HUBS) hub tokens for cfmm_quote_routed_orders /
+ * cfmm_execute_routed_orders, ranked by the best single two-hop route through each.
+ *   candidates  every token h that is a common neighbour of j and i in cfmm_scan_arbitrage's token
+ *               adjacency (built on first use and kept with the pair index; it lists retired pools'
+ *               pairs, so activity is read per call, from the pools), with allowed[h-1] != 0 when
+ *               allowed [n_tokens] is given (NULL: every token).
+ *   exact-in    (kind CFMM_SWAP_EXACT_IN, δ = amount) x_h = the largest f_k(δ) over the active pools
+ *               k of {j, h} with j tendered, out_h = the largest f_k(x_h) over the active pools of
+ *               {h, i} with h tendered.  f_k is the exact-input quote of one pool, cfmm_quote_swaps
+ *               bit for bit (f_k(0) = 0); NaNs are ignored and a pair with no active pool gives 0.
+ *               h is eligible when out_h > 0; rank out_h descending, then h ascending.
+ *   exact-out   (kind CFMM_SWAP_EXACT_OUT, y = amount) c_h = the smallest x*_k(y) over the active
+ *               pools of {h, i} with h tendered, in_h = the smallest x*_k(c_h) over the active pools
+ *               of {j, h} with j tendered.  x*_k is cfmm_quote_swaps_exact_out's search, bit for bit;
+ *               +inf (unreachable, or no active pool) propagates.  h is eligible when in_h is finite;
+ *               rank in_h ascending, then h ascending.
+ * Outputs: the first max_hubs eligible hubs in rank order, as packed CSR: hub_off [q+1] (hub_off[0]
+ * = 0) and hubs [hub_off[q]] (1-based, at most q·max_hubs), ready for the routed calls, which use
+ * them in the listed order; hub_score [hub_off[q]] (NULL: not written) = out_h or in_h; n_eligible
+ * [q] (NULL: not written) = the eligible hubs before truncation.  A row with amount 0 gets no hubs
+ * and n_eligible 0; max_hubs = 0 gives no hubs but still counts the eligible ones.  Max, min and the
+ * ranking do not depend on the evaluation order, so the result is deterministic.
+ *
+ * The score is that of the best single route through h, not of h's share in an optimal split:
+ * cfmm_quote_routed_orders then splits the row optimally over the direct pools and the chosen hubs'
+ * pools.  Routes through two hubs or pools between hubs are not considered (cfmm_solve's).
+ * Execute: pass the rows with these hubs to cfmm_execute_routed_orders.  The hubs are chosen once,
+ * on the state at this call; the execute then re-solves each row on the state the earlier rows left.
+ *
+ * Synchronous; changes no state.  Before cfmm_finalize: CFMM_ERR_STATE.  CFMM_ERR_INVALID before
+ * anything runs for every argument split orders reject, max_hubs outside 0..CFMM_ROUTE_MAX_HUBS, and
+ * a null hub_off or hubs with q > 0.  q == 0 writes hub_off[0] = 0 (when given) and runs nothing. */
+int cfmm_choose_order_hubs(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [q] */,
+                           const int64_t *token_out /* [q] */, const uint8_t *kind /* [q] */,
+                           const double *amount /* [q] */, int max_hubs,
+                           const uint8_t *allowed /* [n_tokens] or NULL */, int64_t *hub_off /* [q+1] */,
+                           int64_t *hubs /* [q·max_hubs] */, double *hub_score /* [q·max_hubs] or NULL */,
+                           int64_t *n_eligible /* [q] or NULL */);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
@@ -807,8 +848,8 @@ int64_t cfmm_launch_count(const cfmm_ctx *ctx);
  * exchange kernel, or 4 = the kernels of cfmm_quote_swaps / cfmm_execute_swaps /
  * cfmm_quote_swaps_exact_out / cfmm_execute_swap_orders / cfmm_quote_paths /
  * cfmm_execute_paths / cfmm_pair_pools / cfmm_quote_split_orders /
- * cfmm_execute_split_orders / cfmm_quote_routed_orders / cfmm_execute_routed_orders,
- * the pair-index build counted as one launch); it
+ * cfmm_execute_split_orders / cfmm_quote_routed_orders / cfmm_execute_routed_orders /
+ * cfmm_choose_order_hubs, the pair-index build counted as one launch); it
  * synchronises on the recorded events.
  * cfmm_profile_reset re-arms the same N pairs. */
 int cfmm_profile_read(cfmm_ctx *ctx, int type, double *total_ms, int64_t *launches);

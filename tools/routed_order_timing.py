@@ -101,7 +101,8 @@ def mirror_pools_of(p, R, g, Ai, w=None, u=None):
     return pools_of
 
 
-def hub(args, rng):
+def hub_set(rng):
+    """The hub set on a new context: (p, n, the non-hub tokens, ν, the mirror's pools_of)."""
     n, md = 2_000, 20_000
     nu = np.exp(rng.uniform(-1, 1, size=n + 1))
     others = np.arange(8, n + 1)
@@ -126,6 +127,11 @@ def hub(args, rng):
     p.finalize()
     pools_of = mirror_pools_of(p, [Rp, Rg], [gp, gg, gu], [Ap, A, A], wg, (cp, off, lt, lq))
     print(json.dumps(dict(set="hub", pools=len(Ap) + 2 * m, tokens=n)), flush=True)
+    return p, n, others, nu, pools_of
+
+
+def hub(args, rng):
+    p, n, others, nu, pools_of = hub_set(rng)
     for q in (1_000, 100_000):
         tin = rng.choice(others, size=q)
         tout = others[(np.searchsorted(others, tin) + rng.integers(1, len(others), size=q)) % len(others)]
