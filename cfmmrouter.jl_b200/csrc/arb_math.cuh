@@ -16,6 +16,14 @@ struct Trade {
   double l1, l2;  // Λ[1], Λ[2]  (received)
 };
 
+// R <- (R + γ·Δ) − Λ (the update the reference's tests use, test/cfmms.jl:10: R⁺ = R + γ*Δ - Λ)
+__device__ __forceinline__ double2 apply_trade(double2 r, double g, double2 d, double2 l) {
+  double2 n;
+  n.x = __dsub_rn(__dadd_rn(r.x, __dmul_rn(g, d.x)), l.x);
+  n.y = __dsub_rn(__dadd_rn(r.y, __dmul_rn(g, d.y)), l.y);
+  return n;
+}
+
 // Julia's max(x, 0) on Float64: NaN propagates; max(-0.0, 0) == +0.0.
 __device__ __forceinline__ double jl_max0(double x) {
   return (x != x) ? x : (x > 0.0 ? x : 0.0);

@@ -8,7 +8,7 @@
 // is the root of "hub h's pools net to zero in h" (an inner ordinal search per hub), and s* is the
 // split's search on N(s), the net intake of j over all the row's pools.  One CTA runs a row: warp 0
 // owns the direct pools, warp 1 + h owns hub h's pools, and warp partials meet in shared memory in
-// a fixed order.  The pool views, legs, boundaries and transitions are split_kernels.cuh's.
+// a fixed order.  The pool views, legs, boundaries, searches and transitions are split_kernels.cuh's.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -19,62 +19,6 @@ namespace cfmm {
 
 constexpr int kRouteMaxHubs = 7;  // CFMM_ROUTE_MAX_HUBS
 constexpr int kRouteThreads = 32 * (1 + kRouteMaxHubs);
-
-// The gallop and bisection of split_row on the ordinals [kSplitOrdMin, kSplitOrdMax], from o.
-// test(c) evaluates at c and returns enough(c) (true at small c); keep(is_lo) files that evaluation
-// as lo's or hi's.  0: a bracket, enough(lo), !enough(hi), hi = lo + 1.  1: enough at o(DBL_MAX)
-// (lo = o(DBL_MAX)).  2: !enough at o(DBL_MIN) (hi = o(DBL_MIN)).  At most 1 + 63 + 62 tests.
-// split_row keeps its own copy of this loop, so that its instructions stay as they were.
-template <class Test, class Keep>
-__device__ __forceinline__ int route_search(int64_t o, int64_t& lo, int64_t& hi, Test&& test, Keep&& keep) {
-  if (test(o)) {
-    lo = o;
-    keep(true);
-    for (int64_t step = 1;; step <<= 1) {
-      if (lo == kSplitOrdMax) return 1;
-      const int64_t c = kSplitOrdMax - lo <= step ? kSplitOrdMax : lo + step;
-      if (test(c)) {
-        lo = c;
-        keep(true);
-      } else {
-        hi = c;
-        keep(false);
-        break;
-      }
-    }
-  } else {
-    hi = o;
-    keep(false);
-    for (int64_t step = 1;; step <<= 1) {
-      if (hi == kSplitOrdMin) return 2;
-      const int64_t c = hi - kSplitOrdMin <= step ? kSplitOrdMin : hi - step;
-      if (test(c)) {
-        lo = c;
-        keep(true);
-        break;
-      }
-      hi = c;
-      keep(false);
-    }
-  }
-  while (hi - lo > 1) {
-    const int64_t mid = lo + ((hi - lo) >> 1);
-    if (test(mid)) {
-      lo = mid;
-      keep(true);
-    } else {
-      hi = mid;
-      keep(false);
-    }
-  }
-  return 0;
-}
-
-// The ordinal a search starts from: o(e) clamped to [o(DBL_MIN), o(DBL_MAX)], o(DBL_MIN) for a NaN.
-__device__ __forceinline__ int64_t route_start(double e) {
-  const int64_t o = !(e >= 0x1p-1022) ? kSplitOrdMin : __double_as_longlong(e);
-  return o > kSplitOrdMax ? kSplitOrdMax : o;
-}
 
 // The rows of one call (device arrays; tokens 1-based).  Row r's pair lists start at
 // r + 2·hub_off[r] in pair / leg_off: (j, i), then (j, h), (h, i) for each of its hubs in order.
@@ -244,7 +188,7 @@ __device__ __forceinline__ void route_row(const PathSets* P, const PairIndexView
       }
     }
     int64_t tprev = 0;
-    if (mine && W.hub) tprev = route_start(sh_b2[w]);
+    if (mine && W.hub) tprev = split_start(sh_b2[w]);
     __syncthreads();
     if (!any) {
       st = 2;  // CFMM_ORDER_UNREACHABLE
@@ -264,7 +208,7 @@ __device__ __forceinline__ void route_row(const PathSets* P, const PairIndexView
         } else if (mine) {
           RouteSums last = {0.0, 0.0, 0.0}, at_hi = last;
           int64_t tlo = 0, thi = 0;
-          const int rc = route_search(
+          const int rc = split_search(
               tprev, tlo, thi,
               [&](int64_t ct) {
                 last = route_sums(P, W, sv, __longlong_as_double(ct), lane);
@@ -313,7 +257,7 @@ __device__ __forceinline__ void route_row(const PathSets* P, const PairIndexView
         }
       };
       int64_t lo = 0, hi = 0;
-      const int rc = route_search(route_start(e), lo, hi, test, keep);
+      const int rc = split_search(split_start(e), lo, hi, test, keep);
       if (rc != 0 || bad) {
         st = 2;
       } else {
@@ -333,50 +277,9 @@ __device__ __forceinline__ void route_row(const PathSets* P, const PairIndexView
     const int64_t base = row + 2 * R.hub_off[row];
     const int64_t l0 = (ARB && !R.leg_off) ? 0 : R.leg_off[w == 0 ? base : base + 2 * w - 1];
     for (int64_t t = lane; t < W.ca + W.cb; t += 32) {
-      Trade tr;
-      tr.d1 = tr.d2 = tr.l1 = tr.l2 = 0.0;
-      if (filled) {
-        bool inb;
-        const SplitPool sp = route_pool(P, W, t, s, tv, inb);
-        tr = split_legs(P, sp);
-        if (EXEC && sp.active) {
-          const SwapSet& S = P->s[sp.k];
-          if ((sp.k >> 1) < 2) {
-            const double2 n =
-                apply_trade(S.R[sp.p], S.gam[sp.p], make_double2(tr.d1, tr.d2), make_double2(tr.l1, tr.l2));
-            S.R[sp.p] = n;
-            if (!in_fast_range(n.x) || !in_fast_range(n.y)) P->out_of_range[sp.k] = 1;
-          } else {
-            const double q = univ3_price(S.u, sp.p);
-            const int off = S.u.tick[sp.p].x;
-            const double qn = univ3_moved_price(q, S.gam[sp.p], __ddiv_rn(sp.v1, sp.v2), S.u.lower[off]);
-            if (qn != q) {
-              reinterpret_cast<double*>(S.u.f1 + sp.p)[1] = qn;
-              reinterpret_cast<int*>(S.u.tick + sp.p)[1] =
-                  univ3_tick_of(S.u.lower + off, univ3_tick_end(S.u, sp.p) - off, qn);
-              uint8_t* f = mv.flag[sp.k & 1];
-              if (!f[sp.p]) {  // rows of one launch share no pool, so the check and the set do not race
-                f[sp.p] = 1;
-                P->moved[sp.k & 1][atomicAdd(P->n_moved + (sp.k & 1), 1ull)] = sp.p;
-              }
-            }
-          }
-          P->touched[sp.k] = 1;
-        }
-        if (sp.sw) {
-          const double d = tr.d1, l = tr.l1;
-          tr.d1 = tr.d2;
-          tr.l1 = tr.l2;
-          tr.d2 = d;
-          tr.l2 = l;
-        }
-      }
-      if (R.leg_delta) {
-        R.leg_delta[2 * (l0 + t)] = tr.d1;
-        R.leg_delta[2 * (l0 + t) + 1] = tr.d2;
-        R.leg_lambda[2 * (l0 + t)] = tr.l1;
-        R.leg_lambda[2 * (l0 + t) + 1] = tr.l2;
-      }
+      bool inb;
+      split_leg<EXEC>(
+          P, filled, [&] { return route_pool(P, W, t, s, tv, inb); }, mv, R.leg_delta, R.leg_lambda, l0 + t);
     }
     if (lane == 0 && W.hub) {
       const int64_t g = R.hub_off[row] + w - 1;

@@ -209,6 +209,62 @@ __device__ __forceinline__ SplitSums split_sums(const PathSets* P, const int64_t
 constexpr int64_t kSplitOrdMin = 0x0010000000000000ll;  // the ordinal of DBL_MIN
 constexpr int64_t kSplitOrdMax = kSwapOrdMax;           // DBL_MAX
 
+// The search of a row's s* (and of a hub's t_h, route_kernels.cuh) on the ordinals
+// [kSplitOrdMin, kSplitOrdMax], from o: gallop 1, 2, 4, … ordinals up or down, then bisect.
+// test(c) evaluates at c and returns enough(c) (true at small c); keep(is_lo) files that evaluation
+// as lo's or hi's.  0: a bracket, enough(lo), !enough(hi), hi = lo + 1.  1: enough at o(DBL_MAX)
+// (lo = o(DBL_MAX)).  2: !enough at o(DBL_MIN) (hi = o(DBL_MIN)).  At most 1 + 63 + 62 tests.
+template <class Test, class Keep>
+__device__ __forceinline__ int split_search(int64_t o, int64_t& lo, int64_t& hi, Test&& test, Keep&& keep) {
+  if (test(o)) {
+    lo = o;
+    keep(true);
+    for (int64_t step = 1;; step <<= 1) {
+      if (lo == kSplitOrdMax) return 1;
+      const int64_t c = kSplitOrdMax - lo <= step ? kSplitOrdMax : lo + step;
+      if (test(c)) {
+        lo = c;
+        keep(true);
+      } else {
+        hi = c;
+        keep(false);
+        break;
+      }
+    }
+  } else {
+    hi = o;
+    keep(false);
+    for (int64_t step = 1;; step <<= 1) {
+      if (hi == kSplitOrdMin) return 2;
+      const int64_t c = hi - kSplitOrdMin <= step ? kSplitOrdMin : hi - step;
+      if (test(c)) {
+        lo = c;
+        keep(true);
+        break;
+      }
+      hi = c;
+      keep(false);
+    }
+  }
+  while (hi - lo > 1) {
+    const int64_t mid = lo + ((hi - lo) >> 1);
+    if (test(mid)) {
+      lo = mid;
+      keep(true);
+    } else {
+      hi = mid;
+      keep(false);
+    }
+  }
+  return 0;
+}
+
+// The ordinal a search starts from: o(e) clamped to [o(DBL_MIN), o(DBL_MAX)], o(DBL_MIN) for a NaN.
+__device__ __forceinline__ int64_t split_start(double e) {
+  const int64_t o = !(e >= 0x1p-1022) ? kSplitOrdMin : __double_as_longlong(e);
+  return o > kSplitOrdMax ? kSplitOrdMax : o;
+}
+
 // The rows of one call (device arrays, row-indexed; tokens 1-based).
 struct SplitRows {
   const int64_t* token_in;
@@ -237,6 +293,58 @@ struct SplitMoved {
   uint8_t* flag[2];
 };
 
+// A row's last pass over one of its pools (split_row, route_row).  For a filled row, the pool
+// pool() builds at the row's ν: its legs; on EXEC, for an active pool, cfmm_apply_trades'
+// transition (two-coin: apply_trade and the out-of-range flag; UniV3: univ3_moved_price and the
+// new current tick written in place, the pool listed once per call).  The legs, (0, 0) when the
+// row did not fill or the pool is retired, go in ingest order to leg l when leg_delta is set.
+template <bool EXEC, class Pool>
+__device__ __forceinline__ void split_leg(const PathSets* P, bool filled, Pool&& pool, const SplitMoved& mv,
+                                          double* leg_delta, double* leg_lambda, int64_t l) {
+  Trade tr;
+  tr.d1 = tr.d2 = tr.l1 = tr.l2 = 0.0;
+  if (filled) {
+    const SplitPool sp = pool();
+    tr = split_legs(P, sp);
+    if (EXEC && sp.active) {
+      const SwapSet& S = P->s[sp.k];
+      if ((sp.k >> 1) < 2) {
+        const double2 n = apply_trade(S.R[sp.p], S.gam[sp.p], make_double2(tr.d1, tr.d2), make_double2(tr.l1, tr.l2));
+        S.R[sp.p] = n;
+        if (!in_fast_range(n.x) || !in_fast_range(n.y)) P->out_of_range[sp.k] = 1;
+      } else {
+        const double q = univ3_price(S.u, sp.p);
+        const double qn = univ3_moved_price(S.u, sp.p, q, S.gam[sp.p], __ddiv_rn(sp.v1, sp.v2));
+        if (qn != q) {
+          const int off = S.u.tick[sp.p].x;
+          reinterpret_cast<double*>(S.u.f1 + sp.p)[1] = qn;
+          reinterpret_cast<int*>(S.u.tick + sp.p)[1] =
+              univ3_tick_of(S.u.lower + off, univ3_tick_end(S.u, sp.p) - off, qn);
+          uint8_t* f = mv.flag[sp.k & 1];
+          if (!f[sp.p]) {  // rows of one launch share no pool, so the check and the set do not race
+            f[sp.p] = 1;
+            P->moved[sp.k & 1][atomicAdd(P->n_moved + (sp.k & 1), 1ull)] = sp.p;
+          }
+        }
+      }
+      P->touched[sp.k] = 1;
+    }
+    if (sp.sw) {
+      const double d = tr.d1, lm = tr.l1;
+      tr.d1 = tr.d2;
+      tr.l1 = tr.l2;
+      tr.d2 = d;
+      tr.l2 = lm;
+    }
+  }
+  if (leg_delta) {
+    leg_delta[2 * l] = tr.d1;
+    leg_delta[2 * l + 1] = tr.d2;
+    leg_lambda[2 * l] = tr.l1;
+    leg_lambda[2 * l + 1] = tr.l2;
+  }
+}
+
 // Row `row` on the current state of its pair's pools, warp-wide (every lane takes every branch).
 // EXEC: the limit decides, and a filled row applies cfmm_apply_trades' transition at its ν to each
 // of the pair's pools.
@@ -246,12 +354,11 @@ __device__ __forceinline__ void split_row(const PathSets* P, const PairIndexView
   const int64_t pr = R.pair[row];
   const int64_t* pools = pr >= 0 ? ix.pool + ix.off[pr] : nullptr;
   const int64_t cnt = pr >= 0 ? ix.off[pr + 1] - ix.off[pr] : 0;
-  const int64_t tj = R.token_in[row] - 1, ti = R.token_out[row] - 1;
+  const int64_t tj = R.token_in[row] - 1;
   const bool out = R.kind[row] == 1;
   const double amt = R.amount[row];
   const double inf = __longlong_as_double(0x7ff0000000000000ll);
   const double lim = R.limit ? R.limit[row] : (out ? inf : 0.0);
-  (void)ti;
   uint8_t st = 0;  // CFMM_ORDER_FILLED
   double s = 0.0;
   SplitSums at = {0.0, 0.0};
@@ -273,64 +380,18 @@ __device__ __forceinline__ void split_row(const PathSets* P, const PairIndexView
     if (!__any_sync(kFull, any)) {
       st = 2;  // CFMM_ORDER_UNREACHABLE
     } else {
-      const auto enough = [&](int64_t o, SplitSums& r) {
-        r = split_sums(P, pools, cnt, tj, __longlong_as_double(o), lane);
-        return out ? r.o >= amt : !(r.n <= amt);  // exact-in: N > δ, a NaN counts as true
-      };
-      int64_t o = !(e >= 0x1p-1022) ? kSplitOrdMin : __double_as_longlong(e);
-      o = o > kSplitOrdMax ? kSplitOrdMax : o;
+      SplitSums r, slo = at, shi = at;
       int64_t lo = 0, hi = 0;
-      SplitSums slo = at, shi = at, r;
-      bool ok = true;
-      if (enough(o, r)) {  // gallop up: lo stays enough
-        lo = o;
-        slo = r;
-        for (int64_t step = 1;; step <<= 1) {
-          if (lo == kSplitOrdMax) {
-            ok = false;
-            break;
-          }
-          const int64_t c = kSplitOrdMax - lo <= step ? kSplitOrdMax : lo + step;
-          if (enough(c, r)) {
-            lo = c;
-            slo = r;
-          } else {
-            hi = c;
-            shi = r;
-            break;
-          }
-        }
-      } else {  // gallop down: hi stays !enough
-        hi = o;
-        shi = r;
-        for (int64_t step = 1;; step <<= 1) {
-          if (hi == kSplitOrdMin) {
-            ok = false;
-            break;
-          }
-          const int64_t c = hi - kSplitOrdMin <= step ? kSplitOrdMin : hi - step;
-          if (enough(c, r)) {
-            lo = c;
-            slo = r;
-            break;
-          }
-          hi = c;
-          shi = r;
-        }
-      }
-      if (!ok) {
+      const int rc = split_search(
+          split_start(e), lo, hi,
+          [&](int64_t c) {
+            r = split_sums(P, pools, cnt, tj, __longlong_as_double(c), lane);
+            return out ? r.o >= amt : !(r.n <= amt);  // exact-in: N > δ, a NaN counts as true
+          },
+          [&](bool is_lo) { (is_lo ? slo : shi) = r; });
+      if (rc != 0) {
         st = 2;
       } else {
-        while (hi - lo > 1) {
-          const int64_t mid = lo + ((hi - lo) >> 1);
-          if (enough(mid, r)) {
-            lo = mid;
-            slo = r;
-          } else {
-            hi = mid;
-            shi = r;
-          }
-        }
         s = __longlong_as_double(out ? lo : hi);
         at = out ? slo : shi;
         if (EXEC && (out ? at.n > lim : at.o < lim)) st = 1;  // CFMM_ORDER_LIMIT; an equal limit fills
@@ -340,49 +401,8 @@ __device__ __forceinline__ void split_row(const PathSets* P, const PairIndexView
   const bool filled = st == 0 && amt > 0.0;
   // legs (ingest order) and, on execute, the transition of each pool
   const int64_t l0 = R.leg_off[row];
-  for (int64_t t = lane; t < cnt; t += 32) {
-    Trade tr;
-    tr.d1 = tr.d2 = tr.l1 = tr.l2 = 0.0;
-    if (filled) {
-      const SplitPool sp = split_pool(P, pools[t], tj, s);
-      tr = split_legs(P, sp);
-      if (EXEC && sp.active) {
-        const SwapSet& S = P->s[sp.k];
-        if ((sp.k >> 1) < 2) {
-          const double2 n = apply_trade(S.R[sp.p], S.gam[sp.p], make_double2(tr.d1, tr.d2), make_double2(tr.l1, tr.l2));
-          S.R[sp.p] = n;
-          if (!in_fast_range(n.x) || !in_fast_range(n.y)) P->out_of_range[sp.k] = 1;
-        } else {
-          const double q = univ3_price(S.u, sp.p);
-          const int off = S.u.tick[sp.p].x;
-          const double qn = univ3_moved_price(q, S.gam[sp.p], __ddiv_rn(sp.v1, sp.v2), S.u.lower[off]);
-          if (qn != q) {
-            reinterpret_cast<double*>(S.u.f1 + sp.p)[1] = qn;
-            reinterpret_cast<int*>(S.u.tick + sp.p)[1] = univ3_tick_of(S.u.lower + off, univ3_tick_end(S.u, sp.p) - off, qn);
-            uint8_t* f = mv.flag[sp.k & 1];
-            if (!f[sp.p]) {
-              f[sp.p] = 1;
-              P->moved[sp.k & 1][atomicAdd(P->n_moved + (sp.k & 1), 1ull)] = sp.p;
-            }
-          }
-        }
-        P->touched[sp.k] = 1;
-      }
-      if (sp.sw) {
-        const double d = tr.d1, l = tr.l1;
-        tr.d1 = tr.d2;
-        tr.l1 = tr.l2;
-        tr.d2 = d;
-        tr.l2 = l;
-      }
-    }
-    if (R.leg_delta) {
-      R.leg_delta[2 * (l0 + t)] = tr.d1;
-      R.leg_delta[2 * (l0 + t) + 1] = tr.d2;
-      R.leg_lambda[2 * (l0 + t)] = tr.l1;
-      R.leg_lambda[2 * (l0 + t) + 1] = tr.l2;
-    }
-  }
+  for (int64_t t = lane; t < cnt; t += 32)
+    split_leg<EXEC>(P, filled, [&] { return split_pool(P, pools[t], tj, s); }, mv, R.leg_delta, R.leg_lambda, l0 + t);
   __syncwarp();  // the next row of this warp reads the state the lanes just wrote
   if (lane == 0) {
     R.paid[row] = filled ? at.n : 0.0;

@@ -112,115 +112,10 @@ __device__ __forceinline__ Univ3Walk univ3_walk(const double* lower, const doubl
   return r;
 }
 
-// Quotes: one thread per row.  rows[j] is the row's index in the call (tender / received
-// [2·row, 2·row+1], ingest order), pos[j] its pool's device position in this set.
-template <int TYPE>
-__global__ void swap_quote_kernel(SwapSet s, const int64_t* __restrict__ rows, const int64_t* __restrict__ pos,
-                                  int64_t n, const double* __restrict__ tender, double* __restrict__ received) {
-  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n) return;
-  const int64_t row = rows[j], p = pos[j];
-  double2 out = make_double2(0.0, 0.0);
-  if (!s.active || s.active[p]) {
-    const double x1 = tender[2 * row], x2 = tender[2 * row + 1];
-    if constexpr (TYPE == 2) {
-      if (x1 > 0.0 || x2 > 0.0) {
-        const int off = s.u.tick[p].x, nt = univ3_tick_end(s.u, p) - off;
-        const bool tok1 = x1 > 0.0;
-        const Univ3Walk wk = univ3_walk(s.u.lower + off, s.u.liq + off, nt, univ3_price(s.u, p), s.u.tick[p].y,
-                                        __dmul_rn(s.gam[p], tok1 ? x1 : x2), tok1);
-        out = tok1 ? make_double2(0.0, wk.lambda) : make_double2(wk.lambda, 0.0);
-      }
-    } else {
-      const bool sw = (s.gidx[p] >> 62) & 1;
-      const double2 w = TYPE == 1 ? s.w[p] : make_double2(0.0, 0.0);
-      const double2 l = two_coin_quote<TYPE>(s.R[p], s.gam[p], w, sw ? x2 : x1, sw ? x1 : x2);
-      out = sw ? make_double2(l.y, l.x) : l;
-    }
-  }
-  received[2 * row] = out.x;
-  received[2 * row + 1] = out.y;
-}
-
-// Execution: one thread per distinct pool.  seg_pos[k] is the k-th pool's device position, its
-// rows are seg_rows[seg_off[k] .. seg_off[k+1]) in batch order.  The thread reads the pool's
-// state once, applies the rows in order (each sees the ones before it), writes every row's
-// received and the final state once.  Two-coin: *out_of_range is raised when a new reserve
-// leaves the guard-free range.  UniV3: the new price goes to the price word of f1, and pools
-// whose price changed are listed in moved (their derived state is rebuilt afterwards by
-// univ3_current_tick_kernel / univ3_ticks_kernel, as after cfmm_apply_trades).
-template <int TYPE>
-__global__ void swap_execute_kernel(SwapSet s, const int64_t* __restrict__ seg_pos,
-                                    const int64_t* __restrict__ seg_off, const int64_t* __restrict__ seg_rows,
-                                    int64_t n_seg, const double* __restrict__ tender,
-                                    double* __restrict__ received, int64_t* __restrict__ moved,
-                                    unsigned long long* __restrict__ n_moved, int* __restrict__ out_of_range) {
-  const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= n_seg) return;
-  const int64_t p = seg_pos[k], r0 = seg_off[k], r1 = seg_off[k + 1];
-  if (s.active && !s.active[p]) {  // retired: receives nothing, its parked state stays
-    for (int64_t r = r0; r < r1; ++r) {
-      const int64_t row = seg_rows[r];
-      received[2 * row] = 0.0;
-      received[2 * row + 1] = 0.0;
-    }
-    return;
-  }
-  const double g = s.gam[p];
-  if constexpr (TYPE == 2) {
-    const int off = s.u.tick[p].x, nt = univ3_tick_end(s.u, p) - off;
-    const double* lower = s.u.lower + off;
-    const double q0 = univ3_price(s.u, p);
-    double q = q0;
-    int cur = s.u.tick[p].y;
-    for (int64_t r = r0; r < r1; ++r) {
-      const int64_t row = seg_rows[r];
-      const double x1 = tender[2 * row], x2 = tender[2 * row + 1];
-      double2 out = make_double2(0.0, 0.0);
-      if (x1 > 0.0 || x2 > 0.0) {
-        const bool tok1 = x1 > 0.0;
-        const Univ3Walk wk = univ3_walk(lower, s.u.liq + off, nt, q, cur, __dmul_rn(g, tok1 ? x1 : x2), tok1);
-        out = tok1 ? make_double2(0.0, wk.lambda) : make_double2(wk.lambda, 0.0);
-        if (wk.moved) {
-          q = wk.price;
-          cur = univ3_tick_of(lower, nt, q);
-        }
-      }
-      received[2 * row] = out.x;
-      received[2 * row + 1] = out.y;
-    }
-    if (q != q0) {
-      reinterpret_cast<double*>(s.u.f1 + p)[1] = q;
-      moved[atomicAdd(n_moved, 1ull)] = p;
-    }
-  } else {
-    const bool sw = (s.gidx[p] >> 62) & 1;
-    const double2 w = TYPE == 1 ? s.w[p] : make_double2(0.0, 0.0);
-    double2 R = s.R[p];
-    for (int64_t r = r0; r < r1; ++r) {
-      const int64_t row = seg_rows[r];
-      const double x1 = tender[2 * row], x2 = tender[2 * row + 1];
-      double2 out = make_double2(0.0, 0.0);
-      if (x1 > 0.0 || x2 > 0.0) {
-        const double d1 = sw ? x2 : x1, d2 = sw ? x1 : x2;
-        const double2 l = two_coin_quote<TYPE>(R, g, w, d1, d2);
-        R.x = __dsub_rn(__dadd_rn(R.x, __dmul_rn(g, d1)), l.x);  // (R + γΔ) − Λ, as apply_trades_kernel
-        R.y = __dsub_rn(__dadd_rn(R.y, __dmul_rn(g, d2)), l.y);
-        out = sw ? make_double2(l.y, l.x) : l;
-      }
-      received[2 * row] = out.x;
-      received[2 * row + 1] = out.y;
-    }
-    s.R[p] = R;
-    if (!in_fast_range(R.x) || !in_fast_range(R.y)) atomicOr(out_of_range, 1);
-  }
-}
-
 // ---- exact-output rows and slippage limits (cfmm_quote_swaps_exact_out / cfmm_execute_swap_orders)
-// f(x) is the exact-input quote of a tender x on one side at the pool's current state: two_coin_out
-// with δ = γ·x, or univ3_walk(..., γ·x, ...).lambda, the operations swap_quote_kernel runs, so f is
-// cfmm_quote_swaps bit for bit (f(0) = 0, as for a zero tender).  The old kernels are unchanged: the
-// helpers they call are the ones the new kernels call.
+// f(x) is the exact-input quote of a tender x > 0 on one side at the pool's current state:
+// two_coin_out with δ = γ·x, or univ3_walk(..., γ·x, ...).lambda.  swap_quote_kernel is f on a
+// row's tendered side, so f is cfmm_quote_swaps bit for bit (a zero tender receives (0, 0)).
 //
 // An exact-output row wanting y > 0 takes x* with f(x*) >= y and f(pred(x*)) < y (or x* = 0),
 // searched on the ordinals of the doubles in [0, DBL_MAX] (a double >= 0 read as an int64 is
@@ -320,8 +215,8 @@ __device__ __forceinline__ double univ3_estimate(const double* lower, const doub
   return __longlong_as_double(0x7ff0000000000000ll);
 }
 
-// One pool at its current state, for the exact-output search and the order rows: a tender of the
-// ingest token tok1 (token 1) or token 2.  f, estimate and the transition of one filled row.
+// One pool at its current state, for every swap kernel: a tender of the ingest token tok1
+// (token 1) or token 2.  f, estimate and the transition of one filled row.
 template <int TYPE>
 struct SwapPool {
   // two-coin
@@ -359,7 +254,8 @@ struct SwapPool {
     return o < 0 ? __longlong_as_double(0x7ff0000000000000ll) : __longlong_as_double(o);
   }
 
-  // Execute a tender x > 0 as swap_execute_kernel does; returns what it received.
+  // Execute a tender x > 0: two-coin reserves move to (R + γΔ) − Λ (apply_trade), a UniV3 pool to
+  // the price its walk ended at and that price's current tick.  Returns what it received.
   __device__ __forceinline__ double execute(double x, bool tok1) {
     if constexpr (TYPE == 2) {
       const Univ3Walk wk = univ3_walk(lower, liq, nt, q, cur, __dmul_rn(g, x), tok1);
@@ -371,8 +267,7 @@ struct SwapPool {
     } else {
       const double d1 = tok1 != sw ? x : 0.0, d2 = tok1 != sw ? 0.0 : x;
       const double2 l = two_coin_quote<TYPE>(R, g, w, d1, d2);
-      R.x = __dsub_rn(__dadd_rn(R.x, __dmul_rn(g, d1)), l.x);  // (R + γΔ) − Λ, as apply_trades_kernel
-      R.y = __dsub_rn(__dadd_rn(R.y, __dmul_rn(g, d2)), l.y);
+      R = apply_trade(R, g, make_double2(d1, d2), l);
       return tok1 != sw ? l.y : l.x;
     }
   }
@@ -395,6 +290,78 @@ __device__ __forceinline__ SwapPool<TYPE> swap_pool(const SwapSet& s, int64_t p)
     P.sw = (s.gidx[p] >> 62) & 1;
   }
   return P;
+}
+
+// ---- kernels, all over SwapPool
+// Quotes (cfmm_quote_swaps): one thread per row.  rows[j] is the row's index in the call (tender / received
+// [2·row, 2·row+1], ingest order), pos[j] its pool's device position in this set.  A retired pool
+// or a zero tender receives (0, 0) and reads nothing of the pool.
+template <int TYPE>
+__global__ void swap_quote_kernel(SwapSet s, const int64_t* __restrict__ rows, const int64_t* __restrict__ pos,
+                                  int64_t n, const double* __restrict__ tender, double* __restrict__ received) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const int64_t row = rows[j], p = pos[j];
+  double2 out = make_double2(0.0, 0.0);
+  if (!s.active || s.active[p]) {
+    const double x1 = tender[2 * row], x2 = tender[2 * row + 1];
+    if (x1 > 0.0 || x2 > 0.0) {
+      const bool tok1 = x1 > 0.0;
+      const double l = swap_pool<TYPE>(s, p).f(tok1 ? x1 : x2, tok1);
+      out = tok1 ? make_double2(0.0, l) : make_double2(l, 0.0);
+    }
+  }
+  received[2 * row] = out.x;
+  received[2 * row + 1] = out.y;
+}
+
+// Execution (cfmm_execute_swaps): one thread per distinct pool.  seg_pos[k] is the k-th pool's device position, its
+// rows are seg_rows[seg_off[k] .. seg_off[k+1]) in batch order.  The thread reads the pool's
+// state once, applies the rows in order (each sees the ones before it), writes every row's
+// received and the final state once.  Two-coin: *out_of_range is raised when a new reserve
+// leaves the guard-free range.  UniV3: the new price goes to the price word of f1, and pools
+// whose price changed are listed in moved (their derived state is rebuilt afterwards by
+// univ3_current_tick_kernel / univ3_ticks_kernel, as after cfmm_apply_trades).
+template <int TYPE>
+__global__ void swap_execute_kernel(SwapSet s, const int64_t* __restrict__ seg_pos,
+                                    const int64_t* __restrict__ seg_off, const int64_t* __restrict__ seg_rows,
+                                    int64_t n_seg, const double* __restrict__ tender,
+                                    double* __restrict__ received, int64_t* __restrict__ moved,
+                                    unsigned long long* __restrict__ n_moved, int* __restrict__ out_of_range) {
+  const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n_seg) return;
+  const int64_t p = seg_pos[k], r0 = seg_off[k], r1 = seg_off[k + 1];
+  if (s.active && !s.active[p]) {  // retired: receives nothing, its parked state stays
+    for (int64_t r = r0; r < r1; ++r) {
+      const int64_t row = seg_rows[r];
+      received[2 * row] = 0.0;
+      received[2 * row + 1] = 0.0;
+    }
+    return;
+  }
+  SwapPool<TYPE> P = swap_pool<TYPE>(s, p);
+  const double q0 = TYPE == 2 ? P.q : 0.0;
+  for (int64_t r = r0; r < r1; ++r) {
+    const int64_t row = seg_rows[r];
+    const double x1 = tender[2 * row], x2 = tender[2 * row + 1];
+    double2 out = make_double2(0.0, 0.0);
+    if (x1 > 0.0 || x2 > 0.0) {
+      const bool tok1 = x1 > 0.0;
+      const double l = P.execute(tok1 ? x1 : x2, tok1);
+      out = tok1 ? make_double2(0.0, l) : make_double2(l, 0.0);
+    }
+    received[2 * row] = out.x;
+    received[2 * row + 1] = out.y;
+  }
+  if constexpr (TYPE == 2) {
+    if (P.q != q0) {
+      reinterpret_cast<double*>(s.u.f1 + p)[1] = P.q;
+      moved[atomicAdd(n_moved, 1ull)] = p;
+    }
+  } else {
+    s.R[p] = P.R;
+    if (!in_fast_range(P.R.x) || !in_fast_range(P.R.y)) atomicOr(out_of_range, 1);
+  }
 }
 
 // Exact-output quotes: one thread per row, addressed as in swap_quote_kernel.  want (0, y) tenders

@@ -290,14 +290,6 @@ __global__ void scatter_trades_kernel(const double2* __restrict__ D,
   outL[o] = swapped ? make_double2(l.y, l.x) : l;
 }
 
-// R <- (R + γ·Δ) − Λ (the update the reference's tests use, test/cfmms.jl:10: R⁺ = R + γ*Δ - Λ)
-__device__ __forceinline__ double2 apply_trade(double2 r, double g, double2 d, double2 l) {
-  double2 n;
-  n.x = __dsub_rn(__dadd_rn(r.x, __dmul_rn(g, d.x)), l.x);
-  n.y = __dsub_rn(__dadd_rn(r.y, __dmul_rn(g, d.y)), l.y);
-  return n;
-}
-
 // apply_trade from the materialised trades of the same device order; *out_of_range is raised when
 // a new reserve leaves the guard-free range.  active (device order, 0 = retired; null = all active)
 // skips retired pools.

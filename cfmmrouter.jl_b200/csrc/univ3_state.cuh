@@ -191,39 +191,33 @@ __global__ void univ3_ticks_kernel(Univ3State s, const int64_t* __restrict__ pos
   }
 }
 
-// The post-trade price of every pool (include/cfmm_b200.h, cfmm_apply_trades), from the ν of the
-// last materialising sweep: p = ν[a]/ν[b] and the no-trade band exactly as univ3_arb computes
-// them; the target p/γ (upper walk) or γ·p (lower walk), unchanged if it is NaN or not > 0, else
-// clamped to the first lower tick.  Pools whose price changes get it stored in f1 and are listed.
-// univ3_moved_price below is the same rule for one pool.
+// The post-trade price of pool p of s (include/cfmm_b200.h, cfmm_apply_trades) at price q, fee g,
+// for pr = ν[a]/ν[b]: the no-trade band exactly as univ3_arb computes it; the target p/γ (upper
+// walk) or γ·p (lower walk), unchanged if it is NaN or not > 0, else clamped to the first lower
+// tick.  Returns q when the price stays.  The first lower tick is only read for a target > 0.
+__device__ __forceinline__ double univ3_moved_price(const Univ3State& s, int64_t p, double q, double g, double pr) {
+  const double lo = __dmul_rn(g, q);
+  if (lo <= pr && pr <= __ddiv_rn(q, g)) return q;
+  const double target = pr < lo ? __ddiv_rn(pr, g) : __dmul_rn(g, pr);
+  if (!(target > 0.0)) return q;
+  const double t1 = s.lower[s.tick[p].x];
+  return target < t1 ? target : t1;
+}
+
+// The post-trade price of every pool, from the ν of the last materialising sweep.  Pools whose
+// price changes get it stored in f1 and are listed.
 __global__ void univ3_move_kernel(Univ3State s, const double* __restrict__ gam, const int2* __restrict__ Ai,
                                   const double* __restrict__ nu, int64_t* __restrict__ moved,
                                   unsigned long long* __restrict__ n_moved) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= s.m) return;
   if (s.active && !s.active[p]) return;  // retired pools do not trade and do not move
-  const double q = univ3_price(s, p), g = gam[p];
+  const double q = univ3_price(s, p);
   const int2 ai = Ai[p];
-  const double pr = __ddiv_rn(nu[ai.x], nu[ai.y]);
-  const double lo = __dmul_rn(g, q);
-  if (lo <= pr && pr <= __ddiv_rn(q, g)) return;
-  const double target = pr < lo ? __ddiv_rn(pr, g) : __dmul_rn(g, pr);
-  if (!(target > 0.0)) return;
-  const double t1 = s.lower[s.tick[p].x];
-  const double qn = target < t1 ? target : t1;
+  const double qn = univ3_moved_price(s, p, q, gam[p], __ddiv_rn(nu[ai.x], nu[ai.y]));
   if (qn == q) return;
   reinterpret_cast<double*>(s.f1 + p)[1] = qn;
   moved[atomicAdd(n_moved, 1ull)] = p;
-}
-
-// univ3_move_kernel's rule for one pool at price q, fee g, for p = ν[a]/ν[b], whose first lower
-// tick is t1: the new price (q when it stays).
-__device__ __forceinline__ double univ3_moved_price(double q, double g, double pr, double t1) {
-  const double lo = __dmul_rn(g, q);
-  if (lo <= pr && pr <= __ddiv_rn(q, g)) return q;
-  const double target = pr < lo ? __ddiv_rn(pr, g) : __dmul_rn(g, pr);
-  if (!(target > 0.0)) return q;
-  return target < t1 ? target : t1;
 }
 
 // ---- liquidity changes (cfmm_modify_univ3_liquidity; include/cfmm_b200.h) ---------------------
