@@ -34,6 +34,9 @@ ORDER_RETIRED = 3
 # cfmm_quote_paths / cfmm_execute_paths
 PATH_MAX_HOPS = 8
 ROUTE_MAX_HUBS = 7  # CFMM_ROUTE_MAX_HUBS
+# cfmm_find_order_paths
+BEST_PATH_MAX_TOKENS = 1024
+PATH_REPEATS_POOL = 4
 
 COMM_HANDLE_BYTES = 128
 
@@ -105,6 +108,9 @@ SYMBOLS = {
                                       _dp]),
     "cfmm_choose_order_hubs": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, C.c_int,
                                          C.POINTER(C.c_uint8), _ip, _ip, _dp, _ip]),
+    "cfmm_find_order_paths": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, C.c_int,
+                                        C.POINTER(C.c_uint8), _ip, C.POINTER(C.c_int), _ip, _ip, _dp, _dp, _dp,
+                                        C.POINTER(C.c_uint8)]),
     "cfmm_modify_univ3_liquidity":(C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),

@@ -1,0 +1,344 @@
+// best_path_kernels.cuh -- the path search of cfmm_find_order_paths (sm_90a, include/cfmm_b200.h).
+// Off the sweep path: no sweep kernel reads anything these kernels add.
+//
+// The intermediate tokens B of a call are dense slots 0 .. nB−1 in token order.  best_path_graph_kernel
+// builds, once per call, each slot's neighbours in B from the token adjacency (arb_scan_kernels.cuh).
+// best_path_kernel runs one order row per CTA: an exact dynamic programme over "at most h hops" on
+// the tokens of B, two levels of amounts and every level's predecessors in shared memory.  Every
+// candidate is one quote, path_hop_f / path_hop_exact_out: cfmm_quote_swaps /
+// cfmm_quote_swaps_exact_out bit for bit.  The rebuilt walk is priced by path_run, the code of
+// cfmm_quote_paths, so its amounts are that call's on the same CSR.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "hub_kernels.cuh"
+
+namespace cfmm {
+
+constexpr int kBestPathMaxTokens = 1024;  // CFMM_BEST_PATH_MAX_TOKENS
+constexpr int kBestPathThreads = 256;
+constexpr int kBestPathMaxHops = 8;       // CFMM_PATH_MAX_HOPS
+
+// The B-subgraph of a call.  Slot s is token tok[s] (0-based, ascending); slot_of[t] is t's slot or
+// −1.  Slot s's neighbours in B are nbr[nB·s + m], m < deg[s], ascending, with pair ids pair[nB·s + m].
+struct BestPathGraph {
+  const int32_t* tok;
+  const int32_t* slot_of;
+  const int32_t* deg;
+  const int16_t* nbr;
+  const int32_t* pair;
+  int nB;
+};
+
+// One warp per slot: its adjacency list filtered to B, compacted in list order with a ballot.
+__global__ void best_path_graph_kernel(AdjView A, const int32_t* __restrict__ tok,
+                                       const int32_t* __restrict__ slot_of, int nB, int32_t* __restrict__ deg,
+                                       int16_t* __restrict__ nbr, int32_t* __restrict__ pair) {
+  const int s = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  const int lane = threadIdx.x & 31;
+  if (s >= nB) return;
+  const int64_t e0 = A.off[tok[s]], e1 = A.off[tok[s] + 1];
+  int n = 0;
+  for (int64_t b = e0; b < e1; b += 32) {
+    const int64_t e = b + lane;
+    const int32_t u = e < e1 ? slot_of[A.nbr[e]] : -1;
+    const unsigned in = __ballot_sync(kFull, u >= 0);
+    if (u >= 0) {
+      const int at = n + __popc(in & ((1u << lane) - 1u));
+      nbr[(int64_t)nB * s + at] = (int16_t)u;
+      pair[(int64_t)nB * s + at] = A.pair[e];
+    }
+    n += __popc(in);
+  }
+  if (lane == 0) deg[s] = n;
+}
+
+// A candidate's rank key: score (the amount, negated for exact-out), then fewer hops, then the
+// smaller predecessor token, then the earlier position in the pair's pool list.  from is how the
+// walk is rebuilt (an edge index, or a slot at the final hop), not part of the order.
+struct BpKey {
+  double s;
+  int32_t hops, tok, pos, from;
+};
+
+__device__ __forceinline__ bool bp_before(const BpKey& a, const BpKey& b) {
+  if (a.s != b.s) return a.s > b.s;
+  if (a.hops != b.hops) return a.hops < b.hops;
+  if (a.tok != b.tok) return a.tok < b.tok;
+  return a.pos < b.pos;
+}
+
+__device__ __forceinline__ BpKey bp_none() { return BpKey{-kPathInf, 0, INT32_MAX, INT32_MAX, -1}; }
+
+__device__ __forceinline__ BpKey bp_warp_best(BpKey k) {
+#pragma unroll
+  for (int m = 16; m >= 1; m >>= 1) {
+    BpKey o;
+    o.s = __shfl_xor_sync(kFull, k.s, m);
+    o.hops = __shfl_xor_sync(kFull, k.hops, m);
+    o.tok = __shfl_xor_sync(kFull, k.tok, m);
+    o.pos = __shfl_xor_sync(kFull, k.pos, m);
+    o.from = __shfl_xor_sync(kFull, k.from, m);
+    if (bp_before(o, k)) k = o;
+  }
+  return k;
+}
+
+// The candidates of one hop over the active pools of pair k: from an amount a of the DP's
+// predecessor token (exact-in: a tendered, the hop pays out; exact-out: a wanted, the hop's tender
+// is the candidate).  tender is the token the hop tenders.  key gets the best, ranked as above.
+__device__ __forceinline__ void bp_hop(const PathSets* P, PairIndexView ix, int32_t k, int64_t tender, double a,
+                                       bool out, int32_t hops, int32_t tok, int32_t from, BpKey& key) {
+  const int64_t e0 = ix.off[k], e1 = ix.off[k + 1];
+  for (int64_t e = e0; e < e1; ++e) {
+    const HubHop h = hub_hop(P, ix.pool[e], tender);
+    if (!h.active) continue;
+    double s;
+    if (!out) {
+      const double v = path_hop_f(P, h.k, h.p, a, h.tok1);
+      if (!(v > 0.0)) continue;  // NaN or nothing out
+      s = v;
+    } else {
+      const double x = path_hop_exact_out(P, h.k, h.p, a, h.tok1);
+      if (!(x < kPathInf)) continue;  // NaN or unreachable
+      s = -x;
+    }
+    const BpKey c{s, hops, tok, (int32_t)(e - e0), from};
+    if (bp_before(c, key)) key = c;
+  }
+}
+
+// The shared-memory layout of one row: two levels of amounts and hop counts, the start- and
+// end-side pairs of every slot, and per level 1 .. H−1 each slot's predecessor (an edge index of
+// the slot, kBpFromSource, or kBpCarry: the level before's value kept) and pool position.
+constexpr int16_t kBpCarry = -1, kBpFromSource = -2;
+
+__host__ __device__ inline size_t best_path_smem(int nB, int H) {
+  const size_t n = (size_t)nB;
+  return 2 * n * sizeof(double) + 2 * n * sizeof(int32_t) + (size_t)(H - 1) * n * (sizeof(int32_t) + sizeof(int16_t)) +
+         2 * n + 32 * sizeof(BpKey) + 16;
+}
+
+// Row r (include/cfmm_b200.h, cfmm_find_order_paths).  The DP runs from the source S (exact-in: j
+// forward; exact-out: i backward) to the sink T.  Outputs: nhop[r], and at H·r .. the hops' set,
+// device position, tendered side, delivered token (1-based), tender and received; value[r], status[r].
+__global__ void __launch_bounds__(kBestPathThreads)
+    best_path_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, BestPathGraph G,
+                     const int64_t* __restrict__ token_in, const int64_t* __restrict__ token_out,
+                     const uint8_t* __restrict__ kind, const double* __restrict__ amount, int H,
+                     int32_t* __restrict__ nhop, uint8_t* __restrict__ hop_set, int64_t* __restrict__ hop_pos,
+                     uint8_t* __restrict__ hop_tok1, int64_t* __restrict__ hop_token, double* __restrict__ tender,
+                     double* __restrict__ received, double* __restrict__ value, uint8_t* __restrict__ status) {
+  extern __shared__ __align__(16) unsigned char bp_smem[];
+  const int64_t r = blockIdx.x;
+  const int nB = G.nB, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarp = blockDim.x >> 5;
+  const int32_t j = (int32_t)(token_in[r] - 1), i = (int32_t)(token_out[r] - 1);
+  const bool out = kind[r] != 0;
+  const double amt = amount[r];
+  const int32_t S = out ? i : j, T = out ? j : i;
+  const double none = out ? kPathInf : 0.0;
+  double* val = reinterpret_cast<double*>(bp_smem);                  // [2][nB]
+  int32_t* spair = reinterpret_cast<int32_t*>(val + 2 * nB);        // [nB] pair {S, b}
+  int32_t* epair = spair + nB;                                       // [nB] pair {b, T}
+  int32_t* ppos = epair + nB;                                        // [H−1][nB]
+  int16_t* pred = reinterpret_cast<int16_t*>(ppos + (size_t)(H - 1) * nB);  // [H−1][nB]
+  uint8_t* hops = reinterpret_cast<uint8_t*>(pred + (size_t)(H - 1) * nB);  // [2][nB]
+  BpKey* red = reinterpret_cast<BpKey*>(
+      (reinterpret_cast<uintptr_t>(hops + 2 * nB) + 15) & ~(uintptr_t)15);  // [nwarp]
+  __shared__ int32_t direct;  // pair {S, T}, −1 when no pool holds it
+  if (!(amt > 0.0)) {  // nothing to route: filled, no hops (uniform across the CTA)
+    if (tid == 0) {
+      nhop[r] = 0;
+      value[r] = 0.0;
+      status[r] = 0;  // CFMM_ORDER_FILLED
+    }
+    return;
+  }
+  for (int s = tid; s < nB; s += blockDim.x) {
+    val[s] = val[nB + s] = none;
+    hops[s] = hops[nB + s] = 0;
+    spair[s] = epair[s] = -1;
+  }
+  if (tid == 0) direct = -1;
+  __syncthreads();
+  // the pairs {S, b} and {b, T}: walk the token's list when it is short, else bisect it per slot
+  for (int side = 0; side < 2; ++side) {
+    const int32_t t = side ? T : S;
+    int32_t* dst = side ? epair : spair;
+    const int64_t a0 = A.off[t], a1 = A.off[t + 1];
+    if (a1 - a0 <= (int64_t)nB) {
+      for (int64_t e = a0 + tid; e < a1; e += blockDim.x) {
+        const int32_t u = G.slot_of[A.nbr[e]];
+        if (u >= 0) dst[u] = A.pair[e];
+      }
+    } else {
+      for (int s = tid; s < nB; s += blockDim.x) {
+        const int32_t b = G.tok[s];
+        int64_t lo = a0, hi = a1;
+        while (lo < hi) {
+          const int64_t mid = (lo + hi) >> 1;
+          if (A.nbr[mid] < b)
+            lo = mid + 1;
+          else
+            hi = mid;
+        }
+        if (lo < a1 && A.nbr[lo] == b) dst[s] = A.pair[lo];
+      }
+    }
+  }
+  if (tid == 0) {
+    int64_t lo = A.off[S], hi = A.off[S + 1];
+    const int64_t a1 = hi;
+    while (lo < hi) {
+      const int64_t mid = (lo + hi) >> 1;
+      if (A.nbr[mid] < T)
+        lo = mid + 1;
+      else
+        hi = mid;
+    }
+    if (lo < a1 && A.nbr[lo] == T) direct = A.pair[lo];
+  }
+  __syncthreads();
+  // level 1: one thread per slot, the pools of {S, b}, from the row's amount
+  int top = 0;  // the last level computed; the levels above it only carry
+  bool more = false;
+  if (H > 1) {
+    int changed = 0;
+    for (int s = tid; s < nB; s += blockDim.x) {
+      const int32_t b = G.tok[s];
+      BpKey key = bp_none();
+      if (b != j && b != i && spair[s] >= 0) bp_hop(P, ix, spair[s], out ? b : S, amt, out, 1, S, kBpFromSource, key);
+      const bool got = key.from != -1;
+      if (got) {
+        val[nB + s] = out ? -key.s : key.s;
+        hops[nB + s] = 1;
+      }
+      pred[s] = got ? kBpFromSource : kBpCarry;
+      ppos[s] = got ? key.pos : 0;
+      changed |= got;
+    }
+    top = 1;
+    more = __syncthreads_or(changed);
+  }
+  // levels 2 .. H−1: warps own destination slots, lanes scan the incoming pools.  A slot changed at
+  // level h−1 iff its hop count is h−1; only those can improve a slot at level h (an unchanged
+  // predecessor's candidates were all candidates of level h−1 already), so the others are skipped.
+  for (int h = 2; more && h < H; ++h) {
+    const double* vp = val + (size_t)((h - 1) & 1) * nB;
+    double* vc = val + (size_t)(h & 1) * nB;
+    const uint8_t* hp = hops + (size_t)((h - 1) & 1) * nB;
+    uint8_t* hc = hops + (size_t)(h & 1) * nB;
+    int changed = 0;
+    for (int s = warp; s < nB; s += nwarp) {
+      const int32_t b = G.tok[s];
+      BpKey key = bp_none();
+      if (b != j && b != i) {
+        const int32_t d = G.deg[s];
+        for (int m = lane; m < d; m += 32) {
+          const int u = G.nbr[(int64_t)nB * s + m];
+          if (hp[u] != h - 1) continue;
+          bp_hop(P, ix, G.pair[(int64_t)nB * s + m], out ? b : G.tok[u], vp[u], out, h, G.tok[u], m, key);
+        }
+      }
+      key = bp_warp_best(key);
+      if (lane == 0) {
+        const double prev = vp[s];
+        const bool better = key.from != -1 && (out ? -key.s < prev : key.s > prev);
+        vc[s] = better ? (out ? -key.s : key.s) : prev;
+        hc[s] = better ? (uint8_t)h : hp[s];
+        pred[(size_t)(h - 1) * nB + s] = better ? (int16_t)key.from : kBpCarry;
+        ppos[(size_t)(h - 1) * nB + s] = better ? key.pos : 0;
+        changed |= better;
+      }
+    }
+    top = h;
+    more = __syncthreads_or(changed);
+  }
+  // the final hop into T, one thread per slot reached at level top, and S itself (the direct pair,
+  // pseudo-slot nB); then the CTA's best
+  {
+    const double* vt = val + (size_t)(top & 1) * nB;
+    const uint8_t* ht = hops + (size_t)(top & 1) * nB;
+    BpKey key = bp_none();
+    for (int s = tid; s <= nB; s += blockDim.x) {
+      if (s == nB) {
+        if (direct >= 0) bp_hop(P, ix, direct, j, amt, out, 1, S, nB, key);
+      } else {
+        const int32_t b = G.tok[s];
+        if (b == j || b == i || epair[s] < 0 || !(out ? vt[s] < kPathInf : vt[s] > 0.0)) continue;
+        bp_hop(P, ix, epair[s], out ? j : b, vt[s], out, ht[s] + 1, b, s, key);
+      }
+    }
+    key = bp_warp_best(key);
+    if (lane == 0) red[warp] = key;
+  }
+  __syncthreads();
+  if (tid != 0) return;
+  BpKey best = red[0];
+  for (int w = 1; w < nwarp; ++w)
+    if (bp_before(red[w], best)) best = red[w];
+  int64_t* row_pos = hop_pos + (int64_t)H * r;
+  uint8_t* row_set = hop_set + (int64_t)H * r;
+  uint8_t* row_tok1 = hop_tok1 + (int64_t)H * r;
+  if (best.from < 0) {
+    nhop[r] = 0;
+    value[r] = 0.0;
+    status[r] = 2;  // CFMM_ORDER_UNREACHABLE
+    return;
+  }
+  // rebuild the walk in DP order: (pair, position, DP-predecessor token, DP-successor token)
+  int32_t wk[kBestPathMaxHops], wpos[kBestPathMaxHops], wfrom[kBestPathMaxHops], wto[kBestPathMaxHops];
+  int n = 0;
+  int s = best.from;
+  wk[n] = s == nB ? direct : epair[s];
+  wpos[n] = best.pos;
+  wfrom[n] = s == nB ? S : G.tok[s];
+  wto[n++] = T;
+  for (int h = top; s != nB && h >= 1; --h) {
+    const int16_t pr = pred[(size_t)(h - 1) * nB + s];
+    if (pr == kBpCarry) continue;
+    const int ps = ppos[(size_t)(h - 1) * nB + s];
+    if (pr == kBpFromSource) {
+      wk[n] = spair[s];
+      wpos[n] = ps;
+      wfrom[n] = S;
+      wto[n++] = G.tok[s];
+      break;
+    }
+    const int u = G.nbr[(int64_t)nB * s + pr];
+    wk[n] = G.pair[(int64_t)nB * s + pr];
+    wpos[n] = ps;
+    wfrom[n] = G.tok[u];
+    wto[n++] = G.tok[s];
+    s = u;
+  }
+  // path order: exact-in walked back from i (reverse it), exact-out forward from j.  Hop g tenders
+  // a and delivers c.
+  bool repeats = false;
+  for (int g = 0; g < n; ++g) {
+    const int w = out ? g : n - 1 - g;
+    const int32_t a = out ? wto[w] : wfrom[w], c = out ? wfrom[w] : wto[w];
+    const HubHop hh = hub_hop(P, ix.pool[ix.off[wk[w]] + wpos[w]], a);
+    row_set[g] = (uint8_t)hh.k;
+    row_pos[g] = hh.p;
+    row_tok1[g] = hh.tok1;
+    hop_token[(int64_t)H * r + g] = c + 1;
+    for (int f = 0; f < g; ++f) repeats |= row_set[f] == row_set[g] && row_pos[f] == row_pos[g];
+  }
+  if (repeats) {
+    nhop[r] = 0;
+    value[r] = 0.0;
+    status[r] = 4;  // CFMM_PATH_REPEATS_POOL
+    return;
+  }
+  const int64_t off[2] = {0, n};
+  uint8_t st;
+  path_run<false>(P, 0, off, row_set, row_pos, row_tok1, kind + r, amount + r, nullptr, tender + (int64_t)H * r,
+                  received + (int64_t)H * r, &st);
+  nhop[r] = n;
+  value[r] = out ? tender[(int64_t)H * r] : received[(int64_t)H * r + n - 1];
+  status[r] = st;
+}
+
+}  // namespace cfmm

@@ -39,6 +39,7 @@
 #include "route_kernels.cuh"
 #include "arb_scan_kernels.cuh"
 #include "hub_kernels.cuh"
+#include "best_path_kernels.cuh"
 #include "univ3_state.cuh"
 
 #include <cub/cub.cuh>
@@ -3707,6 +3708,123 @@ int choose_order_hubs(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const i
   return CFMM_OK;
 }
 
+// ---- best paths through allowed tokens (best_path_kernels.cuh) ----------------------------------
+
+// Every argument of cfmm_find_order_paths, before anything runs: split orders' rows, max_hops, the
+// mask (required) and each row's |B| (the allowed tokens other than its two), and the CSR outputs.
+int check_find_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                     const uint8_t* kind, const double* amount, int max_hops, const uint8_t* allowed,
+                     const int64_t* hop_off, const int* hop_type, const int64_t* hop_pool, const int64_t* hop_token) {
+  const char* what = "find_order_paths";
+  int rc = check_split(ctx, q, token_in, token_out, kind, amount, nullptr, what);
+  if (rc != CFMM_OK) return rc;
+  if (max_hops < 1 || max_hops > CFMM_PATH_MAX_HOPS)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: max_hops %d, not 1..%d", what, max_hops, CFMM_PATH_MAX_HOPS);
+  if (!allowed) return fail(ctx, CFMM_ERR_INVALID, "%s: null allowed (the intermediate tokens are required)", what);
+  if (q == 0) return CFMM_OK;
+  if (!hop_off || !hop_type || !hop_pool || !hop_token)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: null hop_off, hop_type, hop_pool or hop_token", what);
+  int64_t n_allowed = 0;
+  for (int64_t t = 0; t < ctx->n_tokens; ++t) n_allowed += allowed[t] != 0;
+  for (int64_t r = 0; r < q; ++r) {
+    const int64_t nb = n_allowed - (allowed[token_in[r] - 1] != 0) - (allowed[token_out[r] - 1] != 0);
+    if (nb > CFMM_BEST_PATH_MAX_TOKENS)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: %lld intermediate tokens, more than %d", what, (long long)r,
+                  (long long)nb, CFMM_BEST_PATH_MAX_TOKENS);
+  }
+  return CFMM_OK;
+}
+
+int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const uint8_t* kind,
+                     const double* amount, int max_hops, const uint8_t* allowed, int64_t* hop_off, int* hop_type,
+                     int64_t* hop_pool, int64_t* hop_token, double* hop_tender, double* hop_received, double* value,
+                     uint8_t* status) {
+  int rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  if ((rc = ensure_adjacency(ctx)) != CFMM_OK) return rc;
+  auto& ix = ctx->pairs;
+  cudaStream_t st = ctx->stream;
+  OrderSets os;
+  if ((rc = order_sets(ctx, false, os)) != CFMM_OK) return rc;
+  // the call's slots: the allowed tokens, ascending
+  std::vector<int32_t> tok, slot_of((size_t)ctx->n_tokens, -1);
+  for (int64_t t = 0; t < ctx->n_tokens; ++t)
+    if (allowed[t]) {
+      slot_of[(size_t)t] = (int32_t)tok.size();
+      tok.push_back((int32_t)t);
+    }
+  const int nB = (int)tok.size(), H = max_hops;
+  const size_t slots = (size_t)q * (size_t)H, nn = (size_t)nB * (size_t)nB;
+  DevBuf<int64_t> d_in, d_out, d_pos, d_token;
+  DevBuf<int32_t> d_tok, d_slot, d_deg, d_gpair, d_nhop;
+  DevBuf<int16_t> d_gnbr;
+  DevBuf<uint8_t> d_kind, d_set, d_tok1, d_status;
+  DevBuf<double> d_amount, d_tender, d_recv, d_value;
+  CU_TRY(ctx, d_in.upload(token_in, (size_t)q));
+  CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
+  CU_TRY(ctx, d_kind.upload(kind, (size_t)q));
+  CU_TRY(ctx, d_amount.upload(amount, (size_t)q));
+  CU_TRY(ctx, d_tok.upload(tok));
+  CU_TRY(ctx, d_slot.upload(slot_of));
+  CU_TRY(ctx, d_deg.alloc((size_t)nB));
+  CU_TRY(ctx, d_gnbr.alloc(nn));
+  CU_TRY(ctx, d_gpair.alloc(nn));
+  CU_TRY(ctx, d_nhop.alloc((size_t)q));
+  CU_TRY(ctx, d_set.alloc(slots));
+  CU_TRY(ctx, d_pos.alloc(slots));
+  CU_TRY(ctx, d_tok1.alloc(slots));
+  CU_TRY(ctx, d_token.alloc(slots));
+  CU_TRY(ctx, d_tender.alloc(slots));
+  CU_TRY(ctx, d_recv.alloc(slots));
+  CU_TRY(ctx, d_value.alloc((size_t)q));
+  CU_TRY(ctx, d_status.alloc((size_t)q));
+  const size_t smem = cfmm::best_path_smem(nB, H);
+  CU_TRY(ctx, cudaFuncSetAttribute(cfmm::best_path_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const cfmm::PairIndexView pv{ix.off.p, ix.pool.p};
+  const cfmm::AdjView A{ix.adj_off.p, ix.adj_nbr.p, ix.adj_pair.p};
+  const cfmm::BestPathGraph G{d_tok.p, d_slot.p, d_deg.p, d_gnbr.p, d_gpair.p, nB};
+  if ((rc = launch(ctx, kProfSwaps, nB > 0 ? 2 : 1, [&] {
+         if (nB > 0)
+           cfmm::best_path_graph_kernel<<<(unsigned)((32 * (int64_t)nB + 255) / 256), 256, 0, st>>>(
+               A, d_tok.p, d_slot.p, nB, d_deg.p, d_gnbr.p, d_gpair.p);
+         cfmm::best_path_kernel<<<(unsigned)q, cfmm::kBestPathThreads, smem, st>>>(
+             os.d_P.p, pv, A, G, d_in.p, d_out.p, d_kind.p, d_amount.p, H, d_nhop.p, d_set.p, d_pos.p, d_tok1.p,
+             d_token.p, d_tender.p, d_recv.p, d_value.p, d_status.p);
+       })) != CFMM_OK)
+    return rc;
+  std::vector<int32_t> nhop((size_t)q);
+  std::vector<uint8_t> set(slots);
+  std::vector<int64_t> pos(slots), token(slots);
+  std::vector<double> tender(hop_tender ? slots : 0), recv(hop_received ? slots : 0);
+  CU_TRY(ctx, read_back(ctx, nhop.data(), d_nhop.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, set.data(), d_set.p, slots));
+  CU_TRY(ctx, read_back(ctx, pos.data(), d_pos.p, slots));
+  CU_TRY(ctx, read_back(ctx, token.data(), d_token.p, slots));
+  CU_TRY(ctx, read_back(ctx, hop_tender ? tender.data() : nullptr, d_tender.p, slots));
+  CU_TRY(ctx, read_back(ctx, hop_received ? recv.data() : nullptr, d_recv.p, slots));
+  CU_TRY(ctx, read_back(ctx, value, d_value.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, status, d_status.p, (size_t)q));
+  CU_TRY(ctx, cudaStreamSynchronize(st));
+  // pack each row's first nhop[r] slots; (set, device position) -> (type, index in the type's
+  // insertion order), as cfmm_pair_pools reports a pool
+  hop_off[0] = 0;
+  for (int64_t r = 0; r < q; ++r) {
+    const int64_t g = hop_off[r];
+    for (int64_t h = 0; h < nhop[(size_t)r]; ++h) {
+      const size_t w = (size_t)(H * r + h);
+      const int k = set[w];
+      hop_type[g + h] = k >> 1;
+      hop_pool[g + h] = path_set(ctx, k).order[(size_t)pos[w]] + ((k & 1) ? ctx->sets[k >> 1].m : 0);
+      hop_token[g + h] = token[w];
+      if (hop_tender) hop_tender[g + h] = tender[w];
+      if (hop_received) hop_received[g + h] = recv[w];
+    }
+    hop_off[r + 1] = g + nhop[(size_t)r];
+  }
+  return CFMM_OK;
+}
+
 }  // namespace
 
 int cfmm_pair_pools(cfmm_ctx* ctx, int64_t q, const int64_t* token_a, const int64_t* token_b, int64_t* count,
@@ -3832,6 +3950,21 @@ int cfmm_choose_order_hubs(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, co
   }
   return choose_order_hubs(ctx, q, token_in, token_out, kind, amount, max_hubs, allowed, hub_off, hubs, hub_score,
                            n_eligible);
+}
+
+int cfmm_find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                          const uint8_t* kind, const double* amount, int max_hops, const uint8_t* allowed,
+                          int64_t* hop_off, int* hop_type, int64_t* hop_pool, int64_t* hop_token, double* hop_tender,
+                          double* hop_received, double* value, uint8_t* status) {
+  int rc = check_find_paths(ctx, q, token_in, token_out, kind, amount, max_hops, allowed, hop_off, hop_type, hop_pool,
+                            hop_token);
+  if (rc != CFMM_OK) return rc;
+  if (q == 0) {
+    if (hop_off) hop_off[0] = 0;
+    return CFMM_OK;
+  }
+  return find_order_paths(ctx, q, token_in, token_out, kind, amount, max_hops, allowed, hop_off, hop_type, hop_pool,
+                          hop_token, hop_tender, hop_received, value, status);
 }
 
 // ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------

@@ -591,6 +591,28 @@ function choose_order_hubs(ctx, token_in::Vector{Int64}, token_out::Vector{Int64
     return hub_off, hubs[1:n], score[1:n], n_elig
 end
 
+# The best path of each order row through allowed tokens (cfmm_find_order_paths): at most max_hops
+# (1..8) hops, one pool per hop, every intermediate token t with allowed[t] != 0 (required, one entry
+# per token).  Returns (hop_off, hop_type, hop_pool, hop_token, hop_tender, hop_received, value,
+# status); hop_off, hop_type and hop_pool go to quote_paths / execute_paths! as they are.  Never
+# executed, like the rest of this file.
+function find_order_paths(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}, kind::Vector{UInt8},
+                          amount::Vector{Float64}, max_hops::Integer, allowed::Vector{UInt8})
+    q = length(token_in)
+    length(token_out) == length(kind) == length(amount) == q ||
+        throw(ArgumentError("token_in / token_out / kind / amount need q entries"))
+    cap = max(q * max_hops, 1)
+    hop_off, typ, pool, tok = zeros(Int64, q + 1), zeros(Cint, cap), zeros(Int64, cap), zeros(Int64, cap)
+    tender, received, value, status = zeros(cap), zeros(cap), zeros(q), zeros(UInt8, q)
+    chk(ctx, ccall((:cfmm_find_order_paths, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Cint, Ptr{UInt8}, Ptr{Int64},
+         Ptr{Cint}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8}),
+        ctx, q, token_in, token_out, kind, amount, max_hops, allowed, hop_off, typ, pool, tok, tender, received,
+        value, status))
+    n = hop_off[end]
+    return hop_off, typ[1:n], pool[1:n], tok[1:n], tender[1:n], received[1:n], value, status
+end
+
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
 # current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never

@@ -671,6 +671,39 @@ class DevicePools:
         n = int(hub_off[-1])
         return hub_off, hubs[:n].copy(), score[:n].copy(), n_elig
 
+    # -- best paths through allowed tokens (include/cfmm_b200.h, cfmm_find_order_paths) ----------
+    def find_order_paths(self, token_in, token_out, kind, amount, max_hops: int, allowed):
+        """cfmm_find_order_paths: for row j (sell token_in[j] for token_out[j], 1-based; kind 0
+        tenders amount[j], kind 1 wants amount[j]) the best single path of at most max_hops (1..8)
+        hops, one pool per hop, whose intermediate tokens t have allowed[t - 1] (a mask [n_tokens],
+        at most 1024 such tokens per row besides the row's two).  No state changes.  Returns (hop_off
+        [q + 1], hop_type [Σ], hop_pool [Σ], hop_token [Σ] delivered, hop_tender [Σ], hop_received
+        [Σ], value [q], status [q] uint8); the first three go to quote_paths / execute_paths as they
+        are.  Status 0 filled, 2 no path, 4 (PATH_REPEATS_POOL) the best walk uses a pool twice."""
+        tin = np.ascontiguousarray(token_in, dtype=np.int64).reshape(-1)
+        tout = np.ascontiguousarray(token_out, dtype=np.int64).reshape(-1)
+        kind = np.ascontiguousarray(kind, dtype=np.uint8).reshape(-1)
+        amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
+        q = len(tin)
+        if not (len(tout) == len(kind) == len(amount) == q):
+            raise ValueError("find_order_paths: token_in, token_out, kind and amount need one entry per row")
+        mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
+        if len(mask) != self.n_tokens:
+            raise ValueError(f"find_order_paths: allowed must have {self.n_tokens} entries, one per token")
+        u8, i32 = C.POINTER(C.c_uint8), C.POINTER(C.c_int)
+        cap = max(q * max(int(max_hops), 0), 1)
+        hop_off = np.zeros(q + 1, dtype=np.int64)
+        typ, pool, tok = np.zeros(cap, dtype=np.int32), np.zeros(cap, dtype=np.int64), np.zeros(cap, dtype=np.int64)
+        tender, received = np.zeros(cap), np.zeros(cap)
+        value, status = np.zeros(q), np.zeros(q, dtype=np.uint8)
+        self._chk(self._lib.cfmm_find_order_paths(self._ctx, q, _ip(tin), _ip(tout), kind.ctypes.data_as(u8),
+                                                  _dp(amount), int(max_hops), mask.ctypes.data_as(u8), _ip(hop_off),
+                                                  typ.ctypes.data_as(i32), _ip(pool), _ip(tok), _dp(tender),
+                                                  _dp(received), _dp(value), status.ctypes.data_as(u8)))
+        n = int(hop_off[-1])
+        return (hop_off, typ[:n].copy(), pool[:n].copy(), tok[:n].copy(), tender[:n].copy(), received[:n].copy(),
+                value, status)
+
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
         """cfmm_modify_univ3_liquidity: row j adds dL[j] (> 0 mints, < 0 burns) to the ticks of UniV3
@@ -1188,6 +1221,59 @@ class Router:
                                                             "execute_auto_routed_orders")
         hubs = [flat[off[r]:off[r + 1]].tolist() for r in range(len(tin))]
         return self.execute_routed_orders(tin, tout, kinds, amounts, hubs, limits) + (hubs,)
+
+    def _find(self, token_in, token_out, kinds, amounts, allowed, max_hops, limits, what):
+        tin, tout, kinds, amounts, limits = self._split_args(token_in, token_out, kinds, amounts, limits, what)
+        if not 1 <= int(max_hops) <= _lib.PATH_MAX_HOPS:
+            raise ValueError(f"{what}: max_hops must be 1..{_lib.PATH_MAX_HOPS}")
+        if allowed is None:
+            raise ValueError(f"{what}: allowed (a mask over the tokens) is required")
+        found = self._pools.find_order_paths(tin, tout, kinds, amounts, int(max_hops), allowed)
+        off, typ, pool = found[:3]
+        paths = [[self._type_lists[int(typ[h])][int(pool[h])] for h in range(off[r], off[r + 1])]
+                 for r in range(len(tin))]
+        return tin, tout, kinds, amounts, limits, found, paths
+
+    def find_paths(self, token_in, token_out, kinds, amounts, allowed, max_hops: int = _lib.PATH_MAX_HOPS):
+        """Find each order row's best single path on the device (cfmm_find_order_paths): at most
+        max_hops hops from token_in[j] to token_out[j] (1-based), one pool per hop, every intermediate
+        token t with allowed[t - 1] (a mask over the tokens), ranked by the amount out (kind 0, for
+        amounts[j] in) or in (kind 1, for amounts[j] out).  No state changes.  Returns (paths, value
+        [q], status [q]): paths[j] lists r.cfmms positions in hop order (empty without a path), ready
+        for quote_paths / execute_paths with token_in.  Single GPU."""
+        *_, found, paths = self._find(token_in, token_out, kinds, amounts, allowed, max_hops, None, "find_paths")
+        return paths, found[6], found[7]
+
+    def quote_best_paths(self, token_in, token_out, kinds, amounts, allowed, max_hops: int = _lib.PATH_MAX_HOPS):
+        """find_paths, priced: what quote_paths returns for the found paths, bit for bit (the find's
+        amounts are that recursion).  Returns (paid [q], received [q], status [q], paths); a row
+        without a path has paid = received = 0 and the find's status.  No state changes.  Single
+        GPU."""
+        *_, found, paths = self._find(token_in, token_out, kinds, amounts, allowed, max_hops, None,
+                                      "quote_best_paths")
+        off, tender, received, status = found[0], found[4], found[5], found[7]
+        has = np.diff(off) > 0
+        paid, got = np.zeros(len(paths)), np.zeros(len(paths))
+        paid[has], got[has] = tender[off[:-1][has]], received[off[1:][has] - 1]
+        return paid, got, status, paths
+
+    def execute_best_paths(self, token_in, token_out, kinds, amounts, allowed, max_hops: int = _lib.PATH_MAX_HOPS,
+                           limits=None):
+        """find_paths, then execute_paths over the rows that have a path, with the optional limits
+        (kind 0: the minimum received; kind 1: the maximum paid).  Every row's path is found once, on
+        the state at entry; the execute re-prices each path on the state the earlier paths left.
+        Returns what quote_best_paths returns (rows without a path: zeros and the find's status) and
+        refreshes the touched pool objects, as execute_paths does.  Single GPU."""
+        tin, _, kinds, amounts, limits, found, paths = self._find(token_in, token_out, kinds, amounts, allowed,
+                                                                  max_hops, limits, "execute_best_paths")
+        status = found[7].copy()
+        paid, got = np.zeros(len(paths)), np.zeros(len(paths))
+        rows = np.array([r for r in range(len(paths)) if paths[r]], dtype=np.int64)
+        if len(rows):
+            p, g, s, _, _ = self.execute_paths([paths[r] for r in rows], tin[rows], kinds[rows], amounts[rows],
+                                               None if limits is None else limits[rows])
+            paid[rows], got[rows], status[rows] = p, g, s
+        return paid, got, status, paths
 
     def _arbitrage_args(self, base, other, hubs, min_profit, what):
         if self._world > 1:

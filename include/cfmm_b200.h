@@ -701,6 +701,67 @@ int cfmm_choose_order_hubs(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* 
                            int64_t *hubs /* [q·max_hubs] */, double *hub_score /* [q·max_hubs] or NULL */,
                            int64_t *n_eligible /* [q] or NULL */);
 
+/* ---- the best path of each order row through allowed tokens --------------------------------
+ * For each order row (j = token_in[r], i = token_out[r], kind[r], amount[r], split orders' rules),
+ * the best single path of at most H = max_hops (1..CFMM_PATH_MAX_HOPS) hops from j to i whose
+ * intermediate tokens are in B, one pool per hop, as cfmm_execute_paths takes it.
+ *   B           the tokens t with allowed[t-1] != 0 (allowed [n_tokens], required), minus j and i;
+ *               at most CFMM_BEST_PATH_MAX_TOKENS per row.  A token of B can appear more than once
+ *               in a path; j and i appear only at its ends.
+ *   hops        a hop u → v uses one active pool of {u, v}: all three types, appended pools
+ *               included, a pool stored with its tokens exchanged mapped back (the pools
+ *               cfmm_pair_pools lists for {u, v}, retired ones skipped).  f_k is the exact-input
+ *               quote of pool k (cfmm_quote_swaps bit for bit), x*_k the exact-out search
+ *               (cfmm_quote_swaps_exact_out bit for bit), both on the state at this call.
+ *   exact-in    (kind CFMM_SWAP_EXACT_IN, δ = amount) "at most h hops", level by level.  a₀(j) = δ;
+ *               every other token is unreached.  For h = 1 … H−1 and u ∈ B, the candidates are
+ *               f_k(a_{h−1}(u')) over every reached u' ∈ {j} ∪ B and every active pool k of {u', u}
+ *               with u' tendered; a candidate counts only when it is > 0 (NaNs are ignored).
+ *               a_h(u) is the best candidate when it is strictly greater than a_{h−1}(u), else
+ *               a_{h−1}(u) (a reached u stays reached, j keeps δ).  The final hop's candidates are
+ *               f_k(a_{H−1}(u)) over the active pools of {u, i}, u ∈ {j} ∪ B reached; the best is
+ *               the path, its value the i received.
+ *   exact-out   (kind CFMM_SWAP_EXACT_OUT, y = amount) the mirror image, backwards from i: c₀(i) = y;
+ *               for u ∈ B the candidates are x*_k(c_{h−1}(v)) over reached v ∈ {i} ∪ B and the
+ *               active pools k of {u, v} with u tendered, kept when finite; c_h(u) is the best when
+ *               strictly smaller than c_{h−1}(u).  The final hop's candidates are x*_k(c_{H−1}(v))
+ *               over the active pools of {j, v} with j tendered; the value is the j paid.
+ *   ranking     candidates rank by the amount (larger exact-in, smaller exact-out), then fewer
+ *               hops, then the smaller predecessor token (u' exact-in, v exact-out; j or i at the
+ *               first hop of the DP), then the earlier position in {u', u}'s cfmm_pair_pools list.
+ *               That is a total order, so the result does not depend on the evaluation order.
+ * Outputs.  The walk is rebuilt from each level's predecessors, in path order j → … → i, as packed
+ * CSR: hop_off [q+1] (hop_off[0] = 0; at most q·max_hops hops), hop_type / hop_pool (a pool as
+ * cfmm_quote_paths addresses it) and hop_token (1-based, the token each hop delivers; the last is
+ * i).  hop_tender / hop_received (NULL: not written) are the DP's amounts, which are cfmm_quote_paths'
+ * hop_tender / hop_received on the returned path bit for bit (the same recursion: x_{h+1} = λ_h
+ * exact-in, y_{h−1} = x_h exact-out).  value [q] (NULL: not written) = the i received (exact-in) or
+ * the j paid (exact-out), 0 for a row without a path.  status [q] (NULL: not written):
+ *   CFMM_ORDER_FILLED       a path was found (amount 0: no hops, value 0);
+ *   CFMM_ORDER_UNREACHABLE  no path of at most max_hops hops through B: no hops;
+ *   CFMM_PATH_REPEATS_POOL  the best walk holds a gaining cycle that uses one pool twice (under
+ *                           quotes on the unchanged state, a cycle through B can gain); it is not
+ *                           a path cfmm_execute_paths accepts, so no hops are written.
+ * Execute: pass the rows with hops to cfmm_execute_paths (Python Router.execute_best_paths).  The
+ * paths are found once, on the state at this call; the execute re-prices each path on the state
+ * the earlier paths left.
+ *
+ * Synchronous; changes no state.  Before cfmm_finalize: CFMM_ERR_STATE.  CFMM_ERR_INVALID before
+ * anything runs for every argument split orders reject, max_hops outside 1..CFMM_PATH_MAX_HOPS, a
+ * null allowed, a row whose B holds more than CFMM_BEST_PATH_MAX_TOKENS tokens, and a null hop_off,
+ * hop_type, hop_pool or hop_token with q > 0.  q == 0 writes hop_off[0] = 0 (when given) and runs
+ * nothing. */
+#define CFMM_BEST_PATH_MAX_TOKENS 1024
+#define CFMM_PATH_REPEATS_POOL 4
+int cfmm_find_order_paths(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [q] */,
+                          const int64_t *token_out /* [q] */, const uint8_t *kind /* [q] */,
+                          const double *amount /* [q] */, int max_hops /* 1..CFMM_PATH_MAX_HOPS */,
+                          const uint8_t *allowed /* [n_tokens], required */, int64_t *hop_off /* [q+1] */,
+                          int *hop_type /* [q·max_hops] */, int64_t *hop_pool /* [q·max_hops] */,
+                          int64_t *hop_token /* [q·max_hops] */, double *hop_tender /* [q·max_hops] or NULL */,
+                          double *hop_received /* [q·max_hops] or NULL */, double *value /* [q] or NULL */,
+                          uint8_t *status /* [q] or NULL */);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
@@ -849,7 +910,8 @@ int64_t cfmm_launch_count(const cfmm_ctx *ctx);
  * cfmm_quote_swaps_exact_out / cfmm_execute_swap_orders / cfmm_quote_paths /
  * cfmm_execute_paths / cfmm_pair_pools / cfmm_quote_split_orders /
  * cfmm_execute_split_orders / cfmm_quote_routed_orders / cfmm_execute_routed_orders /
- * cfmm_choose_order_hubs, the pair-index build counted as one launch); it
+ * cfmm_choose_order_hubs / cfmm_find_order_paths, the pair-index build counted as one
+ * launch); it
  * synchronises on the recorded events.
  * cfmm_profile_reset re-arms the same N pairs. */
 int cfmm_profile_read(cfmm_ctx *ctx, int type, double *total_ms, int64_t *launches);
