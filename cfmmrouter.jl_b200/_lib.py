@@ -37,6 +37,9 @@ ROUTE_MAX_HUBS = 7  # CFMM_ROUTE_MAX_HUBS
 # cfmm_find_order_paths
 BEST_PATH_MAX_TOKENS = 1024
 PATH_REPEATS_POOL = 4
+# cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders
+SUBGRAPH_MAX_TOKENS = 256
+ORDER_NOT_CONVERGED = 5
 
 COMM_HANDLE_BYTES = 128
 
@@ -47,6 +50,21 @@ class SolveOpts(C.Structure):
 class SolveInfo(C.Structure):
     _fields_ = [("iterations", C.c_int), ("fun_evals", C.c_int), ("status", C.c_int),
                 ("f", C.c_double), ("pg_norm", C.c_double), ("solve_ms", C.c_double)]
+
+
+class SubgraphOpts(C.Structure):
+    _fields_ = [("max_iter", C.c_int), ("max_fun", C.c_int), ("rtol", C.c_double), ("factr", C.c_double)]
+
+
+class SubgraphOut(C.Structure):
+    _fields_ = [("paid", C.POINTER(C.c_double)), ("received", C.POINTER(C.c_double)),
+                ("status", C.POINTER(C.c_uint8)), ("solver_status", C.POINTER(C.c_int)),
+                ("iterations", C.POINTER(C.c_int)), ("fun_evals", C.POINTER(C.c_int)),
+                ("merit", C.POINTER(C.c_double)), ("tok_off", C.POINTER(C.c_int64)), ("tok_cap", C.c_int64),
+                ("token", C.POINTER(C.c_int64)), ("nu", C.POINTER(C.c_double)), ("psi", C.POINTER(C.c_double)),
+                ("leg_off", C.POINTER(C.c_int64)), ("leg_cap", C.c_int64), ("leg_type", C.POINTER(C.c_int)),
+                ("leg_pool", C.POINTER(C.c_int64)), ("leg_delta", C.POINTER(C.c_double)),
+                ("leg_lambda", C.POINTER(C.c_double))]
 
 
 # every symbol include/cfmm_b200.h declares: name -> (restype, argtypes)
@@ -111,6 +129,10 @@ SYMBOLS = {
     "cfmm_find_order_paths": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, C.c_int,
                                         C.POINTER(C.c_uint8), _ip, C.POINTER(C.c_int), _ip, _ip, _dp, _dp, _dp,
                                         C.POINTER(C.c_uint8)]),
+    "cfmm_quote_subgraph_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _dp, C.POINTER(C.c_uint8),
+                                             C.POINTER(SubgraphOpts), C.POINTER(SubgraphOut)]),
+    "cfmm_execute_subgraph_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _dp, _dp, C.POINTER(C.c_uint8),
+                                               C.POINTER(SubgraphOpts), C.POINTER(SubgraphOut)]),
     "cfmm_modify_univ3_liquidity":(C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),

@@ -33,6 +33,8 @@
 #include "sweep_kernels.cuh"
 #include "product_tma.cuh"
 #include "solver.cuh"
+#include "solver_control.cuh"
+#include "subgraph_kernels.cuh"
 #include "swap_kernels.cuh"
 #include "path_kernels.cuh"
 #include "split_kernels.cuh"
@@ -1750,7 +1752,6 @@ int cfmm_solve(cfmm_ctx* ctx, const double* lin, const double* lower, const doub
 
   double h[NG + 8];
   int fevals = 0;
-  const double epsmch = 2.220446049250313e-16;
   auto evaluate = [&](double* f_out) -> int {  // sweep at xt, gt = lin + Ψ, f = linᵀxt + acc
     const double* view = nullptr;
     int r = enqueue_sweep(ctx, q.xt, nullptr, false, st, &view);
@@ -1790,101 +1791,49 @@ int cfmm_solve(cfmm_ctx* ctx, const double* lin, const double* lower, const doub
   if ((rc = evaluate(&f)) != CFMM_OK) return rc;
   if ((rc = commit(0, 0)) != CFMM_OK) return rc;
 
-  int age[M];      // history slots, oldest first
-  int cnt = 0, head = 0, iter = 0, status = 2, small_steps = 0;
+  cfmm::LbfgsHistory hist_ages;  // history slots, oldest first
+  hist_ages.cnt = hist_ages.head = 0;
+  int iter = 0, status = 2, small_steps = 0;
   while (true) {
     if (!(f == f)) { status = 5; break; }            // NaN objective
     if (pgnorm <= o.pgtol) { status = 0; break; }
     if (iter >= o.max_iter) { status = 2; break; }
     if (fevals >= o.max_fun) { status = 3; break; }
-    // ---- two-loop recursion in coefficient space over B = [S Y pg] ------------------------
+    // ---- two-loop recursion in coefficient space over B = [S Y pg] (solver_control.cuh) -------
     cfmm::SolverCoef cf;
-    for (int j = 0; j < K; ++j) cf.c[j] = 0.0;
-    cf.c[K - 1] = 1.0;
-    double t_init = 1.0;
-    if (cnt == 0) {
-      const double nrm = std::sqrt(W[K - 1][K - 1]);
-      t_init = nrm > 0.0 ? std::min(1.0, 1.0 / nrm) : 1.0;   // first step of length <= 1, like L-BFGS-B
-    } else {
-      double alpha[M], rho[M];
-      for (int a = cnt - 1; a >= 0; --a) {
-        const int j = age[a];
-        rho[a] = 1.0 / W[j][M + j];
-        double sq = 0.0;
-        for (int c = 0; c < K; ++c) sq += W[j][c] * cf.c[c];
-        alpha[a] = rho[a] * sq;
-        cf.c[M + j] -= alpha[a];
-      }
-      const int jn = age[cnt - 1];
-      const double gamma = W[jn][M + jn] / W[M + jn][M + jn];
-      for (int c = 0; c < K; ++c) cf.c[c] *= gamma;
-      for (int a = 0; a < cnt; ++a) {
-        const int j = age[a];
-        double yr = 0.0;
-        for (int c = 0; c < K; ++c) yr += W[M + j][c] * cf.c[c];
-        cf.c[j] += alpha[a] - rho[a] * yr;
-      }
-    }
+    const double t_init = cfmm::lbfgs_direction(W, hist_ages, cf.c);
     cfmm::solver_direction_kernel<<<blocks, cfmm::kSolverThreads, 0, st>>>(q, cf);
     ctx->launches++;
     // ---- Armijo backtracking along the projected path ------------------------------------
-    // f is a sum of ~m terms of mixed sign: differences below ~8 eps |f| are rounding noise, and
-    // near the (very flat) optimum of a large market every useful step is that small -- a
-    // plain Armijo test would reject them all.  The slack admits them; pgtol / factr decide when
-    // to stop.
     double t = t_init, f_new = f;
     bool accepted = false, stalled = false;
     for (int ls = 0; ls < 30 && fevals < o.max_fun; ++ls) {
       cfmm::solver_trial_kernel<<<blocks, cfmm::kSolverThreads, 0, st>>>(q, t);
       ctx->launches++;
       if ((rc = evaluate(&f_new)) != CFMM_OK) return rc;
-      const double gdx = h[NG + 0], step2 = h[NG + 2];
-      if (step2 == 0.0) { stalled = true; break; }   // the projected step does not move
-      const double noise = 8.0 * epsmch * std::max(std::max(std::fabs(f), std::fabs(f_new)), 1.0);
-      if (gdx < 0.0 && f_new <= f + 1e-4 * gdx + noise) { accepted = true; break; }
-      if (!(gdx < 0.0) && cnt > 0) break;             // not a descent direction: restart from −pg
-      if (f_new == f_new && f_new < 1e300 && gdx < 0.0) {
-        // minimiser of the quadratic through f, the slope gdx (per unit t) and f_new, kept in [0.1 t, 0.5 t]
-        const double slope = gdx / t, denom = 2.0 * (f_new - f - gdx);
-        double tq = denom > 0.0 ? -slope * t * t / denom : 0.5 * t;
-        t = std::min(0.5 * t, std::max(0.1 * t, tq));
-      } else {
-        t *= 0.1;
-      }
+      const int d = cfmm::lbfgs_trial(f, f_new, h[NG + 0], h[NG + 2], hist_ages.cnt, t);
+      if (d == cfmm::kLsStall) { stalled = true; break; }
+      if (d == cfmm::kLsAccept) { accepted = true; break; }
+      if (d == cfmm::kLsRestart) break;
     }
     if (!accepted) {
-      if (cnt > 0 && !stalled) {  // drop the history and retry with steepest descent
-        cnt = 0;
+      if (hist_ages.cnt > 0 && !stalled) {  // drop the history and retry with steepest descent
+        hist_ages.cnt = 0;
         continue;
       }
       status = stalled ? 1 : 4;
       break;
     }
     // ---- accept: store (s, y), new Gram matrix / projected gradient --------------------------
-    const int slot = head;
+    const int slot = hist_ages.head;
     if ((rc = commit(slot, 1)) != CFMM_OK) return rc;
-    // drop the slot's old pair from the age list, append the new one if its curvature is usable
-    int w = 0;
-    for (int a = 0; a < cnt; ++a)
-      if (age[a] != slot) age[w++] = age[a];
-    cnt = w;
-    const double sy = W[slot][M + slot], yy = W[M + slot][M + slot];
-    if (sy > 1e-10 * yy && yy > 0.0) {
-      age[cnt++] = slot;
-      head = (head + 1) % M;
-    }
+    cfmm::lbfgs_store(W, slot, hist_ages);
     ++iter;
     const double f_old = f;
     f = f_new;
-    // L-BFGS-B's factr test -- on two consecutive steps: one short quasi-Newton step (fresh history,
-    // a bound just hit) is not yet evidence of convergence
-    if (f_old - f <= o.factr * epsmch * std::max(std::max(std::fabs(f_old), std::fabs(f)), 1.0)) {
-      if (++small_steps >= 2) {
-        status = 1;
-        break;
-      }
-    } else {
-      small_steps = 0;
+    if (cfmm::lbfgs_factr(f_old, f, o.factr, small_steps)) {
+      status = 1;
+      break;
     }
   }
   // final ν, and the trades at it (router.jl:106-107)
@@ -3965,6 +3914,270 @@ int cfmm_find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, con
   }
   return find_order_paths(ctx, q, token_in, token_out, kind, amount, max_hops, allowed, hop_off, hop_type, hop_pool,
                           hop_token, hop_tender, hop_received, value, status);
+}
+
+// ---- orders routed over every pool among their allowed tokens (subgraph_kernels.cuh) ------------
+namespace {
+
+// Every argument of cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders, before anything runs.
+int check_subgraph(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const double* amount,
+                   const double* limit, const uint8_t* allowed, const cfmm_subgraph_opts& o, const char* what) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if (q < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: negative row count", what);
+  if (!allowed) return fail(ctx, CFMM_ERR_INVALID, "%s: null allowed (the intermediate tokens are required)", what);
+  if (o.max_iter < 1 || o.max_fun < 1)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: max_iter %d and max_fun %d must be >= 1", what, o.max_iter, o.max_fun);
+  if (!(std::isfinite(o.rtol) && o.rtol > 0.0)) return fail(ctx, CFMM_ERR_INVALID, "%s: rtol %g must be finite and > 0", what, o.rtol);
+  if (!(std::isfinite(o.factr) && o.factr >= 0.0))
+    return fail(ctx, CFMM_ERR_INVALID, "%s: factr %g must be finite and >= 0", what, o.factr);
+  if (q == 0) return CFMM_OK;
+  if (!token_in || !token_out || !amount) return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
+  if ((rc = check_pair_tokens(ctx, q, token_in, token_out, what)) != CFMM_OK) return rc;
+  for (int64_t j = 0; j < q; ++j) {
+    if (!std::isfinite(amount[j]) || amount[j] < 0.0)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: amount %g must be finite and >= 0", what, (long long)j,
+                  amount[j]);
+    if (limit && !(std::isfinite(limit[j]) && limit[j] >= 0.0))
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: limit %g must be finite and >= 0", what, (long long)j,
+                  limit[j]);
+  }
+  int64_t n_allowed = 0;
+  for (int64_t t = 0; t < ctx->n_tokens; ++t) n_allowed += allowed[t] != 0;
+  for (int64_t r = 0; r < q; ++r) {
+    const int64_t nb = n_allowed - (allowed[token_in[r] - 1] != 0) - (allowed[token_out[r] - 1] != 0);
+    if (nb > CFMM_SUBGRAPH_MAX_TOKENS)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: %lld intermediate tokens, more than %d", what, (long long)r,
+                  (long long)nb, CFMM_SUBGRAPH_MAX_TOKENS);
+  }
+  return CFMM_OK;
+}
+
+int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                    const double* amount, const double* limit, const uint8_t* allowed, const cfmm_subgraph_opts& o,
+                    cfmm_subgraph_out* out) {
+  int rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  if ((rc = ensure_adjacency(ctx)) != CFMM_OK) return rc;
+  auto& ix = ctx->pairs;
+  cudaStream_t st = ctx->stream;
+  cfmm_subgraph_out none{};
+  const cfmm_subgraph_out& O = out ? *out : none;
+  // the call's slots: the allowed tokens, ascending; their filtered adjacency and its activity
+  std::vector<int32_t> tok, slot_of((size_t)ctx->n_tokens, -1);
+  for (int64_t t = 0; t < ctx->n_tokens; ++t)
+    if (allowed[t]) {
+      slot_of[(size_t)t] = (int32_t)tok.size();
+      tok.push_back((int32_t)t);
+    }
+  const int nB = (int)tok.size();
+  const size_t nn = (size_t)nB * (size_t)nB;
+  DevBuf<int64_t> d_in, d_out, d_ntok, d_npool;
+  DevBuf<int32_t> d_tok, d_slot, d_deg, d_gpair;
+  DevBuf<int16_t> d_gnbr;
+  DevBuf<uint8_t> d_act;
+  DevBuf<double> d_amount, d_limit;
+  CU_TRY(ctx, d_in.upload(token_in, (size_t)q));
+  CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
+  CU_TRY(ctx, d_amount.upload(amount, (size_t)q));
+  CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
+  CU_TRY(ctx, d_tok.upload(tok));
+  CU_TRY(ctx, d_slot.upload(slot_of));
+  CU_TRY(ctx, d_deg.alloc((size_t)nB));
+  CU_TRY(ctx, d_gnbr.alloc(nn));
+  CU_TRY(ctx, d_gpair.alloc(nn));
+  CU_TRY(ctx, d_act.alloc(nn));
+  CU_TRY(ctx, d_ntok.alloc((size_t)q));
+  CU_TRY(ctx, d_npool.alloc((size_t)q));
+  OrderSets os;
+  if ((rc = order_sets(ctx, false, os)) != CFMM_OK) return rc;
+  const cfmm::PairIndexView pv{ix.off.p, ix.pool.p};
+  const cfmm::AdjView A{ix.adj_off.p, ix.adj_nbr.p, ix.adj_pair.p};
+  const cfmm::BestPathGraph G{d_tok.p, d_slot.p, d_deg.p, d_gnbr.p, d_gpair.p, nB};
+  // a persistent grid: one wave of resident CTAs
+  int& occ = ctx->occupancy[reinterpret_cast<const void*>(&cfmm::subgraph_kernel<false>)];
+  if (occ == 0) {
+    CU_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cfmm::subgraph_kernel<false>,
+                                                              cfmm::kSubgraphThreads, 0));
+    if (occ < 1) return fail(ctx, CFMM_ERR_CUDA, "subgraph_kernel does not fit on an SM");
+  }
+  const int64_t wave = (int64_t)ctx->sm_count * occ;
+  const unsigned plan_grid = (unsigned)std::min<int64_t>(q, wave);
+  if ((rc = launch(ctx, kProfSwaps, nB > 0 ? 3 : 1, [&] {
+         if (nB > 0) {
+           cfmm::best_path_graph_kernel<<<(unsigned)((32 * (int64_t)nB + 255) / 256), 256, 0, st>>>(
+               A, d_tok.p, d_slot.p, nB, d_deg.p, d_gnbr.p, d_gpair.p);
+           cfmm::subgraph_act_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>(os.d_P.p, pv, G, d_act.p);
+         }
+         cfmm::subgraph_plan_kernel<<<plan_grid, cfmm::kSubgraphThreads, 0, st>>>(os.d_P.p, pv, A, G, d_act.p, d_in.p,
+                                                                                  d_out.p, q, d_ntok.p, d_npool.p);
+       })) != CFMM_OK)
+    return rc;
+  std::vector<int64_t> ntok((size_t)q), npool((size_t)q);
+  CU_TRY(ctx, read_back(ctx, ntok.data(), d_ntok.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, npool.data(), d_npool.p, (size_t)q));
+  CU_TRY(ctx, cudaStreamSynchronize(st));
+  std::vector<int64_t> tok_off((size_t)q + 1, 0), leg_off((size_t)q + 1, 0);
+  int64_t max_pool = 0;
+  for (int64_t r = 0; r < q; ++r) {
+    tok_off[(size_t)r + 1] = tok_off[(size_t)r] + ntok[(size_t)r];
+    leg_off[(size_t)r + 1] = leg_off[(size_t)r] + npool[(size_t)r];
+    max_pool = std::max(max_pool, npool[(size_t)r]);
+  }
+  const int64_t NT = tok_off[(size_t)q], L = leg_off[(size_t)q];
+  if (O.tok_off) std::copy(tok_off.begin(), tok_off.end(), O.tok_off);
+  if (O.leg_off) std::copy(leg_off.begin(), leg_off.end(), O.leg_off);
+  const bool want_tok = O.token || O.nu || O.psi, want_leg = O.leg_type || O.leg_pool || O.leg_delta || O.leg_lambda;
+  if (exec && ((want_tok && NT > O.tok_cap) || (want_leg && L > O.leg_cap)))
+    return fail(ctx, CFMM_ERR_INVALID,
+                "execute_subgraph_orders: the outputs need %lld token and %lld leg entries, above tok_cap %lld or "
+                "leg_cap %lld",
+                (long long)NT, (long long)L, (long long)O.tok_cap, (long long)O.leg_cap);
+  const bool toks = want_tok && NT > 0 && NT <= O.tok_cap, legs = want_leg && L > 0 && L <= O.leg_cap;
+  // a size query (no per-row output, and no token or leg output that fits) runs no solve
+  if (!exec && !toks && !legs && !O.paid && !O.received && !O.status && !O.solver_status && !O.iterations &&
+      !O.fun_evals && !O.merit)
+    return CFMM_OK;
+  // outputs and the per-CTA workspace
+  DevBuf<int64_t> d_tok_off, d_leg_off, d_token, d_entry;
+  DevBuf<double> d_paid, d_recv, d_merit, d_nu, d_psi, d_ld, d_ll;
+  DevBuf<uint8_t> d_status;
+  DevBuf<int32_t> d_sst, d_iter, d_fev;
+  CU_TRY(ctx, d_tok_off.upload(tok_off));
+  CU_TRY(ctx, d_leg_off.upload(leg_off));
+  CU_TRY(ctx, d_paid.alloc((size_t)q));
+  CU_TRY(ctx, d_recv.alloc((size_t)q));
+  CU_TRY(ctx, d_merit.alloc((size_t)q));
+  CU_TRY(ctx, d_status.alloc((size_t)q));
+  CU_TRY(ctx, d_sst.alloc((size_t)q));
+  CU_TRY(ctx, d_iter.alloc((size_t)q));
+  CU_TRY(ctx, d_fev.alloc((size_t)q));
+  if (toks) {
+    CU_TRY(ctx, d_token.alloc((size_t)NT));
+    CU_TRY(ctx, d_nu.alloc((size_t)NT));
+    CU_TRY(ctx, d_psi.alloc((size_t)NT));
+  }
+  if (legs) {
+    CU_TRY(ctx, d_entry.alloc((size_t)L));
+    CU_TRY(ctx, d_ld.alloc((size_t)(2 * L)));
+    CU_TRY(ctx, d_ll.alloc((size_t)(2 * L)));
+  }
+  int64_t cap = 1;
+  while (cap < max_pool) cap <<= 1;
+  const int64_t grid = std::min<int64_t>(q, wave);
+  DevBuf<int64_t> w64;
+  DevBuf<int32_t> w32;
+  DevBuf<double> wd;
+  CU_TRY(ctx, w64.alloc((size_t)(2 * cap * grid)));
+  CU_TRY(ctx, w32.alloc((size_t)(4 * cap * grid)));
+  CU_TRY(ctx, wd.alloc((size_t)(2 * cap * grid)));
+  const cfmm::SubgraphWork W{w64.p, w64.p + cap * grid, w32.p, w32.p + cap * grid, w32.p + 2 * cap * grid,
+                             wd.p, wd.p + cap * grid, cap};
+  cfmm::SubgraphRows R{d_in.p,     d_out.p,   d_amount.p, d_limit.p,  o.max_iter, o.max_fun, o.rtol,
+                       o.factr,    d_tok_off.p, d_leg_off.p, d_paid.p, d_recv.p,   d_status.p, d_sst.p,
+                       d_iter.p,   d_fev.p,   d_merit.p,  d_token.p,  d_nu.p,     d_psi.p,   d_entry.p,
+                       d_ld.p,     d_ll.p};
+  OrderSets xs;
+  if (!exec) {
+    if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+           cfmm::subgraph_kernel<false><<<(unsigned)grid, cfmm::kSubgraphThreads, 0, st>>>(
+               os.d_P.p, pv, A, G, d_act.p, R, W, cfmm::SplitMoved{}, nullptr, q);
+         })) != CFMM_OK)
+      return rc;
+  } else {
+    if ((rc = order_sets(ctx, true, xs)) != CFMM_OK) return rc;
+    ctx->state_version++;
+    // levels over the tokens of {j, i} ∪ B (one table of n_tokens entries)
+    int64_t size = ctx->n_tokens, uses = q * (2 + (int64_t)nB);
+    std::vector<int64_t> order, level_off;
+    conflict_levels(
+        q, 1, &size, &uses,
+        [&](int64_t r, auto&& visit) {
+          visit(0, token_in[r] - 1);
+          visit(0, token_out[r] - 1);
+          for (int32_t t : tok)
+            if (t != token_in[r] - 1 && t != token_out[r] - 1) visit(0, t);
+        },
+        order, level_off);
+    DevBuf<int64_t> d_order;
+    CU_TRY(ctx, d_order.upload(order));
+    for (size_t Lv = 1; Lv < level_off.size(); ++Lv) {
+      const int64_t n = level_off[Lv] - level_off[Lv - 1];
+      if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+             cfmm::subgraph_kernel<true><<<(unsigned)std::min<int64_t>(n, grid), cfmm::kSubgraphThreads, 0, st>>>(
+                 xs.d_P.p, pv, A, G, d_act.p, R, W, xs.mv, d_order.p + level_off[Lv - 1], n);
+           })) != CFMM_OK)
+        return rc;
+    }
+    if ((rc = order_bookkeeping(ctx, xs)) != CFMM_OK) return rc;
+  }
+  CU_TRY(ctx, read_back(ctx, O.paid, d_paid.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, O.received, d_recv.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, O.status, d_status.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, O.solver_status, d_sst.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, O.iterations, d_iter.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, O.fun_evals, d_fev.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, O.merit, d_merit.p, (size_t)q));
+  std::vector<int64_t> ent(legs && (O.leg_type || O.leg_pool) ? (size_t)L : 0);
+  if (toks) {
+    CU_TRY(ctx, read_back(ctx, O.token, d_token.p, (size_t)NT));
+    CU_TRY(ctx, read_back(ctx, O.nu, d_nu.p, (size_t)NT));
+    CU_TRY(ctx, read_back(ctx, O.psi, d_psi.p, (size_t)NT));
+  }
+  if (legs) {
+    CU_TRY(ctx, read_back(ctx, ent.empty() ? nullptr : ent.data(), d_entry.p, (size_t)L));
+    CU_TRY(ctx, read_back(ctx, O.leg_delta, d_ld.p, (size_t)(2 * L)));
+    CU_TRY(ctx, read_back(ctx, O.leg_lambda, d_ll.p, (size_t)(2 * L)));
+  }
+  CU_TRY(ctx, cudaStreamSynchronize(st));
+  for (size_t t = 0; t < ent.size(); ++t) {  // (set, device position) -> (type, index in the type's order)
+    const int k = (int)(ent[t] >> cfmm::kPairSetShift);
+    const int64_t p = ent[t] & cfmm::kPairPosMask;
+    if (O.leg_type) O.leg_type[t] = k >> 1;
+    if (O.leg_pool) O.leg_pool[t] = path_set(ctx, k).order[(size_t)p] + ((k & 1) ? ctx->sets[k >> 1].m : 0);
+  }
+  return CFMM_OK;
+}
+
+cfmm_subgraph_opts subgraph_opts(const cfmm_subgraph_opts* in) {
+  if (in) return *in;
+  cfmm_subgraph_opts o;
+  o.max_iter = 1000;
+  o.max_fun = 4000;
+  o.rtol = 1e-4;
+  o.factr = 0.0;
+  return o;
+}
+
+}  // namespace
+
+int cfmm_quote_subgraph_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                               const double* amount, const uint8_t* allowed, const cfmm_subgraph_opts* opts,
+                               cfmm_subgraph_out* out) {
+  const cfmm_subgraph_opts o = subgraph_opts(opts);
+  int rc = check_subgraph(ctx, q, token_in, token_out, amount, nullptr, allowed, o, "quote_subgraph_orders");
+  if (rc != CFMM_OK) return rc;
+  if (q == 0) {
+    if (out && out->tok_off) out->tok_off[0] = 0;
+    if (out && out->leg_off) out->leg_off[0] = 0;
+    return CFMM_OK;
+  }
+  return subgraph_orders(ctx, false, q, token_in, token_out, amount, nullptr, allowed, o, out);
+}
+
+int cfmm_execute_subgraph_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                                 const double* amount, const double* limit, const uint8_t* allowed,
+                                 const cfmm_subgraph_opts* opts, cfmm_subgraph_out* out) {
+  const cfmm_subgraph_opts o = subgraph_opts(opts);
+  int rc = check_subgraph(ctx, q, token_in, token_out, amount, limit, allowed, o, "execute_subgraph_orders");
+  if (rc != CFMM_OK) return rc;
+  if (q == 0) {
+    if (out && out->tok_off) out->tok_off[0] = 0;
+    if (out && out->leg_off) out->leg_off[0] = 0;
+    return CFMM_OK;
+  }
+  return subgraph_orders(ctx, true, q, token_in, token_out, amount, limit, allowed, o, out);
 }
 
 // ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------

@@ -1,0 +1,644 @@
+// subgraph_kernels.cuh -- orders routed over every pool among their allowed tokens: one dual solve
+// per row (sm_90a; cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders, include/cfmm_b200.h).
+// Off the sweep path: no sweep kernel reads anything these kernels add.
+//
+// The call's allowed tokens are best_path_kernels.cuh's slots (BestPathGraph, built once per call by
+// best_path_graph_kernel); subgraph_act_kernel adds, per slot neighbour, whether the pair holds an
+// active pool.  One CTA solves one row at a time (a persistent grid strides over the rows):
+//   setup   the pairs {j, b}, {i, b} and {j, i}, the component T of i over active pools, the local
+//           tokens (0 = i, 1 = j, then T's slots ascending) and the row's pools: every pool of every
+//           pair inside T, bitonic-sorted into global insertion order in the CTA's workspace, with a
+//           per-token incidence list in that order;
+//   solve   cfmm_solve's projected L-BFGS (solver_control.cuh) with every vector in shared memory;
+//           an evaluation writes each pool's contributions to the workspace (split_legs at ν taken at
+//           the pool's stored tokens), then sums them per token in a fixed warp tree;
+//   legs    split_leg over the pools at the final ν: the legs and, on execute, the transition.
+// subgraph_plan_kernel runs the setup only and reports each row's token and pool counts, which size
+// the outputs and the workspace.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "best_path_kernels.cuh"
+#include "solver_control.cuh"
+
+namespace cfmm {
+
+constexpr int kSubgraphMaxTokens = 256;                  // CFMM_SUBGRAPH_MAX_TOKENS
+constexpr int kSubgraphSlots = kSubgraphMaxTokens + 2;  // a call's slots: a row's B plus its j and i
+constexpr int kSubgraphLocal = kSubgraphMaxTokens + 2;  // a row's tokens: i, j and B ∩ T
+constexpr int kSubgraphThreads = 256;
+constexpr int kSubgraphWarps = kSubgraphThreads / 32;
+constexpr double kSubgraphSqrtEps = 1.4901161193847656e-08;  // sqrt(eps), the box of Swap (objectives.jl)
+
+// Per slot neighbour m of slot s (BestPathGraph layout): 1 when the pair holds an active pool.
+__device__ __forceinline__ bool subgraph_pair_active(const PathSets* P, PairIndexView ix, int64_t k) {
+  for (int64_t e = ix.off[k]; e < ix.off[k + 1]; ++e) {
+    const int64_t entry = ix.pool[e];
+    const int set = (int)(entry >> kPairSetShift);
+    const uint8_t* a = P->s[set].active;
+    if (!a || a[entry & kPairPosMask]) return true;
+  }
+  return false;
+}
+
+__global__ void subgraph_act_kernel(const PathSets* __restrict__ P, PairIndexView ix, BestPathGraph G,
+                                    uint8_t* __restrict__ act) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (int64_t)G.nB * G.nB) return;
+  const int s = (int)(t / G.nB), m = (int)(t % G.nB);
+  if (m < G.deg[s]) act[t] = subgraph_pair_active(P, ix, G.pair[t]) ? 1 : 0;
+}
+
+// The rows of one call, their options, and their outputs (device arrays; tokens 1-based).
+struct SubgraphRows {
+  const int64_t* token_in;
+  const int64_t* token_out;
+  const double* amount;
+  const double* limit;  // null: none
+  int max_iter, max_fun;
+  double rtol, factr;
+  const int64_t* tok_off;  // [q+1] (setup counts, scanned)
+  const int64_t* leg_off;  // [q+1]
+  double* paid;
+  double* received;
+  uint8_t* status;
+  int32_t* solver_status;
+  int32_t* iterations;
+  int32_t* fun_evals;
+  double* merit;
+  int64_t* token;  // [tok_off[q]] or null (with nu, psi)
+  double* nu;
+  double* psi;
+  int64_t* leg_entry;  // [leg_off[q]] or null: (set << 56) | device position
+  double* leg_delta;   // [2L] or null (with leg_lambda)
+  double* leg_lambda;
+};
+
+// The CTA's workspace: cap (a power of two) pools.
+struct SubgraphWork {
+  int64_t* ent;
+  int64_t* key;
+  int32_t* ta;  // local token of the pool's stored token 1
+  int32_t* tb;
+  int32_t* inc;  // [2·cap] incidence: 2·pool + side
+  double* ca;    // Λ₁ − Δ₁ (stored order)
+  double* cb;
+  int64_t cap;
+};
+
+// Shared state of one row.
+struct SubgraphSmem {
+  int32_t jpair[kSubgraphSlots], ipair[kSubgraphSlots], cnt[kSubgraphSlots + 1];
+  int16_t lidx[kSubgraphSlots];
+  uint8_t jact[kSubgraphSlots], iact[kSubgraphSlots], in[kSubgraphSlots];
+  int32_t ltok[kSubgraphLocal];
+  int32_t inc_off[kSubgraphLocal + 1];
+  double x[kSubgraphLocal], g[kSubgraphLocal], xt[kSubgraphLocal], gt[kSubgraphLocal], d[kSubgraphLocal],
+      pg[kSubgraphLocal], px[kSubgraphLocal], pt[kSubgraphLocal];
+  double S[kSolverM][kSubgraphLocal], Y[kSolverM][kSubgraphLocal];
+  double W[kSolverK][kSolverK];
+  double c[kSolverK];
+  double red[kSubgraphWarps];
+  unsigned long long mx;
+  int32_t direct, n_loc, jin, npool, direct_cnt;
+  int32_t jslot, islot;
+  int changed;
+};
+
+__device__ __forceinline__ bool sg_slot_ok(const SubgraphSmem& m, int s) { return s != m.jslot && s != m.islot; }
+
+// The pair {t, tok[s]} for every slot s, from t's adjacency list: walked when short, else bisected.
+__device__ __forceinline__ void sg_side_pairs(AdjView A, const BestPathGraph& G, int32_t t, int32_t* dst) {
+  const int64_t a0 = A.off[t], a1 = A.off[t + 1];
+  if (a1 - a0 <= (int64_t)G.nB) {
+    for (int64_t e = a0 + threadIdx.x; e < a1; e += blockDim.x) {
+      const int32_t u = G.slot_of[A.nbr[e]];
+      if (u >= 0) dst[u] = A.pair[e];
+    }
+  } else {
+    for (int s = threadIdx.x; s < G.nB; s += blockDim.x) {
+      const int32_t b = G.tok[s];
+      int64_t lo = a0, hi = a1;
+      while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (A.nbr[mid] < b)
+          lo = mid + 1;
+        else
+          hi = mid;
+      }
+      if (lo < a1 && A.nbr[lo] == b) dst[s] = A.pair[lo];
+    }
+  }
+}
+
+// Setup of row (j, i), 0-based: T, the local tokens and the pool count of every slot (cnt[s], the
+// pools of the pairs {s, i}, {s, j} when j ∈ T, and {s, u} for slots u > s in T) and of {j, i}.
+__device__ void sg_setup(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
+                         const uint8_t* __restrict__ gact, int32_t j, int32_t i, SubgraphSmem& m) {
+  const int tid = threadIdx.x, nB = G.nB;
+  for (int s = tid; s < nB; s += blockDim.x) {
+    m.jpair[s] = m.ipair[s] = -1;
+    m.in[s] = 0;
+    m.lidx[s] = -1;
+  }
+  if (tid == 0) {
+    m.jslot = G.slot_of[j];
+    m.islot = G.slot_of[i];
+    int64_t lo = A.off[j], hi = A.off[j + 1];
+    const int64_t a1 = hi;
+    while (lo < hi) {
+      const int64_t mid = (lo + hi) >> 1;
+      if (A.nbr[mid] < i)
+        lo = mid + 1;
+      else
+        hi = mid;
+    }
+    m.direct = lo < a1 && A.nbr[lo] == i ? A.pair[lo] : -1;
+    m.jin = m.direct >= 0 && subgraph_pair_active(P, ix, m.direct);
+  }
+  __syncthreads();
+  sg_side_pairs(A, G, j, m.jpair);
+  sg_side_pairs(A, G, i, m.ipair);
+  __syncthreads();
+  for (int s = tid; s < nB; s += blockDim.x) {
+    const bool ok = sg_slot_ok(m, s);
+    m.jact[s] = ok && m.jpair[s] >= 0 && subgraph_pair_active(P, ix, m.jpair[s]);
+    m.iact[s] = ok && m.ipair[s] >= 0 && subgraph_pair_active(P, ix, m.ipair[s]);
+    m.in[s] = m.iact[s];
+  }
+  __syncthreads();
+  // the component of i: grow T until no slot joins (every write sets a flag to 1, so the fixed point
+  // does not depend on the order)
+  while (true) {
+    int changed = 0;
+    for (int s = tid; s < nB; s += blockDim.x) {
+      if (m.in[s] || !sg_slot_ok(m, s)) continue;
+      bool join = m.jin && m.jact[s];
+      const int dg = G.deg[s];
+      for (int e = 0; e < dg && !join; ++e) {
+        const int u = G.nbr[(int64_t)nB * s + e];
+        join = m.in[u] && gact[(int64_t)nB * s + e];
+      }
+      if (join) {
+        m.in[s] = 1;
+        changed = 1;
+      }
+    }
+    if (!m.jin) {
+      for (int s = tid; s < nB; s += blockDim.x)
+        if (m.in[s] && m.jact[s]) {
+          m.jin = 1;  // every writer writes 1
+          changed = 1;
+        }
+    }
+    if (!__syncthreads_or(changed)) break;
+  }
+  // local tokens and pool counts
+  for (int s = tid; s < nB; s += blockDim.x) {
+    int32_t c = 0;
+    if (m.in[s]) {
+      const auto pools = [&](int32_t k) { return k >= 0 ? (int32_t)(ix.off[k + 1] - ix.off[k]) : 0; };
+      c = pools(m.ipair[s]) + (m.jin ? pools(m.jpair[s]) : 0);
+      const int dg = G.deg[s];
+      for (int e = 0; e < dg; ++e) {
+        const int u = G.nbr[(int64_t)nB * s + e];
+        if (u > s && m.in[u]) c += pools(G.pair[(int64_t)nB * s + e]);
+      }
+    }
+    m.cnt[s] = c;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    int loc = 2;
+    m.ltok[0] = i;
+    m.ltok[1] = j;
+    for (int s = 0; s < nB; ++s)
+      if (m.in[s]) {
+        m.lidx[s] = (int16_t)loc;
+        m.ltok[loc++] = G.tok[s];
+      }
+    m.n_loc = loc;
+    m.direct_cnt = m.jin && m.direct >= 0 ? (int32_t)(ix.off[m.direct + 1] - ix.off[m.direct]) : 0;
+    int32_t tot = m.direct_cnt;
+    for (int s = 0; s < nB; ++s) {
+      const int32_t c = m.cnt[s];
+      m.cnt[s] = tot;  // exclusive offsets after {j, i}'s pools
+      tot += c;
+    }
+    m.cnt[nB] = tot;
+    m.npool = tot;
+  }
+  __syncthreads();
+}
+
+__device__ __forceinline__ int32_t sg_local(const BestPathGraph& G, const SubgraphSmem& m, int32_t t) {
+  if (t == m.ltok[0]) return 0;
+  if (t == m.ltok[1]) return 1;
+  return m.lidx[G.slot_of[t]];
+}
+
+// Per row: the number of tokens the row lists (T, j omitted when it is not in T) and of its pools.
+__global__ void __launch_bounds__(kSubgraphThreads)
+    subgraph_plan_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, BestPathGraph G,
+                         const uint8_t* __restrict__ gact, const int64_t* __restrict__ token_in,
+                         const int64_t* __restrict__ token_out, int64_t q, int64_t* __restrict__ ntok,
+                         int64_t* __restrict__ npool) {
+  __shared__ SubgraphSmem m;
+  for (int64_t r = blockIdx.x; r < q; r += gridDim.x) {
+    sg_setup(P, ix, A, G, gact, (int32_t)(token_in[r] - 1), (int32_t)(token_out[r] - 1), m);
+    if (threadIdx.x == 0) {
+      ntok[r] = m.n_loc - (m.jin ? 0 : 1);
+      npool[r] = m.npool;
+    }
+    __syncthreads();
+  }
+}
+
+// Sum over the CTA of one value per thread, in a fixed order: the xor butterfly 16 … 1 in each warp,
+// then the warps' sums in warp order from +0.0.  Every thread gets the result.
+__device__ __forceinline__ double sg_cta_sum(double v, SubgraphSmem& m) {
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) v = __dadd_rn(v, __shfl_xor_sync(kFull, v, o));
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) m.red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double t = 0.0;
+#pragma unroll
+  for (int w = 0; w < kSubgraphWarps; ++w) t = __dadd_rn(t, m.red[w]);
+  return t;
+}
+
+// The pool view of workspace pool e at ν = v (local prices).
+__device__ __forceinline__ SplitPool sg_pool(const PathSets* P, const SubgraphWork& w, int64_t e, const double* v) {
+  SplitPool sp = split_pool(P, w.ent[e], -1, 1.0);
+  sp.v1 = v[w.ta[e]];
+  sp.v2 = v[w.tb[e]];
+  return sp;
+}
+
+// One evaluation at ν = xt: every pool's contributions, Ψ_t -> pt, gt = lin + Ψ, and the dual's
+// value linᵀxt + Σ val (returned to every thread).
+__device__ double sg_evaluate(const PathSets* P, const SubgraphWork& w, SubgraphSmem& m, double amt) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int64_t np = m.npool;
+  double vs = 0.0;
+  for (int64_t e = tid; e < np; e += blockDim.x) {
+    const SplitPool sp = sg_pool(P, w, e, m.xt);
+    const Trade tr = split_legs(P, sp);
+    const double a = __dsub_rn(tr.l1, tr.d1), b = __dsub_rn(tr.l2, tr.d2);
+    w.ca[e] = a;
+    w.cb[e] = b;
+    vs = __dadd_rn(vs, __dadd_rn(__dmul_rn(sp.v1, a), __dmul_rn(sp.v2, b)));
+  }
+  const double V = sg_cta_sum(vs, m);  // (its syncs also publish ca, cb)
+  for (int t = warp; t < m.n_loc; t += kSubgraphWarps) {
+    double s = 0.0;
+    for (int k = m.inc_off[t] + lane; k < m.inc_off[t + 1]; k += 32) {
+      const int32_t v = w.inc[k];
+      s = __dadd_rn(s, (v & 1) ? w.cb[v >> 1] : w.ca[v >> 1]);
+    }
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) s = __dadd_rn(s, __shfl_xor_sync(kFull, s, o));
+    if (lane == 0) {
+      m.pt[t] = s;
+      m.gt[t] = __dadd_rn(t == 1 ? amt : 0.0, s);
+    }
+  }
+  __syncthreads();
+  return __dadd_rn(__dmul_rn(amt, m.xt[1]), V);
+}
+
+__device__ __forceinline__ double sg_lower(int t) { return t == 0 ? 1.0 + kSubgraphSqrtEps : kSubgraphSqrtEps; }
+
+// Accept xt: (s, y) into history slot `slot` when store, x <- xt, g <- gt, Ψ, the projected gradient
+// and the Gram matrix of [S Y pg] (one warp per entry group, lanes over the tokens, butterfly).
+// Returns m_r = max_t ν_t·|pg_t| / (δ·ν_j).
+__device__ double sg_commit(SubgraphSmem& m, int slot, bool store, double amt) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = m.n_loc;
+  if (tid == 0) m.mx = 0ull;
+  for (int t = tid; t < n; t += blockDim.x) {
+    const double xn = m.xt[t], gn = m.gt[t];
+    if (store) {
+      m.S[slot][t] = __dsub_rn(xn, m.x[t]);
+      m.Y[slot][t] = __dsub_rn(gn, m.g[t]);
+    }
+    m.x[t] = xn;
+    m.g[t] = gn;
+    m.px[t] = m.pt[t];
+    m.pg[t] = xn <= sg_lower(t) && gn > 0.0 ? 0.0 : gn;
+  }
+  __syncthreads();
+  double mx = 0.0;
+  for (int t = tid; t < n; t += blockDim.x) mx = fmax(mx, __dmul_rn(m.x[t], fabs(m.pg[t])));
+  for (int o = 16; o >= 1; o >>= 1) mx = fmax(mx, __shfl_xor_sync(kFull, mx, o));
+  if (lane == 0) atomicMax(&m.mx, (unsigned long long)__double_as_longlong(mx));  // order-free max
+  const auto col = [&](int c, int t) {
+    return c < kSolverM ? m.S[c][t] : c < 2 * kSolverM ? m.Y[c - kSolverM][t] : m.pg[t];
+  };
+  for (int k = warp; k < kSolverK * kSolverK; k += kSubgraphWarps) {
+    const int r = k / kSolverK, c = k % kSolverK;
+    if (c < r) continue;
+    double s = 0.0;
+    for (int t = lane; t < n; t += 32) s = fma(col(r, t), col(c, t), s);
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) s = __dadd_rn(s, __shfl_xor_sync(kFull, s, o));
+    if (lane == 0) m.W[r][c] = m.W[c][r] = s;
+  }
+  __syncthreads();
+  return __ddiv_rn(__longlong_as_double((long long)m.mx), __dmul_rn(amt, m.x[1]));
+}
+
+// The start ν⁰: ν_i = 1; then breadth-first rounds over the active pools: a token not yet priced
+// gets the largest r(a → b)·ν_b over its pools to tokens priced in earlier rounds, r the no-trade
+// boundary with a in j's role (the arbitrage scan's rate).  A token is priced once, so gaining
+// cycles cannot inflate the start.  Then clamped to the box.  Into xt.
+__device__ void sg_start(const PathSets* P, const SubgraphWork& w, SubgraphSmem& m) {
+  const int tid = threadIdx.x, n = m.n_loc;
+  for (int t = tid; t < n; t += blockDim.x) m.x[t] = m.xt[t] = t == 0 ? 1.0 : 0.0;
+  __syncthreads();
+  unsigned long long* nxt = reinterpret_cast<unsigned long long*>(m.xt);
+  for (int round = 1; round < n; ++round) {
+    int changed = 0;
+    for (int64_t e = tid; e < m.npool; e += blockDim.x) {
+      SplitPool sp = split_pool(P, w.ent[e], -1, 1.0);
+      if (!sp.active) continue;
+      for (int side = 0; side < 2; ++side) {
+        const int32_t a = side ? w.tb[e] : w.ta[e], b = side ? w.ta[e] : w.tb[e];
+        if (m.x[a] != 0.0 || !(m.x[b] > 0.0)) continue;  // a is priced once, from tokens priced before
+        sp.x_is_j = side == 0;
+        const double c = __dmul_rn(split_boundary(P, sp), m.x[b]);
+        if (c > 0.0 && c < kPathInf) {
+          atomicMax(nxt + a, (unsigned long long)__double_as_longlong(c));  // order-free max
+          changed = 1;
+        }
+      }
+    }
+    const bool more = __syncthreads_or(changed);
+    for (int t = tid; t < n; t += blockDim.x) m.x[t] = m.xt[t];
+    __syncthreads();
+    if (!more) break;
+  }
+  for (int t = tid; t < n; t += blockDim.x) m.xt[t] = fmax(m.x[t], sg_lower(t));
+  __syncthreads();
+}
+
+// Row r on the current state.  Returns nothing; writes the row's outputs.  EXEC: the limit decides,
+// and a filled row applies the transition of cfmm_apply_trades at its ν to each of its pools.
+template <bool EXEC>
+__device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
+                             const uint8_t* gact, const SubgraphRows& R, const SubgraphWork& w, const SplitMoved& mv,
+                             int64_t r, SubgraphSmem& m) {
+  __shared__ LbfgsHistory hist;
+  __shared__ double s_f, s_t, s_merit;
+  __shared__ int s_state, s_status, s_iter, s_fev, s_small;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int32_t j = (int32_t)(R.token_in[r] - 1), i = (int32_t)(R.token_out[r] - 1);
+  const double amt = R.amount[r];
+  sg_setup(P, ix, A, G, gact, j, i, m);
+  const int64_t np = m.npool, n = m.n_loc;
+  // the pools: {j, i} first, then each slot's, at the offsets the setup counted
+  if (tid == 0 && m.direct_cnt > 0) {
+    for (int64_t e = ix.off[m.direct]; e < ix.off[m.direct + 1]; ++e) w.ent[e - ix.off[m.direct]] = ix.pool[e];
+  }
+  for (int s = tid; s < G.nB; s += blockDim.x) {
+    if (!m.in[s]) continue;
+    int64_t o = m.cnt[s];
+    const auto put = [&](int64_t k) {
+      if (k < 0) return;
+      for (int64_t e = ix.off[k]; e < ix.off[k + 1]; ++e) w.ent[o++] = ix.pool[e];
+    };
+    put(m.ipair[s]);
+    if (m.jin) put(m.jpair[s]);
+    const int dg = G.deg[s];
+    for (int e = 0; e < dg; ++e) {
+      const int u = G.nbr[(int64_t)G.nB * s + e];
+      if (u > s && m.in[u]) put(G.pair[(int64_t)G.nB * s + e]);
+    }
+  }
+  __syncthreads();
+  // global insertion order: a bitonic sort on (global index, entry), padded to a power of two
+  int64_t p2 = 1;
+  while (p2 < np) p2 <<= 1;
+  for (int64_t e = tid; e < p2; e += blockDim.x) {
+    if (e < np) {
+      const int64_t en = w.ent[e];
+      const int k = (int)(en >> kPairSetShift);
+      w.key[e] = P->s[k].gidx[en & kPairPosMask] & ~(1ll << 62);
+    } else {
+      w.key[e] = INT64_MAX;
+      w.ent[e] = -1;
+    }
+  }
+  __syncthreads();
+  for (int64_t k = 2; k <= p2; k <<= 1)
+    for (int64_t jj = k >> 1; jj > 0; jj >>= 1) {
+      for (int64_t e = tid; e < p2; e += blockDim.x) {
+        const int64_t o = e ^ jj;
+        if (o > e) {
+          const bool up = (e & k) == 0;
+          const int64_t ke = w.key[e], ko = w.key[o];
+          if (up ? ke > ko : ke < ko) {
+            w.key[e] = ko;
+            w.key[o] = ke;
+            const int64_t t = w.ent[e];
+            w.ent[e] = w.ent[o];
+            w.ent[o] = t;
+          }
+        }
+      }
+      __syncthreads();
+    }
+  for (int64_t e = tid; e < np; e += blockDim.x) {
+    const int64_t en = w.ent[e];
+    const int k = (int)(en >> kPairSetShift);
+    const int2 a = P->Ai[k][en & kPairPosMask];
+    w.ta[e] = sg_local(G, m, a.x);
+    w.tb[e] = sg_local(G, m, a.y);
+  }
+  __syncthreads();
+  // incidence lists in pool order: one warp per token, a ballot per 32 pools (count, then fill)
+  for (int t = warp; t < n; t += kSubgraphWarps) {
+    int c = 0;
+    for (int64_t b = 0; b < np; b += 32) {
+      const int64_t e = b + lane;
+      c += __popc(__ballot_sync(kFull, e < np && (w.ta[e] == t || w.tb[e] == t)));
+    }
+    if (lane == 0) m.inc_off[t + 1] = c;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    m.inc_off[0] = 0;
+    for (int t = 0; t < n; ++t) m.inc_off[t + 1] += m.inc_off[t];
+  }
+  __syncthreads();
+  for (int t = warp; t < n; t += kSubgraphWarps) {
+    int c = m.inc_off[t];
+    for (int64_t b = 0; b < np; b += 32) {
+      const int64_t e = b + lane;
+      const bool ha = e < np && w.ta[e] == t, hb = e < np && w.tb[e] == t;
+      const unsigned hit = __ballot_sync(kFull, ha || hb);
+      if (ha || hb) w.inc[c + __popc(hit & ((1u << lane) - 1u))] = (int32_t)(2 * e + (hb ? 1 : 0));
+      c += __popc(hit);
+    }
+  }
+  __syncthreads();
+  // the solve
+  const bool solve = m.jin && amt > 0.0;
+  double f = 0.0, merit = 0.0;
+  int status = -1;
+  if (tid == 0) {
+    s_iter = s_fev = s_small = 0;
+    hist.cnt = hist.head = 0;
+  }
+  if (solve) {
+    for (int t = tid; t < n; t += blockDim.x)  // an empty history, as cfmm_solve's zeroed one
+      for (int a = 0; a < kSolverM; ++a) m.S[a][t] = m.Y[a][t] = 0.0;
+    sg_start(P, w, m);
+    f = sg_evaluate(P, w, m, amt);
+    merit = sg_commit(m, 0, false, amt);
+    if (tid == 0) {
+      s_fev = 1;
+      s_f = f;
+      s_merit = merit;
+    }
+    __syncthreads();
+    while (true) {
+      __syncthreads();  // every thread has read the last decision
+      // state: 0 run, 1 stop
+      if (tid == 0) {
+        s_state = 0;
+        if (!(s_f == s_f)) s_status = 5, s_state = 1;
+        else if (s_merit <= R.rtol) s_status = 0, s_state = 1;
+        else if (s_iter >= R.max_iter) s_status = 2, s_state = 1;
+        else if (s_fev >= R.max_fun) s_status = 3, s_state = 1;
+        else s_t = lbfgs_direction(m.W, hist, m.c);
+      }
+      __syncthreads();
+      if (s_state) break;
+      for (int t = tid; t < n; t += blockDim.x) {
+        double v = __dmul_rn(m.c[kSolverK - 1], m.pg[t]);
+#pragma unroll
+        for (int a = 0; a < kSolverM; ++a) {
+          v = fma(m.c[a], m.S[a][t], v);
+          v = fma(m.c[kSolverM + a], m.Y[a][t], v);
+        }
+        m.d[t] = m.x[t] <= sg_lower(t) && m.g[t] > 0.0 ? 0.0 : -v;
+      }
+      __syncthreads();
+      int dec = kLsRetry;
+      double f_new = s_f;
+      for (int ls = 0; ls < 30 && s_fev < R.max_fun; ++ls) {
+        const double t = s_t;
+        double gd = 0.0, st2 = 0.0;
+        for (int k = tid; k < n; k += blockDim.x) {
+          const double y = fmax(fma(t, m.d[k], m.x[k]), sg_lower(k));
+          m.xt[k] = y;
+          const double dx = __dsub_rn(y, m.x[k]);
+          gd = fma(m.g[k], dx, gd);
+          st2 = fma(dx, dx, st2);
+        }
+        const double gdx = sg_cta_sum(gd, m), step2 = sg_cta_sum(st2, m);
+        f_new = sg_evaluate(P, w, m, amt);
+        if (tid == 0) {
+          ++s_fev;
+          double tn = s_t;
+          s_state = lbfgs_trial(s_f, f_new, gdx, step2, hist.cnt, tn);
+          s_t = tn;
+        }
+        __syncthreads();
+        dec = s_state;
+        __syncthreads();
+        if (dec != kLsRetry) break;
+      }
+      if (dec != kLsAccept) {
+        if (tid == 0) {
+          if (hist.cnt > 0 && dec != kLsStall) {
+            hist.cnt = 0;  // drop the history and retry with steepest descent
+            s_state = 0;
+          } else {
+            s_status = dec == kLsStall ? 1 : 4;
+            s_state = 1;
+          }
+        }
+        __syncthreads();
+        if (s_state) break;
+        continue;
+      }
+      const int slot = hist.head;
+      const double mr = sg_commit(m, slot, true, amt);
+      if (tid == 0) {
+        lbfgs_store(m.W, slot, hist);
+        ++s_iter;
+        const double f_old = s_f;
+        s_f = f_new;
+        s_merit = mr;
+        s_state = lbfgs_factr(f_old, f_new, R.factr, s_small) ? 1 : 0;
+        if (s_state) s_status = 1;
+      }
+      __syncthreads();
+      if (s_state) break;
+    }
+    status = s_status;
+    merit = s_merit;
+  }
+  // status, the limit, the legs (and the transition on execute)
+  const double received = solve ? m.px[0] : 0.0, paid = solve ? __dsub_rn(0.0, m.px[1]) : 0.0;
+  uint8_t st = 0;  // CFMM_ORDER_FILLED (amount 0: zeros, no solve)
+  if (amt > 0.0) {
+    if (!m.jin)
+      st = 2;  // CFMM_ORDER_UNREACHABLE
+    else if (status != 0)
+      st = 5;  // CFMM_ORDER_NOT_CONVERGED
+    else if (EXEC && R.limit && received < R.limit[r])
+      st = 1;  // CFMM_ORDER_LIMIT; an equal limit fills
+  }
+  const bool filled = st == 0 && solve;
+  const int64_t l0 = R.leg_off[r];
+  for (int64_t e = tid; e < np; e += blockDim.x) {
+    if (R.leg_entry) R.leg_entry[l0 + e] = w.ent[e];
+    split_leg<EXEC>(P, filled, [&] { return sg_pool(P, w, e, m.x); }, mv, R.leg_delta, R.leg_lambda, l0 + e);
+  }
+  if (R.token) {
+    int64_t o = R.tok_off[r];
+    for (int t = tid; t < n; t += blockDim.x) {
+      if (t == 1 && !m.jin) continue;
+      const int64_t at = o + (t >= 2 && !m.jin ? t - 1 : t);
+      R.token[at] = m.ltok[t] + 1;
+      R.nu[at] = solve ? m.x[t] : 0.0;
+      R.psi[at] = solve ? m.px[t] : 0.0;
+    }
+  }
+  if (tid == 0) {
+    R.paid[r] = filled ? paid : 0.0;
+    R.received[r] = filled ? received : 0.0;
+    R.status[r] = st;
+    R.solver_status[r] = status;
+    R.iterations[r] = solve ? s_iter : 0;
+    R.fun_evals[r] = solve ? s_fev : 0;
+    R.merit[r] = solve ? merit : 0.0;
+  }
+  __syncthreads();  // the next row reuses the shared state and the workspace
+}
+
+// Rows rows[0 .. n) (null: 0 .. n), one CTA at a time each; CTA b uses workspace b.
+template <bool EXEC>
+__global__ void __launch_bounds__(kSubgraphThreads)
+    subgraph_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, BestPathGraph G,
+                    const uint8_t* __restrict__ gact, SubgraphRows R, SubgraphWork w, SplitMoved mv,
+                    const int64_t* __restrict__ rows, int64_t n) {
+  __shared__ SubgraphSmem m;
+  const int64_t c = w.cap * blockIdx.x;
+  SubgraphWork wb = w;
+  wb.ent += c;
+  wb.key += c;
+  wb.ta += c;
+  wb.tb += c;
+  wb.inc += 2 * c;
+  wb.ca += c;
+  wb.cb += c;
+  for (int64_t k = blockIdx.x; k < n; k += gridDim.x)
+    subgraph_row<EXEC>(P, ix, A, G, gact, R, wb, mv, rows ? rows[k] : k, m);
+}
+
+}  // namespace cfmm

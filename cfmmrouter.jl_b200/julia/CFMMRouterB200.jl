@@ -613,6 +613,70 @@ function find_order_paths(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}
     return hop_off, typ[1:n], pool[1:n], tok[1:n], tender[1:n], received[1:n], value, status
 end
 
+# Orders over every pool among allowed tokens (cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders):
+# row r sells amount[r] of token_in[r] for token_out[r] (exact-in) over every pool among the two and the
+# tokens t with allowed[t] != 0 (required, one entry per token, at most 256 besides the row's two),
+# route! with Swap over those pools, one dual solve per row.  opts = nothing: the defaults.  Returns a
+# NamedTuple of the per-row outputs, the token CSR (tok_off, token, nu, psi) and the legs CSR
+# (leg_off, leg_type, leg_pool, leg_delta / leg_lambda as 2 x L).  Never executed, like the rest of
+# this file.
+struct SubgraphOpts
+    max_iter::Cint
+    max_fun::Cint
+    rtol::Float64
+    factr::Float64
+end
+struct SubgraphOut
+    paid::Ptr{Float64}; received::Ptr{Float64}; status::Ptr{UInt8}
+    solver_status::Ptr{Cint}; iterations::Ptr{Cint}; fun_evals::Ptr{Cint}; merit::Ptr{Float64}
+    tok_off::Ptr{Int64}; tok_cap::Int64; token::Ptr{Int64}; nu::Ptr{Float64}; psi::Ptr{Float64}
+    leg_off::Ptr{Int64}; leg_cap::Int64; leg_type::Ptr{Cint}; leg_pool::Ptr{Int64}
+    leg_delta::Ptr{Float64}; leg_lambda::Ptr{Float64}
+end
+function _subgraph_orders(ctx, execute::Bool, token_in::Vector{Int64}, token_out::Vector{Int64},
+                          amount::Vector{Float64}, allowed::Vector{UInt8}, limit, opts)
+    q = length(token_in)
+    length(token_out) == length(amount) == q || throw(ArgumentError("token_in / token_out / amount need q entries"))
+    limit === nothing || length(limit) == q || throw(ArgumentError("limit needs q entries"))
+    o = opts === nothing ? nothing : Ref(opts)
+    tok_off, leg_off = zeros(Int64, q + 1), zeros(Int64, q + 1)
+    sizes = Ref(SubgraphOut(C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, pointer(tok_off), 0, C_NULL,
+                            C_NULL, C_NULL, pointer(leg_off), 0, C_NULL, C_NULL, C_NULL, C_NULL))
+    GC.@preserve tok_off leg_off chk(ctx, ccall((:cfmm_quote_subgraph_orders, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{UInt8}, Ptr{SubgraphOpts}, Ptr{SubgraphOut}),
+        ctx, q, token_in, token_out, amount, allowed, o === nothing ? C_NULL : o, sizes))
+    NT, L = tok_off[end], leg_off[end]
+    paid, received, merit, status = zeros(q), zeros(q), zeros(q), zeros(UInt8, q)
+    sst, iters, fev = zeros(Cint, q), zeros(Cint, q), zeros(Cint, q)
+    token, nu, psi = zeros(Int64, max(NT, 1)), zeros(max(NT, 1)), zeros(max(NT, 1))
+    ltype, lpool, ld, ll = zeros(Cint, max(L, 1)), zeros(Int64, max(L, 1)), zeros(2, max(L, 1)), zeros(2, max(L, 1))
+    GC.@preserve paid received merit status sst iters fev tok_off token nu psi leg_off ltype lpool ld ll begin
+        out = Ref(SubgraphOut(pointer(paid), pointer(received), pointer(status), pointer(sst), pointer(iters),
+                              pointer(fev), pointer(merit), pointer(tok_off), NT, pointer(token), pointer(nu),
+                              pointer(psi), pointer(leg_off), L, pointer(ltype), pointer(lpool), pointer(ld),
+                              pointer(ll)))
+        if execute
+            chk(ctx, ccall((:cfmm_execute_subgraph_orders, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8},
+                 Ptr{SubgraphOpts}, Ptr{SubgraphOut}),
+                ctx, q, token_in, token_out, amount, limit === nothing ? C_NULL : limit, allowed,
+                o === nothing ? C_NULL : o, out))
+        else
+            chk(ctx, ccall((:cfmm_quote_subgraph_orders, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{UInt8}, Ptr{SubgraphOpts},
+                 Ptr{SubgraphOut}),
+                ctx, q, token_in, token_out, amount, allowed, o === nothing ? C_NULL : o, out))
+        end
+    end
+    return (paid=paid, received=received, status=status, solver_status=sst, iterations=iters, fun_evals=fev,
+            merit=merit, tok_off=tok_off, token=token[1:NT], nu=nu[1:NT], psi=psi[1:NT], leg_off=leg_off,
+            leg_type=ltype[1:L], leg_pool=lpool[1:L], leg_delta=ld[:, 1:L], leg_lambda=ll[:, 1:L])
+end
+quote_subgraph_orders(ctx, token_in, token_out, amount, allowed; opts=nothing) =
+    _subgraph_orders(ctx, false, token_in, token_out, amount, allowed, nothing, opts)
+execute_subgraph_orders!(ctx, token_in, token_out, amount, allowed; limit=nothing, opts=nothing) =
+    _subgraph_orders(ctx, true, token_in, token_out, amount, allowed, limit, opts)
+
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
 # current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never

@@ -11,6 +11,7 @@ from __future__ import annotations
 import ctypes as C
 
 import numpy as np
+from types import SimpleNamespace
 
 from . import _lib
 from .cfmms import CFMM, GeometricMeanTwoCoin, ProductTwoCoin, UniV3
@@ -704,6 +705,79 @@ class DevicePools:
         return (hop_off, typ[:n].copy(), pool[:n].copy(), tok[:n].copy(), tender[:n].copy(), received[:n].copy(),
                 value, status)
 
+    # -- orders over every pool among allowed tokens (include/cfmm_b200.h,
+    #    cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders) ----------------------------------
+    def _subgraph(self, execute, token_in, token_out, amount, allowed, limit, opts):
+        tin = np.ascontiguousarray(token_in, dtype=np.int64).reshape(-1)
+        tout = np.ascontiguousarray(token_out, dtype=np.int64).reshape(-1)
+        amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
+        q = len(tin)
+        if not (len(tout) == len(amount) == q):
+            raise ValueError("subgraph orders: token_in, token_out and amount need one entry per row")
+        if allowed is None:
+            raise ValueError("subgraph orders: allowed (a mask over the tokens) is required")
+        mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
+        if len(mask) != self.n_tokens:
+            raise ValueError(f"subgraph orders: allowed must have {self.n_tokens} entries, one per token")
+        if limit is not None:
+            limit = np.ascontiguousarray(limit, dtype=np.float64).reshape(-1)
+            if len(limit) != q:
+                raise ValueError(f"limit must have {q} entries, one per row")
+        o = None
+        if opts is not None:
+            d = {"max_iter": 1000, "max_fun": 4000, "rtol": 1e-4, "factr": 0.0}
+            d.update(opts)
+            o = _lib.SubgraphOpts(int(d["max_iter"]), int(d["max_fun"]), float(d["rtol"]), float(d["factr"]))
+        u8, i32, i64, f64 = C.POINTER(C.c_uint8), C.POINTER(C.c_int), C.POINTER(C.c_int64), C.POINTER(C.c_double)
+        u8m = mask.ctypes.data_as(u8)
+        # sizes: a quote with tok_cap = leg_cap = 0 (the rows' token sets and pool lists do not depend
+        # on the reserves, so an execute's are the same)
+        tok_off, leg_off = np.zeros(q + 1, dtype=np.int64), np.zeros(q + 1, dtype=np.int64)
+        size = _lib.SubgraphOut()
+        size.tok_off, size.leg_off = tok_off.ctypes.data_as(i64), leg_off.ctypes.data_as(i64)
+        self._chk(self._lib.cfmm_quote_subgraph_orders(self._ctx, q, _ip(tin), _ip(tout), _dp(amount), u8m,
+                                                        None if o is None else C.byref(o), C.byref(size)))
+        NT, L = int(tok_off[-1]), int(leg_off[-1])
+        paid, received, merit = np.zeros(q), np.zeros(q), np.zeros(q)
+        status = np.zeros(q, dtype=np.uint8)
+        sst, iters, fev = (np.zeros(q, dtype=np.int32) for _ in range(3))
+        token, nu, psi = np.zeros(max(NT, 1), dtype=np.int64), np.zeros(max(NT, 1)), np.zeros(max(NT, 1))
+        ltype, lpool = np.zeros(max(L, 1), dtype=np.int32), np.zeros(max(L, 1), dtype=np.int64)
+        ld, ll = np.zeros((max(L, 1), 2)), np.zeros((max(L, 1), 2))
+        out = _lib.SubgraphOut(paid.ctypes.data_as(f64), received.ctypes.data_as(f64), status.ctypes.data_as(u8),
+                               sst.ctypes.data_as(i32), iters.ctypes.data_as(i32), fev.ctypes.data_as(i32),
+                               merit.ctypes.data_as(f64), tok_off.ctypes.data_as(i64), NT, token.ctypes.data_as(i64),
+                               nu.ctypes.data_as(f64), psi.ctypes.data_as(f64), leg_off.ctypes.data_as(i64), L,
+                               ltype.ctypes.data_as(i32), lpool.ctypes.data_as(i64), ld.ctypes.data_as(f64),
+                               ll.ctypes.data_as(f64))
+        if execute:
+            self._chk(self._lib.cfmm_execute_subgraph_orders(self._ctx, q, _ip(tin), _ip(tout), _dp(amount),
+                                                              None if limit is None else _dp(limit), u8m,
+                                                              None if o is None else C.byref(o), C.byref(out)))
+        else:
+            self._chk(self._lib.cfmm_quote_subgraph_orders(self._ctx, q, _ip(tin), _ip(tout), _dp(amount), u8m,
+                                                            None if o is None else C.byref(o), C.byref(out)))
+        return SimpleNamespace(paid=paid, received=received, status=status, solver_status=sst, iterations=iters,
+                               fun_evals=fev, merit=merit, tok_off=tok_off, token=token[:NT], nu=nu[:NT],
+                               psi=psi[:NT], leg_off=leg_off, leg_type=ltype[:L], leg_pool=lpool[:L],
+                               leg_delta=ld[:L], leg_lambda=ll[:L])
+
+    def quote_subgraph_orders(self, token_in, token_out, amount, allowed, opts=None):
+        """cfmm_quote_subgraph_orders: row j sells amount[j] of token_in[j] for token_out[j] (1-based,
+        exact-in) over every pool among the two and the tokens t with allowed[t - 1] (at most 256
+        besides the row's two), split optimally: route! with Swap over the row's pools, solved per row
+        on the device.  opts: dict of max_iter, max_fun, rtol, factr (None: the defaults).  No state
+        changes.  Returns a namespace: paid, received, status (uint8), solver_status, iterations,
+        fun_evals, merit [q]; tok_off [q + 1], token, nu, psi [Σ]; leg_off [q + 1], leg_type, leg_pool
+        [L], leg_delta, leg_lambda [L, 2]."""
+        return self._subgraph(False, token_in, token_out, amount, allowed, None, opts)
+
+    def execute_subgraph_orders(self, token_in, token_out, amount, allowed, limit=None, opts=None):
+        """cfmm_execute_subgraph_orders: the rows of quote_subgraph_orders in batch order, each re-solved
+        on the state the earlier filled rows left; limit[j] (None: none) is the minimum received, and a
+        row below it reverts.  Returns what quote_subgraph_orders returns."""
+        return self._subgraph(True, token_in, token_out, amount, allowed, limit, opts)
+
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
         """cfmm_modify_univ3_liquidity: row j adds dL[j] (> 0 mints, < 0 burns) to the ticks of UniV3
@@ -1274,6 +1348,41 @@ class Router:
                                                None if limits is None else limits[rows])
             paid[rows], got[rows], status[rows] = p, g, s
         return paid, got, status, paths
+
+    def _subgraph_args(self, token_in, token_out, amounts, allowed, limits, what):
+        tin, tout, _, amounts, limits = self._split_args(token_in, token_out, np.zeros(len(np.atleast_1d(token_in))),
+                                                         amounts, limits, what)
+        if allowed is None:
+            raise ValueError(f"{what}: allowed (a mask over the tokens) is required")
+        return tin, tout, amounts, limits
+
+    def quote_subgraph_orders(self, token_in, token_out, amounts, allowed, opts=None):
+        """Sell amounts[j] of token_in[j] for token_out[j] (1-based, exact-in) over every pool among the
+        two and the tokens t with allowed[t - 1] (a mask over the tokens, at most 256 such tokens per
+        row besides its two), split optimally: route! with Swap over those pools, one dual solve per
+        row on the device (cfmm_quote_subgraph_orders).  No state changes.  Returns (paid [q],
+        received [q], status [q], detail): detail is DevicePools.quote_subgraph_orders' namespace
+        (solver status, iterations, ν, Ψ, legs).  Single GPU."""
+        tin, tout, amounts, _ = self._subgraph_args(token_in, token_out, amounts, allowed, None,
+                                                    "quote_subgraph_orders")
+        out = self._pools.quote_subgraph_orders(tin, tout, amounts, allowed, opts)
+        return out.paid, out.received, out.status, out
+
+    def execute_subgraph_orders(self, token_in, token_out, amounts, allowed, limits=None, opts=None):
+        """Execute subgraph orders in order (cfmm_execute_subgraph_orders), each re-solved on the state the
+        earlier filled rows left, with an optional minimum received per row: a row below it reverts.
+        Returns what quote_subgraph_orders returns and refreshes the pool objects the filled rows
+        traded with from the device state, as execute_swaps does.  Single GPU."""
+        tin, tout, amounts, limits = self._subgraph_args(token_in, token_out, amounts, allowed, limits,
+                                                         "execute_subgraph_orders")
+        out = self._pools.execute_subgraph_orders(tin, tout, amounts, allowed, limits, opts)
+        filled = np.flatnonzero(out.status == _lib.ORDER_FILLED)
+        if len(filled):
+            sel = np.concatenate([np.arange(out.leg_off[r], out.leg_off[r + 1]) for r in filled]).astype(np.int64)
+            typ, idx = out.leg_type[sel], out.leg_pool[sel]
+            if len(sel):
+                self._refresh_swapped([(t, None, idx[typ == t]) for t in (0, 1, 2) if np.any(typ == t)])
+        return out.paid, out.received, out.status, out
 
     def _arbitrage_args(self, base, other, hubs, min_profit, what):
         if self._world > 1:

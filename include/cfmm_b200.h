@@ -762,6 +762,102 @@ int cfmm_find_order_paths(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [
                           double *hop_received /* [q·max_hops] or NULL */, double *value /* [q] or NULL */,
                           uint8_t *status /* [q] or NULL */);
 
+/* ---- orders routed over every pool among their allowed tokens ------------------------------
+ * A row sells δ = amount[r] of j = token_in[r] for i = token_out[r] (1-based, distinct; exact-in
+ * only) over every pool among j, i and the allowed tokens, split optimally: route! with
+ * Swap(i, j, δ) (src/objectives.jl:106-146) restricted to the row's pools, one convex dual per row.
+ *   B        the tokens t with allowed[t-1] != 0 (allowed [n_tokens], required), minus j and i; at
+ *            most CFMM_SUBGRAPH_MAX_TOKENS per row.  One mask per call.
+ *   T        the tokens of {j, i} ∪ B connected to i through active pools whose two tokens both lie
+ *            in {j, i} ∪ B.  Pools in a component cut off from i would only trade at ν ≈ √eps.
+ *   pools    every pool of every pair inside T: all three types, appended pools included, retired
+ *            pools listed (they trade (0, 0)), in global insertion order (cfmm_num_pools' numbering).
+ *   tokens   local order: i, j, then B ∩ T ascending.  A row with j ∉ T (amount > 0) is
+ *            CFMM_ORDER_UNREACHABLE; it still lists T (without j) and its pools, with zero legs.
+ * Problem.  Minimise g(ν) = δ·ν_j + Σ_k π_k(ν) over the row's pools k on the box ν_i >= 1 + √eps,
+ * ν_t >= √eps otherwise (no upper bound), π_k(ν) = ν_a·(Λ_a − Δ_a) + ν_b·(Λ_b − Δ_b) at the pool's
+ * legs.  A pool's legs at ν are split orders' (find_arb! of the materialising sweep at ν taken at
+ * the pool's stored tokens, split_legs; cfmm_sweep with materialize = 1 gives the same bits).
+ * Sums, in fixed orders with no atomics, so a row's result does not depend on the batch:
+ *   Ψ_t      over the row's pools that hold t, in pool order, split orders' warp tree (partial l adds
+ *            the entries ≡ l (mod 32) from +0.0, then the xor butterfly 16 … 1); each entry is one
+ *            IEEE subtraction Λ_t − Δ_t.  The gradient is (δ at j, 0 elsewhere) + Ψ.
+ *   value    thread l of 256 adds the terms of pools ≡ l (mod 256) from +0.0 (each term
+ *            ν_a·c_a + ν_b·c_b, IEEE), the xor butterfly in each warp, then the 8 warps in order;
+ *            g = δ·ν_j + that sum.
+ * Optimizer: cfmm_solve's projected L-BFGS (m = 5; its two-loop recursion over [S Y pg], Armijo
+ * backtracking with its noise slack, its restart rule and its factr test on two consecutive steps;
+ * the control code is shared), run by one CTA per row with every vector in shared memory.
+ *   start    ν_i = 1; then breadth-first rounds over the active pools: a token not yet priced gets
+ *            the largest r(a → b)·ν_b over its pools to tokens priced in earlier rounds (r:
+ *            cfmm_scan_arbitrage's rate of one pool), and keeps it; then clamped to the box.
+ *   stop     pg = cfmm_solve's clipped projected gradient, m_r = max_t ν_t·|pg_t| / (δ·ν_j), each
+ *            token's imbalance valued at its price relative to the order's value.  Status 0 when
+ *            m_r <= rtol; 1 (relative decrease <= factr·eps twice, or no move), 2 (max_iter),
+ *            3 (max_fun), 4 (line search failed) and 5 (NaN) as cfmm_solve.
+ * What a fill promises.  A row is CFMM_ORDER_FILLED only at solver status 0; otherwise it is
+ * CFMM_ORDER_NOT_CONVERGED, keeps its m_r and solver status, and its legs, paid and received read
+ * 0.  A filled row has received = Ψ_i, paid = −Ψ_j (within rtol·δ of δ when ν_j is off its bound),
+ * every intermediate's net Ψ_b >= −rtol·δ·ν_j/ν_b, and a duality gap of at most |T|·rtol·δ·ν_j plus
+ * the box's √eps terms.  Amount 0 fills with zeros and runs no solve.
+ * Outputs (cfmm_subgraph_out; every pointer may be NULL):
+ *   per row  paid, received, status (CFMM_ORDER_*), solver_status (−1 when no solve ran),
+ *            iterations, fun_evals, merit (m_r; 0 without a solve);
+ *   tokens   tok_off [q+1]; token (1-based), nu, psi [tok_off[q]] in local order, written when
+ *            tok_off[q] <= tok_cap (ν and Ψ at the last iterate, 0 without a solve);
+ *   legs     leg_off [q+1]; leg_type, leg_pool (a pool as cfmm_quote_swaps takes it), leg_delta,
+ *            leg_lambda ([2L], (Δ, Λ) in ingest token order as cfmm_get_trades lays them out) in
+ *            the row's pool order, written when leg_off[q] <= leg_cap; 0 unless filled.
+ *   Ask a quote with tok_cap = leg_cap = 0 for the sizes first, as with cfmm_pair_pools.
+ * cfmm_quote_subgraph_orders prices every row on the current state on its own; no state changes.
+ * cfmm_execute_subgraph_orders runs the rows in batch order, each re-solved on the state the earlier
+ * filled rows left.  limit (NULL: none) is the minimum received; an equal limit fills, a smaller
+ * received reverts with CFMM_ORDER_LIMIT.  A filled row applies split_leg's transition at its ν to
+ * each active pool (two-coin R <- (R + γΔ) − Λ; UniV3 the q′ rule, current tick updated), then the
+ * bookkeeping of cfmm_execute_swaps runs (state version, guard-free flag, fixed-point scale, UniV3
+ * tick records); the materialised trades stay.  Two rows conflict when they share a token of
+ * {j, i} ∪ B; rows are leveled by cfmm_execute_paths' rule, one launch per level.  With one mask per
+ * call, rows with a non-empty B share its tokens and run one after another.  An execute whose token
+ * or leg outputs are given with a cap below the size is rejected before anything changes.
+ * Options (cfmm_subgraph_opts, NULL: max_iter 1000, max_fun 4000, rtol 1e-4, factr 0: the factr test
+ * then stops only after two steps that do not lower g).  The observed floor of m_r on random
+ * markets whose pools disagree on prices is 1e-9 .. 1e-5 per row (see DESIGN §4.5).
+ * Synchronous.  Before cfmm_finalize: CFMM_ERR_STATE.  q == 0 does nothing.  CFMM_ERR_INVALID before
+ * anything runs for: q < 0, a null token_in, token_out or amount; tokens outside 1..n_tokens or
+ * token_in == token_out; an amount that is NaN, Inf or negative; a null allowed; a row whose B holds
+ * more than CFMM_SUBGRAPH_MAX_TOKENS tokens; max_iter or max_fun < 1, rtol not finite and > 0,
+ * factr not finite and >= 0; a limit that is NaN, negative or +inf. */
+#define CFMM_SUBGRAPH_MAX_TOKENS 256
+#define CFMM_ORDER_NOT_CONVERGED 5
+typedef struct {
+  int max_iter, max_fun;
+  double rtol, factr;
+} cfmm_subgraph_opts;
+typedef struct {
+  double *paid, *received;                       /* [q] */
+  uint8_t *status;                               /* [q] */
+  int *solver_status, *iterations, *fun_evals;   /* [q] */
+  double *merit;                                 /* [q] */
+  int64_t *tok_off;                              /* [q+1] */
+  int64_t tok_cap;
+  int64_t *token;                                /* [tok_off[q]] */
+  double *nu, *psi;                              /* [tok_off[q]] */
+  int64_t *leg_off;                              /* [q+1] */
+  int64_t leg_cap;
+  int *leg_type;                                 /* [leg_off[q]] */
+  int64_t *leg_pool;                             /* [leg_off[q]] */
+  double *leg_delta, *leg_lambda;                /* [2·leg_off[q]] */
+} cfmm_subgraph_out;
+int cfmm_quote_subgraph_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [q] */,
+                               const int64_t *token_out /* [q] */, const double *amount /* [q] */,
+                               const uint8_t *allowed /* [n_tokens], required */,
+                               const cfmm_subgraph_opts *opts /* NULL = defaults */,
+                               cfmm_subgraph_out *out);
+int cfmm_execute_subgraph_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_in,
+                                 const int64_t *token_out, const double *amount,
+                                 const double *limit /* [q] or NULL */, const uint8_t *allowed,
+                                 const cfmm_subgraph_opts *opts, cfmm_subgraph_out *out);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
