@@ -40,6 +40,8 @@ PATH_REPEATS_POOL = 4
 # cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders
 SUBGRAPH_MAX_TOKENS = 256
 ORDER_NOT_CONVERGED = 5
+# cfmm_quote_basket_orders / cfmm_execute_basket_orders
+BASKET_MAX_TOKENS = 16
 
 COMM_HANDLE_BYTES = 128
 
@@ -65,6 +67,10 @@ class SubgraphOut(C.Structure):
                 ("leg_off", C.POINTER(C.c_int64)), ("leg_cap", C.c_int64), ("leg_type", C.POINTER(C.c_int)),
                 ("leg_pool", C.POINTER(C.c_int64)), ("leg_delta", C.POINTER(C.c_double)),
                 ("leg_lambda", C.POINTER(C.c_double))]
+
+
+class BasketOut(SubgraphOut):
+    """cfmm_basket_out: cfmm_subgraph_out's fields, with paid per basket entry."""
 
 
 # every symbol include/cfmm_b200.h declares: name -> (restype, argtypes)
@@ -133,6 +139,10 @@ SYMBOLS = {
                                              C.POINTER(SubgraphOpts), C.POINTER(SubgraphOut)]),
     "cfmm_execute_subgraph_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _dp, _dp, C.POINTER(C.c_uint8),
                                                C.POINTER(SubgraphOpts), C.POINTER(SubgraphOut)]),
+    "cfmm_quote_basket_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, _dp, C.POINTER(C.c_uint8),
+                                           C.POINTER(SubgraphOpts), C.POINTER(BasketOut)]),
+    "cfmm_execute_basket_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, _dp, _dp, C.POINTER(C.c_uint8),
+                                             C.POINTER(SubgraphOpts), C.POINTER(BasketOut)]),
     "cfmm_modify_univ3_liquidity":(C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),

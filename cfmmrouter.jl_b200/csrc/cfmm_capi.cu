@@ -35,6 +35,7 @@
 #include "solver.cuh"
 #include "solver_control.cuh"
 #include "subgraph_kernels.cuh"
+#include "basket_kernels.cuh"
 #include "swap_kernels.cuh"
 #include "path_kernels.cuh"
 #include "split_kernels.cuh"
@@ -3919,9 +3920,8 @@ int cfmm_find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, con
 // ---- orders routed over every pool among their allowed tokens (subgraph_kernels.cuh) ------------
 namespace {
 
-// Every argument of cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders, before anything runs.
-int check_subgraph(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const double* amount,
-                   const double* limit, const uint8_t* allowed, const cfmm_subgraph_opts& o, const char* what) {
+// The context, the row count, the mask and the options of a basket or subgraph call.
+int check_row_opts(cfmm_ctx* ctx, int64_t q, const uint8_t* allowed, const cfmm_subgraph_opts& o, const char* what) {
   int rc = ready(ctx);
   if (rc != CFMM_OK) return rc;
   if (q < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: negative row count", what);
@@ -3931,16 +3931,27 @@ int check_subgraph(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int6
   if (!(std::isfinite(o.rtol) && o.rtol > 0.0)) return fail(ctx, CFMM_ERR_INVALID, "%s: rtol %g must be finite and > 0", what, o.rtol);
   if (!(std::isfinite(o.factr) && o.factr >= 0.0))
     return fail(ctx, CFMM_ERR_INVALID, "%s: factr %g must be finite and >= 0", what, o.factr);
-  if (q == 0) return CFMM_OK;
+  return CFMM_OK;
+}
+
+int check_limit(cfmm_ctx* ctx, const double* limit, int64_t r, const char* what) {
+  if (limit && !(std::isfinite(limit[r]) && limit[r] >= 0.0))
+    return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: limit %g must be finite and >= 0", what, (long long)r, limit[r]);
+  return CFMM_OK;
+}
+
+// Every argument of cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders, before anything runs.
+int check_subgraph(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const double* amount,
+                   const double* limit, const uint8_t* allowed, const cfmm_subgraph_opts& o, const char* what) {
+  int rc = check_row_opts(ctx, q, allowed, o, what);
+  if (rc != CFMM_OK || q == 0) return rc;
   if (!token_in || !token_out || !amount) return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
   if ((rc = check_pair_tokens(ctx, q, token_in, token_out, what)) != CFMM_OK) return rc;
   for (int64_t j = 0; j < q; ++j) {
     if (!std::isfinite(amount[j]) || amount[j] < 0.0)
       return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: amount %g must be finite and >= 0", what, (long long)j,
                   amount[j]);
-    if (limit && !(std::isfinite(limit[j]) && limit[j] >= 0.0))
-      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: limit %g must be finite and >= 0", what, (long long)j,
-                  limit[j]);
+    if ((rc = check_limit(ctx, limit, j, what)) != CFMM_OK) return rc;
   }
   int64_t n_allowed = 0;
   for (int64_t t = 0; t < ctx->n_tokens; ++t) n_allowed += allowed[t] != 0;
@@ -3949,6 +3960,50 @@ int check_subgraph(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int6
     if (nb > CFMM_SUBGRAPH_MAX_TOKENS)
       return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: %lld intermediate tokens, more than %d", what, (long long)r,
                   (long long)nb, CFMM_SUBGRAPH_MAX_TOKENS);
+  }
+  return CFMM_OK;
+}
+
+// Every argument of cfmm_quote_basket_orders / cfmm_execute_basket_orders, before anything runs.
+int check_basket(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                 const int64_t* basket_token, const double* basket_amount, const double* limit,
+                 const uint8_t* allowed, const cfmm_subgraph_opts& o, const char* what) {
+  int rc = check_row_opts(ctx, q, allowed, o, what);
+  if (rc != CFMM_OK || q == 0) return rc;
+  if (!token_out || !basket_off || !basket_token || !basket_amount)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
+  if (basket_off[0] != 0) return fail(ctx, CFMM_ERR_INVALID, "%s: basket_off[0] is %lld, not 0", what, (long long)basket_off[0]);
+  int64_t n_allowed = 0;
+  for (int64_t t = 0; t < ctx->n_tokens; ++t) n_allowed += allowed[t] != 0;
+  for (int64_t r = 0; r < q; ++r) {
+    const int64_t b0 = basket_off[r], K = basket_off[r + 1] - b0, i = token_out[r];
+    if (K < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: basket_off decreases", what, (long long)r);
+    if (K < 1 || K > CFMM_BASKET_MAX_TOKENS)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: %lld basket entries, not 1..%d", what, (long long)r,
+                  (long long)K, CFMM_BASKET_MAX_TOKENS);
+    if (i < 1 || i > ctx->n_tokens)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: token_out %lld outside 1..%lld", what, (long long)r,
+                  (long long)i, (long long)ctx->n_tokens);
+    int64_t n_other = n_allowed - (allowed[i - 1] != 0);  // the row's tokens other than i
+    for (int64_t k = b0; k < b0 + K; ++k) {
+      const int64_t t = basket_token[k];
+      const double a = basket_amount[k];
+      if (t < 1 || t > ctx->n_tokens)
+        return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: basket token %lld outside 1..%lld", what, (long long)r,
+                    (long long)t, (long long)ctx->n_tokens);
+      if (t == i) return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: token_out %lld is in the basket", what, (long long)r, (long long)i);
+      for (int64_t l = b0; l < k; ++l)
+        if (basket_token[l] == t)
+          return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: basket token %lld appears twice", what, (long long)r,
+                      (long long)t);
+      if (!std::isfinite(a) || a < 0.0)
+        return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: amount %g must be finite and >= 0", what, (long long)r, a);
+      n_other += allowed[t - 1] == 0;
+    }
+    if (n_other > CFMM_SUBGRAPH_MAX_TOKENS + 1)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: %lld tokens besides token_out, more than %d", what,
+                  (long long)r, (long long)n_other, CFMM_SUBGRAPH_MAX_TOKENS + 1);
+    if ((rc = check_limit(ctx, limit, r, what)) != CFMM_OK) return rc;
   }
   return CFMM_OK;
 }
@@ -4140,6 +4195,202 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
   return CFMM_OK;
 }
 
+int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                  const int64_t* basket_token, const double* basket_amount, const double* limit,
+                  const uint8_t* allowed, const cfmm_subgraph_opts& o, const cfmm_basket_out& O, const char* what) {
+  int rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  if ((rc = ensure_adjacency(ctx)) != CFMM_OK) return rc;
+  auto& ix = ctx->pairs;
+  cudaStream_t st = ctx->stream;
+  // the call's slots: the allowed tokens, ascending; their filtered adjacency and its activity
+  std::vector<int32_t> tok, slot_of((size_t)ctx->n_tokens, -1);
+  for (int64_t t = 0; t < ctx->n_tokens; ++t)
+    if (allowed[t]) {
+      slot_of[(size_t)t] = (int32_t)tok.size();
+      tok.push_back((int32_t)t);
+    }
+  const int nB = (int)tok.size();
+  const size_t nn = (size_t)nB * (size_t)nB;
+  const int64_t NE = basket_off[q];
+  int K = 0;
+  for (int64_t r = 0; r < q; ++r) K = std::max<int>(K, (int)(basket_off[r + 1] - basket_off[r]));
+  const size_t dyn = cfmm::bk_dyn_bytes(K, nB);
+  DevBuf<int64_t> d_out, d_boff, d_btok, d_ntok, d_npool;
+  DevBuf<int32_t> d_tok, d_slot, d_deg, d_gpair;
+  DevBuf<int16_t> d_gnbr;
+  DevBuf<uint8_t> d_act;
+  DevBuf<double> d_bamt, d_limit;
+  CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
+  CU_TRY(ctx, d_boff.upload(basket_off, (size_t)q + 1));
+  CU_TRY(ctx, d_btok.upload(basket_token, (size_t)NE));
+  CU_TRY(ctx, d_bamt.upload(basket_amount, (size_t)NE));
+  CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
+  CU_TRY(ctx, d_tok.upload(tok));
+  CU_TRY(ctx, d_slot.upload(slot_of));
+  CU_TRY(ctx, d_deg.alloc((size_t)nB));
+  CU_TRY(ctx, d_gnbr.alloc(nn));
+  CU_TRY(ctx, d_gpair.alloc(nn));
+  CU_TRY(ctx, d_act.alloc(nn));
+  CU_TRY(ctx, d_ntok.alloc((size_t)q));
+  CU_TRY(ctx, d_npool.alloc((size_t)q));
+  OrderSets os;
+  if ((rc = order_sets(ctx, false, os)) != CFMM_OK) return rc;
+  const cfmm::PairIndexView pv{ix.off.p, ix.pool.p};
+  const cfmm::AdjView A{ix.adj_off.p, ix.adj_nbr.p, ix.adj_pair.p};
+  const cfmm::BestPathGraph G{d_tok.p, d_slot.p, d_deg.p, d_gnbr.p, d_gpair.p, nB};
+  // a persistent grid: one wave of resident CTAs.  The kernels may take the dynamic shared memory of
+  // the longest basket over the most slots, beyond the 48 KB default; the attribute is set once per
+  // context to that one value (so concurrent calls never lower it), and the occupancy taken there.
+  int& occ = ctx->occupancy[reinterpret_cast<const void*>(&cfmm::basket_kernel<false>)];
+  if (occ == 0) {
+    const int most = (int)cfmm::bk_dyn_bytes(cfmm::kBasketMaxTokens, cfmm::kSubgraphSlots);
+    for (const void* f : {reinterpret_cast<const void*>(&cfmm::basket_plan_kernel),
+                          reinterpret_cast<const void*>(&cfmm::basket_kernel<false>),
+                          reinterpret_cast<const void*>(&cfmm::basket_kernel<true>)})
+      CU_TRY(ctx, cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+    CU_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cfmm::basket_kernel<false>,
+                                                              cfmm::kSubgraphThreads, (size_t)most));
+    if (occ < 1) return fail(ctx, CFMM_ERR_CUDA, "basket_kernel does not fit on an SM");
+  }
+  const int64_t wave = (int64_t)ctx->sm_count * occ;
+  const unsigned plan_grid = (unsigned)std::min<int64_t>(q, wave);
+  if ((rc = launch(ctx, kProfSwaps, nB > 0 ? 3 : 1, [&] {
+         if (nB > 0) {
+           cfmm::best_path_graph_kernel<<<(unsigned)((32 * (int64_t)nB + 255) / 256), 256, 0, st>>>(
+               A, d_tok.p, d_slot.p, nB, d_deg.p, d_gnbr.p, d_gpair.p);
+           cfmm::subgraph_act_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>(os.d_P.p, pv, G, d_act.p);
+         }
+         cfmm::basket_plan_kernel<<<plan_grid, cfmm::kSubgraphThreads, dyn, st>>>(
+             os.d_P.p, pv, A, G, d_act.p, d_boff.p, d_btok.p, d_out.p, q, d_ntok.p, d_npool.p);
+       })) != CFMM_OK)
+    return rc;
+  std::vector<int64_t> ntok((size_t)q), npool((size_t)q);
+  CU_TRY(ctx, read_back(ctx, ntok.data(), d_ntok.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, npool.data(), d_npool.p, (size_t)q));
+  CU_TRY(ctx, cudaStreamSynchronize(st));
+  std::vector<int64_t> tok_off((size_t)q + 1, 0), leg_off((size_t)q + 1, 0);
+  int64_t max_pool = 0;
+  for (int64_t r = 0; r < q; ++r) {
+    tok_off[(size_t)r + 1] = tok_off[(size_t)r] + ntok[(size_t)r];
+    leg_off[(size_t)r + 1] = leg_off[(size_t)r] + npool[(size_t)r];
+    max_pool = std::max(max_pool, npool[(size_t)r]);
+  }
+  const int64_t NT = tok_off[(size_t)q], L = leg_off[(size_t)q];
+  if (O.tok_off) std::copy(tok_off.begin(), tok_off.end(), O.tok_off);
+  if (O.leg_off) std::copy(leg_off.begin(), leg_off.end(), O.leg_off);
+  const bool want_tok = O.token || O.nu || O.psi, want_leg = O.leg_type || O.leg_pool || O.leg_delta || O.leg_lambda;
+  if (exec && ((want_tok && NT > O.tok_cap) || (want_leg && L > O.leg_cap)))
+    return fail(ctx, CFMM_ERR_INVALID,
+                "%s: the outputs need %lld token and %lld leg entries, above tok_cap %lld or leg_cap %lld", what,
+                (long long)NT, (long long)L, (long long)O.tok_cap, (long long)O.leg_cap);
+  const bool toks = want_tok && NT > 0 && NT <= O.tok_cap, legs = want_leg && L > 0 && L <= O.leg_cap;
+  // a size query (no per-row output, and no token or leg output that fits) runs no solve
+  if (!exec && !toks && !legs && !O.paid && !O.received && !O.status && !O.solver_status && !O.iterations &&
+      !O.fun_evals && !O.merit)
+    return CFMM_OK;
+  // outputs and the per-CTA workspace
+  DevBuf<int64_t> d_tok_off, d_leg_off, d_token, d_entry;
+  DevBuf<double> d_paid, d_recv, d_merit, d_nu, d_psi, d_ld, d_ll;
+  DevBuf<uint8_t> d_status;
+  DevBuf<int32_t> d_sst, d_iter, d_fev;
+  CU_TRY(ctx, d_tok_off.upload(tok_off));
+  CU_TRY(ctx, d_leg_off.upload(leg_off));
+  CU_TRY(ctx, d_paid.alloc((size_t)NE));
+  CU_TRY(ctx, d_recv.alloc((size_t)q));
+  CU_TRY(ctx, d_merit.alloc((size_t)q));
+  CU_TRY(ctx, d_status.alloc((size_t)q));
+  CU_TRY(ctx, d_sst.alloc((size_t)q));
+  CU_TRY(ctx, d_iter.alloc((size_t)q));
+  CU_TRY(ctx, d_fev.alloc((size_t)q));
+  if (toks) {
+    CU_TRY(ctx, d_token.alloc((size_t)NT));
+    CU_TRY(ctx, d_nu.alloc((size_t)NT));
+    CU_TRY(ctx, d_psi.alloc((size_t)NT));
+  }
+  if (legs) {
+    CU_TRY(ctx, d_entry.alloc((size_t)L));
+    CU_TRY(ctx, d_ld.alloc((size_t)(2 * L)));
+    CU_TRY(ctx, d_ll.alloc((size_t)(2 * L)));
+  }
+  int64_t cap = 1;
+  while (cap < max_pool) cap <<= 1;
+  const int64_t grid = std::min<int64_t>(q, wave);
+  DevBuf<int64_t> w64;
+  DevBuf<int32_t> w32;
+  DevBuf<double> wd;
+  CU_TRY(ctx, w64.alloc((size_t)(2 * cap * grid)));
+  CU_TRY(ctx, w32.alloc((size_t)(4 * cap * grid)));
+  CU_TRY(ctx, wd.alloc((size_t)(2 * cap * grid)));
+  const cfmm::SubgraphWork W{w64.p, w64.p + cap * grid, w32.p, w32.p + cap * grid, w32.p + 2 * cap * grid,
+                             wd.p, wd.p + cap * grid, cap};
+  cfmm::BasketRows R{d_out.p,     d_boff.p,   d_btok.p,   d_bamt.p,  d_limit.p, o.max_iter, o.max_fun,
+                       o.rtol,      o.factr,    d_tok_off.p, d_leg_off.p, d_paid.p, d_recv.p,   d_status.p,
+                       d_sst.p,     d_iter.p,   d_fev.p,    d_merit.p, d_token.p, d_nu.p,     d_psi.p,
+                       d_entry.p,   d_ld.p,     d_ll.p};
+  OrderSets xs;
+  if (!exec) {
+    if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+           cfmm::basket_kernel<false><<<(unsigned)grid, cfmm::kSubgraphThreads, dyn, st>>>(
+               os.d_P.p, pv, A, G, d_act.p, R, W, cfmm::SplitMoved{}, nullptr, q);
+         })) != CFMM_OK)
+      return rc;
+  } else {
+    if ((rc = order_sets(ctx, true, xs)) != CFMM_OK) return rc;
+    ctx->state_version++;
+    // levels over the tokens of {i} ∪ basket ∪ B (one table of n_tokens entries; a token visited
+    // twice changes nothing)
+    int64_t size = ctx->n_tokens, uses = q * (1 + (int64_t)nB) + NE;
+    std::vector<int64_t> order, level_off;
+    conflict_levels(
+        q, 1, &size, &uses,
+        [&](int64_t r, auto&& visit) {
+          visit(0, token_out[r] - 1);
+          for (int64_t k = basket_off[r]; k < basket_off[r + 1]; ++k) visit(0, basket_token[k] - 1);
+          for (int32_t t : tok) visit(0, t);
+        },
+        order, level_off);
+    DevBuf<int64_t> d_order;
+    CU_TRY(ctx, d_order.upload(order));
+    for (size_t Lv = 1; Lv < level_off.size(); ++Lv) {
+      const int64_t n = level_off[Lv] - level_off[Lv - 1];
+      if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+             cfmm::basket_kernel<true><<<(unsigned)std::min<int64_t>(n, grid), cfmm::kSubgraphThreads, dyn, st>>>(
+                 xs.d_P.p, pv, A, G, d_act.p, R, W, xs.mv, d_order.p + level_off[Lv - 1], n);
+           })) != CFMM_OK)
+        return rc;
+    }
+    if ((rc = order_bookkeeping(ctx, xs)) != CFMM_OK) return rc;
+  }
+  CU_TRY(ctx, read_back(ctx, O.paid, d_paid.p, (size_t)NE));
+  CU_TRY(ctx, read_back(ctx, O.received, d_recv.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, O.status, d_status.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, O.solver_status, d_sst.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, O.iterations, d_iter.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, O.fun_evals, d_fev.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, O.merit, d_merit.p, (size_t)q));
+  std::vector<int64_t> ent(legs && (O.leg_type || O.leg_pool) ? (size_t)L : 0);
+  if (toks) {
+    CU_TRY(ctx, read_back(ctx, O.token, d_token.p, (size_t)NT));
+    CU_TRY(ctx, read_back(ctx, O.nu, d_nu.p, (size_t)NT));
+    CU_TRY(ctx, read_back(ctx, O.psi, d_psi.p, (size_t)NT));
+  }
+  if (legs) {
+    CU_TRY(ctx, read_back(ctx, ent.empty() ? nullptr : ent.data(), d_entry.p, (size_t)L));
+    CU_TRY(ctx, read_back(ctx, O.leg_delta, d_ld.p, (size_t)(2 * L)));
+    CU_TRY(ctx, read_back(ctx, O.leg_lambda, d_ll.p, (size_t)(2 * L)));
+  }
+  CU_TRY(ctx, cudaStreamSynchronize(st));
+  for (size_t t = 0; t < ent.size(); ++t) {  // (set, device position) -> (type, index in the type's order)
+    const int k = (int)(ent[t] >> cfmm::kPairSetShift);
+    const int64_t p = ent[t] & cfmm::kPairPosMask;
+    if (O.leg_type) O.leg_type[t] = k >> 1;
+    if (O.leg_pool) O.leg_pool[t] = path_set(ctx, k).order[(size_t)p] + ((k & 1) ? ctx->sets[k >> 1].m : 0);
+  }
+  return CFMM_OK;
+}
+
 cfmm_subgraph_opts subgraph_opts(const cfmm_subgraph_opts* in) {
   if (in) return *in;
   cfmm_subgraph_opts o;
@@ -4148,6 +4399,22 @@ cfmm_subgraph_opts subgraph_opts(const cfmm_subgraph_opts* in) {
   o.rtol = 1e-4;
   o.factr = 0.0;
   return o;
+}
+
+int basket_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                const int64_t* basket_token, const double* basket_amount, const double* limit, const uint8_t* allowed,
+                const cfmm_subgraph_opts* opts, cfmm_basket_out* out, const char* what) {
+  const cfmm_subgraph_opts o = subgraph_opts(opts);
+  int rc = check_basket(ctx, q, token_out, basket_off, basket_token, basket_amount, limit, allowed, o, what);
+  if (rc != CFMM_OK) return rc;
+  if (q == 0) {
+    if (out && out->tok_off) out->tok_off[0] = 0;
+    if (out && out->leg_off) out->leg_off[0] = 0;
+    return CFMM_OK;
+  }
+  const cfmm_basket_out none{};
+  return basket_orders(ctx, exec, q, token_out, basket_off, basket_token, basket_amount, limit, allowed, o,
+                       out ? *out : none, what);
 }
 
 }  // namespace
@@ -4178,6 +4445,20 @@ int cfmm_execute_subgraph_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_
     return CFMM_OK;
   }
   return subgraph_orders(ctx, true, q, token_in, token_out, amount, limit, allowed, o, out);
+}
+
+int cfmm_quote_basket_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                             const int64_t* basket_token, const double* basket_amount, const uint8_t* allowed,
+                             const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
+  return basket_call(ctx, false, q, token_out, basket_off, basket_token, basket_amount, nullptr, allowed, opts, out,
+                     "quote_basket_orders");
+}
+
+int cfmm_execute_basket_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                               const int64_t* basket_token, const double* basket_amount, const double* limit,
+                               const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
+  return basket_call(ctx, true, q, token_out, basket_off, basket_token, basket_amount, limit, allowed, opts, out,
+                     "execute_basket_orders");
 }
 
 // ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------

@@ -677,6 +677,60 @@ quote_subgraph_orders(ctx, token_in, token_out, amount, allowed; opts=nothing) =
 execute_subgraph_orders!(ctx, token_in, token_out, amount, allowed; limit=nothing, opts=nothing) =
     _subgraph_orders(ctx, true, token_in, token_out, amount, allowed, limit, opts)
 
+# Token baskets over every pool among allowed tokens (cfmm_quote_basket_orders /
+# cfmm_execute_basket_orders): row r sells basket_amount[k] of basket_token[k] for k in
+# basket_off[r]+1 .. basket_off[r+1] (1 to 16 distinct tokens, none of them token_out[r]; basket_off is
+# 0-based, q + 1 entries) for token_out[r], route! with BasketLiquidation over those pools.  Returns the
+# NamedTuple of _subgraph_orders with paid per basket entry.  The output struct has SubgraphOut's layout
+# (cfmm_basket_out).  Never executed, like the rest of this file.
+function _basket_orders(ctx, execute::Bool, token_out::Vector{Int64}, basket_off::Vector{Int64},
+                        basket_token::Vector{Int64}, basket_amount::Vector{Float64}, allowed::Vector{UInt8}, limit,
+                        opts)
+    q = length(token_out)
+    length(basket_off) == q + 1 || throw(ArgumentError("basket_off needs q + 1 entries"))
+    NE = basket_off[end]
+    length(basket_token) == length(basket_amount) == NE ||
+        throw(ArgumentError("basket_token / basket_amount need basket_off[end] entries"))
+    limit === nothing || length(limit) == q || throw(ArgumentError("limit needs q entries"))
+    o = opts === nothing ? nothing : Ref(opts)
+    argt = (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{UInt8}, Ptr{SubgraphOpts},
+            Ptr{SubgraphOut})
+    tok_off, leg_off = zeros(Int64, q + 1), zeros(Int64, q + 1)
+    sizes = Ref(SubgraphOut(C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, pointer(tok_off), 0, C_NULL,
+                            C_NULL, C_NULL, pointer(leg_off), 0, C_NULL, C_NULL, C_NULL, C_NULL))
+    GC.@preserve tok_off leg_off chk(ctx, ccall((:cfmm_quote_basket_orders, LIB), Cint, argt,
+        ctx, q, token_out, basket_off, basket_token, basket_amount, allowed, o === nothing ? C_NULL : o, sizes))
+    NT, L = tok_off[end], leg_off[end]
+    paid, received, merit, status = zeros(max(NE, 1)), zeros(q), zeros(q), zeros(UInt8, q)
+    sst, iters, fev = zeros(Cint, q), zeros(Cint, q), zeros(Cint, q)
+    token, nu, psi = zeros(Int64, max(NT, 1)), zeros(max(NT, 1)), zeros(max(NT, 1))
+    ltype, lpool, ld, ll = zeros(Cint, max(L, 1)), zeros(Int64, max(L, 1)), zeros(2, max(L, 1)), zeros(2, max(L, 1))
+    GC.@preserve paid received merit status sst iters fev tok_off token nu psi leg_off ltype lpool ld ll begin
+        out = Ref(SubgraphOut(pointer(paid), pointer(received), pointer(status), pointer(sst), pointer(iters),
+                              pointer(fev), pointer(merit), pointer(tok_off), NT, pointer(token), pointer(nu),
+                              pointer(psi), pointer(leg_off), L, pointer(ltype), pointer(lpool), pointer(ld),
+                              pointer(ll)))
+        if execute
+            chk(ctx, ccall((:cfmm_execute_basket_orders, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8},
+                 Ptr{SubgraphOpts}, Ptr{SubgraphOut}),
+                ctx, q, token_out, basket_off, basket_token, basket_amount, limit === nothing ? C_NULL : limit,
+                allowed, o === nothing ? C_NULL : o, out))
+        else
+            chk(ctx, ccall((:cfmm_quote_basket_orders, LIB), Cint, argt,
+                ctx, q, token_out, basket_off, basket_token, basket_amount, allowed, o === nothing ? C_NULL : o, out))
+        end
+    end
+    return (paid=paid[1:NE], received=received, status=status, solver_status=sst, iterations=iters,
+            fun_evals=fev, merit=merit, tok_off=tok_off, token=token[1:NT], nu=nu[1:NT], psi=psi[1:NT],
+            leg_off=leg_off, leg_type=ltype[1:L], leg_pool=lpool[1:L], leg_delta=ld[:, 1:L], leg_lambda=ll[:, 1:L])
+end
+quote_basket_orders(ctx, token_out, basket_off, basket_token, basket_amount, allowed; opts=nothing) =
+    _basket_orders(ctx, false, token_out, basket_off, basket_token, basket_amount, allowed, nothing, opts)
+execute_basket_orders!(ctx, token_out, basket_off, basket_token, basket_amount, allowed; limit=nothing,
+                       opts=nothing) =
+    _basket_orders(ctx, true, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts)
+
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
 # current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never

@@ -60,6 +60,26 @@ def pool_file_info(path):
     return t.value, n.value, m.value
 
 
+def _row_args(n_tokens, q, allowed, limit, opts, what):
+    """(the mask as a uint8 pointer, the limits, the options by reference or None) of a subgraph or
+    basket call, with the Python argument errors."""
+    if allowed is None:
+        raise ValueError(f"{what}: allowed (a mask over the tokens) is required")
+    mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
+    if len(mask) != n_tokens:
+        raise ValueError(f"{what}: allowed must have {n_tokens} entries, one per token")
+    if limit is not None:
+        limit = np.ascontiguousarray(limit, dtype=np.float64).reshape(-1)
+        if len(limit) != q:
+            raise ValueError(f"limit must have {q} entries, one per row")
+    o = None
+    if opts is not None:
+        d = {"max_iter": 1000, "max_fun": 4000, "rtol": 1e-4, "factr": 0.0}
+        d.update(opts)
+        o = _lib.SubgraphOpts(int(d["max_iter"]), int(d["max_fun"]), float(d["rtol"]), float(d["factr"]))
+    return mask.ctypes.data_as(C.POINTER(C.c_uint8)), limit, None if o is None else C.byref(o)
+
+
 class DevicePools:
     """One GPU's shard of the pool set: a thin object wrapper over cfmm_ctx."""
 
@@ -714,52 +734,42 @@ class DevicePools:
         q = len(tin)
         if not (len(tout) == len(amount) == q):
             raise ValueError("subgraph orders: token_in, token_out and amount need one entry per row")
-        if allowed is None:
-            raise ValueError("subgraph orders: allowed (a mask over the tokens) is required")
-        mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
-        if len(mask) != self.n_tokens:
-            raise ValueError(f"subgraph orders: allowed must have {self.n_tokens} entries, one per token")
-        if limit is not None:
-            limit = np.ascontiguousarray(limit, dtype=np.float64).reshape(-1)
-            if len(limit) != q:
-                raise ValueError(f"limit must have {q} entries, one per row")
-        o = None
-        if opts is not None:
-            d = {"max_iter": 1000, "max_fun": 4000, "rtol": 1e-4, "factr": 0.0}
-            d.update(opts)
-            o = _lib.SubgraphOpts(int(d["max_iter"]), int(d["max_fun"]), float(d["rtol"]), float(d["factr"]))
+        u8m, limit, po = _row_args(self.n_tokens, q, allowed, limit, opts, "subgraph orders")
+        ti, to, am = _ip(tin), _ip(tout), _dp(amount)
+        lim = None if limit is None else _dp(limit)
+
+        def call(size, out):
+            if execute and not size:
+                return self._lib.cfmm_execute_subgraph_orders(self._ctx, q, ti, to, am, lim, u8m, po, C.byref(out))
+            return self._lib.cfmm_quote_subgraph_orders(self._ctx, q, ti, to, am, u8m, po, C.byref(out))
+        return self._order_solve(q, q, _lib.SubgraphOut, call)
+
+    def _order_solve(self, q, n_paid, out_type, call):
+        """The outputs of a subgraph or basket call: call(True, out) with tok_cap = leg_cap = 0 for the
+        sizes (a row's token set and pool list do not depend on the reserves, so an execute's are the
+        same), then call(False, out) with every output.  Returns them as a namespace."""
         u8, i32, i64, f64 = C.POINTER(C.c_uint8), C.POINTER(C.c_int), C.POINTER(C.c_int64), C.POINTER(C.c_double)
-        u8m = mask.ctypes.data_as(u8)
-        # sizes: a quote with tok_cap = leg_cap = 0 (the rows' token sets and pool lists do not depend
-        # on the reserves, so an execute's are the same)
         tok_off, leg_off = np.zeros(q + 1, dtype=np.int64), np.zeros(q + 1, dtype=np.int64)
-        size = _lib.SubgraphOut()
+        size = out_type()
         size.tok_off, size.leg_off = tok_off.ctypes.data_as(i64), leg_off.ctypes.data_as(i64)
-        self._chk(self._lib.cfmm_quote_subgraph_orders(self._ctx, q, _ip(tin), _ip(tout), _dp(amount), u8m,
-                                                        None if o is None else C.byref(o), C.byref(size)))
+        self._chk(call(True, size))
         NT, L = int(tok_off[-1]), int(leg_off[-1])
-        paid, received, merit = np.zeros(q), np.zeros(q), np.zeros(q)
+        paid, received, merit = np.zeros(max(n_paid, 1)), np.zeros(q), np.zeros(q)
         status = np.zeros(q, dtype=np.uint8)
         sst, iters, fev = (np.zeros(q, dtype=np.int32) for _ in range(3))
         token, nu, psi = np.zeros(max(NT, 1), dtype=np.int64), np.zeros(max(NT, 1)), np.zeros(max(NT, 1))
         ltype, lpool = np.zeros(max(L, 1), dtype=np.int32), np.zeros(max(L, 1), dtype=np.int64)
         ld, ll = np.zeros((max(L, 1), 2)), np.zeros((max(L, 1), 2))
-        out = _lib.SubgraphOut(paid.ctypes.data_as(f64), received.ctypes.data_as(f64), status.ctypes.data_as(u8),
-                               sst.ctypes.data_as(i32), iters.ctypes.data_as(i32), fev.ctypes.data_as(i32),
-                               merit.ctypes.data_as(f64), tok_off.ctypes.data_as(i64), NT, token.ctypes.data_as(i64),
-                               nu.ctypes.data_as(f64), psi.ctypes.data_as(f64), leg_off.ctypes.data_as(i64), L,
-                               ltype.ctypes.data_as(i32), lpool.ctypes.data_as(i64), ld.ctypes.data_as(f64),
-                               ll.ctypes.data_as(f64))
-        if execute:
-            self._chk(self._lib.cfmm_execute_subgraph_orders(self._ctx, q, _ip(tin), _ip(tout), _dp(amount),
-                                                              None if limit is None else _dp(limit), u8m,
-                                                              None if o is None else C.byref(o), C.byref(out)))
-        else:
-            self._chk(self._lib.cfmm_quote_subgraph_orders(self._ctx, q, _ip(tin), _ip(tout), _dp(amount), u8m,
-                                                            None if o is None else C.byref(o), C.byref(out)))
-        return SimpleNamespace(paid=paid, received=received, status=status, solver_status=sst, iterations=iters,
-                               fun_evals=fev, merit=merit, tok_off=tok_off, token=token[:NT], nu=nu[:NT],
-                               psi=psi[:NT], leg_off=leg_off, leg_type=ltype[:L], leg_pool=lpool[:L],
+        out = out_type(paid.ctypes.data_as(f64), received.ctypes.data_as(f64), status.ctypes.data_as(u8),
+                       sst.ctypes.data_as(i32), iters.ctypes.data_as(i32), fev.ctypes.data_as(i32),
+                       merit.ctypes.data_as(f64), tok_off.ctypes.data_as(i64), NT, token.ctypes.data_as(i64),
+                       nu.ctypes.data_as(f64), psi.ctypes.data_as(f64), leg_off.ctypes.data_as(i64), L,
+                       ltype.ctypes.data_as(i32), lpool.ctypes.data_as(i64), ld.ctypes.data_as(f64),
+                       ll.ctypes.data_as(f64))
+        self._chk(call(False, out))
+        return SimpleNamespace(paid=paid[:n_paid], received=received, status=status, solver_status=sst,
+                               iterations=iters, fun_evals=fev, merit=merit, tok_off=tok_off, token=token[:NT],
+                               nu=nu[:NT], psi=psi[:NT], leg_off=leg_off, leg_type=ltype[:L], leg_pool=lpool[:L],
                                leg_delta=ld[:L], leg_lambda=ll[:L])
 
     def quote_subgraph_orders(self, token_in, token_out, amount, allowed, opts=None):
@@ -777,6 +787,47 @@ class DevicePools:
         on the state the earlier filled rows left; limit[j] (None: none) is the minimum received, and a
         row below it reverts.  Returns what quote_subgraph_orders returns."""
         return self._subgraph(True, token_in, token_out, amount, allowed, limit, opts)
+
+    # -- token baskets over every pool among allowed tokens (include/cfmm_b200.h,
+    #    cfmm_quote_basket_orders / cfmm_execute_basket_orders) --------------------------------------
+    def _basket(self, execute, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts):
+        tout = np.ascontiguousarray(token_out, dtype=np.int64).reshape(-1)
+        boff = np.ascontiguousarray(basket_off, dtype=np.int64).reshape(-1)
+        btok = np.ascontiguousarray(basket_token, dtype=np.int64).reshape(-1)
+        bamt = np.ascontiguousarray(basket_amount, dtype=np.float64).reshape(-1)
+        q = len(tout)
+        if len(boff) != q + 1:
+            raise ValueError(f"basket orders: basket_off must have {q + 1} entries, one per row plus one")
+        NE = int(boff[-1])
+        if not (len(btok) == len(bamt) == NE):
+            raise ValueError(f"basket orders: basket_token and basket_amount need basket_off[-1] = {NE} entries")
+        u8m, limit, po = _row_args(self.n_tokens, q, allowed, limit, opts, "basket orders")
+        to, bo, bt, ba = _ip(tout), _ip(boff), _ip(btok), _dp(bamt)
+        lim = None if limit is None else _dp(limit)
+
+        def call(size, out):
+            if execute and not size:
+                return self._lib.cfmm_execute_basket_orders(self._ctx, q, to, bo, bt, ba, lim, u8m, po, C.byref(out))
+            return self._lib.cfmm_quote_basket_orders(self._ctx, q, to, bo, bt, ba, u8m, po, C.byref(out))
+        out = self._order_solve(q, NE, _lib.BasketOut, call)
+        out.basket_off = boff
+        return out
+
+    def quote_basket_orders(self, token_out, basket_off, basket_token, basket_amount, allowed, opts=None):
+        """cfmm_quote_basket_orders: row r sells basket_amount[k] of basket_token[k] for k in
+        basket_off[r] .. basket_off[r + 1] - 1 (1 to 16 distinct tokens, 1-based, none token_out[r])
+        for token_out[r] over every pool among them and the tokens t with allowed[t - 1], split
+        optimally: route! with BasketLiquidation over the row's pools, solved per row on the device.
+        opts as quote_subgraph_orders.  No state changes.  Returns quote_subgraph_orders' namespace,
+        with paid per basket entry and basket_off added."""
+        return self._basket(False, token_out, basket_off, basket_token, basket_amount, allowed, None, opts)
+
+    def execute_basket_orders(self, token_out, basket_off, basket_token, basket_amount, allowed, limit=None,
+                              opts=None):
+        """cfmm_execute_basket_orders: the rows of quote_basket_orders in batch order, each re-solved on
+        the state the earlier filled rows left; limit[r] (None: none) is the minimum received of
+        token_out[r], and a row below it reverts.  Returns what quote_basket_orders returns."""
+        return self._basket(True, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts)
 
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
@@ -1376,13 +1427,69 @@ class Router:
         tin, tout, amounts, limits = self._subgraph_args(token_in, token_out, amounts, allowed, limits,
                                                          "execute_subgraph_orders")
         out = self._pools.execute_subgraph_orders(tin, tout, amounts, allowed, limits, opts)
+        self._refresh_filled(out)
+        return out.paid, out.received, out.status, out
+
+    def _refresh_filled(self, out):
+        """Refresh the pool objects the filled rows of a subgraph or basket execute traded with."""
         filled = np.flatnonzero(out.status == _lib.ORDER_FILLED)
         if len(filled):
             sel = np.concatenate([np.arange(out.leg_off[r], out.leg_off[r + 1]) for r in filled]).astype(np.int64)
             typ, idx = out.leg_type[sel], out.leg_pool[sel]
             if len(sel):
                 self._refresh_swapped([(t, None, idx[typ == t]) for t in (0, 1, 2) if np.any(typ == t)])
-        return out.paid, out.received, out.status, out
+
+    def _basket_args(self, token_out, baskets, allowed, limits, what):
+        """(token_out, basket_off, basket_token, basket_amount, limits) from baskets: one {token:
+        amount} dict or (tokens, amounts) pair per row."""
+        if self._world > 1:
+            raise NotImplementedError(f"{what} drives one GPU")
+        tout = np.asarray(token_out, dtype=np.int64).reshape(-1)
+        if len(baskets) != len(tout):
+            raise ValueError(f"{what}: token_out and baskets need one entry per row")
+        off, toks, amts = [0], [], []
+        for b in baskets:
+            t, a = (list(b.keys()), list(b.values())) if isinstance(b, dict) else (list(b[0]), list(b[1]))
+            if len(t) != len(a):
+                raise ValueError(f"{what}: a basket needs one amount per token")
+            toks += t
+            amts += a
+            off.append(len(toks))
+        if limits is not None:
+            limits = np.asarray(limits, dtype=np.float64).reshape(-1)
+            if len(limits) != len(tout):
+                raise ValueError(f"{what}: limits must have {len(tout)} entries")
+        if allowed is None:
+            raise ValueError(f"{what}: allowed (a mask over the tokens) is required")
+        return (tout, np.array(off, np.int64), np.array(toks, np.int64), np.array(amts, np.float64).reshape(-1),
+                limits)
+
+    @staticmethod
+    def _per_entry(out):
+        return [out.paid[out.basket_off[r]:out.basket_off[r + 1]] for r in range(len(out.basket_off) - 1)]
+
+    def quote_basket_orders(self, token_out, baskets, allowed, opts=None):
+        """Sell each row's basket (baskets[r]: {token: amount} or (tokens, amounts); 1 to 16 distinct
+        1-based tokens, none of them token_out[r]) for token_out[r] over every pool among them and the
+        tokens t with allowed[t - 1] (a mask over the tokens), split optimally: route! with
+        BasketLiquidation(token_out[r], Δin) over those pools, one dual solve per row on the device
+        (cfmm_quote_basket_orders).  No state changes.  Returns (paid per entry as a list of arrays in
+        the basket's order, received [q], status [q], detail): detail is DevicePools.
+        quote_basket_orders' namespace.  Single GPU."""
+        tout, off, toks, amts, _ = self._basket_args(token_out, baskets, allowed, None, "quote_basket_orders")
+        out = self._pools.quote_basket_orders(tout, off, toks, amts, allowed, opts)
+        return self._per_entry(out), out.received, out.status, out
+
+    def execute_basket_orders(self, token_out, baskets, allowed, limits=None, opts=None):
+        """Execute basket orders in order (cfmm_execute_basket_orders), each re-solved on the state the
+        earlier filled rows left, with an optional minimum received per row: a row below it reverts.
+        Returns what quote_basket_orders returns and refreshes the pool objects the filled rows traded
+        with from the device state.  Single GPU."""
+        tout, off, toks, amts, limits = self._basket_args(token_out, baskets, allowed, limits,
+                                                          "execute_basket_orders")
+        out = self._pools.execute_basket_orders(tout, off, toks, amts, allowed, limits, opts)
+        self._refresh_filled(out)
+        return self._per_entry(out), out.received, out.status, out
 
     def _arbitrage_args(self, base, other, hubs, min_profit, what):
         if self._world > 1:

@@ -858,6 +858,77 @@ int cfmm_execute_subgraph_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_
                                  const double *limit /* [q] or NULL */, const uint8_t *allowed,
                                  const cfmm_subgraph_opts *opts, cfmm_subgraph_out *out);
 
+/* ---- token baskets liquidated over every pool among their allowed tokens --------------------
+ * A row sells a basket of tokens for i = token_out[r] over every pool among i, the basket and the
+ * allowed tokens, split optimally: route! with BasketLiquidation(i, Δin) (src/objectives.jl)
+ * restricted to the row's pools, one convex dual per row.  A subgraph order (above) is the basket
+ * of one entry: a one-entry basket row gives that call's outputs bit for bit.
+ *   basket   entries basket_off[r] .. basket_off[r+1] − 1 of basket_token (1-based) and
+ *            basket_amount (δ_k, finite and >= 0): 1 to CFMM_BASKET_MAX_TOKENS entries, distinct, none
+ *            of them i.  basket_off [q+1] starts at 0 and does not decrease.
+ *   B        the allowed tokens (allowed [n_tokens], required; one mask per call) minus i and the
+ *            basket.  A row's tokens other than i (basket ∪ B) number at most
+ *            CFMM_SUBGRAPH_MAX_TOKENS + 1.
+ *   T        the tokens of {i} ∪ basket ∪ B connected to i through active pools whose two tokens both
+ *            lie in that set.  An entry with δ_k > 0 outside T makes the row CFMM_ORDER_UNREACHABLE;
+ *            an entry with δ_k = 0 outside T is dropped from the row's tokens.
+ *   pools    every pool of every pair inside T, in global insertion order, as for subgraph orders.
+ *   tokens   local order: i, then the basket entries in T in the caller's order, then B ∩ T ascending.
+ * Problem.  Minimise g(ν) = Σ_k δ_k·ν_k + Σ_p π_p(ν) on the box of Swap (ν_i >= 1 + √eps, ν_t >= √eps
+ * otherwise).  Legs, sums, optimizer and start are those of subgraph orders, with the gradient
+ * (δ_k at b_k, 0 elsewhere) + Ψ and V = Σ_k δ_k·ν_k added in basket order (the first term alone).
+ *   stop     m_r = max_t ν_t·|pg_t| / V; status 0 when m_r <= rtol.
+ * What a fill promises.  A row fills only at solver status 0 (else CFMM_ORDER_NOT_CONVERGED, with
+ * zero legs, paid and received).  A filled row has received = Ψ_i and paid_k = −Ψ_{b_k}: each basket
+ * token is paid within rtol·V/ν_k of δ_k when ν_k is off its bound; every intermediate's net is
+ * Ψ_b >= −rtol·V/ν_b; and the duality gap is at most |T|·rtol·V plus the box's √eps terms.  A row
+ * whose amounts are all 0 fills with zeros and runs no solve.
+ * Outputs (cfmm_basket_out; every pointer may be NULL): those of cfmm_subgraph_out, except that paid
+ * has one entry per basket entry ([basket_off[q]], 0 for an entry outside T); received and the rest
+ * are per row.  Ask a quote with tok_cap = leg_cap = 0 for the sizes first.
+ * cfmm_quote_basket_orders prices every row on the current state on its own; no state changes.
+ * cfmm_execute_basket_orders runs the rows in batch order, each re-solved on the state the earlier
+ * filled rows left; limit (NULL: none) is the minimum received of i, and an equal limit fills.  A
+ * filled row applies split_leg's transition, then the bookkeeping of cfmm_execute_swaps.  Two rows
+ * conflict when they share a token of {i} ∪ basket ∪ B; rows are leveled by cfmm_execute_paths'
+ * rule, one launch per level (with an empty mask, rows on disjoint tokens run in one launch).  An
+ * execute whose token or leg outputs are given with a cap below the size is rejected before
+ * anything changes.
+ * Options: cfmm_subgraph_opts, with the same defaults.  Synchronous.  Before cfmm_finalize:
+ * CFMM_ERR_STATE.  q == 0 does nothing.  CFMM_ERR_INVALID before anything runs for: the argument
+ * errors of subgraph orders (q, a null array, the mask, the options, amounts, limits); token_out or
+ * a basket token outside 1..n_tokens; basket_off[0] != 0 or a decreasing basket_off; an empty basket
+ * or one longer than CFMM_BASKET_MAX_TOKENS; a basket token that appears twice or equals token_out;
+ * a row with more than CFMM_SUBGRAPH_MAX_TOKENS + 1 tokens besides token_out. */
+#define CFMM_BASKET_MAX_TOKENS 16
+typedef struct {
+  double *paid;                                  /* [basket_off[q]] */
+  double *received;                              /* [q] */
+  uint8_t *status;                               /* [q] */
+  int *solver_status, *iterations, *fun_evals;   /* [q] */
+  double *merit;                                 /* [q] */
+  int64_t *tok_off;                              /* [q+1] */
+  int64_t tok_cap;
+  int64_t *token;                                /* [tok_off[q]] */
+  double *nu, *psi;                              /* [tok_off[q]] */
+  int64_t *leg_off;                              /* [q+1] */
+  int64_t leg_cap;
+  int *leg_type;                                 /* [leg_off[q]] */
+  int64_t *leg_pool;                             /* [leg_off[q]] */
+  double *leg_delta, *leg_lambda;                /* [2·leg_off[q]] */
+} cfmm_basket_out;
+int cfmm_quote_basket_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_out /* [q] */,
+                             const int64_t *basket_off /* [q+1] */,
+                             const int64_t *basket_token /* [basket_off[q]] */,
+                             const double *basket_amount /* [basket_off[q]] */,
+                             const uint8_t *allowed /* [n_tokens], required */,
+                             const cfmm_subgraph_opts *opts /* NULL = defaults */, cfmm_basket_out *out);
+int cfmm_execute_basket_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_out,
+                               const int64_t *basket_off, const int64_t *basket_token,
+                               const double *basket_amount, const double *limit /* [q] or NULL */,
+                               const uint8_t *allowed, const cfmm_subgraph_opts *opts,
+                               cfmm_basket_out *out);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
