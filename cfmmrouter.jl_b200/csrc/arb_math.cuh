@@ -76,9 +76,12 @@ __device__ __forceinline__ Trade product_full(double R1, double R2, double g,
 //   Δ2, Λ1 > 0  <=>  γ·v1·R1 > v2·R2
 // and with γ <= 1 at most one holds.  The non-zero pair shares γ·m, so it
 // costs 3 div + 2 sqrt instead of 6 div + 4 sqrt.
+// A pool without reserves (a padding pool of the device layout, a retired pool) trades nothing at
+// any price; the full forms would give NaN for it where a price is 0, ∞ or NaN (sqrt(∞·0), 0/0).
 __device__ __forceinline__ Trade product_arb(double R1, double R2, double g,
                                              double v1, double v2, bool exact) {
-  if (exact) return product_full(R1, R2, g, v1, v2);
+  const bool no_reserves = R1 == 0.0 && R2 == 0.0;
+  if (exact && !no_reserves) return product_full(R1, R2, g, v1, v2);
   const double uA = __dmul_rn(v1, R1);
   const double uB = __dmul_rn(v2, R2);
   const double tA = __dmul_rn(g, uB);
@@ -109,7 +112,7 @@ __device__ __forceinline__ Trade product_arb(double R1, double R2, double g,
     }
     return t;
   }
-  if (sane && zA && zB) return t;  // strictly inside the no-trade band
+  if ((sane && zA && zB) || no_reserves) return t;  // strictly inside the no-trade band, or no pool
   return product_full(R1, R2, g, v1, v2);
 }
 

@@ -104,6 +104,12 @@ struct ProductPools {
   }
 };
 
+// A ProductTwoCoin pool without reserves (padding, retired) trades nothing (product_arb) and adds no
+// 0·ν terms to acc, which would be NaN at ν = ∞ or NaN.
+template <class Pool>
+__device__ __forceinline__ bool no_reserves(const Pool&) { return false; }
+__device__ __forceinline__ bool no_reserves(const ProductPools::Pool& p) { return p.R.x == 0.0 && p.R.y == 0.0; }
+
 struct GeomeanPools {
   const double2* R;
   const double* gam;
@@ -248,7 +254,7 @@ __global__ void __launch_bounds__(kSweepThreads, MinBlocks<P>::value)
       }
       // dot(Λ, ν[Ai]) − dot(Δ, ν[Ai])
       const double c = (t.l1 * v1[u] + t.l2 * v2[u]) - (t.d1 * v1[u] + t.d2 * v2[u]);
-      if (!skip_acc) acc += ok[u] ? c : 0.0;
+      if (!skip_acc) acc += (ok[u] && !no_reserves(pool[u])) ? c : 0.0;
       if (f2 != 0.0 && !skip_b) red_add(psi + ai[u].y, f2);
       if (!skip_a) warp_segmented_red(psi, ok[u] ? ai[u].x : -1, f1, lane);
     }
