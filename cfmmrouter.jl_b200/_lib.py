@@ -37,7 +37,7 @@ ROUTE_MAX_HUBS = 7  # CFMM_ROUTE_MAX_HUBS
 # cfmm_find_order_paths
 BEST_PATH_MAX_TOKENS = 1024
 PATH_REPEATS_POOL = 4
-# cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders
+# cfmm_quote_subgraph_(swap_)orders / cfmm_execute_subgraph_(swap_)orders
 SUBGRAPH_MAX_TOKENS = 256
 ORDER_NOT_CONVERGED = 5
 # cfmm_quote_basket_orders / cfmm_execute_basket_orders
@@ -139,6 +139,12 @@ SYMBOLS = {
                                              C.POINTER(SubgraphOpts), C.POINTER(SubgraphOut)]),
     "cfmm_execute_subgraph_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _dp, _dp, C.POINTER(C.c_uint8),
                                                C.POINTER(SubgraphOpts), C.POINTER(SubgraphOut)]),
+    "cfmm_quote_subgraph_swap_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp,
+                                                  C.POINTER(C.c_uint8), C.POINTER(SubgraphOpts),
+                                                  C.POINTER(SubgraphOut)]),
+    "cfmm_execute_subgraph_swap_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, _dp,
+                                                    C.POINTER(C.c_uint8), C.POINTER(SubgraphOpts),
+                                                    C.POINTER(SubgraphOut)]),
     "cfmm_quote_basket_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, _dp, C.POINTER(C.c_uint8),
                                            C.POINTER(SubgraphOpts), C.POINTER(BasketOut)]),
     "cfmm_execute_basket_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, _dp, _dp, C.POINTER(C.c_uint8),

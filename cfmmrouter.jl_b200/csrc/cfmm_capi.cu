@@ -3940,18 +3940,29 @@ int check_limit(cfmm_ctx* ctx, const double* limit, int64_t r, const char* what)
   return CFMM_OK;
 }
 
-// Every argument of cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders, before anything runs.
-int check_subgraph(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const double* amount,
-                   const double* limit, const uint8_t* allowed, const cfmm_subgraph_opts& o, const char* what) {
+// Every argument of cfmm_quote_subgraph_swap_orders / cfmm_execute_subgraph_swap_orders, before
+// anything runs.  kind null: every row exact-in.
+int check_subgraph(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const uint8_t* kind,
+                   const double* amount, const double* limit, const uint8_t* allowed, const cfmm_subgraph_opts& o,
+                   const char* what) {
   int rc = check_row_opts(ctx, q, allowed, o, what);
   if (rc != CFMM_OK || q == 0) return rc;
   if (!token_in || !token_out || !amount) return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
   if ((rc = check_pair_tokens(ctx, q, token_in, token_out, what)) != CFMM_OK) return rc;
   for (int64_t j = 0; j < q; ++j) {
+    if (kind && kind[j] > CFMM_SWAP_EXACT_OUT)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: kind %d is neither 0 (exact-in) nor 1 (exact-out)", what,
+                  (long long)j, (int)kind[j]);
     if (!std::isfinite(amount[j]) || amount[j] < 0.0)
       return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: amount %g must be finite and >= 0", what, (long long)j,
                   amount[j]);
-    if ((rc = check_limit(ctx, limit, j, what)) != CFMM_OK) return rc;
+    if (kind && kind[j] == CFMM_SWAP_EXACT_OUT) {  // the maximum paid: +inf allowed
+      if (limit && !(limit[j] >= 0.0))
+        return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: exact-out limit %g must be >= 0", what, (long long)j,
+                    limit[j]);
+    } else if ((rc = check_limit(ctx, limit, j, what)) != CFMM_OK) {
+      return rc;
+    }
   }
   int64_t n_allowed = 0;
   for (int64_t t = 0; t < ctx->n_tokens; ++t) n_allowed += allowed[t] != 0;
@@ -4008,9 +4019,20 @@ int check_basket(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64
   return CFMM_OK;
 }
 
+// The occupancy of a subgraph row kernel, cached per context.
+int subgraph_occupancy(cfmm_ctx* ctx, const void* kernel, int& occ) {
+  int& c = ctx->occupancy[kernel];
+  if (c == 0) {
+    CU_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, kernel, cfmm::kSubgraphThreads, 0));
+    if (c < 1) return fail(ctx, CFMM_ERR_CUDA, "a subgraph row kernel does not fit on an SM");
+  }
+  occ = c;
+  return CFMM_OK;
+}
+
 int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, const int64_t* token_out,
-                    const double* amount, const double* limit, const uint8_t* allowed, const cfmm_subgraph_opts& o,
-                    cfmm_subgraph_out* out) {
+                    const uint8_t* kind, const double* amount, const double* limit, const uint8_t* allowed,
+                    const cfmm_subgraph_opts& o, cfmm_subgraph_out* out) {
   int rc;
   CU_TRY(ctx, cudaSetDevice(ctx->device));
   if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
@@ -4050,14 +4072,15 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
   const cfmm::PairIndexView pv{ix.off.p, ix.pool.p};
   const cfmm::AdjView A{ix.adj_off.p, ix.adj_nbr.p, ix.adj_pair.p};
   const cfmm::BestPathGraph G{d_tok.p, d_slot.p, d_deg.p, d_gnbr.p, d_gpair.p, nB};
-  // a persistent grid: one wave of resident CTAs
-  int& occ = ctx->occupancy[reinterpret_cast<const void*>(&cfmm::subgraph_kernel<false>)];
-  if (occ == 0) {
-    CU_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cfmm::subgraph_kernel<false>,
-                                                              cfmm::kSubgraphThreads, 0));
-    if (occ < 1) return fail(ctx, CFMM_ERR_CUDA, "subgraph_kernel does not fit on an SM");
-  }
-  const int64_t wave = (int64_t)ctx->sm_count * occ;
+  // a persistent grid: one wave of resident CTAs of each kernel that runs
+  int occ = 0, occ_out = 0;
+  const auto kernel = [](auto k) { return reinterpret_cast<const void*>(k); };
+  if ((rc = subgraph_occupancy(ctx, kernel(&cfmm::subgraph_kernel<false>), occ)) != CFMM_OK) return rc;
+  const int64_t n_out = kind ? std::count(kind, kind + q, (uint8_t)CFMM_SWAP_EXACT_OUT) : 0;
+  if (n_out == 0) kind = nullptr;  // every row exact-in: the path of cfmm_quote_subgraph_orders
+  if (n_out > 0 && (rc = subgraph_occupancy(ctx, kernel(&cfmm::subgraph_out_kernel<false>), occ_out)) != CFMM_OK)
+    return rc;
+  const int64_t wave = (int64_t)ctx->sm_count * occ, wave_out = (int64_t)ctx->sm_count * occ_out;
   const unsigned plan_grid = (unsigned)std::min<int64_t>(q, wave);
   if ((rc = launch(ctx, kProfSwaps, nB > 0 ? 3 : 1, [&] {
          if (nB > 0) {
@@ -4120,7 +4143,7 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
   }
   int64_t cap = 1;
   while (cap < max_pool) cap <<= 1;
-  const int64_t grid = std::min<int64_t>(q, wave);
+  const int64_t grid = std::min<int64_t>(q, std::max(wave, wave_out));  // the workspaces
   DevBuf<int64_t> w64;
   DevBuf<int32_t> w32;
   DevBuf<double> wd;
@@ -4133,13 +4156,34 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
                        o.factr,    d_tok_off.p, d_leg_off.p, d_paid.p, d_recv.p,   d_status.p, d_sst.p,
                        d_iter.p,   d_fev.p,   d_merit.p,  d_token.p,  d_nu.p,     d_psi.p,   d_entry.p,
                        d_ld.p,     d_ll.p};
+  // rows[0 .. n_in) exact-in, rows[n_in .. n) exact-out: one launch of each kernel that has rows
+  const auto run = [&](auto exec_tag, const cfmm::PathSets* P, const cfmm::SplitMoved& mv, const int64_t* rows,
+                       int64_t n_in, int64_t n) {
+    constexpr bool X = decltype(exec_tag)::value;
+    return launch(ctx, kProfSwaps, (n_in > 0) + (n > n_in), [&] {
+      if (n_in > 0)
+        cfmm::subgraph_kernel<X><<<(unsigned)std::min(n_in, wave), cfmm::kSubgraphThreads, 0, st>>>(
+            P, pv, A, G, d_act.p, R, W, mv, rows, n_in);
+      if (n > n_in)
+        cfmm::subgraph_out_kernel<X><<<(unsigned)std::min(n - n_in, wave_out), cfmm::kSubgraphThreads, 0, st>>>(
+            P, pv, A, G, d_act.p, R, W, mv, rows + n_in, n - n_in);
+    });
+  };
+  const auto exact_in = [&](int64_t r) { return kind[r] != CFMM_SWAP_EXACT_OUT; };
   OrderSets xs;
-  if (!exec) {
+  if (!exec && !kind) {
     if ((rc = launch(ctx, kProfSwaps, 1, [&] {
            cfmm::subgraph_kernel<false><<<(unsigned)grid, cfmm::kSubgraphThreads, 0, st>>>(
                os.d_P.p, pv, A, G, d_act.p, R, W, cfmm::SplitMoved{}, nullptr, q);
          })) != CFMM_OK)
       return rc;
+  } else if (!exec) {
+    std::vector<int64_t> rows((size_t)q);
+    std::iota(rows.begin(), rows.end(), (int64_t)0);
+    std::stable_partition(rows.begin(), rows.end(), exact_in);
+    DevBuf<int64_t> d_rows;
+    CU_TRY(ctx, d_rows.upload(rows));
+    if ((rc = run(std::false_type{}, os.d_P.p, cfmm::SplitMoved{}, d_rows.p, q - n_out, q)) != CFMM_OK) return rc;
   } else {
     if ((rc = order_sets(ctx, true, xs)) != CFMM_OK) return rc;
     ctx->state_version++;
@@ -4155,10 +4199,21 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
             if (t != token_in[r] - 1 && t != token_out[r] - 1) visit(0, t);
         },
         order, level_off);
+    // a level's rows share no token, so their order does not matter: its exact-in rows go first
+    std::vector<int64_t> level_in(level_off.size(), 0);
+    for (size_t Lv = 1; kind && Lv < level_off.size(); ++Lv) {
+      const auto b = order.begin() + level_off[Lv - 1], e = order.begin() + level_off[Lv];
+      level_in[Lv] = std::stable_partition(b, e, exact_in) - b;
+    }
     DevBuf<int64_t> d_order;
     CU_TRY(ctx, d_order.upload(order));
     for (size_t Lv = 1; Lv < level_off.size(); ++Lv) {
       const int64_t n = level_off[Lv] - level_off[Lv - 1];
+      if (kind) {
+        if ((rc = run(std::true_type{}, xs.d_P.p, xs.mv, d_order.p + level_off[Lv - 1], level_in[Lv], n)) != CFMM_OK)
+          return rc;
+        continue;
+      }
       if ((rc = launch(ctx, kProfSwaps, 1, [&] {
              cfmm::subgraph_kernel<true><<<(unsigned)std::min<int64_t>(n, grid), cfmm::kSubgraphThreads, 0, st>>>(
                  xs.d_P.p, pv, A, G, d_act.p, R, W, xs.mv, d_order.p + level_off[Lv - 1], n);
@@ -4419,32 +4474,44 @@ int basket_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, c
 
 }  // namespace
 
-int cfmm_quote_subgraph_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
-                               const double* amount, const uint8_t* allowed, const cfmm_subgraph_opts* opts,
-                               cfmm_subgraph_out* out) {
+int cfmm_quote_subgraph_swap_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                                    const uint8_t* kind, const double* amount, const uint8_t* allowed,
+                                    const cfmm_subgraph_opts* opts, cfmm_subgraph_out* out) {
   const cfmm_subgraph_opts o = subgraph_opts(opts);
-  int rc = check_subgraph(ctx, q, token_in, token_out, amount, nullptr, allowed, o, "quote_subgraph_orders");
+  int rc = check_subgraph(ctx, q, token_in, token_out, kind, amount, nullptr, allowed, o, "quote_subgraph_orders");
   if (rc != CFMM_OK) return rc;
   if (q == 0) {
     if (out && out->tok_off) out->tok_off[0] = 0;
     if (out && out->leg_off) out->leg_off[0] = 0;
     return CFMM_OK;
   }
-  return subgraph_orders(ctx, false, q, token_in, token_out, amount, nullptr, allowed, o, out);
+  return subgraph_orders(ctx, false, q, token_in, token_out, kind, amount, nullptr, allowed, o, out);
+}
+
+int cfmm_execute_subgraph_swap_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                                      const uint8_t* kind, const double* amount, const double* limit,
+                                      const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_subgraph_out* out) {
+  const cfmm_subgraph_opts o = subgraph_opts(opts);
+  int rc = check_subgraph(ctx, q, token_in, token_out, kind, amount, limit, allowed, o, "execute_subgraph_orders");
+  if (rc != CFMM_OK) return rc;
+  if (q == 0) {
+    if (out && out->tok_off) out->tok_off[0] = 0;
+    if (out && out->leg_off) out->leg_off[0] = 0;
+    return CFMM_OK;
+  }
+  return subgraph_orders(ctx, true, q, token_in, token_out, kind, amount, limit, allowed, o, out);
+}
+
+int cfmm_quote_subgraph_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                               const double* amount, const uint8_t* allowed, const cfmm_subgraph_opts* opts,
+                               cfmm_subgraph_out* out) {
+  return cfmm_quote_subgraph_swap_orders(ctx, q, token_in, token_out, nullptr, amount, allowed, opts, out);
 }
 
 int cfmm_execute_subgraph_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
                                  const double* amount, const double* limit, const uint8_t* allowed,
                                  const cfmm_subgraph_opts* opts, cfmm_subgraph_out* out) {
-  const cfmm_subgraph_opts o = subgraph_opts(opts);
-  int rc = check_subgraph(ctx, q, token_in, token_out, amount, limit, allowed, o, "execute_subgraph_orders");
-  if (rc != CFMM_OK) return rc;
-  if (q == 0) {
-    if (out && out->tok_off) out->tok_off[0] = 0;
-    if (out && out->leg_off) out->leg_off[0] = 0;
-    return CFMM_OK;
-  }
-  return subgraph_orders(ctx, true, q, token_in, token_out, amount, limit, allowed, o, out);
+  return cfmm_execute_subgraph_swap_orders(ctx, q, token_in, token_out, nullptr, amount, limit, allowed, opts, out);
 }
 
 int cfmm_quote_basket_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,

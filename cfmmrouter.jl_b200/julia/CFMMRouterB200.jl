@@ -613,10 +613,13 @@ function find_order_paths(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}
     return hop_off, typ[1:n], pool[1:n], tok[1:n], tender[1:n], received[1:n], value, status
 end
 
-# Orders over every pool among allowed tokens (cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders):
-# row r sells amount[r] of token_in[r] for token_out[r] (exact-in) over every pool among the two and the
-# tokens t with allowed[t] != 0 (required, one entry per token, at most 256 besides the row's two),
-# route! with Swap over those pools, one dual solve per row.  opts = nothing: the defaults.  Returns a
+# Orders over every pool among allowed tokens (cfmm_quote_subgraph_swap_orders /
+# cfmm_execute_subgraph_swap_orders): row r sells amount[r] of token_in[r] for token_out[r] (kind 0,
+# exact-in) or buys amount[r] of token_out[r] paying in token_in[r] (kind 1, exact-out) over every pool
+# among the two and the tokens t with allowed[t] != 0 (required, one entry per token, at most 256 besides
+# the row's two), route! over those pools, one dual solve per row.  kind = nothing: every row exact-in;
+# limit: the minimum received (exact-in) or the maximum paid (exact-out).  opts = nothing: the defaults.
+# Returns a
 # NamedTuple of the per-row outputs, the token CSR (tok_off, token, nu, psi) and the legs CSR
 # (leg_off, leg_type, leg_pool, leg_delta / leg_lambda as 2 x L).  Never executed, like the rest of
 # this file.
@@ -634,48 +637,51 @@ struct SubgraphOut
     leg_delta::Ptr{Float64}; leg_lambda::Ptr{Float64}
 end
 function _subgraph_orders(ctx, execute::Bool, token_in::Vector{Int64}, token_out::Vector{Int64},
-                          amount::Vector{Float64}, allowed::Vector{UInt8}, limit, opts)
+                          amount::Vector{Float64}, allowed::Vector{UInt8}, limit, opts, kind=nothing)
     q = length(token_in)
     length(token_out) == length(amount) == q || throw(ArgumentError("token_in / token_out / amount need q entries"))
     limit === nothing || length(limit) == q || throw(ArgumentError("limit needs q entries"))
+    k = kind === nothing ? C_NULL : (kind isa Integer ? fill(UInt8(kind), q) : Vector{UInt8}(kind))
+    k === C_NULL || length(k) == q || throw(ArgumentError("kind needs q entries"))
     o = opts === nothing ? nothing : Ref(opts)
     tok_off, leg_off = zeros(Int64, q + 1), zeros(Int64, q + 1)
     sizes = Ref(SubgraphOut(C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, pointer(tok_off), 0, C_NULL,
                             C_NULL, C_NULL, pointer(leg_off), 0, C_NULL, C_NULL, C_NULL, C_NULL))
-    GC.@preserve tok_off leg_off chk(ctx, ccall((:cfmm_quote_subgraph_orders, LIB), Cint,
-        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{UInt8}, Ptr{SubgraphOpts}, Ptr{SubgraphOut}),
-        ctx, q, token_in, token_out, amount, allowed, o === nothing ? C_NULL : o, sizes))
+    GC.@preserve tok_off leg_off k chk(ctx, ccall((:cfmm_quote_subgraph_swap_orders, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{UInt8}, Ptr{SubgraphOpts},
+         Ptr{SubgraphOut}),
+        ctx, q, token_in, token_out, k, amount, allowed, o === nothing ? C_NULL : o, sizes))
     NT, L = tok_off[end], leg_off[end]
     paid, received, merit, status = zeros(q), zeros(q), zeros(q), zeros(UInt8, q)
     sst, iters, fev = zeros(Cint, q), zeros(Cint, q), zeros(Cint, q)
     token, nu, psi = zeros(Int64, max(NT, 1)), zeros(max(NT, 1)), zeros(max(NT, 1))
     ltype, lpool, ld, ll = zeros(Cint, max(L, 1)), zeros(Int64, max(L, 1)), zeros(2, max(L, 1)), zeros(2, max(L, 1))
-    GC.@preserve paid received merit status sst iters fev tok_off token nu psi leg_off ltype lpool ld ll begin
+    GC.@preserve paid received merit status sst iters fev tok_off token nu psi leg_off ltype lpool ld ll k begin
         out = Ref(SubgraphOut(pointer(paid), pointer(received), pointer(status), pointer(sst), pointer(iters),
                               pointer(fev), pointer(merit), pointer(tok_off), NT, pointer(token), pointer(nu),
                               pointer(psi), pointer(leg_off), L, pointer(ltype), pointer(lpool), pointer(ld),
                               pointer(ll)))
         if execute
-            chk(ctx, ccall((:cfmm_execute_subgraph_orders, LIB), Cint,
-                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8},
+            chk(ctx, ccall((:cfmm_execute_subgraph_swap_orders, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8},
                  Ptr{SubgraphOpts}, Ptr{SubgraphOut}),
-                ctx, q, token_in, token_out, amount, limit === nothing ? C_NULL : limit, allowed,
+                ctx, q, token_in, token_out, k, amount, limit === nothing ? C_NULL : limit, allowed,
                 o === nothing ? C_NULL : o, out))
         else
-            chk(ctx, ccall((:cfmm_quote_subgraph_orders, LIB), Cint,
-                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{UInt8}, Ptr{SubgraphOpts},
+            chk(ctx, ccall((:cfmm_quote_subgraph_swap_orders, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{UInt8}, Ptr{SubgraphOpts},
                  Ptr{SubgraphOut}),
-                ctx, q, token_in, token_out, amount, allowed, o === nothing ? C_NULL : o, out))
+                ctx, q, token_in, token_out, k, amount, allowed, o === nothing ? C_NULL : o, out))
         end
     end
     return (paid=paid, received=received, status=status, solver_status=sst, iterations=iters, fun_evals=fev,
             merit=merit, tok_off=tok_off, token=token[1:NT], nu=nu[1:NT], psi=psi[1:NT], leg_off=leg_off,
             leg_type=ltype[1:L], leg_pool=lpool[1:L], leg_delta=ld[:, 1:L], leg_lambda=ll[:, 1:L])
 end
-quote_subgraph_orders(ctx, token_in, token_out, amount, allowed; opts=nothing) =
-    _subgraph_orders(ctx, false, token_in, token_out, amount, allowed, nothing, opts)
-execute_subgraph_orders!(ctx, token_in, token_out, amount, allowed; limit=nothing, opts=nothing) =
-    _subgraph_orders(ctx, true, token_in, token_out, amount, allowed, limit, opts)
+quote_subgraph_orders(ctx, token_in, token_out, amount, allowed; opts=nothing, kind=nothing) =
+    _subgraph_orders(ctx, false, token_in, token_out, amount, allowed, nothing, opts, kind)
+execute_subgraph_orders!(ctx, token_in, token_out, amount, allowed; limit=nothing, opts=nothing, kind=nothing) =
+    _subgraph_orders(ctx, true, token_in, token_out, amount, allowed, limit, opts, kind)
 
 # Token baskets over every pool among allowed tokens (cfmm_quote_basket_orders /
 # cfmm_execute_basket_orders): row r sells basket_amount[k] of basket_token[k] for k in

@@ -80,6 +80,29 @@ def _row_args(n_tokens, q, allowed, limit, opts, what):
     return mask.ctypes.data_as(C.POINTER(C.c_uint8)), limit, None if o is None else C.byref(o)
 
 
+def _row_kind(kind, q, limit, what):
+    """The kinds of a subgraph call as a uint8 array (None: every row exact-in, passed as NULL), with
+    the Python argument errors: a scalar applies to every row; a kind other than 0 (exact-in) or 1
+    (exact-out); a limit that is NaN, or +inf on an exact-in row (the minimum received)."""
+    if kind is None:
+        return None
+    k = np.asarray(kind)
+    if k.ndim == 0:
+        k = np.full(q, k)
+    k = k.reshape(-1)
+    if len(k) != q:
+        raise ValueError(f"{what}: kind must have {q} entries, one per row (or be a scalar)")
+    if not np.all(np.isin(k, (_lib.SWAP_EXACT_IN, _lib.SWAP_EXACT_OUT))):
+        raise ValueError(f"{what}: kind must be 0 (exact-in) or 1 (exact-out)")
+    k = np.ascontiguousarray(k, dtype=np.uint8)
+    if limit is not None:
+        if np.any(np.isnan(limit)):
+            raise ValueError(f"{what}: a limit is NaN")
+        if np.any(np.isinf(limit) & (k == _lib.SWAP_EXACT_IN)):
+            raise ValueError(f"{what}: an exact-in limit (the minimum received) is +inf")
+    return k
+
+
 class DevicePools:
     """One GPU's shard of the pool set: a thin object wrapper over cfmm_ctx."""
 
@@ -726,8 +749,8 @@ class DevicePools:
                 value, status)
 
     # -- orders over every pool among allowed tokens (include/cfmm_b200.h,
-    #    cfmm_quote_subgraph_orders / cfmm_execute_subgraph_orders) ----------------------------------
-    def _subgraph(self, execute, token_in, token_out, amount, allowed, limit, opts):
+    #    cfmm_quote_subgraph_swap_orders / cfmm_execute_subgraph_swap_orders) ------------------------
+    def _subgraph(self, execute, token_in, token_out, amount, allowed, limit, opts, kind=None):
         tin = np.ascontiguousarray(token_in, dtype=np.int64).reshape(-1)
         tout = np.ascontiguousarray(token_out, dtype=np.int64).reshape(-1)
         amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
@@ -735,13 +758,16 @@ class DevicePools:
         if not (len(tout) == len(amount) == q):
             raise ValueError("subgraph orders: token_in, token_out and amount need one entry per row")
         u8m, limit, po = _row_args(self.n_tokens, q, allowed, limit, opts, "subgraph orders")
+        kind = _row_kind(kind, q, limit, "subgraph orders")
         ti, to, am = _ip(tin), _ip(tout), _dp(amount)
+        kd = None if kind is None else kind.ctypes.data_as(C.POINTER(C.c_uint8))
         lim = None if limit is None else _dp(limit)
 
         def call(size, out):
             if execute and not size:
-                return self._lib.cfmm_execute_subgraph_orders(self._ctx, q, ti, to, am, lim, u8m, po, C.byref(out))
-            return self._lib.cfmm_quote_subgraph_orders(self._ctx, q, ti, to, am, u8m, po, C.byref(out))
+                return self._lib.cfmm_execute_subgraph_swap_orders(self._ctx, q, ti, to, kd, am, lim, u8m, po,
+                                                                   C.byref(out))
+            return self._lib.cfmm_quote_subgraph_swap_orders(self._ctx, q, ti, to, kd, am, u8m, po, C.byref(out))
         return self._order_solve(q, q, _lib.SubgraphOut, call)
 
     def _order_solve(self, q, n_paid, out_type, call):
@@ -772,21 +798,24 @@ class DevicePools:
                                nu=nu[:NT], psi=psi[:NT], leg_off=leg_off, leg_type=ltype[:L], leg_pool=lpool[:L],
                                leg_delta=ld[:L], leg_lambda=ll[:L])
 
-    def quote_subgraph_orders(self, token_in, token_out, amount, allowed, opts=None):
-        """cfmm_quote_subgraph_orders: row j sells amount[j] of token_in[j] for token_out[j] (1-based,
-        exact-in) over every pool among the two and the tokens t with allowed[t - 1] (at most 256
-        besides the row's two), split optimally: route! with Swap over the row's pools, solved per row
-        on the device.  opts: dict of max_iter, max_fun, rtol, factr (None: the defaults).  No state
-        changes.  Returns a namespace: paid, received, status (uint8), solver_status, iterations,
-        fun_evals, merit [q]; tok_off [q + 1], token, nu, psi [Σ]; leg_off [q + 1], leg_type, leg_pool
-        [L], leg_delta, leg_lambda [L, 2]."""
-        return self._subgraph(False, token_in, token_out, amount, allowed, None, opts)
+    def quote_subgraph_orders(self, token_in, token_out, amount, allowed, opts=None, kind=None):
+        """cfmm_quote_subgraph_swap_orders: row j sells amount[j] of token_in[j] for token_out[j]
+        (1-based; kind 0, exact-in) or buys amount[j] of token_out[j] paying in token_in[j] (kind 1,
+        exact-out) over every pool among the two and the tokens t with allowed[t - 1] (at most 256
+        besides the row's two), split optimally: route! over the row's pools, solved per row on the
+        device.  kind: None (every row exact-in), a scalar, or one entry per row.  opts: dict of
+        max_iter, max_fun, rtol, factr (None: the defaults).  No state changes.  Returns a namespace:
+        paid, received, status (uint8), solver_status, iterations, fun_evals, merit [q]; tok_off
+        [q + 1], token, nu, psi [Σ]; leg_off [q + 1], leg_type, leg_pool [L], leg_delta, leg_lambda
+        [L, 2]."""
+        return self._subgraph(False, token_in, token_out, amount, allowed, None, opts, kind)
 
-    def execute_subgraph_orders(self, token_in, token_out, amount, allowed, limit=None, opts=None):
-        """cfmm_execute_subgraph_orders: the rows of quote_subgraph_orders in batch order, each re-solved
-        on the state the earlier filled rows left; limit[j] (None: none) is the minimum received, and a
-        row below it reverts.  Returns what quote_subgraph_orders returns."""
-        return self._subgraph(True, token_in, token_out, amount, allowed, limit, opts)
+    def execute_subgraph_orders(self, token_in, token_out, amount, allowed, limit=None, opts=None, kind=None):
+        """cfmm_execute_subgraph_swap_orders: the rows of quote_subgraph_orders in batch order, each
+        re-solved on the state the earlier filled rows left; limit[j] (None: none) is the minimum
+        received of an exact-in row and the maximum paid of an exact-out row (+inf allowed), and a row
+        that misses it reverts.  Returns what quote_subgraph_orders returns."""
+        return self._subgraph(True, token_in, token_out, amount, allowed, limit, opts, kind)
 
     # -- token baskets over every pool among allowed tokens (include/cfmm_b200.h,
     #    cfmm_quote_basket_orders / cfmm_execute_basket_orders) --------------------------------------
@@ -1407,26 +1436,29 @@ class Router:
             raise ValueError(f"{what}: allowed (a mask over the tokens) is required")
         return tin, tout, amounts, limits
 
-    def quote_subgraph_orders(self, token_in, token_out, amounts, allowed, opts=None):
-        """Sell amounts[j] of token_in[j] for token_out[j] (1-based, exact-in) over every pool among the
+    def quote_subgraph_orders(self, token_in, token_out, amounts, allowed, opts=None, kind=None):
+        """Sell amounts[j] of token_in[j] for token_out[j] (1-based; kind 0, exact-in), or buy
+        amounts[j] of token_out[j] paying in token_in[j] (kind 1, exact-out), over every pool among the
         two and the tokens t with allowed[t - 1] (a mask over the tokens, at most 256 such tokens per
-        row besides its two), split optimally: route! with Swap over those pools, one dual solve per
-        row on the device (cfmm_quote_subgraph_orders).  No state changes.  Returns (paid [q],
-        received [q], status [q], detail): detail is DevicePools.quote_subgraph_orders' namespace
-        (solver status, iterations, ν, Ψ, legs).  Single GPU."""
+        row besides its two), split optimally: route! over those pools, one dual solve per row on the
+        device (cfmm_quote_subgraph_swap_orders).  kind: None (every row exact-in), a scalar, or one
+        entry per row.  No state changes.  Returns (paid [q], received [q], status [q], detail):
+        detail is DevicePools.quote_subgraph_orders' namespace (solver status, iterations, ν, Ψ,
+        legs).  Single GPU."""
         tin, tout, amounts, _ = self._subgraph_args(token_in, token_out, amounts, allowed, None,
                                                     "quote_subgraph_orders")
-        out = self._pools.quote_subgraph_orders(tin, tout, amounts, allowed, opts)
+        out = self._pools.quote_subgraph_orders(tin, tout, amounts, allowed, opts, kind)
         return out.paid, out.received, out.status, out
 
-    def execute_subgraph_orders(self, token_in, token_out, amounts, allowed, limits=None, opts=None):
-        """Execute subgraph orders in order (cfmm_execute_subgraph_orders), each re-solved on the state the
-        earlier filled rows left, with an optional minimum received per row: a row below it reverts.
-        Returns what quote_subgraph_orders returns and refreshes the pool objects the filled rows
-        traded with from the device state, as execute_swaps does.  Single GPU."""
+    def execute_subgraph_orders(self, token_in, token_out, amounts, allowed, limits=None, opts=None, kind=None):
+        """Execute subgraph orders in order (cfmm_execute_subgraph_swap_orders), each re-solved on the
+        state the earlier filled rows left, with an optional limit per row (exact-in: the minimum
+        received; exact-out: the maximum paid): a row that misses it reverts.  Returns what
+        quote_subgraph_orders returns and refreshes the pool objects the filled rows traded with from
+        the device state, as execute_swaps does.  Single GPU."""
         tin, tout, amounts, limits = self._subgraph_args(token_in, token_out, amounts, allowed, limits,
                                                          "execute_subgraph_orders")
-        out = self._pools.execute_subgraph_orders(tin, tout, amounts, allowed, limits, opts)
+        out = self._pools.execute_subgraph_orders(tin, tout, amounts, allowed, limits, opts, kind)
         self._refresh_filled(out)
         return out.paid, out.received, out.status, out
 

@@ -763,8 +763,8 @@ int cfmm_find_order_paths(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [
                           uint8_t *status /* [q] or NULL */);
 
 /* ---- orders routed over every pool among their allowed tokens ------------------------------
- * A row sells δ = amount[r] of j = token_in[r] for i = token_out[r] (1-based, distinct; exact-in
- * only) over every pool among j, i and the allowed tokens, split optimally: route! with
+ * A row sells δ = amount[r] of j = token_in[r] for i = token_out[r] (1-based, distinct; exact-in:
+ * exact-out rows are below) over every pool among j, i and the allowed tokens, split optimally: route! with
  * Swap(i, j, δ) (src/objectives.jl:106-146) restricted to the row's pools, one convex dual per row.
  *   B        the tokens t with allowed[t-1] != 0 (allowed [n_tokens], required), minus j and i; at
  *            most CFMM_SUBGRAPH_MAX_TOKENS per row.  One mask per call.
@@ -857,6 +857,60 @@ int cfmm_execute_subgraph_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_
                                  const int64_t *token_out, const double *amount,
                                  const double *limit /* [q] or NULL */, const uint8_t *allowed,
                                  const cfmm_subgraph_opts *opts, cfmm_subgraph_out *out);
+
+/* ---- subgraph orders of either kind: exact-in and exact-out rows ----------------------------
+ * cfmm_quote_subgraph_swap_orders / cfmm_execute_subgraph_swap_orders take the arguments of the two
+ * calls above plus kind [q] (NULL: every row exact-in).  A row of kind CFMM_SWAP_EXACT_IN is the
+ * subgraph order above, bit for bit; cfmm_quote_subgraph_orders and cfmm_execute_subgraph_orders
+ * are these calls with kind = NULL.  A row of kind CFMM_SWAP_EXACT_OUT buys y = amount[r] of
+ * i = token_out[r] and pays in j = token_in[r], over the same B, T, pools and local token order
+ * (i, j, then B ∩ T), legs, sums, optimizer and CTA reduction as an exact-in row.
+ * Problem.  The primal is: maximise Ψ_j subject to Ψ_i >= y and Ψ_t >= 0 for every other t in T.
+ * Its dual: minimise g(ν) = −y′·ν_i + Σ_k π_k(ν) on the box ν_j = 1 (lower = upper = 1), ν_t >= √eps
+ * for every other t (i included), with y′ = y·(1 + rtol) rounded up (fma, round toward +inf).  ν_j is
+ * fixed because the optimal value, −paid, is negative and g is positively homogeneous: with only a
+ * lower bound, scaling ν up would drive g to −∞.  The gradient is (−y′ at i, 0 elsewhere) + Ψ; the
+ * value is −y′·ν_i + the pool sum of exact-in rows.
+ *   start    ν_j = 1; then the breadth-first pricing of exact-in rows from j instead of i; then
+ *            clamped to the box.
+ *   box      slot j is clamped to [1, 1], so pg_j = 0 and its step is 0; every other slot uses the
+ *            lower-bound clip of exact-in rows.
+ *   stop     m_r = max_t ν_t·|pg_t| / (y·ν_i), the imbalance valued against the order's value in j.
+ *            Status 0 when m_r <= rtol; the other statuses as for exact-in rows.  Since
+ *            |pg_i| = |Ψ_i − y′| <= rtol·y at the stop, a converged row receives at least y.
+ * Capacity, checked once per row after its pool list is built and before any solve.  C_i is the sum,
+ * over the row's active pools holding i in pool order (per thread, then sg's CTA sum), of what the
+ * pool could ever pay out of i: a two-coin pool's reserve R_i; a UniV3 pool's walk to the end of its
+ * ladder (f(DBL_MAX) of cfmm_quote_swaps_exact_out, the quantity of its unreachable case).  A row is
+ * CFMM_ORDER_UNREACHABLE when j ∉ T or y >= C_i.  A row that passes this check but still cannot be
+ * served (for example i reachable only behind a thin intermediate pool) has an unbounded dual: it
+ * ends at max_iter, max_fun or NaN and is CFMM_ORDER_NOT_CONVERGED, trading nothing.
+ * What a fill promises.  A row fills only at solver status 0 and received >= y; a status-0 row whose
+ * received is below y (rounding) is CFMM_ORDER_NOT_CONVERGED with solver_status 0.  A filled row has
+ * received = Ψ_i in [y, y·(1 + 2·rtol)] when ν_i is off its bound, paid = −Ψ_j, every intermediate
+ * Ψ_b >= −rtol·y·ν_i/ν_b, and a duality gap of at most |T|·rtol·y·ν_i plus the box's √eps terms.
+ * Amount 0 fills with zeros and runs no solve.  The outputs are those of cfmm_subgraph_out.
+ * Execute.  limit (NULL: none) is the maximum paid for an exact-out row (+inf allowed; an equal limit
+ * fills, paid > limit reverts with CFMM_ORDER_LIMIT) and the minimum received for an exact-in row.
+ * The transition, bookkeeping, conflict rule and levels are those of exact-in rows; a level runs its
+ * exact-in rows and its exact-out rows as two launches (they share no token).  A quote runs the
+ * exact-in rows and the exact-out rows as two launches.
+ * Errors: those of the calls above, and CFMM_ERR_INVALID before anything runs for a kind other than
+ * CFMM_SWAP_EXACT_IN or CFMM_SWAP_EXACT_OUT, an exact-in limit that is NaN, negative or +inf, and an
+ * exact-out limit that is NaN or negative. */
+int cfmm_quote_subgraph_swap_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [q] */,
+                                    const int64_t *token_out /* [q] */,
+                                    const uint8_t *kind /* [q] or NULL: all exact-in */,
+                                    const double *amount /* [q] */,
+                                    const uint8_t *allowed /* [n_tokens], required */,
+                                    const cfmm_subgraph_opts *opts /* NULL = defaults */,
+                                    cfmm_subgraph_out *out);
+int cfmm_execute_subgraph_swap_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_in,
+                                      const int64_t *token_out,
+                                      const uint8_t *kind /* [q] or NULL: all exact-in */,
+                                      const double *amount, const double *limit /* [q] or NULL */,
+                                      const uint8_t *allowed, const cfmm_subgraph_opts *opts,
+                                      cfmm_subgraph_out *out);
 
 /* ---- token baskets liquidated over every pool among their allowed tokens --------------------
  * A row sells a basket of tokens for i = token_out[r] over every pool among i, the basket and the

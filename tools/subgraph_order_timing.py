@@ -15,7 +15,16 @@ where the subgraph's received is at least theirs (within 3·rtol) and the median
 configuration runs on 1k rows first; the 100k-row call runs when the 1k-row kernel time predicts at
 most --budget-s seconds for it, and is reported as not run (with the estimate) otherwise.
 
-    python tools/subgraph_order_timing.py [--only hub|headline] [--budget-s 20]
+--kind out quotes exact-out rows (cfmm_quote_subgraph_swap_orders): the same rows are first quoted
+exact-in (untimed), and each row that filled asks for what it received; --kind mixed alternates
+exact-in rows (even) and such exact-out rows (odd) in one call.  The records then also report, for
+the exact-out rows, paid against the exact-in tender δ (the median paid/δ and the fraction within
+(|T| + 1)·rtol·δ + (|T| + 2)·rtol·y·ν_i, the round-trip bound of the tests) and against auto-routed
+and best-path exact-out (the fraction where the subgraph pays at most theirs within 3·rtol, and the
+median ratio).  --B restricts the mask sizes.
+
+    python tools/subgraph_order_timing.py [--only hub|headline] [--budget-s 20] [--kind in|out|mixed]
+                                          [--B 8,64]
 """
 from __future__ import annotations
 
@@ -71,10 +80,37 @@ def compare(p, tin, tout, amt, allowed, o):
     return out
 
 
-def run(p, name, n, pick, amt_of, budget_s):
+def compare_out(p, tin, tout, y, delta, allowed, o, rtol=1e-4):
+    """Paid by the exact-out rows o against the exact-in tender and auto-routed / best-path exact-out."""
+    q = len(tin)
+    kind = np.ones(q, np.uint8)
+    filled = o.status == 0
+    out = {}
+    if np.any(filled):
+        nt = np.diff(o.tok_off)
+        nu_i = o.nu[o.tok_off[:-1]]
+        bound = (nt + 1) * rtol * delta + (nt + 2) * rtol * y * nu_i
+        out["vs_exact_in"] = dict(rows=int(np.sum(filled)),
+                                  median_ratio=round(float(np.median(o.paid[filled] / delta[filled])), 6),
+                                  within_bound=float(np.mean(np.abs(o.paid - delta)[filled] <= bound[filled])))
+    off, flat, _, _ = p.choose_order_hubs(tin, tout, kind, y, 7, allowed)
+    paid_r, _, _, st_r = p.quote_routed_orders(tin, tout, kind, y, off, flat)[:4]
+    value, st_p = p.find_order_paths(tin, tout, kind, y, 4, allowed)[6:]
+    for name, paid, st in (("auto_routed", paid_r, st_r), ("best_path", value, st_p)):
+        both = filled & (st == 0) & (paid > 0)
+        if np.any(both):
+            ratio = o.paid[both] / paid[both]
+            out[name] = dict(rows=int(np.sum(both)), at_most=float(np.mean(ratio <= 1 + 3 * rtol)),
+                             median_ratio=round(float(np.median(ratio)), 6))
+    return out
+
+
+def run(p, name, n, pick, amt_of, budget_s, kind="in", sizes=(8, 64, 256)):
     tin, tout = pick(1, 8)  # the first call builds the pair index and the token adjacency
     p.quote_subgraph_orders(tin, tout, amt_of(tin, tout), np.arange(n) < 8)
-    for nb in (8, 64, 256):
+    if kind != "in":
+        return run_out(p, name, n, pick, amt_of, budget_s, kind, sizes)
+    for nb in sizes:
         allowed = np.arange(n) < nb
         est = None
         for q in (1_000, 100_000):
@@ -92,7 +128,51 @@ def run(p, name, n, pick, amt_of, budget_s):
             est = ms * 100_000 / q
 
 
-def hub(rng, budget_s):
+def run_out(p, name, n, pick, amt_of, budget_s, kind, sizes):
+    for nb in sizes:
+        allowed = np.arange(n) < nb
+        est = None
+        for q in (1_000, 100_000):
+            if q > 1_000 and est > budget_s * 1e3:
+                emit(set=name, B=nb, rows=q, kind=kind, run=False, estimated_kernel_ms=round(est, 1))
+                continue
+            tin, tout = pick(q, nb)
+            delta = amt_of(tin, tout)
+            qi = p.quote_subgraph_orders(tin, tout, delta, allowed)
+            keep = qi.status == 0  # exact-out rows ask for what the exact-in row received
+            k = np.zeros(q, np.uint8) if kind == "mixed" else np.ones(q, np.uint8)
+            if kind == "mixed":
+                k[1::2] = 1
+                keep |= k == 0
+            tin, tout, delta, k = tin[keep], tout[keep], delta[keep], k[keep]
+            amt = np.where(k == 1, qi.received[keep], delta)
+            o, wall, ms, launches = timed(p, lambda: p._subgraph(False, tin, tout, amt, allowed, None, None, k))
+            rec = dict(set=name, B=nb, rows=int(len(tin)), kind=kind, out_rows=int(np.sum(k == 1)),
+                       wall_ms=round(wall, 3), kernel_ms=round(ms, 3), profile_entries=launches)
+            sel = np.flatnonzero(k == 1)
+            rec["exact_out"] = stats(pick_rows(o, sel))
+            if kind == "mixed":
+                rec["exact_in"] = stats(pick_rows(o, np.flatnonzero(k == 0)))
+            if q == 1_000:
+                rec.update(compare_out(p, tin[sel], tout[sel], amt[sel], delta[sel], allowed, pick_rows(o, sel)))
+            emit(**rec)
+            est = ms * 100_000 / q
+
+
+def pick_rows(o, sel):
+    """The per-row outputs of rows sel (with their token and leg offsets), as a namespace."""
+    from types import SimpleNamespace
+    tok = [np.arange(o.tok_off[r], o.tok_off[r + 1]) for r in sel]
+    leg_off = np.concatenate([[0], np.cumsum(np.diff(o.leg_off)[sel])]).astype(np.int64)
+    tok_off = np.concatenate([[0], np.cumsum([len(t) for t in tok])]).astype(np.int64)
+    ti = np.concatenate(tok + [np.zeros(0, np.int64)]).astype(np.int64)
+    return SimpleNamespace(paid=o.paid[sel], received=o.received[sel], status=o.status[sel],
+                           solver_status=o.solver_status[sel], iterations=o.iterations[sel],
+                           fun_evals=o.fun_evals[sel], merit=o.merit[sel], leg_off=leg_off, tok_off=tok_off,
+                           token=o.token[ti], nu=o.nu[ti])
+
+
+def hub(rng, budget_s, kind="in", sizes=(8, 64, 256)):
     p, n, others, nu, _ = hub_set(rng)
 
     def pick(q, nb):
@@ -101,11 +181,11 @@ def hub(rng, budget_s):
         tout = out[(np.searchsorted(out, tin) + rng.integers(1, len(out), size=q)) % len(out)]
         return tin.astype(np.int64), tout.astype(np.int64)
 
-    run(p, "hub", n, pick, lambda tin, tout: 1e-3 * 1e4 / nu[tin], budget_s)
+    run(p, "hub", n, pick, lambda tin, tout: 1e-3 * 1e4 / nu[tin], budget_s, kind, sizes)
     p.close()
 
 
-def headline(rng, budget_s):
+def headline(rng, budget_s, kind="in", sizes=(8, 64, 256)):
     m, n = 10_000_000, 50_000
     R, g, Ai = synth.product_pools(m, n, seed=1234)
     p = cr.DevicePools(n)
@@ -122,7 +202,7 @@ def headline(rng, budget_s):
         side = rng.integers(0, 2, size=q)
         return Ai[sel, side].astype(np.int64), Ai[sel, 1 - side].astype(np.int64)
 
-    run(p, "headline", n, pick, lambda tin, tout: 1e-3 * depth[tin], budget_s)
+    run(p, "headline", n, pick, lambda tin, tout: 1e-3 * depth[tin], budget_s, kind, sizes)
     p.close()
 
 
@@ -130,13 +210,16 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--only", choices=["hub", "headline"])
     ap.add_argument("--budget-s", type=float, default=20.0)
+    ap.add_argument("--kind", choices=["in", "out", "mixed"], default="in")
+    ap.add_argument("--B", default="8,64,256", help="mask sizes, comma-separated")
     args = ap.parse_args()
+    sizes = tuple(int(x) for x in args.B.split(","))
     emit(card=card())
     rng = np.random.default_rng(2029)
     if args.only in (None, "hub"):
-        hub(rng, args.budget_s)
+        hub(rng, args.budget_s, args.kind, sizes)
     if args.only in (None, "headline"):
-        headline(rng, args.budget_s)
+        headline(rng, args.budget_s, args.kind, sizes)
 
 
 if __name__ == "__main__":
