@@ -40,7 +40,7 @@ PATH_REPEATS_POOL = 4
 # cfmm_quote_subgraph_(swap_)orders / cfmm_execute_subgraph_(swap_)orders
 SUBGRAPH_MAX_TOKENS = 256
 ORDER_NOT_CONVERGED = 5
-# cfmm_quote_basket_orders / cfmm_execute_basket_orders
+# cfmm_quote_basket_(swap_)orders / cfmm_execute_basket_(swap_)orders
 BASKET_MAX_TOKENS = 16
 
 COMM_HANDLE_BYTES = 128
@@ -149,6 +149,11 @@ SYMBOLS = {
                                            C.POINTER(SubgraphOpts), C.POINTER(BasketOut)]),
     "cfmm_execute_basket_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, _dp, _dp, C.POINTER(C.c_uint8),
                                              C.POINTER(SubgraphOpts), C.POINTER(BasketOut)]),
+    "cfmm_quote_basket_swap_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, C.POINTER(C.c_uint8), _dp,
+                                                C.POINTER(C.c_uint8), C.POINTER(SubgraphOpts), C.POINTER(BasketOut)]),
+    "cfmm_execute_basket_swap_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, C.POINTER(C.c_uint8), _dp, _dp,
+                                                  C.POINTER(C.c_uint8), C.POINTER(SubgraphOpts),
+                                                  C.POINTER(BasketOut)]),
     "cfmm_modify_univ3_liquidity":(C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),

@@ -18,15 +18,26 @@
 // The basket tokens' slot pairs ({b_k, s} and its activity, K·nB entries each) live in dynamic shared
 // memory (bk_dyn_bytes).  basket_plan_kernel runs the setup only and reports each row's token and pool
 // counts, which size the outputs and the workspace.
+//
+// basket_buy_kernel runs buy rows: rows whose entries include at least one bought entry (kind
+// CFMM_SWAP_EXACT_OUT: buy y_l of b_l).  It is the same row with BUY set at compile time: the local
+// order is the bought entries, then i, then the sold entries, then B ∩ T; lin is δ_k at sold and
+// −y′_l = −y_l·(1 + rtol) (rounded up) at bought entries; ν_i is fixed at 1 and every other slot has
+// ν_t >= √eps; the start prices from i's slot; the stop adds a term per bought entry; and a bought
+// entry's capacity is checked before the solve (sg_capacity at its slot).  One bought entry and no
+// sold entries give subgraph_out_kernel's outputs bit for bit.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "subgraph_kernels.cuh"
 
 namespace cfmm {
 
 constexpr int kBasketMaxTokens = 16;  // CFMM_BASKET_MAX_TOKENS
+constexpr uint8_t kBasketBought = 1;  // CFMM_SWAP_EXACT_OUT, the kind of a bought entry
 
 // The rows of one call, their options, and their outputs (device arrays; tokens 1-based).
 struct BasketRows {
@@ -79,6 +90,38 @@ struct BasketSmem {
   int changed;
 };
 
+// A buy row's shared state: the basket row's, plus the entries' kinds (in the caller's order, staged by
+// basket_buy_kernel), lin per entry and the count of bought entries in T (their local slots
+// 0 .. nout − 1; i's slot is nout).  bamt and blin are indexed by entry in local order, i skipped.
+struct BasketBuySmem : BasketSmem {
+  double blin[kBasketMaxTokens];
+  uint8_t bkind[kBasketMaxTokens];
+  int32_t nout;
+};
+template <bool BUY>
+using BkSmem = std::conditional_t<BUY, BasketBuySmem, BasketSmem>;
+
+// The local slot of entry k (in local order, i skipped), and i's slot.
+template <bool BUY>
+__device__ __forceinline__ int bk_slot(const BkSmem<BUY>& m, int k) {
+  if constexpr (BUY)
+    return k < m.nout ? k : k + 1;
+  else
+    return k + 1;
+}
+template <bool BUY>
+__device__ __forceinline__ int bk_root(const BkSmem<BUY>& m) {
+  if constexpr (BUY)
+    return m.nout;
+  else
+    return 0;
+}
+// The box of slot t: basket rows that of Swap (sg_lower); buy rows ν_i = 1 (bk_fixed) and ν_t >= √eps.
+template <bool BUY>
+__device__ __forceinline__ double bk_lo(int t) { return BUY ? kSubgraphSqrtEps : sg_lower(t); }
+template <bool BUY>
+__device__ __forceinline__ bool bk_fixed(const BkSmem<BUY>& m, int t) { return BUY && t == bk_root<BUY>(m); }
+
 // The dynamic shared memory of a call whose longest basket has K entries: {b_k, s} and its activity.
 __host__ __device__ __forceinline__ size_t bk_dyn_bytes(int K, int nB) {
   return ((size_t)K * (size_t)nB * 5 + 7) & ~(size_t)7;
@@ -99,12 +142,14 @@ __device__ __forceinline__ int32_t bk_pair(AdjView A, int32_t a, int32_t b) {
   return lo < a1 && A.nbr[lo] == b ? A.pair[lo] : -1;
 }
 
-// Setup of the row selling btok[0 .. K) (1-based) for i (0-based): T, the local tokens and the pool
+// Setup of the row trading btok[0 .. K) (1-based) for i (0-based): T, the local tokens and the pool
 // count of every slot (cnt[s], the pools of the pairs {s, i}, {s, b_k} for b_k ∈ T, and {s, u} for
-// slots u > s in T) and of the pairs among i and the basket tokens in T (basket_cnt).
+// slots u > s in T) and of the pairs among i and the basket tokens in T (basket_cnt).  BUY: the local
+// order puts the bought entries (m.bkind) before i; the counts are the same.
+template <bool BUY>
 __device__ void bk_setup(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
                          const uint8_t* __restrict__ gact, const int64_t* __restrict__ btok, int K, int32_t i,
-                         BasketSmem& m) {
+                         BkSmem<BUY>& m) {
   const int tid = threadIdx.x, nB = G.nB;
   int32_t* bpair = reinterpret_cast<int32_t*>(bk_dyn);  // [K][nB]
   uint8_t* bact = bk_dyn + (size_t)4 * K * nB;          // [K][nB]
@@ -198,15 +243,34 @@ __device__ void bk_setup(const PathSets* P, PairIndexView ix, AdjView A, const B
   __syncthreads();
   if (tid == 0) {
     int loc = 1;
-    m.ltok[0] = i;
     int32_t tot = 0;
-    for (int k = 0; k < K; ++k) {
-      m.bloc[k] = -1;
-      if (!m.bin[k]) continue;
-      m.bloc[k] = (int8_t)loc;
-      m.ltok[loc++] = m.btok[k];
-      for (int l = k; l < K; ++l)
-        if (m.bin[l]) tot += pools(m.kpair[k][l]);
+    if constexpr (BUY) {
+      // the bought entries in T in the caller's order, then i, then the sold entries in T
+      loc = 0;
+      for (int pass = 0; pass < 2; ++pass) {
+        if (pass == 1) {
+          m.nout = loc;
+          m.ltok[loc++] = i;
+        }
+        for (int k = 0; k < K; ++k) {
+          if (pass == 0) m.bloc[k] = -1;
+          if (!m.bin[k] || (m.bkind[k] == kBasketBought) != (pass == 0)) continue;
+          m.bloc[k] = (int8_t)loc;
+          m.ltok[loc++] = m.btok[k];
+          for (int l = k; l < K; ++l)
+            if (m.bin[l]) tot += pools(m.kpair[k][l]);
+        }
+      }
+    } else {
+      m.ltok[0] = i;
+      for (int k = 0; k < K; ++k) {
+        m.bloc[k] = -1;
+        if (!m.bin[k]) continue;
+        m.bloc[k] = (int8_t)loc;
+        m.ltok[loc++] = m.btok[k];
+        for (int l = k; l < K; ++l)
+          if (m.bin[l]) tot += pools(m.kpair[k][l]);
+      }
     }
     m.nin = loc - 1;
     for (int s = 0; s < nB; ++s)
@@ -227,10 +291,16 @@ __device__ void bk_setup(const PathSets* P, PairIndexView ix, AdjView A, const B
   __syncthreads();
 }
 
-__device__ __forceinline__ int32_t bk_local(const BestPathGraph& G, const BasketSmem& m, int32_t t) {
-  if (t == m.ltok[0]) return 0;
-  for (int k = 1; k <= m.nin; ++k)
-    if (t == m.ltok[k]) return k;
+template <bool BUY>
+__device__ __forceinline__ int32_t bk_local(const BestPathGraph& G, const BkSmem<BUY>& m, int32_t t) {
+  if constexpr (BUY) {
+    for (int k = 0; k <= m.nin; ++k)  // i and the entries in T
+      if (t == m.ltok[k]) return k;
+  } else {
+    if (t == m.ltok[0]) return 0;
+    for (int k = 1; k <= m.nin; ++k)
+      if (t == m.ltok[k]) return k;
+  }
   return m.lidx[G.slot_of[t]];
 }
 
@@ -243,7 +313,8 @@ __global__ void __launch_bounds__(kSubgraphThreads)
   __shared__ BasketSmem m;
   for (int64_t r = blockIdx.x; r < q; r += gridDim.x) {
     const int64_t b0 = basket_off[r];
-    bk_setup(P, ix, A, G, gact, basket_token + b0, (int)(basket_off[r + 1] - b0), (int32_t)(token_out[r] - 1), m);
+    bk_setup<false>(P, ix, A, G, gact, basket_token + b0, (int)(basket_off[r + 1] - b0), (int32_t)(token_out[r] - 1),
+                    m);
     if (threadIdx.x == 0) {
       ntok[r] = m.n_loc;
       npool[r] = m.npool;
@@ -252,16 +323,19 @@ __global__ void __launch_bounds__(kSubgraphThreads)
   }
 }
 
-// Σ_k δ_k·v_k over the basket tokens in T, in basket order (the first term alone, not 0.0 + it).
-__device__ __forceinline__ double bk_value(const BasketSmem& m, const double* v) {
-  double s = __dmul_rn(m.bamt[0], v[1]);
-  for (int k = 1; k < m.nin; ++k) s = __dadd_rn(s, __dmul_rn(m.bamt[k], v[1 + k]));
+// Σ_k c_k·v_k over the entries in T, in local order (the first term alone, not 0.0 + it).  c = bamt:
+// V (basket rows: δ in basket order); c = blin: a buy row's linear term.
+template <bool BUY>
+__device__ __forceinline__ double bk_value(const BkSmem<BUY>& m, const double* c, const double* v) {
+  double s = __dmul_rn(c[0], v[bk_slot<BUY>(m, 0)]);
+  for (int k = 1; k < m.nin; ++k) s = __dadd_rn(s, __dmul_rn(c[k], v[bk_slot<BUY>(m, k)]));
   return s;
 }
 
 // One evaluation at ν = xt: every pool's contributions, Ψ_t -> pt, gt = lin + Ψ, and the dual's
 // value linᵀxt + Σ val (returned to every thread).
-__device__ double bk_evaluate(const PathSets* P, const SubgraphWork& w, BasketSmem& m) {
+template <bool BUY>
+__device__ double bk_evaluate(const PathSets* P, const SubgraphWork& w, BkSmem<BUY>& m) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int64_t np = m.npool;
   double vs = 0.0;
@@ -284,17 +358,25 @@ __device__ double bk_evaluate(const PathSets* P, const SubgraphWork& w, BasketSm
     for (int o = 16; o >= 1; o >>= 1) s = __dadd_rn(s, __shfl_xor_sync(kFull, s, o));
     if (lane == 0) {
       m.pt[t] = s;
-      m.gt[t] = __dadd_rn(t >= 1 && t <= m.nin ? m.bamt[t - 1] : 0.0, s);
+      if constexpr (BUY)
+        m.gt[t] = __dadd_rn(t == m.nout || t > m.nin ? 0.0 : m.blin[t < m.nout ? t : t - 1], s);
+      else
+        m.gt[t] = __dadd_rn(t >= 1 && t <= m.nin ? m.bamt[t - 1] : 0.0, s);
     }
   }
   __syncthreads();
-  return __dadd_rn(bk_value(m, m.xt), V);
+  if constexpr (BUY)
+    return __dadd_rn(bk_value<BUY>(m, m.blin, m.xt), V);
+  else
+    return __dadd_rn(bk_value<BUY>(m, m.bamt, m.xt), V);
 }
 
 // Accept xt: (s, y) into history slot `slot` when store, x <- xt, g <- gt, Ψ, the projected gradient
 // and the Gram matrix of [S Y pg] (one warp per entry group, lanes over the tokens, butterfly).
-// Returns m_r = max_t ν_t·|pg_t| / Σ_k δ_k·ν_k.
-__device__ double bk_commit(BasketSmem& m, int slot, bool store) {
+// Returns m_r = max_t ν_t·|pg_t| / V, V = Σ_k amount_k·ν_k (y, not y′, at bought entries); a buy
+// row's m_r is at least ν_l·|pg_l| / (y_l·ν_l) for every bought entry with y_l > 0.
+template <bool BUY>
+__device__ double bk_commit(BkSmem<BUY>& m, int slot, bool store) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = m.n_loc;
   if (tid == 0) m.mx = 0ull;
   for (int t = tid; t < n; t += blockDim.x) {
@@ -306,7 +388,7 @@ __device__ double bk_commit(BasketSmem& m, int slot, bool store) {
     m.x[t] = xn;
     m.g[t] = gn;
     m.px[t] = m.pt[t];
-    m.pg[t] = xn <= sg_lower(t) && gn > 0.0 ? 0.0 : gn;
+    m.pg[t] = bk_fixed<BUY>(m, t) || (xn <= bk_lo<BUY>(t) && gn > 0.0) ? 0.0 : gn;
   }
   __syncthreads();
   double mx = 0.0;
@@ -326,36 +408,66 @@ __device__ double bk_commit(BasketSmem& m, int slot, bool store) {
     if (lane == 0) m.W[r][c] = m.W[c][r] = s;
   }
   __syncthreads();
-  return __ddiv_rn(__longlong_as_double((long long)m.mx), bk_value(m, m.x));
+  double mr = __ddiv_rn(__longlong_as_double((long long)m.mx), bk_value<BUY>(m, m.bamt, m.x));
+  if constexpr (BUY) {
+    for (int l = 0; l < m.nout; ++l)
+      if (m.bamt[l] > 0.0)
+        mr = fmax(mr, __ddiv_rn(__dmul_rn(m.x[l], fabs(m.pg[l])), __dmul_rn(m.bamt[l], m.x[l])));
+  }
+  return mr;
 }
 
 // Row r on the current state.  Returns nothing; writes the row's outputs.  EXEC: the limit decides,
-// and a filled row applies the transition of cfmm_apply_trades at its ν to each of its pools.
-template <bool EXEC>
+// and a filled row applies the transition of cfmm_apply_trades at its ν to each of its pools.  BUY:
+// a buy row (its entries' kinds in m.bkind): the dual has lin = δ_k at sold and −y′_l at bought
+// entries and ν_i fixed at 1; a bought entry with y_l at least what the row's pools holding b_l could
+// pay out makes the row unreachable, and a row fills only when every bought entry with y_l > 0
+// receives at least y_l.
+template <bool EXEC, bool BUY = false>
 __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
                              const uint8_t* gact, const BasketRows& R, const SubgraphWork& w, const SplitMoved& mv,
-                             int64_t r, BasketSmem& m) {
+                             int64_t r, BkSmem<BUY>& m) {
   __shared__ LbfgsHistory hist;
   __shared__ double s_f, s_t, s_merit;
   __shared__ int s_state, s_status, s_iter, s_fev, s_small, s_any, s_unreach;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int64_t b0 = R.basket_off[r];
-  bk_setup(P, ix, A, G, gact, R.basket_token + b0, (int)(R.basket_off[r + 1] - b0), (int32_t)(R.token_out[r] - 1),
-           m);
+  bk_setup<BUY>(P, ix, A, G, gact, R.basket_token + b0, (int)(R.basket_off[r + 1] - b0),
+                (int32_t)(R.token_out[r] - 1), m);
   const int64_t np = m.npool, n = m.n_loc;
   // the amounts of the basket tokens in T; a positive amount outside T makes the row unreachable
-  if (tid == 0) {
-    int any = 0, unreach = 0;
-    for (int k = 0; k < m.nK; ++k) {
-      const double a = R.basket_amount[b0 + k];
-      any |= a > 0.0;
-      if (m.bloc[k] >= 0)
-        m.bamt[m.bloc[k] - 1] = a;
-      else
-        unreach |= a > 0.0;
+  if constexpr (BUY) {
+    // bamt and blin by entry in local order (i skipped): δ and δ at sold, y and −y′ at bought entries
+    if (tid == 0) {
+      int any = 0, unreach = 0;
+      for (int k = 0; k < m.nK; ++k) {
+        const double a = R.basket_amount[b0 + k];
+        any |= a > 0.0;
+        if (m.bloc[k] >= 0) {
+          const int e = m.bloc[k] < m.nout ? m.bloc[k] : m.bloc[k] - 1;
+          m.bamt[e] = a;
+          m.blin[e] = m.bkind[k] == kBasketBought ? -__fma_ru(a, R.rtol, a) : a;
+        } else {
+          unreach |= a > 0.0;
+        }
+      }
+      s_any = any;
+      s_unreach = unreach;
     }
-    s_any = any;
-    s_unreach = unreach;
+  } else {
+    if (tid == 0) {
+      int any = 0, unreach = 0;
+      for (int k = 0; k < m.nK; ++k) {
+        const double a = R.basket_amount[b0 + k];
+        any |= a > 0.0;
+        if (m.bloc[k] >= 0)
+          m.bamt[m.bloc[k] - 1] = a;
+        else
+          unreach |= a > 0.0;
+      }
+      s_any = any;
+      s_unreach = unreach;
+    }
   }
   // the pools: those among i and the basket first, then each slot's, at the offsets the setup counted
   if (tid == 0 && m.basket_cnt > 0) {
@@ -421,8 +533,8 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
     const int64_t en = w.ent[e];
     const int k = (int)(en >> kPairSetShift);
     const int2 a = P->Ai[k][en & kPairPosMask];
-    w.ta[e] = bk_local(G, m, a.x);
-    w.tb[e] = bk_local(G, m, a.y);
+    w.ta[e] = bk_local<BUY>(G, m, a.x);
+    w.tb[e] = bk_local<BUY>(G, m, a.y);
   }
   __syncthreads();
   // incidence lists in pool order: one warp per token, a ballot per 32 pools (count, then fill)
@@ -451,6 +563,22 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
     }
   }
   __syncthreads();
+  // buy rows: the capacity of each bought entry over the row's pools, once, before any solve; a
+  // shortfall makes the row unreachable
+  if constexpr (BUY) {
+    if (s_any && !s_unreach) {
+      bool short_cap = false;
+      for (int l = 0; l < m.nout; ++l) {
+        const double y = m.bamt[l];
+        if (!(y > 0.0)) continue;
+        double c = 0.0;
+        for (int64_t e = tid; e < np; e += blockDim.x) c = __dadd_rn(c, sg_capacity(P, w, e, l));
+        short_cap |= y >= sg_cta_sum(c, m);
+      }
+      if (tid == 0 && short_cap) s_unreach = 1;
+      __syncthreads();
+    }
+  }
   // the solve
   const bool any = s_any, solve = any && !s_unreach;
   double f = 0.0, merit = 0.0;
@@ -462,9 +590,12 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
   if (solve) {
     for (int t = tid; t < n; t += blockDim.x)  // an empty history, as cfmm_solve's zeroed one
       for (int a = 0; a < kSolverM; ++a) m.S[a][t] = m.Y[a][t] = 0.0;
-    sg_start(P, w, m);
-    f = bk_evaluate(P, w, m);
-    merit = bk_commit(m, 0, false);
+    if constexpr (BUY)
+      sg_start<BasketBuySmem, true>(P, w, m, bk_root<BUY>(m));
+    else
+      sg_start(P, w, m);
+    f = bk_evaluate<BUY>(P, w, m);
+    merit = bk_commit<BUY>(m, 0, false);
     if (tid == 0) {
       s_fev = 1;
       s_f = f;
@@ -491,7 +622,7 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
           v = fma(m.c[a], m.S[a][t], v);
           v = fma(m.c[kSolverM + a], m.Y[a][t], v);
         }
-        m.d[t] = m.x[t] <= sg_lower(t) && m.g[t] > 0.0 ? 0.0 : -v;
+        m.d[t] = bk_fixed<BUY>(m, t) || (m.x[t] <= bk_lo<BUY>(t) && m.g[t] > 0.0) ? 0.0 : -v;
       }
       __syncthreads();
       int dec = kLsRetry;
@@ -500,14 +631,14 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
         const double t = s_t;
         double gd = 0.0, st2 = 0.0;
         for (int k = tid; k < n; k += blockDim.x) {
-          const double y = fmax(fma(t, m.d[k], m.x[k]), sg_lower(k));
+          const double y = bk_fixed<BUY>(m, k) ? 1.0 : fmax(fma(t, m.d[k], m.x[k]), bk_lo<BUY>(k));
           m.xt[k] = y;
           const double dx = __dsub_rn(y, m.x[k]);
           gd = fma(m.g[k], dx, gd);
           st2 = fma(dx, dx, st2);
         }
         const double gdx = sg_cta_sum(gd, m), step2 = sg_cta_sum(st2, m);
-        f_new = bk_evaluate(P, w, m);
+        f_new = bk_evaluate<BUY>(P, w, m);
         if (tid == 0) {
           ++s_fev;
           double tn = s_t;
@@ -534,7 +665,7 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
         continue;
       }
       const int slot = hist.head;
-      const double mr = bk_commit(m, slot, true);
+      const double mr = bk_commit<BUY>(m, slot, true);
       if (tid == 0) {
         lbfgs_store(m.W, slot, hist);
         ++s_iter;
@@ -551,7 +682,7 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
     merit = s_merit;
   }
   // status, the limit, the legs (and the transition on execute)
-  const double received = solve ? m.px[0] : 0.0;
+  const double received = solve ? m.px[bk_root<BUY>(m)] : 0.0;
   uint8_t st = 0;  // CFMM_ORDER_FILLED (amounts all 0: zeros, no solve)
   if (any) {
     if (s_unreach)
@@ -559,7 +690,13 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
     else if (status != 0)
       st = 5;  // CFMM_ORDER_NOT_CONVERGED
     else if (EXEC && R.limit && received < R.limit[r])
-      st = 1;  // CFMM_ORDER_LIMIT; an equal limit fills
+      st = 1;  // CFMM_ORDER_LIMIT; an equal limit fills (buy rows: received may be negative)
+  }
+  if constexpr (BUY) {
+    // a converged buy row short of a bought y_l > 0 is not converged, whatever its limit
+    if (solve && status == 0)
+      for (int l = 0; l < m.nout; ++l)
+        if (m.bamt[l] > 0.0 && !(m.px[l] >= m.bamt[l])) st = 5;
   }
   const bool filled = st == 0 && solve;
   const int64_t l0 = R.leg_off[r];
@@ -590,7 +727,7 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
   __syncthreads();  // the next row reuses the shared state and the workspace
 }
 
-// Rows rows[0 .. n) (null: 0 .. n), one CTA at a time each; CTA b uses workspace b.
+// Sell-only rows rows[0 .. n) (null: 0 .. n), one CTA at a time each; CTA b uses workspace b.
 template <bool EXEC>
 __global__ void __launch_bounds__(kSubgraphThreads)
     basket_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, BestPathGraph G,
@@ -608,6 +745,22 @@ __global__ void __launch_bounds__(kSubgraphThreads)
   wb.cb += c;
   for (int64_t k = blockIdx.x; k < n; k += gridDim.x)
     basket_row<EXEC>(P, ix, A, G, gact, R, wb, mv, rows ? rows[k] : k, m);
+}
+
+// Buy rows rows[0 .. n), as basket_kernel; kind [basket_off[q]] holds every entry's kind.
+template <bool EXEC>
+__global__ void __launch_bounds__(kSubgraphThreads)
+    basket_buy_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, BestPathGraph G,
+                      const uint8_t* __restrict__ gact, BasketRows R, const uint8_t* __restrict__ kind, SubgraphWork w,
+                      SplitMoved mv, const int64_t* __restrict__ rows, int64_t n) {
+  __shared__ BasketBuySmem m;
+  const SubgraphWork wb = sg_cta_work(w);
+  for (int64_t k = blockIdx.x; k < n; k += gridDim.x) {
+    const int64_t r = rows[k], b0 = R.basket_off[r];
+    // (the previous row ended at a barrier, and the setup's barriers publish these before any read)
+    if (threadIdx.x < R.basket_off[r + 1] - b0) m.bkind[threadIdx.x] = kind[b0 + threadIdx.x];
+    basket_row<EXEC, true>(P, ix, A, G, gact, R, wb, mv, r, m);
+  }
 }
 
 }  // namespace cfmm

@@ -3975,9 +3975,16 @@ int check_subgraph(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int6
   return CFMM_OK;
 }
 
-// Every argument of cfmm_quote_basket_orders / cfmm_execute_basket_orders, before anything runs.
+// Whether row r of a basket call is a buy row: at least one entry of kind CFMM_SWAP_EXACT_OUT.
+bool basket_buy_row(const int64_t* basket_off, const uint8_t* kind, int64_t r) {
+  return kind && std::find(kind + basket_off[r], kind + basket_off[r + 1], (uint8_t)CFMM_SWAP_EXACT_OUT) !=
+                     kind + basket_off[r + 1];
+}
+
+// Every argument of cfmm_quote/execute_basket_orders (kind null) and cfmm_quote/execute_basket_swap_orders,
+// before anything runs.
 int check_basket(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
-                 const int64_t* basket_token, const double* basket_amount, const double* limit,
+                 const int64_t* basket_token, const uint8_t* kind, const double* basket_amount, const double* limit,
                  const uint8_t* allowed, const cfmm_subgraph_opts& o, const char* what) {
   int rc = check_row_opts(ctx, q, allowed, o, what);
   if (rc != CFMM_OK || q == 0) return rc;
@@ -4009,12 +4016,21 @@ int check_basket(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64
                       (long long)t);
       if (!std::isfinite(a) || a < 0.0)
         return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: amount %g must be finite and >= 0", what, (long long)r, a);
+      if (kind && kind[k] > CFMM_SWAP_EXACT_OUT)
+        return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: entry kind %d is neither 0 (sold) nor 1 (bought)", what,
+                    (long long)r, (int)kind[k]);
       n_other += allowed[t - 1] == 0;
     }
     if (n_other > CFMM_SUBGRAPH_MAX_TOKENS + 1)
       return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: %lld tokens besides token_out, more than %d", what,
                   (long long)r, (long long)n_other, CFMM_SUBGRAPH_MAX_TOKENS + 1);
-    if ((rc = check_limit(ctx, limit, r, what)) != CFMM_OK) return rc;
+    if (basket_buy_row(basket_off, kind, r)) {  // the minimum net of token_out: negative and −inf allowed
+      if (limit && !(limit[r] < INFINITY))
+        return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: buy-row limit %g must not be NaN or +inf", what,
+                    (long long)r, limit[r]);
+    } else if ((rc = check_limit(ctx, limit, r, what)) != CFMM_OK) {
+      return rc;
+    }
   }
   return CFMM_OK;
 }
@@ -4250,8 +4266,9 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
   return CFMM_OK;
 }
 
+// kind null: every row sell-only (cfmm_quote/execute_basket_orders).
 int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, const int64_t* basket_off,
-                  const int64_t* basket_token, const double* basket_amount, const double* limit,
+                  const int64_t* basket_token, const uint8_t* kind, const double* basket_amount, const double* limit,
                   const uint8_t* allowed, const cfmm_subgraph_opts& o, const cfmm_basket_out& O, const char* what) {
   int rc;
   CU_TRY(ctx, cudaSetDevice(ctx->device));
@@ -4275,10 +4292,11 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
   DevBuf<int64_t> d_out, d_boff, d_btok, d_ntok, d_npool;
   DevBuf<int32_t> d_tok, d_slot, d_deg, d_gpair;
   DevBuf<int16_t> d_gnbr;
-  DevBuf<uint8_t> d_act;
+  DevBuf<uint8_t> d_act, d_kind;
   DevBuf<double> d_bamt, d_limit;
   CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
   CU_TRY(ctx, d_boff.upload(basket_off, (size_t)q + 1));
+  if (kind) CU_TRY(ctx, d_kind.upload(kind, (size_t)NE));
   CU_TRY(ctx, d_btok.upload(basket_token, (size_t)NE));
   CU_TRY(ctx, d_bamt.upload(basket_amount, (size_t)NE));
   CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
@@ -4309,7 +4327,25 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
                                                               cfmm::kSubgraphThreads, (size_t)most));
     if (occ < 1) return fail(ctx, CFMM_ERR_CUDA, "basket_kernel does not fit on an SM");
   }
-  const int64_t wave = (int64_t)ctx->sm_count * occ;
+  // buy rows run basket_buy_kernel (sized the same way, once per context, when a call first has them)
+  int64_t n_buy = 0;
+  for (int64_t r = 0; r < q; ++r) n_buy += basket_buy_row(basket_off, kind, r);
+  if (n_buy == 0) kind = nullptr;  // every row sell-only: the path of cfmm_quote/execute_basket_orders
+  int occ_buy = 0;
+  if (n_buy > 0) {
+    int& ob = ctx->occupancy[reinterpret_cast<const void*>(&cfmm::basket_buy_kernel<false>)];
+    if (ob == 0) {
+      const int most = (int)cfmm::bk_dyn_bytes(cfmm::kBasketMaxTokens, cfmm::kSubgraphSlots);
+      for (const void* f : {reinterpret_cast<const void*>(&cfmm::basket_buy_kernel<false>),
+                            reinterpret_cast<const void*>(&cfmm::basket_buy_kernel<true>)})
+        CU_TRY(ctx, cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+      CU_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ob, cfmm::basket_buy_kernel<false>,
+                                                                cfmm::kSubgraphThreads, (size_t)most));
+      if (ob < 1) return fail(ctx, CFMM_ERR_CUDA, "basket_buy_kernel does not fit on an SM");
+    }
+    occ_buy = ob;
+  }
+  const int64_t wave = (int64_t)ctx->sm_count * occ, wave_buy = (int64_t)ctx->sm_count * occ_buy;
   const unsigned plan_grid = (unsigned)std::min<int64_t>(q, wave);
   if ((rc = launch(ctx, kProfSwaps, nB > 0 ? 3 : 1, [&] {
          if (nB > 0) {
@@ -4371,7 +4407,7 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
   }
   int64_t cap = 1;
   while (cap < max_pool) cap <<= 1;
-  const int64_t grid = std::min<int64_t>(q, wave);
+  const int64_t grid = std::min<int64_t>(q, std::max(wave, wave_buy));  // the workspaces
   DevBuf<int64_t> w64;
   DevBuf<int32_t> w32;
   DevBuf<double> wd;
@@ -4384,13 +4420,34 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
                        o.rtol,      o.factr,    d_tok_off.p, d_leg_off.p, d_paid.p, d_recv.p,   d_status.p,
                        d_sst.p,     d_iter.p,   d_fev.p,    d_merit.p, d_token.p, d_nu.p,     d_psi.p,
                        d_entry.p,   d_ld.p,     d_ll.p};
+  // rows[0 .. n_sell) sell-only, rows[n_sell .. n) buy rows: one launch of each kernel that has rows
+  const auto run = [&](auto exec_tag, const cfmm::PathSets* P, const cfmm::SplitMoved& mv, const int64_t* rows,
+                       int64_t n_sell, int64_t n) {
+    constexpr bool X = decltype(exec_tag)::value;
+    return launch(ctx, kProfSwaps, (n_sell > 0) + (n > n_sell), [&] {
+      if (n_sell > 0)
+        cfmm::basket_kernel<X><<<(unsigned)std::min(n_sell, wave), cfmm::kSubgraphThreads, dyn, st>>>(
+            P, pv, A, G, d_act.p, R, W, mv, rows, n_sell);
+      if (n > n_sell)
+        cfmm::basket_buy_kernel<X><<<(unsigned)std::min(n - n_sell, wave_buy), cfmm::kSubgraphThreads, dyn, st>>>(
+            P, pv, A, G, d_act.p, R, d_kind.p, W, mv, rows + n_sell, n - n_sell);
+    });
+  };
+  const auto sell_only = [&](int64_t r) { return !basket_buy_row(basket_off, kind, r); };
   OrderSets xs;
-  if (!exec) {
+  if (!exec && !kind) {
     if ((rc = launch(ctx, kProfSwaps, 1, [&] {
            cfmm::basket_kernel<false><<<(unsigned)grid, cfmm::kSubgraphThreads, dyn, st>>>(
                os.d_P.p, pv, A, G, d_act.p, R, W, cfmm::SplitMoved{}, nullptr, q);
          })) != CFMM_OK)
       return rc;
+  } else if (!exec) {
+    std::vector<int64_t> rows((size_t)q);
+    std::iota(rows.begin(), rows.end(), (int64_t)0);
+    std::stable_partition(rows.begin(), rows.end(), sell_only);
+    DevBuf<int64_t> d_rows;
+    CU_TRY(ctx, d_rows.upload(rows));
+    if ((rc = run(std::false_type{}, os.d_P.p, cfmm::SplitMoved{}, d_rows.p, q - n_buy, q)) != CFMM_OK) return rc;
   } else {
     if ((rc = order_sets(ctx, true, xs)) != CFMM_OK) return rc;
     ctx->state_version++;
@@ -4406,10 +4463,22 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
           for (int32_t t : tok) visit(0, t);
         },
         order, level_off);
+    // a level's rows share no token, so their order does not matter: its sell-only rows go first
+    std::vector<int64_t> level_sell(level_off.size(), 0);
+    for (size_t Lv = 1; kind && Lv < level_off.size(); ++Lv) {
+      const auto b = order.begin() + level_off[Lv - 1], e = order.begin() + level_off[Lv];
+      level_sell[Lv] = std::stable_partition(b, e, sell_only) - b;
+    }
     DevBuf<int64_t> d_order;
     CU_TRY(ctx, d_order.upload(order));
     for (size_t Lv = 1; Lv < level_off.size(); ++Lv) {
       const int64_t n = level_off[Lv] - level_off[Lv - 1];
+      if (kind) {
+        if ((rc = run(std::true_type{}, xs.d_P.p, xs.mv, d_order.p + level_off[Lv - 1], level_sell[Lv], n)) !=
+            CFMM_OK)
+          return rc;
+        continue;
+      }
       if ((rc = launch(ctx, kProfSwaps, 1, [&] {
              cfmm::basket_kernel<true><<<(unsigned)std::min<int64_t>(n, grid), cfmm::kSubgraphThreads, dyn, st>>>(
                  xs.d_P.p, pv, A, G, d_act.p, R, W, xs.mv, d_order.p + level_off[Lv - 1], n);
@@ -4457,10 +4526,10 @@ cfmm_subgraph_opts subgraph_opts(const cfmm_subgraph_opts* in) {
 }
 
 int basket_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, const int64_t* basket_off,
-                const int64_t* basket_token, const double* basket_amount, const double* limit, const uint8_t* allowed,
-                const cfmm_subgraph_opts* opts, cfmm_basket_out* out, const char* what) {
+                const int64_t* basket_token, const uint8_t* kind, const double* basket_amount, const double* limit,
+                const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_basket_out* out, const char* what) {
   const cfmm_subgraph_opts o = subgraph_opts(opts);
-  int rc = check_basket(ctx, q, token_out, basket_off, basket_token, basket_amount, limit, allowed, o, what);
+  int rc = check_basket(ctx, q, token_out, basket_off, basket_token, kind, basket_amount, limit, allowed, o, what);
   if (rc != CFMM_OK) return rc;
   if (q == 0) {
     if (out && out->tok_off) out->tok_off[0] = 0;
@@ -4468,7 +4537,7 @@ int basket_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, c
     return CFMM_OK;
   }
   const cfmm_basket_out none{};
-  return basket_orders(ctx, exec, q, token_out, basket_off, basket_token, basket_amount, limit, allowed, o,
+  return basket_orders(ctx, exec, q, token_out, basket_off, basket_token, kind, basket_amount, limit, allowed, o,
                        out ? *out : none, what);
 }
 
@@ -4517,15 +4586,30 @@ int cfmm_execute_subgraph_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_
 int cfmm_quote_basket_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
                              const int64_t* basket_token, const double* basket_amount, const uint8_t* allowed,
                              const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
-  return basket_call(ctx, false, q, token_out, basket_off, basket_token, basket_amount, nullptr, allowed, opts, out,
-                     "quote_basket_orders");
+  return basket_call(ctx, false, q, token_out, basket_off, basket_token, nullptr, basket_amount, nullptr, allowed,
+                     opts, out, "quote_basket_orders");
 }
 
 int cfmm_execute_basket_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
                                const int64_t* basket_token, const double* basket_amount, const double* limit,
                                const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
-  return basket_call(ctx, true, q, token_out, basket_off, basket_token, basket_amount, limit, allowed, opts, out,
-                     "execute_basket_orders");
+  return basket_call(ctx, true, q, token_out, basket_off, basket_token, nullptr, basket_amount, limit, allowed,
+                     opts, out, "execute_basket_orders");
+}
+
+int cfmm_quote_basket_swap_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                                  const int64_t* basket_token, const uint8_t* entry_kind, const double* basket_amount,
+                                  const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
+  return basket_call(ctx, false, q, token_out, basket_off, basket_token, entry_kind, basket_amount, nullptr, allowed,
+                     opts, out, "quote_basket_swap_orders");
+}
+
+int cfmm_execute_basket_swap_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                                    const int64_t* basket_token, const uint8_t* entry_kind,
+                                    const double* basket_amount, const double* limit, const uint8_t* allowed,
+                                    const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
+  return basket_call(ctx, true, q, token_out, basket_off, basket_token, entry_kind, basket_amount, limit, allowed,
+                     opts, out, "execute_basket_swap_orders");
 }
 
 // ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------

@@ -17,7 +17,7 @@
 // linear term, the box, the start's root and the stop's scale of its kind, fixed at compile time.
 // subgraph_plan_kernel runs the setup only and reports each row's token and pool counts, which size
 // the outputs and the workspace (they do not depend on the kind).  basket_kernels.cuh's basket rows share the pair activity, the
-// workspace, the side pairs, the CTA sum, the pool view and the start.
+// workspace, the side pairs, the CTA sum, the pool view, the start and (buy rows) the capacity.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -364,14 +364,15 @@ __device__ double sg_commit(SubgraphSmem& m, int slot, bool store, double amt) {
   return __ddiv_rn(__longlong_as_double((long long)m.mx), __dmul_rn(amt, m.x[OUT ? 0 : 1]));
 }
 
-// The start ν⁰: ν_i = 1 (exact-out: ν_j = 1); then breadth-first rounds over the active pools: a
-// token not yet priced gets the largest r(a → b)·ν_b over its pools to tokens priced in earlier
-// rounds, r the no-trade boundary with a in j's role (the arbitrage scan's rate).  A token is priced
-// once, so gaining cycles cannot inflate the start.  Then clamped to the box.  Into xt.
+// The start ν⁰: ν_root = 1 (slot 0, i; exact-out: slot 1, j; basket buy rows: i's slot); then
+// breadth-first rounds over the active pools: a token not yet priced gets the largest r(a → b)·ν_b
+// over its pools to tokens priced in earlier rounds, r the no-trade boundary with a in j's role (the
+// arbitrage scan's rate).  A token is priced once, so gaining cycles cannot inflate the start.  Then
+// clamped to the box (OUT: the root fixed at 1, every other slot >= √eps).  Into xt.
 template <class Smem, bool OUT = false>
-__device__ void sg_start(const PathSets* P, const SubgraphWork& w, Smem& m) {
+__device__ void sg_start(const PathSets* P, const SubgraphWork& w, Smem& m, int root = OUT ? 1 : 0) {
   const int tid = threadIdx.x, n = m.n_loc;
-  for (int t = tid; t < n; t += blockDim.x) m.x[t] = m.xt[t] = t == (OUT ? 1 : 0) ? 1.0 : 0.0;
+  for (int t = tid; t < n; t += blockDim.x) m.x[t] = m.xt[t] = t == root ? 1.0 : 0.0;
   __syncthreads();
   unsigned long long* nxt = reinterpret_cast<unsigned long long*>(m.xt);
   for (int round = 1; round < n; ++round) {
@@ -395,16 +396,17 @@ __device__ void sg_start(const PathSets* P, const SubgraphWork& w, Smem& m) {
     __syncthreads();
     if (!more) break;
   }
-  for (int t = tid; t < n; t += blockDim.x) m.xt[t] = sg_fixed<OUT>(t) ? 1.0 : fmax(m.x[t], sg_lo<OUT>(t));
+  for (int t = tid; t < n; t += blockDim.x) m.xt[t] = OUT && t == root ? 1.0 : fmax(m.x[t], sg_lo<OUT>(t));
   __syncthreads();
 }
 
-// What workspace pool e could ever pay out of i (slot 0): 0 unless it is active and holds i; a
-// two-coin pool's reserve of i; a UniV3 pool's f(DBL_MAX) for a tender of its other token, the walk
-// to the end of its ladder (swap_crossing's unreachable test).
-__device__ __forceinline__ double sg_capacity(const PathSets* P, const SubgraphWork& w, int64_t e) {
-  const bool a = w.ta[e] == 0;
-  if (!a && w.tb[e] != 0) return 0.0;
+// What workspace pool e could ever pay out of the token at local slot `slot` (exact-out rows: i,
+// slot 0): 0 unless it is active and holds that token; a two-coin pool's reserve of it; a UniV3
+// pool's f(DBL_MAX) for a tender of its other token, the walk to the end of its ladder
+// (swap_crossing's unreachable test).
+__device__ __forceinline__ double sg_capacity(const PathSets* P, const SubgraphWork& w, int64_t e, int32_t slot = 0) {
+  const bool a = w.ta[e] == slot;
+  if (!a && w.tb[e] != slot) return 0.0;
   const SplitPool sp = split_pool(P, w.ent[e], -1, 1.0);
   if (!sp.active) return 0.0;
   const SwapSet& S = P->s[sp.k];

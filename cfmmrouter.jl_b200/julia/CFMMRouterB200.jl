@@ -688,24 +688,33 @@ execute_subgraph_orders!(ctx, token_in, token_out, amount, allowed; limit=nothin
 # basket_off[r]+1 .. basket_off[r+1] (1 to 16 distinct tokens, none of them token_out[r]; basket_off is
 # 0-based, q + 1 entries) for token_out[r], route! with BasketLiquidation over those pools.  Returns the
 # NamedTuple of _subgraph_orders with paid per basket entry.  The output struct has SubgraphOut's layout
-# (cfmm_basket_out).  Never executed, like the rest of this file.
+# (cfmm_basket_out).  entry_kind (nothing: every entry sold) is one UInt8 per basket entry, 0 sold or 1
+# bought, and selects cfmm_quote/execute_basket_swap_orders.  Never executed, like the rest of this file.
 function _basket_orders(ctx, execute::Bool, token_out::Vector{Int64}, basket_off::Vector{Int64},
                         basket_token::Vector{Int64}, basket_amount::Vector{Float64}, allowed::Vector{UInt8}, limit,
-                        opts)
+                        opts, entry_kind=nothing)
     q = length(token_out)
     length(basket_off) == q + 1 || throw(ArgumentError("basket_off needs q + 1 entries"))
     NE = basket_off[end]
     length(basket_token) == length(basket_amount) == NE ||
         throw(ArgumentError("basket_token / basket_amount need basket_off[end] entries"))
     limit === nothing || length(limit) == q || throw(ArgumentError("limit needs q entries"))
+    entry_kind === nothing || length(entry_kind) == NE ||
+        throw(ArgumentError("entry_kind needs basket_off[end] entries"))
     o = opts === nothing ? nothing : Ref(opts)
     argt = (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{UInt8}, Ptr{SubgraphOpts},
             Ptr{SubgraphOut})
+    argk = (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{UInt8},
+            Ptr{SubgraphOpts}, Ptr{SubgraphOut})
+    quote_call(out) = entry_kind === nothing ?
+        ccall((:cfmm_quote_basket_orders, LIB), Cint, argt, ctx, q, token_out, basket_off, basket_token,
+              basket_amount, allowed, o === nothing ? C_NULL : o, out) :
+        ccall((:cfmm_quote_basket_swap_orders, LIB), Cint, argk, ctx, q, token_out, basket_off, basket_token,
+              entry_kind, basket_amount, allowed, o === nothing ? C_NULL : o, out)
     tok_off, leg_off = zeros(Int64, q + 1), zeros(Int64, q + 1)
     sizes = Ref(SubgraphOut(C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, pointer(tok_off), 0, C_NULL,
                             C_NULL, C_NULL, pointer(leg_off), 0, C_NULL, C_NULL, C_NULL, C_NULL))
-    GC.@preserve tok_off leg_off chk(ctx, ccall((:cfmm_quote_basket_orders, LIB), Cint, argt,
-        ctx, q, token_out, basket_off, basket_token, basket_amount, allowed, o === nothing ? C_NULL : o, sizes))
+    GC.@preserve tok_off leg_off chk(ctx, quote_call(sizes))
     NT, L = tok_off[end], leg_off[end]
     paid, received, merit, status = zeros(max(NE, 1)), zeros(q), zeros(q), zeros(UInt8, q)
     sst, iters, fev = zeros(Cint, q), zeros(Cint, q), zeros(Cint, q)
@@ -716,15 +725,20 @@ function _basket_orders(ctx, execute::Bool, token_out::Vector{Int64}, basket_off
                               pointer(fev), pointer(merit), pointer(tok_off), NT, pointer(token), pointer(nu),
                               pointer(psi), pointer(leg_off), L, pointer(ltype), pointer(lpool), pointer(ld),
                               pointer(ll)))
-        if execute
+        if execute && entry_kind !== nothing
+            chk(ctx, ccall((:cfmm_execute_basket_swap_orders, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64},
+                 Ptr{UInt8}, Ptr{SubgraphOpts}, Ptr{SubgraphOut}),
+                ctx, q, token_out, basket_off, basket_token, entry_kind, basket_amount,
+                limit === nothing ? C_NULL : limit, allowed, o === nothing ? C_NULL : o, out))
+        elseif execute
             chk(ctx, ccall((:cfmm_execute_basket_orders, LIB), Cint,
                 (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8},
                  Ptr{SubgraphOpts}, Ptr{SubgraphOut}),
                 ctx, q, token_out, basket_off, basket_token, basket_amount, limit === nothing ? C_NULL : limit,
                 allowed, o === nothing ? C_NULL : o, out))
         else
-            chk(ctx, ccall((:cfmm_quote_basket_orders, LIB), Cint, argt,
-                ctx, q, token_out, basket_off, basket_token, basket_amount, allowed, o === nothing ? C_NULL : o, out))
+            chk(ctx, quote_call(out))
         end
     end
     return (paid=paid[1:NE], received=received, status=status, solver_status=sst, iterations=iters,
@@ -736,6 +750,16 @@ quote_basket_orders(ctx, token_out, basket_off, basket_token, basket_amount, all
 execute_basket_orders!(ctx, token_out, basket_off, basket_token, basket_amount, allowed; limit=nothing,
                        opts=nothing) =
     _basket_orders(ctx, true, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts)
+# Baskets bought and sold together (cfmm_quote/execute_basket_swap_orders): entry_kind[k] is 0 when entry k
+# is sold (up to basket_amount[k]) and 1 when it is bought (at least basket_amount[k]); a row settles in
+# token_out[r], and limit[r] is its minimum net of token_out (negative or -Inf allowed on a buy row).
+quote_basket_swap_orders(ctx, token_out, basket_off, basket_token, entry_kind, basket_amount, allowed;
+                         opts=nothing) =
+    _basket_orders(ctx, false, token_out, basket_off, basket_token, basket_amount, allowed, nothing, opts,
+                   entry_kind)
+execute_basket_swap_orders!(ctx, token_out, basket_off, basket_token, entry_kind, basket_amount, allowed;
+                            limit=nothing, opts=nothing) =
+    _basket_orders(ctx, true, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts, entry_kind)
 
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the

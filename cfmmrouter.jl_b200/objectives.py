@@ -6,7 +6,7 @@ from __future__ import annotations
 
 import numpy as np
 
-__all__ = ["Objective", "LinearNonnegative", "BasketLiquidation", "Swap"]
+__all__ = ["Objective", "LinearNonnegative", "BasketLiquidation", "BasketSwap", "Swap"]
 
 
 class Objective:
@@ -95,6 +95,61 @@ class BasketLiquidation(Objective):
 
     def upper_limit(self):  # objectives.jl:129
         return np.full(len(self.delta_in), np.inf)
+
+
+class BasketSwap(Objective):
+    """Ψ_i − I(Ψ_{-i} + Δin_{-i} − Δout_{-i} >= 0): sell up to Δin and buy at least Δout of the
+    other tokens, maximising the net of token i, which may be negative (the order pays on net).
+    `i` is 1-based.  With Δout all zero it is BasketLiquidation(i, Δin), box included.  Otherwise
+    the conjugate is finite only at ν_i = 1 (Ψ_i is free), where it is (Δin − Δout)ᵀν over the other
+    tokens: the box fixes ν_i = 1 (lower = upper = 1) and keeps ν_t >= √eps for every other t."""
+
+    def __init__(self, i, delta_in, delta_out):
+        delta_in = np.array(delta_in, dtype=np.float64)
+        delta_out = np.array(delta_out, dtype=np.float64)
+        if delta_in.shape != delta_out.shape or delta_in.ndim != 1:
+            raise ValueError("delta_in and delta_out need one entry per token")
+        if not (0 < i <= len(delta_in)):
+            raise ValueError("Invalid index i")
+        self.i = int(i)
+        self.delta_in = delta_in
+        self.delta_out = delta_out
+        self.buys = bool(np.any(np.delete(delta_out, self.i - 1) != 0.0))
+        self._basket = BasketLiquidation(i, delta_in)
+
+    def linear_term(self):
+        if not self.buys:
+            return self._basket.linear_term()
+        lin = self.delta_in - self.delta_out
+        lin[self.i - 1] = 0.0
+        return lin
+
+    def f(self, v):
+        if not self.buys:
+            return self._basket.f(v)
+        if v[self.i - 1] != 1.0:
+            return np.inf
+        return float(np.dot(self.linear_term(), v))
+
+    def grad(self, g, v):
+        if not self.buys:
+            return self._basket.grad(g, v)
+        if v[self.i - 1] != 1.0:
+            g[:] = np.inf
+        else:
+            g[:] = self.linear_term()
+
+    def lower_limit(self):
+        ret = self._basket.lower_limit()
+        if self.buys:
+            ret[self.i - 1] = 1.0
+        return ret
+
+    def upper_limit(self):
+        ret = self._basket.upper_limit()
+        if self.buys:
+            ret[self.i - 1] = 1.0
+        return ret
 
 
 def Swap(i, j, delta, n):

@@ -80,6 +80,26 @@ def _row_args(n_tokens, q, allowed, limit, opts, what):
     return mask.ctypes.data_as(C.POINTER(C.c_uint8)), limit, None if o is None else C.byref(o)
 
 
+def _entry_kind(kind, basket_off, limit, what):
+    """The entry kinds of a basket call as a uint8 array (None: every entry sold, and the call is
+    cfmm_quote/execute_basket_orders), with the Python argument errors: a scalar applies to every
+    entry; a kind other than 0 (sold) or 1 (bought); a NaN limit, or a +inf limit on any row."""
+    if kind is None:
+        return None
+    NE = int(basket_off[-1])
+    k = np.asarray(kind)
+    if k.ndim == 0:
+        k = np.full(NE, k)
+    k = k.reshape(-1)
+    if len(k) != NE:
+        raise ValueError(f"{what}: kind must have {NE} entries, one per basket entry (or be a scalar)")
+    if not np.all(np.isin(k, (_lib.SWAP_EXACT_IN, _lib.SWAP_EXACT_OUT))):
+        raise ValueError(f"{what}: kind must be 0 (sold) or 1 (bought)")
+    if limit is not None and np.any(np.isnan(limit) | (limit == np.inf)):
+        raise ValueError(f"{what}: a limit (the minimum received) is NaN or +inf")
+    return np.ascontiguousarray(k, dtype=np.uint8)
+
+
 def _row_kind(kind, q, limit, what):
     """The kinds of a subgraph call as a uint8 array (None: every row exact-in, passed as NULL), with
     the Python argument errors: a scalar applies to every row; a kind other than 0 (exact-in) or 1
@@ -818,8 +838,8 @@ class DevicePools:
         return self._subgraph(True, token_in, token_out, amount, allowed, limit, opts, kind)
 
     # -- token baskets over every pool among allowed tokens (include/cfmm_b200.h,
-    #    cfmm_quote_basket_orders / cfmm_execute_basket_orders) --------------------------------------
-    def _basket(self, execute, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts):
+    #    cfmm_quote_basket_(swap_)orders / cfmm_execute_basket_(swap_)orders) -------------------------
+    def _basket(self, execute, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts, kind=None):
         tout = np.ascontiguousarray(token_out, dtype=np.int64).reshape(-1)
         boff = np.ascontiguousarray(basket_off, dtype=np.int64).reshape(-1)
         btok = np.ascontiguousarray(basket_token, dtype=np.int64).reshape(-1)
@@ -831,10 +851,18 @@ class DevicePools:
         if not (len(btok) == len(bamt) == NE):
             raise ValueError(f"basket orders: basket_token and basket_amount need basket_off[-1] = {NE} entries")
         u8m, limit, po = _row_args(self.n_tokens, q, allowed, limit, opts, "basket orders")
+        kind = _entry_kind(kind, boff, limit, "basket orders")
         to, bo, bt, ba = _ip(tout), _ip(boff), _ip(btok), _dp(bamt)
         lim = None if limit is None else _dp(limit)
 
         def call(size, out):
+            if kind is not None:
+                kd = kind.ctypes.data_as(C.POINTER(C.c_uint8))
+                if execute and not size:
+                    return self._lib.cfmm_execute_basket_swap_orders(self._ctx, q, to, bo, bt, kd, ba, lim, u8m, po,
+                                                                     C.byref(out))
+                return self._lib.cfmm_quote_basket_swap_orders(self._ctx, q, to, bo, bt, kd, ba, u8m, po,
+                                                               C.byref(out))
             if execute and not size:
                 return self._lib.cfmm_execute_basket_orders(self._ctx, q, to, bo, bt, ba, lim, u8m, po, C.byref(out))
             return self._lib.cfmm_quote_basket_orders(self._ctx, q, to, bo, bt, ba, u8m, po, C.byref(out))
@@ -842,21 +870,26 @@ class DevicePools:
         out.basket_off = boff
         return out
 
-    def quote_basket_orders(self, token_out, basket_off, basket_token, basket_amount, allowed, opts=None):
+    def quote_basket_orders(self, token_out, basket_off, basket_token, basket_amount, allowed, opts=None,
+                            kind=None):
         """cfmm_quote_basket_orders: row r sells basket_amount[k] of basket_token[k] for k in
         basket_off[r] .. basket_off[r + 1] - 1 (1 to 16 distinct tokens, 1-based, none token_out[r])
         for token_out[r] over every pool among them and the tokens t with allowed[t - 1], split
         optimally: route! with BasketLiquidation over the row's pools, solved per row on the device.
-        opts as quote_subgraph_orders.  No state changes.  Returns quote_subgraph_orders' namespace,
-        with paid per basket entry and basket_off added."""
-        return self._basket(False, token_out, basket_off, basket_token, basket_amount, allowed, None, opts)
+        kind (cfmm_quote_basket_swap_orders): None (every entry sold), a scalar, or one entry per basket
+        entry, 0 sold or 1 bought (buy basket_amount[k] of basket_token[k]); a row with a bought entry
+        settles in token_out[r], and its received may be negative.  opts as quote_subgraph_orders.  No
+        state changes.  Returns quote_subgraph_orders' namespace, with paid per basket entry (−Ψ: a
+        bought entry reads at most −amount) and basket_off added."""
+        return self._basket(False, token_out, basket_off, basket_token, basket_amount, allowed, None, opts, kind)
 
     def execute_basket_orders(self, token_out, basket_off, basket_token, basket_amount, allowed, limit=None,
-                              opts=None):
-        """cfmm_execute_basket_orders: the rows of quote_basket_orders in batch order, each re-solved on
-        the state the earlier filled rows left; limit[r] (None: none) is the minimum received of
-        token_out[r], and a row below it reverts.  Returns what quote_basket_orders returns."""
-        return self._basket(True, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts)
+                              opts=None, kind=None):
+        """cfmm_execute_basket_(swap_)orders: the rows of quote_basket_orders in batch order, each
+        re-solved on the state the earlier filled rows left; limit[r] (None: none) is the minimum
+        received of token_out[r] (for a row with a bought entry it may be negative or -inf), and a row
+        below it reverts.  Returns what quote_basket_orders returns."""
+        return self._basket(True, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts, kind)
 
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
@@ -1499,6 +1532,59 @@ class Router:
     @staticmethod
     def _per_entry(out):
         return [out.paid[out.basket_off[r]:out.basket_off[r + 1]] for r in range(len(out.basket_off) - 1)]
+
+    def _swap_basket_args(self, token_out, sells, buys, allowed, limits, what):
+        """_basket_args over each row's sold entries then its bought entries, plus the entry kinds and
+        each row's count of sold entries."""
+        if len(sells) != len(buys):
+            raise ValueError(f"{what}: sells and buys need one entry per row")
+        rows, n_sell = [], []
+        for s, b in zip(sells, buys):
+            st, sa = (list(s.keys()), list(s.values())) if isinstance(s, dict) else (list(s[0]), list(s[1]))
+            bt, ba = (list(b.keys()), list(b.values())) if isinstance(b, dict) else (list(b[0]), list(b[1]))
+            if len(st) != len(sa) or len(bt) != len(ba):
+                raise ValueError(f"{what}: sells and buys need one amount per token")
+            rows.append((st + bt, sa + ba))
+            n_sell.append(len(st))
+        tout, off, toks, amts, limits = self._basket_args(token_out, rows, allowed, limits, what)
+        kind = np.zeros(len(toks), np.uint8)
+        for r, ns in enumerate(n_sell):
+            kind[off[r] + ns:off[r + 1]] = _lib.SWAP_EXACT_OUT
+        return tout, off, toks, amts, kind, limits, n_sell
+
+    @staticmethod
+    def _sold_bought(out, n_sell):
+        per = Router._per_entry(out)
+        return [p[:ns] for p, ns in zip(per, n_sell)], [0.0 - p[ns:] for p, ns in zip(per, n_sell)]
+
+    def quote_basket_swap_orders(self, token_out, sells, buys, allowed, opts=None):
+        """Sell and buy token baskets in one order per row, settled in token_out[r]: sells[r] and
+        buys[r] are {token: amount} or (tokens, amounts) (together 1 to 16 distinct 1-based tokens,
+        none of them token_out[r]; at least one bought token makes the row a buy row).  Each row
+        maximises its net of token_out[r] over every pool among its tokens and the tokens t with
+        allowed[t - 1], selling up to the sold amounts and buying at least the bought ones, one dual
+        solve per row on the device (cfmm_quote_basket_swap_orders).  No state changes.  Returns (sold
+        per row, bought per row as lists of arrays in the caller's order, the net of token_out [q]
+        (negative when the row pays), status [q], detail); detail is DevicePools.quote_basket_orders'
+        namespace.  Single GPU."""
+        tout, off, toks, amts, kind, _, n_sell = self._swap_basket_args(token_out, sells, buys, allowed, None,
+                                                                         "quote_basket_swap_orders")
+        out = self._pools.quote_basket_orders(tout, off, toks, amts, allowed, opts, kind)
+        sold, bought = self._sold_bought(out, n_sell)
+        return sold, bought, out.received, out.status, out
+
+    def execute_basket_swap_orders(self, token_out, sells, buys, allowed, limits=None, opts=None):
+        """Execute basket swap orders in order (cfmm_execute_basket_swap_orders), each re-solved on the
+        state the earlier filled rows left, with an optional minimum net of token_out per row (negative:
+        pay at most -limit; -inf allowed): a row below it reverts.  Returns what
+        quote_basket_swap_orders returns and refreshes the pool objects the filled rows traded with
+        from the device state.  Single GPU."""
+        tout, off, toks, amts, kind, limits, n_sell = self._swap_basket_args(token_out, sells, buys, allowed, limits,
+                                                                             "execute_basket_swap_orders")
+        out = self._pools.execute_basket_orders(tout, off, toks, amts, allowed, limits, opts, kind)
+        self._refresh_filled(out)
+        sold, bought = self._sold_bought(out, n_sell)
+        return sold, bought, out.received, out.status, out
 
     def quote_basket_orders(self, token_out, baskets, allowed, opts=None):
         """Sell each row's basket (baskets[r]: {token: amount} or (tokens, amounts); 1 to 16 distinct

@@ -983,6 +983,65 @@ int cfmm_execute_basket_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_ou
                                const uint8_t *allowed, const cfmm_subgraph_opts *opts,
                                cfmm_basket_out *out);
 
+/* ---- token baskets bought and sold together: basket rows with bought entries -----------------
+ * cfmm_quote_basket_swap_orders / cfmm_execute_basket_swap_orders take the arguments of the two
+ * calls above plus entry_kind [basket_off[q]] (NULL: every entry sold).  An entry of kind
+ * CFMM_SWAP_EXACT_IN sells up to δ_k = basket_amount[k] of b_k; one of kind CFMM_SWAP_EXACT_OUT buys
+ * y_l = basket_amount[l] of b_l.  Every row settles in i = token_out[r].  A row whose entries are all
+ * sold is a basket row above, bit for bit and with the same launches.  A row with at least one bought
+ * entry is a buy row: it has the same B, T, reachability rule (an entry with a positive amount outside
+ * T makes the row CFMM_ORDER_UNREACHABLE; a zero entry outside T is dropped), pools, legs, sums,
+ * optimizer and CTA reduction, with:
+ *   tokens   local order: the bought entries in T in the caller's order, then i, then the sold
+ *            entries in T in the caller's order, then B ∩ T ascending.  With one bought entry and no
+ *            sold entry this is the exact-out subgraph row's order (i, j, B ∩ T).
+ * Problem.  The primal is: maximise Ψ_i (it may be negative: the row pays on net) subject to
+ * Ψ_k >= −δ_k for sold entries, Ψ_l >= y_l for bought entries and Ψ_t >= 0 for every other t in T.
+ * Its dual: minimise g(ν) = Σ_k δ_k·ν_k − Σ_l y′_l·ν_l + Σ_p π_p(ν) on the box ν_i = 1 (lower = upper
+ * = 1), ν_t >= √eps for every other t, with y′ = y·(1 + rtol) rounded up as exact-out rows do.  ν_i is
+ * fixed for the reason it is fixed in exact-out rows.  The gradient is lin + Ψ, lin = δ at sold
+ * entries, −y′ at bought entries and 0 elsewhere; the value is Σ lin_e·ν_e over the entries in local
+ * order (the first term alone) plus the pool sum.
+ *   start    ν_i = 1; the breadth-first pricing of subgraph rows from i's slot; clamped to the box.
+ *   stop     V = Σ_e amount_e·ν_e over the entries in local order (y, not y′);
+ *            m_r = max(max_t ν_t·|pg_t| / V, max over bought l with y_l > 0 of ν_l·|pg_l| / (y_l·ν_l)).
+ *            The second term holds each bought entry to rtol·y_l even when the sold entries dominate
+ *            V.  Status 0 when m_r <= rtol.
+ * Capacity, checked once per row before any solve: for each bought entry with y_l > 0, C_l is the
+ * exact-out rule's capacity at b_l over the row's pools.  The row is CFMM_ORDER_UNREACHABLE when
+ * y_l >= C_l for some l.  A row that passes this check but cannot be served has an unbounded dual and
+ * ends CFMM_ORDER_NOT_CONVERGED, trading nothing.
+ * What a fill promises.  A buy row fills only at solver status 0 with Ψ_l >= y_l for every bought
+ * entry with y_l > 0 (a status-0 row short of one is CFMM_ORDER_NOT_CONVERGED with solver_status 0).
+ * A filled row has: received = Ψ_i (negative when the row pays on net); paid_k = −Ψ_{b_k}, so a
+ * bought entry reads paid_l = −Ψ_l <= −y_l; each sold entry paid within rtol·V/ν_k of δ_k when ν_k is
+ * off its bound; each bought entry receiving Ψ_l in [y_l, y_l·(1 + 2·rtol)] when ν_l is off its bound;
+ * every other token (an intermediate, or a bought entry with y_l = 0) Ψ_b >= −rtol·V/ν_b; and a
+ * duality gap of at most |T|·rtol·V plus the box's √eps terms.  A row whose amounts are all 0 fills
+ * with zeros and runs no solve.  The outputs are those of cfmm_basket_out.
+ * Execute.  limit (NULL: none) is the minimum Ψ_i.  For a buy row it may be negative (pay at most
+ * −limit) or −inf; an equal limit fills and a smaller Ψ_i reverts with CFMM_ORDER_LIMIT.  A sell-only
+ * row's limit follows cfmm_execute_basket_orders.  The transition, bookkeeping, conflict rule
+ * ({i} ∪ entries ∪ B) and levels are those of basket rows; a level runs its sell-only rows and its
+ * buy rows as two launches (they share no token).  A quote runs the sell-only rows and the buy rows
+ * as two launches.
+ * Errors: those of the basket calls, and CFMM_ERR_INVALID before anything runs for an entry kind
+ * other than CFMM_SWAP_EXACT_IN or CFMM_SWAP_EXACT_OUT, and a buy row's limit that is NaN or +inf. */
+int cfmm_quote_basket_swap_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_out /* [q] */,
+                                  const int64_t *basket_off /* [q+1] */,
+                                  const int64_t *basket_token /* [basket_off[q]] */,
+                                  const uint8_t *entry_kind /* [basket_off[q]] or NULL: every entry sold */,
+                                  const double *basket_amount /* [basket_off[q]] */,
+                                  const uint8_t *allowed /* [n_tokens], required */,
+                                  const cfmm_subgraph_opts *opts /* NULL = defaults */,
+                                  cfmm_basket_out *out);
+int cfmm_execute_basket_swap_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_out,
+                                    const int64_t *basket_off, const int64_t *basket_token,
+                                    const uint8_t *entry_kind /* [basket_off[q]] or NULL */,
+                                    const double *basket_amount, const double *limit /* [q] or NULL */,
+                                    const uint8_t *allowed, const cfmm_subgraph_opts *opts,
+                                    cfmm_basket_out *out);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,

@@ -19,7 +19,17 @@ as one cfmm_execute_basket_orders on one copy, and as their entries sold one by 
 cfmm_execute_subgraph_orders per basket, in the same order) on the other: per K, the fraction of rows
 where the basket receives at least the sequence's total (within 3·rtol) and the median ratio.
 
-    python tools/basket_order_timing.py [--only hub|headline] [--budget-s 20]
+With --buy KS,KB the tool times buy rows instead (cfmm_quote_basket_swap_orders): each row sells KS
+and buys KB tokens around its output token (chosen as above, every amount at 1e-3 of a pool's depth),
+|B| in {0, 8, 64}, 1k rows and then 100k under the same budget rule.  Per call it reports what the
+sell-only rows report, and then the same rows quoted the way a caller would have to without buy rows:
+the KS sold tokens as one cfmm_quote_basket_orders row and each bought token as one exact-out
+cfmm_quote_subgraph_swap_orders row paying in the output token (their kernel times summed, and each
+call's fill, iteration and m_r figures).  Buy rows also report their not-converged rows by solver
+status (0: converged short of a bought y, 1: stalled, 2 / 3: max_iter / max_fun) and the median m_r
+those rows reached.
+
+    python tools/basket_order_timing.py [--only hub|headline] [--budget-s 20] [--buy KS,KB]
 """
 from __future__ import annotations
 
@@ -92,6 +102,44 @@ def run(p, name, n, tokens, csr, amt_of, budget_s, rng):
                 est = ms * 100_000 / q
 
 
+def run_buy(p, name, n, tokens, csr, amt_of, budget_s, rng, ks, kb):
+    """Buy rows of ks sold and kb bought entries, then the same rows as a sell-only basket plus kb
+    exact-out rows."""
+    allowed8 = np.arange(n) < 8
+    p.quote_basket_orders([2], [0, 1], [1], [1.0], allowed8)  # builds the pair index and the adjacency
+    for nb in (0, 8, 64):
+        allowed = np.arange(n) < nb
+        est = None
+        for q in (1_000, 100_000):
+            if q > 1_000 and est > budget_s * 1e3:
+                emit(set=name, B=nb, K_sell=ks, K_buy=kb, rows=q, run=False, estimated_kernel_ms=round(est, 1))
+                continue
+            tout, boff, btok, bamt = make_rows(rng, q, (ks + kb,), nb, tokens, csr, amt_of)
+            kind = np.tile(np.r_[np.zeros(ks), np.full(kb, cr._lib.SWAP_EXACT_OUT)].astype(np.uint8), q)
+            o, wall, ms, launches = timed(
+                p, lambda: p._basket(False, tout, boff, btok, bamt, allowed, None, None, kind))
+            nc = o.status == cr._lib.ORDER_NOT_CONVERGED
+            by = {str(v): int(np.sum(o.solver_status[nc] == v)) for v in np.unique(o.solver_status[nc])}
+            emit(set=name, B=nb, K_sell=ks, K_buy=kb, rows=q, mode="buy_rows", wall_ms=round(wall, 3),
+                 kernel_ms=round(ms, 3), profile_entries=launches,
+                 tokens_mean=round(float(np.mean(np.diff(o.tok_off))), 1), not_converged_by_solver_status=by,
+                 merit_nc_median=float(np.median(o.merit[nc])) if np.any(nc) else None, **stats(o))
+            sold = kind == 0
+            split, split_ms = {}, 0.0
+            if ks:
+                s_off = np.arange(0, q * ks + 1, ks, dtype=np.int64)
+                os_, _, ms_s, _ = timed(
+                    p, lambda: p._basket(False, tout, s_off, btok[sold], bamt[sold], allowed, None, None))
+                split["basket"], split_ms = stats(os_), split_ms + ms_s
+            ob, _, ms_b, _ = timed(
+                p, lambda: p._subgraph(False, np.repeat(tout, kb), btok[~sold], bamt[~sold], allowed, None, None,
+                                       cr._lib.SWAP_EXACT_OUT))
+            split["exact_out"], split_ms = stats(ob), split_ms + ms_b
+            emit(set=name, B=nb, K_sell=ks, K_buy=kb, rows=q, mode="basket_plus_exact_out",
+                 kernel_ms=round(split_ms, 3), **split)
+            est = ms * 100_000 / q
+
+
 def disjoint_rows(rng, q, Ks, tokens, csr, amt_of):
     """Up to q rows as make_rows with |B| = 0 whose token sets {i} ∪ basket are pairwise disjoint."""
     off, nbr = csr
@@ -134,13 +182,17 @@ def compare(a, b, name, n, tokens, csr, amt_of, rng):
                  median_ratio=round(float(np.median(ratio)), 6), min_ratio=round(float(np.min(ratio)), 6))
 
 
-def hub(budget_s):
+def hub(budget_s, buy=None):
     p, n, others, nu, pools_of = hub_set(np.random.default_rng(7))
     Ai = hub_pairs(np.random.default_rng(7))
     assert all(len(pools_of(int(a), int(b))) for a, b in Ai[-5:]), "hub_pairs no longer replays hub_set"
     csr = neighbours(Ai, n)
     amt_of = lambda t: 1e-3 * 1e4 / nu[t]  # noqa: E731
     rng = np.random.default_rng(2030)
+    if buy:
+        run_buy(p, "hub", n, others, csr, amt_of, budget_s, rng, *buy)
+        p.close()
+        return
     run(p, "hub", n, others, csr, amt_of, budget_s, rng)
     q, _, _, _, _ = hub_set(np.random.default_rng(7))
     compare(p, q, "hub", n, others, csr, amt_of, rng)
@@ -167,7 +219,7 @@ def hub_pairs(rng):
     return np.concatenate([A, D])
 
 
-def headline(budget_s):
+def headline(budget_s, buy=None):
     m, n = 10_000_000, 50_000
     R, g, Ai = synth.product_pools(m, n, seed=1234)
 
@@ -186,6 +238,10 @@ def headline(budget_s):
     amt_of = lambda t: 1e-3 * depth[t]  # noqa: E731
     rng = np.random.default_rng(2031)
     tokens = np.arange(1, n + 1)
+    if buy:
+        run_buy(p, "headline", n, tokens, csr, amt_of, budget_s, rng, *buy)
+        p.close()
+        return
     run(p, "headline", n, tokens, csr, amt_of, budget_s, rng)
     q = ctx()
     compare(p, q, "headline", n, tokens, csr, amt_of, rng)
@@ -197,12 +253,18 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--only", choices=["hub", "headline"])
     ap.add_argument("--budget-s", type=float, default=20.0)
+    ap.add_argument("--buy", help="KS,KB: time buy rows selling KS and buying KB tokens")
     args = ap.parse_args()
+    buy = None
+    if args.buy:
+        buy = tuple(int(x) for x in args.buy.split(","))
+        if len(buy) != 2 or buy[1] < 1 or buy[0] < 0 or sum(buy) > 16:
+            ap.error("--buy needs KS,KB with KS >= 0, KB >= 1 and KS + KB <= 16")
     emit(card=card())
     if args.only in (None, "hub"):
-        hub(args.budget_s)
+        hub(args.budget_s, buy)
     if args.only in (None, "headline"):
-        headline(args.budget_s)
+        headline(args.budget_s, buy)
 
 
 if __name__ == "__main__":
