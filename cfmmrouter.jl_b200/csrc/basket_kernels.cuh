@@ -4,8 +4,9 @@
 //
 // A row sells a basket of K <= kBasketMaxTokens tokens b_0 .. b_{K-1} for i: route! with
 // BasketLiquidation(i, Δin) over the row's pools.  It is subgraph_kernels.cuh's row with the one side
-// token j generalised to K basket tokens, and shares that file's pair activity (subgraph_act_kernel),
-// workspace, side pairs, CTA sum, pool view and start; subgraph orders keep their own row kernel.
+// token j generalised to K basket tokens.  Its setup (bk_setup) is its own; after it, the row runs
+// that file's pool gather, pool ordering, solve (sg_solve with this file's BkRule) and legs, and
+// subgraph orders keep their own row kernel and setup (DESIGN §4.5).
 //   setup   the pairs {b_k, s} and {i, s} for every slot s, {b_k, i} and {b_k, b_l}; the component T
 //           of i over active pools; the local tokens (0 = i, then the basket tokens in T in basket
 //           order, then T's slots ascending) and the row's pools: every pool of every pair inside T,
@@ -128,20 +129,6 @@ __host__ __device__ __forceinline__ size_t bk_dyn_bytes(int K, int nB) {
 }
 extern __shared__ __align__(8) unsigned char bk_dyn[];
 
-// The pair {a, b} from a's adjacency list (bisected), −1 when there is none.
-__device__ __forceinline__ int32_t bk_pair(AdjView A, int32_t a, int32_t b) {
-  int64_t lo = A.off[a], hi = A.off[a + 1];
-  const int64_t a1 = hi;
-  while (lo < hi) {
-    const int64_t mid = (lo + hi) >> 1;
-    if (A.nbr[mid] < b)
-      lo = mid + 1;
-    else
-      hi = mid;
-  }
-  return lo < a1 && A.nbr[lo] == b ? A.pair[lo] : -1;
-}
-
 // Setup of the row trading btok[0 .. K) (1-based) for i (0-based): T, the local tokens and the pool
 // count of every slot (cnt[s], the pools of the pairs {s, i}, {s, b_k} for b_k ∈ T, and {s, u} for
 // slots u > s in T) and of the pairs among i and the basket tokens in T (basket_cnt).  BUY: the local
@@ -172,14 +159,14 @@ __device__ void bk_setup(const PathSets* P, PairIndexView ix, AdjView A, const B
   for (int e = tid; e < K * K; e += blockDim.x) {
     const int k = e / K, l = e % K;
     if (l < k) continue;
-    const int32_t p = bk_pair(A, m.btok[k], l == k ? i : m.btok[l]);
+    const int32_t p = adj_pair(A, m.btok[k], l == k ? i : m.btok[l]);
     const uint8_t a = p >= 0 && subgraph_pair_active(P, ix, p);
     m.kpair[k][l] = m.kpair[l][k] = p;
     m.kact[k][l] = m.kact[l][k] = a;
   }
   __syncthreads();
-  for (int k = 0; k < K; ++k) sg_side_pairs(A, G, m.btok[k], bpair + (size_t)k * nB);
-  sg_side_pairs(A, G, i, m.ipair);
+  for (int k = 0; k < K; ++k) side_pairs(A, G, m.btok[k], bpair + (size_t)k * nB);
+  side_pairs(A, G, i, m.ipair);
   __syncthreads();
   for (int s = tid; s < nB; s += blockDim.x) {
     const bool ok = !m.side[s];
@@ -332,90 +319,39 @@ __device__ __forceinline__ double bk_value(const BkSmem<BUY>& m, const double* c
   return s;
 }
 
-// One evaluation at ν = xt: every pool's contributions, Ψ_t -> pt, gt = lin + Ψ, and the dual's
-// value linᵀxt + Σ val (returned to every thread).
+// The rules of a basket row (BUY false) or a buy row, as subgraph_kernels.cuh's SgRule: lin is δ_k at
+// the basket tokens (buy rows: blin, δ_k at sold and −y′_l at bought entries), the dual's linear value
+// bk_value over bamt (blin); the box is Swap's (buy rows: ν_i = 1 and ν_t >= √eps), the start's root
+// is i's slot; m_r = mx / V, V = Σ_k amount_k·ν_k (y, not y′, at bought entries), and a buy row's m_r
+// is at least ν_l·|pg_l| / (y_l·ν_l) for every bought entry with y_l > 0.
 template <bool BUY>
-__device__ double bk_evaluate(const PathSets* P, const SubgraphWork& w, BkSmem<BUY>& m) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int64_t np = m.npool;
-  double vs = 0.0;
-  for (int64_t e = tid; e < np; e += blockDim.x) {
-    const SplitPool sp = sg_pool(P, w, e, m.xt);
-    const Trade tr = split_legs(P, sp);
-    const double a = __dsub_rn(tr.l1, tr.d1), b = __dsub_rn(tr.l2, tr.d2);
-    w.ca[e] = a;
-    w.cb[e] = b;
-    vs = __dadd_rn(vs, __dadd_rn(__dmul_rn(sp.v1, a), __dmul_rn(sp.v2, b)));
+struct BkRule {
+  static constexpr bool kOut = BUY;
+  __device__ __forceinline__ double lin_at(const BkSmem<BUY>& m, int t) const {
+    if constexpr (BUY)
+      return t == m.nout || t > m.nin ? 0.0 : m.blin[t < m.nout ? t : t - 1];
+    else
+      return t >= 1 && t <= m.nin ? m.bamt[t - 1] : 0.0;
   }
-  const double V = sg_cta_sum(vs, m);  // (its syncs also publish ca, cb)
-  for (int t = warp; t < m.n_loc; t += kSubgraphWarps) {
-    double s = 0.0;
-    for (int k = m.inc_off[t] + lane; k < m.inc_off[t + 1]; k += 32) {
-      const int32_t v = w.inc[k];
-      s = __dadd_rn(s, (v & 1) ? w.cb[v >> 1] : w.ca[v >> 1]);
+  __device__ __forceinline__ double value(const BkSmem<BUY>& m) const {
+    if constexpr (BUY)
+      return bk_value<BUY>(m, m.blin, m.xt);
+    else
+      return bk_value<BUY>(m, m.bamt, m.xt);
+  }
+  __device__ __forceinline__ double lo(int t) const { return bk_lo<BUY>(t); }
+  __device__ __forceinline__ bool fixed(const BkSmem<BUY>& m, int t) const { return bk_fixed<BUY>(m, t); }
+  __device__ __forceinline__ int root(const BkSmem<BUY>& m) const { return bk_root<BUY>(m); }
+  __device__ __forceinline__ double merit(const BkSmem<BUY>& m, double mx) const {
+    double mr = __ddiv_rn(mx, bk_value<BUY>(m, m.bamt, m.x));
+    if constexpr (BUY) {
+      for (int l = 0; l < m.nout; ++l)
+        if (m.bamt[l] > 0.0)
+          mr = fmax(mr, __ddiv_rn(__dmul_rn(m.x[l], fabs(m.pg[l])), __dmul_rn(m.bamt[l], m.x[l])));
     }
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) s = __dadd_rn(s, __shfl_xor_sync(kFull, s, o));
-    if (lane == 0) {
-      m.pt[t] = s;
-      if constexpr (BUY)
-        m.gt[t] = __dadd_rn(t == m.nout || t > m.nin ? 0.0 : m.blin[t < m.nout ? t : t - 1], s);
-      else
-        m.gt[t] = __dadd_rn(t >= 1 && t <= m.nin ? m.bamt[t - 1] : 0.0, s);
-    }
+    return mr;
   }
-  __syncthreads();
-  if constexpr (BUY)
-    return __dadd_rn(bk_value<BUY>(m, m.blin, m.xt), V);
-  else
-    return __dadd_rn(bk_value<BUY>(m, m.bamt, m.xt), V);
-}
-
-// Accept xt: (s, y) into history slot `slot` when store, x <- xt, g <- gt, Ψ, the projected gradient
-// and the Gram matrix of [S Y pg] (one warp per entry group, lanes over the tokens, butterfly).
-// Returns m_r = max_t ν_t·|pg_t| / V, V = Σ_k amount_k·ν_k (y, not y′, at bought entries); a buy
-// row's m_r is at least ν_l·|pg_l| / (y_l·ν_l) for every bought entry with y_l > 0.
-template <bool BUY>
-__device__ double bk_commit(BkSmem<BUY>& m, int slot, bool store) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = m.n_loc;
-  if (tid == 0) m.mx = 0ull;
-  for (int t = tid; t < n; t += blockDim.x) {
-    const double xn = m.xt[t], gn = m.gt[t];
-    if (store) {
-      m.S[slot][t] = __dsub_rn(xn, m.x[t]);
-      m.Y[slot][t] = __dsub_rn(gn, m.g[t]);
-    }
-    m.x[t] = xn;
-    m.g[t] = gn;
-    m.px[t] = m.pt[t];
-    m.pg[t] = bk_fixed<BUY>(m, t) || (xn <= bk_lo<BUY>(t) && gn > 0.0) ? 0.0 : gn;
-  }
-  __syncthreads();
-  double mx = 0.0;
-  for (int t = tid; t < n; t += blockDim.x) mx = fmax(mx, __dmul_rn(m.x[t], fabs(m.pg[t])));
-  for (int o = 16; o >= 1; o >>= 1) mx = fmax(mx, __shfl_xor_sync(kFull, mx, o));
-  if (lane == 0) atomicMax(&m.mx, (unsigned long long)__double_as_longlong(mx));  // order-free max
-  const auto col = [&](int c, int t) {
-    return c < kSolverM ? m.S[c][t] : c < 2 * kSolverM ? m.Y[c - kSolverM][t] : m.pg[t];
-  };
-  for (int k = warp; k < kSolverK * kSolverK; k += kSubgraphWarps) {
-    const int r = k / kSolverK, c = k % kSolverK;
-    if (c < r) continue;
-    double s = 0.0;
-    for (int t = lane; t < n; t += 32) s = fma(col(r, t), col(c, t), s);
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) s = __dadd_rn(s, __shfl_xor_sync(kFull, s, o));
-    if (lane == 0) m.W[r][c] = m.W[c][r] = s;
-  }
-  __syncthreads();
-  double mr = __ddiv_rn(__longlong_as_double((long long)m.mx), bk_value<BUY>(m, m.bamt, m.x));
-  if constexpr (BUY) {
-    for (int l = 0; l < m.nout; ++l)
-      if (m.bamt[l] > 0.0)
-        mr = fmax(mr, __ddiv_rn(__dmul_rn(m.x[l], fabs(m.pg[l])), __dmul_rn(m.bamt[l], m.x[l])));
-  }
-  return mr;
-}
+};
 
 // Row r on the current state.  Returns nothing; writes the row's outputs.  EXEC: the limit decides,
 // and a filled row applies the transition of cfmm_apply_trades at its ν to each of its pools.  BUY:
@@ -427,10 +363,9 @@ template <bool EXEC, bool BUY = false>
 __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
                              const uint8_t* gact, const BasketRows& R, const SubgraphWork& w, const SplitMoved& mv,
                              int64_t r, BkSmem<BUY>& m) {
-  __shared__ LbfgsHistory hist;
-  __shared__ double s_f, s_t, s_merit;
-  __shared__ int s_state, s_status, s_iter, s_fev, s_small, s_any, s_unreach;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  __shared__ SgSolveState s;
+  __shared__ int s_any, s_unreach;
+  const int tid = threadIdx.x;
   const int64_t b0 = R.basket_off[r];
   bk_setup<BUY>(P, ix, A, G, gact, R.basket_token + b0, (int)(R.basket_off[r + 1] - b0),
                 (int32_t)(R.token_out[r] - 1), m);
@@ -480,89 +415,11 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
       }
   }
   const int32_t* bpair = reinterpret_cast<const int32_t*>(bk_dyn);
-  for (int s = tid; s < G.nB; s += blockDim.x) {
-    if (!m.in[s]) continue;
-    int64_t o = m.cnt[s];
-    const auto put = [&](int64_t k) {
-      if (k < 0) return;
-      for (int64_t e = ix.off[k]; e < ix.off[k + 1]; ++e) w.ent[o++] = ix.pool[e];
-    };
-    put(m.ipair[s]);
+  sg_gather(ix, G, w, m, [&](int s, auto& put) {
     for (int k = 0; k < m.nK; ++k)
       if (m.bin[k]) put(bpair[(size_t)k * G.nB + s]);
-    const int dg = G.deg[s];
-    for (int e = 0; e < dg; ++e) {
-      const int u = G.nbr[(int64_t)G.nB * s + e];
-      if (u > s && m.in[u]) put(G.pair[(int64_t)G.nB * s + e]);
-    }
-  }
-  __syncthreads();
-  // global insertion order: a bitonic sort on (global index, entry), padded to a power of two
-  int64_t p2 = 1;
-  while (p2 < np) p2 <<= 1;
-  for (int64_t e = tid; e < p2; e += blockDim.x) {
-    if (e < np) {
-      const int64_t en = w.ent[e];
-      const int k = (int)(en >> kPairSetShift);
-      w.key[e] = P->s[k].gidx[en & kPairPosMask] & ~(1ll << 62);
-    } else {
-      w.key[e] = INT64_MAX;
-      w.ent[e] = -1;
-    }
-  }
-  __syncthreads();
-  for (int64_t k = 2; k <= p2; k <<= 1)
-    for (int64_t jj = k >> 1; jj > 0; jj >>= 1) {
-      for (int64_t e = tid; e < p2; e += blockDim.x) {
-        const int64_t o = e ^ jj;
-        if (o > e) {
-          const bool up = (e & k) == 0;
-          const int64_t ke = w.key[e], ko = w.key[o];
-          if (up ? ke > ko : ke < ko) {
-            w.key[e] = ko;
-            w.key[o] = ke;
-            const int64_t t = w.ent[e];
-            w.ent[e] = w.ent[o];
-            w.ent[o] = t;
-          }
-        }
-      }
-      __syncthreads();
-    }
-  for (int64_t e = tid; e < np; e += blockDim.x) {
-    const int64_t en = w.ent[e];
-    const int k = (int)(en >> kPairSetShift);
-    const int2 a = P->Ai[k][en & kPairPosMask];
-    w.ta[e] = bk_local<BUY>(G, m, a.x);
-    w.tb[e] = bk_local<BUY>(G, m, a.y);
-  }
-  __syncthreads();
-  // incidence lists in pool order: one warp per token, a ballot per 32 pools (count, then fill)
-  for (int t = warp; t < n; t += kSubgraphWarps) {
-    int c = 0;
-    for (int64_t b = 0; b < np; b += 32) {
-      const int64_t e = b + lane;
-      c += __popc(__ballot_sync(kFull, e < np && (w.ta[e] == t || w.tb[e] == t)));
-    }
-    if (lane == 0) m.inc_off[t + 1] = c;
-  }
-  __syncthreads();
-  if (tid == 0) {
-    m.inc_off[0] = 0;
-    for (int t = 0; t < n; ++t) m.inc_off[t + 1] += m.inc_off[t];
-  }
-  __syncthreads();
-  for (int t = warp; t < n; t += kSubgraphWarps) {
-    int c = m.inc_off[t];
-    for (int64_t b = 0; b < np; b += 32) {
-      const int64_t e = b + lane;
-      const bool ha = e < np && w.ta[e] == t, hb = e < np && w.tb[e] == t;
-      const unsigned hit = __ballot_sync(kFull, ha || hb);
-      if (ha || hb) w.inc[c + __popc(hit & ((1u << lane) - 1u))] = (int32_t)(2 * e + (hb ? 1 : 0));
-      c += __popc(hit);
-    }
-  }
-  __syncthreads();
+  });
+  sg_order_pools(P, w, m, np, n, [&](int32_t t) { return bk_local<BUY>(G, m, t); });
   // buy rows: the capacity of each bought entry over the row's pools, once, before any solve; a
   // shortfall makes the row unreachable
   if constexpr (BUY) {
@@ -579,108 +436,9 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
       __syncthreads();
     }
   }
-  // the solve
   const bool any = s_any, solve = any && !s_unreach;
-  double f = 0.0, merit = 0.0;
-  int status = -1;
-  if (tid == 0) {
-    s_iter = s_fev = s_small = 0;
-    hist.cnt = hist.head = 0;
-  }
-  if (solve) {
-    for (int t = tid; t < n; t += blockDim.x)  // an empty history, as cfmm_solve's zeroed one
-      for (int a = 0; a < kSolverM; ++a) m.S[a][t] = m.Y[a][t] = 0.0;
-    if constexpr (BUY)
-      sg_start<BasketBuySmem, true>(P, w, m, bk_root<BUY>(m));
-    else
-      sg_start(P, w, m);
-    f = bk_evaluate<BUY>(P, w, m);
-    merit = bk_commit<BUY>(m, 0, false);
-    if (tid == 0) {
-      s_fev = 1;
-      s_f = f;
-      s_merit = merit;
-    }
-    __syncthreads();
-    while (true) {
-      __syncthreads();  // every thread has read the last decision
-      // state: 0 run, 1 stop
-      if (tid == 0) {
-        s_state = 0;
-        if (!(s_f == s_f)) s_status = 5, s_state = 1;
-        else if (s_merit <= R.rtol) s_status = 0, s_state = 1;
-        else if (s_iter >= R.max_iter) s_status = 2, s_state = 1;
-        else if (s_fev >= R.max_fun) s_status = 3, s_state = 1;
-        else s_t = lbfgs_direction(m.W, hist, m.c);
-      }
-      __syncthreads();
-      if (s_state) break;
-      for (int t = tid; t < n; t += blockDim.x) {
-        double v = __dmul_rn(m.c[kSolverK - 1], m.pg[t]);
-#pragma unroll
-        for (int a = 0; a < kSolverM; ++a) {
-          v = fma(m.c[a], m.S[a][t], v);
-          v = fma(m.c[kSolverM + a], m.Y[a][t], v);
-        }
-        m.d[t] = bk_fixed<BUY>(m, t) || (m.x[t] <= bk_lo<BUY>(t) && m.g[t] > 0.0) ? 0.0 : -v;
-      }
-      __syncthreads();
-      int dec = kLsRetry;
-      double f_new = s_f;
-      for (int ls = 0; ls < 30 && s_fev < R.max_fun; ++ls) {
-        const double t = s_t;
-        double gd = 0.0, st2 = 0.0;
-        for (int k = tid; k < n; k += blockDim.x) {
-          const double y = bk_fixed<BUY>(m, k) ? 1.0 : fmax(fma(t, m.d[k], m.x[k]), bk_lo<BUY>(k));
-          m.xt[k] = y;
-          const double dx = __dsub_rn(y, m.x[k]);
-          gd = fma(m.g[k], dx, gd);
-          st2 = fma(dx, dx, st2);
-        }
-        const double gdx = sg_cta_sum(gd, m), step2 = sg_cta_sum(st2, m);
-        f_new = bk_evaluate<BUY>(P, w, m);
-        if (tid == 0) {
-          ++s_fev;
-          double tn = s_t;
-          s_state = lbfgs_trial(s_f, f_new, gdx, step2, hist.cnt, tn);
-          s_t = tn;
-        }
-        __syncthreads();
-        dec = s_state;
-        __syncthreads();
-        if (dec != kLsRetry) break;
-      }
-      if (dec != kLsAccept) {
-        if (tid == 0) {
-          if (hist.cnt > 0 && dec != kLsStall) {
-            hist.cnt = 0;  // drop the history and retry with steepest descent
-            s_state = 0;
-          } else {
-            s_status = dec == kLsStall ? 1 : 4;
-            s_state = 1;
-          }
-        }
-        __syncthreads();
-        if (s_state) break;
-        continue;
-      }
-      const int slot = hist.head;
-      const double mr = bk_commit<BUY>(m, slot, true);
-      if (tid == 0) {
-        lbfgs_store(m.W, slot, hist);
-        ++s_iter;
-        const double f_old = s_f;
-        s_f = f_new;
-        s_merit = mr;
-        s_state = lbfgs_factr(f_old, f_new, R.factr, s_small) ? 1 : 0;
-        if (s_state) s_status = 1;
-      }
-      __syncthreads();
-      if (s_state) break;
-    }
-    status = s_status;
-    merit = s_merit;
-  }
+  double merit;
+  const int status = sg_solve(P, w, m, BkRule<BUY>{}, R, n, solve, s, merit);
   // status, the limit, the legs (and the transition on execute)
   const double received = solve ? m.px[bk_root<BUY>(m)] : 0.0;
   uint8_t st = 0;  // CFMM_ORDER_FILLED (amounts all 0: zeros, no solve)
@@ -699,11 +457,7 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
         if (m.bamt[l] > 0.0 && !(m.px[l] >= m.bamt[l])) st = 5;
   }
   const bool filled = st == 0 && solve;
-  const int64_t l0 = R.leg_off[r];
-  for (int64_t e = tid; e < np; e += blockDim.x) {
-    if (R.leg_entry) R.leg_entry[l0 + e] = w.ent[e];
-    split_leg<EXEC>(P, filled, [&] { return sg_pool(P, w, e, m.x); }, mv, R.leg_delta, R.leg_lambda, l0 + e);
-  }
+  sg_legs<EXEC>(P, w, m.x, mv, R, r, np, filled);
   if (R.token) {
     const int64_t o = R.tok_off[r];
     for (int t = tid; t < n; t += blockDim.x) {
@@ -720,8 +474,8 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
     R.received[r] = filled ? received : 0.0;
     R.status[r] = st;
     R.solver_status[r] = status;
-    R.iterations[r] = solve ? s_iter : 0;
-    R.fun_evals[r] = solve ? s_fev : 0;
+    R.iterations[r] = solve ? s.iter : 0;
+    R.fun_evals[r] = solve ? s.fev : 0;
     R.merit[r] = solve ? merit : 0.0;
   }
   __syncthreads();  // the next row reuses the shared state and the workspace
@@ -734,15 +488,7 @@ __global__ void __launch_bounds__(kSubgraphThreads)
                     const uint8_t* __restrict__ gact, BasketRows R, SubgraphWork w, SplitMoved mv,
                     const int64_t* __restrict__ rows, int64_t n) {
   __shared__ BasketSmem m;
-  const int64_t c = w.cap * blockIdx.x;
-  SubgraphWork wb = w;
-  wb.ent += c;
-  wb.key += c;
-  wb.ta += c;
-  wb.tb += c;
-  wb.inc += 2 * c;
-  wb.ca += c;
-  wb.cb += c;
+  const SubgraphWork wb = sg_cta_work(w);
   for (int64_t k = blockIdx.x; k < n; k += gridDim.x)
     basket_row<EXEC>(P, ix, A, G, gact, R, wb, mv, rows ? rows[k] : k, m);
 }

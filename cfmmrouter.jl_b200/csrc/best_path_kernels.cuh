@@ -31,6 +31,42 @@ struct BestPathGraph {
   int nB;
 };
 
+// The position of b in the adjacency list A.nbr[a0 .. a1) (ascending), bisected; a1 when b is absent.
+__device__ __forceinline__ int64_t adj_find(AdjView A, int64_t a0, int64_t a1, int32_t b) {
+  int64_t lo = a0, hi = a1;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (A.nbr[mid] < b)
+      lo = mid + 1;
+    else
+      hi = mid;
+  }
+  return lo < a1 && A.nbr[lo] == b ? lo : a1;
+}
+
+// The pair {a, b} from a's adjacency list, −1 when there is none.
+__device__ __forceinline__ int32_t adj_pair(AdjView A, int32_t a, int32_t b) {
+  const int64_t a0 = A.off[a], a1 = A.off[a + 1], e = adj_find(A, a0, a1, b);
+  return e < a1 ? A.pair[e] : -1;
+}
+
+// The pair {t, tok[s]} into dst[s] for every slot s that has one, from t's adjacency list: walked when
+// it is short, else bisected per slot.
+__device__ __forceinline__ void side_pairs(AdjView A, const BestPathGraph& G, int32_t t, int32_t* dst) {
+  const int64_t a0 = A.off[t], a1 = A.off[t + 1];
+  if (a1 - a0 <= (int64_t)G.nB) {
+    for (int64_t e = a0 + threadIdx.x; e < a1; e += blockDim.x) {
+      const int32_t u = G.slot_of[A.nbr[e]];
+      if (u >= 0) dst[u] = A.pair[e];
+    }
+  } else {
+    for (int s = threadIdx.x; s < G.nB; s += blockDim.x) {
+      const int64_t e = adj_find(A, a0, a1, G.tok[s]);
+      if (e < a1) dst[s] = A.pair[e];
+    }
+  }
+}
+
 // One warp per slot: its adjacency list filtered to B, compacted in list order with a ballot.
 __global__ void best_path_graph_kernel(AdjView A, const int32_t* __restrict__ tok,
                                        const int32_t* __restrict__ slot_of, int nB, int32_t* __restrict__ deg,
@@ -162,42 +198,11 @@ __global__ void __launch_bounds__(kBestPathThreads)
   }
   if (tid == 0) direct = -1;
   __syncthreads();
-  // the pairs {S, b} and {b, T}: walk the token's list when it is short, else bisect it per slot
-  for (int side = 0; side < 2; ++side) {
-    const int32_t t = side ? T : S;
-    int32_t* dst = side ? epair : spair;
-    const int64_t a0 = A.off[t], a1 = A.off[t + 1];
-    if (a1 - a0 <= (int64_t)nB) {
-      for (int64_t e = a0 + tid; e < a1; e += blockDim.x) {
-        const int32_t u = G.slot_of[A.nbr[e]];
-        if (u >= 0) dst[u] = A.pair[e];
-      }
-    } else {
-      for (int s = tid; s < nB; s += blockDim.x) {
-        const int32_t b = G.tok[s];
-        int64_t lo = a0, hi = a1;
-        while (lo < hi) {
-          const int64_t mid = (lo + hi) >> 1;
-          if (A.nbr[mid] < b)
-            lo = mid + 1;
-          else
-            hi = mid;
-        }
-        if (lo < a1 && A.nbr[lo] == b) dst[s] = A.pair[lo];
-      }
-    }
-  }
+  // the pairs {S, b} and {b, T}
+  for (int side = 0; side < 2; ++side) side_pairs(A, G, side ? T : S, side ? epair : spair);
   if (tid == 0) {
-    int64_t lo = A.off[S], hi = A.off[S + 1];
-    const int64_t a1 = hi;
-    while (lo < hi) {
-      const int64_t mid = (lo + hi) >> 1;
-      if (A.nbr[mid] < T)
-        lo = mid + 1;
-      else
-        hi = mid;
-    }
-    if (lo < a1 && A.nbr[lo] == T) direct = A.pair[lo];
+    const int64_t a1 = A.off[S + 1], e = adj_find(A, A.off[S], a1, T);
+    if (e < a1) direct = A.pair[e];
   }
   __syncthreads();
   // level 1: one thread per slot, the pools of {S, b}, from the row's amount

@@ -3660,6 +3660,13 @@ int choose_order_hubs(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const i
 
 // ---- best paths through allowed tokens (best_path_kernels.cuh) ----------------------------------
 
+// The call's allowed tokens; a row's tokens besides its own are these less the row's own among them.
+int64_t count_allowed(const cfmm_ctx* ctx, const uint8_t* allowed) {
+  int64_t n = 0;
+  for (int64_t t = 0; t < ctx->n_tokens; ++t) n += allowed[t] != 0;
+  return n;
+}
+
 // Every argument of cfmm_find_order_paths, before anything runs: split orders' rows, max_hops, the
 // mask (required) and each row's |B| (the allowed tokens other than its two), and the CSR outputs.
 int check_find_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
@@ -3674,8 +3681,7 @@ int check_find_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
   if (q == 0) return CFMM_OK;
   if (!hop_off || !hop_type || !hop_pool || !hop_token)
     return fail(ctx, CFMM_ERR_INVALID, "%s: null hop_off, hop_type, hop_pool or hop_token", what);
-  int64_t n_allowed = 0;
-  for (int64_t t = 0; t < ctx->n_tokens; ++t) n_allowed += allowed[t] != 0;
+  const int64_t n_allowed = count_allowed(ctx, allowed);
   for (int64_t r = 0; r < q; ++r) {
     const int64_t nb = n_allowed - (allowed[token_in[r] - 1] != 0) - (allowed[token_out[r] - 1] != 0);
     if (nb > CFMM_BEST_PATH_MAX_TOKENS)
@@ -3964,8 +3970,7 @@ int check_subgraph(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int6
       return rc;
     }
   }
-  int64_t n_allowed = 0;
-  for (int64_t t = 0; t < ctx->n_tokens; ++t) n_allowed += allowed[t] != 0;
+  const int64_t n_allowed = count_allowed(ctx, allowed);
   for (int64_t r = 0; r < q; ++r) {
     const int64_t nb = n_allowed - (allowed[token_in[r] - 1] != 0) - (allowed[token_out[r] - 1] != 0);
     if (nb > CFMM_SUBGRAPH_MAX_TOKENS)
@@ -3991,8 +3996,7 @@ int check_basket(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64
   if (!token_out || !basket_off || !basket_token || !basket_amount)
     return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
   if (basket_off[0] != 0) return fail(ctx, CFMM_ERR_INVALID, "%s: basket_off[0] is %lld, not 0", what, (long long)basket_off[0]);
-  int64_t n_allowed = 0;
-  for (int64_t t = 0; t < ctx->n_tokens; ++t) n_allowed += allowed[t] != 0;
+  const int64_t n_allowed = count_allowed(ctx, allowed);
   for (int64_t r = 0; r < q; ++r) {
     const int64_t b0 = basket_off[r], K = basket_off[r + 1] - b0, i = token_out[r];
     if (K < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: basket_off decreases", what, (long long)r);
@@ -4035,28 +4039,46 @@ int check_basket(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64
   return CFMM_OK;
 }
 
-// The occupancy of a subgraph row kernel, cached per context.
-int subgraph_occupancy(cfmm_ctx* ctx, const void* kernel, int& occ) {
+// The occupancy of a row kernel, cached per context.  A family with dynamic shared memory (basket rows,
+// dyn: its kernels) may take that of the longest basket over the most slots, beyond the 48 KB default:
+// the attribute of each of its kernels is set once per context to that one value (so concurrent calls
+// never lower it), and the occupancy taken there.
+int row_occupancy(cfmm_ctx* ctx, const void* kernel, std::initializer_list<const void*> dyn, const char* name,
+                  int& occ) {
   int& c = ctx->occupancy[kernel];
   if (c == 0) {
-    CU_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, kernel, cfmm::kSubgraphThreads, 0));
-    if (c < 1) return fail(ctx, CFMM_ERR_CUDA, "a subgraph row kernel does not fit on an SM");
+    const int most = dyn.size() ? (int)cfmm::bk_dyn_bytes(cfmm::kBasketMaxTokens, cfmm::kSubgraphSlots) : 0;
+    for (const void* f : dyn) CU_TRY(ctx, cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+    CU_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, kernel, cfmm::kSubgraphThreads, (size_t)most));
+    if (c < 1) return fail(ctx, CFMM_ERR_CUDA, "%s does not fit on an SM", name);
   }
   occ = c;
   return CFMM_OK;
 }
 
-int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, const int64_t* token_out,
-                    const uint8_t* kind, const double* amount, const double* limit, const uint8_t* allowed,
-                    const cfmm_subgraph_opts& o, cfmm_subgraph_out* out) {
+extern "C++" template <class K>
+const void* kernel_ptr(K* k) {
+  return reinterpret_cast<const void*>(k);
+}
+
+// One subgraph or basket call after its checks, on the device of ctx with its inputs uploaded (R's input
+// pointers and options).  The family gives what differs:
+//   occ, occ2     the occupancy of its two row kernels (occ2 0 when no row takes the second);
+//   n2, second    the number of rows second(r) sends to the second kernel (exact-out rows, buy rows);
+//   K             its longest basket (0: subgraph rows), which sizes the dynamic shared memory;
+//   n_paid        the length of paid (q, or basket_off[q]);
+//   plan(...)     the plan launch; rows(exec_tag, second, ...) a launch of one row kernel;
+//   visit(r, v)   the tokens row r visits besides the slots (a token visited twice changes nothing),
+//                 and uses their count over the call, for the conflict levels of an execute.
+// The driver builds the call's slots and their B-graph, runs the plan, sizes the outputs and the per-CTA
+// workspace, runs the rows (a level's rows, or a quote's, split between the two kernels), and reads back.
+extern "C++" template <class Rows, class Out, class Plan, class RowLaunch, class Second, class Visit>
+int row_orders(cfmm_ctx* ctx, bool exec, int64_t q, const uint8_t* allowed, Rows R, const Out& O, int occ, int occ2,
+               int64_t n2, int K, int64_t n_paid, int64_t uses, const char* what, Plan plan, RowLaunch rows,
+               Second second, Visit visit) {
   int rc;
-  CU_TRY(ctx, cudaSetDevice(ctx->device));
-  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
-  if ((rc = ensure_adjacency(ctx)) != CFMM_OK) return rc;
   auto& ix = ctx->pairs;
   cudaStream_t st = ctx->stream;
-  cfmm_subgraph_out none{};
-  const cfmm_subgraph_out& O = out ? *out : none;
   // the call's slots: the allowed tokens, ascending; their filtered adjacency and its activity
   std::vector<int32_t> tok, slot_of((size_t)ctx->n_tokens, -1);
   for (int64_t t = 0; t < ctx->n_tokens; ++t)
@@ -4065,16 +4087,11 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
       tok.push_back((int32_t)t);
     }
   const int nB = (int)tok.size();
-  const size_t nn = (size_t)nB * (size_t)nB;
-  DevBuf<int64_t> d_in, d_out, d_ntok, d_npool;
+  const size_t nn = (size_t)nB * (size_t)nB, dyn = K > 0 ? cfmm::bk_dyn_bytes(K, nB) : 0;
+  DevBuf<int64_t> d_ntok, d_npool;
   DevBuf<int32_t> d_tok, d_slot, d_deg, d_gpair;
   DevBuf<int16_t> d_gnbr;
   DevBuf<uint8_t> d_act;
-  DevBuf<double> d_amount, d_limit;
-  CU_TRY(ctx, d_in.upload(token_in, (size_t)q));
-  CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
-  CU_TRY(ctx, d_amount.upload(amount, (size_t)q));
-  CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
   CU_TRY(ctx, d_tok.upload(tok));
   CU_TRY(ctx, d_slot.upload(slot_of));
   CU_TRY(ctx, d_deg.alloc((size_t)nB));
@@ -4089,14 +4106,7 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
   const cfmm::AdjView A{ix.adj_off.p, ix.adj_nbr.p, ix.adj_pair.p};
   const cfmm::BestPathGraph G{d_tok.p, d_slot.p, d_deg.p, d_gnbr.p, d_gpair.p, nB};
   // a persistent grid: one wave of resident CTAs of each kernel that runs
-  int occ = 0, occ_out = 0;
-  const auto kernel = [](auto k) { return reinterpret_cast<const void*>(k); };
-  if ((rc = subgraph_occupancy(ctx, kernel(&cfmm::subgraph_kernel<false>), occ)) != CFMM_OK) return rc;
-  const int64_t n_out = kind ? std::count(kind, kind + q, (uint8_t)CFMM_SWAP_EXACT_OUT) : 0;
-  if (n_out == 0) kind = nullptr;  // every row exact-in: the path of cfmm_quote_subgraph_orders
-  if (n_out > 0 && (rc = subgraph_occupancy(ctx, kernel(&cfmm::subgraph_out_kernel<false>), occ_out)) != CFMM_OK)
-    return rc;
-  const int64_t wave = (int64_t)ctx->sm_count * occ, wave_out = (int64_t)ctx->sm_count * occ_out;
+  const int64_t wave = (int64_t)ctx->sm_count * occ, wave2 = (int64_t)ctx->sm_count * occ2;
   const unsigned plan_grid = (unsigned)std::min<int64_t>(q, wave);
   if ((rc = launch(ctx, kProfSwaps, nB > 0 ? 3 : 1, [&] {
          if (nB > 0) {
@@ -4104,257 +4114,7 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
                A, d_tok.p, d_slot.p, nB, d_deg.p, d_gnbr.p, d_gpair.p);
            cfmm::subgraph_act_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>(os.d_P.p, pv, G, d_act.p);
          }
-         cfmm::subgraph_plan_kernel<<<plan_grid, cfmm::kSubgraphThreads, 0, st>>>(os.d_P.p, pv, A, G, d_act.p, d_in.p,
-                                                                                  d_out.p, q, d_ntok.p, d_npool.p);
-       })) != CFMM_OK)
-    return rc;
-  std::vector<int64_t> ntok((size_t)q), npool((size_t)q);
-  CU_TRY(ctx, read_back(ctx, ntok.data(), d_ntok.p, (size_t)q));
-  CU_TRY(ctx, read_back(ctx, npool.data(), d_npool.p, (size_t)q));
-  CU_TRY(ctx, cudaStreamSynchronize(st));
-  std::vector<int64_t> tok_off((size_t)q + 1, 0), leg_off((size_t)q + 1, 0);
-  int64_t max_pool = 0;
-  for (int64_t r = 0; r < q; ++r) {
-    tok_off[(size_t)r + 1] = tok_off[(size_t)r] + ntok[(size_t)r];
-    leg_off[(size_t)r + 1] = leg_off[(size_t)r] + npool[(size_t)r];
-    max_pool = std::max(max_pool, npool[(size_t)r]);
-  }
-  const int64_t NT = tok_off[(size_t)q], L = leg_off[(size_t)q];
-  if (O.tok_off) std::copy(tok_off.begin(), tok_off.end(), O.tok_off);
-  if (O.leg_off) std::copy(leg_off.begin(), leg_off.end(), O.leg_off);
-  const bool want_tok = O.token || O.nu || O.psi, want_leg = O.leg_type || O.leg_pool || O.leg_delta || O.leg_lambda;
-  if (exec && ((want_tok && NT > O.tok_cap) || (want_leg && L > O.leg_cap)))
-    return fail(ctx, CFMM_ERR_INVALID,
-                "execute_subgraph_orders: the outputs need %lld token and %lld leg entries, above tok_cap %lld or "
-                "leg_cap %lld",
-                (long long)NT, (long long)L, (long long)O.tok_cap, (long long)O.leg_cap);
-  const bool toks = want_tok && NT > 0 && NT <= O.tok_cap, legs = want_leg && L > 0 && L <= O.leg_cap;
-  // a size query (no per-row output, and no token or leg output that fits) runs no solve
-  if (!exec && !toks && !legs && !O.paid && !O.received && !O.status && !O.solver_status && !O.iterations &&
-      !O.fun_evals && !O.merit)
-    return CFMM_OK;
-  // outputs and the per-CTA workspace
-  DevBuf<int64_t> d_tok_off, d_leg_off, d_token, d_entry;
-  DevBuf<double> d_paid, d_recv, d_merit, d_nu, d_psi, d_ld, d_ll;
-  DevBuf<uint8_t> d_status;
-  DevBuf<int32_t> d_sst, d_iter, d_fev;
-  CU_TRY(ctx, d_tok_off.upload(tok_off));
-  CU_TRY(ctx, d_leg_off.upload(leg_off));
-  CU_TRY(ctx, d_paid.alloc((size_t)q));
-  CU_TRY(ctx, d_recv.alloc((size_t)q));
-  CU_TRY(ctx, d_merit.alloc((size_t)q));
-  CU_TRY(ctx, d_status.alloc((size_t)q));
-  CU_TRY(ctx, d_sst.alloc((size_t)q));
-  CU_TRY(ctx, d_iter.alloc((size_t)q));
-  CU_TRY(ctx, d_fev.alloc((size_t)q));
-  if (toks) {
-    CU_TRY(ctx, d_token.alloc((size_t)NT));
-    CU_TRY(ctx, d_nu.alloc((size_t)NT));
-    CU_TRY(ctx, d_psi.alloc((size_t)NT));
-  }
-  if (legs) {
-    CU_TRY(ctx, d_entry.alloc((size_t)L));
-    CU_TRY(ctx, d_ld.alloc((size_t)(2 * L)));
-    CU_TRY(ctx, d_ll.alloc((size_t)(2 * L)));
-  }
-  int64_t cap = 1;
-  while (cap < max_pool) cap <<= 1;
-  const int64_t grid = std::min<int64_t>(q, std::max(wave, wave_out));  // the workspaces
-  DevBuf<int64_t> w64;
-  DevBuf<int32_t> w32;
-  DevBuf<double> wd;
-  CU_TRY(ctx, w64.alloc((size_t)(2 * cap * grid)));
-  CU_TRY(ctx, w32.alloc((size_t)(4 * cap * grid)));
-  CU_TRY(ctx, wd.alloc((size_t)(2 * cap * grid)));
-  const cfmm::SubgraphWork W{w64.p, w64.p + cap * grid, w32.p, w32.p + cap * grid, w32.p + 2 * cap * grid,
-                             wd.p, wd.p + cap * grid, cap};
-  cfmm::SubgraphRows R{d_in.p,     d_out.p,   d_amount.p, d_limit.p,  o.max_iter, o.max_fun, o.rtol,
-                       o.factr,    d_tok_off.p, d_leg_off.p, d_paid.p, d_recv.p,   d_status.p, d_sst.p,
-                       d_iter.p,   d_fev.p,   d_merit.p,  d_token.p,  d_nu.p,     d_psi.p,   d_entry.p,
-                       d_ld.p,     d_ll.p};
-  // rows[0 .. n_in) exact-in, rows[n_in .. n) exact-out: one launch of each kernel that has rows
-  const auto run = [&](auto exec_tag, const cfmm::PathSets* P, const cfmm::SplitMoved& mv, const int64_t* rows,
-                       int64_t n_in, int64_t n) {
-    constexpr bool X = decltype(exec_tag)::value;
-    return launch(ctx, kProfSwaps, (n_in > 0) + (n > n_in), [&] {
-      if (n_in > 0)
-        cfmm::subgraph_kernel<X><<<(unsigned)std::min(n_in, wave), cfmm::kSubgraphThreads, 0, st>>>(
-            P, pv, A, G, d_act.p, R, W, mv, rows, n_in);
-      if (n > n_in)
-        cfmm::subgraph_out_kernel<X><<<(unsigned)std::min(n - n_in, wave_out), cfmm::kSubgraphThreads, 0, st>>>(
-            P, pv, A, G, d_act.p, R, W, mv, rows + n_in, n - n_in);
-    });
-  };
-  const auto exact_in = [&](int64_t r) { return kind[r] != CFMM_SWAP_EXACT_OUT; };
-  OrderSets xs;
-  if (!exec && !kind) {
-    if ((rc = launch(ctx, kProfSwaps, 1, [&] {
-           cfmm::subgraph_kernel<false><<<(unsigned)grid, cfmm::kSubgraphThreads, 0, st>>>(
-               os.d_P.p, pv, A, G, d_act.p, R, W, cfmm::SplitMoved{}, nullptr, q);
-         })) != CFMM_OK)
-      return rc;
-  } else if (!exec) {
-    std::vector<int64_t> rows((size_t)q);
-    std::iota(rows.begin(), rows.end(), (int64_t)0);
-    std::stable_partition(rows.begin(), rows.end(), exact_in);
-    DevBuf<int64_t> d_rows;
-    CU_TRY(ctx, d_rows.upload(rows));
-    if ((rc = run(std::false_type{}, os.d_P.p, cfmm::SplitMoved{}, d_rows.p, q - n_out, q)) != CFMM_OK) return rc;
-  } else {
-    if ((rc = order_sets(ctx, true, xs)) != CFMM_OK) return rc;
-    ctx->state_version++;
-    // levels over the tokens of {j, i} ∪ B (one table of n_tokens entries)
-    int64_t size = ctx->n_tokens, uses = q * (2 + (int64_t)nB);
-    std::vector<int64_t> order, level_off;
-    conflict_levels(
-        q, 1, &size, &uses,
-        [&](int64_t r, auto&& visit) {
-          visit(0, token_in[r] - 1);
-          visit(0, token_out[r] - 1);
-          for (int32_t t : tok)
-            if (t != token_in[r] - 1 && t != token_out[r] - 1) visit(0, t);
-        },
-        order, level_off);
-    // a level's rows share no token, so their order does not matter: its exact-in rows go first
-    std::vector<int64_t> level_in(level_off.size(), 0);
-    for (size_t Lv = 1; kind && Lv < level_off.size(); ++Lv) {
-      const auto b = order.begin() + level_off[Lv - 1], e = order.begin() + level_off[Lv];
-      level_in[Lv] = std::stable_partition(b, e, exact_in) - b;
-    }
-    DevBuf<int64_t> d_order;
-    CU_TRY(ctx, d_order.upload(order));
-    for (size_t Lv = 1; Lv < level_off.size(); ++Lv) {
-      const int64_t n = level_off[Lv] - level_off[Lv - 1];
-      if (kind) {
-        if ((rc = run(std::true_type{}, xs.d_P.p, xs.mv, d_order.p + level_off[Lv - 1], level_in[Lv], n)) != CFMM_OK)
-          return rc;
-        continue;
-      }
-      if ((rc = launch(ctx, kProfSwaps, 1, [&] {
-             cfmm::subgraph_kernel<true><<<(unsigned)std::min<int64_t>(n, grid), cfmm::kSubgraphThreads, 0, st>>>(
-                 xs.d_P.p, pv, A, G, d_act.p, R, W, xs.mv, d_order.p + level_off[Lv - 1], n);
-           })) != CFMM_OK)
-        return rc;
-    }
-    if ((rc = order_bookkeeping(ctx, xs)) != CFMM_OK) return rc;
-  }
-  CU_TRY(ctx, read_back(ctx, O.paid, d_paid.p, (size_t)q));
-  CU_TRY(ctx, read_back(ctx, O.received, d_recv.p, (size_t)q));
-  CU_TRY(ctx, read_back(ctx, O.status, d_status.p, (size_t)q));
-  CU_TRY(ctx, read_back(ctx, O.solver_status, d_sst.p, (size_t)q));
-  CU_TRY(ctx, read_back(ctx, O.iterations, d_iter.p, (size_t)q));
-  CU_TRY(ctx, read_back(ctx, O.fun_evals, d_fev.p, (size_t)q));
-  CU_TRY(ctx, read_back(ctx, O.merit, d_merit.p, (size_t)q));
-  std::vector<int64_t> ent(legs && (O.leg_type || O.leg_pool) ? (size_t)L : 0);
-  if (toks) {
-    CU_TRY(ctx, read_back(ctx, O.token, d_token.p, (size_t)NT));
-    CU_TRY(ctx, read_back(ctx, O.nu, d_nu.p, (size_t)NT));
-    CU_TRY(ctx, read_back(ctx, O.psi, d_psi.p, (size_t)NT));
-  }
-  if (legs) {
-    CU_TRY(ctx, read_back(ctx, ent.empty() ? nullptr : ent.data(), d_entry.p, (size_t)L));
-    CU_TRY(ctx, read_back(ctx, O.leg_delta, d_ld.p, (size_t)(2 * L)));
-    CU_TRY(ctx, read_back(ctx, O.leg_lambda, d_ll.p, (size_t)(2 * L)));
-  }
-  CU_TRY(ctx, cudaStreamSynchronize(st));
-  for (size_t t = 0; t < ent.size(); ++t) {  // (set, device position) -> (type, index in the type's order)
-    const int k = (int)(ent[t] >> cfmm::kPairSetShift);
-    const int64_t p = ent[t] & cfmm::kPairPosMask;
-    if (O.leg_type) O.leg_type[t] = k >> 1;
-    if (O.leg_pool) O.leg_pool[t] = path_set(ctx, k).order[(size_t)p] + ((k & 1) ? ctx->sets[k >> 1].m : 0);
-  }
-  return CFMM_OK;
-}
-
-// kind null: every row sell-only (cfmm_quote/execute_basket_orders).
-int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, const int64_t* basket_off,
-                  const int64_t* basket_token, const uint8_t* kind, const double* basket_amount, const double* limit,
-                  const uint8_t* allowed, const cfmm_subgraph_opts& o, const cfmm_basket_out& O, const char* what) {
-  int rc;
-  CU_TRY(ctx, cudaSetDevice(ctx->device));
-  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
-  if ((rc = ensure_adjacency(ctx)) != CFMM_OK) return rc;
-  auto& ix = ctx->pairs;
-  cudaStream_t st = ctx->stream;
-  // the call's slots: the allowed tokens, ascending; their filtered adjacency and its activity
-  std::vector<int32_t> tok, slot_of((size_t)ctx->n_tokens, -1);
-  for (int64_t t = 0; t < ctx->n_tokens; ++t)
-    if (allowed[t]) {
-      slot_of[(size_t)t] = (int32_t)tok.size();
-      tok.push_back((int32_t)t);
-    }
-  const int nB = (int)tok.size();
-  const size_t nn = (size_t)nB * (size_t)nB;
-  const int64_t NE = basket_off[q];
-  int K = 0;
-  for (int64_t r = 0; r < q; ++r) K = std::max<int>(K, (int)(basket_off[r + 1] - basket_off[r]));
-  const size_t dyn = cfmm::bk_dyn_bytes(K, nB);
-  DevBuf<int64_t> d_out, d_boff, d_btok, d_ntok, d_npool;
-  DevBuf<int32_t> d_tok, d_slot, d_deg, d_gpair;
-  DevBuf<int16_t> d_gnbr;
-  DevBuf<uint8_t> d_act, d_kind;
-  DevBuf<double> d_bamt, d_limit;
-  CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
-  CU_TRY(ctx, d_boff.upload(basket_off, (size_t)q + 1));
-  if (kind) CU_TRY(ctx, d_kind.upload(kind, (size_t)NE));
-  CU_TRY(ctx, d_btok.upload(basket_token, (size_t)NE));
-  CU_TRY(ctx, d_bamt.upload(basket_amount, (size_t)NE));
-  CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
-  CU_TRY(ctx, d_tok.upload(tok));
-  CU_TRY(ctx, d_slot.upload(slot_of));
-  CU_TRY(ctx, d_deg.alloc((size_t)nB));
-  CU_TRY(ctx, d_gnbr.alloc(nn));
-  CU_TRY(ctx, d_gpair.alloc(nn));
-  CU_TRY(ctx, d_act.alloc(nn));
-  CU_TRY(ctx, d_ntok.alloc((size_t)q));
-  CU_TRY(ctx, d_npool.alloc((size_t)q));
-  OrderSets os;
-  if ((rc = order_sets(ctx, false, os)) != CFMM_OK) return rc;
-  const cfmm::PairIndexView pv{ix.off.p, ix.pool.p};
-  const cfmm::AdjView A{ix.adj_off.p, ix.adj_nbr.p, ix.adj_pair.p};
-  const cfmm::BestPathGraph G{d_tok.p, d_slot.p, d_deg.p, d_gnbr.p, d_gpair.p, nB};
-  // a persistent grid: one wave of resident CTAs.  The kernels may take the dynamic shared memory of
-  // the longest basket over the most slots, beyond the 48 KB default; the attribute is set once per
-  // context to that one value (so concurrent calls never lower it), and the occupancy taken there.
-  int& occ = ctx->occupancy[reinterpret_cast<const void*>(&cfmm::basket_kernel<false>)];
-  if (occ == 0) {
-    const int most = (int)cfmm::bk_dyn_bytes(cfmm::kBasketMaxTokens, cfmm::kSubgraphSlots);
-    for (const void* f : {reinterpret_cast<const void*>(&cfmm::basket_plan_kernel),
-                          reinterpret_cast<const void*>(&cfmm::basket_kernel<false>),
-                          reinterpret_cast<const void*>(&cfmm::basket_kernel<true>)})
-      CU_TRY(ctx, cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
-    CU_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cfmm::basket_kernel<false>,
-                                                              cfmm::kSubgraphThreads, (size_t)most));
-    if (occ < 1) return fail(ctx, CFMM_ERR_CUDA, "basket_kernel does not fit on an SM");
-  }
-  // buy rows run basket_buy_kernel (sized the same way, once per context, when a call first has them)
-  int64_t n_buy = 0;
-  for (int64_t r = 0; r < q; ++r) n_buy += basket_buy_row(basket_off, kind, r);
-  if (n_buy == 0) kind = nullptr;  // every row sell-only: the path of cfmm_quote/execute_basket_orders
-  int occ_buy = 0;
-  if (n_buy > 0) {
-    int& ob = ctx->occupancy[reinterpret_cast<const void*>(&cfmm::basket_buy_kernel<false>)];
-    if (ob == 0) {
-      const int most = (int)cfmm::bk_dyn_bytes(cfmm::kBasketMaxTokens, cfmm::kSubgraphSlots);
-      for (const void* f : {reinterpret_cast<const void*>(&cfmm::basket_buy_kernel<false>),
-                            reinterpret_cast<const void*>(&cfmm::basket_buy_kernel<true>)})
-        CU_TRY(ctx, cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
-      CU_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ob, cfmm::basket_buy_kernel<false>,
-                                                                cfmm::kSubgraphThreads, (size_t)most));
-      if (ob < 1) return fail(ctx, CFMM_ERR_CUDA, "basket_buy_kernel does not fit on an SM");
-    }
-    occ_buy = ob;
-  }
-  const int64_t wave = (int64_t)ctx->sm_count * occ, wave_buy = (int64_t)ctx->sm_count * occ_buy;
-  const unsigned plan_grid = (unsigned)std::min<int64_t>(q, wave);
-  if ((rc = launch(ctx, kProfSwaps, nB > 0 ? 3 : 1, [&] {
-         if (nB > 0) {
-           cfmm::best_path_graph_kernel<<<(unsigned)((32 * (int64_t)nB + 255) / 256), 256, 0, st>>>(
-               A, d_tok.p, d_slot.p, nB, d_deg.p, d_gnbr.p, d_gpair.p);
-           cfmm::subgraph_act_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>(os.d_P.p, pv, G, d_act.p);
-         }
-         cfmm::basket_plan_kernel<<<plan_grid, cfmm::kSubgraphThreads, dyn, st>>>(
-             os.d_P.p, pv, A, G, d_act.p, d_boff.p, d_btok.p, d_out.p, q, d_ntok.p, d_npool.p);
+         plan(plan_grid, dyn, st, os.d_P.p, pv, A, G, d_act.p, d_ntok.p, d_npool.p);
        })) != CFMM_OK)
     return rc;
   std::vector<int64_t> ntok((size_t)q), npool((size_t)q);
@@ -4388,7 +4148,7 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
   DevBuf<int32_t> d_sst, d_iter, d_fev;
   CU_TRY(ctx, d_tok_off.upload(tok_off));
   CU_TRY(ctx, d_leg_off.upload(leg_off));
-  CU_TRY(ctx, d_paid.alloc((size_t)NE));
+  CU_TRY(ctx, d_paid.alloc((size_t)n_paid));
   CU_TRY(ctx, d_recv.alloc((size_t)q));
   CU_TRY(ctx, d_merit.alloc((size_t)q));
   CU_TRY(ctx, d_status.alloc((size_t)q));
@@ -4407,7 +4167,7 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
   }
   int64_t cap = 1;
   while (cap < max_pool) cap <<= 1;
-  const int64_t grid = std::min<int64_t>(q, std::max(wave, wave_buy));  // the workspaces
+  const int64_t grid = std::min<int64_t>(q, std::max(wave, wave2));  // the workspaces
   DevBuf<int64_t> w64;
   DevBuf<int32_t> w32;
   DevBuf<double> wd;
@@ -4416,78 +4176,71 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
   CU_TRY(ctx, wd.alloc((size_t)(2 * cap * grid)));
   const cfmm::SubgraphWork W{w64.p, w64.p + cap * grid, w32.p, w32.p + cap * grid, w32.p + 2 * cap * grid,
                              wd.p, wd.p + cap * grid, cap};
-  cfmm::BasketRows R{d_out.p,     d_boff.p,   d_btok.p,   d_bamt.p,  d_limit.p, o.max_iter, o.max_fun,
-                       o.rtol,      o.factr,    d_tok_off.p, d_leg_off.p, d_paid.p, d_recv.p,   d_status.p,
-                       d_sst.p,     d_iter.p,   d_fev.p,    d_merit.p, d_token.p, d_nu.p,     d_psi.p,
-                       d_entry.p,   d_ld.p,     d_ll.p};
-  // rows[0 .. n_sell) sell-only, rows[n_sell .. n) buy rows: one launch of each kernel that has rows
-  const auto run = [&](auto exec_tag, const cfmm::PathSets* P, const cfmm::SplitMoved& mv, const int64_t* rows,
-                       int64_t n_sell, int64_t n) {
-    constexpr bool X = decltype(exec_tag)::value;
-    return launch(ctx, kProfSwaps, (n_sell > 0) + (n > n_sell), [&] {
-      if (n_sell > 0)
-        cfmm::basket_kernel<X><<<(unsigned)std::min(n_sell, wave), cfmm::kSubgraphThreads, dyn, st>>>(
-            P, pv, A, G, d_act.p, R, W, mv, rows, n_sell);
-      if (n > n_sell)
-        cfmm::basket_buy_kernel<X><<<(unsigned)std::min(n - n_sell, wave_buy), cfmm::kSubgraphThreads, dyn, st>>>(
-            P, pv, A, G, d_act.p, R, d_kind.p, W, mv, rows + n_sell, n - n_sell);
+  R.tok_off = d_tok_off.p;
+  R.leg_off = d_leg_off.p;
+  R.paid = d_paid.p;
+  R.received = d_recv.p;
+  R.status = d_status.p;
+  R.solver_status = d_sst.p;
+  R.iterations = d_iter.p;
+  R.fun_evals = d_fev.p;
+  R.merit = d_merit.p;
+  R.token = d_token.p;
+  R.nu = d_nu.p;
+  R.psi = d_psi.p;
+  R.leg_entry = d_entry.p;
+  R.leg_delta = d_ld.p;
+  R.leg_lambda = d_ll.p;
+  // rows[0 .. n1) to the first kernel, rows[n1 .. n) to the second: one launch of each kernel that has
+  // rows (rows null: every row to the first)
+  const auto run = [&](auto exec_tag, const cfmm::PathSets* P, const cfmm::SplitMoved& mv, const int64_t* rows_,
+                       int64_t n1, int64_t n) {
+    return launch(ctx, kProfSwaps, (n1 > 0) + (n > n1), [&] {
+      if (n1 > 0) rows(exec_tag, false, (unsigned)std::min(n1, wave), dyn, st, P, pv, A, G, d_act.p, R, W, mv, rows_, n1);
+      if (n > n1)
+        rows(exec_tag, true, (unsigned)std::min(n - n1, wave2), dyn, st, P, pv, A, G, d_act.p, R, W, mv, rows_ + n1,
+             n - n1);
     });
   };
-  const auto sell_only = [&](int64_t r) { return !basket_buy_row(basket_off, kind, r); };
+  const auto first = [&](int64_t r) { return !second(r); };
   OrderSets xs;
-  if (!exec && !kind) {
-    if ((rc = launch(ctx, kProfSwaps, 1, [&] {
-           cfmm::basket_kernel<false><<<(unsigned)grid, cfmm::kSubgraphThreads, dyn, st>>>(
-               os.d_P.p, pv, A, G, d_act.p, R, W, cfmm::SplitMoved{}, nullptr, q);
-         })) != CFMM_OK)
-      return rc;
+  if (!exec && n2 == 0) {
+    if ((rc = run(std::false_type{}, os.d_P.p, cfmm::SplitMoved{}, nullptr, q, q)) != CFMM_OK) return rc;
   } else if (!exec) {
-    std::vector<int64_t> rows((size_t)q);
-    std::iota(rows.begin(), rows.end(), (int64_t)0);
-    std::stable_partition(rows.begin(), rows.end(), sell_only);
+    std::vector<int64_t> order((size_t)q);
+    std::iota(order.begin(), order.end(), (int64_t)0);
+    std::stable_partition(order.begin(), order.end(), first);
     DevBuf<int64_t> d_rows;
-    CU_TRY(ctx, d_rows.upload(rows));
-    if ((rc = run(std::false_type{}, os.d_P.p, cfmm::SplitMoved{}, d_rows.p, q - n_buy, q)) != CFMM_OK) return rc;
+    CU_TRY(ctx, d_rows.upload(order));
+    if ((rc = run(std::false_type{}, os.d_P.p, cfmm::SplitMoved{}, d_rows.p, q - n2, q)) != CFMM_OK) return rc;
   } else {
     if ((rc = order_sets(ctx, true, xs)) != CFMM_OK) return rc;
     ctx->state_version++;
-    // levels over the tokens of {i} ∪ basket ∪ B (one table of n_tokens entries; a token visited
-    // twice changes nothing)
-    int64_t size = ctx->n_tokens, uses = q * (1 + (int64_t)nB) + NE;
+    // levels over the tokens the rows visit and B (one table of n_tokens entries)
+    int64_t size = ctx->n_tokens, use = uses + q * (int64_t)nB;
     std::vector<int64_t> order, level_off;
     conflict_levels(
-        q, 1, &size, &uses,
-        [&](int64_t r, auto&& visit) {
-          visit(0, token_out[r] - 1);
-          for (int64_t k = basket_off[r]; k < basket_off[r + 1]; ++k) visit(0, basket_token[k] - 1);
-          for (int32_t t : tok) visit(0, t);
+        q, 1, &size, &use,
+        [&](int64_t r, auto&& v) {
+          visit(r, v);
+          for (int32_t t : tok) v(0, t);
         },
         order, level_off);
-    // a level's rows share no token, so their order does not matter: its sell-only rows go first
-    std::vector<int64_t> level_sell(level_off.size(), 0);
-    for (size_t Lv = 1; kind && Lv < level_off.size(); ++Lv) {
-      const auto b = order.begin() + level_off[Lv - 1], e = order.begin() + level_off[Lv];
-      level_sell[Lv] = std::stable_partition(b, e, sell_only) - b;
-    }
+    // a level's rows share no token, so their order does not matter: its first kernel's rows go first
     DevBuf<int64_t> d_order;
-    CU_TRY(ctx, d_order.upload(order));
+    std::vector<int64_t> level_first(level_off.size(), 0);
     for (size_t Lv = 1; Lv < level_off.size(); ++Lv) {
-      const int64_t n = level_off[Lv] - level_off[Lv - 1];
-      if (kind) {
-        if ((rc = run(std::true_type{}, xs.d_P.p, xs.mv, d_order.p + level_off[Lv - 1], level_sell[Lv], n)) !=
-            CFMM_OK)
-          return rc;
-        continue;
-      }
-      if ((rc = launch(ctx, kProfSwaps, 1, [&] {
-             cfmm::basket_kernel<true><<<(unsigned)std::min<int64_t>(n, grid), cfmm::kSubgraphThreads, dyn, st>>>(
-                 xs.d_P.p, pv, A, G, d_act.p, R, W, xs.mv, d_order.p + level_off[Lv - 1], n);
-           })) != CFMM_OK)
-        return rc;
+      const auto b = order.begin() + level_off[Lv - 1], e = order.begin() + level_off[Lv];
+      level_first[Lv] = n2 > 0 ? std::stable_partition(b, e, first) - b : e - b;
     }
+    CU_TRY(ctx, d_order.upload(order));
+    for (size_t Lv = 1; Lv < level_off.size(); ++Lv)
+      if ((rc = run(std::true_type{}, xs.d_P.p, xs.mv, d_order.p + level_off[Lv - 1], level_first[Lv],
+                    level_off[Lv] - level_off[Lv - 1])) != CFMM_OK)
+        return rc;
     if ((rc = order_bookkeeping(ctx, xs)) != CFMM_OK) return rc;
   }
-  CU_TRY(ctx, read_back(ctx, O.paid, d_paid.p, (size_t)NE));
+  CU_TRY(ctx, read_back(ctx, O.paid, d_paid.p, (size_t)n_paid));
   CU_TRY(ctx, read_back(ctx, O.received, d_recv.p, (size_t)q));
   CU_TRY(ctx, read_back(ctx, O.status, d_status.p, (size_t)q));
   CU_TRY(ctx, read_back(ctx, O.solver_status, d_sst.p, (size_t)q));
@@ -4513,6 +4266,114 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
     if (O.leg_pool) O.leg_pool[t] = path_set(ctx, k).order[(size_t)p] + ((k & 1) ? ctx->sets[k >> 1].m : 0);
   }
   return CFMM_OK;
+}
+
+// The device, the stream and the token adjacency of a subgraph or basket call.
+int row_begin(cfmm_ctx* ctx) {
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  int rc = use_stream(ctx, ctx->stream);
+  return rc != CFMM_OK ? rc : ensure_adjacency(ctx);
+}
+
+int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                    const uint8_t* kind, const double* amount, const double* limit, const uint8_t* allowed,
+                    const cfmm_subgraph_opts& o, cfmm_subgraph_out* out) {
+  int rc;
+  if ((rc = row_begin(ctx)) != CFMM_OK) return rc;
+  cfmm_subgraph_out none{};
+  DevBuf<int64_t> d_in, d_out;
+  DevBuf<double> d_amount, d_limit;
+  CU_TRY(ctx, d_in.upload(token_in, (size_t)q));
+  CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
+  CU_TRY(ctx, d_amount.upload(amount, (size_t)q));
+  CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
+  int occ = 0, occ_out = 0;
+  const char* name = "a subgraph row kernel";
+  if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::subgraph_kernel<false>), {}, name, occ)) != CFMM_OK) return rc;
+  const int64_t n_out = kind ? std::count(kind, kind + q, (uint8_t)CFMM_SWAP_EXACT_OUT) : 0;
+  if (n_out > 0 && (rc = row_occupancy(ctx, kernel_ptr(&cfmm::subgraph_out_kernel<false>), {}, name, occ_out)) != CFMM_OK)
+    return rc;
+  cfmm::SubgraphRows R{d_in.p, d_out.p, d_amount.p, d_limit.p, o.max_iter, o.max_fun, o.rtol, o.factr};
+  return row_orders(
+      ctx, exec, q, allowed, R, out ? *out : none, occ, occ_out, n_out, 0, q, 2 * q, "execute_subgraph_orders",
+      [&](unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P, cfmm::PairIndexView pv, cfmm::AdjView A,
+          const cfmm::BestPathGraph& G, const uint8_t* act, int64_t* ntok, int64_t* npool) {
+        cfmm::subgraph_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, d_in.p, d_out.p, q,
+                                                                              ntok, npool);
+      },
+      [&](auto exec_tag, bool second, unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P,
+          cfmm::PairIndexView pv, cfmm::AdjView A, const cfmm::BestPathGraph& G, const uint8_t* act,
+          const cfmm::SubgraphRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv, const int64_t* rows,
+          int64_t n) {
+        constexpr bool X = decltype(exec_tag)::value;
+        if (second)
+          cfmm::subgraph_out_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, R, W, mv, rows, n);
+        else
+          cfmm::subgraph_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, R, W, mv, rows, n);
+      },
+      [&](int64_t r) { return kind[r] == CFMM_SWAP_EXACT_OUT; },
+      [&](int64_t r, auto&& visit) {
+        visit(0, token_in[r] - 1);
+        visit(0, token_out[r] - 1);
+      });
+}
+
+// kind null: every row sell-only (cfmm_quote/execute_basket_orders).
+int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                  const int64_t* basket_token, const uint8_t* kind, const double* basket_amount, const double* limit,
+                  const uint8_t* allowed, const cfmm_subgraph_opts& o, const cfmm_basket_out& O, const char* what) {
+  int rc;
+  if ((rc = row_begin(ctx)) != CFMM_OK) return rc;
+  const int64_t NE = basket_off[q];
+  int K = 0;
+  for (int64_t r = 0; r < q; ++r) K = std::max<int>(K, (int)(basket_off[r + 1] - basket_off[r]));
+  DevBuf<int64_t> d_out, d_boff, d_btok;
+  DevBuf<uint8_t> d_kind;
+  DevBuf<double> d_bamt, d_limit;
+  CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
+  CU_TRY(ctx, d_boff.upload(basket_off, (size_t)q + 1));
+  if (kind) CU_TRY(ctx, d_kind.upload(kind, (size_t)NE));
+  CU_TRY(ctx, d_btok.upload(basket_token, (size_t)NE));
+  CU_TRY(ctx, d_bamt.upload(basket_amount, (size_t)NE));
+  CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
+  int occ = 0, occ_buy = 0;
+  if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::basket_kernel<false>),
+                          {kernel_ptr(&cfmm::basket_plan_kernel), kernel_ptr(&cfmm::basket_kernel<false>),
+                           kernel_ptr(&cfmm::basket_kernel<true>)},
+                          "basket_kernel", occ)) != CFMM_OK)
+    return rc;
+  // buy rows run basket_buy_kernel (sized the same way, once per context, when a call first has them)
+  int64_t n_buy = 0;
+  for (int64_t r = 0; r < q; ++r) n_buy += basket_buy_row(basket_off, kind, r);
+  if (n_buy > 0 &&
+      (rc = row_occupancy(ctx, kernel_ptr(&cfmm::basket_buy_kernel<false>),
+                          {kernel_ptr(&cfmm::basket_buy_kernel<false>), kernel_ptr(&cfmm::basket_buy_kernel<true>)},
+                          "basket_buy_kernel", occ_buy)) != CFMM_OK)
+    return rc;
+  cfmm::BasketRows R{d_out.p, d_boff.p, d_btok.p, d_bamt.p, d_limit.p, o.max_iter, o.max_fun, o.rtol, o.factr};
+  return row_orders(
+      ctx, exec, q, allowed, R, O, occ, occ_buy, n_buy, K, NE, q + NE, what,
+      [&](unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P, cfmm::PairIndexView pv, cfmm::AdjView A,
+          const cfmm::BestPathGraph& G, const uint8_t* act, int64_t* ntok, int64_t* npool) {
+        cfmm::basket_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, d_boff.p, d_btok.p,
+                                                                            d_out.p, q, ntok, npool);
+      },
+      [&](auto exec_tag, bool second, unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P,
+          cfmm::PairIndexView pv, cfmm::AdjView A, const cfmm::BestPathGraph& G, const uint8_t* act,
+          const cfmm::BasketRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv, const int64_t* rows,
+          int64_t n) {
+        constexpr bool X = decltype(exec_tag)::value;
+        if (second)
+          cfmm::basket_buy_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, R, d_kind.p, W, mv,
+                                                                                rows, n);
+        else
+          cfmm::basket_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, R, W, mv, rows, n);
+      },
+      [&](int64_t r) { return basket_buy_row(basket_off, kind, r); },
+      [&](int64_t r, auto&& visit) {
+        visit(0, token_out[r] - 1);
+        for (int64_t k = basket_off[r]; k < basket_off[r + 1]; ++k) visit(0, basket_token[k] - 1);
+      });
 }
 
 cfmm_subgraph_opts subgraph_opts(const cfmm_subgraph_opts* in) {

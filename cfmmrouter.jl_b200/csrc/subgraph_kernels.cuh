@@ -14,10 +14,15 @@
 //           the pool's stored tokens), then sums them per token in a fixed warp tree;
 //   legs    split_leg over the pools at the final ν: the legs and, on execute, the transition.
 // subgraph_kernel solves exact-in rows, subgraph_out_kernel exact-out rows: the same row with the
-// linear term, the box, the start's root and the stop's scale of its kind, fixed at compile time.
-// subgraph_plan_kernel runs the setup only and reports each row's token and pool counts, which size
-// the outputs and the workspace (they do not depend on the kind).  basket_kernels.cuh's basket rows share the pair activity, the
-// workspace, the side pairs, the CTA sum, the pool view, the start and (buy rows) the capacity.
+// linear term, the box, the start's root and the stop's scale of its kind (SgRule), fixed at compile
+// time.  subgraph_plan_kernel runs the setup only and reports each row's token and pool counts, which
+// size the outputs and the workspace (they do not depend on the kind).
+//
+// basket_kernels.cuh's rows run everything after their own setup through this file's helpers, which
+// take the row's shared state and its rules as template parameters: the pool gather, the pool
+// ordering, the evaluation, the commit, the L-BFGS driver, the legs, and the pair activity, CTA sum,
+// pool view, start and capacity.  The setups stay per kind: running subgraph rows through the longer
+// basket setup cost 2.3–2.6 % more kernel time on the headline set (DESIGN §4.5).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -111,30 +116,6 @@ struct SubgraphSmem {
 
 __device__ __forceinline__ bool sg_slot_ok(const SubgraphSmem& m, int s) { return s != m.jslot && s != m.islot; }
 
-// The pair {t, tok[s]} for every slot s, from t's adjacency list: walked when short, else bisected.
-__device__ __forceinline__ void sg_side_pairs(AdjView A, const BestPathGraph& G, int32_t t, int32_t* dst) {
-  const int64_t a0 = A.off[t], a1 = A.off[t + 1];
-  if (a1 - a0 <= (int64_t)G.nB) {
-    for (int64_t e = a0 + threadIdx.x; e < a1; e += blockDim.x) {
-      const int32_t u = G.slot_of[A.nbr[e]];
-      if (u >= 0) dst[u] = A.pair[e];
-    }
-  } else {
-    for (int s = threadIdx.x; s < G.nB; s += blockDim.x) {
-      const int32_t b = G.tok[s];
-      int64_t lo = a0, hi = a1;
-      while (lo < hi) {
-        const int64_t mid = (lo + hi) >> 1;
-        if (A.nbr[mid] < b)
-          lo = mid + 1;
-        else
-          hi = mid;
-      }
-      if (lo < a1 && A.nbr[lo] == b) dst[s] = A.pair[lo];
-    }
-  }
-}
-
 // Setup of row (j, i), 0-based: T, the local tokens and the pool count of every slot (cnt[s], the
 // pools of the pairs {s, i}, {s, j} when j ∈ T, and {s, u} for slots u > s in T) and of {j, i}.
 __device__ void sg_setup(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
@@ -148,21 +129,12 @@ __device__ void sg_setup(const PathSets* P, PairIndexView ix, AdjView A, const B
   if (tid == 0) {
     m.jslot = G.slot_of[j];
     m.islot = G.slot_of[i];
-    int64_t lo = A.off[j], hi = A.off[j + 1];
-    const int64_t a1 = hi;
-    while (lo < hi) {
-      const int64_t mid = (lo + hi) >> 1;
-      if (A.nbr[mid] < i)
-        lo = mid + 1;
-      else
-        hi = mid;
-    }
-    m.direct = lo < a1 && A.nbr[lo] == i ? A.pair[lo] : -1;
+    m.direct = adj_pair(A, j, i);
     m.jin = m.direct >= 0 && subgraph_pair_active(P, ix, m.direct);
   }
   __syncthreads();
-  sg_side_pairs(A, G, j, m.jpair);
-  sg_side_pairs(A, G, i, m.ipair);
+  side_pairs(A, G, j, m.jpair);
+  side_pairs(A, G, i, m.ipair);
   __syncthreads();
   for (int s = tid; s < nB; s += blockDim.x) {
     const bool ok = sg_slot_ok(m, s);
@@ -281,12 +253,41 @@ __device__ __forceinline__ SplitPool sg_pool(const PathSets* P, const SubgraphWo
   return sp;
 }
 
-// One evaluation at ν = xt: every pool's contributions, Ψ_t -> pt, gt = lin + Ψ, and the dual's
-// value linᵀxt + Σ val (returned to every thread).  lin is amt at j (slot 1) for exact-in rows and
-// amt = −y′ at i (slot 0) for exact-out rows.
+__device__ __forceinline__ double sg_lower(int t) { return t == 0 ? 1.0 + kSubgraphSqrtEps : kSubgraphSqrtEps; }
+
+// The box of slot t.  Exact-in: ν_i >= 1 + √eps, ν_t >= √eps otherwise.  Exact-out: ν_j = 1 (slot 1
+// is fixed), ν_t >= √eps otherwise, i included.
 template <bool OUT>
-__device__ double sg_evaluate(const PathSets* P, const SubgraphWork& w, SubgraphSmem& m, double amt) {
-  constexpr int kLin = OUT ? 0 : 1;
+__device__ __forceinline__ double sg_lo(int t) { return OUT ? kSubgraphSqrtEps : sg_lower(t); }
+
+// The rules of an exact-in (OUT false) or exact-out row, the only part of the solve that depends on the
+// row kind (basket_kernels.cuh's BkRule gives the same for basket rows):
+//   lin(m, t)     the linear term of slot t's gradient: lin at kLin (amt at j, or −y′ at i), else 0;
+//   value(m)      the dual's linear value at ν = xt, lin·ν_kLin;
+//   lo(t), fixed(m, t)   the box;
+//   kOut, root(m) sg_start's root and clamp (exact-out: slot 1, j, fixed at 1);
+//   merit(m, mx)  m_r from the CTA max mx = max_t ν_t·|pg_t|: mx / (δ·ν_j), or mx / (y·ν_i).
+// Every value is the same IEEE operations in the same order as the rule's other uses, so a one-entry
+// basket row gives an exact-in row's bits and a one-bought-entry buy row an exact-out row's.
+template <bool OUT>
+struct SgRule {
+  static constexpr bool kOut = OUT;
+  static constexpr int kLin = OUT ? 0 : 1;
+  double lin, amt;
+  __device__ __forceinline__ double lin_at(const SubgraphSmem&, int t) const { return t == kLin ? lin : 0.0; }
+  __device__ __forceinline__ double value(const SubgraphSmem& m) const { return __dmul_rn(lin, m.xt[kLin]); }
+  __device__ __forceinline__ double lo(int t) const { return sg_lo<OUT>(t); }
+  __device__ __forceinline__ bool fixed(const SubgraphSmem&, int t) const { return OUT && t == 1; }
+  __device__ __forceinline__ int root(const SubgraphSmem&) const { return OUT ? 1 : 0; }
+  __device__ __forceinline__ double merit(const SubgraphSmem& m, double mx) const {
+    return __ddiv_rn(mx, __dmul_rn(amt, m.x[OUT ? 0 : 1]));
+  }
+};
+
+// One evaluation at ν = xt: every pool's contributions, Ψ_t -> pt, gt = lin + Ψ, and the dual's
+// value linᵀxt + Σ val (returned to every thread).
+template <class Smem, class Rule>
+__device__ double sg_evaluate(const PathSets* P, const SubgraphWork& w, Smem& m, const Rule& rule) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int64_t np = m.npool;
   double vs = 0.0;
@@ -309,27 +310,18 @@ __device__ double sg_evaluate(const PathSets* P, const SubgraphWork& w, Subgraph
     for (int o = 16; o >= 1; o >>= 1) s = __dadd_rn(s, __shfl_xor_sync(kFull, s, o));
     if (lane == 0) {
       m.pt[t] = s;
-      m.gt[t] = __dadd_rn(t == kLin ? amt : 0.0, s);
+      m.gt[t] = __dadd_rn(rule.lin_at(m, t), s);
     }
   }
   __syncthreads();
-  return __dadd_rn(__dmul_rn(amt, m.xt[kLin]), V);
+  return __dadd_rn(rule.value(m), V);
 }
-
-__device__ __forceinline__ double sg_lower(int t) { return t == 0 ? 1.0 + kSubgraphSqrtEps : kSubgraphSqrtEps; }
-
-// The box of slot t.  Exact-in: ν_i >= 1 + √eps, ν_t >= √eps otherwise.  Exact-out: ν_j = 1 (slot 1
-// is fixed: sg_fixed), ν_t >= √eps otherwise, i included.
-template <bool OUT>
-__device__ __forceinline__ double sg_lo(int t) { return OUT ? kSubgraphSqrtEps : sg_lower(t); }
-template <bool OUT>
-__device__ __forceinline__ bool sg_fixed(int t) { return OUT && t == 1; }
 
 // Accept xt: (s, y) into history slot `slot` when store, x <- xt, g <- gt, Ψ, the projected gradient
 // and the Gram matrix of [S Y pg] (one warp per entry group, lanes over the tokens, butterfly).
-// Returns m_r = max_t ν_t·|pg_t| / (δ·ν_j) (exact-in, amt = δ) or / (y·ν_i) (exact-out, amt = y).
-template <bool OUT>
-__device__ double sg_commit(SubgraphSmem& m, int slot, bool store, double amt) {
+// Returns the rule's m_r.
+template <class Smem, class Rule>
+__device__ double sg_commit(Smem& m, int slot, bool store, const Rule& rule) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = m.n_loc;
   if (tid == 0) m.mx = 0ull;
   for (int t = tid; t < n; t += blockDim.x) {
@@ -341,7 +333,7 @@ __device__ double sg_commit(SubgraphSmem& m, int slot, bool store, double amt) {
     m.x[t] = xn;
     m.g[t] = gn;
     m.px[t] = m.pt[t];
-    m.pg[t] = sg_fixed<OUT>(t) || (xn <= sg_lo<OUT>(t) && gn > 0.0) ? 0.0 : gn;
+    m.pg[t] = rule.fixed(m, t) || (xn <= rule.lo(t) && gn > 0.0) ? 0.0 : gn;
   }
   __syncthreads();
   double mx = 0.0;
@@ -361,7 +353,7 @@ __device__ double sg_commit(SubgraphSmem& m, int slot, bool store, double amt) {
     if (lane == 0) m.W[r][c] = m.W[c][r] = s;
   }
   __syncthreads();
-  return __ddiv_rn(__longlong_as_double((long long)m.mx), __dmul_rn(amt, m.x[OUT ? 0 : 1]));
+  return rule.merit(m, __longlong_as_double((long long)m.mx));
 }
 
 // The start ν⁰: ν_root = 1 (slot 0, i; exact-out: slot 1, j; basket buy rows: i's slot); then
@@ -417,28 +409,27 @@ __device__ __forceinline__ double sg_capacity(const PathSets* P, const SubgraphW
   return swap_pool<2>(S, sp.p).f(__longlong_as_double(kSwapOrdMax), !a);
 }
 
-// Row r on the current state.  Returns nothing; writes the row's outputs.  EXEC: the limit decides,
-// and a filled row applies the transition of cfmm_apply_trades at its ν to each of its pools.  OUT:
-// the row buys y = amount of i; its dual has lin = −y′ at i, y′ = y·(1 + rtol) rounded up, and ν_j
-// fixed at 1; it is unreachable when y is at least what its pools holding i could pay out.
-template <bool EXEC, bool OUT>
-__device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
-                             const uint8_t* gact, const SubgraphRows& R, const SubgraphWork& w, const SplitMoved& mv,
-                             int64_t r, SubgraphSmem& m) {
-  __shared__ LbfgsHistory hist;
-  __shared__ double s_f, s_t, s_merit;
-  __shared__ int s_state, s_status, s_iter, s_fev, s_small;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int32_t j = (int32_t)(R.token_in[r] - 1), i = (int32_t)(R.token_out[r] - 1);
-  const double amt = R.amount[r];
-  const double lin = OUT ? -__fma_ru(amt, R.rtol, amt) : amt;
-  sg_setup(P, ix, A, G, gact, j, i, m);
-  const int64_t np = m.npool, n = m.n_loc;
-  // the pools: {j, i} first, then each slot's, at the offsets the setup counted
-  if (tid == 0 && m.direct_cnt > 0) {
-    for (int64_t e = ix.off[m.direct]; e < ix.off[m.direct + 1]; ++e) w.ent[e - ix.off[m.direct]] = ix.pool[e];
-  }
-  for (int s = tid; s < G.nB; s += blockDim.x) {
+// CTA b's workspace: workspace b of w.
+__device__ __forceinline__ SubgraphWork sg_cta_work(const SubgraphWork& w) {
+  const int64_t c = w.cap * blockIdx.x;
+  SubgraphWork wb = w;
+  wb.ent += c;
+  wb.key += c;
+  wb.ta += c;
+  wb.tb += c;
+  wb.inc += 2 * c;
+  wb.ca += c;
+  wb.cb += c;
+  return wb;
+}
+
+// The pools of every slot s in T into the workspace at the offset the setup counted (cnt[s]): {s, i},
+// then the row kind's side pairs of s (side(s, put)), then {s, u} for the slots u > s in T.  Then a
+// barrier, which also publishes the row's leading pools.
+template <class Smem, class Side>
+__device__ __forceinline__ void sg_gather(PairIndexView ix, const BestPathGraph& G, const SubgraphWork& w,
+                                          const Smem& m, Side side) {
+  for (int s = threadIdx.x; s < G.nB; s += blockDim.x) {
     if (!m.in[s]) continue;
     int64_t o = m.cnt[s];
     const auto put = [&](int64_t k) {
@@ -446,7 +437,7 @@ __device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, con
       for (int64_t e = ix.off[k]; e < ix.off[k + 1]; ++e) w.ent[o++] = ix.pool[e];
     };
     put(m.ipair[s]);
-    if (m.jin) put(m.jpair[s]);
+    side(s, put);
     const int dg = G.deg[s];
     for (int e = 0; e < dg; ++e) {
       const int u = G.nbr[(int64_t)G.nB * s + e];
@@ -454,7 +445,16 @@ __device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, con
     }
   }
   __syncthreads();
-  // global insertion order: a bitonic sort on (global index, entry), padded to a power of two
+}
+
+// The row's np pools into global insertion order (a bitonic sort on (global index, entry), padded to a
+// power of two), each pool's stored tokens as local slots (local(t), t 0-based), and for each of the n
+// local tokens an incidence list in pool order (one warp per token, a ballot per 32 pools: count, then
+// fill).
+template <class Smem, class Local>
+__device__ __forceinline__ void sg_order_pools(const PathSets* P, const SubgraphWork& w, Smem& m, int64_t np,
+                                               int64_t n, Local local) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   int64_t p2 = 1;
   while (p2 < np) p2 <<= 1;
   for (int64_t e = tid; e < p2; e += blockDim.x) {
@@ -490,11 +490,10 @@ __device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, con
     const int64_t en = w.ent[e];
     const int k = (int)(en >> kPairSetShift);
     const int2 a = P->Ai[k][en & kPairPosMask];
-    w.ta[e] = sg_local(G, m, a.x);
-    w.tb[e] = sg_local(G, m, a.y);
+    w.ta[e] = local(a.x);
+    w.tb[e] = local(a.y);
   }
   __syncthreads();
-  // incidence lists in pool order: one warp per token, a ballot per 32 pools (count, then fill)
   for (int t = warp; t < n; t += kSubgraphWarps) {
     int c = 0;
     for (int64_t b = 0; b < np; b += 32) {
@@ -520,6 +519,155 @@ __device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, con
     }
   }
   __syncthreads();
+}
+
+// The solve's CTA-wide state: thread 0 decides, every thread reads after a barrier.
+struct SgSolveState {
+  LbfgsHistory hist;
+  double f, t, merit;
+  int state, status, iter, fev, small;
+};
+
+// cfmm_solve's projected L-BFGS (solver_control.cuh) on the row's dual over its n local tokens, every
+// vector in shared memory, from sg_start when solve (else nothing runs).  Returns the solver status
+// (−1: no solve) and sets merit to the last m_r; s keeps the iteration and evaluation counts.
+template <class Smem, class Rule, class Rows>
+__device__ __forceinline__ int sg_solve(const PathSets* P, const SubgraphWork& w, Smem& m, const Rule& rule,
+                                        const Rows& R, int64_t n, bool solve, SgSolveState& s, double& merit) {
+  const int tid = threadIdx.x;
+  double f = 0.0;
+  int status = -1;
+  merit = 0.0;
+  if (tid == 0) {
+    s.iter = s.fev = s.small = 0;
+    s.hist.cnt = s.hist.head = 0;
+  }
+  if (!solve) return status;
+  for (int t = tid; t < n; t += blockDim.x)  // an empty history, as cfmm_solve's zeroed one
+    for (int a = 0; a < kSolverM; ++a) m.S[a][t] = m.Y[a][t] = 0.0;
+  sg_start<Smem, Rule::kOut>(P, w, m, rule.root(m));
+  f = sg_evaluate(P, w, m, rule);
+  merit = sg_commit(m, 0, false, rule);
+  if (tid == 0) {
+    s.fev = 1;
+    s.f = f;
+    s.merit = merit;
+  }
+  __syncthreads();
+  while (true) {
+    __syncthreads();  // every thread has read the last decision
+    // state: 0 run, 1 stop
+    if (tid == 0) {
+      s.state = 0;
+      if (!(s.f == s.f)) s.status = 5, s.state = 1;
+      else if (s.merit <= R.rtol) s.status = 0, s.state = 1;
+      else if (s.iter >= R.max_iter) s.status = 2, s.state = 1;
+      else if (s.fev >= R.max_fun) s.status = 3, s.state = 1;
+      else s.t = lbfgs_direction(m.W, s.hist, m.c);
+    }
+    __syncthreads();
+    if (s.state) break;
+    for (int t = tid; t < n; t += blockDim.x) {
+      double v = __dmul_rn(m.c[kSolverK - 1], m.pg[t]);
+#pragma unroll
+      for (int a = 0; a < kSolverM; ++a) {
+        v = fma(m.c[a], m.S[a][t], v);
+        v = fma(m.c[kSolverM + a], m.Y[a][t], v);
+      }
+      m.d[t] = rule.fixed(m, t) || (m.x[t] <= rule.lo(t) && m.g[t] > 0.0) ? 0.0 : -v;
+    }
+    __syncthreads();
+    int dec = kLsRetry;
+    double f_new = s.f;
+    for (int ls = 0; ls < 30 && s.fev < R.max_fun; ++ls) {
+      const double t = s.t;
+      double gd = 0.0, st2 = 0.0;
+      for (int k = tid; k < n; k += blockDim.x) {
+        const double y = rule.fixed(m, k) ? 1.0 : fmax(fma(t, m.d[k], m.x[k]), rule.lo(k));
+        m.xt[k] = y;
+        const double dx = __dsub_rn(y, m.x[k]);
+        gd = fma(m.g[k], dx, gd);
+        st2 = fma(dx, dx, st2);
+      }
+      const double gdx = sg_cta_sum(gd, m), step2 = sg_cta_sum(st2, m);
+      f_new = sg_evaluate(P, w, m, rule);
+      if (tid == 0) {
+        ++s.fev;
+        double tn = s.t;
+        s.state = lbfgs_trial(s.f, f_new, gdx, step2, s.hist.cnt, tn);
+        s.t = tn;
+      }
+      __syncthreads();
+      dec = s.state;
+      __syncthreads();
+      if (dec != kLsRetry) break;
+    }
+    if (dec != kLsAccept) {
+      if (tid == 0) {
+        if (s.hist.cnt > 0 && dec != kLsStall) {
+          s.hist.cnt = 0;  // drop the history and retry with steepest descent
+          s.state = 0;
+        } else {
+          s.status = dec == kLsStall ? 1 : 4;
+          s.state = 1;
+        }
+      }
+      __syncthreads();
+      if (s.state) break;
+      continue;
+    }
+    const int slot = s.hist.head;
+    const double mr = sg_commit(m, slot, true, rule);
+    if (tid == 0) {
+      lbfgs_store(m.W, slot, s.hist);
+      ++s.iter;
+      const double f_old = s.f;
+      s.f = f_new;
+      s.merit = mr;
+      s.state = lbfgs_factr(f_old, f_new, R.factr, s.small) ? 1 : 0;
+      if (s.state) s.status = 1;
+    }
+    __syncthreads();
+    if (s.state) break;
+  }
+  merit = s.merit;
+  return s.status;
+}
+
+// The legs of the row's np pools at ν = x into leg_off[r] .. (and, filled on execute, the transition).
+template <bool EXEC, class Rows>
+__device__ __forceinline__ void sg_legs(const PathSets* P, const SubgraphWork& w, const double* x, const SplitMoved& mv,
+                                        const Rows& R, int64_t r, int64_t np, bool filled) {
+  const int64_t l0 = R.leg_off[r];
+  for (int64_t e = threadIdx.x; e < np; e += blockDim.x) {
+    if (R.leg_entry) R.leg_entry[l0 + e] = w.ent[e];
+    split_leg<EXEC>(P, filled, [&] { return sg_pool(P, w, e, x); }, mv, R.leg_delta, R.leg_lambda, l0 + e);
+  }
+}
+
+// Row r on the current state.  Returns nothing; writes the row's outputs.  EXEC: the limit decides,
+// and a filled row applies the transition of cfmm_apply_trades at its ν to each of its pools.  OUT:
+// the row buys y = amount of i; its dual has lin = −y′ at i, y′ = y·(1 + rtol) rounded up, and ν_j
+// fixed at 1; it is unreachable when y is at least what its pools holding i could pay out.
+template <bool EXEC, bool OUT>
+__device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
+                             const uint8_t* gact, const SubgraphRows& R, const SubgraphWork& w, const SplitMoved& mv,
+                             int64_t r, SubgraphSmem& m) {
+  __shared__ SgSolveState s;
+  const int tid = threadIdx.x;
+  const int32_t j = (int32_t)(R.token_in[r] - 1), i = (int32_t)(R.token_out[r] - 1);
+  const double amt = R.amount[r];
+  const SgRule<OUT> rule{OUT ? -__fma_ru(amt, R.rtol, amt) : amt, amt};
+  sg_setup(P, ix, A, G, gact, j, i, m);
+  const int64_t np = m.npool, n = m.n_loc;
+  // the pools: {j, i} first, then each slot's, at the offsets the setup counted
+  if (tid == 0 && m.direct_cnt > 0) {
+    for (int64_t e = ix.off[m.direct]; e < ix.off[m.direct + 1]; ++e) w.ent[e - ix.off[m.direct]] = ix.pool[e];
+  }
+  sg_gather(ix, G, w, m, [&](int s, auto& put) {
+    if (m.jin) put(m.jpair[s]);
+  });
+  sg_order_pools(P, w, m, np, n, [&](int32_t t) { return sg_local(G, m, t); });
   // exact-out: the capacity of i over the row's pools, once, before any solve
   bool short_cap = false;
   if constexpr (OUT) {
@@ -529,105 +677,9 @@ __device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, con
       short_cap = amt >= sg_cta_sum(c, m);
     }
   }
-  // the solve
   const bool solve = m.jin && amt > 0.0 && !short_cap;
-  double f = 0.0, merit = 0.0;
-  int status = -1;
-  if (tid == 0) {
-    s_iter = s_fev = s_small = 0;
-    hist.cnt = hist.head = 0;
-  }
-  if (solve) {
-    for (int t = tid; t < n; t += blockDim.x)  // an empty history, as cfmm_solve's zeroed one
-      for (int a = 0; a < kSolverM; ++a) m.S[a][t] = m.Y[a][t] = 0.0;
-    sg_start<SubgraphSmem, OUT>(P, w, m);
-    f = sg_evaluate<OUT>(P, w, m, lin);
-    merit = sg_commit<OUT>(m, 0, false, amt);
-    if (tid == 0) {
-      s_fev = 1;
-      s_f = f;
-      s_merit = merit;
-    }
-    __syncthreads();
-    while (true) {
-      __syncthreads();  // every thread has read the last decision
-      // state: 0 run, 1 stop
-      if (tid == 0) {
-        s_state = 0;
-        if (!(s_f == s_f)) s_status = 5, s_state = 1;
-        else if (s_merit <= R.rtol) s_status = 0, s_state = 1;
-        else if (s_iter >= R.max_iter) s_status = 2, s_state = 1;
-        else if (s_fev >= R.max_fun) s_status = 3, s_state = 1;
-        else s_t = lbfgs_direction(m.W, hist, m.c);
-      }
-      __syncthreads();
-      if (s_state) break;
-      for (int t = tid; t < n; t += blockDim.x) {
-        double v = __dmul_rn(m.c[kSolverK - 1], m.pg[t]);
-#pragma unroll
-        for (int a = 0; a < kSolverM; ++a) {
-          v = fma(m.c[a], m.S[a][t], v);
-          v = fma(m.c[kSolverM + a], m.Y[a][t], v);
-        }
-        m.d[t] = sg_fixed<OUT>(t) || (m.x[t] <= sg_lo<OUT>(t) && m.g[t] > 0.0) ? 0.0 : -v;
-      }
-      __syncthreads();
-      int dec = kLsRetry;
-      double f_new = s_f;
-      for (int ls = 0; ls < 30 && s_fev < R.max_fun; ++ls) {
-        const double t = s_t;
-        double gd = 0.0, st2 = 0.0;
-        for (int k = tid; k < n; k += blockDim.x) {
-          const double y = sg_fixed<OUT>(k) ? 1.0 : fmax(fma(t, m.d[k], m.x[k]), sg_lo<OUT>(k));
-          m.xt[k] = y;
-          const double dx = __dsub_rn(y, m.x[k]);
-          gd = fma(m.g[k], dx, gd);
-          st2 = fma(dx, dx, st2);
-        }
-        const double gdx = sg_cta_sum(gd, m), step2 = sg_cta_sum(st2, m);
-        f_new = sg_evaluate<OUT>(P, w, m, lin);
-        if (tid == 0) {
-          ++s_fev;
-          double tn = s_t;
-          s_state = lbfgs_trial(s_f, f_new, gdx, step2, hist.cnt, tn);
-          s_t = tn;
-        }
-        __syncthreads();
-        dec = s_state;
-        __syncthreads();
-        if (dec != kLsRetry) break;
-      }
-      if (dec != kLsAccept) {
-        if (tid == 0) {
-          if (hist.cnt > 0 && dec != kLsStall) {
-            hist.cnt = 0;  // drop the history and retry with steepest descent
-            s_state = 0;
-          } else {
-            s_status = dec == kLsStall ? 1 : 4;
-            s_state = 1;
-          }
-        }
-        __syncthreads();
-        if (s_state) break;
-        continue;
-      }
-      const int slot = hist.head;
-      const double mr = sg_commit<OUT>(m, slot, true, amt);
-      if (tid == 0) {
-        lbfgs_store(m.W, slot, hist);
-        ++s_iter;
-        const double f_old = s_f;
-        s_f = f_new;
-        s_merit = mr;
-        s_state = lbfgs_factr(f_old, f_new, R.factr, s_small) ? 1 : 0;
-        if (s_state) s_status = 1;
-      }
-      __syncthreads();
-      if (s_state) break;
-    }
-    status = s_status;
-    merit = s_merit;
-  }
+  double merit;
+  const int status = sg_solve(P, w, m, rule, R, n, solve, s, merit);
   // status, the limit, the legs (and the transition on execute)
   const double received = solve ? m.px[0] : 0.0, paid = solve ? __dsub_rn(0.0, m.px[1]) : 0.0;
   uint8_t st = 0;  // CFMM_ORDER_FILLED (amount 0: zeros, no solve)
@@ -640,11 +692,7 @@ __device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, con
       st = 1;  // CFMM_ORDER_LIMIT; an equal limit fills
   }
   const bool filled = st == 0 && solve;
-  const int64_t l0 = R.leg_off[r];
-  for (int64_t e = tid; e < np; e += blockDim.x) {
-    if (R.leg_entry) R.leg_entry[l0 + e] = w.ent[e];
-    split_leg<EXEC>(P, filled, [&] { return sg_pool(P, w, e, m.x); }, mv, R.leg_delta, R.leg_lambda, l0 + e);
-  }
+  sg_legs<EXEC>(P, w, m.x, mv, R, r, np, filled);
   if (R.token) {
     int64_t o = R.tok_off[r];
     for (int t = tid; t < n; t += blockDim.x) {
@@ -660,25 +708,11 @@ __device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, con
     R.received[r] = filled ? received : 0.0;
     R.status[r] = st;
     R.solver_status[r] = status;
-    R.iterations[r] = solve ? s_iter : 0;
-    R.fun_evals[r] = solve ? s_fev : 0;
+    R.iterations[r] = solve ? s.iter : 0;
+    R.fun_evals[r] = solve ? s.fev : 0;
     R.merit[r] = solve ? merit : 0.0;
   }
   __syncthreads();  // the next row reuses the shared state and the workspace
-}
-
-// CTA b's workspace: workspace b of w.
-__device__ __forceinline__ SubgraphWork sg_cta_work(const SubgraphWork& w) {
-  const int64_t c = w.cap * blockIdx.x;
-  SubgraphWork wb = w;
-  wb.ent += c;
-  wb.key += c;
-  wb.ta += c;
-  wb.tb += c;
-  wb.inc += 2 * c;
-  wb.ca += c;
-  wb.cb += c;
-  return wb;
 }
 
 // Exact-in rows rows[0 .. n) (null: 0 .. n), one CTA at a time each; CTA b uses workspace b.
