@@ -158,6 +158,7 @@ SYMBOLS = {
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),
     "cfmm_debug_compact_record": (C.c_int, [_ctx, C.c_int, _ip]),
+    "cfmm_debug_l2_keep": (C.c_int, [_ctx, C.c_int, _ip]),
     "cfmm_set_option": (C.c_int, [_ctx, C.c_char_p, C.c_int64]),
     "cfmm_last_sweep_ms": (C.c_int, [_ctx, C.POINTER(C.c_float)]),
     "cfmm_launch_count": (C.c_int64, [_ctx]),

@@ -151,6 +151,7 @@ struct PoolSet {
   bool rec18_ok = false;
   DevBuf<unsigned> d_rec_hdr;
   int range_pools = 0;         // pools per unit of the range table (96-pool chunks or 192-pool records)
+  int l2_keep = 0;             // keep rule the last TMA launch ran with (> 0: d_packed holds evict_last lines)
   DevBuf<double> d_inv_scale, d_tok_sum;
   bool fixed_ok = false;       // every token fits the fixed-point rules (range, totals)
   // speed-weighted CTA ranges of the TMA kernel (product_tma.cuh): the table passed to the next
@@ -214,6 +215,7 @@ struct cfmm_ctx {
   void* h_bounce[2] = {nullptr, nullptr};
   cudaEvent_t ev_bounce[2] = {nullptr, nullptr};
   int sm_count = 132;  // (H100 SXM; cfmm_create reads the device's own count)
+  int64_t l2_bytes = 50 << 20;  // (H100; cfmm_create reads the device's own size)
   // options
   int exact = 0;
   int debug_skip = 0;  // measurement only (tools/explore.py)
@@ -261,6 +263,7 @@ struct cfmm_ctx {
   int geomean_tma = 1;          // gradient-only GeometricMean sweeps on the TMA kernel (0: first-generation kernel)
   int compact_stream = 1;       // ProductTwoCoin, economized math: 20-byte pool records (γ dictionary, chunk-relative a) when the set allows it
   int compact_record = 0;       // pools per compact record: 96 or 192; 0 = 192 on sets with at least 4 records per resident warp
+  int l2_keep = -1;             // TMA sweeps of streams larger than the L2: keep the first h records of every CTA's range in the L2 (-1 = h by L2 size, 0 = no hints)
   // resident CTAs per SM of every kernel instantiation this context has launched.
   // Per context, not per process: cudaFuncSetAttribute (the > 48 KB dynamic shared
   // memory opt-in) acts on the current device only, and contexts of one process
@@ -874,11 +877,40 @@ int refresh_scale(cfmm_ctx* ctx, PoolSet& s) {
   return CFMM_OK;
 }
 
+// Keep rule of a TMA sweep over the 192-pool records, `stream_bytes` in all (see product_sweep_tma): 0 = no
+// L2 hints, else the first h records of every CTA's range are kept in the L2 across sweeps.  A
+// stream that fits in the L2 stays there without hints.  Else h = the records every warp of a CTA
+// fetches before the CTA's shared counter takes over (two per warp), at most 40 % of the L2 over the
+// grid.  On an H100 (50 MB L2, 264 CTAs) with the headline set's records, h = 8 / 16 / 24 / 32 / 48
+// measured 78.3 / 77.3 / 77.6 / 77.0 / 79.7 against 81.2 µs without hints (DESIGN §4.1 r3 g).
+int l2_keep_of(const cfmm_ctx* ctx, int64_t stream_bytes) {
+  if (ctx->l2_keep == 0 || ctx->l2_bytes <= 0 || stream_bytes <= ctx->l2_bytes) return 0;
+  if (ctx->l2_keep > 0) return ctx->l2_keep;
+  constexpr int L6 = cfmm::kTmaL6;
+  const int64_t ctas = (int64_t)ctx->sm_count * cfmm::tma_ctas_per_sm<0, L6>();
+  const int64_t fit = ctx->l2_bytes * 40 / 100 / (ctas * cfmm::tma_chunk_bytes_c<0, true, L6>());
+  return (int)std::min<int64_t>(2 * cfmm::tma_warps<0, L6>(), fit);
+}
+
+// the kept records of the stream back to evict_normal, once no sweep reads them under the same rule
+int l2_release(cfmm_ctx* ctx, PoolSet& s, cudaStream_t st) {
+  if (s.l2_keep == 0 || !s.d_packed.p) return CFMM_OK;
+  s.l2_keep = 0;
+  cfmm::l2_evict_normal_kernel<<<(unsigned)ctx->sm_count * 4, 256, 0, st>>>(s.d_packed.p, s.d_packed.n);
+  ctx->launches++;
+  CU_TRY(ctx, cudaGetLastError());
+  return CFMM_OK;
+}
+
 // the packed stream of the mode this sweep runs in (rebuilt when the mode or the reserves changed)
 template <int POOL, int L = cfmm::kTmaL>
 int ensure_packed(cfmm_ctx* ctx, PoolSet& s, bool econ, bool fixed, bool compact, cudaStream_t st) {
   const int mode = (econ ? 1 : 0) | (fixed ? 2 : 0) | (compact ? 4 : 0) | (L != cfmm::kTmaL ? 8 : 0);
   if (s.packed_mode == mode) return CFMM_OK;
+  {
+    const int rc = l2_release(ctx, s, st);  // (the buffer is rewritten or freed)
+    if (rc != CFMM_OK) return rc;
+  }
   const size_t wide = (size_t)s.n_chunks * cfmm::tma_chunk_bytes<POOL>();
   const size_t bytes = !compact ? wide
                        : L == cfmm::kTmaL ? (size_t)s.n_chunks * cfmm::tma_chunk_bytes_c<POOL, true>()
@@ -1015,6 +1047,9 @@ int launch_tma_cfg(cfmm_ctx* ctx, PoolSet& s, const double* d_v, double* d_psi, 
     fx.grid_done = ctx->d_grid_done.p;
     ctx->fx_pending.mode = 0;  // consumed
   }
+  const int a_keep = COMPACT && L == cfmm::kTmaL6 ? l2_keep_of(ctx, n_units * cfmm::tma_chunk_bytes_c<POOL, COMPACT, L>()) : 0;
+  if (a_keep != s.l2_keep && (rc = l2_release(ctx, s, st)) != CFMM_OK) return rc;
+  s.l2_keep = a_keep;
   ProfScope prof(ctx, POOL == 0 ? CFMM_POOL_PRODUCT : CFMM_POOL_GEOMEAN, st);
   const unsigned char* a_packed = s.d_packed.p;
   const double* a_gam = COMPACT ? s.d_gtab.p : s.d_gam.p;  // compact stream: the γ dictionary instead of per-pool γ
@@ -1026,12 +1061,12 @@ int launch_tma_cfg(cfmm_ctx* ctx, PoolSet& s, const double* d_v, double* d_psi, 
     // the fused exchange meets at a grid-wide barrier: a COOPERATIVE launch makes the driver
     // guarantee that every CTA is resident (or fail the launch) instead of inferring it
     void* args[] = {&a_packed, &a_gam, const_cast<cfmm::BucketTable*>(&tab), &a_nb, &d_v, &a_scale, &d_psi, &a_n, &a_zero,
-                    &a_range, &a_flags, &fx, &s.ranges, &d_dur, &a_trace};
+                    &a_range, &a_flags, const_cast<int*>(&a_keep), &fx, &s.ranges, &d_dur, &a_trace};
     CU_TRY(ctx, cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(kern), dim3(grid), dim3(kThreads),
                                             args, kSmem, st));
   } else {
     kern<<<grid, kThreads, kSmem, st>>>(a_packed, a_gam, tab, a_nb, d_v, a_scale, d_psi, a_n, a_zero,
-                                        a_range, a_flags, fx, s.ranges, d_dur, a_trace);
+                                        a_range, a_flags, a_keep, fx, s.ranges, d_dur, a_trace);
   }
   if (ctx->d_trace.n) ctx->trace_grid = grid;
   ctx->launches++;
@@ -1284,6 +1319,7 @@ int cfmm_create(cfmm_ctx** out, int device, int64_t n_tokens) {
   cudaDeviceProp prop;
   CREATE_TRY(cudaGetDeviceProperties(&prop, device));
   ctx->sm_count = prop.multiProcessorCount;
+  ctx->l2_bytes = prop.l2CacheSize;
   CREATE_TRY(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
   CREATE_TRY(cudaEventCreateWithFlags(&ctx->ev_order, cudaEventDisableTiming));
   CREATE_TRY(cudaEventCreate(&ctx->ev0));
@@ -1310,6 +1346,8 @@ void drop_graphs(cfmm_ctx* ctx);
 void cfmm_destroy(cfmm_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
+  for (auto& s : ctx->sets)
+    if (ctx->stream) l2_release(ctx, s, ctx->stream);
   if (ctx->stream) cudaStreamSynchronize(ctx->stream);
   ctx->comm.detach();
   drop_graphs(ctx);
@@ -4745,6 +4783,20 @@ int cfmm_debug_compact_record(cfmm_ctx* ctx, int type, int64_t* pools_per_record
   return CFMM_OK;
 }
 
+// Test hook: keep rule of the next gradient-only TMA sweep of the main ProductTwoCoin set (see
+// l2_keep_of; 0 for the other types and for sweeps that do not stream the 192-pool records).
+int cfmm_debug_l2_keep(cfmm_ctx* ctx, int type, int64_t* keep) {
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if ((rc = check_type(ctx, type)) != CFMM_OK) return rc;
+  if (!keep) return fail(ctx, CFMM_ERR_INVALID, "null output");
+  const PoolSet& s = ctx->sets[type];
+  *keep = 0;
+  if (type == CFMM_POOL_PRODUCT && s.tma_ok && ctx->use_tma && compact_record_of(ctx, s) == 192)
+    *keep = l2_keep_of(ctx, s.n_recs * cfmm::tma_chunk_bytes_c<0, true, cfmm::kTmaL6>());
+  return CFMM_OK;
+}
+
 // Test hook: info[8] = {main-set pools, tail pools, main-set padded length, TMA layout built,
 // fixed-point Ψ slice allowed, compact stream allowed, every reserve in the guard-free range,
 // retired pools} of one pool type.
@@ -4791,6 +4843,9 @@ int cfmm_set_option(cfmm_ctx* ctx, const char* key, int64_t value) {
   } else if (!strcmp(key, "compact_record")) {
     if (value != 0 && value != 96 && value != 192) return fail(ctx, CFMM_ERR_INVALID, "compact_record: 0 (by set size), 96 or 192");
     ctx->compact_record = (int)value;
+  } else if (!strcmp(key, "l2_keep")) {
+    if (value < -1 || value > (1 << 20)) return fail(ctx, CFMM_ERR_INVALID, "l2_keep: -1 (by L2 size), 0 (no hints) or records per CTA range");
+    ctx->l2_keep = (int)value;
   } else if (!strcmp(key, "geomean_tma")) {
     ctx->geomean_tma = value != 0;
   } else if (!strcmp(key, "balance")) {

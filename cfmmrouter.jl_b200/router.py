@@ -941,6 +941,13 @@ class DevicePools:
         self._chk(self._lib.cfmm_debug_compact_record(self._ctx, int(pool_type), _ip(out)))
         return int(out[0])
 
+    def l2_keep(self, pool_type: int) -> int:
+        """L2 keep rule of the next gradient-only sweep of the main set: h > 0 = the first h records
+        of every CTA's range stay in the L2 across sweeps, 0 = no L2 hints (cfmm_debug_l2_keep; read-only)."""
+        out = np.zeros(1, dtype=np.int64)
+        self._chk(self._lib.cfmm_debug_l2_keep(self._ctx, int(pool_type), _ip(out)))
+        return int(out[0])
+
     # -- multi-GPU --------------------------------------------------------------
     def detach_group(self):
         self._chk(self._lib.cfmm_comm_detach(self._ctx))

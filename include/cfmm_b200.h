@@ -1165,6 +1165,18 @@ int cfmm_solve(cfmm_ctx *ctx, const double *lin, const double *lower, const doub
  *   "compact_record"   pools per record of that stream: 192 (two chunks of a bucket, one bulk
  *                      copy, six pools per thread), 96, or 0 (default) = 192 when the set has at
  *                      least 4 such records per resident warp, else 96.
+ *   "l2_keep"          gradient sweeps that stream 192-pool records ("compact_record") larger in
+ *                      all than the device's L2:
+ *                      the bulk copies carry L2 eviction hints: the first h records of every
+ *                      CTA's range as evict_last, every other record as evict_first, so that the
+ *                      records each sweep waits for at its start stay in the L2 from one sweep
+ *                      to the next and come from there instead of HBM.  -1 (default) = h chosen
+ *                      from the L2 size (two records per warp of a CTA, the kept records taking
+ *                      at most 40 % of the L2), 0 = no hints, h > 0 = that h.  Streams that fit
+ *                      in the L2 run without hints whatever the value.  Only per-instruction
+ *                      hints: no L2 set-aside, no access-policy window; the kept lines go back
+ *                      to evict_normal when the rule or the stream changes and at cfmm_destroy.
+ *                      Results do not depend on it.
  *   "geomean_tma"      1 (default) = gradient-only GeometricMeanTwoCoin sweeps run on the TMA
  *                      kernel too (48-byte records, same fixed-point slice); 0 = first-generation
  *                      kernel.
@@ -1223,6 +1235,11 @@ int cfmm_debug_pool_set_info(cfmm_ctx *ctx, int type, int64_t *info);
  * pool records) or 0 (no compact stream: other pool types, exact or reference-order
  * math, or a set that does not fit it). */
 int cfmm_debug_compact_record(cfmm_ctx *ctx, int type, int64_t *pools_per_record);
+/* Test hook: the L2 keep rule (option "l2_keep") the next gradient-only sweep of the main
+ * ProductTwoCoin set runs with: h > 0 = the first h records of every CTA's range are kept in the
+ * L2 across sweeps, 0 = no L2 hints (other pool types, a stream other than the 192-pool records, a stream
+ * that fits in the L2, or l2_keep = 0). */
+int cfmm_debug_l2_keep(cfmm_ctx *ctx, int type, int64_t *keep);
 /* Measurement hook (option "trace" = 1): per-CTA phase timestamps of the last TMA gradient
  * sweep, ns of %globaltimer: out[8 * grid] = {entry, price slice ready, own range done,
  * all chunks done, partials flushed, exit, grid barrier passed (fused exchange, else 0),

@@ -8,6 +8,13 @@
 // limit and the median SM clock sampled while the timed launches ran.  Then the headline set's
 // record count (52,099 192-pool records) at 3872 B (201.7 MB, 20 B per pool) and at 3520 B
 // (183.4 MB, 18 B per pool), 2 x 10 warps, interleaved over several rounds.
+// Last, the L2 kept across passes (the H100's L2 holds 50 MB, a 3520-byte headline pass 183.4 MB): the
+// same 3520-byte passes with an .L2::cache_hint policy on every bulk copy.  A fixed subset of the
+// records is "kept" -- record r when r % k == 0, so every CTA keeps the same share of its range -- and
+// the rest "streamed" as evict_first; the kept ones go as evict_normal or as evict_last.  Against that,
+// one createpolicy.fractional policy (evict_last on a fraction 1/k of the lines, evict_first on the
+// rest) on every copy.  Between configurations every line of the buffer goes back to evict_normal
+// (applypriority), so no configuration inherits lines another one kept.
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tma_stream tma_stream.cu -lnvidia-ml
 //        (-L/usr/local/cuda/lib64/stubs where the driver's libnvidia-ml is not on the link path)
 #include <cuda_runtime.h>
@@ -31,20 +38,48 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity) {
       : "memory");
 }
 
+// L2 policy of the bulk copies (kernel parameter `hint`)
+enum Hint {
+  kNoHint = 0,      // plain cp.async.bulk
+  kFirstNormal = 1, // record r % k == 0 evict_normal, the others evict_first
+  kFirstLast = 2,   // record r % k == 0 evict_last, the others evict_first
+  kFractional = 3,  // every copy: createpolicy.fractional evict_last on 1/k of the lines, evict_first on the rest
+  kAllFirst = 4,    // every copy evict_first
+};
+
 template <int REC, int WARPS, int CTAS>
 __global__ void __launch_bounds__(WARPS * 32, CTAS) stream(const unsigned char* __restrict__ src, int n_rec,
-                                                             unsigned* __restrict__ out) {
+                                                             unsigned* __restrict__ out, int hint = kNoHint, int k = 0) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ uint64_t full[WARPS][kStages];
   __shared__ int s_next;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, G = gridDim.x;
   const int c0 = (int)((long long)n_rec * blockIdx.x / G), c1 = (int)((long long)n_rec * (blockIdx.x + 1) / G);
   unsigned char* my = smem + (size_t)warp * kStages * REC;
+  // the two policies, created once per thread: pol_keep for the kept records, pol_stream for the others
+  uint64_t pol_keep = 0, pol_stream = 0;
+  if (hint == kFractional) {
+    const float frac = 1.0f / (float)k;
+    asm volatile("createpolicy.fractional.L2::evict_last.L2::evict_first.b64 %0, %1;" : "=l"(pol_keep) : "f"(frac));
+    pol_stream = pol_keep;
+  } else if (hint != kNoHint) {
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_stream));
+    if (hint == kFirstLast) asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_keep));
+    else if (hint == kFirstNormal) asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol_keep));
+    else pol_keep = pol_stream;
+  }
   auto issue = [&](int r, int st) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&full[warp][st])), "r"(REC) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     smem_u32(my + st * REC)), "l"(src + (size_t)r * REC), "r"(REC), "r"(smem_u32(&full[warp][st]))
-                 : "memory");
+    if (hint == kNoHint) {
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                       smem_u32(my + st * REC)), "l"(src + (size_t)r * REC), "r"(REC), "r"(smem_u32(&full[warp][st]))
+                   : "memory");
+    } else {
+      const uint64_t pol = k > 0 && r % k == 0 ? pol_keep : pol_stream;
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+                       smem_u32(my + st * REC)), "l"(src + (size_t)r * REC), "r"(REC), "r"(smem_u32(&full[warp][st])), "l"(pol)
+                   : "memory");
+    }
   };
   if (lane == 0) {
     for (int s = 0; s < kStages; ++s)
@@ -85,12 +120,19 @@ __global__ void __launch_bounds__(WARPS * 32, CTAS) stream(const unsigned char* 
   if (acc == 0x12345678u) out[0] = acc;
 }
 
+// every 128-byte line of [p, p + bytes) back to evict_normal in the L2
+__global__ void reset_priority(const unsigned char* p, size_t bytes) {
+  for (size_t off = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 128; off < bytes; off += (size_t)gridDim.x * blockDim.x * 128)
+    asm volatile("applypriority.global.L2::evict_normal [%0], 128;" ::"l"(p + off) : "memory");
+}
+
 static nvmlDevice_t g_nvml;
 static bool g_have_nvml = false;
 
 // returns the median launch time in µs (0 when the shape does not fit); n_rec <= 0: kStreamBytes / REC
 template <int REC, int WARPS, int CTAS>
-double run(const unsigned char* d_src, unsigned* d_out, int sms, std::vector<unsigned>& clocks, int n_rec = 0) {
+double run(const unsigned char* d_src, unsigned* d_out, int sms, std::vector<unsigned>& clocks, int n_rec = 0,
+           int hint = kNoHint, int keep_k = 0) {
   constexpr int smem = WARPS * kStages * REC;
   auto k = stream<REC, WARPS, CTAS>;
   cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -105,11 +147,11 @@ double run(const unsigned char* d_src, unsigned* d_out, int sms, std::vector<uns
   constexpr int kLaunches = 200;
   std::vector<cudaEvent_t> ev(kLaunches + 1);
   for (auto& e : ev) cudaEventCreate(&e);
-  for (int i = 0; i < 20; ++i) k<<<grid, WARPS * 32, smem>>>(d_src, n_rec, d_out);
+  for (int i = 0; i < 20; ++i) k<<<grid, WARPS * 32, smem>>>(d_src, n_rec, d_out, hint, keep_k);
   cudaDeviceSynchronize();
   cudaEventRecord(ev[0]);
   for (int i = 0; i < kLaunches; ++i) {
-    k<<<grid, WARPS * 32, smem>>>(d_src, n_rec, d_out);
+    k<<<grid, WARPS * 32, smem>>>(d_src, n_rec, d_out, hint, keep_k);
     cudaEventRecord(ev[i + 1]);
   }
   // sample the SM clock while the timed launches run
@@ -124,8 +166,9 @@ double run(const unsigned char* d_src, unsigned* d_out, int sms, std::vector<uns
   std::sort(t.begin(), t.end());
   const double med_us = t[kLaunches / 2] * 1e3, min_us = t[0] * 1e3;
   const double bytes = (double)n_rec * REC;
-  printf("%5d B  %d x %2d warps  %7d records  %2d KB ring/SM  median %7.2f us  min %7.2f us  %7.1f GB/s (median)\n", REC,
-         CTAS, WARPS, n_rec, CTAS * smem / 1024, med_us, min_us, bytes / (med_us * 1e3));
+  if (hint == kNoHint)
+    printf("%5d B  %d x %2d warps  %7d records  %2d KB ring/SM  median %7.2f us  min %7.2f us  %7.1f GB/s (median)\n", REC,
+           CTAS, WARPS, n_rec, CTAS * smem / 1024, med_us, min_us, bytes / (med_us * 1e3));
   for (auto& e : ev) cudaEventDestroy(e);
   return med_us;
 }
@@ -170,6 +213,39 @@ int main() {
          "%.1f %% less time\n",
          kRounds, t20[0], t20[kRounds - 1], t20[kRounds / 2], t18[0], t18[kRounds - 1], t18[kRounds / 2],
          100.0 * (1.0 - t18[kRounds / 2] / t20[kRounds / 2]));
+  // the L2 kept across passes: per (policy, k) the medians of the rounds, all configurations interleaved
+  {
+    struct Cfg {
+      int hint, k;
+      const char* name;
+    };
+    const Cfg cfgs[] = {{kNoHint, 0, "no hint"},          {kAllFirst, 0, "all evict_first"},
+                        {kFirstNormal, 11, "normal/first"}, {kFirstNormal, 8, "normal/first"},
+                        {kFirstNormal, 6, "normal/first"},  {kFirstNormal, 5, "normal/first"},
+                        {kFirstLast, 11, "last/first"},     {kFirstLast, 8, "last/first"},
+                        {kFirstLast, 6, "last/first"},      {kFirstLast, 5, "last/first"},
+                        {kFractional, 11, "fractional"},    {kFractional, 8, "fractional"},
+                        {kFractional, 6, "fractional"},     {kFractional, 5, "fractional"}};
+    constexpr int kCfgs = sizeof(cfgs) / sizeof(cfgs[0]);
+    const size_t pass_bytes = (size_t)kHeadlineRecords * 3520;
+    std::vector<std::vector<double>> t(kCfgs);
+    for (int r = 0; r < kRounds; ++r)
+      for (int c = 0; c < kCfgs; ++c) {
+        reset_priority<<<sms * 8, 256>>>(d_src, pass_bytes);
+        t[c].push_back(run<3520, 10, 2>(d_src, d_out, sms, clocks, kHeadlineRecords, cfgs[c].hint, cfgs[c].k));
+      }
+    reset_priority<<<sms * 8, 256>>>(d_src, pass_bytes);
+    cudaDeviceSynchronize();
+    printf("L2 kept across 3520-byte headline passes (%.1f MB per pass), %d rounds of medians of 200 back-to-back passes:\n",
+           pass_bytes / 1e6, kRounds);
+    for (int c = 0; c < kCfgs; ++c) {
+      std::sort(t[c].begin(), t[c].end());
+      const int kept = cfgs[c].k > 0 ? (kHeadlineRecords + cfgs[c].k - 1) / cfgs[c].k : 0;
+      printf("  %-16s k = %2d  kept %5.1f MB  %7.2f..%7.2f us  median %7.2f us  %+6.1f %% against no hint\n", cfgs[c].name,
+             cfgs[c].k, kept * 3520 / 1e6, t[c].front(), t[c].back(), t[c][kRounds / 2],
+             100.0 * (t[c][kRounds / 2] / t[0][kRounds / 2] - 1.0));
+    }
+  }
   if (!clocks.empty()) {
     std::sort(clocks.begin(), clocks.end());
     printf("SM clock during the timed launches: median %u MHz (min %u, max %u, %zu samples)\n", clocks[clocks.size() / 2],
