@@ -42,6 +42,8 @@ SUBGRAPH_MAX_TOKENS = 256
 ORDER_NOT_CONVERGED = 5
 # cfmm_quote_basket_(swap_)orders / cfmm_execute_basket_(swap_)orders
 BASKET_MAX_TOKENS = 16
+# cfmm_quote_price_arbitrage / cfmm_execute_price_arbitrage
+PRICE_ARB_MAX_TOKENS = SUBGRAPH_MAX_TOKENS + 2
 
 COMM_HANDLE_BYTES = 128
 
@@ -71,6 +73,11 @@ class SubgraphOut(C.Structure):
 
 class BasketOut(SubgraphOut):
     """cfmm_basket_out: cfmm_subgraph_out's fields, with paid per basket entry."""
+
+
+class PriceArbOut(C.Structure):
+    """cfmm_price_arb_out: cfmm_subgraph_out's fields, with the profit for paid and received."""
+    _fields_ = [("profit", C.POINTER(C.c_double))] + SubgraphOut._fields_[2:]
 
 
 # every symbol include/cfmm_b200.h declares: name -> (restype, argtypes)
@@ -154,6 +161,10 @@ SYMBOLS = {
     "cfmm_execute_basket_swap_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, C.POINTER(C.c_uint8), _dp, _dp,
                                                   C.POINTER(C.c_uint8), C.POINTER(SubgraphOpts),
                                                   C.POINTER(BasketOut)]),
+    "cfmm_quote_price_arbitrage": (C.c_int, [_ctx, C.c_int64, _dp, C.POINTER(C.c_uint8), C.POINTER(SubgraphOpts),
+                                             C.POINTER(PriceArbOut)]),
+    "cfmm_execute_price_arbitrage": (C.c_int, [_ctx, C.c_int64, _dp, _dp, C.POINTER(C.c_uint8),
+                                               C.POINTER(SubgraphOpts), C.POINTER(PriceArbOut)]),
     "cfmm_modify_univ3_liquidity":(C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),

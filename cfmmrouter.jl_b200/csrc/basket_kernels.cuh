@@ -327,6 +327,7 @@ __device__ __forceinline__ double bk_value(const BkSmem<BUY>& m, const double* c
 template <bool BUY>
 struct BkRule {
   static constexpr bool kOut = BUY;
+  static constexpr bool kBoxStart = false;
   __device__ __forceinline__ double lin_at(const BkSmem<BUY>& m, int t) const {
     if constexpr (BUY)
       return t == m.nout || t > m.nin ? 0.0 : m.blin[t < m.nout ? t : t - 1];
@@ -339,9 +340,10 @@ struct BkRule {
     else
       return bk_value<BUY>(m, m.bamt, m.xt);
   }
-  __device__ __forceinline__ double lo(int t) const { return bk_lo<BUY>(t); }
+  __device__ __forceinline__ double lo(const BkSmem<BUY>&, int t) const { return bk_lo<BUY>(t); }
   __device__ __forceinline__ bool fixed(const BkSmem<BUY>& m, int t) const { return bk_fixed<BUY>(m, t); }
   __device__ __forceinline__ int root(const BkSmem<BUY>& m) const { return bk_root<BUY>(m); }
+  __device__ __forceinline__ void evaluated(BkSmem<BUY>&, double) const {}
   __device__ __forceinline__ double merit(const BkSmem<BUY>& m, double mx) const {
     double mr = __ddiv_rn(mx, bk_value<BUY>(m, m.bamt, m.x));
     if constexpr (BUY) {

@@ -36,6 +36,7 @@
 #include "solver_control.cuh"
 #include "subgraph_kernels.cuh"
 #include "basket_kernels.cuh"
+#include "price_arb_kernels.cuh"
 #include "swap_kernels.cuh"
 #include "path_kernels.cuh"
 #include "split_kernels.cuh"
@@ -4107,12 +4108,14 @@ const void* kernel_ptr(K* k) {
 //   n_paid        the length of paid (q, or basket_off[q]);
 //   plan(...)     the plan launch; rows(exec_tag, second, ...) a launch of one row kernel;
 //   visit(r, v)   the tokens row r visits besides the slots (a token visited twice changes nothing),
-//                 and uses their count over the call, for the conflict levels of an execute.
+//                 and uses their count over the call, for the conflict levels of an execute;
+//   all_slots     every row also visits every slot (subgraph and basket rows: B is the whole mask).
 // The driver builds the call's slots and their B-graph, runs the plan, sizes the outputs and the per-CTA
 // workspace, runs the rows (a level's rows, or a quote's, split between the two kernels), and reads back.
 extern "C++" template <class Rows, class Out, class Plan, class RowLaunch, class Second, class Visit>
 int row_orders(cfmm_ctx* ctx, bool exec, int64_t q, const uint8_t* allowed, Rows R, const Out& O, int occ, int occ2,
-               int64_t n2, int K, int64_t n_paid, int64_t uses, const char* what, Plan plan, RowLaunch rows,
+               int64_t n2, int K, int64_t n_paid, int64_t uses, bool all_slots, const char* what, Plan plan,
+               RowLaunch rows,
                Second second, Visit visit) {
   int rc;
   auto& ix = ctx->pairs;
@@ -4255,13 +4258,14 @@ int row_orders(cfmm_ctx* ctx, bool exec, int64_t q, const uint8_t* allowed, Rows
     if ((rc = order_sets(ctx, true, xs)) != CFMM_OK) return rc;
     ctx->state_version++;
     // levels over the tokens the rows visit and B (one table of n_tokens entries)
-    int64_t size = ctx->n_tokens, use = uses + q * (int64_t)nB;
+    int64_t size = ctx->n_tokens, use = uses + (all_slots ? q * (int64_t)nB : 0);
     std::vector<int64_t> order, level_off;
     conflict_levels(
         q, 1, &size, &use,
         [&](int64_t r, auto&& v) {
           visit(r, v);
-          for (int32_t t : tok) v(0, t);
+          if (all_slots)
+            for (int32_t t : tok) v(0, t);
         },
         order, level_off);
     // a level's rows share no token, so their order does not matter: its first kernel's rows go first
@@ -4333,7 +4337,7 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
     return rc;
   cfmm::SubgraphRows R{d_in.p, d_out.p, d_amount.p, d_limit.p, o.max_iter, o.max_fun, o.rtol, o.factr};
   return row_orders(
-      ctx, exec, q, allowed, R, out ? *out : none, occ, occ_out, n_out, 0, q, 2 * q, "execute_subgraph_orders",
+      ctx, exec, q, allowed, R, out ? *out : none, occ, occ_out, n_out, 0, q, 2 * q, true, "execute_subgraph_orders",
       [&](unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P, cfmm::PairIndexView pv, cfmm::AdjView A,
           const cfmm::BestPathGraph& G, const uint8_t* act, int64_t* ntok, int64_t* npool) {
         cfmm::subgraph_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, d_in.p, d_out.p, q,
@@ -4390,7 +4394,7 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
     return rc;
   cfmm::BasketRows R{d_out.p, d_boff.p, d_btok.p, d_bamt.p, d_limit.p, o.max_iter, o.max_fun, o.rtol, o.factr};
   return row_orders(
-      ctx, exec, q, allowed, R, O, occ, occ_buy, n_buy, K, NE, q + NE, what,
+      ctx, exec, q, allowed, R, O, occ, occ_buy, n_buy, K, NE, q + NE, true, what,
       [&](unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P, cfmm::PairIndexView pv, cfmm::AdjView A,
           const cfmm::BestPathGraph& G, const uint8_t* act, int64_t* ntok, int64_t* npool) {
         cfmm::basket_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, d_boff.p, d_btok.p,
@@ -4438,6 +4442,107 @@ int basket_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, c
   const cfmm_basket_out none{};
   return basket_orders(ctx, exec, q, token_out, basket_off, basket_token, kind, basket_amount, limit, allowed, o,
                        out ? *out : none, what);
+}
+
+// ---- arbitrage against external prices over every pool among allowed tokens (price_arb_kernels.cuh)
+
+// Every argument of cfmm_quote/execute_price_arbitrage, before anything runs.
+int check_price_arb(cfmm_ctx* ctx, int64_t q, const double* price, const double* min_profit, const uint8_t* allowed,
+                    const cfmm_subgraph_opts& o, const char* what) {
+  int rc = check_row_opts(ctx, q, allowed, o, what);
+  if (rc != CFMM_OK || q == 0) return rc;
+  if (!price) return fail(ctx, CFMM_ERR_INVALID, "%s: null price", what);
+  const int64_t nA = count_allowed(ctx, allowed);
+  if (nA > CFMM_PRICE_ARB_MAX_TOKENS)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: %lld allowed tokens, more than %d", what, (long long)nA,
+                CFMM_PRICE_ARB_MAX_TOKENS);
+  for (int64_t r = 0; r < q; ++r) {
+    bool any = false;
+    for (int64_t k = 0; k < nA; ++k) {
+      const double c = price[r * nA + k];
+      if (!(std::isfinite(c) && c >= 0.0))
+        return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: price %g of allowed token %lld must be finite and >= 0",
+                    what, (long long)r, c, (long long)k + 1);
+      any |= c > 0.0;
+    }
+    if (!any) return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: no positive price", what, (long long)r);
+    if (min_profit && !(std::isfinite(min_profit[r]) && min_profit[r] >= 0.0))
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: min_profit %g must be finite and >= 0", what, (long long)r,
+                  min_profit[r]);
+  }
+  return CFMM_OK;
+}
+
+// The family's outputs through row_orders: the profit in received, no paid.
+int price_arbitrage(cfmm_ctx* ctx, bool exec, int64_t q, const double* price, const double* min_profit,
+                    const uint8_t* allowed, const cfmm_subgraph_opts& o, const cfmm_price_arb_out& out,
+                    const char* what) {
+  int rc;
+  if ((rc = row_begin(ctx)) != CFMM_OK) return rc;
+  std::vector<int64_t> tokA;  // the columns of price: the allowed tokens, ascending (0-based)
+  for (int64_t t = 0; t < ctx->n_tokens; ++t)
+    if (allowed[t]) tokA.push_back(t);
+  const int64_t nA = (int64_t)tokA.size();
+  DevBuf<double> d_price, d_min;
+  CU_TRY(ctx, d_price.upload(price, (size_t)(q * nA)));
+  CU_TRY(ctx, d_min.upload(min_profit, (size_t)q));
+  int occ = 0;
+  if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::price_arb_kernel<false>), {}, "price_arb_kernel", occ)) != CFMM_OK)
+    return rc;
+  int64_t uses = 0;  // the priced tokens over the call
+  for (int64_t e = 0; e < q * nA; ++e) uses += price[e] > 0.0;
+  cfmm_subgraph_out O{};
+  O.received = out.profit;
+  O.status = out.status;
+  O.solver_status = out.solver_status;
+  O.iterations = out.iterations;
+  O.fun_evals = out.fun_evals;
+  O.merit = out.merit;
+  O.tok_off = out.tok_off;
+  O.tok_cap = out.tok_cap;
+  O.token = out.token;
+  O.nu = out.nu;
+  O.psi = out.psi;
+  O.leg_off = out.leg_off;
+  O.leg_cap = out.leg_cap;
+  O.leg_type = out.leg_type;
+  O.leg_pool = out.leg_pool;
+  O.leg_delta = out.leg_delta;
+  O.leg_lambda = out.leg_lambda;
+  cfmm::PriceArbRows R{d_price.p, d_min.p, o.max_iter, o.max_fun, o.rtol, o.factr};
+  // a row's T lies in its priced tokens: rows whose priced tokens are disjoint share no pool
+  return row_orders(
+      ctx, exec, q, allowed, R, O, occ, 0, 0, 0, 0, uses, false, what,
+      [&](unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets*, cfmm::PairIndexView pv, cfmm::AdjView,
+          const cfmm::BestPathGraph& G, const uint8_t* act, int64_t* ntok, int64_t* npool) {
+        cfmm::price_arb_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(pv, G, act, d_price.p, q, ntok, npool);
+      },
+      [&](auto exec_tag, bool, unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P,
+          cfmm::PairIndexView pv, cfmm::AdjView, const cfmm::BestPathGraph& G, const uint8_t* act,
+          const cfmm::PriceArbRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv, const int64_t* rows,
+          int64_t n) {
+        constexpr bool X = decltype(exec_tag)::value;
+        cfmm::price_arb_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, G, act, R, W, mv, rows, n);
+      },
+      [](int64_t) { return false; },
+      [&](int64_t r, auto&& visit) {
+        for (int64_t k = 0; k < nA; ++k)
+          if (price[r * nA + k] > 0.0) visit(0, tokA[(size_t)k]);
+      });
+}
+
+int price_arb_call(cfmm_ctx* ctx, bool exec, int64_t q, const double* price, const double* min_profit,
+                   const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_price_arb_out* out, const char* what) {
+  const cfmm_subgraph_opts o = subgraph_opts(opts);
+  int rc = check_price_arb(ctx, q, price, min_profit, allowed, o, what);
+  if (rc != CFMM_OK) return rc;
+  if (q == 0) {
+    if (out && out->tok_off) out->tok_off[0] = 0;
+    if (out && out->leg_off) out->leg_off[0] = 0;
+    return CFMM_OK;
+  }
+  const cfmm_price_arb_out none{};
+  return price_arbitrage(ctx, exec, q, price, min_profit, allowed, o, out ? *out : none, what);
 }
 
 }  // namespace
@@ -4509,6 +4614,16 @@ int cfmm_execute_basket_swap_orders(cfmm_ctx* ctx, int64_t q, const int64_t* tok
                                     const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
   return basket_call(ctx, true, q, token_out, basket_off, basket_token, entry_kind, basket_amount, limit, allowed,
                      opts, out, "execute_basket_swap_orders");
+}
+
+int cfmm_quote_price_arbitrage(cfmm_ctx* ctx, int64_t q, const double* price, const uint8_t* allowed,
+                               const cfmm_subgraph_opts* opts, cfmm_price_arb_out* out) {
+  return price_arb_call(ctx, false, q, price, nullptr, allowed, opts, out, "quote_price_arbitrage");
+}
+
+int cfmm_execute_price_arbitrage(cfmm_ctx* ctx, int64_t q, const double* price, const double* min_profit,
+                                 const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_price_arb_out* out) {
+  return price_arb_call(ctx, true, q, price, min_profit, allowed, opts, out, "execute_price_arbitrage");
 }
 
 // ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------

@@ -18,11 +18,11 @@
 // time.  subgraph_plan_kernel runs the setup only and reports each row's token and pool counts, which
 // size the outputs and the workspace (they do not depend on the kind).
 //
-// basket_kernels.cuh's rows run everything after their own setup through this file's helpers, which
-// take the row's shared state and its rules as template parameters: the pool gather, the pool
-// ordering, the evaluation, the commit, the L-BFGS driver, the legs, and the pair activity, CTA sum,
-// pool view, start and capacity.  The setups stay per kind: running subgraph rows through the longer
-// basket setup cost 2.3–2.6 % more kernel time on the headline set (DESIGN §4.5).
+// basket_kernels.cuh's and price_arb_kernels.cuh's rows run everything after their own setup through
+// this file's helpers, which take the row's shared state and its rules as template parameters: the
+// pool gather, the pool ordering, the evaluation, the commit, the L-BFGS driver, the legs, and the
+// pair activity, CTA sum, pool view, start and capacity.  The setups stay per kind: running subgraph
+// rows through the longer basket setup cost 2.3–2.6 % more kernel time on the headline set (DESIGN §4.5).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -264,21 +264,25 @@ __device__ __forceinline__ double sg_lo(int t) { return OUT ? kSubgraphSqrtEps :
 // row kind (basket_kernels.cuh's BkRule gives the same for basket rows):
 //   lin(m, t)     the linear term of slot t's gradient: lin at kLin (amt at j, or −y′ at i), else 0;
 //   value(m)      the dual's linear value at ν = xt, lin·ν_kLin;
-//   lo(t), fixed(m, t)   the box;
+//   lo(m, t), fixed(m, t)   the box;
+//   kBoxStart     false: the start is sg_start's (true: the box's lower bound, sg_box_start);
 //   kOut, root(m) sg_start's root and clamp (exact-out: slot 1, j, fixed at 1);
+//   evaluated(m, f)   sees the dual value f of every evaluation (nothing here);
 //   merit(m, mx)  m_r from the CTA max mx = max_t ν_t·|pg_t|: mx / (δ·ν_j), or mx / (y·ν_i).
 // Every value is the same IEEE operations in the same order as the rule's other uses, so a one-entry
 // basket row gives an exact-in row's bits and a one-bought-entry buy row an exact-out row's.
 template <bool OUT>
 struct SgRule {
   static constexpr bool kOut = OUT;
+  static constexpr bool kBoxStart = false;
   static constexpr int kLin = OUT ? 0 : 1;
   double lin, amt;
   __device__ __forceinline__ double lin_at(const SubgraphSmem&, int t) const { return t == kLin ? lin : 0.0; }
   __device__ __forceinline__ double value(const SubgraphSmem& m) const { return __dmul_rn(lin, m.xt[kLin]); }
-  __device__ __forceinline__ double lo(int t) const { return sg_lo<OUT>(t); }
+  __device__ __forceinline__ double lo(const SubgraphSmem&, int t) const { return sg_lo<OUT>(t); }
   __device__ __forceinline__ bool fixed(const SubgraphSmem&, int t) const { return OUT && t == 1; }
   __device__ __forceinline__ int root(const SubgraphSmem&) const { return OUT ? 1 : 0; }
+  __device__ __forceinline__ void evaluated(SubgraphSmem&, double) const {}
   __device__ __forceinline__ double merit(const SubgraphSmem& m, double mx) const {
     return __ddiv_rn(mx, __dmul_rn(amt, m.x[OUT ? 0 : 1]));
   }
@@ -314,7 +318,9 @@ __device__ double sg_evaluate(const PathSets* P, const SubgraphWork& w, Smem& m,
     }
   }
   __syncthreads();
-  return __dadd_rn(rule.value(m), V);
+  const double f = __dadd_rn(rule.value(m), V);
+  rule.evaluated(m, f);
+  return f;
 }
 
 // Accept xt: (s, y) into history slot `slot` when store, x <- xt, g <- gt, Ψ, the projected gradient
@@ -333,7 +339,7 @@ __device__ double sg_commit(Smem& m, int slot, bool store, const Rule& rule) {
     m.x[t] = xn;
     m.g[t] = gn;
     m.px[t] = m.pt[t];
-    m.pg[t] = rule.fixed(m, t) || (xn <= rule.lo(t) && gn > 0.0) ? 0.0 : gn;
+    m.pg[t] = rule.fixed(m, t) || (xn <= rule.lo(m, t) && gn > 0.0) ? 0.0 : gn;
   }
   __syncthreads();
   double mx = 0.0;
@@ -389,6 +395,13 @@ __device__ void sg_start(const PathSets* P, const SubgraphWork& w, Smem& m, int 
     if (!more) break;
   }
   for (int t = tid; t < n; t += blockDim.x) m.xt[t] = OUT && t == root ? 1.0 : fmax(m.x[t], sg_lo<OUT>(t));
+  __syncthreads();
+}
+
+// The start of a rule with kBoxStart: every slot at its lower bound.  Into x and xt.
+template <class Smem, class Rule>
+__device__ __forceinline__ void sg_box_start(Smem& m, const Rule& rule) {
+  for (int t = threadIdx.x; t < m.n_loc; t += blockDim.x) m.x[t] = m.xt[t] = rule.lo(m, t);
   __syncthreads();
 }
 
@@ -529,8 +542,9 @@ struct SgSolveState {
 };
 
 // cfmm_solve's projected L-BFGS (solver_control.cuh) on the row's dual over its n local tokens, every
-// vector in shared memory, from sg_start when solve (else nothing runs).  Returns the solver status
-// (−1: no solve) and sets merit to the last m_r; s keeps the iteration and evaluation counts.
+// vector in shared memory, from sg_start (kBoxStart: sg_box_start) when solve (else nothing runs).
+// Returns the solver status (−1: no solve) and sets merit to the last m_r; s keeps the iteration and
+// evaluation counts.
 template <class Smem, class Rule, class Rows>
 __device__ __forceinline__ int sg_solve(const PathSets* P, const SubgraphWork& w, Smem& m, const Rule& rule,
                                         const Rows& R, int64_t n, bool solve, SgSolveState& s, double& merit) {
@@ -545,7 +559,10 @@ __device__ __forceinline__ int sg_solve(const PathSets* P, const SubgraphWork& w
   if (!solve) return status;
   for (int t = tid; t < n; t += blockDim.x)  // an empty history, as cfmm_solve's zeroed one
     for (int a = 0; a < kSolverM; ++a) m.S[a][t] = m.Y[a][t] = 0.0;
-  sg_start<Smem, Rule::kOut>(P, w, m, rule.root(m));
+  if constexpr (Rule::kBoxStart)
+    sg_box_start(m, rule);
+  else
+    sg_start<Smem, Rule::kOut>(P, w, m, rule.root(m));
   f = sg_evaluate(P, w, m, rule);
   merit = sg_commit(m, 0, false, rule);
   if (tid == 0) {
@@ -574,7 +591,7 @@ __device__ __forceinline__ int sg_solve(const PathSets* P, const SubgraphWork& w
         v = fma(m.c[a], m.S[a][t], v);
         v = fma(m.c[kSolverM + a], m.Y[a][t], v);
       }
-      m.d[t] = rule.fixed(m, t) || (m.x[t] <= rule.lo(t) && m.g[t] > 0.0) ? 0.0 : -v;
+      m.d[t] = rule.fixed(m, t) || (m.x[t] <= rule.lo(m, t) && m.g[t] > 0.0) ? 0.0 : -v;
     }
     __syncthreads();
     int dec = kLsRetry;
@@ -583,7 +600,7 @@ __device__ __forceinline__ int sg_solve(const PathSets* P, const SubgraphWork& w
       const double t = s.t;
       double gd = 0.0, st2 = 0.0;
       for (int k = tid; k < n; k += blockDim.x) {
-        const double y = rule.fixed(m, k) ? 1.0 : fmax(fma(t, m.d[k], m.x[k]), rule.lo(k));
+        const double y = rule.fixed(m, k) ? 1.0 : fmax(fma(t, m.d[k], m.x[k]), rule.lo(m, k));
         m.xt[k] = y;
         const double dx = __dsub_rn(y, m.x[k]);
         gd = fma(m.g[k], dx, gd);

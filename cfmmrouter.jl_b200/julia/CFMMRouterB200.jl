@@ -761,6 +761,57 @@ execute_basket_swap_orders!(ctx, token_out, basket_off, basket_token, entry_kind
                             limit=nothing, opts=nothing) =
     _basket_orders(ctx, true, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts, entry_kind)
 
+# Arbitrage against external prices (cfmm_quote_price_arbitrage / cfmm_execute_price_arbitrage): price is
+# n_A x q (column r = row r's prices of the allowed tokens, ascending; 0 leaves a token out), and each
+# row maximises price'Ψ with Ψ >= 0 over the pools among its priced tokens (LinearNonnegative).
+# min_profit (nothing: none) is one minimum profit per row.  Returns the NamedTuple of _subgraph_orders
+# with profit for paid and received.  Never executed, like the rest of this file.
+struct PriceArbOut
+    profit::Ptr{Float64}; status::Ptr{UInt8}
+    solver_status::Ptr{Cint}; iterations::Ptr{Cint}; fun_evals::Ptr{Cint}; merit::Ptr{Float64}
+    tok_off::Ptr{Int64}; tok_cap::Int64; token::Ptr{Int64}; nu::Ptr{Float64}; psi::Ptr{Float64}
+    leg_off::Ptr{Int64}; leg_cap::Int64; leg_type::Ptr{Cint}; leg_pool::Ptr{Int64}
+    leg_delta::Ptr{Float64}; leg_lambda::Ptr{Float64}
+end
+function _price_arbitrage(ctx, execute::Bool, price::Matrix{Float64}, allowed::Vector{UInt8}, min_profit, opts)
+    q = size(price, 2)
+    size(price, 1) == count(!=(0), allowed) || throw(ArgumentError("price needs one row per allowed token"))
+    min_profit === nothing || length(min_profit) == q || throw(ArgumentError("min_profit needs q entries"))
+    o = opts === nothing ? nothing : Ref(opts)
+    argq = (Ptr{Cvoid}, Int64, Ptr{Float64}, Ptr{UInt8}, Ptr{SubgraphOpts}, Ptr{PriceArbOut})
+    tok_off, leg_off = zeros(Int64, q + 1), zeros(Int64, q + 1)
+    sizes = Ref(PriceArbOut(C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, pointer(tok_off), 0, C_NULL, C_NULL,
+                            C_NULL, pointer(leg_off), 0, C_NULL, C_NULL, C_NULL, C_NULL))
+    GC.@preserve tok_off leg_off chk(ctx, ccall((:cfmm_quote_price_arbitrage, LIB), Cint, argq, ctx, q, price,
+                                               allowed, o === nothing ? C_NULL : o, sizes))
+    NT, L = tok_off[end], leg_off[end]
+    profit, merit, status = zeros(q), zeros(q), zeros(UInt8, q)
+    sst, iters, fev = zeros(Cint, q), zeros(Cint, q), zeros(Cint, q)
+    token, nu, psi = zeros(Int64, max(NT, 1)), zeros(max(NT, 1)), zeros(max(NT, 1))
+    ltype, lpool, ld, ll = zeros(Cint, max(L, 1)), zeros(Int64, max(L, 1)), zeros(2, max(L, 1)), zeros(2, max(L, 1))
+    GC.@preserve profit merit status sst iters fev tok_off token nu psi leg_off ltype lpool ld ll begin
+        out = Ref(PriceArbOut(pointer(profit), pointer(status), pointer(sst), pointer(iters), pointer(fev),
+                              pointer(merit), pointer(tok_off), NT, pointer(token), pointer(nu), pointer(psi),
+                              pointer(leg_off), L, pointer(ltype), pointer(lpool), pointer(ld), pointer(ll)))
+        if execute
+            chk(ctx, ccall((:cfmm_execute_price_arbitrage, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8}, Ptr{SubgraphOpts}, Ptr{PriceArbOut}),
+                ctx, q, price, min_profit === nothing ? C_NULL : min_profit, allowed, o === nothing ? C_NULL : o,
+                out))
+        else
+            chk(ctx, ccall((:cfmm_quote_price_arbitrage, LIB), Cint, argq, ctx, q, price, allowed,
+                           o === nothing ? C_NULL : o, out))
+        end
+    end
+    return (profit=profit, status=status, solver_status=sst, iterations=iters, fun_evals=fev, merit=merit,
+            tok_off=tok_off, token=token[1:NT], nu=nu[1:NT], psi=psi[1:NT], leg_off=leg_off, leg_type=ltype[1:L],
+            leg_pool=lpool[1:L], leg_delta=ld[:, 1:L], leg_lambda=ll[:, 1:L])
+end
+quote_price_arbitrage(ctx, price, allowed; opts=nothing) =
+    _price_arbitrage(ctx, false, price, allowed, nothing, opts)
+execute_price_arbitrage!(ctx, price, allowed; min_profit=nothing, opts=nothing) =
+    _price_arbitrage(ctx, true, price, allowed, min_profit, opts)
+
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
 # current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never

@@ -806,7 +806,9 @@ class DevicePools:
         token, nu, psi = np.zeros(max(NT, 1), dtype=np.int64), np.zeros(max(NT, 1)), np.zeros(max(NT, 1))
         ltype, lpool = np.zeros(max(L, 1), dtype=np.int32), np.zeros(max(L, 1), dtype=np.int64)
         ld, ll = np.zeros((max(L, 1), 2)), np.zeros((max(L, 1), 2))
-        out = out_type(paid.ctypes.data_as(f64), received.ctypes.data_as(f64), status.ctypes.data_as(u8),
+        head = ((received.ctypes.data_as(f64),) if out_type is _lib.PriceArbOut else
+                (paid.ctypes.data_as(f64), received.ctypes.data_as(f64)))  # price rows: the profit
+        out = out_type(*head, status.ctypes.data_as(u8),
                        sst.ctypes.data_as(i32), iters.ctypes.data_as(i32), fev.ctypes.data_as(i32),
                        merit.ctypes.data_as(f64), tok_off.ctypes.data_as(i64), NT, token.ctypes.data_as(i64),
                        nu.ctypes.data_as(f64), psi.ctypes.data_as(f64), leg_off.ctypes.data_as(i64), L,
@@ -890,6 +892,55 @@ class DevicePools:
         received of token_out[r] (for a row with a bought entry it may be negative or -inf), and a row
         below it reverts.  Returns what quote_basket_orders returns."""
         return self._basket(True, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts, kind)
+
+    # -- arbitrage against external prices over every pool among allowed tokens (include/cfmm_b200.h,
+    #    cfmm_quote_price_arbitrage / cfmm_execute_price_arbitrage) --------------------------------------
+    def _price_arb(self, execute, price, allowed, min_profit, opts):
+        u8m, _, po = _row_args(self.n_tokens, None, allowed, None, opts, "price arbitrage")
+        nA = int(np.count_nonzero(np.asarray(allowed, dtype=bool)))
+        if nA > _lib.PRICE_ARB_MAX_TOKENS:
+            raise ValueError(f"price arbitrage: {nA} allowed tokens, more than {_lib.PRICE_ARB_MAX_TOKENS}")
+        price = np.ascontiguousarray(price, dtype=np.float64)
+        if price.ndim != 2 or price.shape[1] != nA:
+            raise ValueError(f"price arbitrage: price must be [q, {nA}], one column per allowed token")
+        q = price.shape[0]
+        if not np.all(np.isfinite(price) & (price >= 0.0)):
+            raise ValueError("price arbitrage: a price is negative, NaN or Inf")
+        if q and not np.all(np.any(price > 0.0, axis=1)):
+            raise ValueError("price arbitrage: a row has no positive price")
+        lim = None
+        if min_profit is not None:
+            min_profit = np.ascontiguousarray(np.broadcast_to(np.asarray(min_profit, dtype=np.float64), (q,)))
+            if not np.all(np.isfinite(min_profit) & (min_profit >= 0.0)):
+                raise ValueError("price arbitrage: a min_profit is negative, NaN or Inf")
+            lim = _dp(min_profit)
+        pr = _dp(price)
+
+        def call(size, out):
+            if execute and not size:
+                return self._lib.cfmm_execute_price_arbitrage(self._ctx, q, pr, lim, u8m, po, C.byref(out))
+            return self._lib.cfmm_quote_price_arbitrage(self._ctx, q, pr, u8m, po, C.byref(out))
+        out = self._order_solve(q, 0, _lib.PriceArbOut, call)
+        out.profit = out.received
+        del out.paid, out.received
+        return out
+
+    def quote_price_arbitrage(self, price, allowed, opts=None):
+        """cfmm_quote_price_arbitrage: row r values the tokens t with allowed[t - 1] (ascending, at most
+        258) at price[r] (0: the token is not in the row, else finite and > 0) and trades over every pool
+        among its priced tokens to maximise Σ price·Ψ with no token's net negative: route! with
+        LinearNonnegative over the row's pools, solved per row on the device.  opts as
+        quote_subgraph_orders.  No state changes.  Returns a namespace: profit, status (uint8),
+        solver_status, iterations, fun_evals, merit [q]; tok_off [q + 1], token, nu, psi [Σ]; leg_off
+        [q + 1], leg_type, leg_pool [L], leg_delta, leg_lambda [L, 2]."""
+        return self._price_arb(False, price, allowed, None, opts)
+
+    def execute_price_arbitrage(self, price, allowed, min_profit=None, opts=None):
+        """cfmm_execute_price_arbitrage: the rows of quote_price_arbitrage in batch order, each re-solved
+        on the state the earlier filled rows left; min_profit (None, a scalar or one per row; finite and
+        >= 0) is the minimum profit, and a row below it reverts.  Returns what quote_price_arbitrage
+        returns."""
+        return self._price_arb(True, price, allowed, min_profit, opts)
 
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
@@ -1615,6 +1666,35 @@ class Router:
         out = self._pools.execute_basket_orders(tout, off, toks, amts, allowed, limits, opts)
         self._refresh_filled(out)
         return self._per_entry(out), out.received, out.status, out
+
+    def _price_arb_args(self, prices, allowed, what):
+        if self._world > 1:
+            raise NotImplementedError(f"{what} drives one GPU")
+        if allowed is None:
+            raise ValueError(f"{what}: allowed (a mask over the tokens) is required")
+        prices = np.asarray(prices, dtype=np.float64)
+        return prices.reshape(1, -1) if prices.ndim == 1 else prices
+
+    def quote_price_arbitrage(self, prices, allowed, opts=None):
+        """The best trades through every pool among each row's priced tokens against external prices:
+        prices[r] gives one price per token t with allowed[t - 1], ascending (0 leaves a token out of
+        the row; a 1-D array is one row).  Each row maximises Σ price·Ψ with no token's net negative,
+        route! with LinearNonnegative over those pools, one dual solve per row on the device
+        (cfmm_quote_price_arbitrage).  No state changes.  Returns (profit [q], status [q], detail):
+        detail is DevicePools.quote_price_arbitrage's namespace.  Single GPU."""
+        out = self._pools.quote_price_arbitrage(self._price_arb_args(prices, allowed, "quote_price_arbitrage"),
+                                                allowed, opts)
+        return out.profit, out.status, out
+
+    def execute_price_arbitrage(self, prices, allowed, min_profit=None, opts=None):
+        """Execute price arbitrage rows in order (cfmm_execute_price_arbitrage), each re-solved on the
+        state the earlier filled rows left, with an optional minimum profit: a row below it reverts.
+        Returns what quote_price_arbitrage returns and refreshes the pool objects the filled rows traded
+        with from the device state.  Single GPU."""
+        out = self._pools.execute_price_arbitrage(self._price_arb_args(prices, allowed, "execute_price_arbitrage"),
+                                                  allowed, min_profit, opts)
+        self._refresh_filled(out)
+        return out.profit, out.status, out
 
     def _arbitrage_args(self, base, other, hubs, min_profit, what):
         if self._world > 1:

@@ -1042,6 +1042,77 @@ int cfmm_execute_basket_swap_orders(cfmm_ctx *ctx, int64_t q, const int64_t *tok
                                     const uint8_t *allowed, const cfmm_subgraph_opts *opts,
                                     cfmm_basket_out *out);
 
+/* ---- arbitrage against external prices over every pool among allowed tokens ----------------
+ * A row values tokens at external prices c and trades through every pool among its priced tokens to
+ * maximise cᵀΨ with no token's net flow negative: route! with LinearNonnegative(c)
+ * (src/objectives.jl:51-79) restricted to the row's pools, one convex dual per row.
+ *   A        the tokens t with allowed[t-1] != 0 (allowed [n_tokens], required; one mask per call),
+ *            ascending; n_A <= CFMM_PRICE_ARB_MAX_TOKENS.
+ *   price    [q·n_A], row-major, columns in A's order.  Each price is 0 (the token is not in this
+ *            row) or finite and > 0, and every row has a positive price.
+ *   T        the row's priced tokens that hold at least one active pool whose two tokens are both
+ *            priced.  Every component of T is an arbitrage of its own; every token in it has a price.
+ *   pools    every pool of every pair inside T, all three types, appended pools included, retired
+ *            pools listed (they trade (0, 0)), in global insertion order, as for subgraph orders.
+ *   tokens   local order: T ascending.
+ * Problem.  Minimise g(ν) = Σ_p π_p(ν) on the box ν_t >= c_t + 1e-8 (one IEEE addition, as
+ * LinearNonnegative's lower limit), with no upper bound and no linear term.  Legs, the Ψ sums and the
+ * value sum are those of subgraph orders, bit for bit in their operation order; the gradient is Ψ.
+ *   start    ν⁰ = the box's lower bound: the caller's prices are the point the arbitrage is measured
+ *            from (no breadth-first pricing).
+ *   stop     m_r = max_t ν_t·|pg_t| / g(ν) at the committed iterate (g: the committed dual value,
+ *            its profit: π is positively homogeneous, so g = νᵀΨ).  Status 0 when m_r <= rtol; the
+ *            other statuses as cfmm_solve.  mx = max_t ν_t·|pg_t| = 0 gives m_r = 0; mx > 0 with
+ *            g <= 0 gives m_r = +inf.  A row where no pool trades at ν⁰ (T empty included) fills with
+ *            zeros after that one evaluation: solver status 0, 0 iterations, 1 evaluation, m_r = 0.
+ * What a fill promises.  A row fills only at solver status 0 (else CFMM_ORDER_NOT_CONVERGED, with
+ * zero legs and profit; ν, Ψ and m_r stay those of the last iterate).  A filled row has
+ * profit = Σ_t c_t·Ψ_t in local order (the first term alone, then IEEE additions), and, from
+ * m_r <= rtol with ν_t·|pg_t| <= rtol·g:
+ *   each token's net Ψ_t >= −rtol·g/ν_t (the caller funds at most that much of t);
+ *   g − cᵀΨ = Σ_t (ν_t − c_t)·Ψ_t <= |T|·rtol·g + Σ_{t on its bound} 1e-8·max(Ψ_t, 0), each free
+ *   token adding at most (ν_t − c_t)·rtol·g/ν_t <= rtol·g, so the duality gap against the optimum
+ *   (at most g) is at most |T|·rtol·g plus the box terms (up to the rounding of fp64 sums).
+ * Outputs (cfmm_price_arb_out; every pointer may be NULL): per row profit, status (CFMM_ORDER_*),
+ * solver_status, iterations, fun_evals, merit (m_r); tokens and legs as cfmm_subgraph_out.  Ask a
+ * quote with tok_cap = leg_cap = 0 for the sizes first.
+ * cfmm_quote_price_arbitrage prices every row on the current state on its own; no state changes.
+ * cfmm_execute_price_arbitrage runs the rows in batch order, each re-solved on the state the earlier
+ * filled rows left.  min_profit (NULL: none; finite and >= 0) is the minimum profit: an equal profit
+ * fills, a smaller one reverts with CFMM_ORDER_LIMIT.  A filled row applies split_leg's transition at
+ * its ν, then the bookkeeping of cfmm_execute_swaps.  Two rows conflict when their priced tokens
+ * overlap (a row's T lies in them); rows are leveled by cfmm_execute_paths' rule, one launch per
+ * level, so rows on disjoint price subsets share a launch.  An execute whose token or leg outputs are
+ * given with a cap below the size is rejected before anything changes.
+ * Options: cfmm_subgraph_opts, with its defaults.  Single GPU.  Synchronous.  Before cfmm_finalize:
+ * CFMM_ERR_STATE.  q == 0 does nothing.  CFMM_ERR_INVALID before anything runs for: q < 0; a null
+ * price or allowed; more than CFMM_PRICE_ARB_MAX_TOKENS allowed tokens; a price that is negative,
+ * NaN or Inf; a row with no positive price; the option errors of subgraph orders; a min_profit that
+ * is NaN, negative or Inf. */
+#define CFMM_PRICE_ARB_MAX_TOKENS (CFMM_SUBGRAPH_MAX_TOKENS + 2)
+typedef struct {
+  double *profit;                                /* [q] */
+  uint8_t *status;                               /* [q] */
+  int *solver_status, *iterations, *fun_evals;   /* [q] */
+  double *merit;                                 /* [q] */
+  int64_t *tok_off;                              /* [q+1] */
+  int64_t tok_cap;
+  int64_t *token;                                /* [tok_off[q]] */
+  double *nu, *psi;                              /* [tok_off[q]] */
+  int64_t *leg_off;                              /* [q+1] */
+  int64_t leg_cap;
+  int *leg_type;                                 /* [leg_off[q]] */
+  int64_t *leg_pool;                             /* [leg_off[q]] */
+  double *leg_delta, *leg_lambda;                /* [2·leg_off[q]] */
+} cfmm_price_arb_out;
+int cfmm_quote_price_arbitrage(cfmm_ctx *ctx, int64_t q, const double *price /* [q·n_A] */,
+                               const uint8_t *allowed /* [n_tokens], required */,
+                               const cfmm_subgraph_opts *opts /* NULL = defaults */,
+                               cfmm_price_arb_out *out);
+int cfmm_execute_price_arbitrage(cfmm_ctx *ctx, int64_t q, const double *price,
+                                 const double *min_profit /* [q] or NULL */, const uint8_t *allowed,
+                                 const cfmm_subgraph_opts *opts, cfmm_price_arb_out *out);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
