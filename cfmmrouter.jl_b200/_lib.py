@@ -40,7 +40,7 @@ PATH_REPEATS_POOL = 4
 # cfmm_quote_subgraph_(swap_)orders / cfmm_execute_subgraph_(swap_)orders
 SUBGRAPH_MAX_TOKENS = 256
 ORDER_NOT_CONVERGED = 5
-# cfmm_quote_basket_(swap_)orders / cfmm_execute_basket_(swap_)orders
+# cfmm_quote_basket_(swap_)orders / cfmm_execute_basket_(swap_)orders, cfmm_quote/execute_limit_orders
 BASKET_MAX_TOKENS = 16
 # cfmm_quote_price_arbitrage / cfmm_execute_price_arbitrage
 PRICE_ARB_MAX_TOKENS = SUBGRAPH_MAX_TOKENS + 2
@@ -73,6 +73,11 @@ class SubgraphOut(C.Structure):
 
 class BasketOut(SubgraphOut):
     """cfmm_basket_out: cfmm_subgraph_out's fields, with paid per basket entry."""
+
+
+class LimitOut(C.Structure):
+    """cfmm_limit_out: cfmm_basket_out's fields, plus the surplus per row."""
+    _fields_ = SubgraphOut._fields_ + [("surplus", C.POINTER(C.c_double))]
 
 
 class PriceArbOut(C.Structure):
@@ -161,6 +166,10 @@ SYMBOLS = {
     "cfmm_execute_basket_swap_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, C.POINTER(C.c_uint8), _dp, _dp,
                                                   C.POINTER(C.c_uint8), C.POINTER(SubgraphOpts),
                                                   C.POINTER(BasketOut)]),
+    "cfmm_quote_limit_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, _dp, _dp, C.POINTER(C.c_uint8),
+                                          C.POINTER(SubgraphOpts), C.POINTER(LimitOut)]),
+    "cfmm_execute_limit_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, _dp, _dp, _dp, C.POINTER(C.c_uint8),
+                                            C.POINTER(SubgraphOpts), C.POINTER(LimitOut)]),
     "cfmm_quote_price_arbitrage": (C.c_int, [_ctx, C.c_int64, _dp, C.POINTER(C.c_uint8), C.POINTER(SubgraphOpts),
                                              C.POINTER(PriceArbOut)]),
     "cfmm_execute_price_arbitrage": (C.c_int, [_ctx, C.c_int64, _dp, _dp, C.POINTER(C.c_uint8),

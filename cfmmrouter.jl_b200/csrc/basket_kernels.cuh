@@ -27,6 +27,12 @@
 // ν_t >= √eps; the start prices from i's slot; the stop adds a term per bought entry; and a bought
 // entry's capacity is checked before the solve (sg_capacity at its slot).  One bought entry and no
 // sold entries give subgraph_out_kernel's outputs bit for bit.
+//
+// basket_limit_kernel runs limit rows (cfmm_quote_limit_orders / cfmm_execute_limit_orders): a basket
+// row whose entries carry limit prices c_k (units of i per unit of b_k).  It is the basket row with LIM
+// set at compile time: the box of entry k in T is ν_k >= fmax(c_k, √eps) (LimRule's per-slot lo, which
+// also clamps the start), and an entry outside T with c_k > 0 is dropped rather than making the row
+// unreachable.  Every c_k = 0 gives basket_kernel's outputs bit for bit.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -66,6 +72,11 @@ struct BasketRows {
   double* leg_lambda;
 };
 
+// The rows of a limit call: the basket rows', plus each entry's limit price.
+struct LimitRows : BasketRows {
+  const double* limit_price;  // [basket_off[q]]: c_k, the least i per unit of b_k
+};
+
 // Shared state of one row.  kpair[k][l] is the pair {b_k, b_l}, kpair[k][k] the pair {b_k, i};
 // kact the same pairs' activity.
 struct BasketSmem {
@@ -101,6 +112,11 @@ struct BasketBuySmem : BasketSmem {
 };
 template <bool BUY>
 using BkSmem = std::conditional_t<BUY, BasketBuySmem, BasketSmem>;
+
+// A limit row's shared state: the basket row's, plus the lower bound of every local slot (LimRule).
+struct BasketLimitSmem : BasketSmem {
+  double lo[kSubgraphLocal];
+};
 
 // The local slot of entry k (in local order, i skipped), and i's slot.
 template <bool BUY>
@@ -355,16 +371,28 @@ struct BkRule {
   }
 };
 
+// The rules of a limit row: the basket row's (BkRule<false>), with the box read per slot from m.lo:
+// ν_i >= 1 + √eps, ν_k >= fmax(c_k, √eps) at the entries in T, ν_t >= √eps elsewhere.
+struct LimRule : BkRule<false> {
+  __device__ __forceinline__ double lo(const BasketLimitSmem& m, int t) const { return m.lo[t]; }
+};
+
+template <bool BUY, bool LIM>
+using BkRowSmem = std::conditional_t<LIM, BasketLimitSmem, BkSmem<BUY>>;
+template <bool LIM>
+using BkRows = std::conditional_t<LIM, LimitRows, BasketRows>;
+
 // Row r on the current state.  Returns nothing; writes the row's outputs.  EXEC: the limit decides,
 // and a filled row applies the transition of cfmm_apply_trades at its ν to each of its pools.  BUY:
 // a buy row (its entries' kinds in m.bkind): the dual has lin = δ_k at sold and −y′_l at bought
 // entries and ν_i fixed at 1; a bought entry with y_l at least what the row's pools holding b_l could
 // pay out makes the row unreachable, and a row fills only when every bought entry with y_l > 0
-// receives at least y_l.
-template <bool EXEC, bool BUY = false>
+// receives at least y_l.  LIM: a limit row (R.limit_price): the box of entry k in T is
+// ν_k >= fmax(c_k, √eps), and an entry outside T with c_k > 0 is dropped (paid 0).
+template <bool EXEC, bool BUY = false, bool LIM = false>
 __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
-                             const uint8_t* gact, const BasketRows& R, const SubgraphWork& w, const SplitMoved& mv,
-                             int64_t r, BkSmem<BUY>& m) {
+                             const uint8_t* gact, const BkRows<LIM>& R, const SubgraphWork& w, const SplitMoved& mv,
+                             int64_t r, BkRowSmem<BUY, LIM>& m) {
   __shared__ SgSolveState s;
   __shared__ int s_any, s_unreach;
   const int tid = threadIdx.x;
@@ -373,7 +401,28 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
                 (int32_t)(R.token_out[r] - 1), m);
   const int64_t np = m.npool, n = m.n_loc;
   // the amounts of the basket tokens in T; a positive amount outside T makes the row unreachable
-  if constexpr (BUY) {
+  if constexpr (LIM) {
+    // Swap's box, then each entry in T raised to its limit; an entry outside T with c_k > 0 cannot
+    // fill at any price and is dropped, one with c_k = 0 follows the basket rule
+    for (int t = tid; t < n; t += blockDim.x) m.lo[t] = sg_lower(t);
+    __syncthreads();
+    if (tid == 0) {
+      int any = 0, unreach = 0;
+      for (int k = 0; k < m.nK; ++k) {
+        const double a = R.basket_amount[b0 + k], c = R.limit_price[b0 + k];
+        if (m.bloc[k] >= 0) {
+          m.bamt[m.bloc[k] - 1] = a;
+          m.lo[m.bloc[k]] = fmax(c, kSubgraphSqrtEps);
+          any |= a > 0.0;
+        } else if (c == 0.0) {
+          any |= a > 0.0;
+          unreach |= a > 0.0;
+        }
+      }
+      s_any = any;
+      s_unreach = unreach;
+    }
+  } else if constexpr (BUY) {
     // bamt and blin by entry in local order (i skipped): δ and δ at sold, y and −y′ at bought entries
     if (tid == 0) {
       int any = 0, unreach = 0;
@@ -440,7 +489,7 @@ __device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const
   }
   const bool any = s_any, solve = any && !s_unreach;
   double merit;
-  const int status = sg_solve(P, w, m, BkRule<BUY>{}, R, n, solve, s, merit);
+  const int status = sg_solve(P, w, m, std::conditional_t<LIM, LimRule, BkRule<BUY>>{}, R, n, solve, s, merit);
   // status, the limit, the legs (and the transition on execute)
   const double received = solve ? m.px[bk_root<BUY>(m)] : 0.0;
   uint8_t st = 0;  // CFMM_ORDER_FILLED (amounts all 0: zeros, no solve)
@@ -509,6 +558,18 @@ __global__ void __launch_bounds__(kSubgraphThreads)
     if (threadIdx.x < R.basket_off[r + 1] - b0) m.bkind[threadIdx.x] = kind[b0 + threadIdx.x];
     basket_row<EXEC, true>(P, ix, A, G, gact, R, wb, mv, r, m);
   }
+}
+
+// Limit rows rows[0 .. n) (null: 0 .. n), as basket_kernel.
+template <bool EXEC>
+__global__ void __launch_bounds__(kSubgraphThreads)
+    basket_limit_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, BestPathGraph G,
+                        const uint8_t* __restrict__ gact, LimitRows R, SubgraphWork w, SplitMoved mv,
+                        const int64_t* __restrict__ rows, int64_t n) {
+  __shared__ BasketLimitSmem m;
+  const SubgraphWork wb = sg_cta_work(w);
+  for (int64_t k = blockIdx.x; k < n; k += gridDim.x)
+    basket_row<EXEC, false, true>(P, ix, A, G, gact, R, wb, mv, rows ? rows[k] : k, m);
 }
 
 }  // namespace cfmm

@@ -4360,10 +4360,12 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
       });
 }
 
-// kind null: every row sell-only (cfmm_quote/execute_basket_orders).
+// kind null: every row sell-only (cfmm_quote/execute_basket_orders).  limit_price set (kind null): every
+// row a limit row (cfmm_quote/execute_limit_orders), run by basket_limit_kernel.
 int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, const int64_t* basket_off,
-                  const int64_t* basket_token, const uint8_t* kind, const double* basket_amount, const double* limit,
-                  const uint8_t* allowed, const cfmm_subgraph_opts& o, const cfmm_basket_out& O, const char* what) {
+                  const int64_t* basket_token, const uint8_t* kind, const double* basket_amount,
+                  const double* limit_price, const double* limit, const uint8_t* allowed, const cfmm_subgraph_opts& o,
+                  const cfmm_basket_out& O, const char* what) {
   int rc;
   if ((rc = row_begin(ctx)) != CFMM_OK) return rc;
   const int64_t NE = basket_off[q];
@@ -4371,19 +4373,27 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
   for (int64_t r = 0; r < q; ++r) K = std::max<int>(K, (int)(basket_off[r + 1] - basket_off[r]));
   DevBuf<int64_t> d_out, d_boff, d_btok;
   DevBuf<uint8_t> d_kind;
-  DevBuf<double> d_bamt, d_limit;
+  DevBuf<double> d_bamt, d_limit, d_price;
   CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
   CU_TRY(ctx, d_boff.upload(basket_off, (size_t)q + 1));
   if (kind) CU_TRY(ctx, d_kind.upload(kind, (size_t)NE));
   CU_TRY(ctx, d_btok.upload(basket_token, (size_t)NE));
   CU_TRY(ctx, d_bamt.upload(basket_amount, (size_t)NE));
+  if (limit_price) CU_TRY(ctx, d_price.upload(limit_price, (size_t)NE));
   CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
   int occ = 0, occ_buy = 0;
-  if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::basket_kernel<false>),
-                          {kernel_ptr(&cfmm::basket_plan_kernel), kernel_ptr(&cfmm::basket_kernel<false>),
-                           kernel_ptr(&cfmm::basket_kernel<true>)},
-                          "basket_kernel", occ)) != CFMM_OK)
+  if (limit_price) {
+    if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::basket_limit_kernel<false>),
+                            {kernel_ptr(&cfmm::basket_plan_kernel), kernel_ptr(&cfmm::basket_limit_kernel<false>),
+                             kernel_ptr(&cfmm::basket_limit_kernel<true>)},
+                            "basket_limit_kernel", occ)) != CFMM_OK)
+      return rc;
+  } else if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::basket_kernel<false>),
+                                 {kernel_ptr(&cfmm::basket_plan_kernel), kernel_ptr(&cfmm::basket_kernel<false>),
+                                  kernel_ptr(&cfmm::basket_kernel<true>)},
+                                 "basket_kernel", occ)) != CFMM_OK) {
     return rc;
+  }
   // buy rows run basket_buy_kernel (sized the same way, once per context, when a call first has them)
   int64_t n_buy = 0;
   for (int64_t r = 0; r < q; ++r) n_buy += basket_buy_row(basket_off, kind, r);
@@ -4392,7 +4402,9 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
                           {kernel_ptr(&cfmm::basket_buy_kernel<false>), kernel_ptr(&cfmm::basket_buy_kernel<true>)},
                           "basket_buy_kernel", occ_buy)) != CFMM_OK)
     return rc;
-  cfmm::BasketRows R{d_out.p, d_boff.p, d_btok.p, d_bamt.p, d_limit.p, o.max_iter, o.max_fun, o.rtol, o.factr};
+  // (basket_kernel and basket_buy_kernel take the BasketRows part of R)
+  cfmm::LimitRows R{{d_out.p, d_boff.p, d_btok.p, d_bamt.p, d_limit.p, o.max_iter, o.max_fun, o.rtol, o.factr},
+                    d_price.p};
   return row_orders(
       ctx, exec, q, allowed, R, O, occ, occ_buy, n_buy, K, NE, q + NE, true, what,
       [&](unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P, cfmm::PairIndexView pv, cfmm::AdjView A,
@@ -4402,10 +4414,12 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
       },
       [&](auto exec_tag, bool second, unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P,
           cfmm::PairIndexView pv, cfmm::AdjView A, const cfmm::BestPathGraph& G, const uint8_t* act,
-          const cfmm::BasketRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv, const int64_t* rows,
+          const cfmm::LimitRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv, const int64_t* rows,
           int64_t n) {
         constexpr bool X = decltype(exec_tag)::value;
-        if (second)
+        if (limit_price)
+          cfmm::basket_limit_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, R, W, mv, rows, n);
+        else if (second)
           cfmm::basket_buy_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, R, d_kind.p, W, mv,
                                                                                 rows, n);
         else
@@ -4440,8 +4454,72 @@ int basket_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, c
     return CFMM_OK;
   }
   const cfmm_basket_out none{};
-  return basket_orders(ctx, exec, q, token_out, basket_off, basket_token, kind, basket_amount, limit, allowed, o,
-                       out ? *out : none, what);
+  return basket_orders(ctx, exec, q, token_out, basket_off, basket_token, kind, basket_amount, nullptr, limit,
+                       allowed, o, out ? *out : none, what);
+}
+
+// cfmm_quote/execute_limit_orders: the basket calls' checks, then every limit price finite and >= 0,
+// before anything runs; the rows through basket_orders; then each row's surplus on the host.
+int limit_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+               const int64_t* basket_token, const double* basket_amount, const double* limit_price,
+               const double* min_received, const uint8_t* allowed, const cfmm_subgraph_opts* opts,
+               cfmm_limit_out* out, const char* what) {
+  const cfmm_subgraph_opts o = subgraph_opts(opts);
+  int rc = check_basket(ctx, q, token_out, basket_off, basket_token, nullptr, basket_amount, min_received, allowed,
+                        o, what);
+  if (rc != CFMM_OK) return rc;
+  if (q == 0) {
+    if (out && out->tok_off) out->tok_off[0] = 0;
+    if (out && out->leg_off) out->leg_off[0] = 0;
+    return CFMM_OK;
+  }
+  if (!limit_price) return fail(ctx, CFMM_ERR_INVALID, "%s: null limit_price", what);
+  for (int64_t r = 0; r < q; ++r)
+    for (int64_t k = basket_off[r]; k < basket_off[r + 1]; ++k)
+      if (!(std::isfinite(limit_price[k]) && limit_price[k] >= 0.0))
+        return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: limit price %g must be finite and >= 0", what,
+                    (long long)r, limit_price[k]);
+  cfmm_basket_out O{};
+  if (out) {
+    O.paid = out->paid;
+    O.received = out->received;
+    O.status = out->status;
+    O.solver_status = out->solver_status;
+    O.iterations = out->iterations;
+    O.fun_evals = out->fun_evals;
+    O.merit = out->merit;
+    O.tok_off = out->tok_off;
+    O.tok_cap = out->tok_cap;
+    O.token = out->token;
+    O.nu = out->nu;
+    O.psi = out->psi;
+    O.leg_off = out->leg_off;
+    O.leg_cap = out->leg_cap;
+    O.leg_type = out->leg_type;
+    O.leg_pool = out->leg_pool;
+    O.leg_delta = out->leg_delta;
+    O.leg_lambda = out->leg_lambda;
+  }
+  // the surplus needs paid and received, whether or not the caller asked for them
+  const bool surplus = out && out->surplus;
+  std::vector<double> paid(surplus && !O.paid ? (size_t)basket_off[q] : 0),
+      recv(surplus && !O.received ? (size_t)q : 0);
+  if (!paid.empty()) O.paid = paid.data();
+  if (!recv.empty()) O.received = recv.data();
+  if ((rc = basket_orders(ctx, exec, q, token_out, basket_off, basket_token, nullptr, basket_amount, limit_price,
+                          min_received, allowed, o, O, what)) != CFMM_OK)
+    return rc;
+  // S = received − Σ_k c_k·paid_k in entry order: a multiply, then a subtract (no fma)
+  if (surplus)
+    for (int64_t r = 0; r < q; ++r) {
+      double s = O.received[r];
+      for (int64_t k = basket_off[r]; k < basket_off[r + 1]; ++k) {
+        const volatile double cp = limit_price[k] * O.paid[k];
+        s = s - cp;
+      }
+      out->surplus[r] = s;
+    }
+  return CFMM_OK;
 }
 
 // ---- arbitrage against external prices over every pool among allowed tokens (price_arb_kernels.cuh)
@@ -4614,6 +4692,21 @@ int cfmm_execute_basket_swap_orders(cfmm_ctx* ctx, int64_t q, const int64_t* tok
                                     const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
   return basket_call(ctx, true, q, token_out, basket_off, basket_token, entry_kind, basket_amount, limit, allowed,
                      opts, out, "execute_basket_swap_orders");
+}
+
+int cfmm_quote_limit_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                            const int64_t* basket_token, const double* basket_amount, const double* limit_price,
+                            const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_limit_out* out) {
+  return limit_call(ctx, false, q, token_out, basket_off, basket_token, basket_amount, limit_price, nullptr, allowed,
+                    opts, out, "quote_limit_orders");
+}
+
+int cfmm_execute_limit_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                              const int64_t* basket_token, const double* basket_amount, const double* limit_price,
+                              const double* min_received, const uint8_t* allowed, const cfmm_subgraph_opts* opts,
+                              cfmm_limit_out* out) {
+  return limit_call(ctx, true, q, token_out, basket_off, basket_token, basket_amount, limit_price, min_received,
+                    allowed, opts, out, "execute_limit_orders");
 }
 
 int cfmm_quote_price_arbitrage(cfmm_ctx* ctx, int64_t q, const double* price, const uint8_t* allowed,

@@ -18,10 +18,10 @@
 // time.  subgraph_plan_kernel runs the setup only and reports each row's token and pool counts, which
 // size the outputs and the workspace (they do not depend on the kind).
 //
-// basket_kernels.cuh's and price_arb_kernels.cuh's rows run everything after their own setup through
-// this file's helpers, which take the row's shared state and its rules as template parameters: the
-// pool gather, the pool ordering, the evaluation, the commit, the L-BFGS driver, the legs, and the
-// pair activity, CTA sum, pool view, start and capacity.  The setups stay per kind: running subgraph
+// basket_kernels.cuh's rows (limit rows included) and price_arb_kernels.cuh's rows run everything after
+// their own setup through this file's helpers, which take the row's shared state and its rules as
+// template parameters: the pool gather, the pool ordering, the evaluation, the commit, the L-BFGS
+// driver, the legs, and the pair activity, CTA sum, pool view, start and capacity.  The setups stay per kind: running subgraph
 // rows through the longer basket setup cost 2.3–2.6 % more kernel time on the headline set (DESIGN §4.5).
 #pragma once
 #include <cuda_runtime.h>
@@ -264,7 +264,7 @@ __device__ __forceinline__ double sg_lo(int t) { return OUT ? kSubgraphSqrtEps :
 // row kind (basket_kernels.cuh's BkRule gives the same for basket rows):
 //   lin(m, t)     the linear term of slot t's gradient: lin at kLin (amt at j, or −y′ at i), else 0;
 //   value(m)      the dual's linear value at ν = xt, lin·ν_kLin;
-//   lo(m, t), fixed(m, t)   the box;
+//   lo(m, t), fixed(m, t)   the box (sg_start's clamp included);
 //   kBoxStart     false: the start is sg_start's (true: the box's lower bound, sg_box_start);
 //   kOut, root(m) sg_start's root and clamp (exact-out: slot 1, j, fixed at 1);
 //   evaluated(m, f)   sees the dual value f of every evaluation (nothing here);
@@ -362,14 +362,16 @@ __device__ double sg_commit(Smem& m, int slot, bool store, const Rule& rule) {
   return rule.merit(m, __longlong_as_double((long long)m.mx));
 }
 
-// The start ν⁰: ν_root = 1 (slot 0, i; exact-out: slot 1, j; basket buy rows: i's slot); then
-// breadth-first rounds over the active pools: a token not yet priced gets the largest r(a → b)·ν_b
-// over its pools to tokens priced in earlier rounds, r the no-trade boundary with a in j's role (the
-// arbitrage scan's rate).  A token is priced once, so gaining cycles cannot inflate the start.  Then
-// clamped to the box (OUT: the root fixed at 1, every other slot >= √eps).  Into xt.
-template <class Smem, bool OUT = false>
-__device__ void sg_start(const PathSets* P, const SubgraphWork& w, Smem& m, int root = OUT ? 1 : 0) {
-  const int tid = threadIdx.x, n = m.n_loc;
+// The start ν⁰: ν_root = 1 (the rule's root: slot 0, i; exact-out: slot 1, j; basket buy rows: i's
+// slot); then breadth-first rounds over the active pools: a token not yet priced gets the largest
+// r(a → b)·ν_b over its pools to tokens priced in earlier rounds, r the no-trade boundary with a in j's
+// role (the arbitrage scan's rate).  A token is priced once, so gaining cycles cannot inflate the
+// start.  Then clamped to the rule's box (kOut: the root fixed at 1; every other slot >= lo(m, t)).
+// Into xt.
+template <class Smem, class Rule>
+__device__ void sg_start(const PathSets* P, const SubgraphWork& w, Smem& m, const Rule& rule) {
+  constexpr bool OUT = Rule::kOut;
+  const int tid = threadIdx.x, n = m.n_loc, root = rule.root(m);
   for (int t = tid; t < n; t += blockDim.x) m.x[t] = m.xt[t] = t == root ? 1.0 : 0.0;
   __syncthreads();
   unsigned long long* nxt = reinterpret_cast<unsigned long long*>(m.xt);
@@ -394,7 +396,7 @@ __device__ void sg_start(const PathSets* P, const SubgraphWork& w, Smem& m, int 
     __syncthreads();
     if (!more) break;
   }
-  for (int t = tid; t < n; t += blockDim.x) m.xt[t] = OUT && t == root ? 1.0 : fmax(m.x[t], sg_lo<OUT>(t));
+  for (int t = tid; t < n; t += blockDim.x) m.xt[t] = OUT && t == root ? 1.0 : fmax(m.x[t], rule.lo(m, t));
   __syncthreads();
 }
 
@@ -562,7 +564,7 @@ __device__ __forceinline__ int sg_solve(const PathSets* P, const SubgraphWork& w
   if constexpr (Rule::kBoxStart)
     sg_box_start(m, rule);
   else
-    sg_start<Smem, Rule::kOut>(P, w, m, rule.root(m));
+    sg_start(P, w, m, rule);
   f = sg_evaluate(P, w, m, rule);
   merit = sg_commit(m, 0, false, rule);
   if (tid == 0) {

@@ -812,6 +812,69 @@ quote_price_arbitrage(ctx, price, allowed; opts=nothing) =
 execute_price_arbitrage!(ctx, price, allowed; min_profit=nothing, opts=nothing) =
     _price_arbitrage(ctx, true, price, allowed, min_profit, opts)
 
+# Limit orders with partial fills (cfmm_quote_limit_orders / cfmm_execute_limit_orders): the rows of
+# _basket_orders, with limit_price[k] the least token_out[r] per unit of basket_token[k] at the margin
+# (finite, >= 0); an entry sells up to basket_amount[k] while the pools pay at least that.  min_received
+# (nothing: none) is one minimum received per row.  Returns the NamedTuple of _basket_orders plus surplus
+# (received − Σ limit·paid, per row).  Never executed, like the rest of this file.
+struct LimitOut
+    paid::Ptr{Float64}; received::Ptr{Float64}; status::Ptr{UInt8}
+    solver_status::Ptr{Cint}; iterations::Ptr{Cint}; fun_evals::Ptr{Cint}; merit::Ptr{Float64}
+    tok_off::Ptr{Int64}; tok_cap::Int64; token::Ptr{Int64}; nu::Ptr{Float64}; psi::Ptr{Float64}
+    leg_off::Ptr{Int64}; leg_cap::Int64; leg_type::Ptr{Cint}; leg_pool::Ptr{Int64}
+    leg_delta::Ptr{Float64}; leg_lambda::Ptr{Float64}; surplus::Ptr{Float64}
+end
+function _limit_orders(ctx, execute::Bool, token_out::Vector{Int64}, basket_off::Vector{Int64},
+                       basket_token::Vector{Int64}, basket_amount::Vector{Float64}, limit_price::Vector{Float64},
+                       allowed::Vector{UInt8}, min_received, opts)
+    q = length(token_out)
+    length(basket_off) == q + 1 || throw(ArgumentError("basket_off needs q + 1 entries"))
+    NE = basket_off[end]
+    length(basket_token) == length(basket_amount) == length(limit_price) == NE ||
+        throw(ArgumentError("basket_token / basket_amount / limit_price need basket_off[end] entries"))
+    min_received === nothing || length(min_received) == q || throw(ArgumentError("min_received needs q entries"))
+    o = opts === nothing ? nothing : Ref(opts)
+    argq = (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8},
+            Ptr{SubgraphOpts}, Ptr{LimitOut})
+    tok_off, leg_off = zeros(Int64, q + 1), zeros(Int64, q + 1)
+    sizes = Ref(LimitOut(C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, pointer(tok_off), 0, C_NULL,
+                         C_NULL, C_NULL, pointer(leg_off), 0, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL))
+    GC.@preserve tok_off leg_off chk(ctx, ccall((:cfmm_quote_limit_orders, LIB), Cint, argq, ctx, q, token_out,
+                                               basket_off, basket_token, basket_amount, limit_price, allowed,
+                                               o === nothing ? C_NULL : o, sizes))
+    NT, L = tok_off[end], leg_off[end]
+    paid, received, surplus, merit, status = zeros(max(NE, 1)), zeros(q), zeros(q), zeros(q), zeros(UInt8, q)
+    sst, iters, fev = zeros(Cint, q), zeros(Cint, q), zeros(Cint, q)
+    token, nu, psi = zeros(Int64, max(NT, 1)), zeros(max(NT, 1)), zeros(max(NT, 1))
+    ltype, lpool, ld, ll = zeros(Cint, max(L, 1)), zeros(Int64, max(L, 1)), zeros(2, max(L, 1)), zeros(2, max(L, 1))
+    GC.@preserve paid received surplus merit status sst iters fev tok_off token nu psi leg_off ltype lpool ld ll begin
+        out = Ref(LimitOut(pointer(paid), pointer(received), pointer(status), pointer(sst), pointer(iters),
+                           pointer(fev), pointer(merit), pointer(tok_off), NT, pointer(token), pointer(nu),
+                           pointer(psi), pointer(leg_off), L, pointer(ltype), pointer(lpool), pointer(ld),
+                           pointer(ll), pointer(surplus)))
+        if execute
+            chk(ctx, ccall((:cfmm_execute_limit_orders, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+                 Ptr{UInt8}, Ptr{SubgraphOpts}, Ptr{LimitOut}),
+                ctx, q, token_out, basket_off, basket_token, basket_amount, limit_price,
+                min_received === nothing ? C_NULL : min_received, allowed, o === nothing ? C_NULL : o, out))
+        else
+            chk(ctx, ccall((:cfmm_quote_limit_orders, LIB), Cint, argq, ctx, q, token_out, basket_off, basket_token,
+                           basket_amount, limit_price, allowed, o === nothing ? C_NULL : o, out))
+        end
+    end
+    return (paid=paid[1:NE], received=received, surplus=surplus, status=status, solver_status=sst,
+            iterations=iters, fun_evals=fev, merit=merit, tok_off=tok_off, token=token[1:NT], nu=nu[1:NT],
+            psi=psi[1:NT], leg_off=leg_off, leg_type=ltype[1:L], leg_pool=lpool[1:L], leg_delta=ld[:, 1:L],
+            leg_lambda=ll[:, 1:L])
+end
+quote_limit_orders(ctx, token_out, basket_off, basket_token, basket_amount, limit_price, allowed; opts=nothing) =
+    _limit_orders(ctx, false, token_out, basket_off, basket_token, basket_amount, limit_price, allowed, nothing, opts)
+execute_limit_orders!(ctx, token_out, basket_off, basket_token, basket_amount, limit_price, allowed;
+                      min_received=nothing, opts=nothing) =
+    _limit_orders(ctx, true, token_out, basket_off, basket_token, basket_amount, limit_price, allowed,
+                  min_received, opts)
+
 # UniV3 liquidity changes (cfmm_modify_univ3_liquidity / cfmm_get_univ3_ticks).  pools are 0-based
 # UniV3 insertion indices; range is 2 x q (column j = (lo, hi) of row j).  univ3_ticks returns the
 # current ladders of pools first .. first+count-1 in CSR form.  Like the rest of this file, never

@@ -6,7 +6,7 @@ from __future__ import annotations
 
 import numpy as np
 
-__all__ = ["Objective", "LinearNonnegative", "BasketLiquidation", "BasketSwap", "Swap"]
+__all__ = ["Objective", "LinearNonnegative", "BasketLiquidation", "BasketSwap", "LimitBasket", "Swap"]
 
 
 class Objective:
@@ -150,6 +150,61 @@ class BasketSwap(Objective):
         if self.buys:
             ret[self.i - 1] = 1.0
         return ret
+
+
+class LimitBasket(Objective):
+    """Ψ_i + Σ_k c_k·Ψ_k − I(Ψ_k + Δin_k >= 0 at the entries, Ψ_t >= 0 elsewhere, i included): sell
+    up to Δin_k of each token k for as long as the margin pays at least limit_k of token i per unit
+    (a limit order with partial fills, settled in i).  `i` is 1-based; limit is per token (its i
+    entry and the entries of tokens not sold are ignored).  The conjugate is finite only on ν_i >= 1,
+    ν_k >= limit_k and ν_t >= 0, where it is Σ_{k≠i} Δin_k·(ν_k − limit_k): the box is
+    BasketLiquidation's with each sold token's bound raised to fmax(limit_k, √eps), and
+    f(ν) = linᵀν − Σ Δin·limit, so that f(ν*) plus the pools' value is the optimal surplus
+    Ψ_i + Σ_k limit_k·Ψ_k.  With every limit 0 it is BasketLiquidation(i, Δin)."""
+
+    def __init__(self, i, delta_in, limit):
+        delta_in = np.array(delta_in, dtype=np.float64)
+        limit = np.array(limit, dtype=np.float64)
+        if delta_in.shape != limit.shape or delta_in.ndim != 1:
+            raise ValueError("delta_in and limit need one entry per token")
+        if not (0 < i <= len(delta_in)):
+            raise ValueError("Invalid index i")
+        if not np.all(np.isfinite(limit) & (limit >= 0.0)):
+            raise ValueError("every limit must be finite and >= 0")
+        self.i = int(i)
+        self.delta_in = delta_in
+        self.limit = limit
+        self._basket = BasketLiquidation(i, delta_in)
+
+    def _const(self):
+        """Σ_{k≠i} Δin_k·limit_k, in token order."""
+        s = 0.0
+        for k in range(len(self.delta_in)):
+            if k != self.i - 1:
+                s += self.delta_in[k] * self.limit[k]
+        return s
+
+    def linear_term(self):
+        return self._basket.linear_term()
+
+    def f(self, v):
+        if np.any(np.asarray(v) < self.lower_limit()):
+            return np.inf
+        return float(np.dot(self.linear_term(), v)) - self._const()
+
+    def grad(self, g, v):
+        if np.any(np.asarray(v) < self.lower_limit()):
+            g[:] = np.inf
+        else:
+            g[:] = self.linear_term()
+
+    def lower_limit(self):
+        ret = np.fmax(self.limit, np.sqrt(np.finfo(np.float64).eps))
+        ret[self.i - 1] = 1.0 + np.sqrt(np.finfo(np.float64).eps)
+        return ret
+
+    def upper_limit(self):
+        return self._basket.upper_limit()
 
 
 def Swap(i, j, delta, n):

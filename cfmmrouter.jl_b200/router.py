@@ -893,6 +893,62 @@ class DevicePools:
         below it reverts.  Returns what quote_basket_orders returns."""
         return self._basket(True, token_out, basket_off, basket_token, basket_amount, allowed, limit, opts, kind)
 
+    # -- limit orders over every pool among allowed tokens (include/cfmm_b200.h,
+    #    cfmm_quote_limit_orders / cfmm_execute_limit_orders) ----------------------------------------------
+    def _limit(self, execute, token_out, basket_off, basket_token, basket_amount, limit_price, allowed,
+               min_received, opts):
+        tout = np.ascontiguousarray(token_out, dtype=np.int64).reshape(-1)
+        boff = np.ascontiguousarray(basket_off, dtype=np.int64).reshape(-1)
+        btok = np.ascontiguousarray(basket_token, dtype=np.int64).reshape(-1)
+        bamt = np.ascontiguousarray(basket_amount, dtype=np.float64).reshape(-1)
+        lp = np.ascontiguousarray(limit_price, dtype=np.float64).reshape(-1)
+        q = len(tout)
+        if len(boff) != q + 1:
+            raise ValueError(f"limit orders: basket_off must have {q + 1} entries, one per row plus one")
+        NE = int(boff[-1])
+        if not (len(btok) == len(bamt) == len(lp) == NE):
+            raise ValueError(f"limit orders: basket_token, basket_amount and limit_price need basket_off[-1] = {NE} "
+                             "entries")
+        if not np.all(np.isfinite(lp) & (lp >= 0.0)):
+            raise ValueError("limit orders: a limit price is negative, NaN or Inf")
+        u8m, min_received, po = _row_args(self.n_tokens, q, allowed, min_received, opts, "limit orders")
+        to, bo, bt, ba, lpp = _ip(tout), _ip(boff), _ip(btok), _dp(bamt), _dp(lp)
+        lim = None if min_received is None else _dp(min_received)
+        surplus = np.zeros(q)
+
+        def call(size, out):
+            if size:
+                return self._lib.cfmm_quote_limit_orders(self._ctx, q, to, bo, bt, ba, lpp, u8m, po, C.byref(out))
+            out.surplus = surplus.ctypes.data_as(C.POINTER(C.c_double))
+            if execute:
+                return self._lib.cfmm_execute_limit_orders(self._ctx, q, to, bo, bt, ba, lpp, lim, u8m, po,
+                                                           C.byref(out))
+            return self._lib.cfmm_quote_limit_orders(self._ctx, q, to, bo, bt, ba, lpp, u8m, po, C.byref(out))
+        out = self._order_solve(q, NE, _lib.LimitOut, call)
+        out.surplus = surplus
+        out.basket_off = boff
+        return out
+
+    def quote_limit_orders(self, token_out, basket_off, basket_token, basket_amount, limit_price, allowed,
+                           opts=None):
+        """cfmm_quote_limit_orders: row r sells up to basket_amount[k] of basket_token[k] for k in
+        basket_off[r] .. basket_off[r + 1] - 1 (1 to 16 distinct tokens, 1-based, none token_out[r]) for
+        token_out[r], each for as long as the margin pays at least limit_price[k] of token_out[r] per unit
+        (finite, >= 0), over every pool among them and the tokens t with allowed[t - 1]: a basket row
+        with each entry's dual bound raised to its limit, solved per row on the device; rows fill
+        partially.  opts as quote_subgraph_orders.  No state changes.  Returns quote_basket_orders'
+        namespace, with surplus [q] (received - Σ limit·paid) added."""
+        return self._limit(False, token_out, basket_off, basket_token, basket_amount, limit_price, allowed, None,
+                           opts)
+
+    def execute_limit_orders(self, token_out, basket_off, basket_token, basket_amount, limit_price, allowed,
+                             min_received=None, opts=None):
+        """cfmm_execute_limit_orders: the rows of quote_limit_orders in batch order, each re-solved on the
+        state the earlier filled rows left; min_received[r] (None: none) is the minimum received of
+        token_out[r], and a row below it reverts.  Returns what quote_limit_orders returns."""
+        return self._limit(True, token_out, basket_off, basket_token, basket_amount, limit_price, allowed,
+                           min_received, opts)
+
     # -- arbitrage against external prices over every pool among allowed tokens (include/cfmm_b200.h,
     #    cfmm_quote_price_arbitrage / cfmm_execute_price_arbitrage) --------------------------------------
     def _price_arb(self, execute, price, allowed, min_profit, opts):
@@ -1666,6 +1722,52 @@ class Router:
         out = self._pools.execute_basket_orders(tout, off, toks, amts, allowed, limits, opts)
         self._refresh_filled(out)
         return self._per_entry(out), out.received, out.status, out
+
+    def _limit_args(self, token_out, sells, allowed, min_received, what):
+        """_basket_args over sells[r]: {token: (amount, limit)} or (tokens, amounts, limits), plus the
+        limit prices."""
+        rows, lims = [], []
+        for s in sells:
+            if isinstance(s, dict):
+                t = list(s.keys())
+                pairs = [tuple(v) for v in s.values()]
+                if any(len(v) != 2 for v in pairs):
+                    raise ValueError(f"{what}: a sell needs (amount, limit) per token")
+                a, c = [v[0] for v in pairs], [v[1] for v in pairs]
+            else:
+                if len(s) != 3:
+                    raise ValueError(f"{what}: a sell is {{token: (amount, limit)}} or (tokens, amounts, limits)")
+                t, a, c = list(s[0]), list(s[1]), list(s[2])
+                if len(c) != len(t):
+                    raise ValueError(f"{what}: a sell needs one limit per token")
+            rows.append((t, a))
+            lims += c
+        tout, off, toks, amts, min_received = self._basket_args(token_out, rows, allowed, min_received, what)
+        return tout, off, toks, amts, np.array(lims, np.float64).reshape(-1), min_received
+
+    def quote_limit_orders(self, token_out, sells, allowed, opts=None):
+        """Limit orders settled in token_out[r]: sells[r] is {token: (amount, limit)} or (tokens, amounts,
+        limits) (1 to 16 distinct 1-based tokens, none of them token_out[r]).  Each entry sells up to its
+        amount for as long as the margin pays at least `limit` of token_out[r] per unit, over every pool
+        among the row's tokens and the tokens t with allowed[t - 1], one dual solve per row on the device
+        (cfmm_quote_limit_orders); rows fill partially.  To buy with a budget, settle in the bought token
+        and sell the budget token at limit 1 / (the highest price per unit bought).  No state changes.
+        Returns (sold per entry as a list of arrays in the caller's order, received [q], surplus [q],
+        status [q], detail); detail is DevicePools.quote_limit_orders' namespace.  Single GPU."""
+        tout, off, toks, amts, lims, _ = self._limit_args(token_out, sells, allowed, None, "quote_limit_orders")
+        out = self._pools.quote_limit_orders(tout, off, toks, amts, lims, allowed, opts)
+        return self._per_entry(out), out.received, out.surplus, out.status, out
+
+    def execute_limit_orders(self, token_out, sells, allowed, min_received=None, opts=None):
+        """Execute limit orders in order (cfmm_execute_limit_orders), each re-solved on the state the
+        earlier filled rows left, with an optional minimum received per row: a row below it reverts.
+        Returns what quote_limit_orders returns and refreshes the pool objects the filled rows traded
+        with from the device state.  Single GPU."""
+        tout, off, toks, amts, lims, min_received = self._limit_args(token_out, sells, allowed, min_received,
+                                                                     "execute_limit_orders")
+        out = self._pools.execute_limit_orders(tout, off, toks, amts, lims, allowed, min_received, opts)
+        self._refresh_filled(out)
+        return self._per_entry(out), out.received, out.surplus, out.status, out
 
     def _price_arb_args(self, prices, allowed, what):
         if self._world > 1:

@@ -1042,6 +1042,94 @@ int cfmm_execute_basket_swap_orders(cfmm_ctx *ctx, int64_t q, const int64_t *tok
                                     const uint8_t *allowed, const cfmm_subgraph_opts *opts,
                                     cfmm_basket_out *out);
 
+/* ---- limit orders: sell up to an amount at no worse than a limit price, filled partially -----
+ * cfmm_quote_limit_orders / cfmm_execute_limit_orders take the basket calls' arguments plus
+ * limit_price [basket_off[q]].  Row r settles in i = token_out[r]; entry k sells up to
+ * δ_k = basket_amount[k] of b_k (finite, >= 0) for as long as the margin pays at least
+ * c_k = limit_price[k] of i per unit of b_k (finite, >= 0).  B, T, pools, legs, sums, optimizer,
+ * options and CTA reduction are those of basket rows (one allowed mask per call), with:
+ *   reach    an entry outside T with c_k > 0 cannot fill at any price: it is dropped and paid 0.  An
+ *            entry outside T with c_k = 0 follows the basket rule: δ_k > 0 makes the row
+ *            CFMM_ORDER_UNREACHABLE.  A row whose remaining amounts are all 0 fills with zeros and
+ *            runs no solve.
+ *   tokens   local order: i, then the entries in T in the caller's order, then B ∩ T ascending.
+ * Buying with a budget is the same row with the roles swapped: settle in the bought token, sell the
+ * budget token, and set c = 1 / (the highest price paid per unit bought).  Buys capped at a bought
+ * quantity are not offered (their conjugate is piecewise linear in ν).
+ * Problem.  The primal is: maximise S = Ψ_i + Σ_k c_k·Ψ_k subject to Ψ_k >= −δ_k at the entries and
+ * Ψ_t >= 0 for every other t in T (i included).  Its conjugate is finite only on ν_i >= 1, ν_k >= c_k,
+ * ν_t >= 0, where it is Σ_k δ_k·(ν_k − c_k), so the dual is
+ *   g(ν) = Σ_k δ_k·ν_k − Σ_k δ_k·c_k + Σ_p π_p(ν),
+ * the basket row's dual with each entry's lower bound raised to its limit, plus a constant.  The device
+ * minimises it without the constant on the box
+ *   ν_i >= 1 + √eps (Swap's), ν_k >= lo_k = fmax(c_k, √eps) (one IEEE operation: a zero limit gives the
+ *   basket bound bit for bit), ν_t >= √eps for every other token,
+ * with lin = δ_k at the entries.  The value, V = Σ_k δ_k·ν_k and m_r = max_t ν_t·|pg_t| / V are the
+ * basket row's, in the same operation order; status 0 when m_r <= rtol.
+ *   start    the basket row's breadth-first pricing from i, clamped to this box.
+ * Complementary slackness gives the limit-order reading: an entry whose ν_k is above its bound sells
+ * in full (Ψ_k = −δ_k up to the stop); an entry that sells partially has ν_k on c_k, so its last unit
+ * sold at the limit rate (within the box's √eps).  With every c_k = 0 a row is a basket row: the same
+ * outputs bit for bit.
+ * What a fill promises.  A row fills only at solver status 0 (else CFMM_ORDER_NOT_CONVERGED, trading
+ * nothing).  A filled row has received = Ψ_i and paid_k = −Ψ_{b_k} with:
+ *   each paid_k <= δ_k + rtol·V/ν_k (Ψ_k + δ_k is the gradient, within rtol·V/ν_k of 0 off the
+ *   bound and at least −rtol·V/ν_k on it); an entry with ν_k off its bound sells in full, within
+ *   rtol·V/ν_k of δ_k.  paid_k < 0 (the row receives b_k) happens only with ν_k on its bound: the
+ *   primal values b_k at c_k, so when the pools deliver b_k for less than that (through the row's other
+ *   entries, or a cycle), receiving it raises S.  A single entry over pools with no cycle never does;
+ *   every intermediate's net Ψ_b >= −rtol·V/ν_b;
+ *   the surplus S = received − Σ_k c_k·paid_k >= −(|T|·rtol·V + Σ_{t on its bound}
+ *   (lo_t − c_t)·max(Ψ_t + δ_t, 0)), with c_i = 1, and c_t = 0, δ_t = 0 off the entries.
+ * The bound on S: let a_t = Ψ_t + δ_t (δ_t = 0 off the entries), so S = Σ_t c_t·a_t − Σ_k c_k·δ_k.
+ * With pg_t = a_t off the bound, ν_t·|a_t| <= rtol·V; so g(ν) − (S + Σ c_k·δ_k) = Σ_t (ν_t − c_t)·a_t
+ * and each free token adds at most (ν_t − c_t)·|a_t| <= rtol·V, each token on its bound at most
+ * (lo_t − c_t)·max(a_t, 0).  Trading nothing is feasible with S = 0, so the dual optimum (g minus the
+ * constant) is >= 0, and S >= 0 − |T|·rtol·V − the box terms.  A filled row never pays more than its
+ * limits by more than that certified gap (up to the rounding of fp64 sums).  The accuracy is relative
+ * to the order's value V, not to the amount filled: a tiny partial fill is accurate only to rtol·V.
+ * Outputs (cfmm_limit_out; every pointer may be NULL): those of cfmm_basket_out, plus surplus [q],
+ * computed on the host in entry order from the first term received, each term a multiply c_k·paid_k
+ * then a subtract (no fma).  A row that does not fill reads 0.  Ask a quote with
+ * tok_cap = leg_cap = 0 for the sizes first.
+ * cfmm_quote_limit_orders prices every row on the current state on its own; no state changes.
+ * cfmm_execute_limit_orders runs the rows in batch order, each re-solved on the state the earlier
+ * filled rows left; min_received (NULL: none; finite and >= 0) is the minimum received of i: an equal
+ * value fills, a smaller one reverts with CFMM_ORDER_LIMIT.  The transition, bookkeeping, conflict
+ * rule ({i} ∪ entries ∪ B) and levels are those of basket rows.
+ * Single GPU.  Synchronous.  Before cfmm_finalize: CFMM_ERR_STATE.  q == 0 does nothing.
+ * Errors: CFMM_ERR_INVALID before anything runs for the basket calls' argument errors, a null
+ * limit_price, and a limit price that is NaN, Inf or negative. */
+typedef struct {
+  double *paid;                                  /* [basket_off[q]] */
+  double *received;                              /* [q] */
+  uint8_t *status;                               /* [q] */
+  int *solver_status, *iterations, *fun_evals;   /* [q] */
+  double *merit;                                 /* [q] */
+  int64_t *tok_off;                              /* [q+1] */
+  int64_t tok_cap;
+  int64_t *token;                                /* [tok_off[q]] */
+  double *nu, *psi;                              /* [tok_off[q]] */
+  int64_t *leg_off;                              /* [q+1] */
+  int64_t leg_cap;
+  int *leg_type;                                 /* [leg_off[q]] */
+  int64_t *leg_pool;                             /* [leg_off[q]] */
+  double *leg_delta, *leg_lambda;                /* [2·leg_off[q]] */
+  double *surplus;                               /* [q] */
+} cfmm_limit_out;
+int cfmm_quote_limit_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_out /* [q] */,
+                            const int64_t *basket_off /* [q+1] */,
+                            const int64_t *basket_token /* [basket_off[q]] */,
+                            const double *basket_amount /* [basket_off[q]] */,
+                            const double *limit_price /* [basket_off[q]] */,
+                            const uint8_t *allowed /* [n_tokens], required */,
+                            const cfmm_subgraph_opts *opts /* NULL = defaults */, cfmm_limit_out *out);
+int cfmm_execute_limit_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_out,
+                              const int64_t *basket_off, const int64_t *basket_token,
+                              const double *basket_amount, const double *limit_price,
+                              const double *min_received /* [q] or NULL */, const uint8_t *allowed,
+                              const cfmm_subgraph_opts *opts, cfmm_limit_out *out);
+
 /* ---- arbitrage against external prices over every pool among allowed tokens ----------------
  * A row values tokens at external prices c and trades through every pool among its priced tokens to
  * maximise cᵀΨ with no token's net flow negative: route! with LinearNonnegative(c)
