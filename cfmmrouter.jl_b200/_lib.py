@@ -170,6 +170,18 @@ SYMBOLS = {
                                           C.POINTER(SubgraphOpts), C.POINTER(LimitOut)]),
     "cfmm_execute_limit_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, _dp, _dp, _dp, C.POINTER(C.c_uint8),
                                             C.POINTER(SubgraphOpts), C.POINTER(LimitOut)]),
+    "cfmm_quote_subgraph_swap_orders_rows": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, _ip, _ip,
+                                                       C.POINTER(SubgraphOpts), C.POINTER(SubgraphOut)]),
+    "cfmm_execute_subgraph_swap_orders_rows": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, _dp,
+                                                         _ip, _ip, C.POINTER(SubgraphOpts), C.POINTER(SubgraphOut)]),
+    "cfmm_quote_basket_swap_orders_rows": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, C.POINTER(C.c_uint8), _dp, _ip,
+                                                     _ip, C.POINTER(SubgraphOpts), C.POINTER(BasketOut)]),
+    "cfmm_execute_basket_swap_orders_rows": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, C.POINTER(C.c_uint8), _dp,
+                                                       _dp, _ip, _ip, C.POINTER(SubgraphOpts), C.POINTER(BasketOut)]),
+    "cfmm_quote_limit_orders_rows": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, _dp, _dp, _ip, _ip,
+                                               C.POINTER(SubgraphOpts), C.POINTER(LimitOut)]),
+    "cfmm_execute_limit_orders_rows": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _ip, _dp, _dp, _dp, _ip, _ip,
+                                                 C.POINTER(SubgraphOpts), C.POINTER(LimitOut)]),
     "cfmm_quote_price_arbitrage": (C.c_int, [_ctx, C.c_int64, _dp, C.POINTER(C.c_uint8), C.POINTER(SubgraphOpts),
                                              C.POINTER(PriceArbOut)]),
     "cfmm_execute_price_arbitrage": (C.c_int, [_ctx, C.c_int64, _dp, _dp, C.POINTER(C.c_uint8),

@@ -149,8 +149,8 @@ extern __shared__ __align__(8) unsigned char bk_dyn[];
 // count of every slot (cnt[s], the pools of the pairs {s, i}, {s, b_k} for b_k ∈ T, and {s, u} for
 // slots u > s in T) and of the pairs among i and the basket tokens in T (basket_cnt).  BUY: the local
 // order puts the bought entries (m.bkind) before i; the counts are the same.
-template <bool BUY>
-__device__ void bk_setup(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
+template <bool BUY, class Graph>  // BestPathGraph or RowGraph
+__device__ void bk_setup(const PathSets* P, PairIndexView ix, AdjView A, const Graph& G,
                          const uint8_t* __restrict__ gact, const int64_t* __restrict__ btok, int K, int32_t i,
                          BkSmem<BUY>& m) {
   const int tid = threadIdx.x, nB = G.nB;
@@ -294,8 +294,8 @@ __device__ void bk_setup(const PathSets* P, PairIndexView ix, AdjView A, const B
   __syncthreads();
 }
 
-template <bool BUY>
-__device__ __forceinline__ int32_t bk_local(const BestPathGraph& G, const BkSmem<BUY>& m, int32_t t) {
+template <bool BUY, class Graph>
+__device__ __forceinline__ int32_t bk_local(const Graph& G, const BkSmem<BUY>& m, int32_t t) {
   if constexpr (BUY) {
     for (int k = 0; k <= m.nin; ++k)  // i and the entries in T
       if (t == m.ltok[k]) return k;
@@ -389,8 +389,8 @@ using BkRows = std::conditional_t<LIM, LimitRows, BasketRows>;
 // pay out makes the row unreachable, and a row fills only when every bought entry with y_l > 0
 // receives at least y_l.  LIM: a limit row (R.limit_price): the box of entry k in T is
 // ν_k >= fmax(c_k, √eps), and an entry outside T with c_k > 0 is dropped (paid 0).
-template <bool EXEC, bool BUY = false, bool LIM = false>
-__device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
+template <bool EXEC, bool BUY = false, bool LIM = false, class Graph>
+__device__ void basket_row(const PathSets* P, PairIndexView ix, AdjView A, const Graph& G,
                              const uint8_t* gact, const BkRows<LIM>& R, const SubgraphWork& w, const SplitMoved& mv,
                              int64_t r, BkRowSmem<BUY, LIM>& m) {
   __shared__ SgSolveState s;
@@ -570,6 +570,47 @@ __global__ void __launch_bounds__(kSubgraphThreads)
   const SubgraphWork wb = sg_cta_work(w);
   for (int64_t k = blockIdx.x; k < n; k += gridDim.x)
     basket_row<EXEC, false, true>(P, ix, A, G, gact, R, wb, mv, rows ? rows[k] : k, m);
+}
+
+// Per-row masks: basket_plan_kernel with each row's own slot graph.
+__global__ void __launch_bounds__(kSubgraphThreads)
+    basket_rows_plan_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, RowMasks M,
+                            const int64_t* __restrict__ basket_off, const int64_t* __restrict__ basket_token,
+                            const int64_t* __restrict__ token_out, int64_t q, int64_t* __restrict__ ntok,
+                            int64_t* __restrict__ npool) {
+  __shared__ BasketSmem m;
+  for (int64_t r = blockIdx.x; r < q; r += gridDim.x) {
+    const int64_t b0 = basket_off[r];
+    const RowGraph G = row_graph(P, ix, A, M, r);
+    bk_setup<false>(P, ix, A, G, rg_act(M), basket_token + b0, (int)(basket_off[r + 1] - b0),
+                    (int32_t)(token_out[r] - 1), m);
+    if (threadIdx.x == 0) {
+      ntok[r] = m.n_loc;
+      npool[r] = m.npool;
+    }
+    __syncthreads();
+  }
+}
+
+// Per-row masks: sell-only (BUY and LIM false), buy (BUY; kind as basket_buy_kernel's) or limit (LIM)
+// rows rows[0 .. n) (null: 0 .. n), as basket_kernel / basket_buy_kernel / basket_limit_kernel, each
+// over its own slot graph.
+template <bool EXEC, bool BUY, bool LIM>
+__global__ void __launch_bounds__(kSubgraphThreads)
+    basket_rows_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, RowMasks M, BkRows<LIM> R,
+                       const uint8_t* __restrict__ kind, SubgraphWork w, SplitMoved mv,
+                       const int64_t* __restrict__ rows, int64_t n) {
+  __shared__ BkRowSmem<BUY, LIM> m;
+  const SubgraphWork wb = sg_cta_work(w);
+  for (int64_t k = blockIdx.x; k < n; k += gridDim.x) {
+    const int64_t r = rows ? rows[k] : k;
+    if constexpr (BUY) {
+      const int64_t b0 = R.basket_off[r];
+      if (threadIdx.x < R.basket_off[r + 1] - b0) m.bkind[threadIdx.x] = kind[b0 + threadIdx.x];
+    }
+    const RowGraph G = row_graph(P, ix, A, M, r);
+    basket_row<EXEC, BUY, LIM>(P, ix, A, G, rg_act(M), R, wb, mv, r, m);
+  }
 }
 
 }  // namespace cfmm

@@ -51,8 +51,9 @@ __device__ __forceinline__ int32_t adj_pair(AdjView A, int32_t a, int32_t b) {
 }
 
 // The pair {t, tok[s]} into dst[s] for every slot s that has one, from t's adjacency list: walked when
-// it is short, else bisected per slot.
-__device__ __forceinline__ void side_pairs(AdjView A, const BestPathGraph& G, int32_t t, int32_t* dst) {
+// it is short, else bisected per slot.  (Graph: BestPathGraph, or subgraph_kernels.cuh's RowGraph.)
+template <class Graph>
+__device__ __forceinline__ void side_pairs(AdjView A, const Graph& G, int32_t t, int32_t* dst) {
   const int64_t a0 = A.off[t], a1 = A.off[t + 1];
   if (a1 - a0 <= (int64_t)G.nB) {
     for (int64_t e = a0 + threadIdx.x; e < a1; e += blockDim.x) {

@@ -3965,12 +3965,54 @@ int cfmm_find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, con
 // ---- orders routed over every pool among their allowed tokens (subgraph_kernels.cuh) ------------
 namespace {
 
-// The context, the row count, the mask and the options of a basket or subgraph call.
-int check_row_opts(cfmm_ctx* ctx, int64_t q, const uint8_t* allowed, const cfmm_subgraph_opts& o, const char* what) {
+// The allowed tokens of a subgraph, basket or limit call: one mask over the tokens (mask), or a per-row
+// CSR (off [q+1], tok 1-based; the _rows calls).  n_mask: the mask's count, set by the checks.
+struct Allowed {
+  const uint8_t* mask;
+  bool per_row = false;
+  const int64_t* off = nullptr;
+  const int64_t* tok = nullptr;
+  int64_t n_mask = 0;
+  bool rows() const { return per_row; }
+  int64_t count(int64_t r) const { return off ? off[r + 1] - off[r] : n_mask; }
+  // whether row r allows token t (1-based)
+  bool has(int64_t r, int64_t t) const {
+    if (!off) return mask[t - 1] != 0;
+    return std::find(tok + off[r], tok + off[r + 1], t) != tok + off[r + 1];
+  }
+};
+
+// The context, the row count, the allowed tokens and the options of a basket or subgraph call.  A
+// per-row CSR: allow_off non-null, from 0 and not decreasing, allow_token non-null when it lists any
+// token, every token in 1..n_tokens and none twice in one row.
+int check_row_opts(cfmm_ctx* ctx, int64_t q, Allowed& M, const cfmm_subgraph_opts& o, const char* what) {
   int rc = ready(ctx);
   if (rc != CFMM_OK) return rc;
   if (q < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: negative row count", what);
-  if (!allowed) return fail(ctx, CFMM_ERR_INVALID, "%s: null allowed (the intermediate tokens are required)", what);
+  if (!M.rows() && !M.mask)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: null allowed (the intermediate tokens are required)", what);
+  if (M.rows()) {
+    if (!M.off) return fail(ctx, CFMM_ERR_INVALID, "%s: null allow_off", what);
+    if (M.off[0] != 0) return fail(ctx, CFMM_ERR_INVALID, "%s: allow_off[0] is %lld, not 0", what, (long long)M.off[0]);
+    for (int64_t r = 0; r < q; ++r)
+      if (M.off[r + 1] < M.off[r]) return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: allow_off decreases", what, (long long)r);
+    if (M.off[q] > 0 && !M.tok) return fail(ctx, CFMM_ERR_INVALID, "%s: null allow_token", what);
+    std::vector<int64_t> seen((size_t)ctx->n_tokens, -1);  // the last row that listed each token
+    for (int64_t r = 0; r < q; ++r) {
+      for (int64_t k = M.off[r]; k < M.off[r + 1]; ++k) {
+        const int64_t t = M.tok[k];
+        if (t < 1 || t > ctx->n_tokens)
+          return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: allowed token %lld outside 1..%lld", what, (long long)r,
+                      (long long)t, (long long)ctx->n_tokens);
+        if (seen[(size_t)(t - 1)] == r)
+          return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: allowed token %lld listed twice", what, (long long)r,
+                      (long long)t);
+        seen[(size_t)(t - 1)] = r;
+      }
+    }
+  } else {
+    M.n_mask = count_allowed(ctx, M.mask);
+  }
   if (o.max_iter < 1 || o.max_fun < 1)
     return fail(ctx, CFMM_ERR_INVALID, "%s: max_iter %d and max_fun %d must be >= 1", what, o.max_iter, o.max_fun);
   if (!(std::isfinite(o.rtol) && o.rtol > 0.0)) return fail(ctx, CFMM_ERR_INVALID, "%s: rtol %g must be finite and > 0", what, o.rtol);
@@ -3988,9 +4030,9 @@ int check_limit(cfmm_ctx* ctx, const double* limit, int64_t r, const char* what)
 // Every argument of cfmm_quote_subgraph_swap_orders / cfmm_execute_subgraph_swap_orders, before
 // anything runs.  kind null: every row exact-in.
 int check_subgraph(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const uint8_t* kind,
-                   const double* amount, const double* limit, const uint8_t* allowed, const cfmm_subgraph_opts& o,
+                   const double* amount, const double* limit, Allowed& M, const cfmm_subgraph_opts& o,
                    const char* what) {
-  int rc = check_row_opts(ctx, q, allowed, o, what);
+  int rc = check_row_opts(ctx, q, M, o, what);
   if (rc != CFMM_OK || q == 0) return rc;
   if (!token_in || !token_out || !amount) return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
   if ((rc = check_pair_tokens(ctx, q, token_in, token_out, what)) != CFMM_OK) return rc;
@@ -4009,9 +4051,8 @@ int check_subgraph(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int6
       return rc;
     }
   }
-  const int64_t n_allowed = count_allowed(ctx, allowed);
   for (int64_t r = 0; r < q; ++r) {
-    const int64_t nb = n_allowed - (allowed[token_in[r] - 1] != 0) - (allowed[token_out[r] - 1] != 0);
+    const int64_t nb = M.count(r) - M.has(r, token_in[r]) - M.has(r, token_out[r]);
     if (nb > CFMM_SUBGRAPH_MAX_TOKENS)
       return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: %lld intermediate tokens, more than %d", what, (long long)r,
                   (long long)nb, CFMM_SUBGRAPH_MAX_TOKENS);
@@ -4029,13 +4070,12 @@ bool basket_buy_row(const int64_t* basket_off, const uint8_t* kind, int64_t r) {
 // before anything runs.
 int check_basket(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
                  const int64_t* basket_token, const uint8_t* kind, const double* basket_amount, const double* limit,
-                 const uint8_t* allowed, const cfmm_subgraph_opts& o, const char* what) {
-  int rc = check_row_opts(ctx, q, allowed, o, what);
+                 Allowed& M, const cfmm_subgraph_opts& o, const char* what) {
+  int rc = check_row_opts(ctx, q, M, o, what);
   if (rc != CFMM_OK || q == 0) return rc;
   if (!token_out || !basket_off || !basket_token || !basket_amount)
     return fail(ctx, CFMM_ERR_INVALID, "%s: null array argument", what);
   if (basket_off[0] != 0) return fail(ctx, CFMM_ERR_INVALID, "%s: basket_off[0] is %lld, not 0", what, (long long)basket_off[0]);
-  const int64_t n_allowed = count_allowed(ctx, allowed);
   for (int64_t r = 0; r < q; ++r) {
     const int64_t b0 = basket_off[r], K = basket_off[r + 1] - b0, i = token_out[r];
     if (K < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: basket_off decreases", what, (long long)r);
@@ -4045,7 +4085,7 @@ int check_basket(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64
     if (i < 1 || i > ctx->n_tokens)
       return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: token_out %lld outside 1..%lld", what, (long long)r,
                   (long long)i, (long long)ctx->n_tokens);
-    int64_t n_other = n_allowed - (allowed[i - 1] != 0);  // the row's tokens other than i
+    int64_t n_other = M.count(r) - M.has(r, i);  // the row's tokens other than i
     for (int64_t k = b0; k < b0 + K; ++k) {
       const int64_t t = basket_token[k];
       const double a = basket_amount[k];
@@ -4062,7 +4102,7 @@ int check_basket(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64
       if (kind && kind[k] > CFMM_SWAP_EXACT_OUT)
         return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: entry kind %d is neither 0 (sold) nor 1 (bought)", what,
                     (long long)r, (int)kind[k]);
-      n_other += allowed[t - 1] == 0;
+      n_other += !M.has(r, t);
     }
     if (n_other > CFMM_SUBGRAPH_MAX_TOKENS + 1)
       return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: %lld tokens besides token_out, more than %d", what,
@@ -4079,14 +4119,15 @@ int check_basket(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64
 }
 
 // The occupancy of a row kernel, cached per context.  A family with dynamic shared memory (basket rows,
-// dyn: its kernels) may take that of the longest basket over the most slots, beyond the 48 KB default:
+// dyn: its kernels) may take most_dyn (that of the longest basket over the most slots; per-row masks add
+// the row graph's kRowGraphBytes), beyond the 48 KB default:
 // the attribute of each of its kernels is set once per context to that one value (so concurrent calls
 // never lower it), and the occupancy taken there.
 int row_occupancy(cfmm_ctx* ctx, const void* kernel, std::initializer_list<const void*> dyn, const char* name,
-                  int& occ) {
+                  int& occ, size_t most_dyn = cfmm::bk_dyn_bytes(cfmm::kBasketMaxTokens, cfmm::kSubgraphSlots)) {
   int& c = ctx->occupancy[kernel];
   if (c == 0) {
-    const int most = dyn.size() ? (int)cfmm::bk_dyn_bytes(cfmm::kBasketMaxTokens, cfmm::kSubgraphSlots) : 0;
+    const int most = dyn.size() ? (int)most_dyn : 0;
     for (const void* f : dyn) CU_TRY(ctx, cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
     CU_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, kernel, cfmm::kSubgraphThreads, (size_t)most));
     if (c < 1) return fail(ctx, CFMM_ERR_CUDA, "%s does not fit on an SM", name);
@@ -4109,26 +4150,35 @@ const void* kernel_ptr(K* k) {
 //   plan(...)     the plan launch; rows(exec_tag, second, ...) a launch of one row kernel;
 //   visit(r, v)   the tokens row r visits besides the slots (a token visited twice changes nothing),
 //                 and uses their count over the call, for the conflict levels of an execute;
-//   all_slots     every row also visits every slot (subgraph and basket rows: B is the whole mask).
-// The driver builds the call's slots and their B-graph, runs the plan, sizes the outputs and the per-CTA
+//   all_slots     every row also visits every slot (subgraph and basket rows: B is the whole mask, or
+//                 with per-row masks the row's own list).
+// The driver builds the call's slots and their B-graph (per-row masks: uploads the lists and sizes the
+// per-CTA row graphs, which each row's CTA builds), runs the plan, sizes the outputs and the per-CTA
 // workspace, runs the rows (a level's rows, or a quote's, split between the two kernels), and reads back.
+// plan and rows get both the call's graph and the per-row masks (RM.off null with one mask).
 extern "C++" template <class Rows, class Out, class Plan, class RowLaunch, class Second, class Visit>
-int row_orders(cfmm_ctx* ctx, bool exec, int64_t q, const uint8_t* allowed, Rows R, const Out& O, int occ, int occ2,
+int row_orders(cfmm_ctx* ctx, bool exec, int64_t q, const Allowed& M, Rows R, const Out& O, int occ, int occ2,
                int64_t n2, int K, int64_t n_paid, int64_t uses, bool all_slots, const char* what, Plan plan,
                RowLaunch rows,
                Second second, Visit visit) {
   int rc;
   auto& ix = ctx->pairs;
   cudaStream_t st = ctx->stream;
-  // the call's slots: the allowed tokens, ascending; their filtered adjacency and its activity
-  std::vector<int32_t> tok, slot_of((size_t)ctx->n_tokens, -1);
-  for (int64_t t = 0; t < ctx->n_tokens; ++t)
-    if (allowed[t]) {
+  // the call's slots: the allowed tokens, ascending; their filtered adjacency and its activity (none
+  // with per-row masks)
+  std::vector<int32_t> tok, slot_of(M.rows() ? 0 : (size_t)ctx->n_tokens, -1);
+  for (int64_t t = 0; !M.rows() && t < ctx->n_tokens; ++t)
+    if (M.mask[t]) {
       slot_of[(size_t)t] = (int32_t)tok.size();
       tok.push_back((int32_t)t);
     }
   const int nB = (int)tok.size();
-  const size_t nn = (size_t)nB * (size_t)nB, dyn = K > 0 ? cfmm::bk_dyn_bytes(K, nB) : 0;
+  // per-row masks: the longest list sizes each CTA's row graph; its tokens and degrees go after the
+  // basket rows' dynamic shared memory
+  int64_t bmax = 0;
+  for (int64_t r = 0; M.rows() && r < q; ++r) bmax = std::max(bmax, M.count(r));
+  const size_t nn = (size_t)nB * (size_t)nB, goff = K > 0 ? cfmm::bk_dyn_bytes(K, M.rows() ? (int)bmax : nB) : 0,
+               dyn = goff + (M.rows() ? (size_t)cfmm::kRowGraphBytes : 0);
   DevBuf<int64_t> d_ntok, d_npool;
   DevBuf<int32_t> d_tok, d_slot, d_deg, d_gpair;
   DevBuf<int16_t> d_gnbr;
@@ -4149,13 +4199,28 @@ int row_orders(cfmm_ctx* ctx, bool exec, int64_t q, const uint8_t* allowed, Rows
   // a persistent grid: one wave of resident CTAs of each kernel that runs
   const int64_t wave = (int64_t)ctx->sm_count * occ, wave2 = (int64_t)ctx->sm_count * occ2;
   const unsigned plan_grid = (unsigned)std::min<int64_t>(q, wave);
+  const int64_t grid = std::min<int64_t>(q, std::max(wave, wave2));  // the workspaces
+  DevBuf<int64_t> d_aoff, d_atok;
+  DevBuf<int16_t> d_rnbr;
+  DevBuf<int32_t> d_rpair;
+  DevBuf<uint8_t> d_ract;
+  cfmm::RowMasks RM{};
+  if (M.rows()) {
+    const size_t cells = (size_t)(bmax * bmax) * (size_t)grid;
+    CU_TRY(ctx, d_aoff.upload(M.off, (size_t)q + 1));
+    CU_TRY(ctx, d_atok.upload(M.tok, (size_t)M.off[q]));
+    CU_TRY(ctx, d_rnbr.alloc(cells));
+    CU_TRY(ctx, d_rpair.alloc(cells));
+    CU_TRY(ctx, d_ract.alloc(cells));
+    RM = cfmm::RowMasks{d_aoff.p, d_atok.p, d_rnbr.p, d_rpair.p, d_ract.p, bmax * bmax, (int)goff};
+  }
   if ((rc = launch(ctx, kProfSwaps, nB > 0 ? 3 : 1, [&] {
          if (nB > 0) {
            cfmm::best_path_graph_kernel<<<(unsigned)((32 * (int64_t)nB + 255) / 256), 256, 0, st>>>(
                A, d_tok.p, d_slot.p, nB, d_deg.p, d_gnbr.p, d_gpair.p);
            cfmm::subgraph_act_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>(os.d_P.p, pv, G, d_act.p);
          }
-         plan(plan_grid, dyn, st, os.d_P.p, pv, A, G, d_act.p, d_ntok.p, d_npool.p);
+         plan(plan_grid, dyn, st, os.d_P.p, pv, A, G, d_act.p, RM, d_ntok.p, d_npool.p);
        })) != CFMM_OK)
     return rc;
   std::vector<int64_t> ntok((size_t)q), npool((size_t)q);
@@ -4208,7 +4273,6 @@ int row_orders(cfmm_ctx* ctx, bool exec, int64_t q, const uint8_t* allowed, Rows
   }
   int64_t cap = 1;
   while (cap < max_pool) cap <<= 1;
-  const int64_t grid = std::min<int64_t>(q, std::max(wave, wave2));  // the workspaces
   DevBuf<int64_t> w64;
   DevBuf<int32_t> w32;
   DevBuf<double> wd;
@@ -4237,10 +4301,11 @@ int row_orders(cfmm_ctx* ctx, bool exec, int64_t q, const uint8_t* allowed, Rows
   const auto run = [&](auto exec_tag, const cfmm::PathSets* P, const cfmm::SplitMoved& mv, const int64_t* rows_,
                        int64_t n1, int64_t n) {
     return launch(ctx, kProfSwaps, (n1 > 0) + (n > n1), [&] {
-      if (n1 > 0) rows(exec_tag, false, (unsigned)std::min(n1, wave), dyn, st, P, pv, A, G, d_act.p, R, W, mv, rows_, n1);
+      if (n1 > 0)
+        rows(exec_tag, false, (unsigned)std::min(n1, wave), dyn, st, P, pv, A, G, d_act.p, RM, R, W, mv, rows_, n1);
       if (n > n1)
-        rows(exec_tag, true, (unsigned)std::min(n - n1, wave2), dyn, st, P, pv, A, G, d_act.p, R, W, mv, rows_ + n1,
-             n - n1);
+        rows(exec_tag, true, (unsigned)std::min(n - n1, wave2), dyn, st, P, pv, A, G, d_act.p, RM, R, W, mv,
+             rows_ + n1, n - n1);
     });
   };
   const auto first = [&](int64_t r) { return !second(r); };
@@ -4257,14 +4322,17 @@ int row_orders(cfmm_ctx* ctx, bool exec, int64_t q, const uint8_t* allowed, Rows
   } else {
     if ((rc = order_sets(ctx, true, xs)) != CFMM_OK) return rc;
     ctx->state_version++;
-    // levels over the tokens the rows visit and B (one table of n_tokens entries)
-    int64_t size = ctx->n_tokens, use = uses + (all_slots ? q * (int64_t)nB : 0);
+    // levels over the tokens the rows visit and B (one table of n_tokens entries; per-row masks: each
+    // row's own list)
+    int64_t size = ctx->n_tokens, use = uses + (all_slots ? (M.rows() ? M.off[q] : q * (int64_t)nB) : 0);
     std::vector<int64_t> order, level_off;
     conflict_levels(
         q, 1, &size, &use,
         [&](int64_t r, auto&& v) {
           visit(r, v);
-          if (all_slots)
+          if (all_slots && M.rows())
+            for (int64_t k = M.off[r]; k < M.off[r + 1]; ++k) v(0, M.tok[k] - 1);
+          else if (all_slots)
             for (int32_t t : tok) v(0, t);
         },
         order, level_off);
@@ -4318,7 +4386,7 @@ int row_begin(cfmm_ctx* ctx) {
 }
 
 int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, const int64_t* token_out,
-                    const uint8_t* kind, const double* amount, const double* limit, const uint8_t* allowed,
+                    const uint8_t* kind, const double* amount, const double* limit, const Allowed& M,
                     const cfmm_subgraph_opts& o, cfmm_subgraph_out* out) {
   int rc;
   if ((rc = row_begin(ctx)) != CFMM_OK) return rc;
@@ -4331,24 +4399,45 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
   CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
   int occ = 0, occ_out = 0;
   const char* name = "a subgraph row kernel";
-  if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::subgraph_kernel<false>), {}, name, occ)) != CFMM_OK) return rc;
   const int64_t n_out = kind ? std::count(kind, kind + q, (uint8_t)CFMM_SWAP_EXACT_OUT) : 0;
-  if (n_out > 0 && (rc = row_occupancy(ctx, kernel_ptr(&cfmm::subgraph_out_kernel<false>), {}, name, occ_out)) != CFMM_OK)
-    return rc;
+  if (M.rows()) {  // per-row masks: the row graph's dynamic shared memory
+    if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::subgraph_rows_kernel<false, false>),
+                            {kernel_ptr(&cfmm::subgraph_rows_plan_kernel), kernel_ptr(&cfmm::subgraph_rows_kernel<false, false>),
+                             kernel_ptr(&cfmm::subgraph_rows_kernel<true, false>)},
+                            name, occ, cfmm::kRowGraphBytes)) != CFMM_OK)
+      return rc;
+    if (n_out > 0 && (rc = row_occupancy(ctx, kernel_ptr(&cfmm::subgraph_rows_kernel<false, true>),
+                                         {kernel_ptr(&cfmm::subgraph_rows_kernel<false, true>),
+                                          kernel_ptr(&cfmm::subgraph_rows_kernel<true, true>)},
+                                         name, occ_out, cfmm::kRowGraphBytes)) != CFMM_OK)
+      return rc;
+  } else {
+    if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::subgraph_kernel<false>), {}, name, occ)) != CFMM_OK) return rc;
+    if (n_out > 0 && (rc = row_occupancy(ctx, kernel_ptr(&cfmm::subgraph_out_kernel<false>), {}, name, occ_out)) != CFMM_OK)
+      return rc;
+  }
   cfmm::SubgraphRows R{d_in.p, d_out.p, d_amount.p, d_limit.p, o.max_iter, o.max_fun, o.rtol, o.factr};
   return row_orders(
-      ctx, exec, q, allowed, R, out ? *out : none, occ, occ_out, n_out, 0, q, 2 * q, true, "execute_subgraph_orders",
+      ctx, exec, q, M, R, out ? *out : none, occ, occ_out, n_out, 0, q, 2 * q, true, "execute_subgraph_orders",
       [&](unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P, cfmm::PairIndexView pv, cfmm::AdjView A,
-          const cfmm::BestPathGraph& G, const uint8_t* act, int64_t* ntok, int64_t* npool) {
-        cfmm::subgraph_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, d_in.p, d_out.p, q,
-                                                                              ntok, npool);
+          const cfmm::BestPathGraph& G, const uint8_t* act, const cfmm::RowMasks& RM, int64_t* ntok, int64_t* npool) {
+        if (RM.off)
+          cfmm::subgraph_rows_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, RM, d_in.p, d_out.p, q,
+                                                                                     ntok, npool);
+        else
+          cfmm::subgraph_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, d_in.p, d_out.p, q,
+                                                                                ntok, npool);
       },
       [&](auto exec_tag, bool second, unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P,
           cfmm::PairIndexView pv, cfmm::AdjView A, const cfmm::BestPathGraph& G, const uint8_t* act,
-          const cfmm::SubgraphRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv, const int64_t* rows,
-          int64_t n) {
+          const cfmm::RowMasks& RM, const cfmm::SubgraphRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv,
+          const int64_t* rows, int64_t n) {
         constexpr bool X = decltype(exec_tag)::value;
-        if (second)
+        if (RM.off && second)
+          cfmm::subgraph_rows_kernel<X, true><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, RM, R, W, mv, rows, n);
+        else if (RM.off)
+          cfmm::subgraph_rows_kernel<X, false><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, RM, R, W, mv, rows, n);
+        else if (second)
           cfmm::subgraph_out_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, R, W, mv, rows, n);
         else
           cfmm::subgraph_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, R, W, mv, rows, n);
@@ -4364,7 +4453,7 @@ int subgraph_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in
 // row a limit row (cfmm_quote/execute_limit_orders), run by basket_limit_kernel.
 int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, const int64_t* basket_off,
                   const int64_t* basket_token, const uint8_t* kind, const double* basket_amount,
-                  const double* limit_price, const double* limit, const uint8_t* allowed, const cfmm_subgraph_opts& o,
+                  const double* limit_price, const double* limit, const Allowed& M, const cfmm_subgraph_opts& o,
                   const cfmm_basket_out& O, const char* what) {
   int rc;
   if ((rc = row_begin(ctx)) != CFMM_OK) return rc;
@@ -4382,7 +4471,29 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
   if (limit_price) CU_TRY(ctx, d_price.upload(limit_price, (size_t)NE));
   CU_TRY(ctx, d_limit.upload(limit, (size_t)q));
   int occ = 0, occ_buy = 0;
-  if (limit_price) {
+  int64_t n_buy = 0;
+  for (int64_t r = 0; r < q; ++r) n_buy += basket_buy_row(basket_off, kind, r);
+  if (M.rows()) {  // per-row masks: basket_rows_kernel, with the row graph after the basket's bytes
+    const size_t most = cfmm::bk_dyn_bytes(cfmm::kBasketMaxTokens, cfmm::kSubgraphSlots) + cfmm::kRowGraphBytes;
+    const void* plan = kernel_ptr(&cfmm::basket_rows_plan_kernel);
+    if (limit_price) {
+      if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::basket_rows_kernel<false, false, true>),
+                              {plan, kernel_ptr(&cfmm::basket_rows_kernel<false, false, true>),
+                               kernel_ptr(&cfmm::basket_rows_kernel<true, false, true>)},
+                              "basket_rows_kernel", occ, most)) != CFMM_OK)
+        return rc;
+    } else if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::basket_rows_kernel<false, false, false>),
+                                   {plan, kernel_ptr(&cfmm::basket_rows_kernel<false, false, false>),
+                                    kernel_ptr(&cfmm::basket_rows_kernel<true, false, false>)},
+                                   "basket_rows_kernel", occ, most)) != CFMM_OK) {
+      return rc;
+    }
+    if (n_buy > 0 && (rc = row_occupancy(ctx, kernel_ptr(&cfmm::basket_rows_kernel<false, true, false>),
+                                         {kernel_ptr(&cfmm::basket_rows_kernel<false, true, false>),
+                                          kernel_ptr(&cfmm::basket_rows_kernel<true, true, false>)},
+                                         "basket_rows_kernel", occ_buy, most)) != CFMM_OK)
+      return rc;
+  } else if (limit_price) {
     if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::basket_limit_kernel<false>),
                             {kernel_ptr(&cfmm::basket_plan_kernel), kernel_ptr(&cfmm::basket_limit_kernel<false>),
                              kernel_ptr(&cfmm::basket_limit_kernel<true>)},
@@ -4395,9 +4506,7 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
     return rc;
   }
   // buy rows run basket_buy_kernel (sized the same way, once per context, when a call first has them)
-  int64_t n_buy = 0;
-  for (int64_t r = 0; r < q; ++r) n_buy += basket_buy_row(basket_off, kind, r);
-  if (n_buy > 0 &&
+  if (!M.rows() && n_buy > 0 &&
       (rc = row_occupancy(ctx, kernel_ptr(&cfmm::basket_buy_kernel<false>),
                           {kernel_ptr(&cfmm::basket_buy_kernel<false>), kernel_ptr(&cfmm::basket_buy_kernel<true>)},
                           "basket_buy_kernel", occ_buy)) != CFMM_OK)
@@ -4406,18 +4515,32 @@ int basket_orders(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out,
   cfmm::LimitRows R{{d_out.p, d_boff.p, d_btok.p, d_bamt.p, d_limit.p, o.max_iter, o.max_fun, o.rtol, o.factr},
                     d_price.p};
   return row_orders(
-      ctx, exec, q, allowed, R, O, occ, occ_buy, n_buy, K, NE, q + NE, true, what,
+      ctx, exec, q, M, R, O, occ, occ_buy, n_buy, K, NE, q + NE, true, what,
       [&](unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P, cfmm::PairIndexView pv, cfmm::AdjView A,
-          const cfmm::BestPathGraph& G, const uint8_t* act, int64_t* ntok, int64_t* npool) {
-        cfmm::basket_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, d_boff.p, d_btok.p,
-                                                                            d_out.p, q, ntok, npool);
+          const cfmm::BestPathGraph& G, const uint8_t* act, const cfmm::RowMasks& RM, int64_t* ntok, int64_t* npool) {
+        if (RM.off)
+          cfmm::basket_rows_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, RM, d_boff.p, d_btok.p,
+                                                                                   d_out.p, q, ntok, npool);
+        else
+          cfmm::basket_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, d_boff.p, d_btok.p,
+                                                                              d_out.p, q, ntok, npool);
       },
       [&](auto exec_tag, bool second, unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P,
           cfmm::PairIndexView pv, cfmm::AdjView A, const cfmm::BestPathGraph& G, const uint8_t* act,
-          const cfmm::LimitRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv, const int64_t* rows,
-          int64_t n) {
+          const cfmm::RowMasks& RM, const cfmm::LimitRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv,
+          const int64_t* rows, int64_t n) {
         constexpr bool X = decltype(exec_tag)::value;
-        if (limit_price)
+        const cfmm::BasketRows& B = R;
+        if (RM.off && limit_price)
+          cfmm::basket_rows_kernel<X, false, true><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, RM, R, nullptr, W,
+                                                                                             mv, rows, n);
+        else if (RM.off && second)
+          cfmm::basket_rows_kernel<X, true, false><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, RM, B, d_kind.p,
+                                                                                             W, mv, rows, n);
+        else if (RM.off)
+          cfmm::basket_rows_kernel<X, false, false><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, RM, B, nullptr,
+                                                                                              W, mv, rows, n);
+        else if (limit_price)
           cfmm::basket_limit_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, R, W, mv, rows, n);
         else if (second)
           cfmm::basket_buy_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, G, act, R, d_kind.p, W, mv,
@@ -4444,9 +4567,9 @@ cfmm_subgraph_opts subgraph_opts(const cfmm_subgraph_opts* in) {
 
 int basket_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, const int64_t* basket_off,
                 const int64_t* basket_token, const uint8_t* kind, const double* basket_amount, const double* limit,
-                const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_basket_out* out, const char* what) {
+                Allowed M, const cfmm_subgraph_opts* opts, cfmm_basket_out* out, const char* what) {
   const cfmm_subgraph_opts o = subgraph_opts(opts);
-  int rc = check_basket(ctx, q, token_out, basket_off, basket_token, kind, basket_amount, limit, allowed, o, what);
+  int rc = check_basket(ctx, q, token_out, basket_off, basket_token, kind, basket_amount, limit, M, o, what);
   if (rc != CFMM_OK) return rc;
   if (q == 0) {
     if (out && out->tok_off) out->tok_off[0] = 0;
@@ -4454,19 +4577,18 @@ int basket_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, c
     return CFMM_OK;
   }
   const cfmm_basket_out none{};
-  return basket_orders(ctx, exec, q, token_out, basket_off, basket_token, kind, basket_amount, nullptr, limit,
-                       allowed, o, out ? *out : none, what);
+  return basket_orders(ctx, exec, q, token_out, basket_off, basket_token, kind, basket_amount, nullptr, limit, M, o,
+                       out ? *out : none, what);
 }
 
 // cfmm_quote/execute_limit_orders: the basket calls' checks, then every limit price finite and >= 0,
 // before anything runs; the rows through basket_orders; then each row's surplus on the host.
 int limit_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, const int64_t* basket_off,
                const int64_t* basket_token, const double* basket_amount, const double* limit_price,
-               const double* min_received, const uint8_t* allowed, const cfmm_subgraph_opts* opts,
-               cfmm_limit_out* out, const char* what) {
+               const double* min_received, Allowed M, const cfmm_subgraph_opts* opts, cfmm_limit_out* out,
+               const char* what) {
   const cfmm_subgraph_opts o = subgraph_opts(opts);
-  int rc = check_basket(ctx, q, token_out, basket_off, basket_token, nullptr, basket_amount, min_received, allowed,
-                        o, what);
+  int rc = check_basket(ctx, q, token_out, basket_off, basket_token, nullptr, basket_amount, min_received, M, o, what);
   if (rc != CFMM_OK) return rc;
   if (q == 0) {
     if (out && out->tok_off) out->tok_off[0] = 0;
@@ -4507,7 +4629,7 @@ int limit_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, co
   if (!paid.empty()) O.paid = paid.data();
   if (!recv.empty()) O.received = recv.data();
   if ((rc = basket_orders(ctx, exec, q, token_out, basket_off, basket_token, nullptr, basket_amount, limit_price,
-                          min_received, allowed, o, O, what)) != CFMM_OK)
+                          min_received, M, o, O, what)) != CFMM_OK)
     return rc;
   // S = received − Σ_k c_k·paid_k in entry order: a multiply, then a subtract (no fma)
   if (surplus)
@@ -4527,7 +4649,8 @@ int limit_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_out, co
 // Every argument of cfmm_quote/execute_price_arbitrage, before anything runs.
 int check_price_arb(cfmm_ctx* ctx, int64_t q, const double* price, const double* min_profit, const uint8_t* allowed,
                     const cfmm_subgraph_opts& o, const char* what) {
-  int rc = check_row_opts(ctx, q, allowed, o, what);
+  Allowed M{allowed};
+  int rc = check_row_opts(ctx, q, M, o, what);
   if (rc != CFMM_OK || q == 0) return rc;
   if (!price) return fail(ctx, CFMM_ERR_INVALID, "%s: null price", what);
   const int64_t nA = count_allowed(ctx, allowed);
@@ -4590,14 +4713,14 @@ int price_arbitrage(cfmm_ctx* ctx, bool exec, int64_t q, const double* price, co
   cfmm::PriceArbRows R{d_price.p, d_min.p, o.max_iter, o.max_fun, o.rtol, o.factr};
   // a row's T lies in its priced tokens: rows whose priced tokens are disjoint share no pool
   return row_orders(
-      ctx, exec, q, allowed, R, O, occ, 0, 0, 0, 0, uses, false, what,
+      ctx, exec, q, Allowed{allowed}, R, O, occ, 0, 0, 0, 0, uses, false, what,
       [&](unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets*, cfmm::PairIndexView pv, cfmm::AdjView,
-          const cfmm::BestPathGraph& G, const uint8_t* act, int64_t* ntok, int64_t* npool) {
+          const cfmm::BestPathGraph& G, const uint8_t* act, const cfmm::RowMasks&, int64_t* ntok, int64_t* npool) {
         cfmm::price_arb_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(pv, G, act, d_price.p, q, ntok, npool);
       },
       [&](auto exec_tag, bool, unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P,
           cfmm::PairIndexView pv, cfmm::AdjView, const cfmm::BestPathGraph& G, const uint8_t* act,
-          const cfmm::PriceArbRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv, const int64_t* rows,
+          const cfmm::RowMasks&, const cfmm::PriceArbRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv, const int64_t* rows,
           int64_t n) {
         constexpr bool X = decltype(exec_tag)::value;
         cfmm::price_arb_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, G, act, R, W, mv, rows, n);
@@ -4625,32 +4748,36 @@ int price_arb_call(cfmm_ctx* ctx, bool exec, int64_t q, const double* price, con
 
 }  // namespace
 
-int cfmm_quote_subgraph_swap_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
-                                    const uint8_t* kind, const double* amount, const uint8_t* allowed,
-                                    const cfmm_subgraph_opts* opts, cfmm_subgraph_out* out) {
+namespace {
+
+int subgraph_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                  const uint8_t* kind, const double* amount, const double* limit, Allowed M,
+                  const cfmm_subgraph_opts* opts, cfmm_subgraph_out* out, const char* what) {
   const cfmm_subgraph_opts o = subgraph_opts(opts);
-  int rc = check_subgraph(ctx, q, token_in, token_out, kind, amount, nullptr, allowed, o, "quote_subgraph_orders");
+  int rc = check_subgraph(ctx, q, token_in, token_out, kind, amount, limit, M, o, what);
   if (rc != CFMM_OK) return rc;
   if (q == 0) {
     if (out && out->tok_off) out->tok_off[0] = 0;
     if (out && out->leg_off) out->leg_off[0] = 0;
     return CFMM_OK;
   }
-  return subgraph_orders(ctx, false, q, token_in, token_out, kind, amount, nullptr, allowed, o, out);
+  return subgraph_orders(ctx, exec, q, token_in, token_out, kind, amount, limit, M, o, out);
+}
+
+}  // namespace
+
+int cfmm_quote_subgraph_swap_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                                    const uint8_t* kind, const double* amount, const uint8_t* allowed,
+                                    const cfmm_subgraph_opts* opts, cfmm_subgraph_out* out) {
+  return subgraph_call(ctx, false, q, token_in, token_out, kind, amount, nullptr, Allowed{allowed}, opts, out,
+                       "quote_subgraph_orders");
 }
 
 int cfmm_execute_subgraph_swap_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
                                       const uint8_t* kind, const double* amount, const double* limit,
                                       const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_subgraph_out* out) {
-  const cfmm_subgraph_opts o = subgraph_opts(opts);
-  int rc = check_subgraph(ctx, q, token_in, token_out, kind, amount, limit, allowed, o, "execute_subgraph_orders");
-  if (rc != CFMM_OK) return rc;
-  if (q == 0) {
-    if (out && out->tok_off) out->tok_off[0] = 0;
-    if (out && out->leg_off) out->leg_off[0] = 0;
-    return CFMM_OK;
-  }
-  return subgraph_orders(ctx, true, q, token_in, token_out, kind, amount, limit, allowed, o, out);
+  return subgraph_call(ctx, true, q, token_in, token_out, kind, amount, limit, Allowed{allowed}, opts, out,
+                       "execute_subgraph_orders");
 }
 
 int cfmm_quote_subgraph_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
@@ -4668,37 +4795,37 @@ int cfmm_execute_subgraph_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_
 int cfmm_quote_basket_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
                              const int64_t* basket_token, const double* basket_amount, const uint8_t* allowed,
                              const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
-  return basket_call(ctx, false, q, token_out, basket_off, basket_token, nullptr, basket_amount, nullptr, allowed,
-                     opts, out, "quote_basket_orders");
+  return basket_call(ctx, false, q, token_out, basket_off, basket_token, nullptr, basket_amount, nullptr,
+                     Allowed{allowed}, opts, out, "quote_basket_orders");
 }
 
 int cfmm_execute_basket_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
                                const int64_t* basket_token, const double* basket_amount, const double* limit,
                                const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
-  return basket_call(ctx, true, q, token_out, basket_off, basket_token, nullptr, basket_amount, limit, allowed,
-                     opts, out, "execute_basket_orders");
+  return basket_call(ctx, true, q, token_out, basket_off, basket_token, nullptr, basket_amount, limit,
+                     Allowed{allowed}, opts, out, "execute_basket_orders");
 }
 
 int cfmm_quote_basket_swap_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
                                   const int64_t* basket_token, const uint8_t* entry_kind, const double* basket_amount,
                                   const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
-  return basket_call(ctx, false, q, token_out, basket_off, basket_token, entry_kind, basket_amount, nullptr, allowed,
-                     opts, out, "quote_basket_swap_orders");
+  return basket_call(ctx, false, q, token_out, basket_off, basket_token, entry_kind, basket_amount, nullptr,
+                     Allowed{allowed}, opts, out, "quote_basket_swap_orders");
 }
 
 int cfmm_execute_basket_swap_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
                                     const int64_t* basket_token, const uint8_t* entry_kind,
                                     const double* basket_amount, const double* limit, const uint8_t* allowed,
                                     const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
-  return basket_call(ctx, true, q, token_out, basket_off, basket_token, entry_kind, basket_amount, limit, allowed,
-                     opts, out, "execute_basket_swap_orders");
+  return basket_call(ctx, true, q, token_out, basket_off, basket_token, entry_kind, basket_amount, limit,
+                     Allowed{allowed}, opts, out, "execute_basket_swap_orders");
 }
 
 int cfmm_quote_limit_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
                             const int64_t* basket_token, const double* basket_amount, const double* limit_price,
                             const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_limit_out* out) {
-  return limit_call(ctx, false, q, token_out, basket_off, basket_token, basket_amount, limit_price, nullptr, allowed,
-                    opts, out, "quote_limit_orders");
+  return limit_call(ctx, false, q, token_out, basket_off, basket_token, basket_amount, limit_price, nullptr,
+                    Allowed{allowed}, opts, out, "quote_limit_orders");
 }
 
 int cfmm_execute_limit_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
@@ -4706,7 +4833,59 @@ int cfmm_execute_limit_orders(cfmm_ctx* ctx, int64_t q, const int64_t* token_out
                               const double* min_received, const uint8_t* allowed, const cfmm_subgraph_opts* opts,
                               cfmm_limit_out* out) {
   return limit_call(ctx, true, q, token_out, basket_off, basket_token, basket_amount, limit_price, min_received,
-                    allowed, opts, out, "execute_limit_orders");
+                    Allowed{allowed}, opts, out, "execute_limit_orders");
+}
+
+// ---- per-row masks: the calls above with one allowed list per row (the rows' own slot graphs)
+
+int cfmm_quote_subgraph_swap_orders_rows(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                                         const uint8_t* kind, const double* amount, const int64_t* allow_off,
+                                         const int64_t* allow_token, const cfmm_subgraph_opts* opts,
+                                         cfmm_subgraph_out* out) {
+  return subgraph_call(ctx, false, q, token_in, token_out, kind, amount, nullptr, Allowed{nullptr, true, allow_off, allow_token},
+                       opts, out, "quote_subgraph_orders_rows");
+}
+
+int cfmm_execute_subgraph_swap_orders_rows(cfmm_ctx* ctx, int64_t q, const int64_t* token_in,
+                                           const int64_t* token_out, const uint8_t* kind, const double* amount,
+                                           const double* limit, const int64_t* allow_off, const int64_t* allow_token,
+                                           const cfmm_subgraph_opts* opts, cfmm_subgraph_out* out) {
+  return subgraph_call(ctx, true, q, token_in, token_out, kind, amount, limit, Allowed{nullptr, true, allow_off, allow_token},
+                       opts, out, "execute_subgraph_orders_rows");
+}
+
+int cfmm_quote_basket_swap_orders_rows(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                                       const int64_t* basket_token, const uint8_t* entry_kind,
+                                       const double* basket_amount, const int64_t* allow_off,
+                                       const int64_t* allow_token, const cfmm_subgraph_opts* opts,
+                                       cfmm_basket_out* out) {
+  return basket_call(ctx, false, q, token_out, basket_off, basket_token, entry_kind, basket_amount, nullptr,
+                     Allowed{nullptr, true, allow_off, allow_token}, opts, out, "quote_basket_swap_orders_rows");
+}
+
+int cfmm_execute_basket_swap_orders_rows(cfmm_ctx* ctx, int64_t q, const int64_t* token_out,
+                                         const int64_t* basket_off, const int64_t* basket_token,
+                                         const uint8_t* entry_kind, const double* basket_amount, const double* limit,
+                                         const int64_t* allow_off, const int64_t* allow_token,
+                                         const cfmm_subgraph_opts* opts, cfmm_basket_out* out) {
+  return basket_call(ctx, true, q, token_out, basket_off, basket_token, entry_kind, basket_amount, limit,
+                     Allowed{nullptr, true, allow_off, allow_token}, opts, out, "execute_basket_swap_orders_rows");
+}
+
+int cfmm_quote_limit_orders_rows(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                                 const int64_t* basket_token, const double* basket_amount, const double* limit_price,
+                                 const int64_t* allow_off, const int64_t* allow_token, const cfmm_subgraph_opts* opts,
+                                 cfmm_limit_out* out) {
+  return limit_call(ctx, false, q, token_out, basket_off, basket_token, basket_amount, limit_price, nullptr,
+                    Allowed{nullptr, true, allow_off, allow_token}, opts, out, "quote_limit_orders_rows");
+}
+
+int cfmm_execute_limit_orders_rows(cfmm_ctx* ctx, int64_t q, const int64_t* token_out, const int64_t* basket_off,
+                                   const int64_t* basket_token, const double* basket_amount,
+                                   const double* limit_price, const double* min_received, const int64_t* allow_off,
+                                   const int64_t* allow_token, const cfmm_subgraph_opts* opts, cfmm_limit_out* out) {
+  return limit_call(ctx, true, q, token_out, basket_off, basket_token, basket_amount, limit_price, min_received,
+                    Allowed{nullptr, true, allow_off, allow_token}, opts, out, "execute_limit_orders_rows");
 }
 
 int cfmm_quote_price_arbitrage(cfmm_ctx* ctx, int64_t q, const double* price, const uint8_t* allowed,

@@ -58,6 +58,108 @@ __global__ void subgraph_act_kernel(const PathSets* __restrict__ P, PairIndexVie
   if (m < G.deg[s]) act[t] = subgraph_pair_active(P, ix, G.pair[t]) ? 1 : 0;
 }
 
+// ---- per-row masks (the *_rows calls): each row's own slots and their graph, built by its CTA
+
+// Slot lookup in a row's slots: its listed tokens (0-based) ascending in tok[0 .. n), bisected; −1
+// for a token the row does not list.
+struct RowSlotOf {
+  const int32_t* tok;
+  int n;
+  __device__ __forceinline__ int32_t operator[](int32_t t) const {
+    int lo = 0, hi = n;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (tok[mid] < t)
+        lo = mid + 1;
+      else
+        hi = mid;
+    }
+    return lo < n && tok[lo] == t ? lo : -1;
+  }
+};
+
+// One row's slot graph, read through the same members as BestPathGraph: tok and deg in dynamic shared
+// memory, nbr and pair (and the activity beside them) in the CTA's part of the call's RowMasks.
+struct RowGraph {
+  const int32_t* tok;
+  RowSlotOf slot_of;
+  const int32_t* deg;
+  const int16_t* nbr;
+  const int32_t* pair;
+  int nB;
+};
+
+// The per-row masks of a call: row r lists the tokens tok[off[r] .. off[r+1]) (1-based, distinct).
+// Each CTA owns cap = bmax² entries of nbr, pair and act (bmax: the call's longest list); the row's
+// sorted tokens and degrees live at byte goff of the dynamic shared memory (after the basket rows'
+// bk_dyn_bytes).
+struct RowMasks {
+  const int64_t* off;
+  const int64_t* tok;
+  int16_t* nbr;
+  int32_t* pair;
+  uint8_t* act;
+  int64_t cap;
+  int goff;
+};
+constexpr int kRowGraphBytes = 2 * kSubgraphSlots * (int)sizeof(int32_t);  // tok and deg
+
+extern __shared__ __align__(8) unsigned char rg_dyn[];
+
+__device__ __forceinline__ const uint8_t* rg_act(const RowMasks& M) { return M.act + M.cap * blockIdx.x; }
+
+// Row r's slot graph, by the whole CTA: its tokens sorted by rank (they are distinct), then one warp
+// per slot s: the slots among s's token's neighbours, ascending, with their pair and whether it holds
+// an active pool (subgraph_act_kernel's rule), from the adjacency list walked when it is short, else
+// bisected per slot (side_pairs' rule).  Ends at a barrier.
+__device__ RowGraph row_graph(const PathSets* P, PairIndexView ix, AdjView A, const RowMasks& M, int64_t r) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  int32_t* tok = reinterpret_cast<int32_t*>(rg_dyn + M.goff);
+  int32_t* deg = tok + kSubgraphSlots;
+  const int64_t a0 = M.off[r], c = M.cap * blockIdx.x;
+  const int n = (int)(M.off[r + 1] - a0);
+  int16_t* nbr = M.nbr + c;
+  int32_t* pair = M.pair + c;
+  uint8_t* act = M.act + c;
+  for (int k = tid; k < n; k += blockDim.x) deg[k] = (int32_t)(M.tok[a0 + k] - 1);  // (staged in deg)
+  __syncthreads();
+  for (int k = tid; k < n; k += blockDim.x) {
+    const int32_t v = deg[k];
+    int rank = 0;
+    for (int l = 0; l < n; ++l) rank += deg[l] < v;
+    tok[rank] = v;
+  }
+  __syncthreads();
+  const RowGraph G{tok, RowSlotOf{tok, n}, deg, nbr, pair, n};
+  for (int s = warp; s < n; s += kSubgraphWarps) {
+    const int64_t e0 = A.off[tok[s]], e1 = A.off[tok[s] + 1];
+    const bool walk = e1 - e0 <= (int64_t)n;
+    int cnt = 0;
+    for (int64_t b = walk ? e0 : 0; b < (walk ? e1 : (int64_t)n); b += 32) {
+      int32_t u = -1;
+      int64_t e = -1;
+      if (walk) {
+        e = b + lane;
+        if (e < e1) u = G.slot_of[A.nbr[e]];
+      } else if (b + lane < n) {
+        e = adj_find(A, e0, e1, tok[b + lane]);
+        if (e < e1) u = (int32_t)(b + lane);
+      }
+      const unsigned in = __ballot_sync(kFull, u >= 0);
+      if (u >= 0) {
+        const int64_t at = (int64_t)n * s + cnt + __popc(in & ((1u << lane) - 1u));
+        nbr[at] = (int16_t)u;
+        pair[at] = A.pair[e];
+        act[at] = subgraph_pair_active(P, ix, A.pair[e]) ? 1 : 0;
+      }
+      cnt += __popc(in);
+    }
+    if (lane == 0) deg[s] = cnt;
+  }
+  __syncthreads();
+  return G;
+}
+
 // The rows of one call, their options, and their outputs (device arrays; tokens 1-based).
 struct SubgraphRows {
   const int64_t* token_in;
@@ -118,7 +220,8 @@ __device__ __forceinline__ bool sg_slot_ok(const SubgraphSmem& m, int s) { retur
 
 // Setup of row (j, i), 0-based: T, the local tokens and the pool count of every slot (cnt[s], the
 // pools of the pairs {s, i}, {s, j} when j ∈ T, and {s, u} for slots u > s in T) and of {j, i}.
-__device__ void sg_setup(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
+template <class Graph>  // BestPathGraph or RowGraph
+__device__ void sg_setup(const PathSets* P, PairIndexView ix, AdjView A, const Graph& G,
                          const uint8_t* __restrict__ gact, int32_t j, int32_t i, SubgraphSmem& m) {
   const int tid = threadIdx.x, nB = G.nB;
   for (int s = tid; s < nB; s += blockDim.x) {
@@ -207,7 +310,8 @@ __device__ void sg_setup(const PathSets* P, PairIndexView ix, AdjView A, const B
   __syncthreads();
 }
 
-__device__ __forceinline__ int32_t sg_local(const BestPathGraph& G, const SubgraphSmem& m, int32_t t) {
+template <class Graph>
+__device__ __forceinline__ int32_t sg_local(const Graph& G, const SubgraphSmem& m, int32_t t) {
   if (t == m.ltok[0]) return 0;
   if (t == m.ltok[1]) return 1;
   return m.lidx[G.slot_of[t]];
@@ -441,8 +545,8 @@ __device__ __forceinline__ SubgraphWork sg_cta_work(const SubgraphWork& w) {
 // The pools of every slot s in T into the workspace at the offset the setup counted (cnt[s]): {s, i},
 // then the row kind's side pairs of s (side(s, put)), then {s, u} for the slots u > s in T.  Then a
 // barrier, which also publishes the row's leading pools.
-template <class Smem, class Side>
-__device__ __forceinline__ void sg_gather(PairIndexView ix, const BestPathGraph& G, const SubgraphWork& w,
+template <class Smem, class Side, class Graph>
+__device__ __forceinline__ void sg_gather(PairIndexView ix, const Graph& G, const SubgraphWork& w,
                                           const Smem& m, Side side) {
   for (int s = threadIdx.x; s < G.nB; s += blockDim.x) {
     if (!m.in[s]) continue;
@@ -668,8 +772,8 @@ __device__ __forceinline__ void sg_legs(const PathSets* P, const SubgraphWork& w
 // and a filled row applies the transition of cfmm_apply_trades at its ν to each of its pools.  OUT:
 // the row buys y = amount of i; its dual has lin = −y′ at i, y′ = y·(1 + rtol) rounded up, and ν_j
 // fixed at 1; it is unreachable when y is at least what its pools holding i could pay out.
-template <bool EXEC, bool OUT>
-__device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, const BestPathGraph& G,
+template <bool EXEC, bool OUT, class Graph>
+__device__ void subgraph_row(const PathSets* P, PairIndexView ix, AdjView A, const Graph& G,
                              const uint8_t* gact, const SubgraphRows& R, const SubgraphWork& w, const SplitMoved& mv,
                              int64_t r, SubgraphSmem& m) {
   __shared__ SgSolveState s;
@@ -756,6 +860,38 @@ __global__ void __launch_bounds__(kSubgraphThreads)
   const SubgraphWork wb = sg_cta_work(w);
   for (int64_t k = blockIdx.x; k < n; k += gridDim.x)
     subgraph_row<EXEC, true>(P, ix, A, G, gact, R, wb, mv, rows ? rows[k] : k, m);
+}
+
+// Per-row masks: subgraph_plan_kernel with each row's own slot graph.
+__global__ void __launch_bounds__(kSubgraphThreads)
+    subgraph_rows_plan_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, RowMasks M,
+                              const int64_t* __restrict__ token_in, const int64_t* __restrict__ token_out, int64_t q,
+                              int64_t* __restrict__ ntok, int64_t* __restrict__ npool) {
+  __shared__ SubgraphSmem m;
+  for (int64_t r = blockIdx.x; r < q; r += gridDim.x) {
+    const RowGraph G = row_graph(P, ix, A, M, r);
+    sg_setup(P, ix, A, G, rg_act(M), (int32_t)(token_in[r] - 1), (int32_t)(token_out[r] - 1), m);
+    if (threadIdx.x == 0) {
+      ntok[r] = m.n_loc - (m.jin ? 0 : 1);
+      npool[r] = m.npool;
+    }
+    __syncthreads();
+  }
+}
+
+// Per-row masks: exact-in (OUT false) or exact-out rows rows[0 .. n) (null: 0 .. n), as
+// subgraph_kernel / subgraph_out_kernel, each over its own slot graph.
+template <bool EXEC, bool OUT>
+__global__ void __launch_bounds__(kSubgraphThreads)
+    subgraph_rows_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, RowMasks M, SubgraphRows R,
+                         SubgraphWork w, SplitMoved mv, const int64_t* __restrict__ rows, int64_t n) {
+  __shared__ SubgraphSmem m;
+  const SubgraphWork wb = sg_cta_work(w);
+  for (int64_t k = blockIdx.x; k < n; k += gridDim.x) {
+    const int64_t r = rows ? rows[k] : k;
+    const RowGraph G = row_graph(P, ix, A, M, r);
+    subgraph_row<EXEC, OUT>(P, ix, A, G, rg_act(M), R, wb, mv, r, m);
+  }
 }
 
 }  // namespace cfmm

@@ -636,8 +636,14 @@ struct SubgraphOut
     leg_off::Ptr{Int64}; leg_cap::Int64; leg_type::Ptr{Cint}; leg_pool::Ptr{Int64}
     leg_delta::Ptr{Float64}; leg_lambda::Ptr{Float64}
 end
+# Per-row masks (cfmm_*_rows): allowed may instead be one Vector of 1-based tokens per row (for example
+# choose_hubs' lists); each row then runs over its own list.
+_row_csr(lists) = (Int64[0; cumsum(length.(lists))], Int64.(reduce(vcat, lists; init=Int64[])))
 function _subgraph_orders(ctx, execute::Bool, token_in::Vector{Int64}, token_out::Vector{Int64},
-                          amount::Vector{Float64}, allowed::Vector{UInt8}, limit, opts, kind=nothing)
+                          amount::Vector{Float64}, allowed, limit, opts, kind=nothing)
+    allowed isa AbstractVector{<:AbstractVector} &&
+        return _subgraph_orders_rows(ctx, execute, token_in, token_out, amount, _row_csr(allowed)..., limit, opts,
+                                     kind)
     q = length(token_in)
     length(token_out) == length(amount) == q || throw(ArgumentError("token_in / token_out / amount need q entries"))
     limit === nothing || length(limit) == q || throw(ArgumentError("limit needs q entries"))
@@ -678,6 +684,47 @@ function _subgraph_orders(ctx, execute::Bool, token_in::Vector{Int64}, token_out
             merit=merit, tok_off=tok_off, token=token[1:NT], nu=nu[1:NT], psi=psi[1:NT], leg_off=leg_off,
             leg_type=ltype[1:L], leg_pool=lpool[1:L], leg_delta=ld[:, 1:L], leg_lambda=ll[:, 1:L])
 end
+function _subgraph_orders_rows(ctx, execute::Bool, token_in::Vector{Int64}, token_out::Vector{Int64},
+                               amount::Vector{Float64}, allow_off::Vector{Int64}, allow_token::Vector{Int64}, limit,
+                               opts, kind)
+    q = length(token_in)
+    length(token_out) == length(amount) == q || throw(ArgumentError("token_in / token_out / amount need q entries"))
+    length(allow_off) == q + 1 || throw(ArgumentError("allowed needs one token list per row"))
+    k = kind === nothing ? C_NULL : (kind isa Integer ? fill(UInt8(kind), q) : Vector{UInt8}(kind))
+    o = opts === nothing ? nothing : Ref(opts)
+    argq = (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Int64}, Ptr{Int64},
+            Ptr{SubgraphOpts}, Ptr{SubgraphOut})
+    tok_off, leg_off = zeros(Int64, q + 1), zeros(Int64, q + 1)
+    sizes = Ref(SubgraphOut(C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, pointer(tok_off), 0, C_NULL,
+                            C_NULL, C_NULL, pointer(leg_off), 0, C_NULL, C_NULL, C_NULL, C_NULL))
+    GC.@preserve tok_off leg_off k chk(ctx, ccall((:cfmm_quote_subgraph_swap_orders_rows, LIB), Cint, argq, ctx, q,
+                                                 token_in, token_out, k, amount, allow_off, allow_token,
+                                                 o === nothing ? C_NULL : o, sizes))
+    NT, L = tok_off[end], leg_off[end]
+    paid, received, merit, status = zeros(q), zeros(q), zeros(q), zeros(UInt8, q)
+    sst, iters, fev = zeros(Cint, q), zeros(Cint, q), zeros(Cint, q)
+    token, nu, psi = zeros(Int64, max(NT, 1)), zeros(max(NT, 1)), zeros(max(NT, 1))
+    ltype, lpool, ld, ll = zeros(Cint, max(L, 1)), zeros(Int64, max(L, 1)), zeros(2, max(L, 1)), zeros(2, max(L, 1))
+    GC.@preserve paid received merit status sst iters fev tok_off token nu psi leg_off ltype lpool ld ll k begin
+        out = Ref(SubgraphOut(pointer(paid), pointer(received), pointer(status), pointer(sst), pointer(iters),
+                              pointer(fev), pointer(merit), pointer(tok_off), NT, pointer(token), pointer(nu),
+                              pointer(psi), pointer(leg_off), L, pointer(ltype), pointer(lpool), pointer(ld),
+                              pointer(ll)))
+        if execute
+            chk(ctx, ccall((:cfmm_execute_subgraph_swap_orders_rows, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64}, Ptr{Int64},
+                 Ptr{Int64}, Ptr{SubgraphOpts}, Ptr{SubgraphOut}),
+                ctx, q, token_in, token_out, k, amount, limit === nothing ? C_NULL : limit, allow_off, allow_token,
+                o === nothing ? C_NULL : o, out))
+        else
+            chk(ctx, ccall((:cfmm_quote_subgraph_swap_orders_rows, LIB), Cint, argq, ctx, q, token_in, token_out, k,
+                           amount, allow_off, allow_token, o === nothing ? C_NULL : o, out))
+        end
+    end
+    return (paid=paid, received=received, status=status, solver_status=sst, iterations=iters, fun_evals=fev,
+            merit=merit, tok_off=tok_off, token=token[1:NT], nu=nu[1:NT], psi=psi[1:NT], leg_off=leg_off,
+            leg_type=ltype[1:L], leg_pool=lpool[1:L], leg_delta=ld[:, 1:L], leg_lambda=ll[:, 1:L])
+end
 quote_subgraph_orders(ctx, token_in, token_out, amount, allowed; opts=nothing, kind=nothing) =
     _subgraph_orders(ctx, false, token_in, token_out, amount, allowed, nothing, opts, kind)
 execute_subgraph_orders!(ctx, token_in, token_out, amount, allowed; limit=nothing, opts=nothing, kind=nothing) =
@@ -691,8 +738,10 @@ execute_subgraph_orders!(ctx, token_in, token_out, amount, allowed; limit=nothin
 # (cfmm_basket_out).  entry_kind (nothing: every entry sold) is one UInt8 per basket entry, 0 sold or 1
 # bought, and selects cfmm_quote/execute_basket_swap_orders.  Never executed, like the rest of this file.
 function _basket_orders(ctx, execute::Bool, token_out::Vector{Int64}, basket_off::Vector{Int64},
-                        basket_token::Vector{Int64}, basket_amount::Vector{Float64}, allowed::Vector{UInt8}, limit,
+                        basket_token::Vector{Int64}, basket_amount::Vector{Float64}, allowed, limit,
                         opts, entry_kind=nothing)
+    rows = allowed isa AbstractVector{<:AbstractVector}
+    aoff, atok = rows ? _row_csr(allowed) : (Int64[], Int64[])
     q = length(token_out)
     length(basket_off) == q + 1 || throw(ArgumentError("basket_off needs q + 1 entries"))
     NE = basket_off[end]
@@ -706,7 +755,13 @@ function _basket_orders(ctx, execute::Bool, token_out::Vector{Int64}, basket_off
             Ptr{SubgraphOut})
     argk = (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{UInt8},
             Ptr{SubgraphOpts}, Ptr{SubgraphOut})
-    quote_call(out) = entry_kind === nothing ?
+    argr = (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Int64}, Ptr{Int64},
+            Ptr{SubgraphOpts}, Ptr{SubgraphOut})
+    ek = entry_kind === nothing ? C_NULL : entry_kind
+    quote_call(out) = rows ?
+        ccall((:cfmm_quote_basket_swap_orders_rows, LIB), Cint, argr, ctx, q, token_out, basket_off, basket_token,
+              ek, basket_amount, aoff, atok, o === nothing ? C_NULL : o, out) :
+        entry_kind === nothing ?
         ccall((:cfmm_quote_basket_orders, LIB), Cint, argt, ctx, q, token_out, basket_off, basket_token,
               basket_amount, allowed, o === nothing ? C_NULL : o, out) :
         ccall((:cfmm_quote_basket_swap_orders, LIB), Cint, argk, ctx, q, token_out, basket_off, basket_token,
@@ -725,7 +780,13 @@ function _basket_orders(ctx, execute::Bool, token_out::Vector{Int64}, basket_off
                               pointer(fev), pointer(merit), pointer(tok_off), NT, pointer(token), pointer(nu),
                               pointer(psi), pointer(leg_off), L, pointer(ltype), pointer(lpool), pointer(ld),
                               pointer(ll)))
-        if execute && entry_kind !== nothing
+        if execute && rows
+            chk(ctx, ccall((:cfmm_execute_basket_swap_orders_rows, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64},
+                 Ptr{Int64}, Ptr{Int64}, Ptr{SubgraphOpts}, Ptr{SubgraphOut}),
+                ctx, q, token_out, basket_off, basket_token, ek, basket_amount,
+                limit === nothing ? C_NULL : limit, aoff, atok, o === nothing ? C_NULL : o, out))
+        elseif execute && entry_kind !== nothing
             chk(ctx, ccall((:cfmm_execute_basket_swap_orders, LIB), Cint,
                 (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64},
                  Ptr{UInt8}, Ptr{SubgraphOpts}, Ptr{SubgraphOut}),
@@ -826,7 +887,9 @@ struct LimitOut
 end
 function _limit_orders(ctx, execute::Bool, token_out::Vector{Int64}, basket_off::Vector{Int64},
                        basket_token::Vector{Int64}, basket_amount::Vector{Float64}, limit_price::Vector{Float64},
-                       allowed::Vector{UInt8}, min_received, opts)
+                       allowed, min_received, opts)
+    rows = allowed isa AbstractVector{<:AbstractVector}
+    aoff, atok = rows ? _row_csr(allowed) : (Int64[], Int64[])
     q = length(token_out)
     length(basket_off) == q + 1 || throw(ArgumentError("basket_off needs q + 1 entries"))
     NE = basket_off[end]
@@ -839,9 +902,14 @@ function _limit_orders(ctx, execute::Bool, token_out::Vector{Int64}, basket_off:
     tok_off, leg_off = zeros(Int64, q + 1), zeros(Int64, q + 1)
     sizes = Ref(LimitOut(C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, pointer(tok_off), 0, C_NULL,
                          C_NULL, C_NULL, pointer(leg_off), 0, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL))
-    GC.@preserve tok_off leg_off chk(ctx, ccall((:cfmm_quote_limit_orders, LIB), Cint, argq, ctx, q, token_out,
-                                               basket_off, basket_token, basket_amount, limit_price, allowed,
-                                               o === nothing ? C_NULL : o, sizes))
+    argr = (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{Int64},
+            Ptr{Int64}, Ptr{SubgraphOpts}, Ptr{LimitOut})
+    quote_call(out) = rows ?
+        ccall((:cfmm_quote_limit_orders_rows, LIB), Cint, argr, ctx, q, token_out, basket_off, basket_token,
+              basket_amount, limit_price, aoff, atok, o === nothing ? C_NULL : o, out) :
+        ccall((:cfmm_quote_limit_orders, LIB), Cint, argq, ctx, q, token_out, basket_off, basket_token,
+              basket_amount, limit_price, allowed, o === nothing ? C_NULL : o, out)
+    GC.@preserve tok_off leg_off chk(ctx, quote_call(sizes))
     NT, L = tok_off[end], leg_off[end]
     paid, received, surplus, merit, status = zeros(max(NE, 1)), zeros(q), zeros(q), zeros(q), zeros(UInt8, q)
     sst, iters, fev = zeros(Cint, q), zeros(Cint, q), zeros(Cint, q)
@@ -852,15 +920,20 @@ function _limit_orders(ctx, execute::Bool, token_out::Vector{Int64}, basket_off:
                            pointer(fev), pointer(merit), pointer(tok_off), NT, pointer(token), pointer(nu),
                            pointer(psi), pointer(leg_off), L, pointer(ltype), pointer(lpool), pointer(ld),
                            pointer(ll), pointer(surplus)))
-        if execute
+        if execute && rows
+            chk(ctx, ccall((:cfmm_execute_limit_orders_rows, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+                 Ptr{Int64}, Ptr{Int64}, Ptr{SubgraphOpts}, Ptr{LimitOut}),
+                ctx, q, token_out, basket_off, basket_token, basket_amount, limit_price,
+                min_received === nothing ? C_NULL : min_received, aoff, atok, o === nothing ? C_NULL : o, out))
+        elseif execute
             chk(ctx, ccall((:cfmm_execute_limit_orders, LIB), Cint,
                 (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
                  Ptr{UInt8}, Ptr{SubgraphOpts}, Ptr{LimitOut}),
                 ctx, q, token_out, basket_off, basket_token, basket_amount, limit_price,
                 min_received === nothing ? C_NULL : min_received, allowed, o === nothing ? C_NULL : o, out))
         else
-            chk(ctx, ccall((:cfmm_quote_limit_orders, LIB), Cint, argq, ctx, q, token_out, basket_off, basket_token,
-                           basket_amount, limit_price, allowed, o === nothing ? C_NULL : o, out))
+            chk(ctx, quote_call(out))
         end
     end
     return (paid=paid[1:NE], received=received, surplus=surplus, status=status, solver_status=sst,

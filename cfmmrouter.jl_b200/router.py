@@ -60,14 +60,64 @@ def pool_file_info(path):
     return t.value, n.value, m.value
 
 
-def _row_args(n_tokens, q, allowed, limit, opts, what):
-    """(the mask as a uint8 pointer, the limits, the options by reference or None) of a subgraph or
-    basket call, with the Python argument errors."""
+def is_row_lists(allowed):
+    """Whether `allowed` is one token list per row (a list or tuple of sequences, as Router.choose_hubs
+    returns) rather than one mask over the tokens."""
+    return isinstance(allowed, (list, tuple)) and all(isinstance(a, (list, tuple, np.ndarray)) for a in allowed)
+
+
+def pack_row_lists(allowed, n_tokens, own, room, what):
+    """(allow_off [q + 1], allow_token) int64 of the *_rows calls from one list of 1-based tokens per
+    row, with their argument errors: q lists (q = len(own)); integer tokens in 1..n_tokens; none twice
+    in a row; and at most room[r] tokens in row r's list outside own[r], the row's own tokens.  The
+    checks run on the whole CSR at once (a batch holds many rows); an error names the first bad row."""
+    q = len(own)
+    if len(allowed) != q:
+        raise ValueError(f"{what}: allowed needs one token list per row ({q})")
+    rows = [np.asarray(lst).reshape(-1) for lst in allowed]
+    for r, a in enumerate(rows):
+        if len(a) and not np.issubdtype(a.dtype, np.integer):
+            raise ValueError(f"{what}: row {r}: allowed tokens must be integers")
+    lens = np.array([len(a) for a in rows], dtype=np.int64)
+    off = np.zeros(q + 1, dtype=np.int64)
+    np.cumsum(lens, out=off[1:])
+    tok = np.concatenate(rows).astype(np.int64) if off[-1] else np.zeros(0, dtype=np.int64)
+    row = np.repeat(np.arange(q, dtype=np.int64), lens)
+    bad = np.flatnonzero((tok < 1) | (tok > n_tokens))
+    if len(bad):
+        raise ValueError(f"{what}: row {row[bad[0]]}: an allowed token is outside 1..{n_tokens}")
+    key = row * (n_tokens + 1) + tok
+    ks = np.sort(key)
+    dup = np.flatnonzero(ks[1:] == ks[:-1])
+    if len(dup):
+        raise ValueError(f"{what}: row {ks[dup[0]] // (n_tokens + 1)}: an allowed token is listed twice")
+    own_len = np.array([len(o) for o in own], dtype=np.int64)
+    own_key = np.repeat(np.arange(q, dtype=np.int64), own_len) * (n_tokens + 1) + \
+        np.array([t for o in own for t in o], dtype=np.int64)
+    extra = np.bincount(row[~np.isin(key, own_key)], minlength=q)
+    over = np.flatnonzero(extra > np.asarray(room, dtype=np.int64))
+    if len(over):
+        r = over[0]
+        raise ValueError(f"{what}: row {r}: {extra[r]} allowed tokens besides the row's own, more than {room[r]}")
+    return off, np.ascontiguousarray(tok)
+
+
+def _row_args(n_tokens, q, allowed, limit, opts, what, own=None, room=None):
+    """(the allowed tokens as ctypes arguments, the limits, the options by reference or None) of a
+    subgraph, basket or limit call, with the Python argument errors.  The allowed tokens: a namespace
+    with rows (True for one token list per row, which selects the *_rows call: own and room give each
+    row's own tokens and its room, as pack_row_lists takes them) and args (the mask, or allow_off and
+    allow_token)."""
     if allowed is None:
-        raise ValueError(f"{what}: allowed (a mask over the tokens) is required")
-    mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
-    if len(mask) != n_tokens:
-        raise ValueError(f"{what}: allowed must have {n_tokens} entries, one per token")
+        raise ValueError(f"{what}: allowed (a mask over the tokens, or one token list per row) is required")
+    if own is not None and is_row_lists(allowed):
+        off, tok = pack_row_lists(allowed, n_tokens, own, room, what)
+        masks = SimpleNamespace(rows=True, args=(_ip(off), _ip(tok)))
+    else:
+        mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
+        if len(mask) != n_tokens:
+            raise ValueError(f"{what}: allowed must have {n_tokens} entries, one per token")
+        masks = SimpleNamespace(rows=False, args=(mask.ctypes.data_as(C.POINTER(C.c_uint8)),))
     if limit is not None:
         limit = np.ascontiguousarray(limit, dtype=np.float64).reshape(-1)
         if len(limit) != q:
@@ -77,7 +127,15 @@ def _row_args(n_tokens, q, allowed, limit, opts, what):
         d = {"max_iter": 1000, "max_fun": 4000, "rtol": 1e-4, "factr": 0.0}
         d.update(opts)
         o = _lib.SubgraphOpts(int(d["max_iter"]), int(d["max_fun"]), float(d["rtol"]), float(d["factr"]))
-    return mask.ctypes.data_as(C.POINTER(C.c_uint8)), limit, None if o is None else C.byref(o)
+    return masks, limit, None if o is None else C.byref(o)
+
+
+def _basket_room(token_out, basket_off, basket_token):
+    """Each basket or limit row's own tokens (token_out and the entries) and its room for other allowed
+    tokens: CFMM_SUBGRAPH_MAX_TOKENS + 1 tokens besides token_out, entries included."""
+    own = [[int(token_out[r])] + [int(t) for t in basket_token[basket_off[r]:basket_off[r + 1]]]
+           for r in range(len(token_out))]
+    return own, [_lib.SUBGRAPH_MAX_TOKENS + 2 - len(o) for o in own]
 
 
 def _entry_kind(kind, basket_off, limit, what):
@@ -777,17 +835,21 @@ class DevicePools:
         q = len(tin)
         if not (len(tout) == len(amount) == q):
             raise ValueError("subgraph orders: token_in, token_out and amount need one entry per row")
-        u8m, limit, po = _row_args(self.n_tokens, q, allowed, limit, opts, "subgraph orders")
+        own = [(int(a), int(b)) for a, b in zip(tin, tout)]
+        mk, limit, po = _row_args(self.n_tokens, q, allowed, limit, opts, "subgraph orders", own,
+                                  [_lib.SUBGRAPH_MAX_TOKENS] * q)
         kind = _row_kind(kind, q, limit, "subgraph orders")
         ti, to, am = _ip(tin), _ip(tout), _dp(amount)
         kd = None if kind is None else kind.ctypes.data_as(C.POINTER(C.c_uint8))
         lim = None if limit is None else _dp(limit)
+        sfx = "_rows" if mk.rows else ""
 
         def call(size, out):
             if execute and not size:
-                return self._lib.cfmm_execute_subgraph_swap_orders(self._ctx, q, ti, to, kd, am, lim, u8m, po,
-                                                                   C.byref(out))
-            return self._lib.cfmm_quote_subgraph_swap_orders(self._ctx, q, ti, to, kd, am, u8m, po, C.byref(out))
+                return getattr(self._lib, "cfmm_execute_subgraph_swap_orders" + sfx)(self._ctx, q, ti, to, kd, am, lim,
+                                                                                     *mk.args, po, C.byref(out))
+            return getattr(self._lib, "cfmm_quote_subgraph_swap_orders" + sfx)(self._ctx, q, ti, to, kd, am, *mk.args,
+                                                                               po, C.byref(out))
         return self._order_solve(q, q, _lib.SubgraphOut, call)
 
     def _order_solve(self, q, n_paid, out_type, call):
@@ -829,7 +891,8 @@ class DevicePools:
         max_iter, max_fun, rtol, factr (None: the defaults).  No state changes.  Returns a namespace:
         paid, received, status (uint8), solver_status, iterations, fun_evals, merit [q]; tok_off
         [q + 1], token, nu, psi [Σ]; leg_off [q + 1], leg_type, leg_pool [L], leg_delta, leg_lambda
-        [L, 2]."""
+        [L, 2].  allowed may instead be one list of 1-based tokens per row (choose_hubs' output as it is):
+        each row then runs over its own list, as the call with that list as its mask (the *_rows calls)."""
         return self._subgraph(False, token_in, token_out, amount, allowed, None, opts, kind)
 
     def execute_subgraph_orders(self, token_in, token_out, amount, allowed, limit=None, opts=None, kind=None):
@@ -852,12 +915,21 @@ class DevicePools:
         NE = int(boff[-1])
         if not (len(btok) == len(bamt) == NE):
             raise ValueError(f"basket orders: basket_token and basket_amount need basket_off[-1] = {NE} entries")
-        u8m, limit, po = _row_args(self.n_tokens, q, allowed, limit, opts, "basket orders")
+        own, room = _basket_room(tout, boff, btok)
+        mk, limit, po = _row_args(self.n_tokens, q, allowed, limit, opts, "basket orders", own, room)
         kind = _entry_kind(kind, boff, limit, "basket orders")
         to, bo, bt, ba = _ip(tout), _ip(boff), _ip(btok), _dp(bamt)
         lim = None if limit is None else _dp(limit)
 
         def call(size, out):
+            if mk.rows:  # every row kind through the swap calls' _rows form
+                kd = None if kind is None else kind.ctypes.data_as(C.POINTER(C.c_uint8))
+                if execute and not size:
+                    return self._lib.cfmm_execute_basket_swap_orders_rows(self._ctx, q, to, bo, bt, kd, ba, lim,
+                                                                          *mk.args, po, C.byref(out))
+                return self._lib.cfmm_quote_basket_swap_orders_rows(self._ctx, q, to, bo, bt, kd, ba, *mk.args, po,
+                                                                    C.byref(out))
+            u8m = mk.args[0]
             if kind is not None:
                 kd = kind.ctypes.data_as(C.POINTER(C.c_uint8))
                 if execute and not size:
@@ -882,7 +954,9 @@ class DevicePools:
         entry, 0 sold or 1 bought (buy basket_amount[k] of basket_token[k]); a row with a bought entry
         settles in token_out[r], and its received may be negative.  opts as quote_subgraph_orders.  No
         state changes.  Returns quote_subgraph_orders' namespace, with paid per basket entry (−Ψ: a
-        bought entry reads at most −amount) and basket_off added."""
+        bought entry reads at most −amount) and basket_off added.  allowed may instead be one list of
+        1-based tokens per row (choose_hubs' output as it is): each row then runs over its own list, as the
+        call with that list as its mask (the *_rows calls)."""
         return self._basket(False, token_out, basket_off, basket_token, basket_amount, allowed, None, opts, kind)
 
     def execute_basket_orders(self, token_out, basket_off, basket_token, basket_amount, allowed, limit=None,
@@ -911,19 +985,21 @@ class DevicePools:
                              "entries")
         if not np.all(np.isfinite(lp) & (lp >= 0.0)):
             raise ValueError("limit orders: a limit price is negative, NaN or Inf")
-        u8m, min_received, po = _row_args(self.n_tokens, q, allowed, min_received, opts, "limit orders")
+        own, room = _basket_room(tout, boff, btok)
+        mk, min_received, po = _row_args(self.n_tokens, q, allowed, min_received, opts, "limit orders", own, room)
         to, bo, bt, ba, lpp = _ip(tout), _ip(boff), _ip(btok), _dp(bamt), _dp(lp)
         lim = None if min_received is None else _dp(min_received)
         surplus = np.zeros(q)
+        quote = getattr(self._lib, "cfmm_quote_limit_orders" + ("_rows" if mk.rows else ""))
+        execute_ = getattr(self._lib, "cfmm_execute_limit_orders" + ("_rows" if mk.rows else ""))
 
         def call(size, out):
             if size:
-                return self._lib.cfmm_quote_limit_orders(self._ctx, q, to, bo, bt, ba, lpp, u8m, po, C.byref(out))
+                return quote(self._ctx, q, to, bo, bt, ba, lpp, *mk.args, po, C.byref(out))
             out.surplus = surplus.ctypes.data_as(C.POINTER(C.c_double))
             if execute:
-                return self._lib.cfmm_execute_limit_orders(self._ctx, q, to, bo, bt, ba, lpp, lim, u8m, po,
-                                                           C.byref(out))
-            return self._lib.cfmm_quote_limit_orders(self._ctx, q, to, bo, bt, ba, lpp, u8m, po, C.byref(out))
+                return execute_(self._ctx, q, to, bo, bt, ba, lpp, lim, *mk.args, po, C.byref(out))
+            return quote(self._ctx, q, to, bo, bt, ba, lpp, *mk.args, po, C.byref(out))
         out = self._order_solve(q, NE, _lib.LimitOut, call)
         out.surplus = surplus
         out.basket_off = boff
@@ -937,7 +1013,9 @@ class DevicePools:
         (finite, >= 0), over every pool among them and the tokens t with allowed[t - 1]: a basket row
         with each entry's dual bound raised to its limit, solved per row on the device; rows fill
         partially.  opts as quote_subgraph_orders.  No state changes.  Returns quote_basket_orders'
-        namespace, with surplus [q] (received - Σ limit·paid) added."""
+        namespace, with surplus [q] (received - Σ limit·paid) added.  allowed may instead be one list of
+        1-based tokens per row (choose_hubs' output as it is): each row then runs over its own list, as the
+        call with that list as its mask (the *_rows calls)."""
         return self._limit(False, token_out, basket_off, basket_token, basket_amount, limit_price, allowed, None,
                            opts)
 
@@ -952,7 +1030,8 @@ class DevicePools:
     # -- arbitrage against external prices over every pool among allowed tokens (include/cfmm_b200.h,
     #    cfmm_quote_price_arbitrage / cfmm_execute_price_arbitrage) --------------------------------------
     def _price_arb(self, execute, price, allowed, min_profit, opts):
-        u8m, _, po = _row_args(self.n_tokens, None, allowed, None, opts, "price arbitrage")
+        mk, _, po = _row_args(self.n_tokens, None, allowed, None, opts, "price arbitrage")
+        u8m = mk.args[0]
         nA = int(np.count_nonzero(np.asarray(allowed, dtype=bool)))
         if nA > _lib.PRICE_ARB_MAX_TOKENS:
             raise ValueError(f"price arbitrage: {nA} allowed tokens, more than {_lib.PRICE_ARB_MAX_TOKENS}")
@@ -1591,7 +1670,9 @@ class Router:
         device (cfmm_quote_subgraph_swap_orders).  kind: None (every row exact-in), a scalar, or one
         entry per row.  No state changes.  Returns (paid [q], received [q], status [q], detail):
         detail is DevicePools.quote_subgraph_orders' namespace (solver status, iterations, ν, Ψ,
-        legs).  Single GPU."""
+        legs).  Single GPU.  allowed may instead be one list of 1-based tokens per row (choose_hubs' output
+        as it is): each row then runs over its own list, as the call with that list as its mask (the *_rows
+        calls)."""
         tin, tout, amounts, _ = self._subgraph_args(token_in, token_out, amounts, allowed, None,
                                                     "quote_subgraph_orders")
         out = self._pools.quote_subgraph_orders(tin, tout, amounts, allowed, opts, kind)
@@ -1680,7 +1761,9 @@ class Router:
         solve per row on the device (cfmm_quote_basket_swap_orders).  No state changes.  Returns (sold
         per row, bought per row as lists of arrays in the caller's order, the net of token_out [q]
         (negative when the row pays), status [q], detail); detail is DevicePools.quote_basket_orders'
-        namespace.  Single GPU."""
+        namespace.  Single GPU.  allowed may instead be one list of 1-based tokens per row (choose_hubs'
+        output as it is): each row then runs over its own list, as the call with that list as its mask (the
+        *_rows calls)."""
         tout, off, toks, amts, kind, _, n_sell = self._swap_basket_args(token_out, sells, buys, allowed, None,
                                                                          "quote_basket_swap_orders")
         out = self._pools.quote_basket_orders(tout, off, toks, amts, allowed, opts, kind)
@@ -1707,7 +1790,9 @@ class Router:
         BasketLiquidation(token_out[r], Δin) over those pools, one dual solve per row on the device
         (cfmm_quote_basket_orders).  No state changes.  Returns (paid per entry as a list of arrays in
         the basket's order, received [q], status [q], detail): detail is DevicePools.
-        quote_basket_orders' namespace.  Single GPU."""
+        quote_basket_orders' namespace.  Single GPU.  allowed may instead be one list of 1-based tokens per
+        row (choose_hubs' output as it is): each row then runs over its own list, as the call with that list
+        as its mask (the *_rows calls)."""
         tout, off, toks, amts, _ = self._basket_args(token_out, baskets, allowed, None, "quote_basket_orders")
         out = self._pools.quote_basket_orders(tout, off, toks, amts, allowed, opts)
         return self._per_entry(out), out.received, out.status, out
@@ -1753,7 +1838,9 @@ class Router:
         (cfmm_quote_limit_orders); rows fill partially.  To buy with a budget, settle in the bought token
         and sell the budget token at limit 1 / (the highest price per unit bought).  No state changes.
         Returns (sold per entry as a list of arrays in the caller's order, received [q], surplus [q],
-        status [q], detail); detail is DevicePools.quote_limit_orders' namespace.  Single GPU."""
+        status [q], detail); detail is DevicePools.quote_limit_orders' namespace.  Single GPU.  allowed may
+        instead be one list of 1-based tokens per row (choose_hubs' output as it is): each row then runs
+        over its own list, as the call with that list as its mask (the *_rows calls)."""
         tout, off, toks, amts, lims, _ = self._limit_args(token_out, sells, allowed, None, "quote_limit_orders")
         out = self._pools.quote_limit_orders(tout, off, toks, amts, lims, allowed, opts)
         return self._per_entry(out), out.received, out.surplus, out.status, out

@@ -767,7 +767,8 @@ int cfmm_find_order_paths(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [
  * exact-out rows are below) over every pool among j, i and the allowed tokens, split optimally: route! with
  * Swap(i, j, δ) (src/objectives.jl:106-146) restricted to the row's pools, one convex dual per row.
  *   B        the tokens t with allowed[t-1] != 0 (allowed [n_tokens], required), minus j and i; at
- *            most CFMM_SUBGRAPH_MAX_TOKENS per row.  One mask per call.
+ *            most CFMM_SUBGRAPH_MAX_TOKENS per row.  One mask per call (a list per row: the _rows
+ *            calls, "per-row masks" below).
  *   T        the tokens of {j, i} ∪ B connected to i through active pools whose two tokens both lie
  *            in {j, i} ∪ B.  Pools in a component cut off from i would only trade at ν ≈ √eps.
  *   pools    every pool of every pair inside T: all three types, appended pools included, retired
@@ -817,7 +818,8 @@ int cfmm_find_order_paths(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [
  * bookkeeping of cfmm_execute_swaps runs (state version, guard-free flag, fixed-point scale, UniV3
  * tick records); the materialised trades stay.  Two rows conflict when they share a token of
  * {j, i} ∪ B; rows are leveled by cfmm_execute_paths' rule, one launch per level.  With one mask per
- * call, rows with a non-empty B share its tokens and run one after another.  An execute whose token
+ * call, rows with a non-empty B share its tokens and run one after another (per-row masks, below, let
+ * rows on disjoint tokens share a level).  An execute whose token
  * or leg outputs are given with a cap below the size is rejected before anything changes.
  * Options (cfmm_subgraph_opts, NULL: max_iter 1000, max_fun 4000, rtol 1e-4, factr 0: the factr test
  * then stops only after two steps that do not lower g).  The observed floor of m_r on random
@@ -1129,6 +1131,72 @@ int cfmm_execute_limit_orders(cfmm_ctx *ctx, int64_t q, const int64_t *token_out
                               const double *basket_amount, const double *limit_price,
                               const double *min_received /* [q] or NULL */, const uint8_t *allowed,
                               const cfmm_subgraph_opts *opts, cfmm_limit_out *out);
+
+/* ---- per-row masks: each subgraph, basket and limit row over its own allowed tokens -----------
+ * cfmm_{quote,execute}_subgraph_swap_orders_rows, cfmm_{quote,execute}_basket_swap_orders_rows and
+ * cfmm_{quote,execute}_limit_orders_rows take the arguments of the calls without _rows, with one
+ * difference: in place of the mask `allowed` they take a per-row CSR
+ *   allow_off [q+1], allow_token [allow_off[q]] (1-based),
+ * and row r's allowed tokens are allow_token[allow_off[r] .. allow_off[r+1]), in any order.  The list
+ * may be empty and may hold the row's own tokens (j and i; for baskets and limits i and the entries).
+ * Row r is defined exactly as the call without _rows with `allowed` = row r's list: B_r is the list
+ * minus the row's own tokens, and T, the component rule, the pool list in global insertion order, the
+ * local token order (…, then B_r ∩ T ascending), the dual, box, start, optimizer, stop, the fill
+ * promises, the outputs and the execute transition are that call's.  A row's bits depend on its own
+ * tokens and list alone, not on the batch or on the other rows' lists.  What differs:
+ *   size     at most CFMM_SUBGRAPH_MAX_TOKENS tokens in B_r (subgraph rows); basket and limit rows keep
+ *            the basket calls' limit on basket ∪ B_r (CFMM_SUBGRAPH_MAX_TOKENS + 1 tokens besides i).
+ *   work     each row's CTA builds its row's slot graph (the list sorted, the pairs among its tokens and
+ *            their activity) before its setup.  The device workspace adds b² · 7 bytes per resident
+ *            CTA, b the call's longest list (at most CFMM_SUBGRAPH_MAX_TOKENS + 2 tokens: about 466 KB
+ *            per CTA), and the grid stays one wave of resident CTAs, as without _rows.
+ *   execute  two rows conflict when their own token sets {j, i} ∪ B_r (baskets and limits:
+ *            {i} ∪ entries ∪ B_r) intersect; rows are leveled by cfmm_execute_paths' rule over one
+ *            n_tokens table, so rows on disjoint token sets share a level and its launches.
+ * Errors: CFMM_ERR_INVALID before anything runs or changes for every error of the call without _rows
+ * (its null-mask error aside), and for a null allow_off, a null allow_token when allow_off[q] > 0, an
+ * allow_off that does not start at 0 or that decreases, a listed token outside 1..n_tokens, a token
+ * listed twice in one row, and a row over the size limit.  Single GPU. */
+int cfmm_quote_subgraph_swap_orders_rows(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [q] */,
+                                         const int64_t *token_out /* [q] */,
+                                         const uint8_t *kind /* [q] or NULL: all exact-in */,
+                                         const double *amount /* [q] */, const int64_t *allow_off /* [q+1] */,
+                                         const int64_t *allow_token /* [allow_off[q]] */,
+                                         const cfmm_subgraph_opts *opts /* NULL = defaults */,
+                                         cfmm_subgraph_out *out);
+int cfmm_execute_subgraph_swap_orders_rows(cfmm_ctx *ctx, int64_t q, const int64_t *token_in,
+                                           const int64_t *token_out, const uint8_t *kind,
+                                           const double *amount, const double *limit /* [q] or NULL */,
+                                           const int64_t *allow_off, const int64_t *allow_token,
+                                           const cfmm_subgraph_opts *opts, cfmm_subgraph_out *out);
+int cfmm_quote_basket_swap_orders_rows(cfmm_ctx *ctx, int64_t q, const int64_t *token_out /* [q] */,
+                                       const int64_t *basket_off /* [q+1] */,
+                                       const int64_t *basket_token /* [basket_off[q]] */,
+                                       const uint8_t *entry_kind /* [basket_off[q]] or NULL: every entry sold */,
+                                       const double *basket_amount /* [basket_off[q]] */,
+                                       const int64_t *allow_off /* [q+1] */,
+                                       const int64_t *allow_token /* [allow_off[q]] */,
+                                       const cfmm_subgraph_opts *opts /* NULL = defaults */,
+                                       cfmm_basket_out *out);
+int cfmm_execute_basket_swap_orders_rows(cfmm_ctx *ctx, int64_t q, const int64_t *token_out,
+                                         const int64_t *basket_off, const int64_t *basket_token,
+                                         const uint8_t *entry_kind, const double *basket_amount,
+                                         const double *limit /* [q] or NULL */, const int64_t *allow_off,
+                                         const int64_t *allow_token, const cfmm_subgraph_opts *opts,
+                                         cfmm_basket_out *out);
+int cfmm_quote_limit_orders_rows(cfmm_ctx *ctx, int64_t q, const int64_t *token_out /* [q] */,
+                                 const int64_t *basket_off /* [q+1] */,
+                                 const int64_t *basket_token /* [basket_off[q]] */,
+                                 const double *basket_amount /* [basket_off[q]] */,
+                                 const double *limit_price /* [basket_off[q]] */,
+                                 const int64_t *allow_off /* [q+1] */, const int64_t *allow_token /* [allow_off[q]] */,
+                                 const cfmm_subgraph_opts *opts /* NULL = defaults */, cfmm_limit_out *out);
+int cfmm_execute_limit_orders_rows(cfmm_ctx *ctx, int64_t q, const int64_t *token_out,
+                                   const int64_t *basket_off, const int64_t *basket_token,
+                                   const double *basket_amount, const double *limit_price,
+                                   const double *min_received /* [q] or NULL */, const int64_t *allow_off,
+                                   const int64_t *allow_token, const cfmm_subgraph_opts *opts,
+                                   cfmm_limit_out *out);
 
 /* ---- arbitrage against external prices over every pool among allowed tokens ----------------
  * A row values tokens at external prices c and trades through every pool among its priced tokens to
