@@ -800,7 +800,10 @@ int cfmm_find_order_paths(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [
  * CFMM_ORDER_NOT_CONVERGED, keeps its m_r and solver status, and its legs, paid and received read
  * 0.  A filled row has received = Ψ_i, paid = −Ψ_j (within rtol·δ of δ when ν_j is off its bound),
  * every intermediate's net Ψ_b >= −rtol·δ·ν_j/ν_b, and a duality gap of at most |T|·rtol·δ·ν_j plus
- * the box's √eps terms.  Amount 0 fills with zeros and runs no solve.
+ * the box's √eps terms.  Amount 0 fills with zeros and runs no solve.  Non-finite legs (a
+ * GeometricMean closed form that overflows): a line-search trial that meets one backs off and the
+ * row goes on, so it may still fill from finite iterates; a row whose committed iterate holds one
+ * (its reported Ψ or m_r not finite) ends CFMM_ORDER_NOT_CONVERGED, as in every row kind below.
  * Outputs (cfmm_subgraph_out; every pointer may be NULL):
  *   per row  paid, received, status (CFMM_ORDER_*), solver_status (−1 when no solve ran),
  *            iterations, fun_evals, merit (m_r; 0 without a solve);

@@ -49,9 +49,11 @@ def ladder(rng, price, depth):
 
 class PoolSet:
     """Pools given as (type, Ai, state) specs, split into a main set (orient_by_degree = 1) and
-    appended pools per type, some retired; the attributes test_gpu_split_orders' helpers read."""
+    appended pools per type, some retired; the attributes test_gpu_split_orders' helpers read.
+    keep_pairs: retire no pair's last active pool (a retire then never changes which pairs are active).
+    build: make the device context now (else p is None until fresh())."""
 
-    def __init__(self, cr, n, specs, seed, tail=0.2, retire=0.06):
+    def __init__(self, cr, n, specs, seed, tail=0.2, retire=0.06, keep_pairs=False, build=True):
         rng = np.random.default_rng(seed)
         self._cr, self.n = cr, n
         by = {t: [s for s in specs if s[0] == t] for t in (P, G, U)}
@@ -79,7 +81,12 @@ class PoolSet:
                 self.main[t] = tuple(x[:k] for x in data)
                 self.tail[t] = tuple(x[k:] for x in data)
         self.retired = {(t, int(i)) for t in (P, G, U) for i in range(self.m[t]) if rng.random() < retire}
-        self.p = self.fresh()
+        if keep_pairs:
+            by_pair = {}
+            for k in self.keys():
+                by_pair.setdefault(frozenset(int(x) for x in self.Ai[k[0]][k[1]]), []).append(k)
+            self.retired -= {ks[0] for ks in by_pair.values() if all(k in self.retired for k in ks)}
+        self.p = self.fresh() if build else None
 
     def fresh(self):
         kw = {("product", "geomean", "univ3")[t]: self.main[t] for t in (P, G, U) if self.mm[t]}
