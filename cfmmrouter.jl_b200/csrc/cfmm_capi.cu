@@ -44,6 +44,7 @@
 #include "arb_scan_kernels.cuh"
 #include "hub_kernels.cuh"
 #include "best_path_kernels.cuh"
+#include "token_value_kernels.cuh"
 #include "univ3_state.cuh"
 
 #include <cub/cub.cuh>
@@ -284,6 +285,9 @@ struct cfmm_ctx {
     DevBuf<int32_t> adj_nbr, adj_pair;   // [2·n_pairs]
     std::vector<int64_t> adj_off_host;
   } pairs;
+  // the workspace of cfmm_quote_token_values (token_value_kernels.cuh): grown on demand, holds
+  // nothing between calls
+  DevBuf<unsigned char> tv_ws;
   int64_t launches = 0;
   std::string err;
   cfmm::PeerExchange comm;
@@ -3820,7 +3824,207 @@ int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
   return CFMM_OK;
 }
 
+// ---- token values from one root over the whole pool graph (token_value_kernels.cuh) -------------
+
+// Every argument of cfmm_quote_token_values, before anything runs.
+int check_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint8_t* kind, const double* amount,
+                       int max_hops, const double* value, int64_t n_req, const int64_t* req_row,
+                       const int64_t* req_token, const int64_t* hop_off, const int* hop_type, const int64_t* hop_pool,
+                       const int64_t* hop_token) {
+  const char* what = "quote_token_values";
+  int rc = ready(ctx);
+  if (rc != CFMM_OK) return rc;
+  if (q < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: negative row count", what);
+  if (n_req < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: negative request count", what);
+  if (max_hops < 1 || max_hops > CFMM_PATH_MAX_HOPS)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: max_hops %d, not 1..%d", what, max_hops, CFMM_PATH_MAX_HOPS);
+  if (ctx->n_tokens > INT32_MAX || ctx->n_pools > INT32_MAX)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: more than 2^31 - 1 tokens or pools", what);
+  if (q == 0) return CFMM_OK;
+  if (!root || !kind || !amount || !value)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: null root, kind, amount or value", what);
+  for (int64_t r = 0; r < q; ++r) {
+    if (root[r] < 1 || root[r] > ctx->n_tokens)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: root %lld outside 1..%lld", what, (long long)r,
+                  (long long)root[r], (long long)ctx->n_tokens);
+    if (kind[r] > 1) return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: kind %d, not 0 or 1", what, (long long)r, kind[r]);
+    if (!(amount[r] > 0.0) || !std::isfinite(amount[r]))
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: amount %g, not finite and > 0", what, (long long)r, amount[r]);
+  }
+  if (n_req == 0) return CFMM_OK;
+  if (!req_row || !req_token || !hop_off || !hop_type || !hop_pool || !hop_token)
+    return fail(ctx, CFMM_ERR_INVALID, "%s: null req_row, req_token, hop_off, hop_type, hop_pool or hop_token", what);
+  for (int64_t j = 0; j < n_req; ++j) {
+    if (req_row[j] < 0 || req_row[j] >= q)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: request %lld: row %lld outside 0..%lld", what, (long long)j,
+                  (long long)req_row[j], (long long)(q - 1));
+    if (req_token[j] < 1 || req_token[j] > ctx->n_tokens)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: request %lld: token %lld outside 1..%lld", what, (long long)j,
+                  (long long)req_token[j], (long long)ctx->n_tokens);
+  }
+  return CFMM_OK;
+}
+
+// Per-row bytes of the token-value workspace: val, best, lvl and H levels of predecessors.
+size_t token_value_row_bytes(int64_t n, int H) {
+  return (size_t)n * (sizeof(double) + sizeof(unsigned __int128) + 1 + (size_t)H * sizeof(uint64_t));
+}
+constexpr size_t kTokenValueBudget = size_t(512) << 20;  // workspace bytes the rows of one group may take
+
+int quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint8_t* kind, const double* amount,
+                       int max_hops, const uint8_t* allowed, double* value, uint8_t* hops, uint8_t* status,
+                       int64_t* frontier, int64_t n_req, const int64_t* req_row, const int64_t* req_token,
+                       int64_t* hop_off, int* hop_type, int64_t* hop_pool, int64_t* hop_token, double* hop_tender,
+                       double* hop_received, uint8_t* req_status) {
+  int rc;
+  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
+  cudaStream_t st = ctx->stream;
+  OrderSets os;
+  if ((rc = order_sets(ctx, false, os)) != CFMM_OK) return rc;
+  const int64_t n = ctx->n_tokens;
+  const int H = max_hops;
+  cfmm::TvSets S{};
+  for (int k = 0; k < cfmm::kPathSets; ++k) {
+    const PoolSet& s = path_set(ctx, k);
+    S.start[k + 1] = S.start[k] + (s.m > 0 ? s.m_padded : 0);
+  }
+  const int64_t positions = S.start[cfmm::kPathSets];
+  // the group: up to kTvMaxGroup rows, as many as the budget holds (at least one)
+  const size_t row_bytes = token_value_row_bytes(n, H);
+  const int G = (int)std::max<int64_t>(
+      1, std::min<int64_t>({q, (int64_t)cfmm::kTvMaxGroup, (int64_t)(kTokenValueBudget / row_bytes)}));
+  // workspace: [G][n] best (16-byte slots first), val, [G][H][n] pred, [2][n] fmask, [G][H+1] cnt,
+  // [H+1] tot, [G][n] lvl; kept on the context and grown when a call needs more
+  const size_t gn = (size_t)G * (size_t)n;
+  const size_t b_best = 0, b_val = b_best + gn * 16, b_pred = b_val + gn * 8, b_fmask = b_pred + gn * H * 8,
+               b_cnt = b_fmask + 2 * (size_t)n * 8, b_tot = b_cnt + (size_t)G * (H + 1) * 4,
+               b_lvl = (b_tot + (size_t)(H + 1) * 4 + 15) & ~(size_t)15, b_end = b_lvl + gn;
+  if (ctx->tv_ws.n < b_end) CU_TRY(ctx, ctx->tv_ws.alloc(b_end));
+  unsigned char* ws = ctx->tv_ws.p;
+  DevBuf<int64_t> d_root, d_req_row, d_req_tok, d_entry, d_pos, d_token;
+  DevBuf<uint8_t> d_kind, d_allowed, d_hops, d_status, d_set, d_tok1, d_rstatus;
+  DevBuf<double> d_amount, d_value, d_tender, d_recv;
+  DevBuf<int32_t> d_nhop;
+  CU_TRY(ctx, d_root.upload(root, (size_t)q));
+  CU_TRY(ctx, d_kind.upload(kind, (size_t)q));
+  CU_TRY(ctx, d_amount.upload(amount, (size_t)q));
+  CU_TRY(ctx, d_allowed.upload(allowed, (size_t)n));
+  CU_TRY(ctx, d_value.alloc(gn));
+  CU_TRY(ctx, d_hops.alloc(gn));
+  CU_TRY(ctx, d_status.alloc(gn));
+  const size_t slots = (size_t)n_req * (size_t)H;
+  if (n_req > 0) {
+    CU_TRY(ctx, d_req_row.upload(req_row, (size_t)n_req));
+    CU_TRY(ctx, d_req_tok.upload(req_token, (size_t)n_req));
+    CU_TRY(ctx, d_entry.alloc((size_t)std::max<int64_t>(ctx->n_pools, 1)));
+    CU_TRY(ctx, d_nhop.alloc((size_t)n_req));
+    CU_TRY(ctx, d_rstatus.alloc((size_t)n_req));
+    CU_TRY(ctx, d_set.alloc(slots));
+    CU_TRY(ctx, d_pos.alloc(slots));
+    CU_TRY(ctx, d_tok1.alloc(slots));
+    CU_TRY(ctx, d_token.alloc(slots));
+    CU_TRY(ctx, d_tender.alloc(slots));
+    CU_TRY(ctx, d_recv.alloc(slots));
+    if ((rc = launch(ctx, kProfSwaps, 1, [&] {
+           if (positions > 0)
+             cfmm::tv_entry_kernel<<<(unsigned)((positions + 255) / 256), 256, 0, st>>>(os.d_P.p, S, d_entry.p);
+         })) != CFMM_OK)
+      return rc;
+  }
+  std::vector<int32_t> cnt((size_t)G * (H + 1));
+  const unsigned tok_grid = (unsigned)((n + cfmm::kTvThreads - 1) / cfmm::kTvThreads);
+  const unsigned pool_grid = (unsigned)((positions + cfmm::kTvThreads - 1) / cfmm::kTvThreads);
+  for (int64_t r0 = 0; r0 < q; r0 += G) {
+    const int g = (int)std::min<int64_t>(G, q - r0);
+    const size_t gn_g = (size_t)g * (size_t)n;
+    cfmm::TvWork W{d_root.p + r0,
+                   d_kind.p + r0,
+                   d_amount.p + r0,
+                   allowed ? d_allowed.p : nullptr,
+                   g,
+                   H,
+                   n,
+                   reinterpret_cast<double*>(ws + b_val),
+                   reinterpret_cast<unsigned __int128*>(ws + b_best),
+                   ws + b_lvl,
+                   reinterpret_cast<uint64_t*>(ws + b_pred),
+                   reinterpret_cast<uint64_t*>(ws + b_fmask),
+                   reinterpret_cast<int32_t*>(ws + b_cnt),
+                   reinterpret_cast<int32_t*>(ws + b_tot)};
+    bool any_req = false;
+    for (int64_t j = 0; j < n_req && !any_req; ++j) any_req = req_row[j] >= r0 && req_row[j] < r0 + g;
+    if ((rc = launch(ctx, kProfSwaps, 2 + (pool_grid > 0 ? 2 : 1) * H + (any_req ? 1 : 0), [&] {
+           cfmm::tv_init_kernel<<<tok_grid, cfmm::kTvThreads, 0, st>>>(W);
+           for (int h = 1; h <= H; ++h) {
+             if (pool_grid > 0) cfmm::tv_relax_kernel<<<pool_grid, cfmm::kTvThreads, 0, st>>>(os.d_P.p, S, W, h);
+             cfmm::tv_finalize_kernel<<<tok_grid, cfmm::kTvThreads, 0, st>>>(W, h);
+           }
+           cfmm::tv_rebuild_kernel<<<(unsigned)((gn_g + 255) / 256), 256, 0, st>>>(W, d_value.p, d_hops.p, d_status.p);
+           if (any_req)
+             cfmm::tv_path_kernel<<<(unsigned)((n_req + 127) / 128), 128, 0, st>>>(
+                 os.d_P.p, W, r0, d_entry.p, n_req, d_req_row.p, d_req_tok.p, d_nhop.p, d_set.p, d_pos.p, d_tok1.p,
+                 d_token.p, d_tender.p, d_recv.p, d_rstatus.p);
+         })) != CFMM_OK)
+      return rc;
+    CU_TRY(ctx, read_back(ctx, value + r0 * n, d_value.p, gn_g));
+    CU_TRY(ctx, read_back(ctx, hops ? hops + r0 * n : nullptr, d_hops.p, gn_g));
+    CU_TRY(ctx, read_back(ctx, status ? status + r0 * n : nullptr, d_status.p, gn_g));
+    CU_TRY(ctx, read_back(ctx, frontier ? cnt.data() : nullptr, W.cnt, (size_t)g * (H + 1)));
+    CU_TRY(ctx, cudaStreamSynchronize(st));
+    if (frontier)
+      for (int r = 0; r < g; ++r)
+        for (int h = 1; h <= H; ++h) frontier[(r0 + r) * H + h - 1] = cnt[(size_t)r * (H + 1) + h];
+  }
+  if (n_req == 0) return CFMM_OK;
+  std::vector<int32_t> nhop((size_t)n_req);
+  std::vector<uint8_t> set(slots);
+  std::vector<int64_t> pos(slots), token(slots);
+  std::vector<double> tender(hop_tender ? slots : 0), recv(hop_received ? slots : 0);
+  CU_TRY(ctx, read_back(ctx, nhop.data(), d_nhop.p, (size_t)n_req));
+  CU_TRY(ctx, read_back(ctx, set.data(), d_set.p, slots));
+  CU_TRY(ctx, read_back(ctx, pos.data(), d_pos.p, slots));
+  CU_TRY(ctx, read_back(ctx, token.data(), d_token.p, slots));
+  CU_TRY(ctx, read_back(ctx, hop_tender ? tender.data() : nullptr, d_tender.p, slots));
+  CU_TRY(ctx, read_back(ctx, hop_received ? recv.data() : nullptr, d_recv.p, slots));
+  CU_TRY(ctx, read_back(ctx, req_status, d_rstatus.p, (size_t)n_req));
+  CU_TRY(ctx, cudaStreamSynchronize(st));
+  // pack each request's first nhop[j] slots, pools as cfmm_pair_pools reports them (find_order_paths)
+  hop_off[0] = 0;
+  for (int64_t j = 0; j < n_req; ++j) {
+    const int64_t g = hop_off[j];
+    for (int64_t h = 0; h < nhop[(size_t)j]; ++h) {
+      const size_t w = (size_t)(H * j + h);
+      const int k = set[w];
+      hop_type[g + h] = k >> 1;
+      hop_pool[g + h] = path_set(ctx, k).order[(size_t)pos[w]] + ((k & 1) ? ctx->sets[k >> 1].m : 0);
+      hop_token[g + h] = token[w];
+      if (hop_tender) hop_tender[g + h] = tender[w];
+      if (hop_received) hop_received[g + h] = recv[w];
+    }
+    hop_off[j + 1] = g + nhop[(size_t)j];
+  }
+  return CFMM_OK;
+}
+
 }  // namespace
+
+int cfmm_quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint8_t* kind, const double* amount,
+                            int max_hops, const uint8_t* allowed, double* value, uint8_t* hops, uint8_t* status,
+                            int64_t* frontier, int64_t n_req, const int64_t* req_row, const int64_t* req_token,
+                            int64_t* hop_off, int* hop_type, int64_t* hop_pool, int64_t* hop_token,
+                            double* hop_tender, double* hop_received, uint8_t* req_status) {
+  int rc = check_token_values(ctx, q, root, kind, amount, max_hops, value, n_req, req_row, req_token, hop_off,
+                              hop_type, hop_pool, hop_token);
+  if (rc != CFMM_OK) return rc;
+  if (q == 0) {
+    if (hop_off) hop_off[0] = 0;
+    return CFMM_OK;
+  }
+  return quote_token_values(ctx, q, root, kind, amount, max_hops, allowed, value, hops, status, frontier, n_req,
+                            req_row, req_token, hop_off, hop_type, hop_pool, hop_token, hop_tender, hop_received,
+                            req_status);
+}
 
 int cfmm_pair_pools(cfmm_ctx* ctx, int64_t q, const int64_t* token_a, const int64_t* token_b, int64_t* count,
                     int64_t cap, int* type_out, int64_t* pool_out, uint8_t* active_out) {

@@ -613,6 +613,36 @@ function find_order_paths(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}
     return hop_off, typ[1:n], pool[1:n], tok[1:n], tender[1:n], received[1:n], value, status
 end
 
+# Every token's value against each row's root (cfmm_quote_token_values): kind 0 spends amount[r] of
+# root[r], kind 1 receives amount[r] of it; the best walk of at most max_hops (1..8) hops to (kind 0) or
+# from (kind 1) every token through tokens t with allowed[t] != 0 (nothing: every token).  value, hops
+# and status are n_tokens x q (column r is row r); frontier is max_hops x q, the tokens changed per
+# level.  req_row (0-based) / req_token (1-based) name the walks to return, as quote_paths /
+# execute_paths! take them.  Never executed, like the rest of this file.
+function quote_token_values(ctx, n_tokens::Integer, root::Vector{Int64}, kind::Vector{UInt8},
+                            amount::Vector{Float64}, max_hops::Integer, allowed=nothing;
+                            req_row::Vector{Int64}=Int64[], req_token::Vector{Int64}=Int64[])
+    q, k = length(root), length(req_row)
+    length(kind) == length(amount) == q || throw(ArgumentError("root / kind / amount need q entries"))
+    length(req_token) == k || throw(ArgumentError("req_row / req_token need one entry per request"))
+    value, hops, status = zeros(n_tokens, q), zeros(UInt8, n_tokens, q), zeros(UInt8, n_tokens, q)
+    frontier = zeros(Int64, max_hops, q)
+    cap = max(k * max_hops, 1)
+    hop_off, typ, pool, tok = zeros(Int64, k + 1), zeros(Cint, cap), zeros(Int64, cap), zeros(Int64, cap)
+    tender, received, req_status = zeros(cap), zeros(cap), zeros(UInt8, max(k, 1))
+    mask = allowed === nothing ? C_NULL : Vector{UInt8}(allowed)
+    chk(ctx, ccall((:cfmm_quote_token_values, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Cint, Ptr{UInt8}, Ptr{Float64}, Ptr{UInt8},
+         Ptr{UInt8}, Ptr{Int64}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Cint}, Ptr{Int64}, Ptr{Int64},
+         Ptr{Float64}, Ptr{Float64}, Ptr{UInt8}),
+        ctx, q, root, kind, amount, max_hops, mask, value, hops, status, frontier, k, req_row, req_token,
+        hop_off, typ, pool, tok, tender, received, req_status))
+    n = hop_off[end]
+    return (value=value, hops=hops, status=status, frontier=frontier, hop_off=hop_off, hop_type=typ[1:n],
+            hop_pool=pool[1:n], hop_token=tok[1:n], hop_tender=tender[1:n], hop_received=received[1:n],
+            req_status=req_status[1:k])
+end
+
 # Orders over every pool among allowed tokens (cfmm_quote_subgraph_swap_orders /
 # cfmm_execute_subgraph_swap_orders): row r sells amount[r] of token_in[r] for token_out[r] (kind 0,
 # exact-in) or buys amount[r] of token_out[r] paying in token_in[r] (kind 1, exact-out) over every pool

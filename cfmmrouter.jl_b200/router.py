@@ -826,6 +826,53 @@ class DevicePools:
         return (hop_off, typ[:n].copy(), pool[:n].copy(), tok[:n].copy(), tender[:n].copy(), received[:n].copy(),
                 value, status)
 
+    # -- token values against one root (include/cfmm_b200.h, cfmm_quote_token_values) -------------
+    def quote_token_values(self, root, kind, amount, max_hops: int, allowed=None, requests=None):
+        """cfmm_quote_token_values: for row r (root[r] 1-based; kind 0 spends amount[r] of the root,
+        kind 1 receives amount[r] of it) the best walk of at most max_hops (1..8) hops between the root
+        and every token, through tokens t with allowed[t - 1] (a mask [n_tokens]; None: every token).
+        No state changes.  Returns (value [q, n_tokens], hops [q, n_tokens] uint8, status [q, n_tokens]
+        uint8, frontier [q, max_hops]: the tokens changed per level); with requests = (rows [k] 0-based,
+        tokens [k] 1-based) also (hop_off [k + 1], hop_type, hop_pool, hop_token, hop_tender,
+        hop_received, req_status [k]), the walks as quote_paths / execute_paths take them (exact-in
+        from the root, exact-out into it)."""
+        root = np.ascontiguousarray(root, dtype=np.int64).reshape(-1)
+        kind = np.ascontiguousarray(kind, dtype=np.uint8).reshape(-1)
+        amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
+        q, n, H = len(root), self.n_tokens, int(max_hops)
+        if not (len(kind) == len(amount) == q):
+            raise ValueError("quote_token_values: root, kind and amount need one entry per row")
+        u8, i32 = C.POINTER(C.c_uint8), C.POINTER(C.c_int)
+        mask = None
+        if allowed is not None:
+            mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
+            if len(mask) != n:
+                raise ValueError(f"quote_token_values: allowed must have {n} entries, one per token")
+        rows = toks = np.zeros(0, dtype=np.int64)
+        if requests is not None:
+            rows = np.ascontiguousarray(requests[0], dtype=np.int64).reshape(-1)
+            toks = np.ascontiguousarray(requests[1], dtype=np.int64).reshape(-1)
+            if len(rows) != len(toks):
+                raise ValueError("quote_token_values: requests need one row per token")
+        k = len(rows)
+        value = np.zeros((q, n))
+        hops, status = np.zeros((q, n), dtype=np.uint8), np.zeros((q, n), dtype=np.uint8)
+        frontier = np.zeros((q, max(H, 0)), dtype=np.int64)
+        cap = max(k * max(H, 0), 1)
+        hop_off = np.zeros(k + 1, dtype=np.int64)
+        typ, pool, tok = np.zeros(cap, dtype=np.int32), np.zeros(cap, dtype=np.int64), np.zeros(cap, dtype=np.int64)
+        tender, received, rstatus = np.zeros(cap), np.zeros(cap), np.zeros(max(k, 1), dtype=np.uint8)
+        self._chk(self._lib.cfmm_quote_token_values(
+            self._ctx, q, _ip(root), kind.ctypes.data_as(u8), _dp(amount), H,
+            None if mask is None else mask.ctypes.data_as(u8), _dp(value), hops.ctypes.data_as(u8),
+            status.ctypes.data_as(u8), _ip(frontier), k, _ip(rows), _ip(toks), _ip(hop_off),
+            typ.ctypes.data_as(i32), _ip(pool), _ip(tok), _dp(tender), _dp(received), rstatus.ctypes.data_as(u8)))
+        if requests is None:
+            return value, hops, status, frontier
+        m = int(hop_off[-1])
+        return (value, hops, status, frontier, hop_off, typ[:m].copy(), pool[:m].copy(), tok[:m].copy(),
+                tender[:m].copy(), received[:m].copy(), rstatus[:k].copy())
+
     # -- orders over every pool among allowed tokens (include/cfmm_b200.h,
     #    cfmm_quote_subgraph_swap_orders / cfmm_execute_subgraph_swap_orders) ------------------------
     def _subgraph(self, execute, token_in, token_out, amount, allowed, limit, opts, kind=None):
@@ -1654,6 +1701,39 @@ class Router:
                                                None if limits is None else limits[rows])
             paid[rows], got[rows], status[rows] = p, g, s
         return paid, got, status, paths
+
+    def quote_token_values(self, roots, kinds, amounts, max_hops: int = _lib.PATH_MAX_HOPS, allowed=None):
+        """Value every token against each row's root on the device (cfmm_quote_token_values): kind 0
+        rows spend amounts[r] of roots[r] (1-based) and get, per token, the most of it that a walk of at
+        most max_hops hops delivers; kind 1 rows receive amounts[r] of the root and get, per token, the
+        least of it that such a walk must be paid.  Walks pass through tokens t with allowed[t - 1] (a
+        mask over the tokens; None: every token), one pool per hop.  No state changes.  Returns (value,
+        hops, status), each [q, n_tokens]: value 0 (kind 0) or inf (kind 1) where no walk reaches.
+        Single GPU."""
+        if self._world > 1:
+            raise NotImplementedError("quote_token_values drives one GPU")
+        if not 1 <= int(max_hops) <= _lib.PATH_MAX_HOPS:
+            raise ValueError(f"quote_token_values: max_hops must be 1..{_lib.PATH_MAX_HOPS}")
+        return self._pools.quote_token_values(roots, kinds, amounts, int(max_hops), allowed)[:3]
+
+    def token_paths(self, root, kind, amount, tokens, max_hops: int = _lib.PATH_MAX_HOPS, allowed=None):
+        """The walks behind quote_token_values for one root and the given tokens (1-based): kind 0
+        from the root to each token, kind 1 from each token into the root.  Returns (paths, token_in,
+        value, status): paths[j] lists r.cfmms positions in hop order (empty for the root, an unreached
+        token or a walk that repeats a pool), ready for quote_paths / execute_paths with token_in[j]
+        and the same kind and amount; value[j] the token's value.  No state changes.  Single GPU."""
+        if self._world > 1:
+            raise NotImplementedError("token_paths drives one GPU")
+        if not 1 <= int(max_hops) <= _lib.PATH_MAX_HOPS:
+            raise ValueError(f"token_paths: max_hops must be 1..{_lib.PATH_MAX_HOPS}")
+        tokens = np.asarray(tokens, dtype=np.int64).reshape(-1)
+        got = self._pools.quote_token_values([root], [kind], [amount], int(max_hops), allowed,
+                                             (np.zeros(len(tokens), dtype=np.int64), tokens))
+        value, off, typ, pool, st = got[0], got[4], got[5], got[6], got[10]
+        paths = [[self._type_lists[int(typ[h])][int(pool[h])] for h in range(off[j], off[j + 1])]
+                 for j in range(len(tokens))]
+        token_in = tokens.copy() if int(kind) == 1 else np.full(len(tokens), int(root), dtype=np.int64)
+        return paths, token_in, value[0, tokens - 1], st
 
     def _subgraph_args(self, token_in, token_out, amounts, allowed, limits, what):
         tin, tout, _, amounts, limits = self._split_args(token_in, token_out, np.zeros(len(np.atleast_1d(token_in))),

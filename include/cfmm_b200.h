@@ -762,6 +762,84 @@ int cfmm_find_order_paths(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [
                           double *hop_received /* [q·max_hops] or NULL */, double *value /* [q] or NULL */,
                           uint8_t *status /* [q] or NULL */);
 
+/* ---- every token's value against one root over the whole pool graph -------------------------
+ * For each row r (a root S = root[r], 1-based; kind[r]; amount[r] finite and > 0), the best walk of at
+ * most H = max_hops (1..CFMM_PATH_MAX_HOPS) hops between S and every token, one pool per hop: what
+ * each token is worth in S at this size, as an executable path.  No cap on the tokens.
+ *   allowed     a mask [n_tokens] (NULL: every token); only allowed tokens are reached.  The root is
+ *               always allowed, is never a destination and so appears only at one end of a walk;
+ *               every other token may repeat.
+ *   hops        a hop u → v uses one active pool of {u, v}: the pools cfmm_find_order_paths uses (all
+ *               three types, appended pools included, a pool stored with its tokens exchanged mapped
+ *               back, retired pools skipped).  f_k and x*_k are cfmm_quote_swaps /
+ *               cfmm_quote_swaps_exact_out bit for bit, on the state at this call.
+ *   exact-in    (CFMM_SWAP_EXACT_IN, "spend δ = amount of S: how much of each token t") a₀(S) = δ,
+ *               every other token unreached (0).  For h = 1 … H and allowed t != S the candidates are
+ *               f_k(a_{h−1}(u)) over every reached u and every active pool k of {u, t} with u
+ *               tendered; a candidate counts only when it is > 0 (NaNs are ignored).  a_h(t) is the
+ *               best candidate when it is strictly greater than a_{h−1}(t), else a_{h−1}(t).
+ *   exact-out   (CFMM_SWAP_EXACT_OUT, "receive y = amount of S: how much of each token t must be
+ *               paid") the mirror image, backwards from S: c₀(S) = y, every other token unreached
+ *               (+inf); the candidates for u are x*_k(c_{h−1}(v)) over reached v and the active pools
+ *               k of {u, v} with u tendered, kept when finite; c_h(u) is the best when strictly
+ *               smaller than c_{h−1}(u).
+ *   ranking     by the amount (larger exact-in, smaller exact-out), then the smaller neighbour token
+ *               (u exact-in, v exact-out), then the smaller global insertion index of the pool (within
+ *               a pair, the order of its cfmm_pair_pools list): cfmm_find_order_paths' ranking without
+ *               its "fewer hops" key.  Every candidate that can win at level h comes from a token that
+ *               changed at level h−1, so it has exactly h hops: a candidate from an unchanged token
+ *               repeats one of an earlier level, which the target's value already matches or beats,
+ *               and cannot be strictly better.  The result therefore depends neither on the order the
+ *               candidates are evaluated in nor on whether unchanged tokens are skipped; the device
+ *               skips them (a level relaxes only the pools of the previous level's changed tokens)
+ *               and stops once no token changed.
+ *   against cfmm_find_order_paths  On a graph without gaining cycles through allowed tokens (every
+ *               pool's marginal price agrees with one price vector, fees > 0) the value and walk of
+ *               (S, t) are cfmm_find_order_paths(S, t, allowed, H)'s.  With a gaining cycle the two may
+ *               differ: here t is also an intermediate of other walks and keeps the value the cycle
+ *               gives it, where cfmm_find_order_paths never passes through its destination.
+ * Outputs per (row, token), row-major [q·n_tokens]:
+ *   value       a_H(t) exact-in (0 unreached), c_H(t) exact-out (+inf unreached); the root holds the
+ *               row's amount.
+ *   hops        (NULL: not written) the length of the best walk; 0 for the root and unreached tokens.
+ *   status      (NULL: not written) CFMM_ORDER_FILLED: reached, and the walk uses distinct pools (the
+ *               root: 0 hops); CFMM_ORDER_UNREACHABLE; CFMM_PATH_REPEATS_POOL: the best walk holds a
+ *               gaining cycle through one pool twice, value still the DP's amount (as
+ *               cfmm_find_order_paths' DP).
+ * frontier [q·max_hops] (NULL: not written): the tokens whose value changed at level h = 1 … H.  A
+ * row whose entry for h = H is 0 has converged: more hops would change nothing.
+ * Paths on request: the n_req pairs (req_row[j] 0-based, req_token[j] 1-based) get their walks as
+ * cfmm_execute_paths takes them, packed CSR: hop_off [n_req+1] (hop_off[0] = 0; at most
+ * n_req·max_hops hops), hop_type / hop_pool (a pool as cfmm_quote_paths addresses it), hop_token (the
+ * token each hop delivers, 1-based), hop_tender / hop_received (NULL: not written), and req_status
+ * [n_req] (NULL: not written) as status above.  Exact-in walks run root → t (token_in = the root),
+ * exact-out walks t → root (token_in = t).  The amounts are cfmm_quote_paths' on that CSR bit for bit
+ * (the walk is priced by its code), and the path's end amount is value.  The root itself gives 0 hops
+ * and FILLED; an unreached or REPEATS_POOL request gives no hops.
+ * Rows run in groups sized to a workspace kept on the context (freed with it); a row's outputs do not
+ * depend on the other rows of the call or their order.
+ *
+ * Synchronous; changes no state.  Single GPU.  Before cfmm_finalize: CFMM_ERR_STATE.  CFMM_ERR_INVALID
+ * before anything runs for q < 0, n_req < 0, a root outside 1..n_tokens, a kind other than 0 or 1, an
+ * amount that is NaN, infinite, 0 or negative, max_hops outside 1..CFMM_PATH_MAX_HOPS, a request row
+ * outside 0..q−1 or token outside 1..n_tokens, a null root, kind, amount or value with q > 0, and a
+ * null req_row, req_token, hop_off, hop_type, hop_pool or hop_token with n_req > 0.  q == 0 writes
+ * hop_off[0] = 0 (when given) and runs nothing. */
+int cfmm_quote_token_values(cfmm_ctx *ctx, int64_t q, const int64_t *root /* [q] */,
+                            const uint8_t *kind /* [q] */, const double *amount /* [q] */,
+                            int max_hops /* 1..CFMM_PATH_MAX_HOPS */,
+                            const uint8_t *allowed /* [n_tokens] or NULL */,
+                            double *value /* [q·n_tokens] */, uint8_t *hops /* [q·n_tokens] or NULL */,
+                            uint8_t *status /* [q·n_tokens] or NULL */,
+                            int64_t *frontier /* [q·max_hops] or NULL */, int64_t n_req,
+                            const int64_t *req_row /* [n_req] */, const int64_t *req_token /* [n_req] */,
+                            int64_t *hop_off /* [n_req+1] */, int *hop_type /* [n_req·max_hops] */,
+                            int64_t *hop_pool /* [n_req·max_hops] */,
+                            int64_t *hop_token /* [n_req·max_hops] */,
+                            double *hop_tender /* [n_req·max_hops] or NULL */,
+                            double *hop_received /* [n_req·max_hops] or NULL */,
+                            uint8_t *req_status /* [n_req] or NULL */);
+
 /* ---- orders routed over every pool among their allowed tokens ------------------------------
  * A row sells δ = amount[r] of j = token_in[r] for i = token_out[r] (1-based, distinct; exact-in:
  * exact-out rows are below) over every pool among j, i and the allowed tokens, split optimally: route! with
@@ -1432,8 +1510,8 @@ int64_t cfmm_launch_count(const cfmm_ctx *ctx);
  * cfmm_quote_swaps_exact_out / cfmm_execute_swap_orders / cfmm_quote_paths /
  * cfmm_execute_paths / cfmm_pair_pools / cfmm_quote_split_orders /
  * cfmm_execute_split_orders / cfmm_quote_routed_orders / cfmm_execute_routed_orders /
- * cfmm_choose_order_hubs / cfmm_find_order_paths, the pair-index build counted as one
- * launch); it
+ * cfmm_choose_order_hubs / cfmm_find_order_paths / cfmm_quote_token_values, the pair-index
+ * build counted as one launch); it
  * synchronises on the recorded events.
  * cfmm_profile_reset re-arms the same N pairs. */
 int cfmm_profile_read(cfmm_ctx *ctx, int type, double *total_ms, int64_t *launches);
