@@ -151,6 +151,13 @@ SYMBOLS = {
                                           C.POINTER(C.c_uint8), _dp, C.POINTER(C.c_uint8), C.POINTER(C.c_uint8), _ip,
                                           C.c_int64, _ip, _ip, _ip, C.POINTER(C.c_int), _ip, _ip, _dp, _dp,
                                           C.POINTER(C.c_uint8)]),
+    "cfmm_find_order_paths_net": (C.c_int, [_ctx, C.c_int64, _ip, _ip, C.POINTER(C.c_uint8), _dp, C.c_int,
+                                            C.POINTER(C.c_uint8), _dp, _ip, C.POINTER(C.c_int), _ip, _ip, _dp, _dp,
+                                            _dp, C.POINTER(C.c_uint8), _dp]),
+    "cfmm_quote_token_values_net": (C.c_int, [_ctx, C.c_int64, _ip, C.POINTER(C.c_uint8), _dp, C.c_int,
+                                              C.POINTER(C.c_uint8), _dp, _dp, C.POINTER(C.c_uint8),
+                                              C.POINTER(C.c_uint8), _dp, _ip, C.c_int64, _ip, _ip, _ip,
+                                              C.POINTER(C.c_int), _ip, _ip, _dp, _dp, C.POINTER(C.c_uint8)]),
     "cfmm_quote_subgraph_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _dp, C.POINTER(C.c_uint8),
                                              C.POINTER(SubgraphOpts), C.POINTER(SubgraphOut)]),
     "cfmm_execute_subgraph_orders": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _dp, _dp, C.POINTER(C.c_uint8),

@@ -3714,8 +3714,8 @@ int64_t count_allowed(const cfmm_ctx* ctx, const uint8_t* allowed) {
 // mask (required) and each row's |B| (the allowed tokens other than its two), and the CSR outputs.
 int check_find_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
                      const uint8_t* kind, const double* amount, int max_hops, const uint8_t* allowed,
-                     const int64_t* hop_off, const int* hop_type, const int64_t* hop_pool, const int64_t* hop_token) {
-  const char* what = "find_order_paths";
+                     const int64_t* hop_off, const int* hop_type, const int64_t* hop_pool, const int64_t* hop_token,
+                     const char* what = "find_order_paths") {
   int rc = check_split(ctx, q, token_in, token_out, kind, amount, nullptr, what);
   if (rc != CFMM_OK) return rc;
   if (max_hops < 1 || max_hops > CFMM_PATH_MAX_HOPS)
@@ -3734,10 +3734,21 @@ int check_find_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
   return CFMM_OK;
 }
 
+// The per-hop costs of the _net calls: n of them, each >= 0 (+inf allowed), before anything runs.
+int check_hop_cost(cfmm_ctx* ctx, const double* hop_cost, int64_t n, const char* what) {
+  if (n > 0 && !hop_cost) return fail(ctx, CFMM_ERR_INVALID, "%s: null hop_cost", what);
+  for (int64_t k = 0; k < n; ++k)
+    if (!(hop_cost[k] >= 0.0))
+      return fail(ctx, CFMM_ERR_INVALID, "%s: hop_cost[%lld] %g, not >= 0", what, (long long)k, hop_cost[k]);
+  return CFMM_OK;
+}
+
+// hop_cost (cfmm_find_order_paths_net): the best filled max_hops = L result net of hop_cost[r] per
+// hop, its net into net (NULL: not written); null: cfmm_find_order_paths.
 int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out, const uint8_t* kind,
                      const double* amount, int max_hops, const uint8_t* allowed, int64_t* hop_off, int* hop_type,
                      int64_t* hop_pool, int64_t* hop_token, double* hop_tender, double* hop_received, double* value,
-                     uint8_t* status) {
+                     uint8_t* status, const double* hop_cost = nullptr, double* net = nullptr) {
   int rc;
   CU_TRY(ctx, cudaSetDevice(ctx->device));
   if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
@@ -3759,7 +3770,7 @@ int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
   DevBuf<int32_t> d_tok, d_slot, d_deg, d_gpair, d_nhop;
   DevBuf<int16_t> d_gnbr;
   DevBuf<uint8_t> d_kind, d_set, d_tok1, d_status;
-  DevBuf<double> d_amount, d_tender, d_recv, d_value;
+  DevBuf<double> d_amount, d_tender, d_recv, d_value, d_cost, d_net;
   CU_TRY(ctx, d_in.upload(token_in, (size_t)q));
   CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
   CU_TRY(ctx, d_kind.upload(kind, (size_t)q));
@@ -3778,8 +3789,14 @@ int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
   CU_TRY(ctx, d_recv.alloc(slots));
   CU_TRY(ctx, d_value.alloc((size_t)q));
   CU_TRY(ctx, d_status.alloc((size_t)q));
+  if (hop_cost) {
+    CU_TRY(ctx, d_cost.upload(hop_cost, (size_t)q));
+    CU_TRY(ctx, d_net.alloc((size_t)q));
+  }
   const size_t smem = cfmm::best_path_smem(nB, H);
-  CU_TRY(ctx, cudaFuncSetAttribute(cfmm::best_path_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CU_TRY(ctx, cudaFuncSetAttribute(hop_cost ? reinterpret_cast<const void*>(cfmm::best_path_net_kernel)
+                                            : reinterpret_cast<const void*>(cfmm::best_path_kernel),
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const cfmm::PairIndexView pv{ix.off.p, ix.pool.p};
   const cfmm::AdjView A{ix.adj_off.p, ix.adj_nbr.p, ix.adj_pair.p};
   const cfmm::BestPathGraph G{d_tok.p, d_slot.p, d_deg.p, d_gnbr.p, d_gpair.p, nB};
@@ -3787,9 +3804,14 @@ int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
          if (nB > 0)
            cfmm::best_path_graph_kernel<<<(unsigned)((32 * (int64_t)nB + 255) / 256), 256, 0, st>>>(
                A, d_tok.p, d_slot.p, nB, d_deg.p, d_gnbr.p, d_gpair.p);
-         cfmm::best_path_kernel<<<(unsigned)q, cfmm::kBestPathThreads, smem, st>>>(
-             os.d_P.p, pv, A, G, d_in.p, d_out.p, d_kind.p, d_amount.p, H, d_nhop.p, d_set.p, d_pos.p, d_tok1.p,
-             d_token.p, d_tender.p, d_recv.p, d_value.p, d_status.p);
+         if (hop_cost)
+           cfmm::best_path_net_kernel<<<(unsigned)q, cfmm::kBestPathThreads, smem, st>>>(
+               os.d_P.p, pv, A, G, d_in.p, d_out.p, d_kind.p, d_amount.p, H, d_nhop.p, d_set.p, d_pos.p, d_tok1.p,
+               d_token.p, d_tender.p, d_recv.p, d_value.p, d_status.p, d_cost.p, d_net.p);
+         else
+           cfmm::best_path_kernel<<<(unsigned)q, cfmm::kBestPathThreads, smem, st>>>(
+               os.d_P.p, pv, A, G, d_in.p, d_out.p, d_kind.p, d_amount.p, H, d_nhop.p, d_set.p, d_pos.p, d_tok1.p,
+               d_token.p, d_tender.p, d_recv.p, d_value.p, d_status.p);
        })) != CFMM_OK)
     return rc;
   std::vector<int32_t> nhop((size_t)q);
@@ -3804,6 +3826,7 @@ int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
   CU_TRY(ctx, read_back(ctx, hop_received ? recv.data() : nullptr, d_recv.p, slots));
   CU_TRY(ctx, read_back(ctx, value, d_value.p, (size_t)q));
   CU_TRY(ctx, read_back(ctx, status, d_status.p, (size_t)q));
+  CU_TRY(ctx, read_back(ctx, hop_cost ? net : nullptr, d_net.p, (size_t)q));
   CU_TRY(ctx, cudaStreamSynchronize(st));
   // pack each row's first nhop[r] slots; (set, device position) -> (type, index in the type's
   // insertion order), as cfmm_pair_pools reports a pool
@@ -3830,8 +3853,7 @@ int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
 int check_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint8_t* kind, const double* amount,
                        int max_hops, const double* value, int64_t n_req, const int64_t* req_row,
                        const int64_t* req_token, const int64_t* hop_off, const int* hop_type, const int64_t* hop_pool,
-                       const int64_t* hop_token) {
-  const char* what = "quote_token_values";
+                       const int64_t* hop_token, const char* what = "quote_token_values") {
   int rc = ready(ctx);
   if (rc != CFMM_OK) return rc;
   if (q < 0) return fail(ctx, CFMM_ERR_INVALID, "%s: negative row count", what);
@@ -3865,17 +3887,22 @@ int check_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint
   return CFMM_OK;
 }
 
-// Per-row bytes of the token-value workspace: val, best, lvl and H levels of predecessors.
-size_t token_value_row_bytes(int64_t n, int H) {
-  return (size_t)n * (sizeof(double) + sizeof(unsigned __int128) + 1 + (size_t)H * sizeof(uint64_t));
+// Per-row bytes of the token-value workspace: val, best, lvl and H levels of predecessors; with net,
+// also the selected level's value, net and level.
+size_t token_value_row_bytes(int64_t n, int H, bool with_net) {
+  return (size_t)n * (sizeof(double) + sizeof(unsigned __int128) + 1 + (size_t)H * sizeof(uint64_t) +
+                      (with_net ? 2 * sizeof(double) + 1 : 0));
 }
 constexpr size_t kTokenValueBudget = size_t(512) << 20;  // workspace bytes the rows of one group may take
 
+// hop_cost (cfmm_quote_token_values_net): per (row, token) the best filled max_hops = L result net
+// of hop_cost[t] per hop, its net into net (NULL: not written); null: cfmm_quote_token_values.
 int quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint8_t* kind, const double* amount,
                        int max_hops, const uint8_t* allowed, double* value, uint8_t* hops, uint8_t* status,
                        int64_t* frontier, int64_t n_req, const int64_t* req_row, const int64_t* req_token,
                        int64_t* hop_off, int* hop_type, int64_t* hop_pool, int64_t* hop_token, double* hop_tender,
-                       double* hop_received, uint8_t* req_status) {
+                       double* hop_received, uint8_t* req_status, const double* hop_cost = nullptr,
+                       double* net = nullptr) {
   int rc;
   CU_TRY(ctx, cudaSetDevice(ctx->device));
   if ((rc = use_stream(ctx, ctx->stream)) != CFMM_OK) return rc;
@@ -3891,7 +3918,7 @@ int quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint
   }
   const int64_t positions = S.start[cfmm::kPathSets];
   // the group: up to kTvMaxGroup rows, as many as the budget holds (at least one)
-  const size_t row_bytes = token_value_row_bytes(n, H);
+  const size_t row_bytes = token_value_row_bytes(n, H, hop_cost != nullptr);
   const int G = (int)std::max<int64_t>(
       1, std::min<int64_t>({q, (int64_t)cfmm::kTvMaxGroup, (int64_t)(kTokenValueBudget / row_bytes)}));
   // workspace: [G][n] best (16-byte slots first), val, [G][H][n] pred, [2][n] fmask, [G][H+1] cnt,
@@ -3900,11 +3927,14 @@ int quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint
   const size_t b_best = 0, b_val = b_best + gn * 16, b_pred = b_val + gn * 8, b_fmask = b_pred + gn * H * 8,
                b_cnt = b_fmask + 2 * (size_t)n * 8, b_tot = b_cnt + (size_t)G * (H + 1) * 4,
                b_lvl = (b_tot + (size_t)(H + 1) * 4 + 15) & ~(size_t)15, b_end = b_lvl + gn;
-  if (ctx->tv_ws.n < b_end) CU_TRY(ctx, ctx->tv_ws.alloc(b_end));
+  // with net: [G][n] selected value and net, [G][n] selected level, after the rest
+  const size_t b_nval = (b_end + 15) & ~(size_t)15, b_nnet = b_nval + gn * 8, b_nlvl = b_nnet + gn * 8,
+               b_all = hop_cost ? b_nlvl + gn : b_end;
+  if (ctx->tv_ws.n < b_all) CU_TRY(ctx, ctx->tv_ws.alloc(b_all));
   unsigned char* ws = ctx->tv_ws.p;
   DevBuf<int64_t> d_root, d_req_row, d_req_tok, d_entry, d_pos, d_token;
   DevBuf<uint8_t> d_kind, d_allowed, d_hops, d_status, d_set, d_tok1, d_rstatus;
-  DevBuf<double> d_amount, d_value, d_tender, d_recv;
+  DevBuf<double> d_amount, d_value, d_tender, d_recv, d_cost, d_net;
   DevBuf<int32_t> d_nhop;
   CU_TRY(ctx, d_root.upload(root, (size_t)q));
   CU_TRY(ctx, d_kind.upload(kind, (size_t)q));
@@ -3913,6 +3943,12 @@ int quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint
   CU_TRY(ctx, d_value.alloc(gn));
   CU_TRY(ctx, d_hops.alloc(gn));
   CU_TRY(ctx, d_status.alloc(gn));
+  if (hop_cost) {
+    CU_TRY(ctx, d_cost.upload(hop_cost, (size_t)n));
+    CU_TRY(ctx, d_net.alloc(gn));
+  }
+  const cfmm::TvNet N{d_cost.p, reinterpret_cast<double*>(ws + b_nval), reinterpret_cast<double*>(ws + b_nnet),
+                      ws + b_nlvl};
   const size_t slots = (size_t)n_req * (size_t)H;
   if (n_req > 0) {
     CU_TRY(ctx, d_req_row.upload(req_row, (size_t)n_req));
@@ -3954,14 +3990,24 @@ int quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint
                    reinterpret_cast<int32_t*>(ws + b_tot)};
     bool any_req = false;
     for (int64_t j = 0; j < n_req && !any_req; ++j) any_req = req_row[j] >= r0 && req_row[j] < r0 + g;
-    if ((rc = launch(ctx, kProfSwaps, 2 + (pool_grid > 0 ? 2 : 1) * H + (any_req ? 1 : 0), [&] {
+    const unsigned gn_grid = (unsigned)((gn_g + 255) / 256);
+    const int64_t n_launch = 2 + (pool_grid > 0 ? 2 : 1) * H + (hop_cost ? H : 0) + (any_req ? 1 : 0);
+    if ((rc = launch(ctx, kProfSwaps, n_launch, [&] {
            cfmm::tv_init_kernel<<<tok_grid, cfmm::kTvThreads, 0, st>>>(W);
            for (int h = 1; h <= H; ++h) {
              if (pool_grid > 0) cfmm::tv_relax_kernel<<<pool_grid, cfmm::kTvThreads, 0, st>>>(os.d_P.p, S, W, h);
              cfmm::tv_finalize_kernel<<<tok_grid, cfmm::kTvThreads, 0, st>>>(W, h);
+             if (hop_cost) cfmm::tv_select_kernel<<<gn_grid, 256, 0, st>>>(W, N, h);
            }
-           cfmm::tv_rebuild_kernel<<<(unsigned)((gn_g + 255) / 256), 256, 0, st>>>(W, d_value.p, d_hops.p, d_status.p);
-           if (any_req)
+           if (hop_cost)
+             cfmm::tv_rebuild_net_kernel<<<gn_grid, 256, 0, st>>>(W, N, d_value.p, d_hops.p, d_status.p, d_net.p);
+           else
+             cfmm::tv_rebuild_kernel<<<gn_grid, 256, 0, st>>>(W, d_value.p, d_hops.p, d_status.p);
+           if (any_req && hop_cost)
+             cfmm::tv_path_net_kernel<<<(unsigned)((n_req + 127) / 128), 128, 0, st>>>(
+                 os.d_P.p, W, N, r0, d_entry.p, n_req, d_req_row.p, d_req_tok.p, d_nhop.p, d_set.p, d_pos.p,
+                 d_tok1.p, d_token.p, d_tender.p, d_recv.p, d_rstatus.p);
+           else if (any_req)
              cfmm::tv_path_kernel<<<(unsigned)((n_req + 127) / 128), 128, 0, st>>>(
                  os.d_P.p, W, r0, d_entry.p, n_req, d_req_row.p, d_req_tok.p, d_nhop.p, d_set.p, d_pos.p, d_tok1.p,
                  d_token.p, d_tender.p, d_recv.p, d_rstatus.p);
@@ -3971,6 +4017,7 @@ int quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint
     CU_TRY(ctx, read_back(ctx, hops ? hops + r0 * n : nullptr, d_hops.p, gn_g));
     CU_TRY(ctx, read_back(ctx, status ? status + r0 * n : nullptr, d_status.p, gn_g));
     CU_TRY(ctx, read_back(ctx, frontier ? cnt.data() : nullptr, W.cnt, (size_t)g * (H + 1)));
+    CU_TRY(ctx, read_back(ctx, hop_cost && net ? net + r0 * n : nullptr, d_net.p, gn_g));
     CU_TRY(ctx, cudaStreamSynchronize(st));
     if (frontier)
       for (int r = 0; r < g; ++r)
@@ -4024,6 +4071,25 @@ int cfmm_quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const
   return quote_token_values(ctx, q, root, kind, amount, max_hops, allowed, value, hops, status, frontier, n_req,
                             req_row, req_token, hop_off, hop_type, hop_pool, hop_token, hop_tender, hop_received,
                             req_status);
+}
+
+int cfmm_quote_token_values_net(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint8_t* kind,
+                                const double* amount, int max_hops, const uint8_t* allowed, const double* hop_cost,
+                                double* value, uint8_t* hops, uint8_t* status, double* net, int64_t* frontier,
+                                int64_t n_req, const int64_t* req_row, const int64_t* req_token, int64_t* hop_off,
+                                int* hop_type, int64_t* hop_pool, int64_t* hop_token, double* hop_tender,
+                                double* hop_received, uint8_t* req_status) {
+  const char* what = "quote_token_values_net";
+  int rc = check_token_values(ctx, q, root, kind, amount, max_hops, value, n_req, req_row, req_token, hop_off,
+                              hop_type, hop_pool, hop_token, what);
+  if (rc != CFMM_OK || (rc = check_hop_cost(ctx, hop_cost, ctx->n_tokens, what)) != CFMM_OK) return rc;
+  if (q == 0) {
+    if (hop_off) hop_off[0] = 0;
+    return CFMM_OK;
+  }
+  return quote_token_values(ctx, q, root, kind, amount, max_hops, allowed, value, hops, status, frontier, n_req,
+                            req_row, req_token, hop_off, hop_type, hop_pool, hop_token, hop_tender, hop_received,
+                            req_status, hop_cost, net);
 }
 
 int cfmm_pair_pools(cfmm_ctx* ctx, int64_t q, const int64_t* token_a, const int64_t* token_b, int64_t* count,
@@ -4164,6 +4230,23 @@ int cfmm_find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, con
   }
   return find_order_paths(ctx, q, token_in, token_out, kind, amount, max_hops, allowed, hop_off, hop_type, hop_pool,
                           hop_token, hop_tender, hop_received, value, status);
+}
+
+int cfmm_find_order_paths_net(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const int64_t* token_out,
+                              const uint8_t* kind, const double* amount, int max_hops, const uint8_t* allowed,
+                              const double* hop_cost, int64_t* hop_off, int* hop_type, int64_t* hop_pool,
+                              int64_t* hop_token, double* hop_tender, double* hop_received, double* value,
+                              uint8_t* status, double* net) {
+  const char* what = "find_order_paths_net";
+  int rc = check_find_paths(ctx, q, token_in, token_out, kind, amount, max_hops, allowed, hop_off, hop_type, hop_pool,
+                            hop_token, what);
+  if (rc != CFMM_OK || (rc = check_hop_cost(ctx, hop_cost, q, what)) != CFMM_OK) return rc;
+  if (q == 0) {
+    if (hop_off) hop_off[0] = 0;
+    return CFMM_OK;
+  }
+  return find_order_paths(ctx, q, token_in, token_out, kind, amount, max_hops, allowed, hop_off, hop_type, hop_pool,
+                          hop_token, hop_tender, hop_received, value, status, hop_cost, net);
 }
 
 // ---- orders routed over every pool among their allowed tokens (subgraph_kernels.cuh) ------------

@@ -643,6 +643,59 @@ function quote_token_values(ctx, n_tokens::Integer, root::Vector{Int64}, kind::V
             req_status=req_status[1:k])
 end
 
+# find_order_paths net of a per-hop cost (cfmm_find_order_paths_net): hop_cost[r] is row r's cost of one
+# hop in the token it settles in (token_out kind 0, token_in kind 1), >= 0, Inf allowed.  Among
+# max_hops = 1..max_hops, the filled result whose value net of the costs is best (the larger on a tie).
+# Returns find_order_paths' tuple and net.  Never executed, like the rest of this file.
+function find_order_paths_net(ctx, token_in::Vector{Int64}, token_out::Vector{Int64}, kind::Vector{UInt8},
+                              amount::Vector{Float64}, max_hops::Integer, allowed::Vector{UInt8},
+                              hop_cost::Vector{Float64})
+    q = length(token_in)
+    length(token_out) == length(kind) == length(amount) == length(hop_cost) == q ||
+        throw(ArgumentError("token_in / token_out / kind / amount / hop_cost need q entries"))
+    cap = max(q * max_hops, 1)
+    hop_off, typ, pool, tok = zeros(Int64, q + 1), zeros(Cint, cap), zeros(Int64, cap), zeros(Int64, cap)
+    tender, received, value, status, net = zeros(cap), zeros(cap), zeros(q), zeros(UInt8, q), zeros(q)
+    chk(ctx, ccall((:cfmm_find_order_paths_net, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Cint, Ptr{UInt8}, Ptr{Float64},
+         Ptr{Int64}, Ptr{Cint}, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8},
+         Ptr{Float64}),
+        ctx, q, token_in, token_out, kind, amount, max_hops, allowed, hop_cost, hop_off, typ, pool, tok, tender,
+        received, value, status, net))
+    n = hop_off[end]
+    return hop_off, typ[1:n], pool[1:n], tok[1:n], tender[1:n], received[1:n], value, status, net
+end
+
+# quote_token_values net of a per-hop cost (cfmm_quote_token_values_net): hop_cost[t] is the cost of
+# one hop in units of token t (n_tokens entries, >= 0, Inf allowed).  Per (row, token), among max_hops =
+# 1..max_hops the filled result whose value net of the costs is best (the larger on a tie); the requested
+# walks are the selected ones.  Returns quote_token_values' named tuple with net (n_tokens x q).  Never
+# executed, like the rest of this file.
+function quote_token_values_net(ctx, n_tokens::Integer, root::Vector{Int64}, kind::Vector{UInt8},
+                                amount::Vector{Float64}, max_hops::Integer, hop_cost::Vector{Float64},
+                                allowed=nothing; req_row::Vector{Int64}=Int64[], req_token::Vector{Int64}=Int64[])
+    q, k = length(root), length(req_row)
+    length(kind) == length(amount) == q || throw(ArgumentError("root / kind / amount need q entries"))
+    length(hop_cost) == n_tokens || throw(ArgumentError("hop_cost needs one entry per token"))
+    length(req_token) == k || throw(ArgumentError("req_row / req_token need one entry per request"))
+    value, hops, status = zeros(n_tokens, q), zeros(UInt8, n_tokens, q), zeros(UInt8, n_tokens, q)
+    net, frontier = zeros(n_tokens, q), zeros(Int64, max_hops, q)
+    cap = max(k * max_hops, 1)
+    hop_off, typ, pool, tok = zeros(Int64, k + 1), zeros(Cint, cap), zeros(Int64, cap), zeros(Int64, cap)
+    tender, received, req_status = zeros(cap), zeros(cap), zeros(UInt8, max(k, 1))
+    mask = allowed === nothing ? C_NULL : Vector{UInt8}(allowed)
+    chk(ctx, ccall((:cfmm_quote_token_values_net, LIB), Cint,
+        (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{UInt8}, Ptr{Float64}, Cint, Ptr{UInt8}, Ptr{Float64}, Ptr{Float64},
+         Ptr{UInt8}, Ptr{UInt8}, Ptr{Float64}, Ptr{Int64}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Ptr{Cint},
+         Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{UInt8}),
+        ctx, q, root, kind, amount, max_hops, mask, hop_cost, value, hops, status, net, frontier, k, req_row,
+        req_token, hop_off, typ, pool, tok, tender, received, req_status))
+    n = hop_off[end]
+    return (value=value, hops=hops, status=status, net=net, frontier=frontier, hop_off=hop_off,
+            hop_type=typ[1:n], hop_pool=pool[1:n], hop_token=tok[1:n], hop_tender=tender[1:n],
+            hop_received=received[1:n], req_status=req_status[1:k])
+end
+
 # Orders over every pool among allowed tokens (cfmm_quote_subgraph_swap_orders /
 # cfmm_execute_subgraph_swap_orders): row r sells amount[r] of token_in[r] for token_out[r] (kind 0,
 # exact-in) or buys amount[r] of token_out[r] paying in token_in[r] (kind 1, exact-out) over every pool

@@ -181,6 +181,94 @@ def _row_kind(kind, q, limit, what):
     return k
 
 
+def _order_paths(pools, token_in, token_out, kind, amount, max_hops, allowed, hop_cost):
+    """DevicePools.find_order_paths (hop_cost None) and find_order_paths_net."""
+    tin = np.ascontiguousarray(token_in, dtype=np.int64).reshape(-1)
+    tout = np.ascontiguousarray(token_out, dtype=np.int64).reshape(-1)
+    kind = np.ascontiguousarray(kind, dtype=np.uint8).reshape(-1)
+    amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
+    q = len(tin)
+    if not (len(tout) == len(kind) == len(amount) == q):
+        raise ValueError("find_order_paths: token_in, token_out, kind and amount need one entry per row")
+    mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
+    if len(mask) != pools.n_tokens:
+        raise ValueError(f"find_order_paths: allowed must have {pools.n_tokens} entries, one per token")
+    u8, i32 = C.POINTER(C.c_uint8), C.POINTER(C.c_int)
+    cap = max(q * max(int(max_hops), 0), 1)
+    hop_off = np.zeros(q + 1, dtype=np.int64)
+    typ, pool, tok = np.zeros(cap, dtype=np.int32), np.zeros(cap, dtype=np.int64), np.zeros(cap, dtype=np.int64)
+    tender, received = np.zeros(cap), np.zeros(cap)
+    value, status = np.zeros(q), np.zeros(q, dtype=np.uint8)
+    outs = (_ip(hop_off), typ.ctypes.data_as(i32), _ip(pool), _ip(tok), _dp(tender), _dp(received), _dp(value),
+            status.ctypes.data_as(u8))
+    if hop_cost is None:
+        pools._chk(pools._lib.cfmm_find_order_paths(pools._ctx, q, _ip(tin), _ip(tout), kind.ctypes.data_as(u8),
+                                                  _dp(amount), int(max_hops), mask.ctypes.data_as(u8), *outs))
+    else:
+        cost = np.ascontiguousarray(hop_cost, dtype=np.float64).reshape(-1)
+        if len(cost) != q:
+            raise ValueError("find_order_paths_net: hop_cost needs one entry per row")
+        net = np.zeros(q)
+        pools._chk(pools._lib.cfmm_find_order_paths_net(pools._ctx, q, _ip(tin), _ip(tout), kind.ctypes.data_as(u8),
+                                                      _dp(amount), int(max_hops), mask.ctypes.data_as(u8),
+                                                      _dp(cost), *outs, _dp(net)))
+    n = int(hop_off[-1])
+    found = (hop_off, typ[:n].copy(), pool[:n].copy(), tok[:n].copy(), tender[:n].copy(), received[:n].copy(),
+             value, status)
+    return found if hop_cost is None else found + (net,)
+
+
+def _token_values(pools, root, kind, amount, max_hops, allowed, requests, hop_cost):
+    """DevicePools.quote_token_values (hop_cost None) and quote_token_values_net."""
+    root = np.ascontiguousarray(root, dtype=np.int64).reshape(-1)
+    kind = np.ascontiguousarray(kind, dtype=np.uint8).reshape(-1)
+    amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
+    q, n, H = len(root), pools.n_tokens, int(max_hops)
+    if not (len(kind) == len(amount) == q):
+        raise ValueError("quote_token_values: root, kind and amount need one entry per row")
+    u8, i32 = C.POINTER(C.c_uint8), C.POINTER(C.c_int)
+    mask = None
+    if allowed is not None:
+        mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
+        if len(mask) != n:
+            raise ValueError(f"quote_token_values: allowed must have {n} entries, one per token")
+    rows = toks = np.zeros(0, dtype=np.int64)
+    if requests is not None:
+        rows = np.ascontiguousarray(requests[0], dtype=np.int64).reshape(-1)
+        toks = np.ascontiguousarray(requests[1], dtype=np.int64).reshape(-1)
+        if len(rows) != len(toks):
+            raise ValueError("quote_token_values: requests need one row per token")
+    k = len(rows)
+    value = np.zeros((q, n))
+    hops, status = np.zeros((q, n), dtype=np.uint8), np.zeros((q, n), dtype=np.uint8)
+    frontier = np.zeros((q, max(H, 0)), dtype=np.int64)
+    cap = max(k * max(H, 0), 1)
+    hop_off = np.zeros(k + 1, dtype=np.int64)
+    typ, pool, tok = np.zeros(cap, dtype=np.int32), np.zeros(cap, dtype=np.int64), np.zeros(cap, dtype=np.int64)
+    tender, received, rstatus = np.zeros(cap), np.zeros(cap), np.zeros(max(k, 1), dtype=np.uint8)
+    ins = (pools._ctx, q, _ip(root), kind.ctypes.data_as(u8), _dp(amount), H,
+           None if mask is None else mask.ctypes.data_as(u8))
+    reqs = (_ip(frontier), k, _ip(rows), _ip(toks), _ip(hop_off), typ.ctypes.data_as(i32), _ip(pool), _ip(tok),
+            _dp(tender), _dp(received), rstatus.ctypes.data_as(u8))
+    if hop_cost is None:
+        pools._chk(pools._lib.cfmm_quote_token_values(*ins, _dp(value), hops.ctypes.data_as(u8),
+                                                    status.ctypes.data_as(u8), *reqs))
+        head = (value, hops, status, frontier)
+    else:
+        cost = np.ascontiguousarray(hop_cost, dtype=np.float64).reshape(-1)
+        if len(cost) != n:
+            raise ValueError(f"quote_token_values_net: hop_cost must have {n} entries, one per token")
+        net = np.zeros((q, n))
+        pools._chk(pools._lib.cfmm_quote_token_values_net(*ins, _dp(cost), _dp(value), hops.ctypes.data_as(u8),
+                                                        status.ctypes.data_as(u8), _dp(net), *reqs))
+        head = (value, hops, status, net, frontier)
+    if requests is None:
+        return head
+    m = int(hop_off[-1])
+    return head + (hop_off, typ[:m].copy(), pool[:m].copy(), tok[:m].copy(), tender[:m].copy(),
+                   received[:m].copy(), rstatus[:k].copy())
+
+
 class DevicePools:
     """One GPU's shard of the pool set: a thin object wrapper over cfmm_ctx."""
 
@@ -802,29 +890,13 @@ class DevicePools:
         [q + 1], hop_type [Σ], hop_pool [Σ], hop_token [Σ] delivered, hop_tender [Σ], hop_received
         [Σ], value [q], status [q] uint8); the first three go to quote_paths / execute_paths as they
         are.  Status 0 filled, 2 no path, 4 (PATH_REPEATS_POOL) the best walk uses a pool twice."""
-        tin = np.ascontiguousarray(token_in, dtype=np.int64).reshape(-1)
-        tout = np.ascontiguousarray(token_out, dtype=np.int64).reshape(-1)
-        kind = np.ascontiguousarray(kind, dtype=np.uint8).reshape(-1)
-        amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
-        q = len(tin)
-        if not (len(tout) == len(kind) == len(amount) == q):
-            raise ValueError("find_order_paths: token_in, token_out, kind and amount need one entry per row")
-        mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
-        if len(mask) != self.n_tokens:
-            raise ValueError(f"find_order_paths: allowed must have {self.n_tokens} entries, one per token")
-        u8, i32 = C.POINTER(C.c_uint8), C.POINTER(C.c_int)
-        cap = max(q * max(int(max_hops), 0), 1)
-        hop_off = np.zeros(q + 1, dtype=np.int64)
-        typ, pool, tok = np.zeros(cap, dtype=np.int32), np.zeros(cap, dtype=np.int64), np.zeros(cap, dtype=np.int64)
-        tender, received = np.zeros(cap), np.zeros(cap)
-        value, status = np.zeros(q), np.zeros(q, dtype=np.uint8)
-        self._chk(self._lib.cfmm_find_order_paths(self._ctx, q, _ip(tin), _ip(tout), kind.ctypes.data_as(u8),
-                                                  _dp(amount), int(max_hops), mask.ctypes.data_as(u8), _ip(hop_off),
-                                                  typ.ctypes.data_as(i32), _ip(pool), _ip(tok), _dp(tender),
-                                                  _dp(received), _dp(value), status.ctypes.data_as(u8)))
-        n = int(hop_off[-1])
-        return (hop_off, typ[:n].copy(), pool[:n].copy(), tok[:n].copy(), tender[:n].copy(), received[:n].copy(),
-                value, status)
+        return _order_paths(self, token_in, token_out, kind, amount, max_hops, allowed, None)
+
+    def find_order_paths_net(self, token_in, token_out, kind, amount, max_hops: int, allowed, hop_cost):
+        """cfmm_find_order_paths_net: find_order_paths at the max_hops = L (1..max_hops) whose filled
+        result is best net of hop_cost[j] per hop (row j's cost in the token it settles in: token_out
+        kind 0, token_in kind 1; the larger L on a tie).  Returns find_order_paths' tuple and net [q]."""
+        return _order_paths(self, token_in, token_out, kind, amount, max_hops, allowed, hop_cost)
 
     # -- token values against one root (include/cfmm_b200.h, cfmm_quote_token_values) -------------
     def quote_token_values(self, root, kind, amount, max_hops: int, allowed=None, requests=None):
@@ -836,42 +908,14 @@ class DevicePools:
         tokens [k] 1-based) also (hop_off [k + 1], hop_type, hop_pool, hop_token, hop_tender,
         hop_received, req_status [k]), the walks as quote_paths / execute_paths take them (exact-in
         from the root, exact-out into it)."""
-        root = np.ascontiguousarray(root, dtype=np.int64).reshape(-1)
-        kind = np.ascontiguousarray(kind, dtype=np.uint8).reshape(-1)
-        amount = np.ascontiguousarray(amount, dtype=np.float64).reshape(-1)
-        q, n, H = len(root), self.n_tokens, int(max_hops)
-        if not (len(kind) == len(amount) == q):
-            raise ValueError("quote_token_values: root, kind and amount need one entry per row")
-        u8, i32 = C.POINTER(C.c_uint8), C.POINTER(C.c_int)
-        mask = None
-        if allowed is not None:
-            mask = np.ascontiguousarray(allowed, dtype=bool).reshape(-1).astype(np.uint8)
-            if len(mask) != n:
-                raise ValueError(f"quote_token_values: allowed must have {n} entries, one per token")
-        rows = toks = np.zeros(0, dtype=np.int64)
-        if requests is not None:
-            rows = np.ascontiguousarray(requests[0], dtype=np.int64).reshape(-1)
-            toks = np.ascontiguousarray(requests[1], dtype=np.int64).reshape(-1)
-            if len(rows) != len(toks):
-                raise ValueError("quote_token_values: requests need one row per token")
-        k = len(rows)
-        value = np.zeros((q, n))
-        hops, status = np.zeros((q, n), dtype=np.uint8), np.zeros((q, n), dtype=np.uint8)
-        frontier = np.zeros((q, max(H, 0)), dtype=np.int64)
-        cap = max(k * max(H, 0), 1)
-        hop_off = np.zeros(k + 1, dtype=np.int64)
-        typ, pool, tok = np.zeros(cap, dtype=np.int32), np.zeros(cap, dtype=np.int64), np.zeros(cap, dtype=np.int64)
-        tender, received, rstatus = np.zeros(cap), np.zeros(cap), np.zeros(max(k, 1), dtype=np.uint8)
-        self._chk(self._lib.cfmm_quote_token_values(
-            self._ctx, q, _ip(root), kind.ctypes.data_as(u8), _dp(amount), H,
-            None if mask is None else mask.ctypes.data_as(u8), _dp(value), hops.ctypes.data_as(u8),
-            status.ctypes.data_as(u8), _ip(frontier), k, _ip(rows), _ip(toks), _ip(hop_off),
-            typ.ctypes.data_as(i32), _ip(pool), _ip(tok), _dp(tender), _dp(received), rstatus.ctypes.data_as(u8)))
-        if requests is None:
-            return value, hops, status, frontier
-        m = int(hop_off[-1])
-        return (value, hops, status, frontier, hop_off, typ[:m].copy(), pool[:m].copy(), tok[:m].copy(),
-                tender[:m].copy(), received[:m].copy(), rstatus[:k].copy())
+        return _token_values(self, root, kind, amount, max_hops, allowed, requests, None)
+
+    def quote_token_values_net(self, root, kind, amount, max_hops: int, hop_cost, allowed=None, requests=None):
+        """cfmm_quote_token_values_net: per (row, token) quote_token_values at the max_hops = L
+        (1..max_hops) whose filled result is best net of hop_cost[t - 1] per hop (the cost of a hop in
+        units of token t, [n_tokens]; the larger L on a tie).  Returns quote_token_values' tuple with
+        net [q, n_tokens] after status; the requested walks are the selected levels'."""
+        return _token_values(self, root, kind, amount, max_hops, allowed, requests, hop_cost)
 
     # -- orders over every pool among allowed tokens (include/cfmm_b200.h,
     #    cfmm_quote_subgraph_swap_orders / cfmm_execute_subgraph_swap_orders) ------------------------
@@ -1229,6 +1273,26 @@ class DevicePools:
             self.close()
         except Exception:
             pass
+
+
+def pack_hop_cost(hop_cost, n_tokens, settle, what):
+    """A Router call's hop_cost as the _net calls take it: a scalar (every entry), or one cost per token
+    ([n_tokens], e.g. Router.hop_costs), each >= 0 (inf allowed: no walk pays for itself).  settle:
+    each row's settlement token (1-based), which picks a per-token cost for the row; None: the costs
+    per token, as they are."""
+    c = np.asarray(hop_cost, dtype=np.float64)
+    size = n_tokens if settle is None else len(settle)
+    if c.ndim == 0:
+        c = np.full(size, float(c))
+    else:
+        c = c.reshape(-1)
+        if len(c) != n_tokens:
+            raise ValueError(f"{what}: hop_cost must be a scalar or have {n_tokens} entries, one per token")
+        if settle is not None:
+            c = c[np.asarray(settle, dtype=np.int64) - 1]
+    if not np.all(c >= 0.0):
+        raise ValueError(f"{what}: hop_cost must be >= 0 (inf allowed), not NaN or negative")
+    return np.ascontiguousarray(c)
 
 
 def _pack(cfmms):
@@ -1649,50 +1713,62 @@ class Router:
         hubs = [flat[off[r]:off[r + 1]].tolist() for r in range(len(tin))]
         return self.execute_routed_orders(tin, tout, kinds, amounts, hubs, limits) + (hubs,)
 
-    def _find(self, token_in, token_out, kinds, amounts, allowed, max_hops, limits, what):
+    def _find(self, token_in, token_out, kinds, amounts, allowed, max_hops, limits, what, hop_cost=None):
         tin, tout, kinds, amounts, limits = self._split_args(token_in, token_out, kinds, amounts, limits, what)
         if not 1 <= int(max_hops) <= _lib.PATH_MAX_HOPS:
             raise ValueError(f"{what}: max_hops must be 1..{_lib.PATH_MAX_HOPS}")
         if allowed is None:
             raise ValueError(f"{what}: allowed (a mask over the tokens) is required")
-        found = self._pools.find_order_paths(tin, tout, kinds, amounts, int(max_hops), allowed)
+        if hop_cost is None:
+            found = self._pools.find_order_paths(tin, tout, kinds, amounts, int(max_hops), allowed)
+        else:
+            settle = np.where(np.asarray(kinds).astype(np.int64) == 1, tin, tout)
+            found = self._pools.find_order_paths_net(tin, tout, kinds, amounts, int(max_hops), allowed,
+                                                     pack_hop_cost(hop_cost, len(self.v), settle, what))
         off, typ, pool = found[:3]
         paths = [[self._type_lists[int(typ[h])][int(pool[h])] for h in range(off[r], off[r + 1])]
                  for r in range(len(tin))]
         return tin, tout, kinds, amounts, limits, found, paths
 
-    def find_paths(self, token_in, token_out, kinds, amounts, allowed, max_hops: int = _lib.PATH_MAX_HOPS):
+    def find_paths(self, token_in, token_out, kinds, amounts, allowed, max_hops: int = _lib.PATH_MAX_HOPS,
+                   hop_cost=None):
         """Find each order row's best single path on the device (cfmm_find_order_paths): at most
         max_hops hops from token_in[j] to token_out[j] (1-based), one pool per hop, every intermediate
         token t with allowed[t - 1] (a mask over the tokens), ranked by the amount out (kind 0, for
         amounts[j] in) or in (kind 1, for amounts[j] out).  No state changes.  Returns (paths, value
         [q], status [q]): paths[j] lists r.cfmms positions in hop order (empty without a path), ready
-        for quote_paths / execute_paths with token_in.  Single GPU."""
-        *_, found, paths = self._find(token_in, token_out, kinds, amounts, allowed, max_hops, None, "find_paths")
-        return paths, found[6], found[7]
+        for quote_paths / execute_paths with token_in.  hop_cost (a scalar, or per token as hop_costs
+        returns it; row j pays its settlement token's, token_out kind 0 and token_in kind 1): the path
+        whose amount net of hop_cost per hop is best (cfmm_find_order_paths_net), and net [q] is
+        returned last.  Single GPU."""
+        *_, found, paths = self._find(token_in, token_out, kinds, amounts, allowed, max_hops, None, "find_paths",
+                                      hop_cost)
+        return (paths, found[6], found[7]) + tuple(found[8:])
 
-    def quote_best_paths(self, token_in, token_out, kinds, amounts, allowed, max_hops: int = _lib.PATH_MAX_HOPS):
+    def quote_best_paths(self, token_in, token_out, kinds, amounts, allowed, max_hops: int = _lib.PATH_MAX_HOPS,
+                         hop_cost=None):
         """find_paths, priced: what quote_paths returns for the found paths, bit for bit (the find's
         amounts are that recursion).  Returns (paid [q], received [q], status [q], paths); a row
-        without a path has paid = received = 0 and the find's status.  No state changes.  Single
-        GPU."""
+        without a path has paid = received = 0 and the find's status.  hop_cost: as find_paths, with
+        net [q] returned last.  No state changes.  Single GPU."""
         *_, found, paths = self._find(token_in, token_out, kinds, amounts, allowed, max_hops, None,
-                                      "quote_best_paths")
+                                      "quote_best_paths", hop_cost)
         off, tender, received, status = found[0], found[4], found[5], found[7]
         has = np.diff(off) > 0
         paid, got = np.zeros(len(paths)), np.zeros(len(paths))
         paid[has], got[has] = tender[off[:-1][has]], received[off[1:][has] - 1]
-        return paid, got, status, paths
+        return (paid, got, status, paths) + tuple(found[8:])
 
     def execute_best_paths(self, token_in, token_out, kinds, amounts, allowed, max_hops: int = _lib.PATH_MAX_HOPS,
-                           limits=None):
+                           limits=None, hop_cost=None):
         """find_paths, then execute_paths over the rows that have a path, with the optional limits
         (kind 0: the minimum received; kind 1: the maximum paid).  Every row's path is found once, on
         the state at entry; the execute re-prices each path on the state the earlier paths left.
         Returns what quote_best_paths returns (rows without a path: zeros and the find's status) and
-        refreshes the touched pool objects, as execute_paths does.  Single GPU."""
+        refreshes the touched pool objects, as execute_paths does.  hop_cost: as find_paths, with the
+        find's net [q] returned last.  Single GPU."""
         tin, _, kinds, amounts, limits, found, paths = self._find(token_in, token_out, kinds, amounts, allowed,
-                                                                  max_hops, limits, "execute_best_paths")
+                                                                  max_hops, limits, "execute_best_paths", hop_cost)
         status = found[7].copy()
         paid, got = np.zeros(len(paths)), np.zeros(len(paths))
         rows = np.array([r for r in range(len(paths)) if paths[r]], dtype=np.int64)
@@ -1700,40 +1776,67 @@ class Router:
             p, g, s, _, _ = self.execute_paths([paths[r] for r in rows], tin[rows], kinds[rows], amounts[rows],
                                                None if limits is None else limits[rows])
             paid[rows], got[rows], status[rows] = p, g, s
-        return paid, got, status, paths
+        return (paid, got, status, paths) + tuple(found[8:])
 
-    def quote_token_values(self, roots, kinds, amounts, max_hops: int = _lib.PATH_MAX_HOPS, allowed=None):
+    def quote_token_values(self, roots, kinds, amounts, max_hops: int = _lib.PATH_MAX_HOPS, allowed=None,
+                           hop_cost=None):
         """Value every token against each row's root on the device (cfmm_quote_token_values): kind 0
         rows spend amounts[r] of roots[r] (1-based) and get, per token, the most of it that a walk of at
         most max_hops hops delivers; kind 1 rows receive amounts[r] of the root and get, per token, the
         least of it that such a walk must be paid.  Walks pass through tokens t with allowed[t - 1] (a
         mask over the tokens; None: every token), one pool per hop.  No state changes.  Returns (value,
         hops, status), each [q, n_tokens]: value 0 (kind 0) or inf (kind 1) where no walk reaches.
-        Single GPU."""
+        hop_cost (a scalar, or the cost of one hop in each token, as hop_costs returns it): per token
+        the walk whose amount net of the token's hop_cost per hop is best
+        (cfmm_quote_token_values_net), and net [q, n_tokens] is returned last.  Single GPU."""
         if self._world > 1:
             raise NotImplementedError("quote_token_values drives one GPU")
         if not 1 <= int(max_hops) <= _lib.PATH_MAX_HOPS:
             raise ValueError(f"quote_token_values: max_hops must be 1..{_lib.PATH_MAX_HOPS}")
-        return self._pools.quote_token_values(roots, kinds, amounts, int(max_hops), allowed)[:3]
+        if hop_cost is None:
+            return self._pools.quote_token_values(roots, kinds, amounts, int(max_hops), allowed)[:3]
+        cost = pack_hop_cost(hop_cost, len(self.v), None, "quote_token_values")
+        value, hops, status, net, _ = self._pools.quote_token_values_net(roots, kinds, amounts, int(max_hops), cost,
+                                                                         allowed)
+        return value, hops, status, net
 
-    def token_paths(self, root, kind, amount, tokens, max_hops: int = _lib.PATH_MAX_HOPS, allowed=None):
+    def hop_costs(self, gas_token, gas_per_hop, max_hops: int = _lib.PATH_MAX_HOPS, allowed=None):
+        """What gas_per_hop of gas_token (1-based) buys of each token: the exact-in token values rooted
+        at the gas token, [n_tokens].  The gas token gets gas_per_hop and unreached tokens inf (no walk
+        into them pays for itself).  Ready as the hop_cost of find_paths, quote_token_values and the
+        other path calls.  No state changes.  Single GPU."""
+        value, _, status = self.quote_token_values([gas_token], [0], [gas_per_hop], max_hops, allowed)
+        cost = value[0].copy()
+        cost[status[0] == _lib.ORDER_UNREACHABLE] = np.inf
+        return cost
+
+    def token_paths(self, root, kind, amount, tokens, max_hops: int = _lib.PATH_MAX_HOPS, allowed=None,
+                    hop_cost=None):
         """The walks behind quote_token_values for one root and the given tokens (1-based): kind 0
         from the root to each token, kind 1 from each token into the root.  Returns (paths, token_in,
         value, status): paths[j] lists r.cfmms positions in hop order (empty for the root, an unreached
         token or a walk that repeats a pool), ready for quote_paths / execute_paths with token_in[j]
-        and the same kind and amount; value[j] the token's value.  No state changes.  Single GPU."""
+        and the same kind and amount; value[j] the token's value.  hop_cost: as quote_token_values,
+        the walks net of it, with net [len(tokens)] returned last.  No state changes.  Single GPU."""
         if self._world > 1:
             raise NotImplementedError("token_paths drives one GPU")
         if not 1 <= int(max_hops) <= _lib.PATH_MAX_HOPS:
             raise ValueError(f"token_paths: max_hops must be 1..{_lib.PATH_MAX_HOPS}")
         tokens = np.asarray(tokens, dtype=np.int64).reshape(-1)
-        got = self._pools.quote_token_values([root], [kind], [amount], int(max_hops), allowed,
-                                             (np.zeros(len(tokens), dtype=np.int64), tokens))
+        req = (np.zeros(len(tokens), dtype=np.int64), tokens)
+        if hop_cost is None:
+            got = self._pools.quote_token_values([root], [kind], [amount], int(max_hops), allowed, req)
+        else:
+            cost = pack_hop_cost(hop_cost, len(self.v), None, "token_paths")
+            got = self._pools.quote_token_values_net([root], [kind], [amount], int(max_hops), cost, allowed, req)
+            net = got[3]
+            got = got[:3] + got[4:]
         value, off, typ, pool, st = got[0], got[4], got[5], got[6], got[10]
         paths = [[self._type_lists[int(typ[h])][int(pool[h])] for h in range(off[j], off[j + 1])]
                  for j in range(len(tokens))]
         token_in = tokens.copy() if int(kind) == 1 else np.full(len(tokens), int(root), dtype=np.int64)
-        return paths, token_in, value[0, tokens - 1], st
+        out = (paths, token_in, value[0, tokens - 1], st)
+        return out if hop_cost is None else out + (net[0, tokens - 1],)
 
     def _subgraph_args(self, token_in, token_out, amounts, allowed, limits, what):
         tin, tout, _, amounts, limits = self._split_args(token_in, token_out, np.zeros(len(np.atleast_1d(token_in))),

@@ -840,6 +840,74 @@ int cfmm_quote_token_values(cfmm_ctx *ctx, int64_t q, const int64_t *root /* [q]
                             double *hop_received /* [n_req·max_hops] or NULL */,
                             uint8_t *req_status /* [n_req] or NULL */);
 
+/* ---- best paths and token values net of a per-hop cost ---------------------------------------
+ * cfmm_find_order_paths and cfmm_quote_token_values rank walks by amount alone, so a hop that adds
+ * one ulp wins.  On a chain each hop costs gas.  The _net calls return, per row (best paths) or per
+ * (row, token) (token values), the result whose amount net of a fixed cost per hop is best.
+ *   definition  P_L is the existing call's result with max_hops = L.  For L = 1 … H:
+ *               eligible  P_L is CFMM_ORDER_FILLED;
+ *               net       exact-in net_L = v_L − n_L·κ, exact-out net_L = v_L + n_L·κ (v_L the value,
+ *                         n_L the hops, κ the hop cost), one IEEE multiply and then one IEEE add or
+ *                         subtract, no fma;
+ *               selection the eligible L with the best net: larger exact-in, smaller exact-out; on a
+ *                         tie the larger L.
+ *               Outputs are P_L's: hops, amounts, walk and value, and net.  No eligible L: P_H as it
+ *               is, with net = value.  The root, and a row of amount 0, keep their outputs, with
+ *               net = value.  κ = +inf is allowed (no walk into that token pays for itself): every
+ *               n >= 1 nets ∓inf, so the tie rule gives the largest filled L, P_H when it fills.
+ *   exactness   Each level's predecessors are kept, and a winner at level h has exactly h hops.  If the
+ *               best walk W* by net has k hops and amount A*, P_k amounts to at least A* with at most k
+ *               hops, so its net is at least A* − k·κ (exact-in; the mirror image exact-out).  The
+ *               selection over L is therefore the optimum over every walk the DP ranks.
+ *   κ = 0       Outputs are the existing call's bit for bit wherever the selection picks L = H.  It
+ *               picks a shorter L only when (a) the existing call reports CFMM_PATH_REPEATS_POOL at H
+ *               and a shorter L fills, or (b) rounding makes a shorter walk's quote strictly better:
+ *               fl(f) need not be monotone in its input even though f is.  Both are improvements.
+ *   limits      The costs are charged at the end, in the destination's units: intermediates are not
+ *               charged, and costs that depend on the pool type (UniV3 tick crossings) are not modelled.
+ *               The DP stays the existing one; the hop count is only a tie-break of its ranking, so a
+ *               walk that is worse by amount but shorter is found only when it is some level's best.
+ * cfmm_find_order_paths_net  cfmm_find_order_paths' arguments, plus hop_cost [q]: row r's κ in its
+ *               settlement token (the token_out exact-in, the token_in exact-out), and net [q] (NULL: not
+ *               written).  The final pass runs after every level of the DP instead of once: up to H
+ *               final passes per row.
+ * cfmm_quote_token_values_net  cfmm_quote_token_values' arguments, plus hop_cost [n_tokens]: κ_t, the
+ *               cost of one hop in units of token t, shared by every row, and net [q·n_tokens] (NULL:
+ *               not written).  The requested walks are those of the selected level.  frontier is the
+ *               DP's, unchanged.  One more per-(row, token) pass per level; the workspace holds 17 more
+ *               bytes per (row, token), so groups can be smaller.
+ * Costs in every token: cfmm_quote_token_values (exact-in) rooted at the gas token with the gas of one
+ * hop as its amount gives what a hop costs in each token (Python Router.hop_costs).
+ *
+ * Synchronous; change no state.  CFMM_ERR_INVALID before anything runs for every argument the existing
+ * call rejects, and for a null hop_cost (token values: always; best paths: with q > 0) or a hop_cost
+ * that is NaN or negative. */
+int cfmm_find_order_paths_net(cfmm_ctx *ctx, int64_t q, const int64_t *token_in /* [q] */,
+                              const int64_t *token_out /* [q] */, const uint8_t *kind /* [q] */,
+                              const double *amount /* [q] */, int max_hops /* 1..CFMM_PATH_MAX_HOPS */,
+                              const uint8_t *allowed /* [n_tokens], required */,
+                              const double *hop_cost /* [q] */, int64_t *hop_off /* [q+1] */,
+                              int *hop_type /* [q·max_hops] */, int64_t *hop_pool /* [q·max_hops] */,
+                              int64_t *hop_token /* [q·max_hops] */,
+                              double *hop_tender /* [q·max_hops] or NULL */,
+                              double *hop_received /* [q·max_hops] or NULL */, double *value /* [q] or NULL */,
+                              uint8_t *status /* [q] or NULL */, double *net /* [q] or NULL */);
+int cfmm_quote_token_values_net(cfmm_ctx *ctx, int64_t q, const int64_t *root /* [q] */,
+                                const uint8_t *kind /* [q] */, const double *amount /* [q] */,
+                                int max_hops /* 1..CFMM_PATH_MAX_HOPS */,
+                                const uint8_t *allowed /* [n_tokens] or NULL */,
+                                const double *hop_cost /* [n_tokens] */, double *value /* [q·n_tokens] */,
+                                uint8_t *hops /* [q·n_tokens] or NULL */,
+                                uint8_t *status /* [q·n_tokens] or NULL */, double *net /* [q·n_tokens] or NULL */,
+                                int64_t *frontier /* [q·max_hops] or NULL */, int64_t n_req,
+                                const int64_t *req_row /* [n_req] */, const int64_t *req_token /* [n_req] */,
+                                int64_t *hop_off /* [n_req+1] */, int *hop_type /* [n_req·max_hops] */,
+                                int64_t *hop_pool /* [n_req·max_hops] */,
+                                int64_t *hop_token /* [n_req·max_hops] */,
+                                double *hop_tender /* [n_req·max_hops] or NULL */,
+                                double *hop_received /* [n_req·max_hops] or NULL */,
+                                uint8_t *req_status /* [n_req] or NULL */);
+
 /* ---- orders routed over every pool among their allowed tokens ------------------------------
  * A row sells δ = amount[r] of j = token_in[r] for i = token_out[r] (1-based, distinct; exact-in:
  * exact-out rows are below) over every pool among j, i and the allowed tokens, split optimally: route! with
