@@ -7,7 +7,7 @@
 // the tokens of B, two levels of amounts and every level's predecessors in shared memory.  Every
 // candidate is one quote, path_hop_f / path_hop_exact_out: cfmm_quote_swaps /
 // cfmm_quote_swaps_exact_out bit for bit.  The rebuilt walk is priced by path_run, the code of
-// cfmm_quote_paths, so its amounts are that call's on the same CSR.  best_path_net_kernel
+// cfmm_quote_paths, so its amounts are that call's on the same CSR.  best_path_kernel<true>
 // (cfmm_find_order_paths_net) runs the same DP with the final pass after every level and emits the
 // max_hops = L result that is best net of a per-hop cost.
 #pragma once
@@ -222,8 +222,7 @@ __device__ __forceinline__ int bp_next_level(const PathSets* P, PairIndexView ix
 
 // The final hop into T, one thread per slot reached at level top, and S itself (the direct pair,
 // pseudo-slot nB): each warp's best into red[warp].  This is the final hop of the DP with
-// max_hops = top + 1.  (best_path_net_kernel's copies of best_path_kernel's steps, which keeps its
-// own inline code and so its SASS.)
+// max_hops = top + 1.
 __device__ __forceinline__ void bp_final_pass(const PathSets* P, PairIndexView ix, const BestPathGraph& G,
                                               const int32_t* epair, const int32_t& direct, int32_t j, int32_t i,
                                               int32_t S, bool out, double amt, int top, const double* val,
@@ -252,9 +251,42 @@ __device__ __forceinline__ BpKey bp_cta_best(const BpKey* red, int nwarp) {
   return best;
 }
 
+// A walk of n steps in DP order, step w through the pool entry(w) (set << kPairSetShift | device
+// position) from token from[w] to token to[w], written in path order to one row's hop slots: set,
+// device position, tendered side, delivered token 1-based.  An exact-in DP runs back from the sink
+// (path hop g is step n−1−g, which tenders from and delivers to); an exact-out DP runs forward from
+// the token delivered last (path hop g is step g, which tenders to and delivers from).  Returns
+// whether the walk uses a pool twice.  (Also token_value_kernels.cuh's requested walks.)
+template <class Entry>
+__device__ __forceinline__ bool walk_hops(const PathSets* P, int n, Entry entry, const int32_t* from,
+                                          const int32_t* to, bool out, uint8_t* row_set, int64_t* row_pos,
+                                          uint8_t* row_tok1, int64_t* row_token) {
+  bool repeats = false;
+  for (int g = 0; g < n; ++g) {
+    const int w = out ? g : n - 1 - g;
+    const int32_t a = out ? to[w] : from[w], c = out ? from[w] : to[w];
+    const HubHop hh = hub_hop(P, entry(w), a);
+    row_set[g] = (uint8_t)hh.k;
+    row_pos[g] = hh.p;
+    row_tok1[g] = hh.tok1;
+    row_token[g] = c + 1;
+    for (int f = 0; f < g; ++f) repeats |= row_set[f] == row_set[g] && row_pos[f] == row_pos[g];
+  }
+  return repeats;
+}
+
+// The n hops of one row's slots priced by path_run (cfmm_quote_paths' code, as a one-path CSR):
+// each hop's tender and received, and the walk's status into *st.
+__device__ __forceinline__ void walk_price(const PathSets* P, int n, const uint8_t* row_set, const int64_t* row_pos,
+                                           const uint8_t* row_tok1, const uint8_t* kind, const double* amount,
+                                           double* tender, double* received, uint8_t* st) {
+  const int64_t off[2] = {0, n};
+  path_run<false>(P, 0, off, row_set, row_pos, row_tok1, kind, amount, nullptr, tender, received, st);
+}
+
 // The walk of the final-hop winner best after level top, rebuilt from the predecessors in DP order
-// and written in path order to the row's hop slots (set, device position, tendered side, delivered
-// token 1-based).  Returns the hop count; repeats: whether the walk uses a pool twice.
+// and written to the row's hop slots by walk_hops.  Returns the hop count; repeats: whether the walk
+// uses a pool twice.
 __device__ __forceinline__ int bp_walk(const PathSets* P, PairIndexView ix, const BestPathGraph& G,
                                        const int32_t* spair, const int32_t* epair, const int32_t& direct,
                                        const int16_t* pred, const int32_t* ppos, int32_t S, int32_t T, bool out,
@@ -287,24 +319,13 @@ __device__ __forceinline__ int bp_walk(const PathSets* P, PairIndexView ix, cons
     wto[n++] = G.tok[s];
     s = u;
   }
-  // path order: exact-in walked back from i (reverse it), exact-out forward from j.  Hop g tenders
-  // a and delivers c.
-  repeats = false;
-  for (int g = 0; g < n; ++g) {
-    const int w = out ? g : n - 1 - g;
-    const int32_t a = out ? wto[w] : wfrom[w], c = out ? wfrom[w] : wto[w];
-    const HubHop hh = hub_hop(P, ix.pool[ix.off[wk[w]] + wpos[w]], a);
-    row_set[g] = (uint8_t)hh.k;
-    row_pos[g] = hh.p;
-    row_tok1[g] = hh.tok1;
-    row_token[g] = c + 1;
-    for (int f = 0; f < g; ++f) repeats |= row_set[f] == row_set[g] && row_pos[f] == row_pos[g];
-  }
+  repeats = walk_hops(P, n, [&](int w) { return ix.pool[ix.off[wk[w]] + wpos[w]]; }, wfrom, wto, out, row_set,
+                      row_pos, row_tok1, row_token);
   return n;
 }
 
 // Row r's outputs for the final-hop winner best after level top: no path, a walk that repeats a
-// pool, or the walk priced by path_run (cfmm_quote_paths' code).
+// pool, or the walk priced by walk_price.
 __device__ __forceinline__ void bp_emit(const PathSets* P, PairIndexView ix, const BestPathGraph& G,
                                         const int32_t* spair, const int32_t* epair, const int32_t& direct,
                                         const int16_t* pred, const int32_t* ppos, int32_t S, int32_t T, bool out,
@@ -330,220 +351,34 @@ __device__ __forceinline__ void bp_emit(const PathSets* P, PairIndexView ix, con
     status[r] = 4;  // CFMM_PATH_REPEATS_POOL
     return;
   }
-  const int64_t off[2] = {0, n};
   uint8_t st;
-  path_run<false>(P, 0, off, row_set, row_pos, row_tok1, kind + r, amount + r, nullptr, tender + (int64_t)H * r,
-                  received + (int64_t)H * r, &st);
+  walk_price(P, n, row_set, row_pos, row_tok1, kind + r, amount + r, tender + (int64_t)H * r, received + (int64_t)H * r,
+             &st);
   nhop[r] = n;
   value[r] = out ? tender[(int64_t)H * r] : received[(int64_t)H * r + n - 1];
   status[r] = st;
 }
 
-// Row r (include/cfmm_b200.h, cfmm_find_order_paths).  The DP runs from the source S (exact-in: j
-// forward; exact-out: i backward) to the sink T.  Outputs: nhop[r], and at H·r .. the hops' set,
-// device position, tendered side, delivered token (1-based), tender and received; value[r], status[r].
+// Row r (include/cfmm_b200.h).  The DP runs from the source S (exact-in: j forward; exact-out: i
+// backward) to the sink T.  Outputs: nhop[r], and at H·r .. the hops' set, device position, tendered
+// side, delivered token (1-based), tender and received; value[r], status[r].
+// kNet = false (cfmm_find_order_paths): the final pass after the last level computed, whose winner is
+// emitted.  hop_cost and net are not read.
+// kNet = true (cfmm_find_order_paths_net): the final pass after every level, so the CTA's best final
+// hop of the DP with max_hops = L is kept at lk[L − 1] for L = 1 .. top + 1 (a level that changed
+// nothing ends the DP: the levels and final passes after it repeat it).  Thread 0 then rebuilds each
+// L's walk, checks it for repeats, and emits the filled L whose value net of hop_cost[r] per hop is
+// best (the larger L on a tie); none filled: the max_hops = H outputs.  net[r] (NULL: not written) is
+// the emitted net, or the value.
+template <bool kNet>
 __global__ void __launch_bounds__(kBestPathThreads)
     best_path_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, BestPathGraph G,
                      const int64_t* __restrict__ token_in, const int64_t* __restrict__ token_out,
                      const uint8_t* __restrict__ kind, const double* __restrict__ amount, int H,
                      int32_t* __restrict__ nhop, uint8_t* __restrict__ hop_set, int64_t* __restrict__ hop_pos,
                      uint8_t* __restrict__ hop_tok1, int64_t* __restrict__ hop_token, double* __restrict__ tender,
-                     double* __restrict__ received, double* __restrict__ value, uint8_t* __restrict__ status) {
-  extern __shared__ __align__(16) unsigned char bp_smem[];
-  const int64_t r = blockIdx.x;
-  const int nB = G.nB, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarp = blockDim.x >> 5;
-  const int32_t j = (int32_t)(token_in[r] - 1), i = (int32_t)(token_out[r] - 1);
-  const bool out = kind[r] != 0;
-  const double amt = amount[r];
-  const int32_t S = out ? i : j, T = out ? j : i;
-  const double none = out ? kPathInf : 0.0;
-  double* val = reinterpret_cast<double*>(bp_smem);                  // [2][nB]
-  int32_t* spair = reinterpret_cast<int32_t*>(val + 2 * nB);        // [nB] pair {S, b}
-  int32_t* epair = spair + nB;                                       // [nB] pair {b, T}
-  int32_t* ppos = epair + nB;                                        // [H−1][nB]
-  int16_t* pred = reinterpret_cast<int16_t*>(ppos + (size_t)(H - 1) * nB);  // [H−1][nB]
-  uint8_t* hops = reinterpret_cast<uint8_t*>(pred + (size_t)(H - 1) * nB);  // [2][nB]
-  BpKey* red = reinterpret_cast<BpKey*>(
-      (reinterpret_cast<uintptr_t>(hops + 2 * nB) + 15) & ~(uintptr_t)15);  // [nwarp]
-  __shared__ int32_t direct;  // pair {S, T}, −1 when no pool holds it
-  if (!(amt > 0.0)) {  // nothing to route: filled, no hops (uniform across the CTA)
-    if (tid == 0) {
-      nhop[r] = 0;
-      value[r] = 0.0;
-      status[r] = 0;  // CFMM_ORDER_FILLED
-    }
-    return;
-  }
-  for (int s = tid; s < nB; s += blockDim.x) {
-    val[s] = val[nB + s] = none;
-    hops[s] = hops[nB + s] = 0;
-    spair[s] = epair[s] = -1;
-  }
-  if (tid == 0) direct = -1;
-  __syncthreads();
-  // the pairs {S, b} and {b, T}
-  for (int side = 0; side < 2; ++side) side_pairs(A, G, side ? T : S, side ? epair : spair);
-  if (tid == 0) {
-    const int64_t a1 = A.off[S + 1], e = adj_find(A, A.off[S], a1, T);
-    if (e < a1) direct = A.pair[e];
-  }
-  __syncthreads();
-  // level 1: one thread per slot, the pools of {S, b}, from the row's amount
-  int top = 0;  // the last level computed; the levels above it only carry
-  bool more = false;
-  if (H > 1) {
-    int changed = 0;
-    for (int s = tid; s < nB; s += blockDim.x) {
-      const int32_t b = G.tok[s];
-      BpKey key = bp_none();
-      if (b != j && b != i && spair[s] >= 0) bp_hop(P, ix, spair[s], out ? b : S, amt, out, 1, S, kBpFromSource, key);
-      const bool got = key.from != -1;
-      if (got) {
-        val[nB + s] = out ? -key.s : key.s;
-        hops[nB + s] = 1;
-      }
-      pred[s] = got ? kBpFromSource : kBpCarry;
-      ppos[s] = got ? key.pos : 0;
-      changed |= got;
-    }
-    top = 1;
-    more = __syncthreads_or(changed);
-  }
-  // levels 2 .. H−1: warps own destination slots, lanes scan the incoming pools.  A slot changed at
-  // level h−1 iff its hop count is h−1; only those can improve a slot at level h (an unchanged
-  // predecessor's candidates were all candidates of level h−1 already), so the others are skipped.
-  for (int h = 2; more && h < H; ++h) {
-    const double* vp = val + (size_t)((h - 1) & 1) * nB;
-    double* vc = val + (size_t)(h & 1) * nB;
-    const uint8_t* hp = hops + (size_t)((h - 1) & 1) * nB;
-    uint8_t* hc = hops + (size_t)(h & 1) * nB;
-    int changed = 0;
-    for (int s = warp; s < nB; s += nwarp) {
-      const int32_t b = G.tok[s];
-      BpKey key = bp_none();
-      if (b != j && b != i) {
-        const int32_t d = G.deg[s];
-        for (int m = lane; m < d; m += 32) {
-          const int u = G.nbr[(int64_t)nB * s + m];
-          if (hp[u] != h - 1) continue;
-          bp_hop(P, ix, G.pair[(int64_t)nB * s + m], out ? b : G.tok[u], vp[u], out, h, G.tok[u], m, key);
-        }
-      }
-      key = bp_warp_best(key);
-      if (lane == 0) {
-        const double prev = vp[s];
-        const bool better = key.from != -1 && (out ? -key.s < prev : key.s > prev);
-        vc[s] = better ? (out ? -key.s : key.s) : prev;
-        hc[s] = better ? (uint8_t)h : hp[s];
-        pred[(size_t)(h - 1) * nB + s] = better ? (int16_t)key.from : kBpCarry;
-        ppos[(size_t)(h - 1) * nB + s] = better ? key.pos : 0;
-        changed |= better;
-      }
-    }
-    top = h;
-    more = __syncthreads_or(changed);
-  }
-  // the final hop into T, one thread per slot reached at level top, and S itself (the direct pair,
-  // pseudo-slot nB); then the CTA's best
-  {
-    const double* vt = val + (size_t)(top & 1) * nB;
-    const uint8_t* ht = hops + (size_t)(top & 1) * nB;
-    BpKey key = bp_none();
-    for (int s = tid; s <= nB; s += blockDim.x) {
-      if (s == nB) {
-        if (direct >= 0) bp_hop(P, ix, direct, j, amt, out, 1, S, nB, key);
-      } else {
-        const int32_t b = G.tok[s];
-        if (b == j || b == i || epair[s] < 0 || !(out ? vt[s] < kPathInf : vt[s] > 0.0)) continue;
-        bp_hop(P, ix, epair[s], out ? j : b, vt[s], out, ht[s] + 1, b, s, key);
-      }
-    }
-    key = bp_warp_best(key);
-    if (lane == 0) red[warp] = key;
-  }
-  __syncthreads();
-  if (tid != 0) return;
-  BpKey best = red[0];
-  for (int w = 1; w < nwarp; ++w)
-    if (bp_before(red[w], best)) best = red[w];
-  int64_t* row_pos = hop_pos + (int64_t)H * r;
-  uint8_t* row_set = hop_set + (int64_t)H * r;
-  uint8_t* row_tok1 = hop_tok1 + (int64_t)H * r;
-  if (best.from < 0) {
-    nhop[r] = 0;
-    value[r] = 0.0;
-    status[r] = 2;  // CFMM_ORDER_UNREACHABLE
-    return;
-  }
-  // rebuild the walk in DP order: (pair, position, DP-predecessor token, DP-successor token)
-  int32_t wk[kBestPathMaxHops], wpos[kBestPathMaxHops], wfrom[kBestPathMaxHops], wto[kBestPathMaxHops];
-  int n = 0;
-  int s = best.from;
-  wk[n] = s == nB ? direct : epair[s];
-  wpos[n] = best.pos;
-  wfrom[n] = s == nB ? S : G.tok[s];
-  wto[n++] = T;
-  for (int h = top; s != nB && h >= 1; --h) {
-    const int16_t pr = pred[(size_t)(h - 1) * nB + s];
-    if (pr == kBpCarry) continue;
-    const int ps = ppos[(size_t)(h - 1) * nB + s];
-    if (pr == kBpFromSource) {
-      wk[n] = spair[s];
-      wpos[n] = ps;
-      wfrom[n] = S;
-      wto[n++] = G.tok[s];
-      break;
-    }
-    const int u = G.nbr[(int64_t)nB * s + pr];
-    wk[n] = G.pair[(int64_t)nB * s + pr];
-    wpos[n] = ps;
-    wfrom[n] = G.tok[u];
-    wto[n++] = G.tok[s];
-    s = u;
-  }
-  // path order: exact-in walked back from i (reverse it), exact-out forward from j.  Hop g tenders
-  // a and delivers c.
-  bool repeats = false;
-  for (int g = 0; g < n; ++g) {
-    const int w = out ? g : n - 1 - g;
-    const int32_t a = out ? wto[w] : wfrom[w], c = out ? wfrom[w] : wto[w];
-    const HubHop hh = hub_hop(P, ix.pool[ix.off[wk[w]] + wpos[w]], a);
-    row_set[g] = (uint8_t)hh.k;
-    row_pos[g] = hh.p;
-    row_tok1[g] = hh.tok1;
-    hop_token[(int64_t)H * r + g] = c + 1;
-    for (int f = 0; f < g; ++f) repeats |= row_set[f] == row_set[g] && row_pos[f] == row_pos[g];
-  }
-  if (repeats) {
-    nhop[r] = 0;
-    value[r] = 0.0;
-    status[r] = 4;  // CFMM_PATH_REPEATS_POOL
-    return;
-  }
-  const int64_t off[2] = {0, n};
-  uint8_t st;
-  path_run<false>(P, 0, off, row_set, row_pos, row_tok1, kind + r, amount + r, nullptr, tender + (int64_t)H * r,
-                  received + (int64_t)H * r, &st);
-  nhop[r] = n;
-  value[r] = out ? tender[(int64_t)H * r] : received[(int64_t)H * r + n - 1];
-  status[r] = st;
-}
-
-// Row r of cfmm_find_order_paths_net: best_path_kernel's DP with the final pass run after every
-// level, so the CTA's best final hop of the DP with max_hops = L is kept at lk[L − 1] for L = 1 ..
-// top + 1 (a level that changed nothing ends the DP: the levels and final passes after it repeat
-// it).  Thread 0 then rebuilds each L's walk, checks it for repeats, and emits the filled L whose
-// value net of hop_cost[r] per hop is best (the larger L on a tie); none filled: the max_hops = H
-// outputs.  net[r] (NULL: not written) is the emitted net, or the value.
-__global__ void __launch_bounds__(kBestPathThreads)
-    best_path_net_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, BestPathGraph G,
-                         const int64_t* __restrict__ token_in, const int64_t* __restrict__ token_out,
-                         const uint8_t* __restrict__ kind, const double* __restrict__ amount, int H,
-                         int32_t* __restrict__ nhop, uint8_t* __restrict__ hop_set, int64_t* __restrict__ hop_pos,
-                         uint8_t* __restrict__ hop_tok1, int64_t* __restrict__ hop_token,
-                         double* __restrict__ tender, double* __restrict__ received, double* __restrict__ value,
-                         uint8_t* __restrict__ status, const double* __restrict__ hop_cost,
-                         double* __restrict__ net) {
+                     double* __restrict__ received, double* __restrict__ value, uint8_t* __restrict__ status,
+                     const double* __restrict__ hop_cost, double* __restrict__ net) {
   extern __shared__ __align__(16) unsigned char bp_smem[];
   const int64_t r = blockIdx.x;
   const int nB = G.nB, tid = threadIdx.x, nwarp = blockDim.x >> 5;
@@ -567,7 +402,7 @@ __global__ void __launch_bounds__(kBestPathThreads)
       nhop[r] = 0;
       value[r] = 0.0;
       status[r] = 0;  // CFMM_ORDER_FILLED
-      if (net) net[r] = 0.0;
+      if (kNet && net) net[r] = 0.0;
     }
     return;
   }
@@ -578,33 +413,42 @@ __global__ void __launch_bounds__(kBestPathThreads)
   }
   if (tid == 0) direct = -1;
   __syncthreads();
+  // the pairs {S, b} and {b, T}
   for (int side = 0; side < 2; ++side) side_pairs(A, G, side ? T : S, side ? epair : spair);
   if (tid == 0) {
     const int64_t a1 = A.off[S + 1], e = adj_find(A, A.off[S], a1, T);
     if (e < a1) direct = A.pair[e];
   }
   __syncthreads();
-  // the final pass after level top: the best of the DP with max_hops = top + 1.  red is free again
-  // once thread 0 has read it: the next writes follow the next level's barrier.
+  // kNet: the final pass after level top, the best of the DP with max_hops = top + 1, into lk[top].
+  // red is free again once thread 0 has read it: the next writes follow the next level's barrier.
   const auto keep = [&](int top) {
     bp_final_pass(P, ix, G, epair, direct, j, i, S, out, amt, top, val, hops, red);
     __syncthreads();
     if (tid == 0) lk[top] = bp_cta_best(red, nwarp);
   };
-  keep(0);
-  int top = 0;
+  if (kNet) keep(0);
+  int top = 0;  // the last level computed; the levels above it only carry
   bool more = false;
   if (H > 1) {
     const int changed = bp_first_level(P, ix, G, spair, j, i, S, out, amt, val, hops, pred, ppos);
     top = 1;
     more = __syncthreads_or(changed);
-    keep(1);
+    if (kNet) keep(1);
   }
   for (int h = 2; more && h < H; ++h) {
     const int changed = bp_next_level(P, ix, G, j, i, out, h, val, hops, pred, ppos);
     top = h;
     more = __syncthreads_or(changed);
-    keep(h);
+    if (kNet) keep(h);
+  }
+  if (!kNet) {
+    bp_final_pass(P, ix, G, epair, direct, j, i, S, out, amt, top, val, hops, red);
+    __syncthreads();
+    if (tid == 0)
+      bp_emit(P, ix, G, spair, epair, direct, pred, ppos, S, T, out, top, bp_cta_best(red, nwarp), r, H, kind, amount,
+              nhop, hop_set, hop_pos, hop_tok1, hop_token, tender, received, value, status);
+    return;
   }
   if (tid != 0) return;
   // each L's walk, rebuilt into the row's hop slots for the repeat check, and a filled L's net: one

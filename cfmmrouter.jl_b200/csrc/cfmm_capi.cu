@@ -3703,6 +3703,68 @@ int choose_order_hubs(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const i
 
 // ---- best paths through allowed tokens (best_path_kernels.cuh) ----------------------------------
 
+// Pool p of path set k as cfmm_pair_pools reports it: its index in its type's insertion order.
+int64_t pool_id(cfmm_ctx* ctx, int k, int64_t p) {
+  return path_set(ctx, k).order[(size_t)p] + ((k & 1) ? ctx->sets[k >> 1].m : 0);
+}
+
+// The walks of a path search, H hop slots per entry (a row, or a requested walk): nhop per entry, and
+// per slot the set, device position, tendered side, delivered token (1-based), tender and received.
+struct HopSlots {
+  int64_t k = 0;
+  int H = 0;
+  DevBuf<int32_t> nhop;
+  DevBuf<uint8_t> set, tok1;
+  DevBuf<int64_t> pos, token;
+  DevBuf<double> tender, received;
+
+  int alloc(cfmm_ctx* ctx, int64_t entries, int max_hops) {
+    k = entries;
+    H = max_hops;
+    const size_t slots = (size_t)k * (size_t)H;
+    CU_TRY(ctx, nhop.alloc((size_t)k));
+    CU_TRY(ctx, set.alloc(slots));
+    CU_TRY(ctx, pos.alloc(slots));
+    CU_TRY(ctx, tok1.alloc(slots));
+    CU_TRY(ctx, token.alloc(slots));
+    CU_TRY(ctx, tender.alloc(slots));
+    CU_TRY(ctx, received.alloc(slots));
+    return CFMM_OK;
+  }
+
+  // After the launches, with the call's other read-backs enqueued: each entry's first nhop slots as
+  // cfmm_execute_paths' CSR, pools as cfmm_pair_pools reports them.  Synchronises the stream.
+  int pack(cfmm_ctx* ctx, int64_t* hop_off, int* hop_type, int64_t* hop_pool, int64_t* hop_token, double* hop_tender,
+           double* hop_received) {
+    const size_t slots = (size_t)k * (size_t)H;
+    std::vector<int32_t> n((size_t)k);
+    std::vector<uint8_t> s(slots);
+    std::vector<int64_t> p(slots), t(slots);
+    std::vector<double> x(hop_tender ? slots : 0), y(hop_received ? slots : 0);
+    CU_TRY(ctx, read_back(ctx, n.data(), nhop.p, (size_t)k));
+    CU_TRY(ctx, read_back(ctx, s.data(), set.p, slots));
+    CU_TRY(ctx, read_back(ctx, p.data(), pos.p, slots));
+    CU_TRY(ctx, read_back(ctx, t.data(), token.p, slots));
+    CU_TRY(ctx, read_back(ctx, hop_tender ? x.data() : nullptr, tender.p, slots));
+    CU_TRY(ctx, read_back(ctx, hop_received ? y.data() : nullptr, received.p, slots));
+    CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    hop_off[0] = 0;
+    for (int64_t e = 0; e < k; ++e) {
+      const int64_t g = hop_off[e];
+      for (int64_t h = 0; h < n[(size_t)e]; ++h) {
+        const size_t w = (size_t)(H * e + h);
+        hop_type[g + h] = s[w] >> 1;
+        hop_pool[g + h] = pool_id(ctx, s[w], p[w]);
+        hop_token[g + h] = t[w];
+        if (hop_tender) hop_tender[g + h] = x[w];
+        if (hop_received) hop_received[g + h] = y[w];
+      }
+      hop_off[e + 1] = g + n[(size_t)e];
+    }
+    return CFMM_OK;
+  }
+};
+
 // The call's allowed tokens; a row's tokens besides its own are these less the row's own among them.
 int64_t count_allowed(const cfmm_ctx* ctx, const uint8_t* allowed) {
   int64_t n = 0;
@@ -3765,12 +3827,13 @@ int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
       tok.push_back((int32_t)t);
     }
   const int nB = (int)tok.size(), H = max_hops;
-  const size_t slots = (size_t)q * (size_t)H, nn = (size_t)nB * (size_t)nB;
-  DevBuf<int64_t> d_in, d_out, d_pos, d_token;
-  DevBuf<int32_t> d_tok, d_slot, d_deg, d_gpair, d_nhop;
+  const size_t nn = (size_t)nB * (size_t)nB;
+  DevBuf<int64_t> d_in, d_out;
+  DevBuf<int32_t> d_tok, d_slot, d_deg, d_gpair;
   DevBuf<int16_t> d_gnbr;
-  DevBuf<uint8_t> d_kind, d_set, d_tok1, d_status;
-  DevBuf<double> d_amount, d_tender, d_recv, d_value, d_cost, d_net;
+  DevBuf<uint8_t> d_kind, d_status;
+  DevBuf<double> d_amount, d_value, d_cost, d_net;
+  HopSlots hs;
   CU_TRY(ctx, d_in.upload(token_in, (size_t)q));
   CU_TRY(ctx, d_out.upload(token_out, (size_t)q));
   CU_TRY(ctx, d_kind.upload(kind, (size_t)q));
@@ -3780,13 +3843,7 @@ int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
   CU_TRY(ctx, d_deg.alloc((size_t)nB));
   CU_TRY(ctx, d_gnbr.alloc(nn));
   CU_TRY(ctx, d_gpair.alloc(nn));
-  CU_TRY(ctx, d_nhop.alloc((size_t)q));
-  CU_TRY(ctx, d_set.alloc(slots));
-  CU_TRY(ctx, d_pos.alloc(slots));
-  CU_TRY(ctx, d_tok1.alloc(slots));
-  CU_TRY(ctx, d_token.alloc(slots));
-  CU_TRY(ctx, d_tender.alloc(slots));
-  CU_TRY(ctx, d_recv.alloc(slots));
+  if ((rc = hs.alloc(ctx, q, H)) != CFMM_OK) return rc;
   CU_TRY(ctx, d_value.alloc((size_t)q));
   CU_TRY(ctx, d_status.alloc((size_t)q));
   if (hop_cost) {
@@ -3794,9 +3851,8 @@ int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
     CU_TRY(ctx, d_net.alloc((size_t)q));
   }
   const size_t smem = cfmm::best_path_smem(nB, H);
-  CU_TRY(ctx, cudaFuncSetAttribute(hop_cost ? reinterpret_cast<const void*>(cfmm::best_path_net_kernel)
-                                            : reinterpret_cast<const void*>(cfmm::best_path_kernel),
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const auto kernel = hop_cost ? cfmm::best_path_kernel<true> : cfmm::best_path_kernel<false>;
+  CU_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const cfmm::PairIndexView pv{ix.off.p, ix.pool.p};
   const cfmm::AdjView A{ix.adj_off.p, ix.adj_nbr.p, ix.adj_pair.p};
   const cfmm::BestPathGraph G{d_tok.p, d_slot.p, d_deg.p, d_gnbr.p, d_gpair.p, nB};
@@ -3804,47 +3860,15 @@ int find_order_paths(cfmm_ctx* ctx, int64_t q, const int64_t* token_in, const in
          if (nB > 0)
            cfmm::best_path_graph_kernel<<<(unsigned)((32 * (int64_t)nB + 255) / 256), 256, 0, st>>>(
                A, d_tok.p, d_slot.p, nB, d_deg.p, d_gnbr.p, d_gpair.p);
-         if (hop_cost)
-           cfmm::best_path_net_kernel<<<(unsigned)q, cfmm::kBestPathThreads, smem, st>>>(
-               os.d_P.p, pv, A, G, d_in.p, d_out.p, d_kind.p, d_amount.p, H, d_nhop.p, d_set.p, d_pos.p, d_tok1.p,
-               d_token.p, d_tender.p, d_recv.p, d_value.p, d_status.p, d_cost.p, d_net.p);
-         else
-           cfmm::best_path_kernel<<<(unsigned)q, cfmm::kBestPathThreads, smem, st>>>(
-               os.d_P.p, pv, A, G, d_in.p, d_out.p, d_kind.p, d_amount.p, H, d_nhop.p, d_set.p, d_pos.p, d_tok1.p,
-               d_token.p, d_tender.p, d_recv.p, d_value.p, d_status.p);
+         kernel<<<(unsigned)q, cfmm::kBestPathThreads, smem, st>>>(
+             os.d_P.p, pv, A, G, d_in.p, d_out.p, d_kind.p, d_amount.p, H, hs.nhop.p, hs.set.p, hs.pos.p, hs.tok1.p,
+             hs.token.p, hs.tender.p, hs.received.p, d_value.p, d_status.p, d_cost.p, d_net.p);
        })) != CFMM_OK)
     return rc;
-  std::vector<int32_t> nhop((size_t)q);
-  std::vector<uint8_t> set(slots);
-  std::vector<int64_t> pos(slots), token(slots);
-  std::vector<double> tender(hop_tender ? slots : 0), recv(hop_received ? slots : 0);
-  CU_TRY(ctx, read_back(ctx, nhop.data(), d_nhop.p, (size_t)q));
-  CU_TRY(ctx, read_back(ctx, set.data(), d_set.p, slots));
-  CU_TRY(ctx, read_back(ctx, pos.data(), d_pos.p, slots));
-  CU_TRY(ctx, read_back(ctx, token.data(), d_token.p, slots));
-  CU_TRY(ctx, read_back(ctx, hop_tender ? tender.data() : nullptr, d_tender.p, slots));
-  CU_TRY(ctx, read_back(ctx, hop_received ? recv.data() : nullptr, d_recv.p, slots));
   CU_TRY(ctx, read_back(ctx, value, d_value.p, (size_t)q));
   CU_TRY(ctx, read_back(ctx, status, d_status.p, (size_t)q));
   CU_TRY(ctx, read_back(ctx, hop_cost ? net : nullptr, d_net.p, (size_t)q));
-  CU_TRY(ctx, cudaStreamSynchronize(st));
-  // pack each row's first nhop[r] slots; (set, device position) -> (type, index in the type's
-  // insertion order), as cfmm_pair_pools reports a pool
-  hop_off[0] = 0;
-  for (int64_t r = 0; r < q; ++r) {
-    const int64_t g = hop_off[r];
-    for (int64_t h = 0; h < nhop[(size_t)r]; ++h) {
-      const size_t w = (size_t)(H * r + h);
-      const int k = set[w];
-      hop_type[g + h] = k >> 1;
-      hop_pool[g + h] = path_set(ctx, k).order[(size_t)pos[w]] + ((k & 1) ? ctx->sets[k >> 1].m : 0);
-      hop_token[g + h] = token[w];
-      if (hop_tender) hop_tender[g + h] = tender[w];
-      if (hop_received) hop_received[g + h] = recv[w];
-    }
-    hop_off[r + 1] = g + nhop[(size_t)r];
-  }
-  return CFMM_OK;
+  return hs.pack(ctx, hop_off, hop_type, hop_pool, hop_token, hop_tender, hop_received);
 }
 
 // ---- token values from one root over the whole pool graph (token_value_kernels.cuh) -------------
@@ -3932,10 +3956,10 @@ int quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint
                b_all = hop_cost ? b_nlvl + gn : b_end;
   if (ctx->tv_ws.n < b_all) CU_TRY(ctx, ctx->tv_ws.alloc(b_all));
   unsigned char* ws = ctx->tv_ws.p;
-  DevBuf<int64_t> d_root, d_req_row, d_req_tok, d_entry, d_pos, d_token;
-  DevBuf<uint8_t> d_kind, d_allowed, d_hops, d_status, d_set, d_tok1, d_rstatus;
-  DevBuf<double> d_amount, d_value, d_tender, d_recv, d_cost, d_net;
-  DevBuf<int32_t> d_nhop;
+  DevBuf<int64_t> d_root, d_req_row, d_req_tok, d_entry;
+  DevBuf<uint8_t> d_kind, d_allowed, d_hops, d_status, d_rstatus;
+  DevBuf<double> d_amount, d_value, d_cost, d_net;
+  HopSlots hs;
   CU_TRY(ctx, d_root.upload(root, (size_t)q));
   CU_TRY(ctx, d_kind.upload(kind, (size_t)q));
   CU_TRY(ctx, d_amount.upload(amount, (size_t)q));
@@ -3947,21 +3971,16 @@ int quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint
     CU_TRY(ctx, d_cost.upload(hop_cost, (size_t)n));
     CU_TRY(ctx, d_net.alloc(gn));
   }
-  const cfmm::TvNet N{d_cost.p, reinterpret_cast<double*>(ws + b_nval), reinterpret_cast<double*>(ws + b_nnet),
-                      ws + b_nlvl};
-  const size_t slots = (size_t)n_req * (size_t)H;
+  // no selection without costs: every output from the last level a token changed at
+  const cfmm::TvNet N = hop_cost ? cfmm::TvNet{d_cost.p, reinterpret_cast<double*>(ws + b_nval),
+                                               reinterpret_cast<double*>(ws + b_nnet), ws + b_nlvl}
+                                 : cfmm::TvNet{};
   if (n_req > 0) {
     CU_TRY(ctx, d_req_row.upload(req_row, (size_t)n_req));
     CU_TRY(ctx, d_req_tok.upload(req_token, (size_t)n_req));
     CU_TRY(ctx, d_entry.alloc((size_t)std::max<int64_t>(ctx->n_pools, 1)));
-    CU_TRY(ctx, d_nhop.alloc((size_t)n_req));
     CU_TRY(ctx, d_rstatus.alloc((size_t)n_req));
-    CU_TRY(ctx, d_set.alloc(slots));
-    CU_TRY(ctx, d_pos.alloc(slots));
-    CU_TRY(ctx, d_tok1.alloc(slots));
-    CU_TRY(ctx, d_token.alloc(slots));
-    CU_TRY(ctx, d_tender.alloc(slots));
-    CU_TRY(ctx, d_recv.alloc(slots));
+    if ((rc = hs.alloc(ctx, n_req, H)) != CFMM_OK) return rc;
     if ((rc = launch(ctx, kProfSwaps, 1, [&] {
            if (positions > 0)
              cfmm::tv_entry_kernel<<<(unsigned)((positions + 255) / 256), 256, 0, st>>>(os.d_P.p, S, d_entry.p);
@@ -3999,18 +4018,11 @@ int quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint
              cfmm::tv_finalize_kernel<<<tok_grid, cfmm::kTvThreads, 0, st>>>(W, h);
              if (hop_cost) cfmm::tv_select_kernel<<<gn_grid, 256, 0, st>>>(W, N, h);
            }
-           if (hop_cost)
-             cfmm::tv_rebuild_net_kernel<<<gn_grid, 256, 0, st>>>(W, N, d_value.p, d_hops.p, d_status.p, d_net.p);
-           else
-             cfmm::tv_rebuild_kernel<<<gn_grid, 256, 0, st>>>(W, d_value.p, d_hops.p, d_status.p);
-           if (any_req && hop_cost)
-             cfmm::tv_path_net_kernel<<<(unsigned)((n_req + 127) / 128), 128, 0, st>>>(
-                 os.d_P.p, W, N, r0, d_entry.p, n_req, d_req_row.p, d_req_tok.p, d_nhop.p, d_set.p, d_pos.p,
-                 d_tok1.p, d_token.p, d_tender.p, d_recv.p, d_rstatus.p);
-           else if (any_req)
+           cfmm::tv_rebuild_kernel<<<gn_grid, 256, 0, st>>>(W, N, d_value.p, d_hops.p, d_status.p, d_net.p);
+           if (any_req)
              cfmm::tv_path_kernel<<<(unsigned)((n_req + 127) / 128), 128, 0, st>>>(
-                 os.d_P.p, W, r0, d_entry.p, n_req, d_req_row.p, d_req_tok.p, d_nhop.p, d_set.p, d_pos.p, d_tok1.p,
-                 d_token.p, d_tender.p, d_recv.p, d_rstatus.p);
+                 os.d_P.p, W, N, r0, d_entry.p, n_req, d_req_row.p, d_req_tok.p, hs.nhop.p, hs.set.p, hs.pos.p,
+                 hs.tok1.p, hs.token.p, hs.tender.p, hs.received.p, d_rstatus.p);
          })) != CFMM_OK)
       return rc;
     CU_TRY(ctx, read_back(ctx, value + r0 * n, d_value.p, gn_g));
@@ -4024,34 +4036,8 @@ int quote_token_values(cfmm_ctx* ctx, int64_t q, const int64_t* root, const uint
         for (int h = 1; h <= H; ++h) frontier[(r0 + r) * H + h - 1] = cnt[(size_t)r * (H + 1) + h];
   }
   if (n_req == 0) return CFMM_OK;
-  std::vector<int32_t> nhop((size_t)n_req);
-  std::vector<uint8_t> set(slots);
-  std::vector<int64_t> pos(slots), token(slots);
-  std::vector<double> tender(hop_tender ? slots : 0), recv(hop_received ? slots : 0);
-  CU_TRY(ctx, read_back(ctx, nhop.data(), d_nhop.p, (size_t)n_req));
-  CU_TRY(ctx, read_back(ctx, set.data(), d_set.p, slots));
-  CU_TRY(ctx, read_back(ctx, pos.data(), d_pos.p, slots));
-  CU_TRY(ctx, read_back(ctx, token.data(), d_token.p, slots));
-  CU_TRY(ctx, read_back(ctx, hop_tender ? tender.data() : nullptr, d_tender.p, slots));
-  CU_TRY(ctx, read_back(ctx, hop_received ? recv.data() : nullptr, d_recv.p, slots));
   CU_TRY(ctx, read_back(ctx, req_status, d_rstatus.p, (size_t)n_req));
-  CU_TRY(ctx, cudaStreamSynchronize(st));
-  // pack each request's first nhop[j] slots, pools as cfmm_pair_pools reports them (find_order_paths)
-  hop_off[0] = 0;
-  for (int64_t j = 0; j < n_req; ++j) {
-    const int64_t g = hop_off[j];
-    for (int64_t h = 0; h < nhop[(size_t)j]; ++h) {
-      const size_t w = (size_t)(H * j + h);
-      const int k = set[w];
-      hop_type[g + h] = k >> 1;
-      hop_pool[g + h] = path_set(ctx, k).order[(size_t)pos[w]] + ((k & 1) ? ctx->sets[k >> 1].m : 0);
-      hop_token[g + h] = token[w];
-      if (hop_tender) hop_tender[g + h] = tender[w];
-      if (hop_received) hop_received[g + h] = recv[w];
-    }
-    hop_off[j + 1] = g + nhop[(size_t)j];
-  }
-  return CFMM_OK;
+  return hs.pack(ctx, hop_off, hop_type, hop_pool, hop_token, hop_tender, hop_received);
 }
 
 }  // namespace
@@ -4660,7 +4646,7 @@ int row_orders(cfmm_ctx* ctx, bool exec, int64_t q, const Allowed& M, Rows R, co
     const int k = (int)(ent[t] >> cfmm::kPairSetShift);
     const int64_t p = ent[t] & cfmm::kPairPosMask;
     if (O.leg_type) O.leg_type[t] = k >> 1;
-    if (O.leg_pool) O.leg_pool[t] = path_set(ctx, k).order[(size_t)p] + ((k & 1) ? ctx->sets[k >> 1].m : 0);
+    if (O.leg_pool) O.leg_pool[t] = pool_id(ctx, k, p);
   }
   return CFMM_OK;
 }

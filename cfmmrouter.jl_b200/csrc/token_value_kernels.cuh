@@ -22,13 +22,13 @@
 // A level whose previous level changed no token of any row of the group returns at once, so a call
 // launches a fixed number of kernels and stops early without a host round trip.
 // cfmm_quote_token_values_net adds tv_select_kernel after each finalize (the best level net of a
-// per-hop cost, per row and token) and runs tv_rebuild_net_kernel / tv_path_net_kernel from the
-// selected level.
+// per-hop cost, per row and token), and tv_rebuild_kernel / tv_path_kernel walk from the selected
+// level.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "hub_kernels.cuh"
+#include "best_path_kernels.cuh"
 
 namespace cfmm {
 
@@ -204,37 +204,11 @@ __device__ __forceinline__ int tv_walk_from(const TvWork& W, int r, int64_t t, i
   return n;
 }
 
-// The walk from the level t last changed at: the walk of the DP with max_hops = H.
-__device__ __forceinline__ int tv_walk(const TvWork& W, int r, int64_t t, int32_t* tok, int32_t* nbr, uint32_t* gi) {
-  return tv_walk_from(W, r, t, W.lvl[(int64_t)r * W.n + t], tok, nbr, gi);
-}
-
 __device__ __forceinline__ bool tv_repeats(const uint32_t* gi, int n) {
   bool rep = false;
   for (int a = 1; a < n; ++a)
     for (int b = 0; b < a; ++b) rep |= gi[a] == gi[b];
   return rep;
-}
-
-// Per (row, token) of the group: value, hops and status at [r·n + t] of the group's outputs.
-__global__ void tv_rebuild_kernel(TvWork W, double* __restrict__ value, uint8_t* __restrict__ hops,
-                                  uint8_t* __restrict__ status) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (int64_t)W.G * W.n) return;
-  const int r = (int)(i / W.n);
-  const int64_t t = i - (int64_t)r * W.n;
-  const uint8_t L = W.lvl[i];
-  value[i] = W.val[i];
-  if (L == kTvNever || L == 0) {
-    hops[i] = 0;
-    status[i] = L == 0 ? 0 : 2;  // CFMM_ORDER_FILLED (the root), CFMM_ORDER_UNREACHABLE
-    return;
-  }
-  int32_t tok[kTvMaxHops], nbr[kTvMaxHops];
-  uint32_t gi[kTvMaxHops];
-  const int n = tv_walk(W, r, t, tok, nbr, gi);
-  hops[i] = (uint8_t)n;
-  status[i] = tv_repeats(gi, n) ? 4 : 0;  // CFMM_PATH_REPEATS_POOL, CFMM_ORDER_FILLED
 }
 
 // The entry (set << kPairSetShift | device position) of every pool at its global insertion index.
@@ -248,66 +222,6 @@ __global__ void tv_entry_kernel(const PathSets* __restrict__ P, TvSets S, int64_
   if (g >= 0) entry[g & ~(1ll << 62)] = ((int64_t)k << kPairSetShift) | p;
 }
 
-// Request j's walk (n steps in DP order, tv_walk's arrays) in path order at H·j .. (set, device
-// position, tendered side, delivered token 1-based), priced by path_run into tender, received and
-// status[j].
-__device__ __forceinline__ void tv_path_emit(const PathSets* P, const TvWork& W, int r, int64_t j, int n,
-                                             const int32_t* tok, const int32_t* nbr, const uint32_t* gi,
-                                             const int64_t* entry, uint8_t* hop_set, int64_t* hop_pos,
-                                             uint8_t* hop_tok1, int64_t* hop_token, double* tender, double* received,
-                                             uint8_t* status) {
-  const bool out = tv_out(W, r);
-  uint8_t* row_set = hop_set + (int64_t)W.H * j;
-  int64_t* row_pos = hop_pos + (int64_t)W.H * j;
-  uint8_t* row_tok1 = hop_tok1 + (int64_t)W.H * j;
-  for (int g = 0; g < n; ++g) {
-    // exact-in: DP step w (nbr tendered, tok delivered) is path hop n−1−w; exact-out: DP step w
-    // (tok tendered, nbr delivered) is path hop w
-    const int w = out ? g : n - 1 - g;
-    const int32_t a = out ? tok[w] : nbr[w], c = out ? nbr[w] : tok[w];
-    const HubHop hh = hub_hop(P, entry[gi[w]], a);
-    row_set[g] = (uint8_t)hh.k;
-    row_pos[g] = hh.p;
-    row_tok1[g] = hh.tok1;
-    hop_token[(int64_t)W.H * j + g] = c + 1;
-  }
-  const int64_t off[2] = {0, n};
-  path_run<false>(P, 0, off, row_set, row_pos, row_tok1, W.kind + r, W.amount + r, nullptr,
-                  tender + (int64_t)W.H * j, received + (int64_t)W.H * j, status + j);
-}
-
-// Requested (row, token) pairs j with row in the group (row0 .. row0 + G): the walk in path order
-// at H·j .. (set, device position, tendered side, delivered token 1-based), priced by path_run.
-// Exact-in walks run root → t, exact-out walks t → root.  nhop[j] = 0 for the root, an unreached
-// token and a walk that repeats a pool.
-__global__ void tv_path_kernel(const PathSets* __restrict__ P, TvWork W, int64_t row0, const int64_t* __restrict__ entry,
-                               int64_t n_req, const int64_t* __restrict__ req_row,
-                               const int64_t* __restrict__ req_token, int32_t* __restrict__ nhop,
-                               uint8_t* __restrict__ hop_set, int64_t* __restrict__ hop_pos,
-                               uint8_t* __restrict__ hop_tok1, int64_t* __restrict__ hop_token,
-                               double* __restrict__ tender, double* __restrict__ received,
-                               uint8_t* __restrict__ status) {
-  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n_req || req_row[j] < row0 || req_row[j] >= row0 + W.G) return;
-  const int r = (int)(req_row[j] - row0);
-  const int64_t t = req_token[j] - 1;
-  const uint8_t L = W.lvl[(int64_t)r * W.n + t];
-  nhop[j] = 0;
-  if (L == kTvNever || L == 0) {
-    status[j] = L == 0 ? 0 : 2;
-    return;
-  }
-  int32_t tok[kTvMaxHops], nbr[kTvMaxHops];
-  uint32_t gi[kTvMaxHops];
-  const int n = tv_walk(W, r, t, tok, nbr, gi);
-  if (tv_repeats(gi, n)) {
-    status[j] = 4;
-    return;
-  }
-  tv_path_emit(P, W, r, j, n, tok, nbr, gi, entry, hop_set, hop_pos, hop_tok1, hop_token, tender, received, status);
-  nhop[j] = n;
-}
-
 // ---- net of a per-hop cost (cfmm_quote_token_values_net) -------------------------------------------
 // The DP with max_hops = L is the first L levels of this one: token t's value, walk and hops at L are
 // those of the last level ≤ L it changed at.  So after each level h a token that changed at h is a
@@ -317,7 +231,7 @@ struct TvNet {
   const double* cost;  // [n] κ_t, per hop in units of token t
   double* val;         // [G][n] the selected level's value
   double* net;         // [G][n] its net
-  uint8_t* lvl;        // [G][n] the selected level (kTvNever: no level filled yet)
+  uint8_t* lvl;        // [G][n] the selected level (kTvNever: no level filled yet); null: no selection
 };
 
 // value ∓ n·κ: one IEEE multiply, then one add (exact-out) or subtract (exact-in); no fma.
@@ -346,43 +260,51 @@ __global__ void tv_select_kernel(TvWork W, TvNet N, int h) {
   N.lvl[i] = (uint8_t)h;
 }
 
-// tv_rebuild_kernel at the selected level; a token with none (the root, unreached, or no level filled)
-// gets tv_rebuild_kernel's outputs and net = value.
-__global__ void tv_rebuild_net_kernel(TvWork W, TvNet N, double* __restrict__ value, uint8_t* __restrict__ hops,
-                                      uint8_t* __restrict__ status, double* __restrict__ net) {
+// ---- the outputs ------------------------------------------------------------------------------------
+// A (row, token)'s outputs come from the level selected by tv_select_kernel when there is one (N.lvl
+// null: cfmm_quote_token_values, none), else from the last level the token changed at: the DP with
+// max_hops = H.
+
+// Per (row, token) of the group: value, hops and status at [r·n + t] of the group's outputs; net
+// (NULL: not written) gets the selected net, or the value when none is selected.
+__global__ void tv_rebuild_kernel(TvWork W, TvNet N, double* __restrict__ value, uint8_t* __restrict__ hops,
+                                  uint8_t* __restrict__ status, double* __restrict__ net) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)W.G * W.n) return;
   const int r = (int)(i / W.n);
   const int64_t t = i - (int64_t)r * W.n;
-  const bool sel = N.lvl[i] != kTvNever;
+  const bool sel = N.lvl && N.lvl[i] != kTvNever;
   const uint8_t L = sel ? N.lvl[i] : W.lvl[i];
   value[i] = sel ? N.val[i] : W.val[i];
   if (net) net[i] = sel ? N.net[i] : value[i];
   if (L == kTvNever || L == 0) {
     hops[i] = 0;
-    status[i] = L == 0 ? 0 : 2;
+    status[i] = L == 0 ? 0 : 2;  // CFMM_ORDER_FILLED (the root), CFMM_ORDER_UNREACHABLE
     return;
   }
   int32_t tok[kTvMaxHops], nbr[kTvMaxHops];
   uint32_t gi[kTvMaxHops];
   const int n = tv_walk_from(W, r, t, L, tok, nbr, gi);
   hops[i] = (uint8_t)n;
-  status[i] = tv_repeats(gi, n) ? 4 : 0;
+  status[i] = tv_repeats(gi, n) ? 4 : 0;  // CFMM_PATH_REPEATS_POOL, CFMM_ORDER_FILLED
 }
 
-// tv_path_kernel at the selected level.
-__global__ void tv_path_net_kernel(const PathSets* __restrict__ P, TvWork W, TvNet N, int64_t row0,
-                                   const int64_t* __restrict__ entry, int64_t n_req,
-                                   const int64_t* __restrict__ req_row, const int64_t* __restrict__ req_token,
-                                   int32_t* __restrict__ nhop, uint8_t* __restrict__ hop_set,
-                                   int64_t* __restrict__ hop_pos, uint8_t* __restrict__ hop_tok1,
-                                   int64_t* __restrict__ hop_token, double* __restrict__ tender,
-                                   double* __restrict__ received, uint8_t* __restrict__ status) {
+// Requested (row, token) pairs j with row in the group (row0 .. row0 + G): the walk in path order at
+// H·j .. (set, device position, tendered side, delivered token 1-based), priced by path_run.
+// Exact-in walks run root → t, exact-out walks t → root.  nhop[j] = 0 for the root, an unreached
+// token and a walk that repeats a pool.
+__global__ void tv_path_kernel(const PathSets* __restrict__ P, TvWork W, TvNet N, int64_t row0,
+                               const int64_t* __restrict__ entry, int64_t n_req, const int64_t* __restrict__ req_row,
+                               const int64_t* __restrict__ req_token, int32_t* __restrict__ nhop,
+                               uint8_t* __restrict__ hop_set, int64_t* __restrict__ hop_pos,
+                               uint8_t* __restrict__ hop_tok1, int64_t* __restrict__ hop_token,
+                               double* __restrict__ tender, double* __restrict__ received,
+                               uint8_t* __restrict__ status) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n_req || req_row[j] < row0 || req_row[j] >= row0 + W.G) return;
   const int r = (int)(req_row[j] - row0);
   const int64_t t = req_token[j] - 1, i = (int64_t)r * W.n + t;
-  const uint8_t L = N.lvl[i] != kTvNever ? N.lvl[i] : W.lvl[i];
+  const uint8_t L = N.lvl && N.lvl[i] != kTvNever ? N.lvl[i] : W.lvl[i];
   nhop[j] = 0;
   if (L == kTvNever || L == 0) {
     status[j] = L == 0 ? 0 : 2;
@@ -391,11 +313,16 @@ __global__ void tv_path_net_kernel(const PathSets* __restrict__ P, TvWork W, TvN
   int32_t tok[kTvMaxHops], nbr[kTvMaxHops];
   uint32_t gi[kTvMaxHops];
   const int n = tv_walk_from(W, r, t, L, tok, nbr, gi);
-  if (tv_repeats(gi, n)) {
+  uint8_t* row_set = hop_set + (int64_t)W.H * j;
+  int64_t* row_pos = hop_pos + (int64_t)W.H * j;
+  uint8_t* row_tok1 = hop_tok1 + (int64_t)W.H * j;
+  if (walk_hops(P, n, [&](int w) { return entry[gi[w]]; }, nbr, tok, tv_out(W, r), row_set, row_pos, row_tok1,
+                hop_token + (int64_t)W.H * j)) {
     status[j] = 4;
     return;
   }
-  tv_path_emit(P, W, r, j, n, tok, nbr, gi, entry, hop_set, hop_pos, hop_tok1, hop_token, tender, received, status);
+  walk_price(P, n, row_set, row_pos, row_tok1, W.kind + r, W.amount + r, tender + (int64_t)W.H * j,
+             received + (int64_t)W.H * j, status + j);
   nhop[j] = n;
 }
 
