@@ -9,13 +9,14 @@ the repo root:  `import cfmmrouter_b200 as cr`.)
 """
 from ._lib import CFMMError, LIB_PATH, load as load_library
 from .cfmms import CFMM, GeometricMeanTwoCoin, ProductTwoCoin, UniV3
-from .objectives import BasketLiquidation, BasketSwap, LimitBasket, LinearNonnegative, Objective, Swap
+from .objectives import (BasketLiquidation, BasketSwap, LimitBasket, LinearHoldings, LinearNonnegative, Objective,
+                         Swap)
 from .router import (DevicePools, Router, find_arb, netflows, netflows_, pool_file_info, route,
                      shard_range, update_reserves, write_pool_file)
 
 __all__ = [
     "CFMM", "ProductTwoCoin", "GeometricMeanTwoCoin", "UniV3",
-    "Objective", "LinearNonnegative", "BasketLiquidation", "BasketSwap", "LimitBasket", "Swap",
+    "Objective", "LinearNonnegative", "LinearHoldings", "BasketLiquidation", "BasketSwap", "LimitBasket", "Swap",
     "Router", "route", "find_arb", "netflows", "netflows_", "update_reserves",
     "DevicePools", "shard_range", "write_pool_file", "pool_file_info", "CFMMError", "LIB_PATH", "load_library",
 ]

@@ -60,6 +60,11 @@ class SubgraphOpts(C.Structure):
     _fields_ = [("max_iter", C.c_int), ("max_fun", C.c_int), ("rtol", C.c_double), ("factr", C.c_double)]
 
 
+class PriceArbOpts(C.Structure):
+    """cfmm_price_arb_opts: cfmm_subgraph_opts' fields, plus the absolute stop atol."""
+    _fields_ = SubgraphOpts._fields_ + [("atol", C.c_double)]
+
+
 class SubgraphOut(C.Structure):
     _fields_ = [("paid", C.POINTER(C.c_double)), ("received", C.POINTER(C.c_double)),
                 ("status", C.POINTER(C.c_uint8)), ("solver_status", C.POINTER(C.c_int)),
@@ -197,6 +202,10 @@ SYMBOLS = {
                                              C.POINTER(PriceArbOut)]),
     "cfmm_execute_price_arbitrage": (C.c_int, [_ctx, C.c_int64, _dp, _dp, C.POINTER(C.c_uint8),
                                                C.POINTER(SubgraphOpts), C.POINTER(PriceArbOut)]),
+    "cfmm_quote_price_arbitrage_rows": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _dp, _dp, C.POINTER(PriceArbOpts),
+                                                  C.POINTER(PriceArbOut)]),
+    "cfmm_execute_price_arbitrage_rows": (C.c_int, [_ctx, C.c_int64, _ip, _ip, _dp, _dp, _dp,
+                                                    C.POINTER(PriceArbOpts), C.POINTER(PriceArbOut)]),
     "cfmm_modify_univ3_liquidity":(C.c_int, [_ctx, C.c_int64, _ip, _dp, _dp]),
     "cfmm_get_univ3_ticks": (C.c_int, [_ctx, C.c_int64, C.c_int64, _ip, _dp, _dp]),
     "cfmm_debug_pool_set_info": (C.c_int, [_ctx, C.c_int, _ip]),

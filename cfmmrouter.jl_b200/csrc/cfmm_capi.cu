@@ -4947,24 +4947,8 @@ int check_price_arb(cfmm_ctx* ctx, int64_t q, const double* price, const double*
   return CFMM_OK;
 }
 
-// The family's outputs through row_orders: the profit in received, no paid.
-int price_arbitrage(cfmm_ctx* ctx, bool exec, int64_t q, const double* price, const double* min_profit,
-                    const uint8_t* allowed, const cfmm_subgraph_opts& o, const cfmm_price_arb_out& out,
-                    const char* what) {
-  int rc;
-  if ((rc = row_begin(ctx)) != CFMM_OK) return rc;
-  std::vector<int64_t> tokA;  // the columns of price: the allowed tokens, ascending (0-based)
-  for (int64_t t = 0; t < ctx->n_tokens; ++t)
-    if (allowed[t]) tokA.push_back(t);
-  const int64_t nA = (int64_t)tokA.size();
-  DevBuf<double> d_price, d_min;
-  CU_TRY(ctx, d_price.upload(price, (size_t)(q * nA)));
-  CU_TRY(ctx, d_min.upload(min_profit, (size_t)q));
-  int occ = 0;
-  if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::price_arb_kernel<false>), {}, "price_arb_kernel", occ)) != CFMM_OK)
-    return rc;
-  int64_t uses = 0;  // the priced tokens over the call
-  for (int64_t e = 0; e < q * nA; ++e) uses += price[e] > 0.0;
+// The family's outputs as row_orders takes them: the profit in received, no paid.
+cfmm_subgraph_out price_arb_outputs(const cfmm_price_arb_out& out) {
   cfmm_subgraph_out O{};
   O.received = out.profit;
   O.status = out.status;
@@ -4983,10 +4967,31 @@ int price_arbitrage(cfmm_ctx* ctx, bool exec, int64_t q, const double* price, co
   O.leg_pool = out.leg_pool;
   O.leg_delta = out.leg_delta;
   O.leg_lambda = out.leg_lambda;
+  return O;
+}
+
+// The profit of a price row through row_orders.
+int price_arbitrage(cfmm_ctx* ctx, bool exec, int64_t q, const double* price, const double* min_profit,
+                    const uint8_t* allowed, const cfmm_subgraph_opts& o, const cfmm_price_arb_out& out,
+                    const char* what) {
+  int rc;
+  if ((rc = row_begin(ctx)) != CFMM_OK) return rc;
+  std::vector<int64_t> tokA;  // the columns of price: the allowed tokens, ascending (0-based)
+  for (int64_t t = 0; t < ctx->n_tokens; ++t)
+    if (allowed[t]) tokA.push_back(t);
+  const int64_t nA = (int64_t)tokA.size();
+  DevBuf<double> d_price, d_min;
+  CU_TRY(ctx, d_price.upload(price, (size_t)(q * nA)));
+  CU_TRY(ctx, d_min.upload(min_profit, (size_t)q));
+  int occ = 0;
+  if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::price_arb_kernel<false>), {}, "price_arb_kernel", occ)) != CFMM_OK)
+    return rc;
+  int64_t uses = 0;  // the priced tokens over the call
+  for (int64_t e = 0; e < q * nA; ++e) uses += price[e] > 0.0;
   cfmm::PriceArbRows R{d_price.p, d_min.p, o.max_iter, o.max_fun, o.rtol, o.factr};
   // a row's T lies in its priced tokens: rows whose priced tokens are disjoint share no pool
   return row_orders(
-      ctx, exec, q, Allowed{allowed}, R, O, occ, 0, 0, 0, 0, uses, false, what,
+      ctx, exec, q, Allowed{allowed}, R, price_arb_outputs(out), occ, 0, 0, 0, 0, uses, false, what,
       [&](unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets*, cfmm::PairIndexView pv, cfmm::AdjView,
           const cfmm::BestPathGraph& G, const uint8_t* act, const cfmm::RowMasks&, int64_t* ntok, int64_t* npool) {
         cfmm::price_arb_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(pv, G, act, d_price.p, q, ntok, npool);
@@ -5017,6 +5022,85 @@ int price_arb_call(cfmm_ctx* ctx, bool exec, int64_t q, const double* price, con
   }
   const cfmm_price_arb_out none{};
   return price_arbitrage(ctx, exec, q, price, min_profit, allowed, o, out ? *out : none, what);
+}
+
+// ---- inventory rows: one token list per row, with holdings (price_arb_kernels.cuh, InvRule)
+
+// Every argument of cfmm_quote/execute_price_arbitrage_rows, before anything runs.
+int check_price_arb_rows(cfmm_ctx* ctx, int64_t q, Allowed& M, const double* price, const double* holding,
+                         const double* min_profit, const cfmm_price_arb_opts& po, const char* what) {
+  const cfmm_subgraph_opts o{po.max_iter, po.max_fun, po.rtol, po.factr};
+  int rc = check_row_opts(ctx, q, M, o, what);
+  if (rc != CFMM_OK) return rc;
+  if (!(std::isfinite(po.atol) && po.atol >= 0.0))
+    return fail(ctx, CFMM_ERR_INVALID, "%s: atol %g must be finite and >= 0", what, po.atol);
+  if (q == 0) return CFMM_OK;
+  if (!price) return fail(ctx, CFMM_ERR_INVALID, "%s: null price", what);
+  for (int64_t r = 0; r < q; ++r) {
+    const int64_t n = M.count(r);
+    if (n < 1 || n > CFMM_PRICE_ARB_MAX_TOKENS)
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: %lld listed tokens, not 1..%d", what, (long long)r,
+                  (long long)n, CFMM_PRICE_ARB_MAX_TOKENS);
+    bool any = false;
+    for (int64_t k = M.off[r]; k < M.off[r + 1]; ++k) {
+      if (!(std::isfinite(price[k]) && price[k] >= 0.0))
+        return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: price %g of token %lld must be finite and >= 0", what,
+                    (long long)r, price[k], (long long)M.tok[k]);
+      if (holding && !(std::isfinite(holding[k]) && holding[k] >= 0.0))
+        return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: holding %g of token %lld must be finite and >= 0", what,
+                    (long long)r, holding[k], (long long)M.tok[k]);
+      any |= price[k] > 0.0;
+    }
+    if (!any) return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: no positive price", what, (long long)r);
+    if (min_profit && !(std::isfinite(min_profit[r]) && min_profit[r] >= 0.0))
+      return fail(ctx, CFMM_ERR_INVALID, "%s: row %lld: min_profit %g must be finite and >= 0", what, (long long)r,
+                  min_profit[r]);
+  }
+  return CFMM_OK;
+}
+
+int price_arb_rows_call(cfmm_ctx* ctx, bool exec, int64_t q, const int64_t* allow_off, const int64_t* allow_token,
+                        const double* price, const double* holding, const double* min_profit,
+                        const cfmm_price_arb_opts* opts, cfmm_price_arb_out* out, const char* what) {
+  const cfmm_subgraph_opts d = subgraph_opts(nullptr);
+  const cfmm_price_arb_opts po = opts ? *opts : cfmm_price_arb_opts{d.max_iter, d.max_fun, d.rtol, d.factr, 0.0};
+  Allowed M{nullptr, true, allow_off, allow_token};
+  int rc = check_price_arb_rows(ctx, q, M, price, holding, min_profit, po, what);
+  if (rc != CFMM_OK) return rc;
+  if (q == 0) {
+    if (out && out->tok_off) out->tok_off[0] = 0;
+    if (out && out->leg_off) out->leg_off[0] = 0;
+    return CFMM_OK;
+  }
+  if ((rc = row_begin(ctx)) != CFMM_OK) return rc;
+  const size_t NL = (size_t)allow_off[q];
+  DevBuf<double> d_price, d_hold, d_min;
+  CU_TRY(ctx, d_price.upload(price, NL));
+  CU_TRY(ctx, d_hold.upload(holding, NL));
+  CU_TRY(ctx, d_min.upload(min_profit, (size_t)q));
+  int occ = 0;
+  if ((rc = row_occupancy(ctx, kernel_ptr(&cfmm::price_arb_rows_kernel<false>),
+                          {kernel_ptr(&cfmm::price_arb_rows_plan_kernel), kernel_ptr(&cfmm::price_arb_rows_kernel<false>),
+                           kernel_ptr(&cfmm::price_arb_rows_kernel<true>)},
+                          "price_arb_rows_kernel", occ, cfmm::kRowGraphBytes)) != CFMM_OK)
+    return rc;
+  const cfmm_price_arb_out none{};
+  cfmm::InvArbRows R{{d_price.p, d_min.p, po.max_iter, po.max_fun, po.rtol, po.factr}, d_hold.p, po.atol};
+  // a row's T lies in its list: rows on disjoint lists share no pool
+  return row_orders(
+      ctx, exec, q, M, R, price_arb_outputs(out ? *out : none), occ, 0, 0, 0, 0, 0, true, what,
+      [&](unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P, cfmm::PairIndexView pv, cfmm::AdjView A,
+          const cfmm::BestPathGraph&, const uint8_t*, const cfmm::RowMasks& RM, int64_t* ntok, int64_t* npool) {
+        cfmm::price_arb_rows_plan_kernel<<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, RM, q, ntok, npool);
+      },
+      [&](auto exec_tag, bool, unsigned grid, size_t dyn, cudaStream_t st, const cfmm::PathSets* P,
+          cfmm::PairIndexView pv, cfmm::AdjView A, const cfmm::BestPathGraph&, const uint8_t*,
+          const cfmm::RowMasks& RM, const cfmm::InvArbRows& R, const cfmm::SubgraphWork& W, const cfmm::SplitMoved& mv,
+          const int64_t* rows, int64_t n) {
+        constexpr bool X = decltype(exec_tag)::value;
+        cfmm::price_arb_rows_kernel<X><<<grid, cfmm::kSubgraphThreads, dyn, st>>>(P, pv, A, RM, R, W, mv, rows, n);
+      },
+      [](int64_t) { return false; }, [](int64_t, auto&&) {});
 }
 
 }  // namespace
@@ -5169,6 +5253,20 @@ int cfmm_quote_price_arbitrage(cfmm_ctx* ctx, int64_t q, const double* price, co
 int cfmm_execute_price_arbitrage(cfmm_ctx* ctx, int64_t q, const double* price, const double* min_profit,
                                  const uint8_t* allowed, const cfmm_subgraph_opts* opts, cfmm_price_arb_out* out) {
   return price_arb_call(ctx, true, q, price, min_profit, allowed, opts, out, "execute_price_arbitrage");
+}
+
+int cfmm_quote_price_arbitrage_rows(cfmm_ctx* ctx, int64_t q, const int64_t* allow_off, const int64_t* allow_token,
+                                    const double* price, const double* holding, const cfmm_price_arb_opts* opts,
+                                    cfmm_price_arb_out* out) {
+  return price_arb_rows_call(ctx, false, q, allow_off, allow_token, price, holding, nullptr, opts, out,
+                             "quote_price_arbitrage_rows");
+}
+
+int cfmm_execute_price_arbitrage_rows(cfmm_ctx* ctx, int64_t q, const int64_t* allow_off, const int64_t* allow_token,
+                                      const double* price, const double* holding, const double* min_profit,
+                                      const cfmm_price_arb_opts* opts, cfmm_price_arb_out* out) {
+  return price_arb_rows_call(ctx, true, q, allow_off, allow_token, price, holding, min_profit, opts, out,
+                             "execute_price_arbitrage_rows");
 }
 
 // ---- UniV3 liquidity changes: mint / burn rows, ladders that grow (univ3_state.cuh) ----------

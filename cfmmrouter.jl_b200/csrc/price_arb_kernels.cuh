@@ -14,6 +14,10 @@
 //   legs    split_leg over the pools at the final ν: the legs and, on execute, the transition.
 // price_arb_plan_kernel runs the setup only and reports each row's token and pool counts, which size
 // the outputs and the workspace.
+//
+// Inventory rows (cfmm_quote/execute_price_arbitrage_rows, at the end of this file) run the same row
+// body over each row's own slot graph (row_graph), with per-token holdings the net may spend and an
+// absolute stop beside the relative one (InvRule, InvArbRows).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -68,26 +72,11 @@ struct PriceArbSmem {
   int32_t n_loc, npool;
 };
 
-// Setup of the row with prices price[0 .. nB) (slot order): T, the local tokens, their prices and box,
-// and the pool count of every slot (cnt[s], the pools of the pairs {s, u} for slots u > s in T).
-__device__ void pa_setup(PairIndexView ix, const BestPathGraph& G, const uint8_t* __restrict__ gact,
-                         const double* __restrict__ price, PriceArbSmem& m) {
+// The local tokens of T (m.in) and the pool count of every slot (cnt[s], the pools of the pairs {s, u},
+// u > s in T, as exclusive offsets), after a barrier that published m.in.  Ends at a barrier.
+template <class Smem, class Graph>  // BestPathGraph or RowGraph
+__device__ __forceinline__ void pa_local(PairIndexView ix, const Graph& G, Smem& m) {
   const int tid = threadIdx.x, nB = G.nB;
-  for (int s = tid; s < nB; s += blockDim.x) {
-    m.ipair[s] = -1;
-    m.lidx[s] = -1;
-    m.priced[s] = price[s] > 0.0;
-  }
-  __syncthreads();
-  for (int s = tid; s < nB; s += blockDim.x) {
-    bool t = false;
-    if (m.priced[s]) {
-      const int dg = G.deg[s];
-      for (int e = 0; e < dg && !t; ++e) t = m.priced[G.nbr[(int64_t)nB * s + e]] && gact[(int64_t)nB * s + e];
-    }
-    m.in[s] = t;
-  }
-  __syncthreads();
   for (int s = tid; s < nB; s += blockDim.x) {
     int32_t c = 0;
     if (m.in[s]) {
@@ -118,6 +107,29 @@ __device__ void pa_setup(PairIndexView ix, const BestPathGraph& G, const uint8_t
     m.npool = tot;
   }
   __syncthreads();
+}
+
+// Setup of the row with prices price[0 .. nB) (slot order): T, the local tokens, their prices and box,
+// and the pool count of every slot (cnt[s], the pools of the pairs {s, u} for slots u > s in T).
+__device__ void pa_setup(PairIndexView ix, const BestPathGraph& G, const uint8_t* __restrict__ gact,
+                         const double* __restrict__ price, PriceArbSmem& m) {
+  const int tid = threadIdx.x, nB = G.nB;
+  for (int s = tid; s < nB; s += blockDim.x) {
+    m.ipair[s] = -1;
+    m.lidx[s] = -1;
+    m.priced[s] = price[s] > 0.0;
+  }
+  __syncthreads();
+  for (int s = tid; s < nB; s += blockDim.x) {
+    bool t = false;
+    if (m.priced[s]) {
+      const int dg = G.deg[s];
+      for (int e = 0; e < dg && !t; ++e) t = m.priced[G.nbr[(int64_t)nB * s + e]] && gact[(int64_t)nB * s + e];
+    }
+    m.in[s] = t;
+  }
+  __syncthreads();
+  pa_local(ix, G, m);
   for (int s = tid; s < nB; s += blockDim.x)
     if (m.in[s]) {
       const double c = price[s];
@@ -163,21 +175,21 @@ __global__ void __launch_bounds__(kSubgraphThreads)
   }
 }
 
-// Row r on the current state.  Returns nothing; writes the row's outputs.  EXEC: min_profit decides,
-// and a filled row applies the transition of cfmm_apply_trades at its ν to each of its pools.
-template <bool EXEC>
-__device__ void price_arb_row(const PathSets* P, PairIndexView ix, const BestPathGraph& G, const uint8_t* gact,
-                              const PriceArbRows& R, const SubgraphWork& w, const SplitMoved& mv, int64_t r,
-                              PriceArbSmem& m) {
+// Row r on the current state, after setup() (pa_setup, or inv_setup and inv_values) filled m.
+// Returns nothing; writes the row's outputs.  EXEC: min_profit decides, and a filled row applies the
+// transition of cfmm_apply_trades at its ν to each of its pools.
+template <bool EXEC, class Rule, class Graph, class Rows, class Smem, class Setup>
+__device__ void price_arb_row(const PathSets* P, PairIndexView ix, const Graph& G, const Rows& R,
+                              const SubgraphWork& w, const SplitMoved& mv, int64_t r, Smem& m, Setup setup) {
   __shared__ SgSolveState s;
   __shared__ double s_profit;
   const int tid = threadIdx.x;
-  pa_setup(ix, G, gact, R.price + r * G.nB, m);
+  setup();
   const int64_t np = m.npool, n = m.n_loc;
   sg_gather(ix, G, w, m, [](int, auto&) {});
   sg_order_pools(P, w, m, np, n, [&](int32_t t) { return (int32_t)m.lidx[G.slot_of[t]]; });
   double merit;
-  const int status = sg_solve(P, w, m, LnRule{}, R, n, true, s, merit);
+  const int status = sg_solve(P, w, m, Rule{}, R, n, true, s, merit);
   // the profit Σ_t c_t·Ψ_t in local order, from the first term
   if (tid == 0) {
     double pr = 0.0;
@@ -223,8 +235,187 @@ __global__ void __launch_bounds__(kSubgraphThreads)
                      const int64_t* __restrict__ rows, int64_t n) {
   __shared__ PriceArbSmem m;
   const SubgraphWork wb = sg_cta_work(w);
-  for (int64_t k = blockIdx.x; k < n; k += gridDim.x)
-    price_arb_row<EXEC>(P, ix, G, gact, R, wb, mv, rows ? rows[k] : k, m);
+  for (int64_t k = blockIdx.x; k < n; k += gridDim.x) {
+    const int64_t r = rows ? rows[k] : k;
+    price_arb_row<EXEC, LnRule>(P, ix, G, R, wb, mv, r, m, [&] { pa_setup(ix, G, gact, R.price + r * G.nB, m); });
+  }
+}
+
+// ---- inventory rows (cfmm_quote/execute_price_arbitrage_rows): each row over its own listed tokens L,
+// with a price c_t >= 0 and a holding h_t >= 0 per listed token, solving route! with
+// cᵀΨ − I(Ψ + h >= 0) over every pool among T.  T is the listed tokens with an active pool to another
+// listed token (a price of 0 keeps the token, valued at 0); the pools and the local order are the
+// price row's.  The dual is G(ν) = Σ_p π_p(ν) + hᵀν on the price row's box, started at its lower
+// bound; P̄ = G − hᵀc = π(ν) + hᵀ(ν − c) >= 0 bounds the profit.  The stop is m_r = mx / P̄ <= rtol or
+// mx <= atol, with mx = max_t s_t·|pg_t| and s_t = max(ν_t, c̄), c̄ the least positive price the row
+// lists.  A priced token has ν_t > c_t >= c̄, so s_t = ν_t there, as in the price row; a token priced 0
+// sits near ν_t = 1e-8, and the floor c̄ keeps its term in token units (a unit of it weighs at least
+// the cheapest priced token) instead of letting 1e-8·|pg_t| hide an overdraft of ~1e8·ε units.  A
+// row that holds nothing runs LnRule's operations: every listed price > 0 and atol 0 give the price
+// row over its list, bit for bit.
+//
+// Why the fill promise holds (ε = max(rtol·P̄, atol), so s_t·|pg_t| <= ε at the stop): the gradient is
+// g_t = h_t + Ψ_t.  A free token has |h_t + Ψ_t| <= ε/s_t; one on its bound has pg_t = 0 only when
+// g_t > 0, else |g_t| <= ε/s_t: in both cases Ψ_t >= −h_t − ε/s_t, so no token is overdrawn by more
+// than ε/c̄ units.  π is positively homogeneous, so π(ν) = νᵀΨ and P̄ − cᵀΨ = νᵀΨ + hᵀ(ν − c) − cᵀΨ =
+// Σ_t (ν_t − c_t)(Ψ_t + h_t).  A free token adds at most (ν_t − c_t)·ε/s_t <= ε; a token on its bound
+// adds 1e-8·(Ψ_t + h_t) (ν_t − c_t = 1e-8 up to the rounding of c_t + 1e-8).  So P̄ − cᵀΨ <= |T|·ε +
+// Σ_{t on its bound} 1e-8·(Ψ_t + h_t).  P̄ bounds the optimum profit from above (weak duality); cᵀΨ
+// exceeds it by at most the overdraft valued at ν, Σ_t (ν_t − c_t)·max(−Ψ_t − h_t, 0) <= |T|·ε.
+
+// The rows of an inventory call: price (PriceArbRows::price) and hold are aligned with the call's
+// allow_token ([allow_off[q]]); hold null: every holding 0.
+struct InvArbRows : PriceArbRows {
+  const double* hold;
+  double atol;
+};
+
+// An inventory row's shared state: the price row's, with h_t in local order (+0.0 where nothing is
+// held), the local tokens with h_t > 0 ascending, and hᵀc over them.  The box c_t + 1e-8 is not
+// stored but recomputed (InvRule::lo), which keeps the state within the 48 KB of static shared memory.
+struct InvArbSmem {
+  int32_t ipair[kSubgraphSlots], cnt[kSubgraphSlots + 1];
+  int16_t lidx[kSubgraphSlots];
+  uint8_t in[kSubgraphSlots];
+  int32_t ltok[kSubgraphLocal];
+  int32_t inc_off[kSubgraphLocal + 1];
+  double x[kSubgraphLocal], g[kSubgraphLocal], xt[kSubgraphLocal], gt[kSubgraphLocal], d[kSubgraphLocal],
+      pg[kSubgraphLocal], px[kSubgraphLocal], pt[kSubgraphLocal];
+  double S[kSolverM][kSubgraphLocal], Y[kSolverM][kSubgraphLocal];
+  double W[kSolverK][kSolverK];
+  double c[kSolverK];
+  double red[kSubgraphWarps];
+  double price[kSubgraphLocal], h[kSubgraphLocal];  // c_t and h_t in local order
+  int16_t held[kSubgraphLocal];
+  double gv, hc, cbar;  // cbar: c̄, the least positive price of the row's list
+  unsigned long long mx;
+  int32_t n_loc, npool, nheld;
+};
+
+// Setup of row r over its slot graph G (every slot listed): T (the slots with an active pool to
+// another slot), the local tokens and the pool counts.  Ends at a barrier.
+__device__ __forceinline__ void inv_setup(PairIndexView ix, const RowGraph& G, const uint8_t* __restrict__ gact,
+                                          InvArbSmem& m) {
+  const int tid = threadIdx.x, nB = G.nB;
+  for (int s = tid; s < nB; s += blockDim.x) {
+    m.ipair[s] = -1;
+    m.lidx[s] = -1;
+    bool t = false;
+    const int dg = G.deg[s];
+    for (int e = 0; e < dg && !t; ++e) t = gact[(int64_t)nB * s + e];
+    m.in[s] = t;
+  }
+  __syncthreads();
+  pa_local(ix, G, m);
+}
+
+// Row r's prices and holdings into local order: entry k of the row's list (caller order) goes to
+// its slot's local token.  Then the held tokens, hᵀc in local order (the first term alone) and c̄.
+__device__ __forceinline__ void inv_values(const RowGraph& G, const RowMasks& M, const InvArbRows& R, int64_t r,
+                                           InvArbSmem& m) {
+  const int tid = threadIdx.x;
+  const int64_t a0 = M.off[r];
+  for (int k = tid; k < G.nB; k += blockDim.x) {
+    const int l = m.lidx[G.slot_of[(int32_t)(M.tok[a0 + k] - 1)]];
+    if (l < 0) continue;
+    const double c = R.price[a0 + k], h = R.hold ? R.hold[a0 + k] : 0.0;
+    m.price[l] = c;
+    m.h[l] = h > 0.0 ? h : 0.0;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    int nh = 0;
+    double hc = 0.0;
+    for (int t = 0; t < m.n_loc; ++t)
+      if (m.h[t] > 0.0) {
+        const double v = __dmul_rn(m.h[t], m.price[t]);
+        hc = nh == 0 ? v : __dadd_rn(hc, v);
+        m.held[nh++] = (int16_t)t;
+      }
+    m.nheld = nh;
+    m.hc = hc;
+    double cb = __longlong_as_double(0x7ff0000000000000ll);  // the row has a positive price (checked)
+    for (int k = 0; k < G.nB; ++k) {
+      const double c = R.price[a0 + k];
+      if (c > 0.0) cb = fmin(cb, c);
+    }
+    m.cbar = cb;
+  }
+  __syncthreads();
+}
+
+// The rules of an inventory row: LnRule's box (c_t + 1e-8, the same IEEE addition), start and
+// evaluation record, with lin = h, the linear value hᵀν over the held tokens (sg_cta_sum's fixed
+// order over them in local order), and m_r = mx / P̄ with P̄ = g − hᵀc (0 when mx = 0; +inf when
+// P̄ <= 0 < mx).  With nothing held: LnRule's 0.0 and mx / g.
+struct InvRule {
+  static constexpr bool kOut = false;
+  static constexpr bool kBoxStart = true;
+  __device__ __forceinline__ double lin_at(const InvArbSmem& m, int t) const { return m.h[t]; }
+  // called by every thread of the CTA (sg_evaluate), so the sum may take the CTA's barriers
+  __device__ __forceinline__ double value(InvArbSmem& m) const {
+    if (m.nheld == 0) return 0.0;
+    double v = 0.0;
+    for (int k = threadIdx.x; k < m.nheld; k += blockDim.x) v = __dadd_rn(v, __dmul_rn(m.h[m.held[k]], m.xt[m.held[k]]));
+    return sg_cta_sum(v, m);
+  }
+  __device__ __forceinline__ double lo(const InvArbSmem& m, int t) const { return __dadd_rn(m.price[t], kPriceArbBox); }
+  __device__ __forceinline__ bool fixed(const InvArbSmem&, int) const { return false; }
+  __device__ __forceinline__ int root(const InvArbSmem&) const { return 0; }
+  __device__ __forceinline__ void evaluated(InvArbSmem& m, double f) const {
+    if (threadIdx.x == 0) m.gv = f;  // read after sg_commit's barriers
+  }
+  __device__ __forceinline__ double merit(const InvArbSmem& m, double mx) const {
+    if (!(mx > 0.0)) return 0.0;
+    const double pb = m.nheld ? __dsub_rn(m.gv, m.hc) : m.gv;
+    return pb > 0.0 ? __ddiv_rn(mx, pb) : __longlong_as_double(0x7ff0000000000000ll);
+  }
+};
+
+// The stop's scale of an inventory row: s_t = max(ν_t, c̄) (ν_t itself wherever c_t > 0).
+__device__ __forceinline__ double sg_stop_scale(const InvArbSmem& m, const InvRule&, int t) {
+  return fmax(m.x[t], m.cbar);
+}
+
+// The absolute stop of inventory rows: mx <= atol at the committed iterate (atol 0: only mx = 0, where
+// m_r is 0 already).
+template <class Smem>
+__device__ __forceinline__ bool sg_atol_met(const Smem& m, const InvArbRows& R) {
+  return __longlong_as_double((long long)m.mx) <= R.atol;
+}
+
+// Per row: the number of its tokens in T and of its pools.
+__global__ void __launch_bounds__(kSubgraphThreads)
+    price_arb_rows_plan_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, RowMasks M, int64_t q,
+                               int64_t* __restrict__ ntok, int64_t* __restrict__ npool) {
+  __shared__ InvArbSmem m;
+  for (int64_t r = blockIdx.x; r < q; r += gridDim.x) {
+    const RowGraph G = row_graph(P, ix, A, M, r);
+    inv_setup(ix, G, rg_act(M), m);
+    if (threadIdx.x == 0) {
+      ntok[r] = m.n_loc;
+      npool[r] = m.npool;
+    }
+    __syncthreads();
+  }
+}
+
+// Inventory rows rows[0 .. n) (null: 0 .. n), one CTA at a time each over its own slot graph; CTA b
+// uses workspace b.
+template <bool EXEC>
+__global__ void __launch_bounds__(kSubgraphThreads)
+    price_arb_rows_kernel(const PathSets* __restrict__ P, PairIndexView ix, AdjView A, RowMasks M, InvArbRows R,
+                          SubgraphWork w, SplitMoved mv, const int64_t* __restrict__ rows, int64_t n) {
+  __shared__ InvArbSmem m;
+  const SubgraphWork wb = sg_cta_work(w);
+  for (int64_t k = blockIdx.x; k < n; k += gridDim.x) {
+    const int64_t r = rows ? rows[k] : k;
+    const RowGraph G = row_graph(P, ix, A, M, r);
+    price_arb_row<EXEC, InvRule>(P, ix, G, R, wb, mv, r, m, [&] {
+      inv_setup(ix, G, rg_act(M), m);
+      inv_values(G, M, R, r, m);
+    });
+  }
 }
 
 }  // namespace cfmm

@@ -427,6 +427,11 @@ __device__ double sg_evaluate(const PathSets* P, const SubgraphWork& w, Smem& m,
   return f;
 }
 
+// The scale of token t's term in the stop's mx = max_t scale_t·|pg_t|: ν_t, the value at ν of a unit
+// of t's projected gradient.  Inventory rows (price_arb_kernels.cuh) floor it.
+template <class Smem, class Rule>
+__device__ __forceinline__ double sg_stop_scale(const Smem& m, const Rule&, int t) { return m.x[t]; }
+
 // Accept xt: (s, y) into history slot `slot` when store, x <- xt, g <- gt, Ψ, the projected gradient
 // and the Gram matrix of [S Y pg] (one warp per entry group, lanes over the tokens, butterfly).
 // Returns the rule's m_r.
@@ -447,7 +452,7 @@ __device__ double sg_commit(Smem& m, int slot, bool store, const Rule& rule) {
   }
   __syncthreads();
   double mx = 0.0;
-  for (int t = tid; t < n; t += blockDim.x) mx = fmax(mx, __dmul_rn(m.x[t], fabs(m.pg[t])));
+  for (int t = tid; t < n; t += blockDim.x) mx = fmax(mx, __dmul_rn(sg_stop_scale(m, rule, t), fabs(m.pg[t])));
   for (int o = 16; o >= 1; o >>= 1) mx = fmax(mx, __shfl_xor_sync(kFull, mx, o));
   if (lane == 0) atomicMax(&m.mx, (unsigned long long)__double_as_longlong(mx));  // order-free max
   const auto col = [&](int c, int t) {
@@ -640,6 +645,11 @@ __device__ __forceinline__ void sg_order_pools(const PathSets* P, const Subgraph
   __syncthreads();
 }
 
+// The absolute floor beside the relative stop: whether the committed mx = max_t ν_t·|pg_t| (m.mx) is at
+// most the rows' atol.  Only rows that carry an atol have one (price_arb_kernels.cuh's InvArbRows).
+template <class Smem, class Rows>
+__device__ __forceinline__ bool sg_atol_met(const Smem&, const Rows&) { return false; }
+
 // The solve's CTA-wide state: thread 0 decides, every thread reads after a barrier.
 struct SgSolveState {
   LbfgsHistory hist;
@@ -683,7 +693,7 @@ __device__ __forceinline__ int sg_solve(const PathSets* P, const SubgraphWork& w
     if (tid == 0) {
       s.state = 0;
       if (!(s.f == s.f)) s.status = 5, s.state = 1;
-      else if (s.merit <= R.rtol) s.status = 0, s.state = 1;
+      else if (s.merit <= R.rtol || sg_atol_met(m, R)) s.status = 0, s.state = 1;
       else if (s.iter >= R.max_iter) s.status = 2, s.state = 1;
       else if (s.fev >= R.max_fun) s.status = 3, s.state = 1;
       else s.t = lbfgs_direction(m.W, s.hist, m.c);

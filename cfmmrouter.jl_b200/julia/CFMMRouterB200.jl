@@ -956,6 +956,59 @@ quote_price_arbitrage(ctx, price, allowed; opts=nothing) =
 execute_price_arbitrage!(ctx, price, allowed; min_profit=nothing, opts=nothing) =
     _price_arbitrage(ctx, true, price, allowed, min_profit, opts)
 
+# Arbitrage from inventory (cfmm_quote_price_arbitrage_rows / cfmm_execute_price_arbitrage_rows): row r
+# lists allow_token[allow_off[r]+1 : allow_off[r+1]] (1-based tokens, any order), with price and holding
+# (nothing: none held) aligned with allow_token; each row maximises price'Ψ with Ψ + holding >= 0 over the
+# pools among its tokens.  opts is a PriceArbOpts (atol: the absolute stop).  Returns _price_arbitrage's
+# NamedTuple.  Never executed, like the rest of this file.
+struct PriceArbOpts
+    max_iter::Cint; max_fun::Cint; rtol::Float64; factr::Float64; atol::Float64
+end
+function _price_arbitrage_rows(ctx, execute::Bool, allow_off::Vector{Int64}, allow_token::Vector{Int64},
+                               price::Vector{Float64}, holding, min_profit, opts)
+    q = length(allow_off) - 1
+    length(price) == length(allow_token) || throw(ArgumentError("price needs one entry per listed token"))
+    holding === nothing || length(holding) == length(allow_token) ||
+        throw(ArgumentError("holding needs one entry per listed token"))
+    min_profit === nothing || length(min_profit) == q || throw(ArgumentError("min_profit needs q entries"))
+    o = opts === nothing ? nothing : Ref(opts)
+    h = holding === nothing ? C_NULL : holding
+    argq = (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{PriceArbOpts},
+            Ptr{PriceArbOut})
+    tok_off, leg_off = zeros(Int64, q + 1), zeros(Int64, q + 1)
+    sizes = Ref(PriceArbOut(C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, C_NULL, pointer(tok_off), 0, C_NULL, C_NULL,
+                            C_NULL, pointer(leg_off), 0, C_NULL, C_NULL, C_NULL, C_NULL))
+    GC.@preserve tok_off leg_off chk(ctx, ccall((:cfmm_quote_price_arbitrage_rows, LIB), Cint, argq, ctx, q,
+                                               allow_off, allow_token, price, h, o === nothing ? C_NULL : o, sizes))
+    NT, L = tok_off[end], leg_off[end]
+    profit, merit, status = zeros(q), zeros(q), zeros(UInt8, q)
+    sst, iters, fev = zeros(Cint, q), zeros(Cint, q), zeros(Cint, q)
+    token, nu, psi = zeros(Int64, max(NT, 1)), zeros(max(NT, 1)), zeros(max(NT, 1))
+    ltype, lpool, ld, ll = zeros(Cint, max(L, 1)), zeros(Int64, max(L, 1)), zeros(2, max(L, 1)), zeros(2, max(L, 1))
+    GC.@preserve profit merit status sst iters fev tok_off token nu psi leg_off ltype lpool ld ll begin
+        out = Ref(PriceArbOut(pointer(profit), pointer(status), pointer(sst), pointer(iters), pointer(fev),
+                              pointer(merit), pointer(tok_off), NT, pointer(token), pointer(nu), pointer(psi),
+                              pointer(leg_off), L, pointer(ltype), pointer(lpool), pointer(ld), pointer(ll)))
+        if execute
+            chk(ctx, ccall((:cfmm_execute_price_arbitrage_rows, LIB), Cint,
+                (Ptr{Cvoid}, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+                 Ptr{PriceArbOpts}, Ptr{PriceArbOut}),
+                ctx, q, allow_off, allow_token, price, h, min_profit === nothing ? C_NULL : min_profit,
+                o === nothing ? C_NULL : o, out))
+        else
+            chk(ctx, ccall((:cfmm_quote_price_arbitrage_rows, LIB), Cint, argq, ctx, q, allow_off, allow_token, price,
+                           h, o === nothing ? C_NULL : o, out))
+        end
+    end
+    return (profit=profit, status=status, solver_status=sst, iterations=iters, fun_evals=fev, merit=merit,
+            tok_off=tok_off, token=token[1:NT], nu=nu[1:NT], psi=psi[1:NT], leg_off=leg_off, leg_type=ltype[1:L],
+            leg_pool=lpool[1:L], leg_delta=ld[:, 1:L], leg_lambda=ll[:, 1:L])
+end
+quote_price_arbitrage_rows(ctx, allow_off, allow_token, price; holding=nothing, opts=nothing) =
+    _price_arbitrage_rows(ctx, false, allow_off, allow_token, price, holding, nothing, opts)
+execute_price_arbitrage_rows!(ctx, allow_off, allow_token, price; holding=nothing, min_profit=nothing, opts=nothing) =
+    _price_arbitrage_rows(ctx, true, allow_off, allow_token, price, holding, min_profit, opts)
+
 # Limit orders with partial fills (cfmm_quote_limit_orders / cfmm_execute_limit_orders): the rows of
 # _basket_orders, with limit_price[k] the least token_out[r] per unit of basket_token[k] at the margin
 # (finite, >= 0); an entry sells up to basket_amount[k] while the pools pay at least that.  min_received

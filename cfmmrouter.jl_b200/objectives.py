@@ -6,7 +6,8 @@ from __future__ import annotations
 
 import numpy as np
 
-__all__ = ["Objective", "LinearNonnegative", "BasketLiquidation", "BasketSwap", "LimitBasket", "Swap"]
+__all__ = ["Objective", "LinearNonnegative", "LinearHoldings", "BasketLiquidation", "BasketSwap", "LimitBasket",
+           "Swap"]
 
 
 class Objective:
@@ -53,6 +54,54 @@ class LinearNonnegative(Objective):
         return np.zeros_like(self.c)
 
     def upper_limit(self):  # objectives.jl:79
+        return np.full_like(self.c, np.inf)
+
+
+class LinearHoldings(Objective):
+    """U(Ψ) = cᵀΨ − I(Ψ + h ≥ 0): value the net trade at outside prices c ≥ 0, where the net may
+    spend up to the holdings h ≥ 0.  The conjugate is finite only on ν ≥ c, where it is
+    hᵀ(ν − c): the box is LinearNonnegative's, c + 1e-8, and f(ν) = linᵀν − hᵀc with lin = h, so
+    that f(ν*) plus the pools' value bounds the profit cᵀΨ.  With h = 0 it is LinearNonnegative(c)
+    (with prices of 0 allowed); c = e_i with h = Δin is BasketLiquidation(i, Δin) and c = (1 at i,
+    limit_k at each sold k) is LimitBasket, each up to its box."""
+
+    def __init__(self, c, h):
+        c = np.array(c, dtype=np.float64)
+        h = np.array(h, dtype=np.float64)
+        if c.ndim != 1 or c.shape != h.shape:
+            raise ValueError("c and h need one entry per token")
+        if not np.all(np.isfinite(c) & (c >= 0.0)):
+            raise ValueError("every price must be finite and >= 0")
+        if not np.all(np.isfinite(h) & (h >= 0.0)):
+            raise ValueError("every holding must be finite and >= 0")
+        self.c = c
+        self.h = h
+
+    def _const(self):
+        """Σ_t h_t·c_t, in token order."""
+        s = 0.0
+        for t in range(len(self.c)):
+            s += self.h[t] * self.c[t]
+        return s
+
+    def linear_term(self):
+        return self.h.copy()
+
+    def f(self, v):
+        if np.any(np.asarray(v) < self.c):
+            return np.inf
+        return float(np.dot(self.h, v)) - self._const()
+
+    def grad(self, g, v):
+        if np.any(np.asarray(v) < self.c):
+            g[:] = np.inf
+        else:
+            g[:] = self.h
+
+    def lower_limit(self):
+        return self.c + 1e-8
+
+    def upper_limit(self):
         return np.full_like(self.c, np.inf)
 
 

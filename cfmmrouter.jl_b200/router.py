@@ -130,6 +130,17 @@ def _row_args(n_tokens, q, allowed, limit, opts, what, own=None, room=None):
     return masks, limit, None if o is None else C.byref(o)
 
 
+def _price_arb_opts(opts):
+    """cfmm_price_arb_opts by reference from a dict of max_iter, max_fun, rtol, factr and atol (None:
+    NULL, the defaults)."""
+    if opts is None:
+        return None
+    d = {"max_iter": 1000, "max_fun": 4000, "rtol": 1e-4, "factr": 0.0, "atol": 0.0}
+    d.update(opts)
+    return C.byref(_lib.PriceArbOpts(int(d["max_iter"]), int(d["max_fun"]), float(d["rtol"]), float(d["factr"]),
+                                     float(d["atol"])))
+
+
 def _basket_room(token_out, basket_off, basket_token):
     """Each basket or limit row's own tokens (token_out and the entries) and its room for other allowed
     tokens: CFMM_SUBGRAPH_MAX_TOKENS + 1 tokens besides token_out, entries included."""
@@ -1168,6 +1179,71 @@ class DevicePools:
         returns."""
         return self._price_arb(True, price, allowed, min_profit, opts)
 
+    # -- arbitrage from inventory, one token list per row (include/cfmm_b200.h,
+    #    cfmm_quote_price_arbitrage_rows / cfmm_execute_price_arbitrage_rows) ----------------------------
+    def _price_arb_rows(self, execute, allow_off, allow_token, price, holding, min_profit, opts):
+        what = "inventory arbitrage"
+        off = np.ascontiguousarray(allow_off, dtype=np.int64).reshape(-1)
+        tok = np.ascontiguousarray(allow_token, dtype=np.int64).reshape(-1)
+        q = len(off) - 1
+        if q < 0 or off[0] != 0 or np.any(np.diff(off) < 0) or off[-1] != len(tok):
+            raise ValueError(f"{what}: allow_off must start at 0, not decrease and end at len(allow_token)")
+        n = np.diff(off)
+        if np.any((n < 1) | (n > _lib.PRICE_ARB_MAX_TOKENS)):
+            raise ValueError(f"{what}: every row lists 1 to {_lib.PRICE_ARB_MAX_TOKENS} tokens")
+        price = np.ascontiguousarray(price, dtype=np.float64).reshape(-1)
+        if len(price) != len(tok):
+            raise ValueError(f"{what}: price needs one entry per listed token ({len(tok)})")
+        if not np.all(np.isfinite(price) & (price >= 0.0)):
+            raise ValueError(f"{what}: a price is negative, NaN or Inf")
+        if q and not np.all(np.maximum.reduceat(price, off[:-1]) > 0.0):
+            raise ValueError(f"{what}: a row has no positive price")
+        hp = None
+        if holding is not None:
+            holding = np.ascontiguousarray(holding, dtype=np.float64).reshape(-1)
+            if len(holding) != len(tok):
+                raise ValueError(f"{what}: holding needs one entry per listed token ({len(tok)})")
+            if not np.all(np.isfinite(holding) & (holding >= 0.0)):
+                raise ValueError(f"{what}: a holding is negative, NaN or Inf")
+            hp = _dp(holding)
+        lim = None
+        if min_profit is not None:
+            min_profit = np.ascontiguousarray(np.broadcast_to(np.asarray(min_profit, dtype=np.float64), (q,)))
+            if not np.all(np.isfinite(min_profit) & (min_profit >= 0.0)):
+                raise ValueError(f"{what}: a min_profit is negative, NaN or Inf")
+            lim = _dp(min_profit)
+        if opts is not None and not (np.isfinite(opts.get("atol", 0.0)) and opts.get("atol", 0.0) >= 0.0):
+            raise ValueError(f"{what}: atol must be finite and >= 0")
+        po, ao, at, pr = _price_arb_opts(opts), _ip(off), _ip(tok), _dp(price)
+
+        def call(size, out):
+            if execute and not size:
+                return self._lib.cfmm_execute_price_arbitrage_rows(self._ctx, q, ao, at, pr, hp, lim, po, C.byref(out))
+            return self._lib.cfmm_quote_price_arbitrage_rows(self._ctx, q, ao, at, pr, hp, po, C.byref(out))
+        out = self._order_solve(q, 0, _lib.PriceArbOut, call)
+        out.profit = out.received
+        del out.paid, out.received
+        return out
+
+    def quote_price_arbitrage_rows(self, allow_off, allow_token, price, holding=None, opts=None):
+        """cfmm_quote_price_arbitrage_rows: row r lists the tokens allow_token[allow_off[r] ..
+        allow_off[r + 1]) (1-based, distinct, 1 to 258, any order), with price and holding aligned with
+        allow_token (price finite and >= 0, a positive one per row; holding None: all 0, else finite and
+        >= 0).  Each row trades over every pool among its tokens that have an active pool to another
+        listed token, maximising Σ price·Ψ with Ψ + holding >= 0 (a price of 0 keeps the token as an
+        intermediate), one dual solve per row on the device.  opts: dict of max_iter, max_fun, rtol,
+        factr and atol (the absolute stop on max ν·|pg|, default 0).  No state changes.  Returns
+        quote_price_arbitrage's namespace."""
+        return self._price_arb_rows(False, allow_off, allow_token, price, holding, None, opts)
+
+    def execute_price_arbitrage_rows(self, allow_off, allow_token, price, holding=None, min_profit=None,
+                                     opts=None):
+        """cfmm_execute_price_arbitrage_rows: the rows of quote_price_arbitrage_rows in batch order, each
+        re-solved on the state the earlier filled rows left (rows on disjoint lists share a launch);
+        min_profit (None, a scalar or one per row; finite and >= 0) reverts a row below it.  Returns
+        what quote_price_arbitrage_rows returns."""
+        return self._price_arb_rows(True, allow_off, allow_token, price, holding, min_profit, opts)
+
     # -- UniV3 liquidity changes (include/cfmm_b200.h, cfmm_modify_univ3_liquidity) ---------------
     def modify_univ3_liquidity(self, pools, lo, hi, dL):
         """cfmm_modify_univ3_liquidity: row j adds dL[j] (> 0 mints, < 0 burns) to the ticks of UniV3
@@ -2065,6 +2141,44 @@ class Router:
         with from the device state.  Single GPU."""
         out = self._pools.execute_price_arbitrage(self._price_arb_args(prices, allowed, "execute_price_arbitrage"),
                                                   allowed, min_profit, opts)
+        self._refresh_filled(out)
+        return out.profit, out.status, out
+
+    def _inventory_args(self, tokens, prices, holdings, what):
+        """(allow_off, allow_token, price, holding) from one token list per row and one price (and
+        holding) list per row aligned with it."""
+        if self._world > 1:
+            raise NotImplementedError(f"{what} drives one GPU")
+        if not is_row_lists(tokens):
+            raise ValueError(f"{what}: tokens must be one list of 1-based tokens per row")
+        q = len(tokens)
+        off, tok = pack_row_lists(tokens, len(self.v), [[]] * q, [_lib.PRICE_ARB_MAX_TOKENS] * q, what)
+
+        def aligned(vals, name):
+            if len(vals) != q or any(len(np.atleast_1d(v)) != len(t) for v, t in zip(vals, tokens)):
+                raise ValueError(f"{what}: {name} needs one list per row, aligned with its tokens")
+            return np.concatenate([np.asarray(v, dtype=np.float64).reshape(-1) for v in vals]) if q else np.zeros(0)
+        return off, tok, aligned(prices, "prices"), None if holdings is None else aligned(holdings, "holdings")
+
+    def quote_inventory_arbitrage(self, tokens, prices, holdings=None, opts=None):
+        """The best trades against external prices from inventory: row r lists tokens[r] (1-based,
+        distinct, 1 to 258) with prices[r] and holdings[r] aligned with it (holdings None: nothing
+        held).  Each row maximises Σ price·Ψ over every pool among its tokens, where a token's net may
+        spend up to its holding (route! with cᵀΨ − I(Ψ + h >= 0)), one dual solve per row on the device
+        (cfmm_quote_price_arbitrage_rows).  opts as DevicePools.quote_price_arbitrage_rows, "atol"
+        included.  No state changes.  Returns (profit [q], status [q], detail): detail is
+        DevicePools.quote_price_arbitrage_rows' namespace.  Single GPU."""
+        off, tok, pr, h = self._inventory_args(tokens, prices, holdings, "quote_inventory_arbitrage")
+        out = self._pools.quote_price_arbitrage_rows(off, tok, pr, h, opts)
+        return out.profit, out.status, out
+
+    def execute_inventory_arbitrage(self, tokens, prices, holdings=None, min_profit=None, opts=None):
+        """Execute inventory arbitrage rows in order (cfmm_execute_price_arbitrage_rows), each re-solved
+        on the state the earlier filled rows left, with an optional minimum profit: a row below it
+        reverts.  Returns what quote_inventory_arbitrage returns and refreshes the pool objects the
+        filled rows traded with from the device state.  Single GPU."""
+        off, tok, pr, h = self._inventory_args(tokens, prices, holdings, "execute_inventory_arbitrage")
+        out = self._pools.execute_price_arbitrage_rows(off, tok, pr, h, min_profit, opts)
         self._refresh_filled(out)
         return out.profit, out.status, out
 

@@ -1418,6 +1418,73 @@ int cfmm_execute_price_arbitrage(cfmm_ctx *ctx, int64_t q, const double *price,
                                  const double *min_profit /* [q] or NULL */, const uint8_t *allowed,
                                  const cfmm_subgraph_opts *opts, cfmm_price_arb_out *out);
 
+/* ---- arbitrage against external prices from inventory: one token list per row, with holdings ----
+ * A row values its own tokens at external prices c and trades through every pool among them to
+ * maximise cᵀΨ, where the net may spend up to what the caller holds: route! with the objective
+ * cᵀΨ − I(Ψ + h >= 0) restricted to the row's pools.  h = 0 is LinearNonnegative(c); c = e_i with
+ * h = Δin is BasketLiquidation(i, Δin); c = 1 at i and limit_k at each sold k is LimitBasket.
+ *   L_r      the row's tokens allow_token[allow_off[r] .. allow_off[r+1]) (1-based, distinct, any
+ *            order, 1 to CFMM_PRICE_ARB_MAX_TOKENS of them).
+ *   price    aligned with allow_token: c_t finite and >= 0, and every row has a c_t > 0.  A token
+ *            priced 0 stays in the row as an intermediate valued at 0 (unlike the one-mask call).
+ *   holding  aligned with allow_token, or NULL (every h_t = 0): h_t finite and >= 0.
+ *   T        the listed tokens that hold an active pool to another listed token.
+ *   pools    every pool of every pair inside T, as the one-mask call (global insertion order,
+ *            retired pools listed); local token order T ascending.
+ * Problem.  Minimise G(ν) = Σ_p π_p(ν) + hᵀν on the box ν_t >= c_t + 1e-8 (one IEEE addition), with
+ * no upper bound; the linear term is h, and hᵀν is summed over the held tokens in a fixed order (the
+ * CTA sum's tree over them in local order).  P̄ = G − hᵀc = π(ν) + hᵀ(ν − c) >= 0 on the box bounds
+ * the profit from above.
+ *   start    the box's lower bound, as the one-mask call.
+ *   stop     mx = max_t s_t·|pg_t| with s_t = max(ν_t, c̄), c̄ the least positive price the row lists,
+ *            and m_r = mx / P̄ at the committed iterate (0 when mx = 0, +inf when P̄ <= 0 < mx).
+ *            Status 0 when m_r <= rtol or mx <= atol (atol in the price unit, default 0); the other
+ *            statuses as cfmm_solve.  A priced token has ν_t > c_t >= c̄, so s_t = ν_t there; the floor
+ *            c̄ keeps a price-0 token, which sits near ν_t = 1e-8, measured in token units.  atol > 0
+ *            lets a row with nothing worth doing stop at once instead of running to max_iter as g goes
+ *            to 0 with mx.
+ * What a fill promises (ε = max(rtol·P̄, atol); derived in price_arb_kernels.cuh):
+ *   Ψ_t >= −h_t − ε/max(ν_t, c̄) for every token: the row spends at most its holding, up to ε/c̄ units
+ *   of any token;
+ *   profit = Σ_t c_t·Ψ_t in local order (the first term alone, then IEEE additions);
+ *   P̄ − cᵀΨ = Σ_t (ν_t − c_t)(Ψ_t + h_t) <= |T|·ε + Σ_{t on its bound} 1e-8·(Ψ_t + h_t).  P̄ bounds
+ *   the optimum profit from above; cᵀΨ exceeds P̄ by at most the overdraft valued at ν,
+ *   Σ_t (ν_t − c_t)·max(−Ψ_t − h_t, 0) <= |T|·ε (up to the rounding of fp64 sums).
+ * A row with no holding, atol 0 and every listed price > 0 runs the one-mask call's operations (lin 0,
+ * linear value 0.0, s_t = ν_t, m_r = mx / g): its outputs equal cfmm_quote_price_arbitrage's with its list as the
+ * mask and its prices, bit for bit.
+ * Outputs: cfmm_price_arb_out, as the one-mask call (a row fills only at solver status 0).
+ * cfmm_quote_price_arbitrage_rows prices every row on the current state on its own; no state changes.
+ * cfmm_execute_price_arbitrage_rows runs the rows in batch order, each re-solved on the state the
+ * earlier filled rows left; min_profit (NULL: none; finite and >= 0) reverts a row below it with
+ * CFMM_ORDER_LIMIT (an equal profit fills).  Two rows conflict when their lists intersect; rows are
+ * leveled by cfmm_execute_paths' rule, so rows on disjoint lists share a level and its launch.  An
+ * execute whose token or leg outputs are given with a cap below the size is rejected before anything
+ * changes.  Each row's CTA builds its slot graph as the _rows order calls do (b² · 7 bytes of device
+ * workspace per resident CTA, b the longest list).
+ * Options: cfmm_price_arb_opts (NULL: cfmm_subgraph_opts' defaults and atol 0).  Single GPU.
+ * Synchronous.  Before cfmm_finalize: CFMM_ERR_STATE.  q == 0 does nothing.  CFMM_ERR_INVALID before
+ * anything runs for: q < 0; a null allow_off, a null allow_token when allow_off[q] > 0, a null price;
+ * an allow_off that does not start at 0 or that decreases; a list that is empty or longer than
+ * CFMM_PRICE_ARB_MAX_TOKENS; a token outside 1..n_tokens or listed twice in a row; a price or holding
+ * that is negative, NaN or Inf; a row with no positive price; the option errors of subgraph orders;
+ * an atol that is not finite or is < 0; a min_profit that is NaN, negative or Inf. */
+typedef struct {
+  int max_iter, max_fun;
+  double rtol, factr;
+  double atol; /* the absolute stop on max_t ν_t·|pg_t|, >= 0 */
+} cfmm_price_arb_opts;
+int cfmm_quote_price_arbitrage_rows(cfmm_ctx *ctx, int64_t q, const int64_t *allow_off /* [q+1] */,
+                                    const int64_t *allow_token /* [allow_off[q]] */,
+                                    const double *price /* [allow_off[q]] */,
+                                    const double *holding /* [allow_off[q]] or NULL */,
+                                    const cfmm_price_arb_opts *opts /* NULL = defaults */,
+                                    cfmm_price_arb_out *out);
+int cfmm_execute_price_arbitrage_rows(cfmm_ctx *ctx, int64_t q, const int64_t *allow_off,
+                                      const int64_t *allow_token, const double *price, const double *holding,
+                                      const double *min_profit /* [q] or NULL */,
+                                      const cfmm_price_arb_opts *opts, cfmm_price_arb_out *out);
+
 /* ---- UniV3 liquidity changes: mint and burn price ranges ---------------------------------
  * A UniV3 pool's ladder is T₁ > T₂ > … > Tₙ (lower_ticks); tick i holds liquidity Lᵢ on the
  * prices (Tᵢ₊₁, Tᵢ], the last tick Lₙ on (0, Tₙ] (tick_high_price / tick_low_price,
